@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — BASELINE.json's metric on BASELINE.json's configs, all five under one clock.
 
-  python bench.py --gpus N --steps K --warmup W            # this repo (sm_100a kernels through the C ABI)
+  python bench.py --gpus N --steps K --warmup W            # this repo (sm_90a kernels through the C ABI)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU kernels on the host cores
 
 ONE JSON line on stdout (rank 0). The headline fields are BASELINE `configs[1]` (workload `c2`); `"configs": {"c1": …, "c3": …,
@@ -50,14 +50,11 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 SEED = 20260922
 LATENT = 32      # intrinsic dimensionality of the synthetic embedding model
 NOISE = 0.25     # isotropic noise relative to the per-coordinate signal
-IMMA_PEAK_TOPS = 917.0   # tools/micro/imma_rate.cu on B200: legacy IMMA.16832 issue rate, 2*16*8*32 ops each (profiles/r2_imma_rate.md)
-UMMA_I8_PEAK_TOPS = 4559.0  # tools/micro/umma_rate.cu on B200: tcgen05.mma kind::i8 128x256x32 at 128 cycles each on all 148 SMs
-
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel, from the committed `ncu --set full` captures
-# under profiles/ ; key = (workload, n, nq, rerankK)
-NCU_TRAFFIC = {("c2", 1_000_000, 10_000, 100): 93.085e9,   # profiles/r2b_ncu_search_c2.md
-               ("c3", 1_000_000, 10_000, 100): 16.377e9,   # profiles/r2b_ncu_search_c3.md
-               ("c4", 1_000_000, 1000, 100): 0.790e9}      # profiles/r2_ncu_bq_umma.md (the tcgen05 filter launch)
+# NVIDIA's H100 SXM data sheet (700 W card): dense INT8 tensor-core rate and HBM3 bandwidth. Data-sheet figures, not measured.
+I8_PEAK_TOPS = 1979.0
+HBM_PEAK_GBS = 3350.0
+# what the timed paths computed in their last step, written by --dump-outputs: name -> array
+DUMP = {}
 
 
 def log(*a):
@@ -90,7 +87,7 @@ def gen_unit_rows_device(torch, seed, n, dim, dist="latent", chunk=262144, devic
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -160,7 +157,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return HBM_PEAK_GBS, "H100 SXM data sheet (not measured)"
 
 
 def recall_at_k(found, truth, k):
@@ -420,6 +417,7 @@ def bench_c2(cx, w):
     a = cx.args
     topK, rerankK = a.topk, a.topk * a.overquery
     r = search_legs(cx, w, w.vec, None, topK, rerankK, a.steps, a.warmup)
+    DUMP.update(c2_nodes=r["nodes"], c2_scores=r["scores"])
     total_q = a.steps * a.nq * cx.world
     peak, peak_src = measured_peaks()
     per_unit = a.dim * 4 + 8
@@ -430,14 +428,14 @@ def bench_c2(cx, w):
            "config": {"workload": "c2: synthetic %dx%d float32 unit rows (%s, generated on the device), DOT_PRODUCT, graph M=32 ef=100 overflow=1.2 alpha=1.2 "
                                   "hierarchy, GraphSearcher top-%d rerankK=%d, %d queries/step/GPU" % (a.n, a.dim, a.dist, topK, rerankK, a.nq),
                       "parallelism": "replica per GPU, queries sharded (no data-path collective)",
-                      "l2": "inputs %.2f GB >> 126 MB L2 (random row gathers)" % (a.n * a.dim * 4 / 1e9)},
+                      "l2": "inputs %.2f GB >> 50 MB L2 (random row gathers)" % (a.n * a.dim * 4 / 1e9)},
            "value": total_q / (r["dev_ms"] / 1e3), "ms_per_step": r["dev_ms"] / a.steps, "recall_at_10": r["recall"],
            "scored_vectors_per_sec": r["scored"] / (r["dev_ms"] / 1e3), "visited_per_query": r["visited"] / float(a.nq),
            "wall_ms_per_step": 1e3 * r["wall_s"] / a.steps, "clocks_timed_region": r["clock_window"],
            "e2e": {"value": total_q / r["e2e_s"], "unit": "queries/s", "h2d_bytes_per_step": r["h2d"], "d2h_bytes_per_step": r["d2h"]},
            "gpu_launches": r["launches"], "build_seconds": w.build_s,
            "roofline": {"kernel": "graph_search_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                        "traffic": NCU_TRAFFIC.get(("c2", a.n, a.nq, rerankK)), "peak_source": peak_src,
+                        "traffic": None, "peak_source": peak_src,
                         "algorithmic_bytes_per_launch": algo_bytes / a.steps, "algorithmic_bytes_per_scored_vector": per_unit}}
     if cx.rank == 0 and not a.no_cpu:
         out["parity"] = parity_search(cx, w, r["nodes"], r["scores"], topK, rerankK, None, a.parity_queries)
@@ -543,6 +541,7 @@ def bench_c3(cx, w, steps):
     pqv = jv.PQVectors(codes, cb, a.dim, 256)
     w.gi.fuse_pq(pqv)
     r = search_legs(cx, w, pqv, w.vec, topK, rerankK, steps, 3)
+    DUMP.update(c3_nodes=r["nodes"], c3_scores=r["scores"])
     total_q = steps * a.nq * cx.world
     peak, peak_src = measured_peaks()
     adc = (r["visited"] + a.nq) * steps  # this rank
@@ -558,10 +557,9 @@ def bench_c3(cx, w, steps):
            "e2e": {"value": total_q / r["e2e_s"], "unit": "queries/s", "h2d_bytes_per_step": r["h2d"], "d2h_bytes_per_step": r["d2h"]},
            "gpu_launches": r["launches"],
            "roofline": {"kernel": "graph_search_kernel<PQ> (fused records)", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                        "traffic": NCU_TRAFFIC.get(("c3", a.n, a.nq, rerankK)), "peak_source": peak_src, "adc_frac_of_code_stream_roofline": adc / (r["dev_ms"] / 1e3) / adc_roof,
+                        "traffic": None, "peak_source": peak_src, "adc_frac_of_code_stream_roofline": adc / (r["dev_ms"] / 1e3) / adc_roof,
                         "lut_gathers_per_sec": adc * M / (r["dev_ms"] / 1e3),
-                        "note": "not HBM bound: a hop is a dependent chain (record -> visited.add -> %d LUT gathers per candidate out of an L2-resident 96 KB table -> merge) and "
-                                "no unit is saturated in the ncu capture (L2 34%%, DRAM 22%%, issue slots 52%%: profiles/r2b_ncu_search_c3.md); "
+                        "note": "not HBM bound: a hop is a dependent chain (record -> visited.add -> %d LUT gathers per candidate out of an L2-resident 96 KB table -> merge); "
                                 "code-stream roofline = peak / M = %.1f G vec/s" % (M, adc_roof / 1e9)}}
     if cx.rank == 0 and not a.no_cpu:
         pq = {"codebooks": cb, "codes": codes, "M": M}
@@ -598,9 +596,10 @@ def bench_c1(cx, steps):
         dev_ms += res.device_ms
         scored += res.visitedCount + 100
         t0 = time.perf_counter()
-        nodes, _, _ = jv.topk_bruteforce(vec, VSF.EUCLIDEAN, queries, 100)
+        nodes, bf_scores, _ = jv.topk_bruteforce(vec, VSF.EUCLIDEAN, queries, 100)
         t_bf += time.perf_counter() - t0
     launches = lib.jv_kernel_launch_count() - l0
+    DUMP.update(c1_nodes=res.nodes, c1_scores=res.scores, c1_bruteforce_nodes=nodes, c1_bruteforce_scores=bf_scores)
     peak, _ = measured_peaks()
     out = {"metric": "queries_per_sec_at_recall@100", "unit": "queries/s", "n_gpus": 1, "steps": steps, "warmup": 3, "higher_is_better": True,
            "dtype": "f32", "data": "siftsmall (tests/golden/siftsmall)",
@@ -671,6 +670,9 @@ def bench_c4(cx, steps):
     dev_s = ev0.elapsed_time(ev1) / 1e3
     launches = lib.jv_kernel_launch_count() - l0
     unresolved = sb.status()
+    kh = keys.cpu().numpy()
+    hi32 = (kh >> 32).astype(np.int32)
+    DUMP.update(c4_scores=(hi32 ^ ((hi32 >> 31) & 0x7fffffff)).view(np.float32), c4_nodes=~(kh & 0xffffffff).astype(np.int64) & 0xffffffff)
     # e2e: host queries in (pinned), host keys out
     hq = torch.from_numpy(queries).pin_memory()
     cx.barrier()
@@ -684,7 +686,6 @@ def bench_c4(cx, steps):
     pairs = float(steps) * nq * n
     ops = pairs * 2.0 * (W * 64)  # u8 multiply-adds of the contraction, both counted
     umma = os.environ.get("JV_BQ_FILTER", "u")[0] != "i" and W % 2 == 0 and W <= 32
-    tpeak = UMMA_I8_PEAK_TOPS if umma else IMMA_PEAK_TOPS
     out = {"metric": "queries_per_sec_bq_bruteforce", "unit": "queries/s", "n_gpus": cx.world, "steps": steps, "warmup": 33, "higher_is_better": True,
            "scaling": "strong", "dtype": "u8 x u8 -> s32 (exact)", "data": "synthetic",
            "config": {"workload": "c4: synthetic %dx%d BQ (sign bits of N(0,1) rows), Hamming top-%d, %d queries/step, base range-sharded over %d GPU(s)" % (n, dim, k, nq, cx.world),
@@ -693,13 +694,10 @@ def bench_c4(cx, steps):
            "value": steps * nq / dev_s, "ms_per_step": 1e3 * dev_s / steps, "pairs_per_sec": pairs / dev_s, "unresolved_queries": unresolved,
            "e2e": {"value": steps * nq / e2e_s, "unit": "queries/s", "h2d_bytes_per_step": int(queries.nbytes), "d2h_bytes_per_step": int(nq * k * 8)},
            "gpu_launches": launches,
-           "roofline": {"kernel": "bq_umma_filter_kernel (tcgen05.mma kind::i8, TMEM accumulators)" if umma else "bq_imma_kernel (IMMA.16832 u8)",
-                        "bound": "tensor", "achieved": ops / cx.world / dev_s / 1e12, "peak": tpeak, "unit": "TOP/s",
-                        "frac": ops / cx.world / dev_s / 1e12 / tpeak,
-                        "traffic": NCU_TRAFFIC.get(("c4", n, nq, k)) if cx.world == 1 else None,
-                        "peak_source": ("measured issue rate of tcgen05.mma kind::i8 on B200 (tools/micro/umma_rate.cu, profiles/r2_umma_rate.md)" if umma else
-                                        "measured issue rate of the legacy IMMA.16832 path on B200 (tools/micro/imma_rate.cu, profiles/r2_imma_rate.md)") +
-                                       "; MEASURED_PEAKS.json has no integer entry",
+           "roofline": {"kernel": "bq_wgmma_filter_kernel (wgmma u8, register accumulators)" if umma else "bq_imma_kernel (IMMA.16832 u8)",
+                        "bound": "tensor", "achieved": ops / cx.world / dev_s / 1e12, "peak": I8_PEAK_TOPS, "unit": "TOP/s",
+                        "frac": ops / cx.world / dev_s / 1e12 / I8_PEAK_TOPS, "traffic": None,
+                        "peak_source": "H100 SXM data sheet, dense INT8 (not measured)",
                         "note": "whole step in the denominator (sample pass + thresholds + filter pass + select)",
                         "hbm_unique_GBps": float(steps) * (hi - lo) * W * 8 / dev_s / 1e9}}
     if cx.rank == 0 and not a.no_cpu:
@@ -772,6 +770,11 @@ def bench_c5(cx):
     gt, _, _ = jv.topk_bruteforce(vec, VSF.DOT_PRODUCT, queries, 10)
     res = jv.GraphSearcher(gi).search(vec, queries, VSF.DOT_PRODUCT, 10, 100, reranker=nvq)
     rec = recall_at_k(res.nodes, gt, 10)
+    if cx.args.dump_outputs:
+        _, adj0 = gi.level(0)
+        rows = np.sort(np.random.default_rng(SEED + 52).choice(n, min(n, 65536), replace=False))
+        DUMP.update(c5_adjacency_sample_rows=rows, c5_adjacency_sample=adj0[rows], c5_search_nodes=res.nodes, c5_search_scores=res.scores)
+        del adj0
     peak, peak_src = measured_peaks()
     out = {"metric": "build_inserts_per_sec", "unit": "vectors/s", "n_gpus": cx.world, "steps": 1, "warmup": 0, "higher_is_better": True,
            "scaling": "strong", "dtype": "f32", "data": "synthetic",
@@ -820,6 +823,20 @@ def bench_c5(cx):
 
 
 # ------------------------------------------------------------------------------------------------ driver
+def dump_outputs(d):
+    """DUMP as DIR/<name>.npy: float arrays as float32 / float64, integer ids as float64 (exact below 2^53)"""
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, arr in sorted(DUMP.items()):
+        arr = np.asarray(arr)
+        arr = arr.astype(np.float64) if arr.dtype.kind in "iub" else arr.astype(arr.dtype if arr.dtype in (np.float32, np.float64) else np.float32)
+        total += arr.nbytes
+        if total > 64 << 20:
+            raise RuntimeError("--dump-outputs: %s would take the dump past 64 MB" % name)
+        np.save(os.path.join(d, name + ".npy"), arr)
+    log("dumped %d arrays (%.1f MB) to %s" % (len(DUMP), total / 1e6, d))
+
+
 def guarded(name, fn):
     t0 = time.time()
     try:
@@ -855,6 +872,8 @@ def main():
                     "(ncu --profile-from-start off then lists exactly the launches of the timed region)")
     ap.add_argument("--sweep", action="store_true", help="also report overquery 1/2/5/10")
     ap.add_argument("--dist", default="latent", choices=["latent", "iid"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what each timed path computed in its last step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else max(args.warmup, 1)
 
@@ -923,7 +942,7 @@ def main():
             if cx.rank == 0 and not args.no_cpu:
                 cb, _ = cpu_baseline_search(cx, w, args.topk, args.topk * args.overquery, None)
                 out["cpu_baseline"] = cb
-        c3 = guarded("c3", lambda: bench_c3(cx, w, max(3, min(args.steps, 10)))) if single in (None, "c3") else None
+        c3 = guarded("c3", lambda: bench_c3(cx, w, args.steps)) if single in (None, "c3") else None
         if single == "c3":
             out = c3
         elif c3 is not None:
@@ -933,13 +952,13 @@ def main():
         del w
         cx.torch.cuda.empty_cache()
     if single in (None, "c1") and cx.rank == 0:
-        c1 = guarded("c1", lambda: bench_c1(cx, max(3, min(args.steps, 10))))
+        c1 = guarded("c1", lambda: bench_c1(cx, args.steps))
         if single == "c1":
             out = c1
         else:
             out.setdefault("configs", {})["c1"] = c1
     if single in (None, "c4"):
-        c4 = guarded("c4", lambda: bench_c4(cx, max(10, args.steps)))
+        c4 = guarded("c4", lambda: bench_c4(cx, args.steps))
         if single == "c4":
             out = c4
         else:
@@ -954,8 +973,8 @@ def main():
     if cx.rank == 0:
         tr = out.get("clocks_timed_region")
         if tr:
-            # the headline workload's own window (load loop + timed steps): an HBM-saturating kernel sits at the 1000 W cap and the SM
-            # clock drops below max there (sw_power_cap), which the whole-run median hides
+            # the headline workload's own window (load loop + timed steps): an HBM-saturating kernel can sit at the card's power cap and
+            # the SM clock drop below max there (sw_power_cap), which the whole-run median hides
             clocks = dict(clocks, sm_mhz=tr["sm_mhz"], sm_mhz_min=tr["sm_mhz_min"], power_w=tr["power_w"], samples_timed_region=tr["samples"],
                           sm_mhz_whole_run=clocks.get("sm_mhz"))
         out["clocks"] = clocks
@@ -964,6 +983,8 @@ def main():
             par.update({k: (v.get("parity", {}) or {}).get("ok") for k, v in out["configs"].items()})
             out["parity_all_ok"] = all(v is True for v in par.values())
             out["parity_by_config"] = par
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs)
         print(json.dumps(out), flush=True)
     if cx.td is not None:
         cx.td.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * jvector_b200.h — C ABI of libjvector_b200.so, the B200 (sm_100a) replacement for JVector's libjvector.so.
+ * jvector_b200.h — C ABI of libjvector_b200.so, the H100 (sm_90a) replacement for JVector's libjvector.so.
  *
  * Two groups of entry points:
  *
@@ -25,7 +25,7 @@
  * pointers borrowed for the duration of the call unless the name ends in _device. Scores are the reference's
  * similarity scores (base:vector/VectorSimilarityFunction.java:37-69), higher = closer. Top-k keys are the
  * reference's 64-bit ordering key (base:graph/NodeQueue.java:125-137). No CPU fallback exists: without an
- * sm_100 device jv_gpu_init() fails and every other jv_ call returns JV_ERR_NO_DEVICE.
+ * sm_90 device jv_gpu_init() fails and every other jv_ call returns JV_ERR_NO_DEVICE.
  */
 #ifndef JVECTOR_B200_H
 #define JVECTOR_B200_H
@@ -76,7 +76,7 @@ enum { JV_EUCLIDEAN = 0, JV_DOT_PRODUCT = 1, JV_COSINE = 2 }; /* VectorSimilarit
 
 enum {
     JV_OK = 0,
-    JV_ERR_NO_DEVICE = -1,   /* no CUDA device / not sm_100 / jv_gpu_init not called */
+    JV_ERR_NO_DEVICE = -1,   /* no CUDA device / not sm_90 / jv_gpu_init not called */
     JV_ERR_INVALID = -2,     /* bad argument */
     JV_ERR_CUDA = -3,        /* CUDA runtime error, see jv_last_error() */
     JV_ERR_OOM = -4,

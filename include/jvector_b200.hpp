@@ -32,7 +32,7 @@ inline void check(int rc)
 {
     if (rc != JV_OK) throw Error(rc, jv_last_error());
 }
-/// NativeVectorizationProvider's constructor: throws when no sm_100 device can be bound (caller falls back to Panama)
+/// NativeVectorizationProvider's constructor: throws when no sm_90 device can be bound (caller falls back to Panama)
 inline void init(int device = 0) { check(jv_gpu_init(device)); }
 
 class Vectors {

@@ -1,4 +1,4 @@
-"""jvector_b200 — B200 (sm_100a) implementation of JVector's distance / quantised-scoring hot path.
+"""jvector_b200 — H100 (sm_90a) implementation of JVector's distance / quantised-scoring hot path.
 
 The product is the C-ABI library `lib/libjvector_b200.so` (include/jvector_b200.h). This package is the host-side
 mirror of the reference's interface for that path, used by the tests and the bench:

@@ -131,7 +131,7 @@ def check(rc):
 
 
 def init(device=None):
-    """Bind the process to a B200. Raises when no sm_100 device is present."""
+    """Bind the process to an H100. Raises when no sm_90 device is present."""
     global _inited
     lib = load()
     if _inited:

@@ -1,4 +1,4 @@
-"""Compiles libjvector_b200.so in-tree with nvcc for sm_100a (no GPU needed: nvcc cross-compiles)."""
+"""Compiles libjvector_b200.so in-tree with nvcc for sm_90a (no GPU needed: nvcc cross-compiles)."""
 import os
 import subprocess
 import sys
@@ -13,7 +13,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CU = ["kernels_batch.cu", "bq_imma.cu", "bq_umma.cu", "search.cu", "build.cu", "api.cu"]
 CPP = ["legacy_host.cpp", "legacy_simd.cpp", "legacy_avx512.cpp"]
 HEADERS = ["common.cuh", "scorers.cuh", "kernels.h", "legacy_avx512.h", os.path.join("..", "..", "include", "jvector_b200.h")]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # -fmad=false: only explicit fmaf() fuses (NVQ bit tricks and score maps must round like the reference's scalar code)
 EXTRA = os.environ.get("JV_NVCC_EXTRA", "").split()
 NVFLAGS = EXTRA + ["-O3", "-std=c++17", "-lineinfo", "-fmad=false", "-Xcompiler", "-fPIC,-fvisibility=hidden,-O3", "-Xptxas", "-v"]

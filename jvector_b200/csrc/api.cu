@@ -1,5 +1,5 @@
 // api.cu — the C ABI of include/jvector_b200.h, batched GPU group: handle management, host<->HBM staging, launches.
-// No CPU fallback lives here: without an sm_100 device every entry point returns JV_ERR_NO_DEVICE.
+// No CPU fallback lives here: without an sm_90 device every entry point returns JV_ERR_NO_DEVICE.
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -258,7 +258,7 @@ static int bind_device(int device)
     if (device < 0 || device >= n || device >= MAX_DEVICES) return fail(JV_ERR_INVALID, "device index out of range");
     cudaDeviceProp p;
     CK(cudaGetDeviceProperties(&p, device), "cudaGetDeviceProperties");
-    if (p.major != 10) return fail(JV_ERR_NO_DEVICE, "device is not sm_100 (this library carries sm_100a code only)");
+    if (p.major != 9 || p.minor != 0) return fail(JV_ERR_NO_DEVICE, "device is not sm_90 (this library carries sm_90a code only)");
     CK(cudaSetDevice(device), "cudaSetDevice");
     g_sm_counts[device] = p.multiProcessorCount;
     g_mask |= 1u << device;
@@ -310,7 +310,7 @@ int jv_gpu_set_device(int device)
 uint32_t jv_gpu_bound_mask(void) { return g_mask; }
 
 const char *jv_last_error(void) { return t_err.c_str(); }
-const char *jv_version(void) { return "jvector-b200 0.1 (sm_100a)"; }
+const char *jv_version(void) { return "jvector-b200 0.1 (sm_90a)"; }
 int jv_gpu_sm_count(void) { return g_default_device >= 0 ? g_sm_counts[t_device >= 0 ? t_device : g_default_device] : 0; }
 int64_t jv_kernel_launch_count(void) { return (int64_t)g_launches.load(); }
 

@@ -4,8 +4,7 @@
 // hd = popcount(a ^ b) (base:vector/DefaultVectorUtilSupport.java:342-348). For a batch of queries against every row that is
 // a dense binary contraction: hd = popc(a) + popc(b) - 2 * <a, b> over {0,1} operands, and <a, b> accumulates exactly in
 // int32. The kernel expands bit words to {0,1} bytes in registers and feeds IMMA.16832 (mma.sync m16n8k32 u8 x u8 -> s32,
-// native SASS on sm_100a; measured issue rate 112 G IMMA/s = 917 Tops, profiles/r2_imma_rate.md), so the popcount loop of
-// round 1 (POPC / LOP3 bound at 92 G pairs/s) becomes tensor-pipe bound. Integer arithmetic: keys are bit-identical to the
+// native SASS on sm_90a), so a popcount loop (POPC / LOP3 bound) becomes tensor-pipe bound. Integer arithmetic: keys are bit-identical to the
 // scalar restatement.
 //
 // Top-k without a sort of the scores: Hamming distances live in [0, dim], so thresholds are integers.
@@ -427,7 +426,7 @@ static int bq_imma_sample_rows(long long n)
     return (int)(n < s ? n : s);
 }
 
-constexpr int NQ_ALIGN = 256;  // query count padded to the tcgen05 tile (a multiple of the IMMA tile)
+constexpr int NQ_ALIGN = 256;  // query count padded to the wgmma tile (a multiple of the IMMA tile)
 
 size_t bq_imma_scratch_bytes(long long n, int nq, int W)
 {
@@ -438,7 +437,7 @@ size_t bq_imma_scratch_bytes(long long n, int nq, int W)
     b += 64 + 256;                                           // counters
     b += (size_t)nq_pad * bq_imma_sample_rows(n) * 2 + 256;  // hdm
     b += (size_t)nq * BQ_IMMA_CAP * 8 + 256;                 // buf
-    b += bq_umma_image_bytes(nq, W) + 256;                   // pre-swizzled query images of the tcgen05 filter pass
+    b += bq_umma_image_bytes(nq, W) + 256;                   // pre-swizzled query images of the wgmma filter pass
     return b + 1024;
 }
 
@@ -453,7 +452,7 @@ cudaError_t launch_bq_topk_imma(const DataDesc &d, const float *queries_dev, int
 {
     if (nq <= 0) return cudaSuccess;
     const int nq_pad = (nq + NQ_ALIGN - 1) / NQ_ALIGN * NQ_ALIGN, W32 = 2 * d.W;
-    // the full filter pass runs on tcgen05 (bq_umma.cu: 2.4x the IMMA kernel of this file on c4) whenever the shape allows;
+    // the full filter pass runs on the warpgroup MMA (bq_umma.cu) whenever the shape allows;
     // JV_BQ_FILTER=imma forces the legacy-MMA kernel (the sample pass and the redo passes always use it)
     const char *fm = getenv("JV_BQ_FILTER");
     const bool use_umma = !(fm && fm[0] == 'i') && bq_umma_supported(d);

@@ -1,25 +1,21 @@
-// bq_umma.cu — the FILTER pass of the BQ Hamming top-k (see bq_imma.cu for the whole pipeline) on the 5th-generation tensor
-// cores: tcgen05.mma kind::i8 (u8 x u8 -> s32, exact), accumulators in TMEM, operands in shared memory in the canonical K-major
-// SWIZZLE_128B layout, warp-specialised roles connected by mbarriers.
+// bq_umma.cu — the FILTER pass of the BQ Hamming top-k (see bq_imma.cu for the whole pipeline) on Hopper's warpgroup tensor-core
+// instructions: wgmma.mma_async kind u8 x u8 -> s32 (exact), operands in shared memory in the canonical K-major SWIZZLE_128B
+// layout, accumulators in the registers of the two consumer warpgroups, producer and consumers connected by mbarriers.
 //
 //   D[128 rows][256 queries] += A[128][K] * B[256][K]^T,  A bytes in {0, 2^s}, B bytes in {0, 2^(7-s)} expanded from bit words
 //   (D = 128 * popcount(row & query), exact in s32), K = dim rounded to 128
 //
-// Why a second kernel next to the IMMA one: the legacy IMMA path tops out at 917 TOP/s and re-expands both operands in every
-// warp tile; here the row tile is expanded ONCE per CTA tile into shared memory (producer warps), the query tile arrives as a
-// pre-expanded, pre-swizzled 32 KB image by one bulk copy, and one elected thread issues 128 x 256 x 32 MMAs.
+// Why a second kernel next to the IMMA one: the mma.sync path re-expands both operands in every warp tile; here the row tile is
+// expanded ONCE per CTA tile into shared memory by the producer warpgroup, and the query tile arrives as a pre-expanded,
+// pre-swizzled 32 KB image by one bulk copy.
 //
-// Roles (640 threads): warp 0 = B producer (cp.async.bulk of the query image chunk), warp 1 = MMA issuer + TMEM owner,
-// warps 4-7 and 16-19 = two epilogue groups, one per accumulator buffer, so each has two tiles' worth of MMA time to drain its
-// tile (tcgen05.ld: warp w may touch TMEM lanes 32 (w % 4) ..), warps 8-15 = A producers (two threads per row:
-// 64 bits -> 64 bytes each, swizzled 128-bit stores, fence.proxy.async, arrive). Pipelines: full[s] / empty[s] over 4 operand
-// stages of 48 KB, tmem_full[a] / tmem_empty[a] over two 256-column accumulators, so the epilogue of one tile overlaps the MMAs
-// of the next. The epilogue is branch-free per column: thresholds of the query tile sit in shared memory, a column costs
-// IADD3 + ISETP + SEL into a survivor bit mask; the rare survivors (about 0.3 %) are re-read from TMEM in a warp-uniform loop and go
-// to a per-warp shared-memory queue (ballot slots, no atomics) that the warp flushes after handing the accumulator back. Row
-// popcounts come from the producers. Round-2 profiles (profiles/r2_ncu_bq_umma.md): the first version's per-element LDG + branch
-// epilogue kept the MMA thread waiting half its time (6.8 ms); this one runs the filter pass in 2 ms.
-// Every spin-wait is bounded and traps: a wrong barrier count aborts the launch instead of hanging the device.
+// Roles (384 threads): warpgroup 0 = producers (one thread per row: 128 bits -> 128 bytes per stage, swizzled 16-byte stores,
+// fence.proxy.async, arrive; thread 0 also issues the cp.async.bulk of the query image chunk), warpgroups 1 and 2 = consumers,
+// each owning 64 rows of the tile: 4 x wgmma m64n256k32 per stage into 128 s32 registers per thread, then the epilogue on those
+// registers. Pipeline: full[s] / empty[s] over 4 operand stages of 48 KB; a consumer keeps one wgmma group in flight and hands a
+// stage back when the group that read it has completed. Epilogue: thresholds of the query tile sit in shared memory; a column
+// costs IADD + ISETP; the rare survivors (about 0.3 %) append their keys with one atomic each. Row popcounts come from the
+// producers. Every spin-wait is bounded and traps: a wrong barrier count aborts the launch instead of hanging the device.
 #include <limits.h>
 
 #include "kernels.h"
@@ -28,18 +24,15 @@ namespace jv {
 
 namespace {
 
-constexpr int UM = 128;           // rows per tile (MMA M)
-constexpr int UN = 256;           // queries per tile (MMA N)
+constexpr int UM = 128;           // rows per tile (two consumer warpgroups x wgmma M = 64)
+constexpr int UN = 256;           // queries per tile (wgmma N)
 constexpr int UKC = 128;          // K bytes per stage (one 128-byte swizzle atom wide)
 constexpr int USTAGES = 4;
-constexpr int UTHREADS = 640;
+constexpr int UTHREADS = 384;
 constexpr int A_STAGE_BYTES = UM * UKC;  // 16 KB
 constexpr int B_STAGE_BYTES = UN * UKC;  // 32 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int N_A_PRODUCERS = 256;  // two threads per row
-constexpr int NPAR = 8;               // ring of row-popcount buffers: the producers run up to USTAGES stages (= tiles when K is one
-                                      // chunk) ahead of the MMA, which runs up to 2 tiles ahead of the epilogue
-constexpr int WQ_CAP = 256;           // survivor queue of one epilogue warp and tile (expected ~25 entries); overflow appends directly
+constexpr int NPAR = 8;  // ring of row-popcount buffers: the producers run at most USTAGES stages (= tiles when K is one chunk) ahead
 
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar)
 {
@@ -51,39 +44,41 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, unsigned phase)
         if (spins > (1u << 28)) __trap();  // a pipeline bug must abort the launch, not hang the device
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// shared-memory matrix descriptor, K-major, SWIZZLE_128B (cute/arch/mma_sm100_desc.hpp SmemDescriptor; canonical layout
-// ((8,n),2):((8,SBO),1) in 16-byte units): rows 128 B apart inside an 8-row atom, atoms SBO = 1024 B apart
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr)
+// wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: rows 128 B apart inside an 8-row atom, atoms SBO = 1024 B apart
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);  // start address, bits [0,14)
     d |= (uint64_t)1 << 16;                       // leading byte offset (unused by swizzled K-major layouts), bits [16,30)
     d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset, bits [32,46)
-    d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell), bits [46,48)
-    d |= (uint64_t)2 << 61;                       // layout type SWIZZLE_128B, bits [61,64)
+    d |= (uint64_t)1 << 62;                       // layout type SWIZZLE_128B, bits [62,64)
     return d;
 }
 
-// instruction descriptor (InstrDescriptor): c = S32 (2) at [4,6), a = b = U8 (0), K-major both, N >> 3 at [17,23), M >> 4 at [24,29)
-constexpr uint32_t UMMA_IDESC = (2u << 4) | ((uint32_t)(UN >> 3) << 17) | ((uint32_t)(UM >> 4) << 24);
-
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
+// D[64][256] (+)= A[64][32] * B[256][32]^T, u8 x u8 -> s32. Accumulator fragment: register 4 j + 2 h + e holds row
+// 16 (warp % 4) + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.
+__device__ __forceinline__ void wgmma_u8_m64n256k32(uint32_t (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k32.s32.u8.u8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p;\n\t"
+        "}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
+__device__ __forceinline__ void acc_fence(uint32_t (&d)[128])
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+#pragma unroll
+    for (int i = 0; i < 128; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
 
 // the query tile as shared-memory images: [qtile][kchunk][UN rows x 128 B], swizzled exactly as the MMA reads it
@@ -124,18 +119,14 @@ struct UmmaParams {
     long long id_base;
 };
 
-__global__ void __launch_bounds__(UTHREADS, 1) bq_umma_filter_kernel(UmmaParams P)
+__global__ void __launch_bounds__(UTHREADS, 1) bq_wgmma_filter_kernel(UmmaParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *stage0 = smem;  // USTAGES x (A 16 KB | B 32 KB), 1024-byte aligned
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + USTAGES * STAGE_BYTES);
     uint64_t *empty = full + USTAGES;
-    uint64_t *tmem_full = empty + USTAGES;
-    uint64_t *tmem_empty = tmem_full + 2;
-    uint32_t *tmem_base_slot = reinterpret_cast<uint32_t *>(tmem_empty + 2);
-    int *s_t2 = reinterpret_cast<int *>(smem + USTAGES * STAGE_BYTES + 256);  // [2 groups][UN] thresholds of the group's query tile
-    int *s_parh = s_t2 + 2 * UN;                                                  // [NPAR tiles][2 halves][UM] row popcounts from the producers
-    int2 *s_hits = reinterpret_cast<int2 *>(s_parh + NPAR * 2 * UM);                 // [8 warps][WQ_CAP] (row << 16 | column, par - 2 dot)
+    int *s_t2 = reinterpret_cast<int *>(smem + USTAGES * STAGE_BYTES + 256);  // [UN] thresholds of the current query tile
+    int *s_par = s_t2 + UN;                                                     // [NPAR tiles][UM] row popcounts from the producers
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const long long row_tiles = (P.n + UM - 1) / UM;
@@ -143,185 +134,40 @@ __global__ void __launch_bounds__(UTHREADS, 1) bq_umma_filter_kernel(UmmaParams 
 
     if (tid == 0) {
         for (int s = 0; s < USTAGES; s++) {
-            mbar_init(&full[s], N_A_PRODUCERS + 1);  // 256 row producers + the bulk copy's arrive.expect_tx
-            mbar_init(&empty[s], 1);                 // one tcgen05.commit
-        }
-        for (int a = 0; a < 2; a++) {
-            mbar_init(&tmem_full[a], 1);
-            mbar_init(&tmem_empty[a], 128);
+            mbar_init(&full[s], UM + 1);  // 128 row producers + the bulk copy's arrive.expect_tx
+            mbar_init(&empty[s], 8);      // one arrive per consumer warp
         }
         mbar_fence_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
 
-    if (warp == 0) {
-        // ===== B producer: one bulk copy of the query image chunk per stage =====
-        if (lane == 0) {
-            int stage = 0;
-            unsigned phase = 0;
-            for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-                const int qt = (int)(tile / row_tiles);
-                for (int kc = 0; kc < P.kchunks; kc++) {
-                    mbar_wait_bounded(&empty[stage], phase ^ 1);
-                    mbar_expect_tx(&full[stage], B_STAGE_BYTES);
-                    bulk_g2s(stage0 + stage * STAGE_BYTES + A_STAGE_BYTES, P.images + ((size_t)qt * P.kchunks + kc) * B_STAGE_BYTES, B_STAGE_BYTES, &full[stage]);
-                    if (++stage == USTAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            int stage = 0, acc = 0;
-            unsigned phase = 0, acc_phase = 0;
-            for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-                mbar_wait_bounded(&tmem_empty[acc], acc_phase ^ 1);  // the epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d = tmem_base + (uint32_t)(acc * UN);
-                for (int kc = 0; kc < P.kchunks; kc++) {
-                    mbar_wait_bounded(&full[stage], phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(stage0 + stage * STAGE_BYTES), b_addr = a_addr + A_STAGE_BYTES;
-#pragma unroll
-                    for (int k = 0; k < UKC / 32; k++)
-                        umma_i8(d, umma_desc(a_addr + 32 * k), umma_desc(b_addr + 32 * k), UMMA_IDESC, (kc | k) != 0 ? 1u : 0u);
-                    umma_commit(&empty[stage]);  // frees the stage when these MMAs have read it
-                    if (++stage == USTAGES) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tmem_full[acc]);    // accumulator complete
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if ((warp >= 4 && warp < 8) || warp >= 16) {
-        // ===== epilogue: thread = one row of the tile = one TMEM lane; group g drains accumulator buffer g (every other tile) =====
-        const int grp = warp >= 16 ? 1 : 0, wq4 = warp & 3;
-        const int ltid = wq4 * 32 + lane;
-        const int acc = grp;
-        int cur_qt = -1;
-        unsigned acc_phase = 0;
-        int *my_t2 = s_t2 + grp * UN;
-        int2 *wq = s_hits + (grp * 4 + wq4) * WQ_CAP;  // this warp's private survivor queue: no atomics, no cross-warp barrier
-        const uint32_t lt_mask = (1u << lane) - 1u;
-        auto append = [&](int q, long long rr, int x) {  // x = par - 2 dot
-            const int hd = x + __ldg(P.pb + q);
-            const long long key = topk_key(bq_score_from_hd(hd, P.dim), (int32_t)(rr + P.id_base));
-            const int pos = atomicAdd(&P.cnt[q], 1);
-            if (pos < P.cap) P.buf[(size_t)q * P.cap + pos] = key;
-        };
-        int it = 0;
-        for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, it++) {
-            if ((it & 1) != grp) continue;
-            const int qt = (int)(tile / row_tiles), tbuf = it & (NPAR - 1);
-            const long long row0 = (tile % row_tiles) * UM, rr = row0 + ltid;
-            if (qt != cur_qt) {  // the thresholds of this query tile (padding queries never pass)
-                if (grp == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-                else asm volatile("bar.sync 2, 128;" ::: "memory");
-                for (int c = ltid; c < UN; c += 128) {
-                    const int q = qt * UN + c;
-                    my_t2[c] = q < P.nq ? 128 * __ldg(P.t2 + q) : INT_MIN;  // the accumulators hold 128 * dot
-                }
-                cur_qt = qt;
-                if (grp == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-                else asm volatile("bar.sync 2, 128;" ::: "memory");
-            }
-            mbar_wait_bounded(&tmem_full[acc], acc_phase);
-            tc_fence_after();
-            // the row's popcount, summed by the two producer threads of the row while they expanded it (ordered before the
-            // accumulator's completion through full[] -> MMA -> tmem_full[])
-            const int par = s_parh[(tbuf * 2 + 0) * UM + ltid] + s_parh[(tbuf * 2 + 1) * UM + ltid];
-            const int par128 = rr < P.n ? par << 7 : INT_MAX;  // rows past the end never pass
-            const uint32_t taddr = tmem_base + ((uint32_t)(wq4 * 32) << 16) + (uint32_t)(acc * UN);
-            int wcount = 0;  // warp-uniform
-#pragma unroll 1
-            for (int g = 0; g < UN / 32; g++) {
-                uint32_t v[32];
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-                      "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-                      "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-                      "=r"(v[31])
-                    : "r"(taddr + (uint32_t)(g * 32)));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                const int4 *tp = reinterpret_cast<const int4 *>(my_t2 + g * 32);
-                // pass 1, branch-free: one bit per column that survives (independent LEA / ISETP / SEL chains; the round-2 profile
-                // showed a per-column branch costing ~90 cycles of dependent issue). hd - pb = par - 2 dot <= t2  <=>
-                // 2 (128 dot) + 128 t2 >= 128 par
-                uint32_t mask = 0;
-#pragma unroll
-                for (int c4 = 0; c4 < 8; c4++) {
-                    const int4 t = tp[c4];  // one broadcast LDS.128 per four columns
-                    const int tt[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        const int c = c4 * 4 + e;
-                        mask |= (2 * (int)v[c] + tt[e] >= par128) ? (1u << c) : 0u;
-                    }
-                }
-                // pass 2: only the columns in which some lane of the warp has a survivor (about 3 of 32). The loop is warp-uniform;
-                // the column's accumulator is read back from TMEM with a one-column load (the column index is warp-uniform, a
-                // register array could only be indexed statically); slots in the warp's queue come from a ballot.
-                uint32_t um = __reduce_or_sync(0xffffffffu, mask);
-                while (um) {
-                    const int c = __ffs(um) - 1;
-                    um &= um - 1;
-                    uint32_t dcol;
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(dcol) : "r"(taddr + (uint32_t)(g * 32 + c)));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    const bool hit = (mask >> c) & 1u;
-                    const uint32_t b = __ballot_sync(0xffffffffu, hit);
-                    if (hit) {
-                        const int x = par - ((int)dcol >> 6);  // par - 2 dot
-                        const int slot = wcount + __popc(b & lt_mask);
-                        if (slot < WQ_CAP) wq[slot] = make_int2((ltid << 16) | (g * 32 + c), x);
-                        else append(qt * UN + g * 32 + c, rr, x);
-                    }
-                    wcount += __popc(b);
-                }
-            }
-            // the accumulator is drained: hand it back before the (slower) global flush of the queue
-            tc_fence_before();
-            mbar_arrive(&tmem_empty[acc]);
-            acc_phase ^= 1;
-            __syncwarp();
-            const int nh = min(wcount, WQ_CAP);
-            for (int i = lane; i < nh; i += 32) {
-                const int2 h = wq[i];
-                append(qt * UN + (h.x & 0xffff), row0 + (h.x >> 16), h.y);
-            }
-            __syncwarp();
-        }
-    } else if (warp >= 8 && warp < 16) {
-        // ===== A producers: two threads per row; 64 bits -> 64 bytes per stage and thread, swizzled 16-byte chunks =====
-        const int t = (warp - 8) * 32 + lane, r = t & 127, half = t >> 7;
+    if (warp < 4) {
+        // ===== producers: thread r expands row r of the tile; thread 0 also brings in the query image chunk =====
+        const int r = tid;
         int stage = 0, tbuf = 0;
         unsigned phase = 0;
         for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+            const int qt = (int)(tile / row_tiles);
             const long long rr = (tile % row_tiles) * UM + r;
             const bool live = rr < P.n;
-            const uint2 *rp = reinterpret_cast<const uint2 *>(P.rows + (size_t)(live ? rr : 0) * P.W32) + half;
-            uint2 w = make_uint2(0u, 0u);
+            const uint4 *rp = reinterpret_cast<const uint4 *>(P.rows + (size_t)(live ? rr : 0) * P.W32);
+            uint4 w = make_uint4(0u, 0u, 0u, 0u);
             if (live) w = __ldg(rp);
             int pc = 0;
             for (int kc = 0; kc < P.kchunks; kc++) {
-                uint2 wn = make_uint2(0u, 0u);
-                if (live && kc + 1 < P.kchunks) wn = __ldg(rp + 2 * (kc + 1));  // the next chunk's words are in flight during this one
+                uint4 wn = make_uint4(0u, 0u, 0u, 0u);
+                if (live && kc + 1 < P.kchunks) wn = __ldg(rp + kc + 1);  // the next chunk's words are in flight during this one
                 mbar_wait_bounded(&empty[stage], phase ^ 1);
+                if (r == 0) {
+                    mbar_expect_tx(&full[stage], B_STAGE_BYTES);
+                    bulk_g2s(stage0 + stage * STAGE_BYTES + A_STAGE_BYTES, P.images + ((size_t)qt * P.kchunks + kc) * B_STAGE_BYTES, B_STAGE_BYTES, &full[stage]);
+                }
                 unsigned char *dst = stage0 + stage * STAGE_BYTES + (r >> 3) * 1024 + (r & 7) * 128;
-                const uint32_t ws[2] = {w.x, w.y};
+                const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
-                for (int jj = 0; jj < 4; jj++) {
-                    const int j = half * 4 + jj, sb = (jj & 1) * 4;
-                    const uint32_t word = ws[jj >> 1];
+                for (int j = 0; j < 8; j++) {
+                    const int sb = (j & 1) * 4;
+                    const uint32_t word = ws[j >> 1];
                     uint4 v;  // bit (8 b + s) of the word -> byte b of output word s, value 2^s: one AND per output word
                     v.x = word & (0x01010101u << (sb + 0));
                     v.y = word & (0x01010101u << (sb + 1));
@@ -329,8 +175,8 @@ __global__ void __launch_bounds__(UTHREADS, 1) bq_umma_filter_kernel(UmmaParams 
                     v.w = word & (0x01010101u << (sb + 3));
                     *reinterpret_cast<uint4 *>(dst + ((j ^ (r & 7)) << 4)) = v;
                 }
-                pc += __popc(w.x) + __popc(w.y);
-                if (kc + 1 == P.kchunks) s_parh[(tbuf * 2 + half) * UM + r] = pc;  // this half row's popcount, for the epilogue
+                pc += __popc(w.x) + __popc(w.y) + __popc(w.z) + __popc(w.w);
+                if (kc + 1 == P.kchunks) s_par[tbuf * UM + r] = pc;  // this row's popcount, for the epilogue
                 fence_proxy_async();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
                 mbar_arrive(&full[stage]);
                 if (++stage == USTAGES) { stage = 0; phase ^= 1; }
@@ -338,11 +184,77 @@ __global__ void __launch_bounds__(UTHREADS, 1) bq_umma_filter_kernel(UmmaParams 
             }
             tbuf = (tbuf + 1) & (NPAR - 1);
         }
+    } else {
+        // ===== consumers: warpgroup cw owns rows [64 cw, 64 cw + 64) of every tile =====
+        const int cw = (warp >> 2) - 1, ctid = tid - 128;
+        const int rbase = 64 * cw + 16 * (warp & 3) + (lane >> 2);  // fragment rows rbase and rbase + 8
+        const int cbase = 2 * (lane & 3);                           // fragment columns 8 j + cbase (+ 1)
+        uint32_t d[128];
+#pragma unroll
+        for (int i = 0; i < 128; i++) d[i] = 0u;
+        int stage = 0, cur_qt = -1, it = 0;
+        unsigned phase = 0;
+        for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, it++) {
+            const int qt = (int)(tile / row_tiles), tbuf = it & (NPAR - 1);
+            const long long row0 = (tile % row_tiles) * UM;
+            if (qt != cur_qt) {  // the thresholds of this query tile (padding queries never pass)
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                for (int c = ctid; c < UN; c += 256) {
+                    const int q = qt * UN + c;
+                    s_t2[c] = q < P.nq ? 128 * __ldg(P.t2 + q) : INT_MIN;  // the accumulators hold 128 * dot
+                }
+                cur_qt = qt;
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+            }
+            int prev = -1;
+            for (int kc = 0; kc < P.kchunks; kc++) {
+                mbar_wait_bounded(&full[stage], phase);
+                const uint32_t a_addr = smem_u32(stage0 + stage * STAGE_BYTES) + cw * (64 / 8) * 1024, b_addr = smem_u32(stage0 + stage * STAGE_BYTES) + A_STAGE_BYTES;
+                acc_fence(d);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < UKC / 32; k++) wgmma_u8_m64n256k32(d, wgmma_desc(a_addr + 32 * k), wgmma_desc(b_addr + 32 * k), (kc | k) != 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<1>();  // the group of the previous stage has read its operands
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                prev = stage;
+                if (++stage == USTAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            acc_fence(d);
+            // the row popcounts were written before the producers' arrive on the last stage (ordered through full[] -> here);
+            // read them before that stage goes back to the producers
+            int par[2], par128[2];
+            long long rr[2];
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                rr[h] = row0 + rbase + 8 * h;
+                par[h] = s_par[tbuf * UM + rbase + 8 * h];
+                par128[h] = rr[h] < P.n ? par[h] << 7 : INT_MAX;  // rows past the end never pass
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[prev]);
+            // hd - pb = par - 2 dot <= t2  <=>  2 (128 dot) + 128 t2 >= 128 par
+#pragma unroll
+            for (int j = 0; j < UN / 8; j++) {
+                const int2 t = *reinterpret_cast<const int2 *>(s_t2 + 8 * j + cbase);
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int v = (int)d[4 * j + 2 * h + e];
+                        if (2 * v + (e ? t.y : t.x) >= par128[h]) {
+                            const int q = qt * UN + 8 * j + cbase + e;
+                            const int hd = par[h] - (v >> 6) + __ldg(P.pb + q);
+                            const long long key = topk_key(bq_score_from_hd(hd, P.dim), (int32_t)(rr[h] + P.id_base));
+                            const int pos = atomicAdd(&P.cnt[q], 1);
+                            if (pos < P.cap) P.buf[(size_t)q * P.cap + pos] = key;
+                        }
+                    }
+                }
+            }
+        }
     }
-    // teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
 }
 
 }  // namespace
@@ -376,11 +288,11 @@ cudaError_t launch_bq_umma_filter(const DataDesc &d, const uint32_t *qbits_dev, 
     P.rows = reinterpret_cast<const uint32_t *>(d.words);
     P.n = d.n; P.W32 = W32; P.dim = d.dim; P.kchunks = kchunks; P.images = images_dev; P.qtiles = qtiles; P.nq = nq; P.t2 = t2_dev; P.pb = pb_dev;
     P.buf = buf_dev; P.cnt = cnt_dev; P.cap = cap; P.id_base = id_base;
-    const size_t smem = (size_t)USTAGES * STAGE_BYTES + 256 + 2 * UN * sizeof(int) + NPAR * 2 * UM * sizeof(int) + 8 * WQ_CAP * sizeof(int2);
-    if ((e = cudaFuncSetAttribute(bq_umma_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+    const size_t smem = (size_t)USTAGES * STAGE_BYTES + 256 + UN * sizeof(int) + NPAR * UM * sizeof(int);
+    if ((e = cudaFuncSetAttribute(bq_wgmma_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
     const long long tiles = ((d.n + UM - 1) / UM) * qtiles;
     const int grid = (int)(tiles < sm_count ? tiles : sm_count);
-    bq_umma_filter_kernel<<<grid, UTHREADS, smem, s>>>(P);
+    bq_wgmma_filter_kernel<<<grid, UTHREADS, smem, s>>>(P);
     g_launches++;
     return cudaGetLastError();
 }

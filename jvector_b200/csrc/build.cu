@@ -442,53 +442,67 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
 }
 
 // ------------------------------------------------------------------------------------------------
-// prune_gram_tc_kernel: the same kernel with the Gram product on the 5th-generation tensor cores. The candidate x candidate
-// matrix is GEMM-shaped work (X X^T, X = the candidate rows), 72 % of prune_gram_kernel<128>'s time on the CUDA cores
-// (profiles/r2_build_prune.md). fp32 products are kept by the 3xTF32 split: x = hi + lo with hi = x truncated to tf32's 10
-// mantissa bits and lo = x - hi (exact), D += hi hi^T + hi lo^T + lo hi^T (the dropped lo lo^T term is 2^-22 relative), fp32
-// accumulation in TMEM. Per 32-float K chunk all 256 threads stage the rows into two K-major SWIZZLE_128B tiles (hi | lo, TILE
-// rows x 128 B each; the same tile is the A and the B operand), double buffered, and one thread issues 12
-// tcgen05.mma.kind::tf32 (M = 128, N = TILE, K = 8); the next chunk's global loads are in flight while it does. The similarity
-// matrix C overlays the staging area once the last MMA has completed. The scores against v (the sort keys) stay exact fp32.
-// For TILE = 64 the A operand still spans 128 rows (M = 128): rows 64..127 read whatever follows the tile and produce
-// accumulator rows that are never read.
+// prune_gram_tc_kernel: the same kernel with the Gram product on the tensor cores (Hopper wgmma). The candidate x candidate
+// matrix is GEMM-shaped work (X X^T, X = the candidate rows). fp32 products are kept by the 3xTF32 split: x = hi + lo with
+// hi = x truncated to tf32's 10 mantissa bits and lo = x - hi (exact), D += hi hi^T + hi lo^T + lo hi^T (the dropped lo lo^T term
+// is 2^-22 relative), fp32 accumulation in registers. Per 32-float K chunk all 256 threads stage the rows into two K-major
+// SWIZZLE_128B tiles (hi | lo, TILE rows x 128 B each; the same tile is the A and the B operand), double buffered, and each of
+// the two warpgroups issues wgmma.m64nNk8.tf32 for its half of the columns (N = TILE / 2) over the TILE / 64 row blocks; the
+// next chunk's global loads are in flight while they run. The similarity matrix C overlays the staging area once the last
+// group has completed. The scores against v (the sort keys) stay exact fp32.
 // ------------------------------------------------------------------------------------------------
 namespace tc {
 __device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr)
 {
     uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);  // start address
+    d |= (uint64_t)1 << 16;                       // leading byte offset (unused by swizzled K-major layouts)
+    d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset: 8-row atoms 1024 B apart
+    d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
     return d;
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
+// D[64][N] (+)= A[64][8] * B[N][8]^T in tf32 with fp32 accumulation. Fragment: register 4 j + 2 h + e holds row
+// 16 (warp % 4) + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.
+template <int N>
+__device__ __forceinline__ void mma_tf32(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void mma_tf32<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void commit(uint64_t *bar)
+template <>
+__device__ __forceinline__ void mma_tf32<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void wait_bounded(uint64_t *bar, unsigned parity)
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R])
 {
-    for (unsigned spins = 0; !mbar_try_wait(bar, parity); ++spins)
-        if (spins > (1u << 28)) __trap();
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 template <int TILE>
 struct Layout {
     static constexpr int TILE_BYTES = TILE * 128;                  // one operand tile: TILE rows x 32 floats
     static constexpr int STAGE_BYTES = 2 * TILE_BYTES;             // hi | lo
-    static constexpr int STAGES_END = 2 * STAGE_BYTES + (TILE < 128 ? (128 - TILE) * 128 : 0);  // + what an M = 128 A operand over-reads
+    static constexpr int STAGES_END = 2 * STAGE_BYTES;
     static constexpr int C_BYTES = (TILE * (TILE + 1) * 4 + 15) & ~15;
     static constexpr int AREA = ((STAGES_END > C_BYTES ? STAGES_END : C_BYTES) + 1023) & ~1023;
 };
@@ -502,7 +516,7 @@ static size_t gram_tc_smem_bytes(const DataDesc &d)
 }
 
 template <int METRIC, int TILE>
-__global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 3 : 4) prune_gram_tc_kernel(PruneParams P)
+__global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram_tc_kernel(PruneParams P)
 {
     using L = tc::Layout<TILE>;
     constexpr int CP = TILE + 1;
@@ -518,8 +532,6 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 3 : 4) prune_gram
     uint8_t *state = reinterpret_cast<uint8_t *>(ids + TILE);
     __shared__ float red[36];
     __shared__ int s_next;
-    __shared__ __align__(8) uint64_t mma_bar[2];
-    __shared__ uint32_t tmem_slot;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NW = PRUNE_THREADS / 32;
@@ -527,22 +539,10 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 3 : 4) prune_gram
     float alpha_max = 1.0f;
     for (float a = 1.0f; a <= P.alpha + 1e-6f; a += 0.2f) alpha_max = a;
 
-    if (tid == 0) {
-        mbar_init(&mma_bar[0], 1);
-        mbar_init(&mma_bar[1], 1);
-        mbar_fence_init();
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(TILE) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_slot;
-    // c = F32 (1) at [4,6), a = b = TF32 (2) at [7,10) / [10,13), K-major both, N >> 3 at [17,23), M >> 4 at [24,29)
-    constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TILE >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    unsigned commits0 = 0u, commits1 = 0u;  // commits issued per staging buffer so far (every thread keeps the same count)
+    // warpgroup wg computes columns [wg N, wg N + N) of every 64-row block of the Gram matrix
+    constexpr int N = TILE / 2, MB = TILE / 64, R = N / 2;
+    const int wg = warp >> 2;
+    float acc[MB][R];
     const int nchunks = (P.d.stride + 31) / 32;
     const int c4 = tid & 7, r0 = tid >> 3;
 
@@ -607,7 +607,10 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 3 : 4) prune_gram
         for (int j = 0; j < PASSES; j++) pre[j] = (rowp[j] && 4 * c4 < P.d.stride) ? __ldg(reinterpret_cast<const float4 *>(rowp[j])) : make_float4(0.f, 0.f, 0.f, 0.f);
         for (int c = 0; c < nchunks; c++) {
             const int b = c & 1;
-            if (c >= 2) tc::wait_bounded(&mma_bar[b], ((b ? commits1 : commits0) - 1u) & 1u);  // the MMAs of chunk c - 2 have read this buffer
+            if (c >= 2) {  // the MMAs of chunk c - 2 (both warpgroups) have read this buffer
+                asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+                __syncthreads();
+            }
             unsigned char *hi_t = area + b * L::STAGE_BYTES, *lo_t = hi_t + L::TILE_BYTES;
 #pragma unroll
             for (int j = 0; j < PASSES; j++) {
@@ -630,50 +633,41 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 3 : 4) prune_gram
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncthreads();
-            if (tid == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            {
                 const uint32_t ah = smem_u32(hi_t), al = smem_u32(lo_t);
 #pragma unroll
-                for (int ks = 0; ks < 4; ks++) {
-                    const uint64_t dh = tc::desc_sw128(ah + 32 * ks), dl = tc::desc_sw128(al + 32 * ks);
-                    tc::mma_tf32(tmem, dh, dh, IDESC, (c | ks) != 0 ? 1u : 0u);
-                    tc::mma_tf32(tmem, dh, dl, IDESC, 1u);
-                    tc::mma_tf32(tmem, dl, dh, IDESC, 1u);
-                }
-                tc::commit(&mma_bar[b]);
-            }
-            if (b) commits1++;
-            else commits0++;
-        }
-        if (commits0) tc::wait_bounded(&mma_bar[0], (commits0 - 1u) & 1u);
-        if (commits1) tc::wait_bounded(&mma_bar[1], (commits1 - 1u) & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        __syncthreads();  // every thread is past its waits: the staging area may now be overwritten by C
-        {
-            // TMEM -> C: warp w reads lanes 32 (w % 4) .. (its quarter of the rows) and half of the columns
-            const int quarter = warp & 3, half = warp >> 2;
-            if (quarter * 32 < TILE) {
-                const int i = quarter * 32 + lane;
-#pragma unroll 1
-                for (int cg = 0; cg < TILE / 64; cg++) {
-                    const int col0 = half * (TILE / 2) + cg * 32;
-                    uint32_t t[32];
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(t[0]), "=r"(t[1]), "=r"(t[2]), "=r"(t[3]), "=r"(t[4]), "=r"(t[5]), "=r"(t[6]), "=r"(t[7]), "=r"(t[8]), "=r"(t[9]), "=r"(t[10]),
-                          "=r"(t[11]), "=r"(t[12]), "=r"(t[13]), "=r"(t[14]), "=r"(t[15]), "=r"(t[16]), "=r"(t[17]), "=r"(t[18]), "=r"(t[19]), "=r"(t[20]),
-                          "=r"(t[21]), "=r"(t[22]), "=r"(t[23]), "=r"(t[24]), "=r"(t[25]), "=r"(t[26]), "=r"(t[27]), "=r"(t[28]), "=r"(t[29]), "=r"(t[30]),
-                          "=r"(t[31])
-                        : "r"(tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)col0));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                for (int mb = 0; mb < MB; mb++) tc::acc_fence(acc[mb]);
+                asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-                    for (int j = 0; j < 32; j++) C[i * CP + col0 + j] = __uint_as_float(t[j]);
+                for (int ks = 0; ks < 4; ks++) {
+                    const uint64_t bh = tc::desc_sw128(ah + wg * (N / 8) * 1024 + 32 * ks), bl = tc::desc_sw128(al + wg * (N / 8) * 1024 + 32 * ks);
+#pragma unroll
+                    for (int mb = 0; mb < MB; mb++) {
+                        const uint64_t dh = tc::desc_sw128(ah + mb * 8 * 1024 + 32 * ks), dl = tc::desc_sw128(al + mb * 8 * 1024 + 32 * ks);
+                        tc::mma_tf32<N>(acc[mb], dh, bh, (c | ks) != 0 ? 1u : 0u);
+                        tc::mma_tf32<N>(acc[mb], dh, bl, 1u);
+                        tc::mma_tf32<N>(acc[mb], dl, bh, 1u);
+                    }
                 }
+                asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
             }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+        for (int mb = 0; mb < MB; mb++) tc::acc_fence(acc[mb]);
+        __syncthreads();  // both warpgroups are past their waits: the staging area may now be overwritten by C
+#pragma unroll
+        for (int mb = 0; mb < MB; mb++) {
+            const int i = 64 * mb + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+            for (int j = 0; j < N / 8; j++) {
+                const int col = wg * N + 8 * j + 2 * (lane & 3);
+                C[i * CP + col] = acc[mb][4 * j];
+                C[i * CP + col + 1] = acc[mb][4 * j + 1];
+                C[(i + 8) * CP + col] = acc[mb][4 * j + 2];
+                C[(i + 8) * CP + col + 1] = acc[mb][4 * j + 3];
+            }
+        }
         __syncthreads();
         // raw dot products -> the reference's similarity scores (needs the diagonal for L2 / cosine)
         if (METRIC != JV_METRIC_DOT) {
@@ -732,9 +726,6 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 3 : 4) prune_gram
         }
         __syncthreads();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TILE) : "memory");
 }
 
 template <int TILE>
@@ -886,7 +877,7 @@ static cudaError_t launch_prune_t(const PruneParams &P, int grid, size_t smem, c
     // candidate sets that fit a tile go through the Gram-matrix kernel; anything larger keeps the incremental kernel
     const int ncmax = P.mode == 0 ? P.cand_stride + P.window : P.row_cap;
     cudaError_t e;
-    // Gram products on the tensor cores (tcgen05, 3xTF32) unless JV_PRUNE_GRAM=ffma asks for the CUDA-core kernel
+    // Gram products on the tensor cores (wgmma, 3xTF32) unless JV_PRUNE_GRAM=ffma asks for the CUDA-core kernel
     static const bool use_tc = !(getenv("JV_PRUNE_GRAM") && getenv("JV_PRUNE_GRAM")[0] == 'f');
     if (ncmax <= 64 && use_tc) {
         const size_t gs = gram_tc_smem_bytes<64>(P.d);
@@ -1030,7 +1021,7 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
 }
 
 // the next batch: 1/32 of what is already inserted, at most max_batch — every batch searches a graph that already holds 97 % of the
-// nodes a sequential build would show it. Measured on 100k rows (profiles/r2_build_quality.md): recall@10 at rerankK 100 is 0.950
+// nodes a sequential build would show it. Measured on 100k rows: recall@10 at rerankK 100 is 0.950
 // with inserted / 2, 0.9585 with / 8, 0.9624 with / 32, against 0.9631 for the reference-order (sequential) builder.
 bool builder_next_batch(GraphBuilder *B, int *first, int *count)
 {

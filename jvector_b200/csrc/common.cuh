@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for the sm_100a scoring kernels.
+// common.cuh — shared device helpers for the sm_90a scoring kernels.
 // Compiled with -fmad=false: every fused multiply-add in this library is an explicit fmaf()/__fmaf_rn(), so the
 // NVQ bit tricks and the similarity->score maps round exactly like the reference's scalar code.
 #pragma once

@@ -1,4 +1,4 @@
-// kernels.h — host-callable launchers of the sm_100a kernels (internal; the public surface is include/jvector_b200.h)
+// kernels.h — host-callable launchers of the sm_90a kernels (internal; the public surface is include/jvector_b200.h)
 #pragma once
 #include <atomic>
 #include <cuda_runtime.h>
@@ -82,7 +82,7 @@ size_t bq_imma_scratch_bytes(long long n, int nq, int W);
 // the integer-threshold path could not resolve (a Hamming bin wider than the buffer) — the caller falls back for those batches
 cudaError_t launch_bq_topk_imma(const DataDesc &d, const float *queries_dev, int nq, int k, long long id_base, void *scratch_dev,
                                 long long *keys_out_dev, int *unresolved_dev, int sm_count, cudaStream_t s);
-// ---- bq_umma.cu: the filter pass of the same pipeline on tcgen05 (kind::i8, TMEM accumulators) ----
+// ---- bq_umma.cu: the filter pass of the same pipeline on the warpgroup MMA (wgmma u8, register accumulators) ----
 bool bq_umma_supported(const DataDesc &d);
 size_t bq_umma_image_bytes(int nq, int W);
 cudaError_t launch_bq_umma_filter(const DataDesc &d, const uint32_t *qbits_dev, int nq, int nq_pad, const int *t2_dev, const int *pb_dev, long long *buf_dev,

@@ -555,7 +555,9 @@ cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *b
         if (d.kind == KIND_BQ && d.W <= 32) {
             // popcount-bound: every CTA walks a slice of the rows against ALL active queries (rows in registers, queries in smem)
             long long want = (d.n + BQF_THREADS - 1) / BQF_THREADS;
-            int gridx = (int)(want < 148 * 8 ? want : 148 * 8);
+            int dev = 0, sms = 0;
+            if ((e = cudaGetDevice(&dev)) != cudaSuccess || (e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+            int gridx = (int)(want < sms * 8LL ? want : sms * 8LL);
 #define CALLBQ(MW) topk_filter_bq_kernel<MW><<<gridx, BQF_THREADS, 0, s>>>(d, blobs_dev, blob_floats(d), active, ts.thr, ts.buf, ts.cnt, ts.cap, qlist)
             if (d.W <= 4) CALLBQ(4);
             else if (d.W <= 8) CALLBQ(8);

@@ -238,7 +238,7 @@ void nvq_shuffle_query_in_place_8bit(float *vector, size_t length)
     (void)length;
 }
 
-const char *jvector_simd_get_active_isa(void) { return "sm_100a"; }
+const char *jvector_simd_get_active_isa(void) { return "sm_90a"; }
 
 const char *jvector_simd_get_max_isa_env(void)
 {

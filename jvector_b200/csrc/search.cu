@@ -175,7 +175,7 @@ __device__ __forceinline__ void heap_down(long long *h, int size, int pos)
 #define JV_SEARCH_MINB 5
 #endif
 #ifndef JV_SEARCH_MINB_PQ
-#define JV_SEARCH_MINB_PQ 6  // tools/sweep_pq_minb.sh: 5 -> 777k q/s, 6 -> 817k, 8 -> 592k (c3, LUT in L2)
+#define JV_SEARCH_MINB_PQ 6
 #endif
 // CTA width per walking scorer. fp32 / NVQ rows are scored a warp per row and, with every new row already on its way to L2
 // (bulk prefetch), the walk gains from MORE queries in flight rather than more warps per query: 128 threads, 10 CTAs per SM
@@ -806,7 +806,7 @@ static size_t search_smem_bytes(const DataDesc &approx, const DataDesc *rerank, 
 #define JV_SEARCH_MINB_ROWS_WIDE 8
 #endif
 constexpr int MINB_DEFAULT = JV_SEARCH_MINB, MINB_PQ_LITE = JV_SEARCH_MINB_PQ, MINB_PQ_WIDE = JV_SEARCH_MINB_PQ_WIDE;
-constexpr int MINB_ROWS = JV_SEARCH_MINB_ROWS, MINB_ROWS_WIDE = JV_SEARCH_MINB_ROWS_WIDE;  // fp32 / NVQ walks (56 registers at 128 threads, 9 CTAs per SM. c2, burst: 9 x 56 registers 14.24 ms, 8 x 64 registers 13.84 ms; sustained under the 1000 W cap — what bench.py times — 14.2 ms vs 14.8 ms: 9 x 56 ships)
+constexpr int MINB_ROWS = JV_SEARCH_MINB_ROWS, MINB_ROWS_WIDE = JV_SEARCH_MINB_ROWS_WIDE;  // fp32 / NVQ walks (56 registers at 128 threads, 9 CTAs per SM)
 
 template <int KIND, int METRIC, int MINB, bool VSM>
 static cudaError_t occupancy_of(size_t smem, int *blocks_per_sm)
@@ -866,10 +866,10 @@ cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const Gr
     if (cap < rerankK) return cudaErrorInvalidValue;
     plan->list_cap = cap;
     plan->list_alloc = cap > plan->sort_pow2 ? cap : plan->sort_pow2;
-    // PQ: a LUT of M*k fp32 (96 KB at M=96) in shared memory limits residency to 2 CTAs per SM, and the walk is a latency chain
-    // (profiles/r1_search_phase_cycles.md). When five LUTs do not fit an SM's shared memory the LUT lives in an L2-resident
+    // PQ: a LUT of M*k fp32 (96 KB at M=96) in shared memory limits residency to 2 CTAs per SM, and the walk is a latency chain.
+    // When five LUTs do not fit an SM's shared memory the LUT lives in an L2-resident
     // global slice per CTA instead: residency becomes register-limited (5 CTAs per SM) and the gathers are served by L2.
-    // Measured on c3: 19.25 ms -> 13.1 ms per 10 000 queries. JV_PQ_LUT=smem|l2 overrides.
+    // JV_PQ_LUT=smem|l2 overrides.
     // Round 2: the LUT may be SPLIT — rows of the first pq_smem_m sub-spaces in shared memory, the rest in the L2 slice — which
     // trades L2 gather traffic against residency continuously (JV_PQ_LUT=smem|l2 or JV_PQ_LUT_SMEM_M=<sub-spaces> override).
     plan->blob_in_global = 0;

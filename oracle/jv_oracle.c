@@ -658,7 +658,7 @@ const char *jvo_ref_isa(void) { return REF.isa ? REF.isa() : "port"; }
  * WARP-ORDER restatements. The float sums of the path are defined up to the order of the additions (SURVEY A.2: the scalar
  * provider sums sequentially, Panama keeps 2 vector accumulators, the native library 4 Highway accumulators; the reference's
  * tests accept 1e-4). A traversal, however, is only reproducible id for id when both sides produce the SAME bits, so the
- * oracle can also evaluate every score in the one order the sm_100a kernels use (jvector_b200/csrc/scorers.cuh): elements
+ * oracle can also evaluate every score in the one order the sm_90a kernels use (jvector_b200/csrc/scorers.cuh): elements
  * dealt to 32 (fp32 rows, NVQ bytes) or 8 (PQ code rows) lane accumulators, fused multiply-adds, lanes folded by a xor
  * butterfly; block-wide sums (query norms) over 256 strided accumulators folded warp by warp. Same arithmetic, same formulas
  * (cited at each function), one fixed member of the family of orders the reference itself ships.

@@ -124,7 +124,7 @@ typedef struct {
 } jvo_search_stats;
 
 /* order 0 (default): sequential sums, or the reference's kernels after jvo_use_ref; order 1: the summation order of the
- * sm_100a kernels (32 / 8 lane accumulators + xor butterfly, see "WARP-ORDER restatements" in jv_oracle.c), which makes a
+ * sm_90a kernels (32 / 8 lane accumulators + xor butterfly, see "WARP-ORDER restatements" in jv_oracle.c), which makes a
  * traversal reproducible id for id. Same formulas either way. */
 void jvo_scorer_set_order(jvo_scorer *s, int order);
 float jvo_compare_f32_warp(int metric, const float *q, const float *row, int dim);

@@ -227,8 +227,9 @@ def read_ivecs(path):
 
 def load_siftsmall():
     d = os.path.join(GOLDEN, "siftsmall")
-    return (read_fvecs(os.path.join(d, "siftsmall_base.fvecs")), read_fvecs(os.path.join(d, "siftsmall_query.fvecs")),
-            read_ivecs(os.path.join(d, "siftsmall_groundtruth.ivecs")))
+    # SIFT descriptors are integers in [0, 255]: the base is stored as uint8 (exactly the float32 rows of siftsmall_base.fvecs)
+    base = np.load(os.path.join(d, "siftsmall_base.npz"))["base"].astype(np.float32)
+    return (base, read_fvecs(os.path.join(d, "siftsmall_query.fvecs")), read_ivecs(os.path.join(d, "siftsmall_groundtruth.ivecs")))
 
 
 KERNEL_TEST_SIZES = [1, 3, 4, 5, 7, 8, 9, 15, 16, 17, 19, 32, 33, 37, 64, 71, 100, 128, 255]  # native-c:tests/test_helpers.cpp:49-76

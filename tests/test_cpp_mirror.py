@@ -1,5 +1,5 @@
 """The C++ host mirror (include/jvector_b200.hpp) compiles against the C ABI and behaves like the reference's provider:
-on a box without an sm_100 device it fails loudly (no CPU fallback); on the GPU box it matches the oracle."""
+on a box without an sm_90 device it fails loudly (no CPU fallback); on the GPU box it matches the oracle."""
 import os
 import subprocess
 

@@ -1,6 +1,6 @@
-"""Parity tests proper: the sm_100a kernels, called through the C ABI, against the CPU oracle on the same seeded inputs.
+"""Parity tests proper: the sm_90a kernels, called through the C ABI, against the CPU oracle on the same seeded inputs.
 Bar (BASELINE.json north_star): bit-exact for BQ/Hamming, code bytes and integer top-k ordering; within 1e-5 relative
-for float32 similarity scores. Run on the B200 box: pytest -m gpu."""
+for float32 similarity scores. Run on an H100: pytest -m gpu."""
 import ctypes as C
 
 import numpy as np
@@ -264,7 +264,7 @@ def test_bq_bruteforce_tensor_core_contraction_exact(jv, oracle, dim, n, nq, k):
 
 @pytest.mark.parametrize("filter_kernel", ["umma", "imma"])
 def test_bq_bruteforce_filter_kernels_exact(jv, filter_kernel):
-    # the same top-k with the filter pass forced onto tcgen05 (kind::i8, TMEM accumulators, csrc/bq_umma.cu: the default where the
+    # the same top-k with the filter pass forced onto wgmma (u8, register accumulators, csrc/bq_umma.cu: the default where the
     # shape allows) and onto the legacy-MMA kernel (csrc/bq_imma.cu: the fallback), each in its own process
     import os
     import subprocess

@@ -309,17 +309,23 @@ def test_scorer_contexts_port_equals_ref(oracle, ref):
     for i in range(n):
         oracle.jvo_nvq_encode(fp(data[i]), fp(mean), dim, nsub, 1, fp(params[i]), bp(bys[i]))
     q = o.random_unit_vectors(rng, 1, dim)[0]
-    res = {}
-    for use_ref in (False, True):
+    def scores(use_ref):
         assert oracle.jvo_use_ref(o.REF_SO.encode() if use_ref else None) == 0
-        for metric in (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE):
-            ctxs = {"f32": oracle.jvo_scorer_f32(metric, fp(data), n, dim, fp(q)),
-                    "pq": oracle.jvo_scorer_pq(metric, fp(cb), M, k, dim, None, bp(codes), n, fp(q)),
-                    "nvq": oracle.jvo_scorer_nvq(metric, fp(mean), dim, nsub, fp(params), bp(bys), n, fp(q))}
-            for name, c in ctxs.items():
-                res[(use_ref, metric, name)] = np.array([oracle.jvo_scorer_score(c, i) for i in range(n)], np.float32)
+        out = np.empty((3, 3, n), np.float32)
+        for mi, metric in enumerate((o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)):
+            ctxs = (oracle.jvo_scorer_f32(metric, fp(data), n, dim, fp(q)),
+                    oracle.jvo_scorer_pq(metric, fp(cb), M, k, dim, None, bp(codes), n, fp(q)),
+                    oracle.jvo_scorer_nvq(metric, fp(mean), dim, nsub, fp(params), bp(bys), n, fp(q)))
+            for ci, c in enumerate(ctxs):
+                out[mi, ci] = [oracle.jvo_scorer_score(c, i) for i in range(n)]
                 oracle.jvo_scorer_free(c)
-    oracle.jvo_use_ref(None)
+        oracle.jvo_use_ref(None)
+        return out
+
+    # the scorer contexts driving the reference's kernels (their answers replayed where the reference library is absent)
+    both = (scores(False), ref.capture("scorer_contexts_on_ref", lambda: scores(True)))
+    res = {(use_ref, metric, name): both[use_ref][mi, ci] for use_ref in (False, True)
+           for mi, metric in enumerate((o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)) for ci, name in enumerate(("f32", "pq", "nvq"))}
     for metric in (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE):
         for name in ("f32", "pq", "nvq"):
             np.testing.assert_allclose(res[(False, metric, name)], res[(True, metric, name)], rtol=1e-5, atol=1e-6)

@@ -1,5 +1,5 @@
-"""Run by tests/test_gpu_parity.py::test_bq_bruteforce_filter_kernels_exact (argument: umma | imma) in a SUBPROCESS (a faulting tcgen05 pipeline traps and
-poisons the CUDA context; it must not take the other tests with it): BQ top-k with the filter pass on tcgen05 (JV_BQ_FILTER=umma)
+"""Run by tests/test_gpu_parity.py::test_bq_bruteforce_filter_kernels_exact (argument: umma | imma) in a SUBPROCESS (a faulting wgmma pipeline traps and
+poisons the CUDA context; it must not take the other tests with it): BQ top-k with the filter pass on wgmma (JV_BQ_FILTER=umma)
 against the oracle's scalar popcount restatement, bit for bit."""
 import os
 import sys

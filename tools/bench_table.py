@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Turn bench.py JSON lines (the b200 arm and, optionally, the reference arm) into the markdown table kept in profiles/.
+"""Turn bench.py JSON lines (the b200 arm and, optionally, the reference arm) into a markdown table.
 usage: tools/bench_table.py <b200.json> [reference.json]"""
 import json
 import sys

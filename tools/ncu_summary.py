@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (raw page + SASS source page) into markdown for profiles/.
+"""Summarise an .ncu-rep (raw page + SASS source page) into markdown.
 usage: tools/ncu_summary.py <rep> <title> [algorithmic_bytes]   (NCU_INDEX=i picks the i-th profiled launch of the report, default 0)"""
 import csv
 import io
