@@ -14,7 +14,8 @@
 //     does not take, and for the re-run of a query that outgrew it — an open-addressing table of 32-bit ids in a per-CTA slice
 //     of global scratch (visited_insert).
 // Every hop is: read one adjacency row (FusedPQ: one record) -> filter through visited, requesting every new row from DRAM
-// with one bulk L2 prefetch -> score the survivors with the row scorers of scorers.cuh -> parallel rank-merge into the list.
+// with one bulk L2 prefetch (not for fp32 batches that fill the GPU, see launch_search) -> score the survivors with the row
+// scorers of scorers.cuh -> parallel rank-merge into the list.
 #include <limits.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -64,6 +65,7 @@ struct SearchParams {
     int early_pf;      // request the adjacency / FusedPQ record of a new candidate that lands among the next two pops at score time
     int pq_rows;       // PQ walk: lane = candidate, warp = partial sum (score_pq_partial) instead of an 8-lane group per candidate
     int row_prefetch;  // fp32 / NVQ walks: 1 = a bulk L2 prefetch of every newly visited row is issued by the thread that discovered it
+                       // (fp32: only for a batch that does not fill the GPU)
     unsigned long long *dbg;  // JV_SEARCH_PROFILE builds only: per-phase cycle totals
 };
 
@@ -1032,7 +1034,10 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     P.vis_slots_log = plan.vis_slots_log;
     P.vis_rlog = plan.vis_rlog;
     P.vis_idmask = plan.vis_idmask;
-    P.row_prefetch = plan.row_prefetch;
+    // fp32: only a batch that does not fill the GPU (latency bound, L2 to spare) prefetches its rows. A full batch would keep up to
+    // 9 CTAs x 28 rows x 3 KB per SM waiting in L2, twice an H100 SM's ~380 KB share: rows were evicted before their demand load and
+    // read from DRAM twice (c2: 35.2 ms with the prefetch, 30.7 ms without)
+    P.row_prefetch = (approx.kind == KIND_F32 && nq > plan.ctas) ? 0 : plan.row_prefetch;
     P.pq_rows = plan.pq_rows;
     {
         // on for the latency-bound walks (PQ / BQ: c3 12.0 -> 11.5 ms); off where HBM is already saturated and a wasted adjacency
