@@ -117,7 +117,9 @@ JV_API int jv_dataset_register_bq(const uint64_t *words, int64_t n, int dim, jv_
 JV_API int jv_dataset_register_nvq(const uint8_t *bytes, const float *params, int64_t n, int dim, int nsub,
                                    const float *mean, jv_dataset *out);
 /* rows already in HBM on the calling thread's device (e.g. produced by another kernel): BORROWED, not copied — the caller keeps
- * them alive until jv_dataset_free. 16-byte aligned, row_stride = dim rounded up to 4 floats, padding floats zero. */
+ * them alive and UNCHANGED until jv_dataset_free. 16-byte aligned, row_stride = dim rounded up to 4 floats, padding floats zero.
+ * (A graph searched over them assumes unchanged rows already; so does the row sketch that the first DOT_PRODUCT graph search of a
+ * batch larger than the GPU's resident CTAs derives from them: int8 codes + 8 bytes per row, built once, freed with the handle.) */
 JV_API int jv_dataset_adopt_f32_device(const float *rows_device, int64_t n, int dim, int row_stride, jv_dataset *out);
 JV_API int jv_dataset_device(jv_dataset ds);
 /* ImmutablePQVectors' code-vs-code scoring (base:quantization/ImmutablePQVectors.java:63-105): build the triangular

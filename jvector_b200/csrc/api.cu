@@ -158,6 +158,12 @@ struct jv_dataset_s {
     DataDesc d;
     std::vector<void *> allocs;
     size_t bytes = 0;
+    // fp32 row sketch (row_sketch_kernel): built by the first search that can use it (search_device), freed with the data set.
+    // Not part of `d`: only the search kernel's fp32 DOT walks read it, the builder and the batch scorers never see it
+    int8_t *sketch = nullptr;
+    float2 *sketch_meta = nullptr;
+    bool sketch_failed = false;  // the allocation failed once: walk without it from then on
+    std::mutex sketch_mu;
     int alloc(void **p, size_t n)
     {
         CK(cudaMalloc(p, n ? n : 16), "cudaMalloc(dataset)");
@@ -168,6 +174,8 @@ struct jv_dataset_s {
     ~jv_dataset_s()
     {
         for (void *p : allocs) cudaFree(p);
+        cudaFree(sketch);
+        cudaFree(sketch_meta);
     }
 };
 
@@ -1068,6 +1076,32 @@ int jv_graph_download(jv_graph g, int level, int32_t *node_ids_out, int32_t *adj
     return JV_OK;
 }
 
+// the fp32 row sketch of a data set (row_sketch_kernel), built once. Complete when this returns: another thread's stream may read it
+static int ensure_sketch(jv_dataset ds, cudaStream_t s)
+{
+    std::lock_guard<std::mutex> lk(ds->sketch_mu);
+    if (ds->sketch || ds->sketch_failed) return JV_OK;
+    const int ss = (ds->d.stride + 7) & ~7;
+    int8_t *sk = nullptr;
+    float2 *meta = nullptr;
+    if (cudaMalloc(&sk, (size_t)ds->d.n * ss) != cudaSuccess || cudaMalloc(&meta, (size_t)ds->d.n * sizeof(float2)) != cudaSuccess) {
+        cudaGetLastError();  // out of memory: not an error of the search, which walks without the sketch
+        cudaFree(sk);
+        ds->sketch_failed = true;
+        return JV_OK;
+    }
+    cudaError_t e = launch_row_sketch(ds->d.rows, ds->d.n, ds->d.stride, ss, sk, meta, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        cudaFree(sk);
+        cudaFree(meta);
+        CK(e, "row_sketch");
+    }
+    ds->sketch = sk;
+    ds->sketch_meta = meta;
+    return JV_OK;
+}
+
 static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int metric, const float *queries_dev, int nq, int topK, int rerankK,
                          const SearchFilter *filter, int32_t *nodes_dev, float *scores_dev, jv_search_stats *stats)
 {
@@ -1091,6 +1125,16 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
     const char *lcap_env = getenv("JV_LIST_CAP");
     const int cap_hint = cap_env ? atoi(cap_env) : 0, lcap_hint = lcap_env ? atoi(lcap_env) : 0;
     CK(plan_search(approx->d, rr, g->g, topK, rerankK, nq, cap_hint > 0 ? cap_hint : 0, lcap_hint > 0 ? lcap_hint : 0, g_sm_count, &plan), "plan_search");
+    // An fp32 DOT walk of a batch that fills the GPU drops hopeless neighbours on a bound from the row sketch (launch_search): the
+    // first such batch builds the sketch. Without it (the allocation failed) the walk reads every full row, with the same answers.
+    DataDesc ad = approx->d;
+    if (ad.kind == KIND_F32 && metric == JV_METRIC_DOT && nq > plan.ctas && (rc = ensure_sketch(approx, s))) return rc;
+    if (ad.kind == KIND_F32) {
+        std::lock_guard<std::mutex> lk(approx->sketch_mu);
+        ad.sketch = approx->sketch;
+        ad.sketch_meta = approx->sketch_meta;
+        ad.sketch_stride = (ad.stride + 7) & ~7;
+    }
     const size_t aux = sizeof(SearchCounters) + 64 + (size_t)nq + (size_t)nq * 4 + 64;
     if ((rc = t_ctx.ensure(5, search_scratch_bytes(plan))) || (rc = t_ctx.ensure(3, aux))) return rc;
     char *a = (char *)t_ctx.dbuf[3];
@@ -1100,7 +1144,7 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
     int32_t *dindex = (int32_t *)(a + sizeof(SearchCounters) + 64 + (((size_t)nq + 63) & ~(size_t)63));
     CK(cudaMemsetAsync(dcnt, 0, sizeof(SearchCounters), s), "memset counters");
     CK(cudaEventRecord(t_ctx.ev0, s), "event");
-    CK(launch_search(g->g, approx->d, rr, metric, queries_dev, nq, topK, rerankK, plan, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover, nullptr, 0, filter, s),
+    CK(launch_search(g->g, ad, rr, metric, queries_dev, nq, topK, rerankK, plan, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover, nullptr, 0, filter, s),
        "launch_search");
     CK(cudaEventRecord(t_ctx.ev1, s), "event");
     SearchCounters hc;
@@ -1137,7 +1181,7 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         unsigned long long zero = 0;
         CK(cudaMemcpyAsync(&dcnt->overflowed, &zero, sizeof(zero), cudaMemcpyHostToDevice, s), "reset overflow");
         CK(cudaEventRecord(t_ctx.ev0, s), "event");
-        CK(launch_search(g->g, approx->d, rr, metric, queries_dev, (int)idx.size(), topK, rerankK, p2, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover,
+        CK(launch_search(g->g, ad, rr, metric, queries_dev, (int)idx.size(), topK, rerankK, p2, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover,
                          dindex, 0, filter, s),
            "launch_search(retry)");
         CK(cudaEventRecord(t_ctx.ev1, s), "event");

@@ -66,6 +66,8 @@ cudaError_t launch_topk_merge(const long long *keys_in_dev, int nq, int parts, i
 // the same for keys laid out [parts][nq][k] (shard-major, what peer copies / all_gather produce)
 cudaError_t launch_topk_merge_strided(const long long *keys_in_dev, int nq, int parts, int k, long long *keys_out_dev, cudaStream_t s);
 
+// int8 row sketch + {scale, radius} per row of an fp32 data set (the search kernel's sketch bound, see sketch_bound_pair)
+cudaError_t launch_row_sketch(const float *rows_dev, long long n, int stride, int sketch_stride, int8_t *sketch_dev, float2 *meta_dev, cudaStream_t s);
 cudaError_t launch_bq_encode(const float *rows_dev, long long n, int dim, int row_stride, unsigned long long *words_dev, cudaStream_t s);
 cudaError_t launch_pq_encode(const DataDesc &pq, const float *rows_dev, long long n, int row_stride, uint8_t *codes_dev, cudaStream_t s);
 cudaError_t launch_pq_self_magnitudes(const DataDesc &pq, float *mag_dev, cudaStream_t s);

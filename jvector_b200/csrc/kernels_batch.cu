@@ -729,6 +729,52 @@ cudaError_t launch_bq_encode(const float *rows_dev, long long n, int dim, int ro
     return cudaGetLastError();
 }
 
+// Row sketch of an fp32 data set (the bound of sketch_bound_pair, scorers.cuh): one warp per row. s = max|x| / 127, codes
+// round(x / s) in [-127, 127] (all 0 for a zero row), x_hat = s c. The radius r = ||x - x_hat|| + gamma (||x|| + ||x_hat||),
+// gamma = (stride + 8) 2^-23, is summed in fp64 rounding every step upward (x - x_hat itself is exact in fp64) and rounded up to
+// fp32. Padding codes up to sketch_stride are zero.
+__global__ void __launch_bounds__(256) row_sketch_kernel(const float *__restrict__ rows, long long n, int stride, int sketch_stride, int8_t *__restrict__ sketch,
+                                                         float2 *__restrict__ meta)
+{
+    const long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n) return;
+    const float *x = rows + r * stride;
+    float m = 0.f;
+    for (int i = lane; i < stride; i += 32) m = fmaxf(m, fabsf(x[i]));
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(FULL, m, o));
+    const float s = __fdiv_rn(m, 127.0f);
+    double dd = 0.0, xx = 0.0, hh = 0.0;
+    for (int i = lane; i < sketch_stride; i += 32) {
+        const float v = i < stride ? x[i] : 0.f;
+        const int c = s > 0.f ? min(127, max(-127, __float2int_rn(__fdiv_rn(v, s)))) : 0;
+        sketch[r * sketch_stride + i] = (int8_t)c;
+        const double xh = (double)c * (double)s, df = (double)v - xh;
+        dd = __dadd_ru(dd, __dmul_ru(df, df));
+        xx = __dadd_ru(xx, __dmul_ru((double)v, (double)v));
+        hh = __dadd_ru(hh, __dmul_ru(xh, xh));
+    }
+    for (int o = 16; o; o >>= 1) {
+        dd = __dadd_ru(dd, __shfl_xor_sync(FULL, dd, o));
+        xx = __dadd_ru(xx, __shfl_xor_sync(FULL, xx, o));
+        hh = __dadd_ru(hh, __shfl_xor_sync(FULL, hh, o));
+    }
+    if (lane == 0) {
+        const double gamma = (double)(stride + 8) * 0x1p-23;
+        const double rad = __dadd_ru(__dsqrt_ru(dd), __dmul_ru(gamma, __dadd_ru(__dsqrt_ru(xx), __dsqrt_ru(hh))));
+        meta[r] = make_float2(s, __double2float_ru(rad));
+    }
+}
+
+cudaError_t launch_row_sketch(const float *rows_dev, long long n, int stride, int sketch_stride, int8_t *sketch_dev, float2 *meta_dev, cudaStream_t s)
+{
+    if (n <= 0) return cudaSuccess;
+    const long long blocks = (n * 32 + 255) / 256;
+    row_sketch_kernel<<<(unsigned)blocks, 256, 0, s>>>(rows_dev, n, stride, sketch_stride, sketch_dev, meta_dev);
+    g_launches++;
+    return cudaGetLastError();
+}
+
 // ProductQuantization.encode (ProductQuantization.java:507-520): code[m] = argmin_c ||v[off_m..] - centroid_{m,c}||^2, first
 // minimum wins. One warp per (row, subspace); lanes stride over the k centroids, then an arg-min shuffle that prefers
 // the smaller index on ties.

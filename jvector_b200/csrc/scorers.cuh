@@ -22,6 +22,12 @@ struct DataDesc {
     // f32: rows [n][stride] fp32, stride = dim rounded up to 4, zero padded
     const float *rows;
     int stride;
+    // f32 row sketch (row_sketch_kernel): [n][sketch_stride] int8 codes round(x / s), s = max|x| / 127 (sketch_stride = stride
+    // rounded up to 8, zero padded) and [n] {s, radius}. Set only for the search kernel's fp32 DOT walks that fill the GPU (api.cu,
+    // search.cu); nullptr elsewhere
+    const int8_t *sketch;
+    const float2 *sketch_meta;
+    int sketch_stride;
     // pq: codes [n][code_stride] u8 (code_stride = M rounded up to 4), codebooks concatenated, codebook m at k*sub_offsets[m]
     const uint8_t *codes;
     int M, k, code_stride;
@@ -95,7 +101,13 @@ __device__ inline void prepare_blob(const DataDesc &d, int metric, const float *
             acc = fmaf(v, v, acc);
         }
         float qn = block_sum(acc, red);
-        if (tid == 0) { blob[d.stride] = qn; blob[d.stride + 1] = 0.f; blob[d.stride + 2] = 0.f; blob[d.stride + 3] = 0.f; }
+        // blob[stride + 1] = an upper bound of ||q|| for the row-sketch bound (sketch_bound_pair): qn is q . q summed in fp32, within
+        // gamma = (stride + 8) 2^-23 relative (any order of depth < stride + 8) plus what underflow can drop, (stride + 512) 2^-149
+        if (tid == 0) {
+            const float kq = __fmul_rn((float)(d.stride + 512), 0x1p-149f);
+            const float g2 = __fadd_rn(1.0f, __fmul_rn((float)(d.stride + 8), 0x1p-22f));  // 1 + 2 gamma, exact
+            blob[d.stride] = qn; blob[d.stride + 1] = __fsqrt_ru(__fmul_ru(__fadd_ru(qn, kq), g2)); blob[d.stride + 2] = 0.f; blob[d.stride + 3] = 0.f;
+        }
     } else if (d.kind == KIND_PQ) {
         // LUT[m*k + c] = metric(centroid_{m,c}, q'[off_m..]) — PQDecoder.java:48-53, DefaultVectorUtilSupport.java:351-365.
         // One warp per sub-space m (its sizes / offset / query fragment are warp-uniform), lanes stride over the k centroids:
@@ -255,6 +267,46 @@ __device__ __forceinline__ void score_f32_pair(const DataDesc &d, const float *b
     }
     outA = score_map(METRIC, sa);
     outB = score_map(METRIC, sb);
+}
+
+// Upper bounds of the DOT_PRODUCT scores score_f32 would give two rows, from their int8 sketches (row_sketch_kernel) at a quarter
+// of the bytes. With c the codes as fp32, s_c = fl(q . c) in any order, x_hat = s c, gamma = (stride + 8) 2^-23 (the relative error
+// bound of an fp32 sum of depth < stride + 8, met by this sum and by score_f32's) and kd = (stride + 512) 2^-149 (what underflow can
+// add to one such sum):
+//   fl(q . x) <= q . x + gamma ||q|| ||x|| + kd = q . x_hat + q . (x - x_hat) + gamma ||q|| ||x|| + kd
+//             <= s s_c + ||q|| (||x - x_hat|| + gamma (||x|| + ||x_hat||)) + kd (1 + s) = s s_c + ||q|| r + kd (1 + s),
+// evaluated rounding upward; score_map is monotone, so the bound survives it. blob[stride + 1] is ||q|| rounded up (prepare_blob).
+// Both rows' loads are in flight before either reduction, as in score_f32_pair.
+__device__ __forceinline__ void sketch_bound_pair(const DataDesc &d, const float *blob, int nodeA, int nodeB, int lane, float &outA, float &outB)
+{
+    const uint2 *ra = reinterpret_cast<const uint2 *>(d.sketch + (size_t)nodeA * d.sketch_stride);
+    const uint2 *rb = reinterpret_cast<const uint2 *>(d.sketch + (size_t)nodeB * d.sketch_stride);
+    const float2 ma = __ldg(d.sketch_meta + nodeA), mb = __ldg(d.sketch_meta + nodeB);  // {s, r}
+    const float4 *q4 = reinterpret_cast<const float4 *>(blob);
+    const int n8 = d.sketch_stride >> 3;  // 8 codes per load; a stride of 8 m + 4 ends in 4 padding codes, read against q = 0
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
+#pragma unroll 3
+    for (int i = lane; i < n8; i += 32) {
+        const uint2 x = ldg_stream_u2(ra + i);
+        const uint2 y = ldg_stream_u2(rb + i);
+        const float4 qa = q4[2 * i], qb = 8 * i + 4 < d.stride ? q4[2 * i + 1] : z4;
+        const float q[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+#pragma unroll
+        for (int j = 0; j < 8; j += 2) {
+            const unsigned wx = j < 4 ? x.x : x.y, wy = j < 4 ? y.x : y.y;
+            const int sh = 8 * (j & 3);
+            a0 = fmaf(q[j], (float)(int8_t)(wx >> sh), a0); a1 = fmaf(q[j + 1], (float)(int8_t)(wx >> (sh + 8)), a1);
+            b0 = fmaf(q[j], (float)(int8_t)(wy >> sh), b0); b1 = fmaf(q[j + 1], (float)(int8_t)(wy >> (sh + 8)), b1);
+        }
+    }
+    const float sa = group_sum<32>(a0 + a1), sb = group_sum<32>(b0 + b1);
+    const float qn = blob[d.stride + 1];
+    const float kd = __fmul_rn((float)(d.stride + 512), 0x1p-149f);
+    const float ua = __fadd_ru(__fmaf_ru(qn, ma.y, __fmul_ru(sa, ma.x)), __fmaf_ru(kd, ma.x, kd));
+    const float ub = __fadd_ru(__fmaf_ru(qn, mb.y, __fmul_ru(sb, mb.x)), __fmaf_ru(kd, mb.x, kd));
+    outA = score_map(JV_METRIC_DOT, ua);
+    outB = score_map(JV_METRIC_DOT, ub);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -200,6 +200,30 @@ static int search_threads_of(int kind) { return (kind == KIND_F32 || kind == KIN
 #define JV_ACC(slot, a, b)
 #endif
 
+// optional drop statistics of the fp32 DOT walk (tools/row_bound_stats.py: build with -DJV_ROW_BOUND_STATS); compiled out of the
+// product build. [0] level-0 rows scored, [1] of them dropped by JV_EMIT against a full list; plus a 1-in-64 sample of the drops
+// as {query, row, key of the list's last entry}
+#ifdef JV_ROW_BOUND_STATS
+constexpr int RBS_CAP = 1 << 20;
+struct RbsSample { int32_t q, row; long long last_key; };
+__device__ unsigned long long g_rbs_count[3];  // scored, dropped, samples taken
+__device__ RbsSample g_rbs_sample[RBS_CAP];
+#define JV_RBS_SCORED(n_) do { if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0) atomicAdd(&g_rbs_count[0], (unsigned long long)(n_)); } while (0)
+#define JV_RBS_DROP(f_)                                                                                                       \
+    do {                                                                                                                      \
+        if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0) {                                                        \
+            atomicAdd(&g_rbs_count[1], 1ull);                                                                                 \
+            if ((((unsigned)(f_) * 2654435761u) ^ ((unsigned)qi * 40503u)) % 64u == 0u) {                                     \
+                const unsigned long long k_ = atomicAdd(&g_rbs_count[2], 1ull);                                               \
+                if (k_ < RBS_CAP) g_rbs_sample[k_] = RbsSample{qi, (f_), cur[LC - 1]};                                        \
+            }                                                                                                                 \
+        }                                                                                                                     \
+    } while (0)
+#else
+#define JV_RBS_SCORED(n_)
+#define JV_RBS_DROP(f_)
+#endif
+
 // flags of a list entry
 constexpr uint8_t F_EXPANDED = 1;  // popped from the candidate queue at this level
 constexpr uint8_t F_ACCEPTED = 2;  // acceptOrds.get(node) && score >= threshold (what addTopCandidate requires at level 0)
@@ -473,22 +497,49 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
             if (KIND == KIND_PQ && P.g.fused) bulk_prefetch_l2(P.g.fused + (size_t)(f_) * P.g.fused_rec, (unsigned)P.g.fused_rec);  \
             else prefetch_l2(P.g.adj0 + (size_t)(f_) * degree);                                                                     \
         }                                                                                                                           \
-        if (dead < 0 && size == LC && key_ < cur[LC - 1]) atomicMax(&s_drop[sel], float_to_sortable(sc_));                          \
-        else {                                                                                                                      \
+        if (dead < 0 && size == LC && key_ < cur[LC - 1]) {                                                                         \
+            JV_RBS_DROP(f_);                                                                                                        \
+            atomicMax(&s_drop[sel], float_to_sortable(sc_));                                                                        \
+        } else {                                                                                                                    \
             const int m_ = atomicAdd(&s_m, 1);                                                                                      \
             cand_keys[m_] = key_;                                                                                                   \
             if (P.filtered) cand_acc[m_] = ((!acc || ((acc[(f_) >> 5] >> ((f_) & 31)) & 1u)) && (sc_) >= P.threshold) ? F_ACCEPTED : 0; \
         }                                                                                                                           \
     } while (0)
                 if (KIND == KIND_F32) {
+                    // DOT walk with a full list and a row sketch (launch_search): a row whose score's upper bound from its sketch
+                    // (half the bytes) already falls under the list's last key would be dropped by JV_EMIT whatever its exact score,
+                    // so it is dropped on the bound, which also stands in for its score in s_drop (>= the exact one: the check after
+                    // the merge stays conservative). Only the others read their full rows, scored exactly as below.
+                    const bool sketched = METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && P.approx.sketch != nullptr;
                     // two rows per warp at a time: twice the loads in flight, query fragment read once
                     for (int i = group; i < n; i += 2 * NG) {
                         const int32_t fa = cand_ids[i];
                         const bool two = i + NG < n;
                         const int32_t fb = two ? cand_ids[i + NG] : fa;
+                        bool xa = true, xb = two;  // exact score needed
+                        if (sketched) {
+                            float ua, ub;
+                            sketch_bound_pair(P.approx, blobA, fa, fb, lane, ua, ub);
+                            const long long last = cur[LC - 1];
+                            xa = !(topk_key(ua, fa) < last);
+                            xb = two && !(topk_key(ub, fb) < last);
+                            if (lane == 0) {
+                                if (!xa) atomicMax(&s_drop[sel], float_to_sortable(ua));
+                                if (two && !xb) atomicMax(&s_drop[sel], float_to_sortable(ub));
+                            }
+                            if (!xa && !xb) continue;
+                            if (!xa || !xb) {
+                                const int32_t f = xa ? fa : fb;
+                                const float sc = score_f32<METRIC>(P.approx, blobA, f, lane);
+                                if (lane == 0) JV_EMIT(sc, f);
+                                continue;
+                            }
+                        }
                         float sa, sb;
                         score_f32_pair<METRIC>(P.approx, blobA, fa, fb, lane, sa, sb);
                         if (lane == 0) {
+                            JV_RBS_SCORED(two ? 2 : 1);
                             JV_EMIT(sa, fa);
                             if (two) JV_EMIT(sb, fb);
                         }
@@ -1038,6 +1089,15 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     // 9 CTAs x 28 rows x 3 KB per SM waiting in L2, twice an H100 SM's ~380 KB share: rows were evicted before their demand load and
     // read from DRAM twice (c2: 35.2 ms with the prefetch, 30.7 ms without)
     P.row_prefetch = (approx.kind == KIND_F32 && nq > plan.ctas) ? 0 : plan.row_prefetch;
+    // The same batches, when they are DOT walks, drop hopeless neighbours on the bound of their row sketch (sketch_bound_pair) where
+    // the caller passes one: HBM bound, half the bytes per dropped row. A latency-bound batch reads the rows it prefetched anyway.
+    if (!(approx.kind == KIND_F32 && metric == JV_METRIC_DOT && nq > plan.ctas)) {
+        P.approx.sketch = nullptr;
+        P.approx.sketch_meta = nullptr;
+    }
+#ifdef JV_ROW_BOUND_STATS
+    P.approx.sketch = nullptr;  // the drop statistics describe the walk that reads every row
+#endif
     P.pq_rows = plan.pq_rows;
     {
         // on for the latency-bound walks (PQ / BQ: c3 12.0 -> 11.5 ms); off where HBM is already saturated and a wasted adjacency
@@ -1057,9 +1117,15 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     cudaMemsetAsync(dbg_dev, 0, 8 * sizeof(unsigned long long), s);
     P.dbg = dbg_dev;
 #endif
+#ifdef JV_ROW_BOUND_STATS
+    {
+        const unsigned long long z[3] = {0, 0, 0};
+        cudaMemcpyToSymbolAsync(g_rbs_count, z, sizeof(z), 0, cudaMemcpyHostToDevice, s);
+    }
+#endif
     cudaError_t e = cudaMemsetAsync(work_counter_dev, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
-#define CALL(K, M, B, V)                                                                                                              \
+#define CALL(K, M, B, V)                                                                                                            \
     do {                                                                                                                              \
         e = cudaFuncSetAttribute(graph_search_kernel<K, M, B, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
         if (e == cudaSuccess) graph_search_kernel<K, M, B, V><<<plan.ctas, SearchThreads<K>::value, plan.smem_bytes, s>>>(P);               \
@@ -1076,6 +1142,23 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
         const double it = h[5] ? (double)h[5] : 1.0, nqd = (double)nq;
         fprintf(stderr, "[search profile] kind=%d nq=%d iterations/q=%.1f scored/it=%.1f cycles/it: gather=%.0f score=%.0f merge=%.0f | per query: prepare+clear=%.0f rerank+out=%.0f total=%.0f\n",
                 approx.kind, nq, it / nqd, (double)h[6] / it, (double)h[1] / it, (double)h[2] / it, (double)h[3] / it, (double)h[0] / nqd, (double)h[4] / nqd, (double)h[7] / nqd);
+    }
+#endif
+#ifdef JV_ROW_BOUND_STATS
+    // one record per launch appended to $JV_ROW_BOUND_STATS_OUT: u64 scored, dropped, samples; then the samples (16 B each)
+    if (const char *out = getenv("JV_ROW_BOUND_STATS_OUT")) {
+        unsigned long long c[3];
+        cudaStreamSynchronize(s);
+        cudaMemcpyFromSymbol(c, g_rbs_count, sizeof(c));
+        if (c[2] > (unsigned long long)RBS_CAP) c[2] = RBS_CAP;
+        RbsSample *h = (RbsSample *)malloc(sizeof(RbsSample) * (c[2] ? c[2] : 1));
+        cudaMemcpyFromSymbol(h, g_rbs_sample, sizeof(RbsSample) * c[2]);
+        if (FILE *f = fopen(out, "ab")) {
+            fwrite(c, sizeof(c), 1, f);
+            fwrite(h, sizeof(RbsSample), c[2], f);
+            fclose(f);
+        }
+        free(h);
     }
 #endif
     return cudaGetLastError();
