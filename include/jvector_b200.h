@@ -320,6 +320,30 @@ JV_API int jv_builder_free(jv_builder b);
 /* counters of this thread's last jv_graph_build (level 0): vectors scored by the insert searches, batches, back-links dropped */
 JV_API int jv_graph_build_stats(int64_t *scored_vectors, int64_t *batches, int64_t *dropped_backlinks);
 
+/* GraphIndexBuilder.removeDeletedNodes (base:graph/GraphIndexBuilder.java:689-799) on the device: the nodes set in deleted_bits
+ * are taken out of every level, and every live row that named one of them is re-pruned (retainDiverse at `alpha`, exact fp32
+ * scores over `f32`, which must be the graph's own rows) over its live neighbours and the live neighbours of its deleted ones.
+ * A row whose deleted neighbours offer no live candidate tries 2 * degree random live members of its level instead; the
+ * generator is a fixed function of (seed, level, node, attempt), so the result is reproducible. Rows that named no deleted node
+ * are copied unchanged.
+ * The result is a NEW graph (`g` is not modified; searches holding it keep a consistent snapshot) without FusedPQ records.
+ * Removed ids stay as holes: their level-0 rows are -1, they belong to no upper level, no row names them, and the new graph
+ * remembers them (a later removal counts them as gone). If the entry node is deleted, the new entry is the lowest live id of the
+ * highest level that keeps a live member, and emptied levels above it are dropped. With every node deleted the graph has entry
+ * -1 and one level; searching it returns -1 / 0 padded results. Degrees above 64 are JV_ERR_UNSUPPORTED. */
+typedef struct {
+    int32_t live_nodes;       /* level-0 nodes left (graph.size(0) after the call) */
+    int32_t removed;          /* nodes removed by this call */
+    int64_t repaired_rows;    /* rows (all levels) that lost a neighbour and were re-pruned */
+    int64_t candidates;       /* distinct candidates scored, summed over the repaired rows */
+    int32_t max_candidates;   /* largest candidate set of one row */
+    int64_t random_fallbacks; /* rows whose deleted neighbours offered no live candidate */
+    double device_ms;
+} jv_remove_stats;
+JV_API int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha, uint64_t seed,
+                                   const uint32_t *deleted_bits /* host, bit (node & 31) of word (node >> 5) */,
+                                   jv_graph *out, jv_remove_stats *stats);
+
 /* device-memory helpers for callers that keep queries/results in HBM (bench `value` leg) */
 JV_API int jv_device_malloc(void **out, size_t bytes);
 JV_API int jv_device_free(void *p);

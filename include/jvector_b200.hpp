@@ -166,7 +166,18 @@ public:
         check(jv_graph_build(v.handle(), (int)vsf_, &p_, &g, &deviceMs));
         return GraphIndex(g);
     }
+    /// markNodeDeleted + removeDeletedNodes (GraphIndexBuilder.java:678-799): a NEW graph without the nodes whose bit is set in
+    /// deletedBits (bit node & 31 of word node >> 5), their neighbours' lists repaired on the device; `graph` is left as it is.
+    /// Until then, search the marked graph with acceptOrds excluding them. Counters go to removeStats.
+    GraphIndex removeDeletedNodes(const GraphIndex &graph, const F32Vectors &v, const std::vector<uint32_t> &deletedBits)
+    {
+        if ((int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "removeDeletedNodes: deletedBits shorter than the graph");
+        jv_graph g = nullptr;
+        check(jv_graph_remove_deleted(graph.handle(), v.handle(), (int)vsf_, p_.alpha, p_.seed, deletedBits.data(), &g, &removeStats));
+        return GraphIndex(g);
+    }
     double deviceMs = 0;
+    jv_remove_stats removeStats = {};
 
 private:
     VectorSimilarityFunction vsf_;

@@ -36,6 +36,11 @@ class BuildParams(C.Structure):
                 ("add_hierarchy", C.c_int), ("seed", C.c_uint64), ("max_batch", C.c_int), ("concurrent_window", C.c_int)]
 
 
+class RemoveStats(C.Structure):
+    _fields_ = [("live_nodes", C.c_int32), ("removed", C.c_int32), ("repaired_rows", C.c_int64), ("candidates", C.c_int64),
+                ("max_candidates", C.c_int32), ("random_fallbacks", C.c_int64), ("device_ms", C.c_double)]
+
+
 # every symbol include/jvector_b200.h declares: (name, restype, argtypes)
 _F, _I, _Z, _P, _L = C.c_float, C.c_int, C.c_size_t, C.c_void_p, C.c_int64
 SYMBOLS = [
@@ -94,6 +99,7 @@ SYMBOLS = [
     ("jv_graph_search_batch_device_ex", _I, [_P, _P, _P, _I, _P, _I, _I, _I, C.POINTER(SearchOptions), _P, _P, C.POINTER(SearchStats)]),
     ("jv_graph_build", _I, [_P, _I, C.POINTER(BuildParams), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_graph_build_stats", _I, [i64p, i64p, i64p]),
+    ("jv_graph_remove_deleted", _I, [_P, _P, _I, _F, C.c_uint64, C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(RemoveStats)]),
     ("jv_builder_create", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]), ("jv_builder_info", _I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     ("jv_builder_next_batch", _I, [_P, i32p, i32p]), ("jv_builder_insert_slice", _I, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     ("jv_builder_apply_new", _I, [_P, C.c_int32, C.c_int32, _P, _P, i32p]), ("jv_builder_reprune_slice", _I, [_P, C.c_int32, C.c_int32, _P, _P]),

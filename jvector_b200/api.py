@@ -417,3 +417,36 @@ class GraphIndexBuilder:
         lib.jv_graph_build_stats(C.byref(s), C.byref(b), C.byref(d))
         self.scored_vectors, self.batches, self.dropped_backlinks = s.value, b.value, d.value
         return GraphIndex(_handle=h)
+
+    def removeDeletedNodes(self, graph, vectors, deleted):
+        """GraphIndexBuilder.markNodeDeleted + cleanup's removeDeletedNodes (GraphIndexBuilder.java:689-799) on the device.
+
+        deleted: bool mask [n] or an array of node ids. Returns a NEW GraphIndex (`graph` is left as it is) in which those nodes are
+        holes — no row names them, their own rows are empty, they belong to no upper level — and every live row that named one
+        was re-pruned with this builder's similarity function and alpha over its live neighbours and its deleted neighbours' live
+        neighbours (random live members of its level, seeded by this builder's seed, when those offer none). The result carries
+        `.remove_stats` (jv_remove_stats as a dict) and no FusedPQ records: call fuse_pq on it again if needed.
+
+        Until this is called, a graph with marked nodes is searched with GraphSearcher.search(..., acceptOrds=~deleted): the marked
+        nodes stay on the search paths but are never returned."""
+        lib = nat.init()
+        n = graph.info()["n"]
+        d = np.asarray(deleted)
+        if d.dtype == bool:
+            if d.shape != (n,):
+                raise ValueError("deleted mask has shape %s, the graph has %d nodes" % (d.shape, n))
+            mask = d
+        else:
+            ids = d.astype(np.int64).ravel()
+            if ids.size and (ids.min() < 0 or ids.max() >= n):
+                raise ValueError("deleted ids outside [0, %d)" % n)
+            mask = np.zeros(n, bool)
+            mask[ids] = True
+        bits = pack_accept_bits(mask)
+        st = nat.RemoveStats()
+        h = C.c_void_p()
+        check(lib.jv_graph_remove_deleted(graph._h, vectors._h, int(self.vsf), float(self.params.alpha), int(self.params.seed),
+                                          bits.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(h), C.byref(st)))
+        out = GraphIndex(_handle=h)
+        out.remove_stats = {name: getattr(st, name) for name, _ in nat.RemoveStats._fields_}
+        return out

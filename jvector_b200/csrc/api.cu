@@ -197,6 +197,7 @@ struct jv_graph_s {
     long long *upper_off = nullptr;
     std::vector<std::vector<int32_t>> level_ids;  // host copies, level >= 1
     std::vector<std::vector<int32_t>> level_adj;
+    std::vector<uint32_t> removed;  // ids taken out by jv_graph_remove_deleted (holes), bit (id & 31) of word (id >> 5); empty = none
     ~jv_graph_s()
     {
         cudaFree(adj0); cudaFree(upper_row); cudaFree(upper_adj); cudaFree(upper_off); cudaFree(fused);
@@ -1117,6 +1118,14 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
     if (rc) return rc;
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
+    if (g->g.entry_node < 0) {
+        // every node was removed (jv_graph_remove_deleted): no entry point, nothing to walk
+        CK(cudaMemsetAsync(nodes_dev, 0xff, (size_t)nq * topK * 4, s), "memset nodes");
+        CK(cudaMemsetAsync(scores_dev, 0, (size_t)nq * topK * 4, s), "memset scores");
+        CK(cudaStreamSynchronize(s), "sync");
+        if (stats) memset(stats, 0, sizeof(*stats));
+        return JV_OK;
+    }
     const DataDesc *rr = reranker ? &reranker->d : nullptr;
     SearchPlan plan;
     // JV_VISITED_CAP / JV_LIST_CAP: first visited-table / candidate-list sizes (testing and tuning knobs; queries that outgrow
@@ -1570,6 +1579,153 @@ int jv_graph_build_stats(int64_t *scored_vectors, int64_t *batches, int64_t *dro
     if (scored_vectors) *scored_vectors = t_build_stats.searched;
     if (batches) *batches = t_build_stats.batches;
     if (dropped_backlinks) *dropped_backlinks = t_build_stats.dropped_backlinks;
+    return JV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ removeDeletedNodes
+static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bits[(size_t)v >> 5] >> (v & 31)) & 1u; }
+
+// one level of the repair on the device (repair_level, build.cu); level L >= 1 also hands back its repaired rows
+static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset f32, int metric, float alpha, uint64_t seed, int level, const std::vector<uint32_t> &dead,
+                                const uint32_t *dead_dev, RepairStats *st, std::vector<int32_t> *adj_out, cudaStream_t s)
+{
+    const int n = g->g.n, degree = g->g.degree;
+    const std::vector<int32_t> *ids = level ? &g->level_ids[level - 1] : nullptr;
+    const int rows = level ? (int)ids->size() : n;
+    std::vector<int32_t> members;
+    for (int r = 0; r < rows; r++) {
+        const int v = ids ? (*ids)[r] : r;
+        if (!bit_of(dead, v)) members.push_back(v);
+    }
+    std::sort(members.begin(), members.end());
+    int32_t *dmem = nullptr, *dids = nullptr, *dold = nullptr, *dnew = nullptr;
+    cudaError_t e = cudaMalloc((void **)&dmem, std::max<size_t>(members.size(), 1) * 4);
+    if (e == cudaSuccess && !members.empty()) e = cudaMemcpyAsync(dmem, members.data(), members.size() * 4, cudaMemcpyHostToDevice, s);
+    if (level == 0) {
+        dold = g->adj0;
+        dnew = ng->adj0;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dnew, dold, (size_t)n * degree * 4, cudaMemcpyDeviceToDevice, s);
+    } else {
+        const std::vector<int32_t> &adj = g->level_adj[level - 1];
+        if (e == cudaSuccess) e = cudaMalloc((void **)&dids, (size_t)rows * 4);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&dold, adj.size() * 4);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&dnew, adj.size() * 4);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dids, ids->data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dold, adj.data(), adj.size() * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dnew, adj.data(), adj.size() * 4, cudaMemcpyHostToDevice, s);
+    }
+    const int32_t *rowmap = level ? g->upper_row + (size_t)(level - 1) * n : nullptr;
+    if (e == cudaSuccess)
+        e = repair_level(f32->d, metric, alpha, degree, rows, dold, dnew, dids, rowmap, dead_dev, dmem, (int)members.size(), seed, level, g_sm_count, st, s);
+    if (e == cudaSuccess && level == 0) e = launch_clear_dead_rows(dnew, n, degree, dead_dev, s);
+    if (e == cudaSuccess && level > 0) {
+        adj_out->resize((size_t)rows * degree);
+        e = cudaMemcpyAsync(adj_out->data(), dnew, adj_out->size() * 4, cudaMemcpyDeviceToHost, s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    else cudaStreamSynchronize(s);
+    cudaFree(dmem);
+    cudaFree(dids);
+    if (level > 0) {
+        cudaFree(dold);
+        cudaFree(dnew);
+    }
+    return e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted");
+}
+
+int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
+                            jv_remove_stats *stats)
+{
+    ON_DEVICE_OF(g);
+    if (!f32 || !deleted_bits || !out || !stats) return fail(JV_ERR_INVALID, "graph_remove_deleted: null argument");
+    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "graph_remove_deleted: needs the graph's fp32 data set");
+    if (f32->d.n != g->g.n || f32->device != g->device) return fail(JV_ERR_INVALID, "graph_remove_deleted: data set and graph differ in size or device");
+    if (!(alpha >= 1.0f)) return fail(JV_ERR_INVALID, "graph_remove_deleted: need alpha >= 1");
+    int rc = check_metric(f32->d, metric);
+    if (rc) return rc;
+    if (g->g.degree > 64)
+        return fail(JV_ERR_UNSUPPORTED, "graph_remove_deleted: degree " + std::to_string(g->g.degree) + " > 64, the largest row the prune kernels handle");
+    if ((rc = t_ctx.init())) return rc;
+    cudaStream_t s = t_ctx.stream;
+    const int n = g->g.n, degree = g->g.degree;
+    const size_t W = ((size_t)n + 31) / 32;
+    // deleted now or removed earlier: both are gone from the new graph
+    std::vector<uint32_t> dead(deleted_bits, deleted_bits + W);
+    if (n & 31) dead[W - 1] &= (1u << (n & 31)) - 1u;
+    long long holes = 0, gone = 0;
+    for (size_t w = 0; w < W; w++) {
+        const uint32_t h = g->removed.empty() ? 0u : g->removed[w];
+        holes += __builtin_popcount(h);
+        dead[w] |= h;
+        gone += __builtin_popcount(dead[w]);
+    }
+    jv_graph ng = new jv_graph_s();
+    ng->device = g->device;
+    memset(&ng->g, 0, sizeof(GraphDesc));
+    ng->g.n = n; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_node = -1; ng->g.entry_level = 0;
+    ng->removed = dead;
+    uint32_t *dead_dev = nullptr;
+    RepairStats st;
+    memset(&st, 0, sizeof(st));
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    cudaEventRecord(e0, s);
+    cudaError_t e = cudaMalloc((void **)&ng->adj0, (size_t)n * degree * 4);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&dead_dev, W * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dead_dev, dead.data(), W * 4, cudaMemcpyHostToDevice, s);
+    rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted: allocation");
+    ng->g.adj0 = ng->adj0;
+    if (!rc) rc = remove_deleted_level(g, ng, f32, metric, alpha, seed, 0, dead, dead_dev, &st, nullptr, s);
+    // upper levels: repaired on the device like level 0, then their deleted members are dropped from the host copies
+    for (int level = 1; !rc && level < g->g.levels; level++) {
+        std::vector<int32_t> adj;
+        rc = remove_deleted_level(g, ng, f32, metric, alpha, seed, level, dead, dead_dev, &st, &adj, s);
+        if (rc) break;
+        const std::vector<int32_t> &ids = g->level_ids[level - 1];
+        std::vector<int32_t> nids, nadj;
+        for (size_t r = 0; r < ids.size(); r++) {
+            if (bit_of(dead, ids[r])) continue;
+            nids.push_back(ids[r]);
+            nadj.insert(nadj.end(), adj.begin() + r * degree, adj.begin() + (r + 1) * degree);
+        }
+        ng->level_ids.push_back(std::move(nids));
+        ng->level_adj.push_back(std::move(nadj));
+    }
+    if (!rc) {
+        // entry (GraphIndexBuilder.java:769-786): kept while it lives; otherwise the lowest live id of the highest level that still has a
+        // live member, with the emptied levels above it dropped (the entry must belong to the top level)
+        int entry = g->g.entry_node;
+        if (entry < 0 || bit_of(dead, entry)) {
+            entry = -1;
+            int top = (int)ng->level_ids.size();
+            while (top > 0 && ng->level_ids[top - 1].empty()) top--;
+            ng->level_ids.resize(top);
+            ng->level_adj.resize(top);
+            if (top > 0) entry = *std::min_element(ng->level_ids[top - 1].begin(), ng->level_ids[top - 1].end());
+            else
+                for (int v = 0; v < n; v++)
+                    if (!bit_of(dead, v)) { entry = v; break; }
+        }
+        ng->g.entry_node = entry;
+        rc = graph_rebuild_upper(ng);
+    }
+    cudaEventRecord(e1, s);
+    cudaStreamSynchronize(s);
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    cudaFree(dead_dev);
+    if (rc) { delete ng; return rc; }
+    stats->live_nodes = (int32_t)(n - gone);
+    stats->removed = (int32_t)(gone - holes);
+    stats->repaired_rows = st.repaired_rows;
+    stats->candidates = st.candidates;
+    stats->max_candidates = st.max_candidates;
+    stats->random_fallbacks = st.random_fallbacks;
+    stats->device_ms = ms;
+    *out = ng;
     return JV_OK;
 }
 

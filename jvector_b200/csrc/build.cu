@@ -58,6 +58,11 @@ struct PruneParams {
     int *out_deg;
     int out_stride, out_base;
     int list_base;  // mode 1: nodes = list[list_base + i]
+    // mode 2 (repair of deleted neighbours): row i of this launch is a = list[i] of the repaired rows, node = row_node[a], candidates =
+    // cand[cand_off[a] .. + cand_cnt[a]) (ragged), result to out_rows[a * out_stride ..] and out_deg[a]
+    const int32_t *row_node;
+    const long long *cand_off;
+    const int *cand_cnt;
 };
 
 // candidate i of node v: the search result while i < cand_stride, then the in-progress window (skipping v itself)
@@ -126,16 +131,18 @@ __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const f
 // c at or after the cursor with M[c] <= score(c) * alpha", a flag scan. A candidate whose M[c] already exceeds
 // score(c) * alpha_max can never be selected in any pass (M only grows) and is dropped from further updates. The selection
 // sequence — and therefore the neighbour list — is exactly the reference loop's, including the alpha = 1.0, 1.2 passes.
-template <int METRIC>
+// MAXC: candidate capacity (power of two). The builder uses PRUNE_MAXC; the repair of deleted neighbours also instantiates
+// larger capacities so that no candidate set is ever clipped.
+template <int METRIC, int MAXC = PRUNE_MAXC>
 __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *blob = reinterpret_cast<float *>(smem_raw);                       // stride + 4
     float *newrow = blob + P.d.stride + 4;                                   // stride: the most recently selected row
-    long long *keys = reinterpret_cast<long long *>(newrow + P.d.stride);    // PRUNE_MAXC
-    float *maxsim = reinterpret_cast<float *>(keys + PRUNE_MAXC);            // PRUNE_MAXC
-    int32_t *sel_ids = reinterpret_cast<int32_t *>(maxsim + PRUNE_MAXC);     // 128
-    uint8_t *state = reinterpret_cast<uint8_t *>(sel_ids + 128);             // PRUNE_MAXC: 0 eligible, 1 selected, 2 dropped
+    long long *keys = reinterpret_cast<long long *>(newrow + P.d.stride);    // MAXC
+    float *maxsim = reinterpret_cast<float *>(keys + MAXC);                  // MAXC
+    int32_t *sel_ids = reinterpret_cast<int32_t *>(maxsim + MAXC);           // 128
+    uint8_t *state = reinterpret_cast<uint8_t *>(sel_ids + 128);             // MAXC: 0 eligible, 1 selected, 2 dropped
     __shared__ float red[36];
     __shared__ int s_next;
 
@@ -148,21 +155,25 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
     for (float a = 1.0f; a <= P.alpha + 1e-6f; a += 0.2f) alpha_max = a;
 
     for (int it = blockIdx.x; it < total; it += gridDim.x) {
-        const int v = P.mode == 0 ? P.node_base + it : P.list[P.list_base + it];
+        const int a = P.mode == 2 ? P.list[it] : 0;
+        const int v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
         const int32_t *cand;
         int nc, ncs;
         if (P.mode == 0) {
             cand = P.cand + (size_t)it * P.cand_stride;
             ncs = P.cand_stride;
             nc = ncs + P.window;
+        } else if (P.mode == 2) {
+            cand = P.cand + P.cand_off[a];
+            ncs = nc = P.cand_cnt[a];
         } else {
             cand = P.adj + (size_t)v * P.row_cap;
             ncs = nc = min(P.deg[v], P.row_cap);
         }
-        nc = min(nc, PRUNE_MAXC);
+        nc = min(nc, MAXC);
         prepare_blob(P.d, P.metric, P.d.rows + (size_t)v * P.d.stride, blob, red);
         // exact scores of the candidates against v, as sortable keys (two rows per warp at a time)
-        for (int i = warp; i < PRUNE_MAXC; i += 2 * NW) {
+        for (int i = warp; i < MAXC; i += 2 * NW) {
             const int i2 = i + NW;
             const int32_t ca = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1, cb = i2 < nc ? prune_candidate(P, cand, ncs, v, i2) : -1;
             const bool va = ca >= 0 && ca != v, vb = cb >= 0 && cb != v;
@@ -175,15 +186,15 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             }
             if (lane == 0) {
                 keys[i] = ka;
-                if (i2 < PRUNE_MAXC) keys[i2] = kb;
+                if (i2 < MAXC) keys[i2] = kb;
             }
         }
         __syncthreads();
-        bitonic_sort_desc_prune(keys, PRUNE_MAXC);
+        bitonic_sort_desc_prune(keys, MAXC);
         // valid keys form a prefix (KEY_MIN sorts last); duplicates are adjacent after the sort and are dropped
         int nvalid;
         {
-            int lo = 0, hi = PRUNE_MAXC;
+            int lo = 0, hi = MAXC;
             while (lo < hi) {
                 const int mid = (lo + hi) >> 1;
                 if (keys[mid] != KEY_MIN) lo = mid + 1;
@@ -191,7 +202,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             }
             nvalid = lo;
         }
-        for (int i = tid; i < PRUNE_MAXC; i += PRUNE_THREADS) {
+        for (int i = tid; i < MAXC; i += PRUNE_THREADS) {
             maxsim[i] = -3.0e38f;
             state[i] = (i < nvalid && !(i > 0 && keys[i - 1] == keys[i])) ? 0 : 2;
         }
@@ -237,12 +248,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
         __syncthreads();
         if (tid == 0) {
             int w = 0;
-            int32_t *row = P.out_rows ? P.out_rows + (size_t)(P.out_base + it) * P.out_stride : P.adj + (size_t)v * P.row_cap;
+            const int oi = P.mode == 2 ? a : P.out_base + it;
+            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
             const int width = P.out_rows ? P.out_stride : P.row_cap;
             for (int i = 0; i < nvalid; i++)
                 if (state[i] == 1) row[w++] = key_node(keys[i]);
             for (int i = w; i < width; i++) row[i] = -1;
-            if (P.out_rows) P.out_deg[P.out_base + it] = w;
+            if (P.out_rows) P.out_deg[oi] = w;
             else P.deg[v] = w;
             if (P.mode == 1 && P.mark) P.mark[v] = 0;
         }
@@ -285,13 +297,17 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
     for (float a = 1.0f; a <= P.alpha + 1e-6f; a += 0.2f) alpha_max = a;
 
     for (int it = blockIdx.x; it < total; it += gridDim.x) {
-        const int v = P.mode == 0 ? P.node_base + it : P.list[P.list_base + it];
+        const int a = P.mode == 2 ? P.list[it] : 0;
+        const int v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
         const int32_t *cand;
         int nc, ncs;
         if (P.mode == 0) {
             cand = P.cand + (size_t)it * P.cand_stride;
             ncs = P.cand_stride;
             nc = ncs + P.window;
+        } else if (P.mode == 2) {
+            cand = P.cand + P.cand_off[a];
+            ncs = nc = P.cand_cnt[a];
         } else {
             cand = P.adj + (size_t)v * P.row_cap;
             ncs = nc = min(P.deg[v], P.row_cap);
@@ -428,12 +444,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
         __syncthreads();
         if (tid == 0) {
             int w = 0;
-            int32_t *row = P.out_rows ? P.out_rows + (size_t)(P.out_base + it) * P.out_stride : P.adj + (size_t)v * P.row_cap;
+            const int oi = P.mode == 2 ? a : P.out_base + it;
+            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
             const int width = P.out_rows ? P.out_stride : P.row_cap;
             for (int i = 0; i < nvalid; i++)
                 if (state[i] == 1) row[w++] = ids[i];
             for (int i = w; i < width; i++) row[i] = -1;
-            if (P.out_rows) P.out_deg[P.out_base + it] = w;
+            if (P.out_rows) P.out_deg[oi] = w;
             else P.deg[v] = w;
             if (P.mode == 1 && P.mark) P.mark[v] = 0;
         }
@@ -547,13 +564,17 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
     const int c4 = tid & 7, r0 = tid >> 3;
 
     for (int it = blockIdx.x; it < total; it += gridDim.x) {
-        const int v = P.mode == 0 ? P.node_base + it : P.list[P.list_base + it];
+        const int a = P.mode == 2 ? P.list[it] : 0;
+        const int v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
         const int32_t *cand;
         int nc, ncs;
         if (P.mode == 0) {
             cand = P.cand + (size_t)it * P.cand_stride;
             ncs = P.cand_stride;
             nc = ncs + P.window;
+        } else if (P.mode == 2) {
+            cand = P.cand + P.cand_off[a];
+            ncs = nc = P.cand_cnt[a];
         } else {
             cand = P.adj + (size_t)v * P.row_cap;
             ncs = nc = min(P.deg[v], P.row_cap);
@@ -715,12 +736,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
         __syncthreads();
         if (tid == 0) {
             int w = 0;
-            int32_t *row = P.out_rows ? P.out_rows + (size_t)(P.out_base + it) * P.out_stride : P.adj + (size_t)v * P.row_cap;
+            const int oi = P.mode == 2 ? a : P.out_base + it;
+            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
             const int width = P.out_rows ? P.out_stride : P.row_cap;
             for (int i = 0; i < nvalid; i++)
                 if (state[i] == 1) row[w++] = ids[i];
             for (int i = w; i < width; i++) row[i] = -1;
-            if (P.out_rows) P.out_deg[P.out_base + it] = w;
+            if (P.out_rows) P.out_deg[oi] = w;
             else P.deg[v] = w;
             if (P.mode == 1 && P.mark) P.mark[v] = 0;
         }
@@ -865,9 +887,9 @@ cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int 
     return cudaGetLastError();
 }
 
-static size_t prune_smem_bytes(const DataDesc &d)
+static size_t prune_smem_bytes(const DataDesc &d, int maxc = PRUNE_MAXC)
 {
-    size_t b = (size_t)(d.stride + 4) * 4 + (size_t)d.stride * 4 + (size_t)PRUNE_MAXC * 8 + (size_t)PRUNE_MAXC * 4 + 128 * 4 + PRUNE_MAXC;
+    size_t b = (size_t)(d.stride + 4) * 4 + (size_t)d.stride * 4 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
     return (b + 15) & ~(size_t)15;
 }
 
@@ -1183,6 +1205,329 @@ cudaError_t build_graph_flat(const DataDesc &d, int metric, const BuildParams &b
     if (err == cudaSuccess) err = builder_finish(B, adj_out_dev, stats, s);
     else if (stats) *stats = B->st;
     builder_free(B);
+    return err;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Repair of deleted neighbours (GraphIndexBuilder.removeDeletedNodes, base:graph/GraphIndexBuilder.java:689-799), one level at a time:
+//   count  : one warp per row flags the live rows that name a deleted node and sizes their candidate segment
+//   gather : one CTA per flagged row writes its live neighbours, the live 2-hop ids through its deleted neighbours (the FreshDiskANN
+//            rule, :705-721) — or, when there are no such ids, random live members of the level (:743-759) — sorted and deduplicated
+//   prune  : the builder's prune kernels (mode 2, ragged candidates, out of place), dispatched by candidate count so no set is clipped
+//   scatter: the pruned rows replace the old ones in the output adjacency
+// Nothing depends on timing: compaction and offsets come from cub scans, the dedup from a sort, and the prune is deterministic.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool dead_bit(const uint32_t *bits, int v) { return (bits[v >> 5] >> (v & 31)) & 1u; }
+
+__global__ void __launch_bounds__(256) repair_count_kernel(const int32_t *__restrict__ adj, int rows, int degree, const int32_t *__restrict__ ids,
+                                                           const int32_t *__restrict__ rowmap, const uint32_t *__restrict__ dead, unsigned char *flag,
+                                                           long long *cnt)
+{
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (warp >= rows) return;
+    const int r = (int)warp;
+    const int v = ids ? ids[r] : r;
+    int live = 0, two = 0, hit = 0;
+    if (!dead_bit(dead, v)) {
+        for (int s = lane; s < degree; s += 32) {
+            const int32_t j = adj[(size_t)r * degree + s];
+            if (j < 0) continue;
+            if (!dead_bit(dead, j)) { live++; continue; }
+            hit = 1;
+            const int rj = rowmap ? rowmap[j] : j;
+            if (rj < 0) continue;
+            for (int t = 0; t < degree; t++) {
+                const int32_t k = adj[(size_t)rj * degree + t];
+                if (k >= 0 && k != v && !dead_bit(dead, k)) two++;
+            }
+        }
+    }
+    live = group_sum<32>(live);
+    two = group_sum<32>(two);
+    hit = __any_sync(FULL, hit);
+    if (lane == 0) {
+        flag[r] = hit ? 1 : 0;
+        // the random fallback adds at most `degree` picks; 2 * degree keeps the segment a multiple of the row width
+        cnt[r] = hit ? (long long)live + two + (two == 0 ? 2 * degree : 0) : 0;
+    }
+}
+
+// the counter-based generator of the random fallback: a pure function of (seed, level, node, attempt)
+__host__ __device__ __forceinline__ uint64_t repair_mix(uint64_t x)
+{
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+__host__ __device__ __forceinline__ uint64_t repair_random(uint64_t seed, int level, int node, int attempt)
+{
+    return repair_mix(repair_mix(repair_mix(seed ^ (uint64_t)(uint32_t)level) ^ (uint64_t)(uint32_t)node) ^ (uint64_t)(uint32_t)attempt);
+}
+
+__device__ __forceinline__ void bitonic_sort_asc_int(int32_t *keys, int n_pow2)
+{
+    for (int k = 2; k <= n_pow2; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < n_pow2; i += blockDim.x) {
+                const int ixj = i ^ j;
+                if (ixj > i) {
+                    const int32_t a = keys[i], b = keys[ixj];
+                    const bool asc = (i & k) == 0;
+                    if (asc ? (a > b) : (a < b)) { keys[i] = b; keys[ixj] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// slot layout of a row's shared buffer (cap >= degree * (degree + 2), a power of two >= 256):
+//   [0, degree)                           the live neighbours
+//   degree + s * degree + t               entry t of the row of deleted neighbour s (live, != v)
+//   degree * (degree + 1) + p             random pick p of the fallback
+__global__ void __launch_bounds__(256) repair_gather_kernel(const int32_t *__restrict__ adj, int degree, const int32_t *__restrict__ ids,
+                                                            const int32_t *__restrict__ rowmap, const uint32_t *__restrict__ dead,
+                                                            const int32_t *__restrict__ aff, int naff, const long long *__restrict__ off_all, int cap,
+                                                            const int32_t *__restrict__ members, int nmembers, unsigned long long seed, int level,
+                                                            int32_t *cand, int32_t *row_node, long long *cand_off, int *cand_cnt, unsigned char *fallback)
+{
+    extern __shared__ int32_t buf[];
+    __shared__ int32_t s_row[64];
+    __shared__ int s_any;
+    using BlockScan = cub::BlockScan<int, 256>;
+    __shared__ typename BlockScan::TempStorage scan_tmp;
+    const int tid = threadIdx.x;
+    const int per = cap / 256;
+    for (int a = blockIdx.x; a < naff; a += gridDim.x) {
+        const int r = aff[a];
+        const int v = ids ? ids[r] : r;
+        for (int i = tid; i < cap; i += 256) buf[i] = INT_MAX;
+        if (tid < degree) s_row[tid] = adj[(size_t)r * degree + tid];
+        if (tid == 0) s_any = 0;
+        __syncthreads();
+        for (int x = tid; x < degree * (degree + 1); x += 256) {
+            if (x < degree) {
+                const int32_t j = s_row[x];
+                if (j >= 0 && !dead_bit(dead, j)) buf[x] = j;
+            } else {
+                const int s = (x - degree) / degree, t = (x - degree) - s * degree;
+                const int32_t j = s_row[s];
+                if (j < 0 || !dead_bit(dead, j)) continue;
+                const int rj = rowmap ? rowmap[j] : j;
+                if (rj < 0) continue;
+                const int32_t k = adj[(size_t)rj * degree + t];
+                if (k >= 0 && k != v && !dead_bit(dead, k)) {
+                    buf[x] = k;
+                    s_any = 1;  // every writer stores the same value
+                }
+            }
+        }
+        __syncthreads();
+        const bool fb = s_any == 0;
+        if (fb && tid == 0 && nmembers > 0) {
+            // no 2-hop candidate: up to 2 * degree random live members of the level, skipping v and repeats, until degree are found
+            int32_t *pick = buf + degree * (degree + 1);
+            int np = 0;
+            for (int at = 0; at < 2 * degree && np < degree; at++) {
+                const int32_t k = members[repair_random(seed, level, v, at) % (uint64_t)nmembers];
+                bool dup = k == v;
+                for (int p = 0; p < np && !dup; p++) dup = pick[p] == k;
+                if (!dup) pick[np++] = k;
+            }
+        }
+        __syncthreads();
+        bitonic_sort_asc_int(buf, cap);
+        // distinct ids, compacted in ascending order into the row's segment
+        int c = 0;
+        for (int i = tid * per; i < (tid + 1) * per; i++)
+            c += buf[i] != INT_MAX && (i == 0 || buf[i - 1] != buf[i]);
+        int pre, total;
+        BlockScan(scan_tmp).ExclusiveSum(c, pre, total);
+        const long long off = off_all[r];
+        for (int i = tid * per; i < (tid + 1) * per; i++)
+            if (buf[i] != INT_MAX && (i == 0 || buf[i - 1] != buf[i])) cand[off + pre++] = buf[i];
+        if (tid == 0) {
+            row_node[a] = v;
+            cand_off[a] = off;
+            cand_cnt[a] = total;
+            fallback[a] = fb ? 1 : 0;
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(256) repair_scatter_kernel(int32_t *adj, int degree, const int32_t *aff, int naff, const int32_t *rows)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)naff * degree) return;
+    const int a = (int)(idx / degree), t = (int)(idx - (long long)a * degree);
+    adj[(size_t)aff[a] * degree + t] = rows[idx];
+}
+
+__global__ void __launch_bounds__(256) clear_dead_rows_kernel(int32_t *adj, int n, int degree, const uint32_t *dead)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)n * degree) return;
+    if (dead_bit(dead, (int)(idx / degree))) adj[idx] = -1;
+}
+
+cudaError_t launch_clear_dead_rows(int32_t *adj_dev, int n, int degree, const uint32_t *dead_dev, cudaStream_t s)
+{
+    const long long total = (long long)n * degree;
+    clear_dead_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(adj_dev, n, degree, dead_dev);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+// the prune tiers of the repair: TILE-candidate Gram kernels on the tensor cores, then the incremental kernel at growing capacity
+constexpr int REPAIR_TIERS = 5;
+constexpr int REPAIR_TIER_MAX[REPAIR_TIERS] = {64, 128, 256, 1024, 8192};
+
+template <int METRIC>
+static cudaError_t launch_repair_prune_t(const PruneParams &P, int tier, int grid, cudaStream_t s)
+{
+    cudaError_t e;
+#define JV_PRUNE_LAUNCH(KERNEL, SMEM)                                                                                   \
+    do {                                                                                                                \
+        const size_t sm_ = (SMEM);                                                                                      \
+        if ((e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_)) != cudaSuccess) return e; \
+        KERNEL<<<grid, PRUNE_THREADS, sm_, s>>>(P);                                                                     \
+    } while (0)
+    switch (tier) {
+    case 0: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 64>), gram_tc_smem_bytes<64>(P.d)); break;
+    case 1: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 128>), gram_tc_smem_bytes<128>(P.d)); break;
+    case 2: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 256>), prune_smem_bytes(P.d, 256)); break;
+    case 3: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 1024>), prune_smem_bytes(P.d, 1024)); break;
+    default: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 8192>), prune_smem_bytes(P.d, 8192)); break;
+    }
+#undef JV_PRUNE_LAUNCH
+    g_launches++;
+    return cudaGetLastError();
+}
+
+static cudaError_t launch_repair_prune(const PruneParams &P, int tier, int grid, cudaStream_t s)
+{
+    if (P.metric == JV_METRIC_EUCLIDEAN) return launch_repair_prune_t<JV_METRIC_EUCLIDEAN>(P, tier, grid, s);
+    if (P.metric == JV_METRIC_DOT) return launch_repair_prune_t<JV_METRIC_DOT>(P, tier, grid, s);
+    return launch_repair_prune_t<JV_METRIC_COSINE>(P, tier, grid, s);
+}
+
+cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new, const int32_t *ids_dev,
+                         const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev, int nmembers, uint64_t seed, int level,
+                         int sm_count, RepairStats *st, cudaStream_t s)
+{
+    cudaError_t err = cudaSuccess;
+    if (rows <= 0) return cudaSuccess;
+    if (degree < 1 || degree > 64) return cudaErrorInvalidValue;
+    unsigned char *flag = nullptr, *fallback = nullptr;
+    long long *cnt = nullptr, *off_all = nullptr, *cand_off = nullptr;
+    int32_t *iota = nullptr, *aff = nullptr, *cand = nullptr, *row_node = nullptr, *out_rows = nullptr, *tier_list = nullptr;
+    int *naff_dev = nullptr, *cand_cnt = nullptr, *out_deg = nullptr;
+    void *tmp = nullptr;
+    int naff = 0;
+    long long total = 0;
+    std::vector<int> hcnt;
+    std::vector<unsigned char> hfb;
+    std::vector<int32_t> tiers[REPAIR_TIERS];
+    std::vector<int32_t> hlist;
+    size_t tb = 0, t1 = 0, t2 = 0;
+#define R_TRY(x)                                 \
+    do {                                         \
+        err = (x);                               \
+        if (err != cudaSuccess) goto done;       \
+    } while (0)
+    R_TRY(cudaMalloc(&flag, (size_t)rows));
+    R_TRY(cudaMalloc(&cnt, (size_t)rows * 8));
+    R_TRY(cudaMalloc(&off_all, (size_t)rows * 8));
+    R_TRY(cudaMalloc(&iota, (size_t)rows * 4));
+    R_TRY(cudaMalloc(&aff, (size_t)rows * 4));
+    R_TRY(cudaMalloc(&naff_dev, 16));
+    repair_count_kernel<<<(unsigned)(((long long)rows * 32 + 255) / 256), 256, 0, s>>>(adj_old, rows, degree, ids_dev, rowmap_dev, dead_dev, flag, cnt);
+    g_launches++;
+    iota_kernel<<<(rows + 255) / 256, 256, 0, s>>>(iota, rows);
+    g_launches++;
+    R_TRY(cudaGetLastError());
+    cub::DeviceScan::ExclusiveSum(nullptr, t1, cnt, off_all, rows, s);
+    cub::DeviceSelect::Flagged(nullptr, t2, iota, flag, aff, naff_dev, rows, s);
+    tb = std::max(t1, t2) + 256;
+    R_TRY(cudaMalloc(&tmp, tb));
+    t1 = tb;
+    R_TRY(cub::DeviceScan::ExclusiveSum(tmp, t1, cnt, off_all, rows, s));
+    g_launches++;
+    t2 = tb;
+    R_TRY(cub::DeviceSelect::Flagged(tmp, t2, iota, flag, aff, naff_dev, rows, s));
+    g_launches++;
+    {
+        long long last[2] = {0, 0};
+        R_TRY(cudaMemcpyAsync(&naff, naff_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
+        R_TRY(cudaMemcpyAsync(&last[0], off_all + rows - 1, 8, cudaMemcpyDeviceToHost, s));
+        R_TRY(cudaMemcpyAsync(&last[1], cnt + rows - 1, 8, cudaMemcpyDeviceToHost, s));
+        R_TRY(cudaStreamSynchronize(s));
+        total = last[0] + last[1];
+    }
+    if (naff == 0) goto done;
+    R_TRY(cudaMalloc(&cand, (size_t)std::max(total, 1ll) * 4));
+    R_TRY(cudaMalloc(&row_node, (size_t)naff * 4));
+    R_TRY(cudaMalloc(&cand_off, (size_t)naff * 8));
+    R_TRY(cudaMalloc(&cand_cnt, (size_t)naff * 4));
+    R_TRY(cudaMalloc(&fallback, (size_t)naff));
+    R_TRY(cudaMalloc(&out_rows, (size_t)naff * degree * 4));
+    R_TRY(cudaMalloc(&out_deg, (size_t)naff * 4));
+    R_TRY(cudaMalloc(&tier_list, (size_t)naff * 4));
+    {
+        int cap = 256;
+        while (cap < degree * (degree + 2)) cap <<= 1;
+        const size_t gsm = (size_t)cap * 4;
+        R_TRY(cudaFuncSetAttribute(repair_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm));
+        repair_gather_kernel<<<std::min(naff, sm_count * 8), 256, gsm, s>>>(adj_old, degree, ids_dev, rowmap_dev, dead_dev, aff, naff, off_all, cap, members_dev,
+                                                                           nmembers, (unsigned long long)seed, level, cand, row_node, cand_off, cand_cnt, fallback);
+        g_launches++;
+        R_TRY(cudaGetLastError());
+    }
+    hcnt.resize(naff);
+    hfb.resize(naff);
+    R_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)naff * 4, cudaMemcpyDeviceToHost, s));
+    R_TRY(cudaMemcpyAsync(hfb.data(), fallback, (size_t)naff, cudaMemcpyDeviceToHost, s));
+    R_TRY(cudaStreamSynchronize(s));
+    for (int a = 0; a < naff; a++) {
+        int t = 0;
+        while (t < REPAIR_TIERS - 1 && hcnt[a] > REPAIR_TIER_MAX[t]) t++;
+        tiers[t].push_back(a);
+        st->candidates += hcnt[a];
+        st->max_candidates = std::max(st->max_candidates, hcnt[a]);
+        st->random_fallbacks += hfb[a];
+        st->tier_rows[t]++;
+    }
+    st->repaired_rows += naff;
+    for (int t = 0; t < REPAIR_TIERS; t++) hlist.insert(hlist.end(), tiers[t].begin(), tiers[t].end());
+    R_TRY(cudaMemcpyAsync(tier_list, hlist.data(), (size_t)naff * 4, cudaMemcpyHostToDevice, s));
+    {
+        PruneParams P;
+        memset(&P, 0, sizeof(P));
+        P.d = d; P.metric = metric; P.degree = degree; P.row_cap = degree; P.alpha = alpha; P.mode = 2;
+        P.cand = cand; P.row_node = row_node; P.cand_off = cand_off; P.cand_cnt = cand_cnt;
+        P.out_rows = out_rows; P.out_deg = out_deg; P.out_stride = degree;
+        int first = 0;
+        for (int t = 0; t < REPAIR_TIERS; t++) {
+            const int c = (int)tiers[t].size();
+            if (c == 0) continue;
+            P.list = tier_list + first;
+            P.count = c;
+            R_TRY(launch_repair_prune(P, t, std::min(c, sm_count * 5), s));
+            first += c;
+        }
+    }
+    repair_scatter_kernel<<<(unsigned)(((long long)naff * degree + 255) / 256), 256, 0, s>>>(adj_new, degree, aff, naff, out_rows);
+    g_launches++;
+    R_TRY(cudaGetLastError());
+    R_TRY(cudaStreamSynchronize(s));  // the scratch below is freed on return
+done:
+#undef R_TRY
+    if (err != cudaSuccess) cudaStreamSynchronize(s);
+    cudaFree(flag); cudaFree(cnt); cudaFree(off_all); cudaFree(iota); cudaFree(aff); cudaFree(naff_dev); cudaFree(tmp);
+    cudaFree(cand); cudaFree(row_node); cudaFree(cand_off); cudaFree(cand_cnt); cudaFree(fallback); cudaFree(out_rows); cudaFree(out_deg); cudaFree(tier_list);
     return err;
 }
 

@@ -161,4 +161,18 @@ int builder_degree(const GraphBuilder *B);
 int builder_max_batch(const GraphBuilder *B);
 cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s);
 
+// removeDeletedNodes on one level (see build.cu). rows: members of the level; row r is node ids_dev[r] (nullptr: node r, level 0);
+// rowmap_dev[node] = the node's row on this level (nullptr: identity). dead_dev: bitset of deleted nodes (bit node & 31 of word
+// node >> 5). members_dev: the level's live members, ascending (random fallback). adj_new must hold a copy of adj_old: the repaired
+// rows are written into it, every other row is left as it is. Synchronises `s`.
+struct RepairStats {
+    long long repaired_rows, candidates, random_fallbacks;
+    int max_candidates;
+    long long tier_rows[5];  // rows pruned with <= 64, <= 128, <= 256, <= 1024, more candidates
+};
+cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new, const int32_t *ids_dev,
+                         const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev, int nmembers, uint64_t seed, int level,
+                         int sm_count, RepairStats *st, cudaStream_t s);
+cudaError_t launch_clear_dead_rows(int32_t *adj_dev, int n, int degree, const uint32_t *dead_dev, cudaStream_t s);
+
 }  // namespace jv
