@@ -650,35 +650,14 @@ static int topk_device_generic(jv_dataset ds, int metric, const float *queries_d
     int rc;
     const size_t bf = (size_t)blob_floats(ds->d);
     const int chunk_max = (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)512 << 20) / (bf * 4)));
-    TopkScratch ts;
-    ts.S = (int)std::min<long long>(ds->d.n, 16384);
-    {
-        // expected survivors of the aggressive threshold (see launch_topk_bruteforce): j n / S with j - 6 sqrt(j) >= k S / n
-        const double f = (double)ts.S / (double)ds->d.n, kf = k * f;
-        int ja = k;
-        for (int j = 1; j < k; j++)
-            if ((double)j - 6.0 * sqrt((double)j) >= kf) { ja = j; break; }
-        const double expect = ds->d.n <= ts.S ? (double)ds->d.n : ja / f;
-        ts.cap = expect * 2 > 8192 ? 16384 : (expect * 2 > 4096 ? 8192 : 4096);
-        if (ts.cap < ts.S && ds->d.n <= ts.S) ts.cap = 16384;
-    }
     for (int q0 = 0; q0 < nq; q0 += chunk_max) {
         const int cq = std::min(chunk_max, nq - q0);
-        if ((rc = t_ctx.ensure(4, (size_t)cq * bf * 4)) || (rc = t_ctx.ensure(1, (size_t)ts.S * 4 + (size_t)cq * ts.S * 4 + 64)) ||
-            (rc = t_ctx.ensure(2, (size_t)cq * 16 + (size_t)cq * 12 + 64 + (size_t)cq * ts.cap * 8)) || (rc = t_ctx.ensure(3, 64)))
+        if ((rc = t_ctx.ensure(4, (size_t)cq * bf * 4)) || (rc = t_ctx.ensure(2, topk_scratch_bytes(ds->d, cq, k))) || (rc = t_ctx.ensure(3, 64)))
             return rc;
-        ts.sample_ids = (int32_t *)t_ctx.dbuf[1];
-        ts.sample_scores = (float *)((char *)t_ctx.dbuf[1] + (((size_t)ts.S * 4 + 15) & ~(size_t)15));
-        ts.buf = (long long *)t_ctx.dbuf[2];
-        ts.thr = ts.buf + (size_t)cq * ts.cap;
-        ts.thr_safe = ts.thr + cq;
-        ts.cnt = (int *)(ts.thr_safe + cq);
-        ts.qlist_a = ts.cnt + cq;
-        ts.qlist_b = ts.qlist_a + cq;
         int *dflag = (int *)t_ctx.dbuf[3];
         CK(cudaMemsetAsync(dflag, 0, sizeof(int), s), "memset flag");
         CK(launch_prepare(ds->d, metric, queries_dev + (size_t)q0 * ds->d.dim, cq, (float *)t_ctx.dbuf[4], s), "prepare");
-        CK(launch_topk_bruteforce(ds->d, metric, (const float *)t_ctx.dbuf[4], cq, k, ts, keys_dev + (size_t)q0 * k, dflag, s), "topk");
+        CK(launch_topk_bruteforce(ds->d, metric, (const float *)t_ctx.dbuf[4], cq, k, t_ctx.dbuf[2], keys_dev + (size_t)q0 * k, dflag, s), "topk");
         if (id_base) CK(launch_key_rebase(keys_dev + (size_t)q0 * k, (long long)cq * k, (long long)id_base, s), "rebase");
         int flag = 0;
         CK(cudaMemcpyAsync(&flag, dflag, sizeof(int), cudaMemcpyDeviceToHost, s), "D2H flag");
@@ -696,13 +675,22 @@ static int topk_bq_imma_enqueue(jv_dataset ds, const float *queries_dev, int nq,
 {
     int rc;
     const int chunk = std::min(nq, IMMA_QUERY_CHUNK);
-    if ((rc = t_ctx.ensure(7, bq_imma_scratch_bytes(ds->d.n, chunk, ds->d.W) + 64))) return rc;
-    int *tmp = (int *)((char *)t_ctx.dbuf[7] + bq_imma_scratch_bytes(ds->d.n, chunk, ds->d.W));
+    // slot 7: the launcher's scratch, then the status word of the chunks after the first (carved over nullptr: the slot's size)
+    void *scratch;
+    int *tmp;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        scratch = c.take<char>(bq_imma_scratch_bytes(ds->d.n, chunk, ds->d.W));
+        tmp = c.take<int>(1);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.ensure(7, carve(nullptr)))) return rc;
+    carve(t_ctx.dbuf[7]);
     for (int q0 = 0; q0 < nq; q0 += chunk) {
         const int cq = std::min(chunk, nq - q0);
         // one status word per call: chunks after the first accumulate through a scratch word
         int *st = q0 == 0 ? status_dev : tmp;
-        CK(launch_bq_topk_imma(ds->d, queries_dev + (size_t)q0 * ds->d.dim, cq, k, (long long)id_base, t_ctx.dbuf[7], keys_dev + (size_t)q0 * k, st, g_sm_count, s), "bq_topk_imma");
+        CK(launch_bq_topk_imma(ds->d, queries_dev + (size_t)q0 * ds->d.dim, cq, k, (long long)id_base, scratch, keys_dev + (size_t)q0 * k, st, g_sm_count, s), "bq_topk_imma");
         if (q0 > 0) CK(launch_add_int(status_dev, tmp, s), "status");
     }
     return JV_OK;
@@ -1082,7 +1070,7 @@ static int ensure_sketch(jv_dataset ds, cudaStream_t s)
 {
     std::lock_guard<std::mutex> lk(ds->sketch_mu);
     if (ds->sketch || ds->sketch_failed) return JV_OK;
-    const int ss = (ds->d.stride + 7) & ~7;
+    const int ss = sketch_stride(ds->d.stride);
     int8_t *sk = nullptr;
     float2 *meta = nullptr;
     if (cudaMalloc(&sk, (size_t)ds->d.n * ss) != cudaSuccess || cudaMalloc(&meta, (size_t)ds->d.n * sizeof(float2)) != cudaSuccess) {
@@ -1134,23 +1122,31 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
     const char *lcap_env = getenv("JV_LIST_CAP");
     const int cap_hint = cap_env ? atoi(cap_env) : 0, lcap_hint = lcap_env ? atoi(lcap_env) : 0;
     CK(plan_search(approx->d, rr, g->g, topK, rerankK, nq, cap_hint > 0 ? cap_hint : 0, lcap_hint > 0 ? lcap_hint : 0, g_sm_count, &plan), "plan_search");
-    // An fp32 DOT walk of a batch that fills the GPU drops hopeless neighbours on a bound from the row sketch (launch_search): the
-    // first such batch builds the sketch. Without it (the allocation failed) the walk reads every full row, with the same answers.
+    // A walk that drops hopeless neighbours on a bound from the row sketch (launch_search): the first such batch builds the sketch.
+    // Without it (the allocation failed) the walk reads every full row, with the same answers.
     DataDesc ad = approx->d;
-    if (ad.kind == KIND_F32 && metric == JV_METRIC_DOT && nq > plan.ctas && (rc = ensure_sketch(approx, s))) return rc;
+    if (search_uses_sketch(ad, metric, plan, nq) && (rc = ensure_sketch(approx, s))) return rc;
     if (ad.kind == KIND_F32) {
         std::lock_guard<std::mutex> lk(approx->sketch_mu);
         ad.sketch = approx->sketch;
         ad.sketch_meta = approx->sketch_meta;
-        ad.sketch_stride = (ad.stride + 7) & ~7;
+        ad.sketch_stride = sketch_stride(ad.stride);
     }
-    const size_t aux = sizeof(SearchCounters) + 64 + (size_t)nq + (size_t)nq * 4 + 64;
-    if ((rc = t_ctx.ensure(5, search_scratch_bytes(plan))) || (rc = t_ctx.ensure(3, aux))) return rc;
-    char *a = (char *)t_ctx.dbuf[3];
-    SearchCounters *dcnt = (SearchCounters *)a;
-    int *dwork = (int *)(a + sizeof(SearchCounters));
-    uint8_t *dover = (uint8_t *)(a + sizeof(SearchCounters) + 64);
-    int32_t *dindex = (int32_t *)(a + sizeof(SearchCounters) + 64 + (((size_t)nq + 63) & ~(size_t)63));
+    // slot 3: counters, work counter, per-query overflow codes, retry index (carved over nullptr: the slot's size)
+    SearchCounters *dcnt;
+    int *dwork;
+    uint8_t *dover;
+    int32_t *dindex;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dcnt = c.take<SearchCounters>(1);
+        dwork = c.take<int>(1);
+        dover = c.take<uint8_t>(nq);
+        dindex = c.take<int32_t>(nq);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.ensure(5, search_scratch_bytes(plan))) || (rc = t_ctx.ensure(3, carve(nullptr)))) return rc;
+    carve(t_ctx.dbuf[3]);
     CK(cudaMemsetAsync(dcnt, 0, sizeof(SearchCounters), s), "memset counters");
     CK(cudaEventRecord(t_ctx.ev0, s), "event");
     CK(launch_search(g->g, ad, rr, metric, queries_dev, nq, topK, rerankK, plan, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover, nullptr, 0, filter, s),

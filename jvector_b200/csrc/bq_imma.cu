@@ -322,23 +322,6 @@ __device__ __forceinline__ int hd_of_key(long long key, int dim)
     return h;
 }
 
-__device__ __forceinline__ void bitonic_sort_desc_smem(long long *keys, int n_pow2)
-{
-    for (int k = 2; k <= n_pow2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < n_pow2; i += blockDim.x) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const long long a = keys[i], b = keys[ixj];
-                    const bool desc = (i & k) == 0;
-                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
 // pass: 0 = after the aggressive filter, 1 = after the first redo. Writes keys_out[q][0..k) when the query is resolved;
 // otherwise sets the next threshold and appends q to qlist_next (count in counters[pass + 1... see launcher]).
 __global__ void __launch_bounds__(256) bq_select_kernel(const long long *__restrict__ buf, int *__restrict__ cnt, int cap, int k, long long n_rows, int dim,
@@ -382,11 +365,10 @@ __global__ void __launch_bounds__(256) bq_select_kernel(const long long *__restr
                 if (hd_of_key(key, dim) <= hb) skeys[atomicAdd(&s_m, 1)] = key;
             }
             __syncthreads();
-            int p2 = 1;
-            while (p2 < take) p2 <<= 1;
+            const int p2 = next_pow2(take);
             for (int i = take + threadIdx.x; i < p2; i += blockDim.x) skeys[i] = KEY_MIN;
             __syncthreads();
-            bitonic_sort_desc_smem(skeys, p2);
+            bitonic_sort_desc(skeys, p2);
             for (int i = threadIdx.x; i < k; i += blockDim.x) keys_out[(size_t)q * k + i] = i < want ? skeys[i] : KEY_MIN;
             if (threadIdx.x == 0) thr[q] = -1;
             return;
@@ -428,18 +410,36 @@ static int bq_imma_sample_rows(long long n)
 
 constexpr int NQ_ALIGN = 256;  // query count padded to the wgmma tile (a multiple of the IMMA tile)
 
-size_t bq_imma_scratch_bytes(long long n, int nq, int W)
-{
-    const int nq_pad = (nq + NQ_ALIGN - 1) / NQ_ALIGN * NQ_ALIGN, W32 = 2 * W;
-    size_t b = 0;
-    b += (size_t)nq_pad * W32 * 4 + 256;                     // qbits
-    b += ((size_t)nq_pad * 4 + 256) * 7;                     // pb, thr, safe, t2, cnt, qlist a / b
-    b += 64 + 256;                                           // counters
-    b += (size_t)nq_pad * bq_imma_sample_rows(n) * 2 + 256;  // hdm
-    b += (size_t)nq * BQ_IMMA_CAP * 8 + 256;                 // buf
-    b += bq_umma_image_bytes(nq, W) + 256;                   // pre-swizzled query images of the wgmma filter pass
-    return b + 1024;
-}
+// launch_bq_topk_imma's device scratch for nq queries, carved from `base` (nullptr: only measured)
+struct BqScratch {
+    uint32_t *qbits;                                    // [nq_pad][W32]
+    int *pb, *thr, *safe, *t2, *cnt, *qla, *qlb;        // [nq_pad] each
+    int *counters;                                      // redo list lengths
+    unsigned short *hdm;                                // [nq_pad][S]
+    long long *buf;                                     // [nq][BQ_IMMA_CAP]
+    uint8_t *images;                                    // pre-swizzled query images of the wgmma filter pass
+    size_t bytes;
+    BqScratch(long long n, int nq, int W, void *base)
+    {
+        const int nq_pad = (nq + NQ_ALIGN - 1) / NQ_ALIGN * NQ_ALIGN;
+        Carver c(base);
+        qbits = c.take<uint32_t>((size_t)nq_pad * 2 * W);
+        pb = c.take<int>(nq_pad);
+        thr = c.take<int>(nq_pad);
+        safe = c.take<int>(nq_pad);
+        t2 = c.take<int>(nq_pad);
+        cnt = c.take<int>(nq_pad);
+        qla = c.take<int>(nq_pad);
+        qlb = c.take<int>(nq_pad);
+        counters = c.take<int>(16);
+        hdm = c.take<unsigned short>((size_t)nq_pad * bq_imma_sample_rows(n));
+        buf = c.take<long long>((size_t)nq * BQ_IMMA_CAP);
+        images = c.take<uint8_t>(bq_umma_image_bytes(nq, W));
+        bytes = c.bytes;
+    }
+};
+
+size_t bq_imma_scratch_bytes(long long n, int nq, int W) { return BqScratch(n, nq, W, nullptr).bytes; }
 
 bool bq_imma_supported(const DataDesc &d, int k)
 {
@@ -456,29 +456,16 @@ cudaError_t launch_bq_topk_imma(const DataDesc &d, const float *queries_dev, int
     // JV_BQ_FILTER=imma forces the legacy-MMA kernel (the sample pass and the redo passes always use it)
     const char *fm = getenv("JV_BQ_FILTER");
     const bool use_umma = !(fm && fm[0] == 'i') && bq_umma_supported(d);
-    char *p = reinterpret_cast<char *>(scratch_dev);
-    auto take = [&p](size_t bytes) { char *r = p; p += (bytes + 255) & ~(size_t)255; return r; };
-    uint32_t *qbits = reinterpret_cast<uint32_t *>(take((size_t)nq_pad * W32 * 4));
-    int *pb = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *thr = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *safe = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *t2 = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *cnt = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *qla = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *qlb = reinterpret_cast<int *>(take((size_t)nq_pad * 4));
-    int *counters = reinterpret_cast<int *>(take(64));
+    const BqScratch b(d.n, nq, d.W, scratch_dev);
     const int S = bq_imma_sample_rows(d.n);
-    unsigned short *hdm = reinterpret_cast<unsigned short *>(take((size_t)nq_pad * S * 2));
-    long long *buf = reinterpret_cast<long long *>(take((size_t)nq * BQ_IMMA_CAP * 8));
-    uint8_t *images = reinterpret_cast<uint8_t *>(take(bq_umma_image_bytes(nq, d.W)));
     cudaError_t e;
 
-    bq_pack_queries_kernel<<<(nq_pad * 32 + 255) / 256, 256, 0, s>>>(queries_dev, nq, nq_pad, d.dim, W32, qbits, pb);
+    bq_pack_queries_kernel<<<(nq_pad * 32 + 255) / 256, 256, 0, s>>>(queries_dev, nq, nq_pad, d.dim, W32, b.qbits, b.pb);
     g_launches++;
     ImmaParams P;
     P.rows = reinterpret_cast<const uint32_t *>(d.words);
-    P.n = d.n; P.W32 = W32; P.dim = d.dim; P.qbits = qbits; P.nq_pad = nq_pad; P.nq = nq; P.qlist = nullptr; P.n_active = nullptr;
-    P.t2 = t2; P.pb = pb; P.buf = buf; P.cnt = cnt; P.cap = BQ_IMMA_CAP; P.id_base = id_base; P.S = S; P.hdm = hdm;
+    P.n = d.n; P.W32 = W32; P.dim = d.dim; P.qbits = b.qbits; P.nq_pad = nq_pad; P.nq = nq; P.qlist = nullptr; P.n_active = nullptr;
+    P.t2 = b.t2; P.pb = b.pb; P.buf = b.buf; P.cnt = b.cnt; P.cap = BQ_IMMA_CAP; P.id_base = id_base; P.S = S; P.hdm = b.hdm;
     const size_t smem = (size_t)(BM + BN) * (W32 + 4) * 4 + (size_t)(BM + 2 * BN) * 4;
     if ((e = cudaFuncSetAttribute(bq_imma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
     if ((e = cudaFuncSetAttribute(bq_imma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
@@ -495,14 +482,9 @@ cudaError_t launch_bq_topk_imma(const DataDesc &d, const float *queries_dev, int
     }
     // 3. thresholds
     const int whole = d.n <= S ? 1 : 0;
-    int ja = k;
-    if (!whole) {
-        const double kf = (double)k * S / (double)d.n;
-        for (int j = 1; j < k; j++)
-            if ((double)j - 6.0 * sqrt((double)j) >= kf) { ja = j; break; }
-    }
+    const int ja = topk_aggressive_rank(k, S, d.n);
     const size_t hsm = (size_t)2 * (d.dim + 1) * 4;
-    bq_threshold_kernel<<<nq, 256, hsm, s>>>(hdm, S, d.dim, k, ja, whole, pb, thr, safe, t2, cnt, counters);
+    bq_threshold_kernel<<<nq, 256, hsm, s>>>(b.hdm, S, d.dim, k, ja, whole, b.pb, b.thr, b.safe, b.t2, b.cnt, b.counters);
     g_launches++;
     if ((e = cudaMemsetAsync(unresolved_dev, 0, sizeof(int), s)) != cudaSuccess) return e;
     // 4./5. filter + select, then two unconditional redo rounds over the (normally empty) lists
@@ -510,20 +492,20 @@ cudaError_t launch_bq_topk_imma(const DataDesc &d, const float *queries_dev, int
     const size_t ssm = hsm + 8 + (size_t)sort_cap * 8;
     if ((e = cudaFuncSetAttribute(bq_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm)) != cudaSuccess) return e;
     for (int pass = 0; pass < 3; pass++) {
-        const int *qlist = pass == 0 ? nullptr : (pass == 1 ? qla : qlb);
-        const int *nact = pass == 0 ? nullptr : &counters[pass - 1];
-        int *qnext = pass == 0 ? qla : (pass == 1 ? qlb : nullptr);
-        int *nnext = pass == 2 ? nullptr : &counters[pass];
+        const int *qlist = pass == 0 ? nullptr : (pass == 1 ? b.qla : b.qlb);
+        const int *nact = pass == 0 ? nullptr : &b.counters[pass - 1];
+        int *qnext = pass == 0 ? b.qla : (pass == 1 ? b.qlb : nullptr);
+        int *nnext = pass == 2 ? nullptr : &b.counters[pass];
         P.qlist = qlist;
         P.n_active = nact;
         if (pass == 0 && use_umma) {
-            if ((e = launch_bq_umma_filter(d, qbits, nq, nq_pad, t2, pb, buf, cnt, BQ_IMMA_CAP, id_base, images, sm_count, s)) != cudaSuccess) return e;
+            if ((e = launch_bq_umma_filter(d, b.qbits, nq, nq_pad, b.t2, b.pb, b.buf, b.cnt, BQ_IMMA_CAP, id_base, b.images, sm_count, s)) != cudaSuccess) return e;
         } else {
             dim3 grid = row_grid(pass == 0 ? nq_pad / BN : 1, d.n);
             bq_imma_kernel<0><<<grid, IMMA_THREADS, smem, s>>>(P);
             g_launches++;
         }
-        bq_select_kernel<<<pass == 0 ? nq : min(nq, 65535), 256, ssm, s>>>(buf, cnt, BQ_IMMA_CAP, k, d.n, d.dim, pb, thr, safe, t2, keys_out_dev, qlist, nact, qnext,
+        bq_select_kernel<<<pass == 0 ? nq : min(nq, 65535), 256, ssm, s>>>(b.buf, b.cnt, BQ_IMMA_CAP, k, d.n, d.dim, b.pb, b.thr, b.safe, b.t2, keys_out_dev, qlist, nact, qnext,
                                                                            nnext, sort_cap, unresolved_dev);
         g_launches++;
     }

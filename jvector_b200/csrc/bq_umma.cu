@@ -43,18 +43,6 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, unsigned phase)
     for (unsigned spins = 0; !mbar_try_wait(bar, phase); ++spins)
         if (spins > (1u << 28)) __trap();  // a pipeline bug must abort the launch, not hang the device
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: rows 128 B apart inside an 8-row atom, atoms SBO = 1024 B apart
-__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr)
-{
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);  // start address, bits [0,14)
-    d |= (uint64_t)1 << 16;                       // leading byte offset (unused by swizzled K-major layouts), bits [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset, bits [32,46)
-    d |= (uint64_t)1 << 62;                       // layout type SWIZZLE_128B, bits [62,64)
-    return d;
-}
 
 // D[64][256] (+)= A[64][32] * B[256][32]^T, u8 x u8 -> s32. Accumulator fragment: register 4 j + 2 h + e holds row
 // 16 (warp % 4) + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.
@@ -69,16 +57,6 @@ __device__ __forceinline__ void wgmma_u8_m64n256k32(uint32_t (&d)[128], uint64_t
         "}\n"
         : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
-__device__ __forceinline__ void acc_fence(uint32_t (&d)[128])
-{
-#pragma unroll
-    for (int i = 0; i < 128; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
 
 // the query tile as shared-memory images: [qtile][kchunk][UN rows x 128 B], swizzled exactly as the MMA reads it

@@ -78,23 +78,6 @@ __device__ __forceinline__ int32_t prune_candidate(const PruneParams &P, const i
     return w;
 }
 
-__device__ __forceinline__ void bitonic_sort_desc_prune(long long *keys, int n_pow2)
-{
-    for (int k = 2; k <= n_pow2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < n_pow2; i += blockDim.x) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const long long a = keys[i], b = keys[ixj];
-                    const bool desc = (i & k) == 0;
-                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
 // similarity score of candidate row `c` (global) against a cached row `srow` (shared or global), one warp
 template <int METRIC>
 __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const float4 *srow, int n4, int lane)
@@ -190,7 +173,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             }
         }
         __syncthreads();
-        bitonic_sort_desc_prune(keys, MAXC);
+        bitonic_sort_desc(keys, MAXC);
         // valid keys form a prefix (KEY_MIN sorts last); duplicates are adjacent after the sort and are dropped
         int nvalid;
         {
@@ -331,7 +314,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
             }
         }
         __syncthreads();
-        bitonic_sort_desc_prune(keys, TILE);
+        bitonic_sort_desc(keys, TILE);
         int nvalid;
         {
             int lo = 0, hi = TILE;
@@ -469,15 +452,6 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
 // group has completed. The scores against v (the sort keys) stay exact fp32.
 // ------------------------------------------------------------------------------------------------
 namespace tc {
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr)
-{
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);  // start address
-    d |= (uint64_t)1 << 16;                       // leading byte offset (unused by swizzled K-major layouts)
-    d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset: 8-row atoms 1024 B apart
-    d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
-    return d;
-}
 // D[64][N] (+)= A[64][8] * B[N][8]^T in tf32 with fp32 accumulation. Fragment: register 4 j + 2 h + e holds row
 // 16 (warp % 4) + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.
 template <int N>
@@ -507,13 +481,6 @@ __device__ __forceinline__ void mma_tf32<64>(float (&d)[32], uint64_t adesc, uin
         "}\n"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
-// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
-template <int R>
-__device__ __forceinline__ void acc_fence(float (&d)[R])
-{
-#pragma unroll
-    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 template <int TILE>
 struct Layout {
@@ -598,7 +565,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
             }
         }
         __syncthreads();
-        bitonic_sort_desc_prune(keys, TILE);
+        bitonic_sort_desc(keys, TILE);
         int nvalid;
         {
             int lo = 0, hi = TILE;
@@ -629,7 +596,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
         for (int c = 0; c < nchunks; c++) {
             const int b = c & 1;
             if (c >= 2) {  // the MMAs of chunk c - 2 (both warpgroups) have read this buffer
-                asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+                wgmma_wait<1>();
                 __syncthreads();
             }
             unsigned char *hi_t = area + b * L::STAGE_BYTES, *lo_t = hi_t + L::TILE_BYTES;
@@ -652,30 +619,30 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
                 for (int j = 0; j < PASSES; j++)
                     pre[j] = (rowp[j] && k1 < P.d.stride) ? __ldg(reinterpret_cast<const float4 *>(rowp[j] + (c + 1) * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             __syncthreads();
             {
                 const uint32_t ah = smem_u32(hi_t), al = smem_u32(lo_t);
 #pragma unroll
-                for (int mb = 0; mb < MB; mb++) tc::acc_fence(acc[mb]);
-                asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+                for (int mb = 0; mb < MB; mb++) acc_fence(acc[mb]);
+                wgmma_fence();
 #pragma unroll
                 for (int ks = 0; ks < 4; ks++) {
-                    const uint64_t bh = tc::desc_sw128(ah + wg * (N / 8) * 1024 + 32 * ks), bl = tc::desc_sw128(al + wg * (N / 8) * 1024 + 32 * ks);
+                    const uint64_t bh = wgmma_desc(ah + wg * (N / 8) * 1024 + 32 * ks), bl = wgmma_desc(al + wg * (N / 8) * 1024 + 32 * ks);
 #pragma unroll
                     for (int mb = 0; mb < MB; mb++) {
-                        const uint64_t dh = tc::desc_sw128(ah + mb * 8 * 1024 + 32 * ks), dl = tc::desc_sw128(al + mb * 8 * 1024 + 32 * ks);
+                        const uint64_t dh = wgmma_desc(ah + mb * 8 * 1024 + 32 * ks), dl = wgmma_desc(al + mb * 8 * 1024 + 32 * ks);
                         tc::mma_tf32<N>(acc[mb], dh, bh, (c | ks) != 0 ? 1u : 0u);
                         tc::mma_tf32<N>(acc[mb], dh, bl, 1u);
                         tc::mma_tf32<N>(acc[mb], dl, bh, 1u);
                     }
                 }
-                asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+                wgmma_commit();
             }
         }
-        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        wgmma_wait<0>();
 #pragma unroll
-        for (int mb = 0; mb < MB; mb++) tc::acc_fence(acc[mb]);
+        for (int mb = 0; mb < MB; mb++) acc_fence(acc[mb]);
         __syncthreads();  // both warpgroups are past their waits: the staging area may now be overwritten by C
 #pragma unroll
         for (int mb = 0; mb < MB; mb++) {

@@ -128,5 +128,62 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned phase)
     while (!mbar_try_wait(bar, phase)) {
     }
 }
+// generic-proxy shared-memory stores -> visible to the async proxy (wgmma operand reads, bulk copies)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---- warpgroup MMA (wgmma) plumbing shared by every wgmma kernel; the instruction-shape wrappers stay with their callers ----
+// shared-memory matrix descriptor, K-major, SWIZZLE_128B: rows 128 B apart inside an 8-row atom, atoms SBO = 1024 B apart
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr)
+{
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);  // start address, bits [0,14)
+    d |= (uint64_t)1 << 16;                       // leading byte offset (unused by swizzled K-major layouts), bits [16,30)
+    d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset, bits [32,46)
+    d |= (uint64_t)1 << 62;                       // layout type SWIZZLE_128B, bits [62,64)
+    return d;
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R])
+{
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int R>
+__device__ __forceinline__ void acc_fence(uint32_t (&d)[R])
+{
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// block-wide bitonic sort of keys[0..n_pow2) (shared memory, n_pow2 a power of two), descending; ends on a barrier
+__device__ __forceinline__ void bitonic_sort_desc(long long *keys, int n_pow2)
+{
+    for (int k = 2; k <= n_pow2; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < n_pow2; i += blockDim.x) {
+                const int ixj = i ^ j;
+                if (ixj > i) {
+                    const long long a = keys[i], b = keys[ixj];
+                    const bool desc = (i & k) == 0;
+                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// smallest power of two >= v (1 for v <= 1)
+__host__ __device__ __forceinline__ int next_pow2(int v)
+{
+    int p = 1;
+    while (p < v) p <<= 1;
+    return p;
+}
 
 }  // namespace jv

@@ -11,6 +11,21 @@ namespace jv {
 extern std::atomic<long long> g_launches;  // kernels launched by this library (jv_kernel_launch_count)
 constexpr int MAX_DEGREE = 128;            // widest adjacency row the search kernel accepts
 
+// Carves a device scratch block into pieces, each starting 256-byte aligned. Over base == nullptr the same sequence of take()
+// calls only measures the block, so one layout gives both the block's size and its pointers.
+struct Carver {
+    uintptr_t base;
+    size_t bytes = 0;
+    explicit Carver(void *p) : base(reinterpret_cast<uintptr_t>(p)) {}
+    template <typename T>
+    T *take(size_t count)
+    {
+        T *r = reinterpret_cast<T *>(base + bytes);
+        bytes += (count * sizeof(T) + 255) & ~(size_t)255;
+        return r;
+    }
+};
+
 struct GraphDesc {
     int32_t n;
     int degree;
@@ -45,17 +60,11 @@ cudaError_t launch_score_ragged(const DataDesc &d, int metric, const float *blob
                                 int *done_counter = nullptr, int *host_flag = nullptr, int seq = 0);
 cudaError_t launch_score_pairs(const DataDesc &d, int metric, const int32_t *a_dev, const int32_t *b_dev, int n, float *out_dev, cudaStream_t s);
 
-struct TopkScratch {
-    int32_t *sample_ids;   // [S]
-    float *sample_scores;  // [nq][S]
-    long long *thr;        // [nq]
-    long long *thr_safe;   // [nq]
-    long long *buf;        // [nq][cap]
-    int *cnt;              // [nq]
-    int *qlist_a, *qlist_b;  // [nq] each: queries still unresolved after a pass
-    int S, cap;
-};
-cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, const TopkScratch &ts,
+// sampled top-k: the rank j of the aggressive threshold among S sampled rows of n (k when the sample is the whole set)
+int topk_aggressive_rank(int k, int S, long long n);
+// device scratch of launch_topk_bruteforce for nq queries
+size_t topk_scratch_bytes(const DataDesc &d, int nq, int k);
+cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, void *scratch_dev,
                                    long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s);
 
 cudaError_t launch_add_int(int *dst_dev, const int *src_dev, cudaStream_t s);
@@ -124,6 +133,9 @@ struct SearchFilter {
 cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const GraphDesc &g, int topK, int rerankK, int nq,
                         int visited_cap_hint, int list_cap_hint, int sm_count, SearchPlan *plan);
 size_t search_scratch_bytes(const SearchPlan &p);
+// whether a walk of nq queries under `plan` drops neighbours on the fp32 row sketch (launch_row_sketch) when DataDesc has one
+bool search_uses_sketch(const DataDesc &approx, int metric, const SearchPlan &plan, int nq);
+int sketch_stride(int stride);  // int8 sketch bytes per row of an fp32 data set of `stride` floats
 cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const DataDesc *rerank, int metric, const float *queries_dev,
                           int nq, int topK, int rerankK, const SearchPlan &plan, void *scratch_dev, int *work_counter_dev,
                           int32_t *nodes_out_dev, float *scores_out_dev, SearchCounters *counters_dev, uint8_t *overflow_flags_dev,

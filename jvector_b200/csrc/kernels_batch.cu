@@ -186,23 +186,6 @@ cudaError_t launch_score_pairs(const DataDesc &d, int metric, const int32_t *a_d
 // brute-force top-k: sample -> per-query threshold -> filtered full pass -> per-query sort.
 // Keys are the reference's 64-bit ordering key (NodeQueue.java:125-137), so ties go to the smaller node id.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void bitonic_sort_desc(long long *keys, int n_pow2)
-{
-    for (int k = 2; k <= n_pow2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < n_pow2; i += blockDim.x) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const long long a = keys[i], b = keys[ixj];
-                    const bool desc = (i & k) == 0;
-                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
 // Leaves the P largest of keys[0..n_pow2) sorted descending in keys[0..P) (P, n_pow2 powers of two, P <= n_pow2):
 // sort every P-chunk (alternating directions), then halve: element-wise max of neighbouring chunks is a bitonic sequence
 // holding the best P of the pair; re-sort it with one bitonic merge. ~ (log^2 P + 2 log P) / 2 full-width stages instead of
@@ -275,11 +258,7 @@ __global__ void __launch_bounds__(256) topk_threshold_kernel(const float *__rest
     for (int i = threadIdx.x; i < S_pow2; i += blockDim.x)
         skeys[i] = i < S ? topk_key(sample_scores[(size_t)q * S + i], sample_ids[i]) : KEY_MIN;
     __syncthreads();
-    {
-        int P = 1;
-        while (P < k) P <<= 1;
-        bitonic_top_desc(skeys, S_pow2, P);  // j_aggr <= k: both thresholds live in the top k of the sample
-    }
+    bitonic_top_desc(skeys, S_pow2, next_pow2(k));  // j_aggr <= k: both thresholds live in the top k of the sample
     if (threadIdx.x == 0) {
         const long long safe = (!whole && k <= S) ? skeys[k - 1] : KEY_MIN;
         thr_safe[q] = safe;
@@ -496,11 +475,7 @@ __global__ void __launch_bounds__(256) topk_select_kernel(const long long *__res
     const int m = min(c, cap);
     for (int i = threadIdx.x; i < cap_pow2; i += blockDim.x) skeys[i] = i < m ? buf[(size_t)q * cap + i] : KEY_MIN;
     __syncthreads();
-    {
-        int P = 1;
-        while (P < k) P <<= 1;
-        bitonic_top_desc(skeys, cap_pow2, P);  // only the best k are emitted (or used as the tightened threshold)
-    }
+    bitonic_top_desc(skeys, cap_pow2, next_pow2(k));  // only the best k are emitted (or used as the tightened threshold)
     const long long need = n_rows < (long long)k ? n_rows : (long long)k;
     if (c <= cap && (c >= need || t == thr_safe[q])) {
         // exact: every key >= thr was captured and there are at least k of them (or the threshold was the guaranteed one)
@@ -514,18 +489,57 @@ __global__ void __launch_bounds__(256) topk_select_kernel(const long long *__res
     }
 }
 
-static int next_pow2(int v)
+// aggressive threshold = j-th best of the sample with the smallest j such that j - 6 sqrt(j) >= k S / n: the j-th best of a
+// random sample has rank ~ j n / S (std sqrt(j) n / S) in the full set, so fewer than k survivors is a > 6 sigma event
+int topk_aggressive_rank(int k, int S, long long n)
 {
-    int p = 1;
-    while (p < v) p <<= 1;
-    return p;
+    if (n <= S) return k;
+    const double kf = (double)k * S / (double)n;
+    for (int j = 1; j < k; j++)
+        if ((double)j - 6.0 * sqrt((double)j) >= kf) return j;
+    return k;
 }
 
-cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, const TopkScratch &ts,
+// launch_topk_bruteforce's device scratch for nq queries, carved from `base` (nullptr: only measured)
+struct TopkScratch {
+    int S, cap;              // sampled rows, captured keys per query
+    int32_t *sample_ids;     // [S]
+    float *sample_scores;    // [nq][S]
+    long long *thr;          // [nq]
+    long long *thr_safe;     // [nq]
+    long long *buf;          // [nq][cap]
+    int *cnt;                // [nq]
+    int *qlist_a, *qlist_b;  // [nq] each: queries still unresolved after a pass
+    size_t bytes;
+    TopkScratch(const DataDesc &d, int nq, int k, void *base)
+    {
+        S = d.n < 16384 ? (int)d.n : 16384;
+        // room for twice the expected survivors of the aggressive threshold (j n / S); a whole-set sample captures every row
+        const double f = (double)S / (double)d.n;
+        const double expect = d.n <= S ? (double)d.n : topk_aggressive_rank(k, S, d.n) / f;
+        cap = expect * 2 > 8192 ? 16384 : (expect * 2 > 4096 ? 8192 : 4096);
+        if (cap < S && d.n <= S) cap = 16384;
+        Carver c(base);
+        sample_ids = c.take<int32_t>(S);
+        sample_scores = c.take<float>((size_t)nq * S);
+        thr = c.take<long long>(nq);
+        thr_safe = c.take<long long>(nq);
+        buf = c.take<long long>((size_t)nq * cap);
+        cnt = c.take<int>(nq);
+        qlist_a = c.take<int>(nq);
+        qlist_b = c.take<int>(nq);
+        bytes = c.bytes;
+    }
+};
+
+size_t topk_scratch_bytes(const DataDesc &d, int nq, int k) { return TopkScratch(d, nq, k, nullptr).bytes; }
+
+cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, void *scratch_dev,
                                    long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s)
 {
     if (nq <= 0) return cudaSuccess;
     cudaError_t e;
+    const TopkScratch ts(d, nq, k, scratch_dev);
     const int S = ts.S;
     topk_sample_ids_kernel<<<(S + 255) / 256, 256, 0, s>>>(ts.sample_ids, S, d.n);
     g_launches++;
@@ -534,14 +548,7 @@ cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *b
     if ((size_t)S2 * sizeof(long long) > 48 * 1024)
         if ((e = cudaFuncSetAttribute(topk_threshold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S2 * (int)sizeof(long long))) != cudaSuccess) return e;
     const int whole = d.n <= S ? 1 : 0;
-    // aggressive threshold = j-th best of the sample with the smallest j such that j - 6 sqrt(j) >= k S / n: the j-th best of a
-    // random sample has rank ~ j n / S (std sqrt(j) n / S) in the full set, so fewer than k survivors is a > 6 sigma event
-    int ja = k;
-    if (!whole) {
-        const double kf = (double)k * S / (double)d.n;
-        for (int j = 1; j < k; j++)
-            if ((double)j - 6.0 * sqrt((double)j) >= kf) { ja = j; break; }
-    }
+    const int ja = topk_aggressive_rank(k, S, d.n);
     topk_threshold_kernel<<<nq, 256, (size_t)S2 * sizeof(long long), s>>>(ts.sample_scores, ts.sample_ids, S, S2, k, ja, whole, ts.thr, ts.thr_safe, ts.cnt);
     g_launches++;
     const int cap2 = next_pow2(ts.cap);

@@ -122,23 +122,6 @@ __device__ __forceinline__ int count_greater_desc(const long long *a, int n, lon
     return lo;
 }
 
-__device__ __forceinline__ void bitonic_sort_desc_block(long long *keys, int n_pow2)
-{
-    for (int k = 2; k <= n_pow2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < n_pow2; i += blockDim.x) {
-                const int ixj = i ^ j;
-                if (ixj > i) {
-                    const long long a = keys[i], b = keys[ixj];
-                    const bool desc = (i & k) == 0;
-                    if (desc ? (a < b) : (a > b)) { keys[i] = b; keys[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
 // The reference's result queue is a BoundedLongHeap (min-heap of keys, 1-based array): its ARRAY ORDER decides which of two
 // equal exact scores survives NodeQueue.rerank, so the device keeps the same array with the same sift procedures
 // (base:util/AbstractLongHeap.java:158-187 upHeap / downHeap, base:util/BoundedLongHeap.java:60-70,100-104 push / updateTop).
@@ -754,7 +737,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 __syncthreads();
                 for (int i = tid; i < P.sort_pow2; i += SEARCH_THREADS) nxt[i] = i < hs ? cur[i] : KEY_MIN;
                 __syncthreads();
-                bitonic_sort_desc_block(nxt, P.sort_pow2);
+                bitonic_sort_desc(nxt, P.sort_pow2);
                 reranked = (unsigned)nrr;
                 const bool boundary_tie = nrr > P.topK && key_score(nxt[P.topK - 1]) == key_score(nxt[P.topK]);
                 if (!boundary_tie) {
@@ -784,7 +767,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 // no reranker: the best topK of the results by approximate key (GraphSearcher.java:478-486, :494-500)
                 for (int i = tid; i < P.sort_pow2; i += SEARCH_THREADS) nxt[i] = i < hs ? heap[1 + i] : KEY_MIN;
                 __syncthreads();
-                bitonic_sort_desc_block(nxt, P.sort_pow2);
+                bitonic_sort_desc(nxt, P.sort_pow2);
                 for (int i = tid; i < P.topK; i += SEARCH_THREADS) {
                     if (i < hs) { no[i] = key_node(nxt[i]); so[i] = key_score(nxt[i]); }
                     else { no[i] = -1; so[i] = 0.f; }
@@ -808,13 +791,6 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         }
 #endif
     }
-}
-
-static int next_pow2i(int v)
-{
-    int p = 1;
-    while (p < v) p <<= 1;
-    return p;
 }
 
 // shared-memory floats of the walking scorer's prepared query: everything, except for a PQ LUT of which only the rows of the
@@ -908,7 +884,7 @@ cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const Gr
 {
     if (g.degree > MAX_DEGREE || rerankK < 1 || topK < 1 || topK > rerankK) return cudaErrorInvalidValue;
     plan->threads = search_threads_of(approx.kind);
-    plan->sort_pow2 = next_pow2i(rerankK);
+    plan->sort_pow2 = next_pow2(rerankK);
     // The list keeps rerankK entries plus a tie tail (see the kernel header). Continuous scores tie rarely: the slack that
     // rounds rerankK up to a multiple of 32 is enough; BQ scores take at most dim + 1 values, so whole groups tie at the
     // boundary. A query whose tail does not fit reports overflow code 2 and is re-run with list_cap_hint = 4x.
@@ -951,10 +927,10 @@ cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const Gr
         plan->smem_bytes = search_smem_bytes(approx, rerank, rerankK, plan->list_alloc, 0, 0, prd);
     }
     if (plan->smem_bytes > 227 * 1024) return cudaErrorInvalidValue;
-    int vcap = visited_cap_hint > 0 ? visited_cap_hint : next_pow2i(4 * rerankK * (g.degree > 16 ? g.degree : 16));
+    int vcap = visited_cap_hint > 0 ? visited_cap_hint : next_pow2(4 * rerankK * (g.degree > 16 ? g.degree : 16));
     if (vcap < 2048) vcap = 2048;
     if (vcap > (1 << 22)) vcap = 1 << 22;
-    plan->visited_cap = next_pow2i(vcap);
+    plan->visited_cap = next_pow2(vcap);
     // Visited set in shared memory (16-bit slots, see visited_insert_smem): no L2 round trip per neighbour, no 64 KB table to clear
     // per query, nothing of it in L2. Taken on the first attempt when the table a walk of this effort needs fits 32 KB and every
     // region keeps at least 32 slots; a query that outgrows it (or fills one region) is re-run on the global table
@@ -968,7 +944,7 @@ cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const Gr
         const char *vs = getenv("JV_VISITED_SMEM_SLOTS");
         int bits = 15;
         while ((1ll << bits) < g.n) bits++;
-        int slots = vs ? next_pow2i(atoi(vs)) : plan->visited_cap / 2;
+        int slots = vs ? next_pow2(atoi(vs)) : plan->visited_cap / 2;
         int slog = 0;
         while ((1 << slog) < slots) slog++;
         // many regions (large n) want more slots each: grow the table up to 32 KB (10M nodes: 512 regions of 32 slots, ~6 expected
@@ -1027,12 +1003,34 @@ cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const Gr
     return cudaSuccess;
 }
 
-size_t search_scratch_bytes(const SearchPlan &p)
+// launch_search's device scratch, carved from `base` (nullptr: only measured): the per-CTA visited tables (unused when the visited
+// set lives in shared memory), then the per-CTA L2 slices of the LUT when plan.blob_in_global
+struct SearchScratch {
+    int32_t *visited_tables;
+    float *blob_global;
+    size_t bytes;
+    SearchScratch(const SearchPlan &p, void *base)
+    {
+        Carver c(base);
+        visited_tables = c.take<int32_t>(p.vis_slots_log ? 1 : (size_t)p.ctas * p.visited_cap);
+        blob_global = p.blob_in_global ? c.take<float>((size_t)p.ctas * p.blob_floats) : nullptr;
+        bytes = c.bytes;
+    }
+};
+
+size_t search_scratch_bytes(const SearchPlan &p) { return SearchScratch(p, nullptr).bytes; }
+
+// a batch with more queries than resident CTAs fills the GPU: bandwidth bound rather than latency bound
+static bool fills_gpu(const SearchPlan &plan, int nq) { return nq > plan.ctas; }
+
+// fp32 DOT walks of such batches drop hopeless neighbours on the bound of their row sketch (sketch_bound_pair): HBM bound, half the
+// bytes per dropped row. A latency-bound batch reads the rows it prefetched anyway.
+bool search_uses_sketch(const DataDesc &approx, int metric, const SearchPlan &plan, int nq)
 {
-    size_t b = p.vis_slots_log ? 256 : (size_t)p.ctas * p.visited_cap * sizeof(int32_t);
-    if (p.blob_in_global) b += (size_t)p.ctas * p.blob_floats * sizeof(float) + 256;
-    return b;
+    return approx.kind == KIND_F32 && metric == JV_METRIC_DOT && fills_gpu(plan, nq);
 }
+
+int sketch_stride(int stride) { return (stride + 7) & ~7; }
 
 cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const DataDesc *rerank, int metric, const float *queries_dev,
                           int nq, int topK, int rerankK, const SearchPlan &plan, void *scratch_dev, int *work_counter_dev,
@@ -1070,7 +1068,9 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     int lg = 0;
     while ((1 << lg) < plan.visited_cap) lg++;
     P.visited_shift = 32 - lg;
-    P.visited_tables = reinterpret_cast<int32_t *>(scratch_dev);
+    const SearchScratch scratch(plan, scratch_dev);
+    P.visited_tables = scratch.visited_tables;
+    P.blob_global = scratch.blob_global;
     P.work_counter = work_counter_dev;
     P.nodes_out = nodes_out_dev;
     P.scores_out = scores_out_dev;
@@ -1081,17 +1081,15 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     P.pq_smem_m = plan.pq_smem_m;
     P.smemA_floats = search_smemA_floats(approx, plan.pq_smem_m);
     P.blobR_floats = rerank ? blob_floats(*rerank) : 0;
-    P.blob_global = nullptr;
     P.vis_slots_log = plan.vis_slots_log;
     P.vis_rlog = plan.vis_rlog;
     P.vis_idmask = plan.vis_idmask;
     // fp32: only a batch that does not fill the GPU (latency bound, L2 to spare) prefetches its rows. A full batch would keep up to
     // 9 CTAs x 28 rows x 3 KB per SM waiting in L2, twice an H100 SM's ~380 KB share: rows were evicted before their demand load and
     // read from DRAM twice (c2: 35.2 ms with the prefetch, 30.7 ms without)
-    P.row_prefetch = (approx.kind == KIND_F32 && nq > plan.ctas) ? 0 : plan.row_prefetch;
-    // The same batches, when they are DOT walks, drop hopeless neighbours on the bound of their row sketch (sketch_bound_pair) where
-    // the caller passes one: HBM bound, half the bytes per dropped row. A latency-bound batch reads the rows it prefetched anyway.
-    if (!(approx.kind == KIND_F32 && metric == JV_METRIC_DOT && nq > plan.ctas)) {
+    P.row_prefetch = (approx.kind == KIND_F32 && fills_gpu(plan, nq)) ? 0 : plan.row_prefetch;
+    // the same batches, when they are DOT walks, use the row sketch where the caller passes one
+    if (!search_uses_sketch(approx, metric, plan, nq)) {
         P.approx.sketch = nullptr;
         P.approx.sketch_meta = nullptr;
     }
@@ -1104,11 +1102,7 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
         // line costs more than an early one saves (fp32 / NVQ: c2 13.8 vs 14.0 ms). JV_EARLY_PREFETCH=0|1 overrides.
         const char *ep = getenv("JV_EARLY_PREFETCH");
         // (a batch that does not fill the GPU is latency bound whatever the scorer: on as well)
-        P.early_pf = ep ? atoi(ep) : ((approx.kind == KIND_PQ || approx.kind == KIND_BQ || nq <= plan.ctas) ? 1 : 0);
-    }
-    if (plan.blob_in_global) {
-        size_t off = ((plan.vis_slots_log ? 256 : (size_t)plan.ctas * plan.visited_cap * sizeof(int32_t)) + 255) & ~(size_t)255;
-        P.blob_global = reinterpret_cast<float *>(reinterpret_cast<char *>(scratch_dev) + off);
+        P.early_pf = ep ? atoi(ep) : ((approx.kind == KIND_PQ || approx.kind == KIND_BQ || !fills_gpu(plan, nq)) ? 1 : 0);
     }
     P.dbg = nullptr;
 #ifdef JV_SEARCH_PROFILE
