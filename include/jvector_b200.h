@@ -174,7 +174,8 @@ JV_API int jv_topk_merge_device(const int64_t *keys_in_device, int nq, int parts
 /* Stream-ordered forms for callers that own a CUDA stream (the multi-process bench puts the local top-k, the NCCL all-gather and
  * the merge on ONE stream with no host synchronisation in between). BQ data sets only (the tensor-core contraction of
  * csrc/bq_imma.cu); *status_device receives the number of queries left unresolved (0 normally; non-zero = call the synchronous
- * form, which falls back to the key-threshold kernels). cuda_stream: a cudaStream_t. */
+ * form, which falls back to the key-threshold kernels). cuda_stream: a cudaStream_t. The device scratch of the async top-k
+ * belongs to the calling thread's context for that device, so async calls from one thread must be ordered on one stream. */
 JV_API int jv_topk_bruteforce_device_async(jv_dataset ds, int metric, const float *queries_device, int nq, int k, int64_t id_base,
                                            int64_t *keys_out_device, int32_t *status_device, void *cuda_stream);
 /* keys_in: SHARD-MAJOR [parts][nq][k], exactly what an all-gather of the per-rank [nq][k] arrays produces */

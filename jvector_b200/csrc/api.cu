@@ -6,12 +6,14 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <string>
 #include <vector>
 
 #include "../../include/jvector_b200.h"
+#include "host_mem.h"
 #include "kernels.h"
 
 using namespace jv;
@@ -66,25 +68,34 @@ int cuda_fail(cudaError_t e, const char *what)
 #define g_sm_count (g_sm_counts[t_active])
 
 // per-thread, per-device stream + growable staging buffers (callers are ForkJoinPool workers: no global locks on the score
-// path); released when the thread exits
+// path); released when the thread exits. Each buffer has one role. A buffer whose contents outlive the call that filled it (the
+// async top-k scratch, the copy stream's watermark) is used by nothing else.
 struct ThreadCtx {
-    static constexpr int SLOTS = 8;
     int device = -1;
     cudaStream_t stream = nullptr;
-    void *dbuf[SLOTS] = {};
-    size_t dcap[SLOTS] = {};
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    DeviceBuffer input;         // host queries / rows / points of the call
+    DeviceBuffer aux;           // small per-call inputs: ids, offsets, centroids, codebooks, sub-vector layouts
+    DeviceBuffer blobs;         // prepared queries
+    DeviceBuffer output;        // what the call downloads: scores, keys, codes, assignments, search nodes + scores
+    DeviceBuffer topk_scratch;  // generic top-k: the launcher's scratch
+    DeviceBuffer bq_scratch;    // synchronous BQ top-k: the launcher's scratch + status word
+    DeviceBuffer flag;          // synchronous top-k: overflow flag / unresolved count, read back before the call returns
+    DeviceBuffer bq_async;      // jv_topk_bruteforce_device_async: still read on the caller's stream after the call returns
+    DeviceBuffer search_scratch, search_aux;  // the search kernel's scratch; its counters and per-query overflow codes
+    DeviceBuffer accept_bits;   // host-pointer searches: the uploaded acceptOrds bitsets
+    DeviceBuffer watermark;     // host-pointer searches: the arrival watermark the copy stream writes
+    StreamTimer timer;
     // host-pointer searches: a second stream carries the query chunks while the search kernel already runs (arrival watermark)
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_copy = nullptr;
-    int *marks_pinned = nullptr;  // pinned: the watermark values the copy stream writes behind each chunk
+    PinnedBuffer marks;  // the watermark values the copy stream writes behind each chunk
     static constexpr int MARKS = 16;
     int init_copy()
     {
         if (copy_stream) return JV_OK;
         CK(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking), "cudaStreamCreate(copy)");
         CK(cudaEventCreateWithFlags(&ev_copy, cudaEventDisableTiming), "cudaEventCreate(copy)");
-        CK(cudaHostAlloc((void **)&marks_pinned, MARKS * sizeof(int), cudaHostAllocDefault), "cudaHostAlloc(marks)");
+        CK(marks.grow(MARKS * sizeof(int)), "cudaHostAlloc(marks)");
         return JV_OK;
     }
     int init()
@@ -92,41 +103,32 @@ struct ThreadCtx {
         if (stream) return JV_OK;
         device = t_active;
         CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking), "cudaStreamCreate");
-        CK(cudaEventCreate(&ev0), "cudaEventCreate");
-        CK(cudaEventCreate(&ev1), "cudaEventCreate");
         return JV_OK;
     }
-    int ensure(int slot, size_t bytes)
+    template <typename F>
+    void each_owner(F f)
     {
-        if (bytes <= dcap[slot]) return JV_OK;
-        if (dbuf[slot]) cudaFree(dbuf[slot]);
-        dbuf[slot] = nullptr;
-        dcap[slot] = 0;
-        size_t want = bytes + bytes / 4 + 256;
-        CK(cudaMalloc(&dbuf[slot], want), "cudaMalloc(staging)");
-        dcap[slot] = want;
-        return JV_OK;
+        for (DeviceBuffer *b : {&input, &aux, &blobs, &output, &topk_scratch, &bq_scratch, &flag, &bq_async, &search_scratch, &search_aux, &accept_bits, &watermark})
+            f(*b);
+        f(marks);
+        f(timer);
     }
     ~ThreadCtx()
     {
         if (!stream) return;
         int cur = -1;
-        if (cudaGetDevice(&cur) != cudaSuccess) return;  // runtime already torn down at process exit: nothing left to free
-        if (cudaSetDevice(device) != cudaSuccess) return;
+        if (cudaGetDevice(&cur) != cudaSuccess || cudaSetDevice(device) != cudaSuccess) {
+            each_owner([](auto &o) { o.abandon(); });  // runtime already torn down at process exit: nothing left to free
+            return;
+        }
         cudaStreamSynchronize(stream);
-        for (int i = 0; i < SLOTS; i++)
-            if (dbuf[i]) cudaFree(dbuf[i]);
-        cudaEventDestroy(ev0);
-        cudaEventDestroy(ev1);
+        if (copy_stream) cudaStreamSynchronize(copy_stream);
+        each_owner([](auto &o) { o.reset(); });
         cudaStreamDestroy(stream);
         if (copy_stream) {
-            cudaStreamSynchronize(copy_stream);
             cudaStreamDestroy(copy_stream);
             cudaEventDestroy(ev_copy);
-            cudaFreeHost(marks_pinned);
-            copy_stream = nullptr;
         }
-        stream = nullptr;
         if (cur >= 0) cudaSetDevice(cur);
     }
 };
@@ -137,17 +139,33 @@ thread_local BuildStats t_build_stats = {0, 0, 0, 0, 0};
 
 int round4(int v) { return (v + 3) & ~3; }
 
-void pq_layout(int dim, int M, std::vector<int> &sizes, std::vector<int> &offsets)
+int grow(DeviceBuffer &b, size_t bytes)
 {
-    // base:quantization/ProductQuantization.java:535-550
-    sizes.resize(M);
-    offsets.resize(M);
+    CK(b.grow(bytes), "cudaMalloc(staging)");
+    return JV_OK;
+}
+
+// the sub-vector split of `dim` into M parts (base:quantization/ProductQuantization.java:535-550; NVQuantization.java:236-251
+// uses the same), enqueued on `s` into layout_dev: sizes [M], then offsets [M]
+cudaError_t upload_layout(int dim, int M, int *layout_dev, cudaStream_t s)
+{
+    std::vector<int> h(2 * (size_t)M);
     int base = dim / M, rem = dim % M, off = 0;
     for (int m = 0; m < M; m++) {
-        sizes[m] = base + (m < rem ? 1 : 0);
-        offsets[m] = off;
-        off += sizes[m];
+        h[m] = base + (m < rem ? 1 : 0);
+        h[M + m] = off;
+        off += h[m];
     }
+    return cudaMemcpyAsync(layout_dev, h.data(), h.size() * 4, cudaMemcpyHostToDevice, s);
+}
+
+// n host rows of row_bytes into device rows of stride_bytes, the padding zeroed
+cudaError_t upload_padded(void *dev, const void *host, size_t n, size_t row_bytes, size_t stride_bytes)
+{
+    if (stride_bytes == row_bytes) return cudaMemcpy(dev, host, n * row_bytes, cudaMemcpyHostToDevice);
+    cudaError_t e = cudaMemset(dev, 0, n * stride_bytes);
+    if (e == cudaSuccess) e = cudaMemcpy2D(dev, stride_bytes, host, row_bytes, row_bytes, n, cudaMemcpyHostToDevice);
+    return e;
 }
 
 }  // namespace
@@ -156,26 +174,19 @@ struct jv_dataset_s {
     int device = 0;
     bool borrowed_rows = false;  // jv_dataset_adopt_f32_device: rows belong to the caller
     DataDesc d;
-    std::vector<void *> allocs;
+    std::vector<DeviceBuffer> allocs;
     size_t bytes = 0;
     // fp32 row sketch (row_sketch_kernel): built by the first search that can use it (search_device), freed with the data set.
     // Not part of `d`: only the search kernel's fp32 DOT walks read it, the builder and the batch scorers never see it
-    int8_t *sketch = nullptr;
-    float2 *sketch_meta = nullptr;
+    DeviceBuffer sketch, sketch_meta;
     bool sketch_failed = false;  // the allocation failed once: walk without it from then on
     std::mutex sketch_mu;
-    int alloc(void **p, size_t n)
+    template <typename T>
+    int alloc(T **p, size_t n)
     {
-        CK(cudaMalloc(p, n ? n : 16), "cudaMalloc(dataset)");
-        allocs.push_back(*p);
+        CK(alloc_owned(allocs, *p, n ? n : 16), "cudaMalloc(dataset)");
         bytes += n;
         return JV_OK;
-    }
-    ~jv_dataset_s()
-    {
-        for (void *p : allocs) cudaFree(p);
-        cudaFree(sketch);
-        cudaFree(sketch_meta);
     }
 };
 
@@ -183,25 +194,17 @@ struct jv_query_s {
     int device = 0;
     jv_dataset ds;
     int metric;
-    float *blob = nullptr;
-    int pooled = 0;  // blob belongs to a jv_query_batch
+    DeviceBuffer blob;
 };
 
 struct jv_graph_s {
     int device = 0;
     GraphDesc g;
-    uint8_t *fused = nullptr;  // FusedPQ records
-    int32_t *adj0 = nullptr;
-    int32_t *upper_row = nullptr;
-    int32_t *upper_adj = nullptr;
-    long long *upper_off = nullptr;
+    DeviceBuffer fused;  // FusedPQ records
+    DeviceBuffer adj0, upper_row, upper_adj, upper_off;
     std::vector<std::vector<int32_t>> level_ids;  // host copies, level >= 1
     std::vector<std::vector<int32_t>> level_adj;
     std::vector<uint32_t> removed;  // ids taken out by jv_graph_remove_deleted (holes), bit (id & 31) of word (id >> 5); empty = none
-    ~jv_graph_s()
-    {
-        cudaFree(adj0); cudaFree(upper_row); cudaFree(upper_adj); cudaFree(upper_off); cudaFree(fused);
-    }
 };
 
 struct jv_multi_s {
@@ -211,6 +214,7 @@ struct jv_multi_s {
     std::vector<int64_t> lo;        // shard i holds rows [lo[i], lo[i + 1])
     std::vector<jv_dataset> shards;
     std::vector<ThreadCtx *> ctx;   // one persistent context per shard (worker threads come and go)
+    DeviceBuffer gathered;          // on the first shard's device: the shards' top-k keys [parts][nq][k], then the merged [nq][k]
 };
 
 static void shard_ranges(int64_t n, int parts, std::vector<int64_t> &lo)
@@ -328,7 +332,7 @@ int jv_dataset_register_f32(const float *rows, int64_t n, int dim, jv_dataset *o
 {
     NEED_INIT();
     if (!rows || !out || n <= 0 || dim <= 0 || n > 0x7fffffffLL) return fail(JV_ERR_INVALID, "register_f32: bad arguments");
-    jv_dataset ds = new jv_dataset_s();
+    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s());
     ds->device = t_active;
     memset(&ds->d, 0, sizeof(DataDesc));
     ds->d.kind = KIND_F32;
@@ -336,18 +340,11 @@ int jv_dataset_register_f32(const float *rows, int64_t n, int dim, jv_dataset *o
     ds->d.n = n;
     ds->d.stride = round4(dim);
     float *dev = nullptr;
-    int rc = ds->alloc((void **)&dev, (size_t)n * ds->d.stride * sizeof(float));
-    if (rc) { delete ds; return rc; }
-    cudaError_t e;
-    if (ds->d.stride == dim) e = cudaMemcpy(dev, rows, (size_t)n * dim * sizeof(float), cudaMemcpyHostToDevice);
-    else {
-        e = cudaMemset(dev, 0, (size_t)n * ds->d.stride * sizeof(float));
-        if (e == cudaSuccess)
-            e = cudaMemcpy2D(dev, (size_t)ds->d.stride * 4, rows, (size_t)dim * 4, (size_t)dim * 4, (size_t)n, cudaMemcpyHostToDevice);
-    }
-    if (e != cudaSuccess) { delete ds; return cuda_fail(e, "upload rows"); }
+    int rc = ds->alloc(&dev, (size_t)n * ds->d.stride * sizeof(float));
+    if (rc) return rc;
+    CK(upload_padded(dev, rows, (size_t)n, (size_t)dim * 4, (size_t)ds->d.stride * 4), "upload rows");
     ds->d.rows = dev;
-    *out = ds;
+    *out = ds.release();
     return JV_OK;
 }
 
@@ -356,39 +353,28 @@ int jv_dataset_register_pq(const uint8_t *codes, int64_t n, int dim, int M, int 
     NEED_INIT();
     if (!codes || !codebooks || !out || n <= 0 || dim <= 0 || M <= 0 || M > dim || k <= 0 || k > 256 || n > 0x7fffffffLL)
         return fail(JV_ERR_INVALID, "register_pq: bad arguments");
-    jv_dataset ds = new jv_dataset_s();
+    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s());
     ds->device = t_active;
     memset(&ds->d, 0, sizeof(DataDesc));
     DataDesc &d = ds->d;
     d.kind = KIND_PQ; d.dim = dim; d.n = n; d.M = M; d.k = k; d.code_stride = round4(M);
-    std::vector<int> sizes, offsets;
-    pq_layout(dim, M, sizes, offsets);
     uint8_t *dcodes = nullptr;
     float *dcb = nullptr, *dcen = nullptr, *dmag = nullptr;
-    int *dsz = nullptr, *doff = nullptr;
+    int *dlay = nullptr;
     int rc;
-    if ((rc = ds->alloc((void **)&dcodes, (size_t)n * d.code_stride)) || (rc = ds->alloc((void **)&dcb, (size_t)k * dim * 4)) ||
-        (rc = ds->alloc((void **)&dsz, (size_t)M * 4)) || (rc = ds->alloc((void **)&doff, (size_t)M * 4)) ||
-        (rc = ds->alloc((void **)&dmag, (size_t)M * k * 4)) || (centroid && (rc = ds->alloc((void **)&dcen, (size_t)dim * 4)))) {
-        delete ds;
+    if ((rc = ds->alloc(&dcodes, (size_t)n * d.code_stride)) || (rc = ds->alloc(&dcb, (size_t)k * dim * 4)) || (rc = ds->alloc(&dlay, (size_t)M * 8)) ||
+        (rc = ds->alloc(&dmag, (size_t)M * k * 4)) || (centroid && (rc = ds->alloc(&dcen, (size_t)dim * 4))))
         return rc;
-    }
-    cudaError_t e;
-    if (d.code_stride == M) e = cudaMemcpy(dcodes, codes, (size_t)n * M, cudaMemcpyHostToDevice);
-    else {
-        e = cudaMemset(dcodes, 0, (size_t)n * d.code_stride);
-        if (e == cudaSuccess) e = cudaMemcpy2D(dcodes, d.code_stride, codes, M, M, (size_t)n, cudaMemcpyHostToDevice);
-    }
+    cudaError_t e = upload_padded(dcodes, codes, (size_t)n, (size_t)M, (size_t)d.code_stride);
     if (e == cudaSuccess) e = cudaMemcpy(dcb, codebooks, (size_t)k * dim * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(dsz, sizes.data(), (size_t)M * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(doff, offsets.data(), (size_t)M * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = upload_layout(dim, M, dlay, 0);
     if (e == cudaSuccess && centroid) e = cudaMemcpy(dcen, centroid, (size_t)dim * 4, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { delete ds; return cuda_fail(e, "upload pq"); }
-    d.codes = dcodes; d.codebooks = dcb; d.sub_sizes = dsz; d.sub_offsets = doff; d.centroid = dcen; d.mag = dmag;
+    CK(e, "upload pq");
+    d.codes = dcodes; d.codebooks = dcb; d.sub_sizes = dlay; d.sub_offsets = dlay + M; d.centroid = dcen; d.mag = dmag;
     e = launch_pq_self_magnitudes(d, dmag, 0);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { delete ds; return cuda_fail(e, "pq self magnitudes"); }
-    *out = ds;
+    CK(e, "pq self magnitudes");
+    *out = ds.release();
     return JV_OK;
 }
 
@@ -396,17 +382,40 @@ int jv_dataset_register_bq(const uint64_t *words, int64_t n, int dim, jv_dataset
 {
     NEED_INIT();
     if (!words || !out || n <= 0 || dim <= 0 || n > 0x7fffffffLL) return fail(JV_ERR_INVALID, "register_bq: bad arguments");
-    jv_dataset ds = new jv_dataset_s();
+    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s());
     ds->device = t_active;
     memset(&ds->d, 0, sizeof(DataDesc));
     ds->d.kind = KIND_BQ; ds->d.dim = dim; ds->d.n = n; ds->d.W = (dim + 63) / 64;
     unsigned long long *dw = nullptr;
-    int rc = ds->alloc((void **)&dw, (size_t)n * ds->d.W * 8);
-    if (rc) { delete ds; return rc; }
-    cudaError_t e = cudaMemcpy(dw, words, (size_t)n * ds->d.W * 8, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { delete ds; return cuda_fail(e, "upload bq"); }
+    int rc = ds->alloc(&dw, (size_t)n * ds->d.W * 8);
+    if (rc) return rc;
+    CK(cudaMemcpy(dw, words, (size_t)n * ds->d.W * 8, cudaMemcpyHostToDevice), "upload bq");
     ds->d.words = dw;
-    *out = ds;
+    *out = ds.release();
+    return JV_OK;
+}
+
+// a new NVQ data set of n rows on the current device: bytes and params allocated for the caller to fill, the zero-padded mean
+// and the sub-vector layout enqueued on `s`
+static int nvq_dataset(int64_t n, int dim, int nsub, const float *mean, cudaStream_t s, std::unique_ptr<jv_dataset_s> &ds, uint8_t **bytes_dev,
+                       float **params_dev)
+{
+    ds.reset(new jv_dataset_s());
+    ds->device = t_active;
+    memset(&ds->d, 0, sizeof(DataDesc));
+    DataDesc &d = ds->d;
+    d.kind = KIND_NVQ; d.dim = dim; d.n = n; d.nsub = nsub; d.stride = round4(dim); d.byte_stride = round4(dim);
+    float *dm = nullptr;
+    int *dlay = nullptr;
+    int rc;
+    if ((rc = ds->alloc(bytes_dev, (size_t)n * d.byte_stride)) || (rc = ds->alloc(params_dev, (size_t)n * nsub * 16)) ||
+        (rc = ds->alloc(&dm, (size_t)d.stride * 4)) || (rc = ds->alloc(&dlay, (size_t)nsub * 8)))
+        return rc;
+    cudaError_t e = cudaMemsetAsync(dm, 0, (size_t)d.stride * 4, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dm, mean, (size_t)dim * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = upload_layout(dim, nsub, dlay, s);
+    CK(e, "upload nvq");
+    d.bytes = *bytes_dev; d.params = *params_dev; d.mean = dm; d.sub_sizes = dlay; d.sub_offsets = dlay + nsub;
     return JV_OK;
 }
 
@@ -415,37 +424,16 @@ int jv_dataset_register_nvq(const uint8_t *bytes, const float *params, int64_t n
     NEED_INIT();
     if (!bytes || !params || !mean || !out || n <= 0 || dim <= 0 || nsub <= 0 || nsub > dim || n > 0x7fffffffLL)
         return fail(JV_ERR_INVALID, "register_nvq: bad arguments");
-    jv_dataset ds = new jv_dataset_s();
-    ds->device = t_active;
-    memset(&ds->d, 0, sizeof(DataDesc));
-    DataDesc &d = ds->d;
-    d.kind = KIND_NVQ; d.dim = dim; d.n = n; d.nsub = nsub; d.stride = round4(dim); d.byte_stride = round4(dim);
-    std::vector<int> sizes, offsets;
-    pq_layout(dim, nsub, sizes, offsets);  // base:quantization/NVQuantization.java:236-251 uses the same split
-    uint8_t *db = nullptr;
-    float *dp = nullptr, *dm = nullptr;
-    int *dsz = nullptr, *doff = nullptr;
+    std::unique_ptr<jv_dataset_s> ds;
+    uint8_t *db;
+    float *dp;
     int rc;
-    if ((rc = ds->alloc((void **)&db, (size_t)n * d.byte_stride)) || (rc = ds->alloc((void **)&dp, (size_t)n * nsub * 16)) ||
-        (rc = ds->alloc((void **)&dm, (size_t)d.stride * 4)) || (rc = ds->alloc((void **)&dsz, (size_t)nsub * 4)) ||
-        (rc = ds->alloc((void **)&doff, (size_t)nsub * 4))) {
-        delete ds;
-        return rc;
-    }
-    cudaError_t e;
-    if (d.byte_stride == dim) e = cudaMemcpy(db, bytes, (size_t)n * dim, cudaMemcpyHostToDevice);
-    else {
-        e = cudaMemset(db, 0, (size_t)n * d.byte_stride);
-        if (e == cudaSuccess) e = cudaMemcpy2D(db, d.byte_stride, bytes, dim, dim, (size_t)n, cudaMemcpyHostToDevice);
-    }
+    if ((rc = t_ctx.init()) || (rc = nvq_dataset(n, dim, nsub, mean, t_ctx.stream, ds, &db, &dp))) return rc;
+    cudaError_t e = upload_padded(db, bytes, (size_t)n, (size_t)dim, (size_t)ds->d.byte_stride);
     if (e == cudaSuccess) e = cudaMemcpy(dp, params, (size_t)n * nsub * 16, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemset(dm, 0, (size_t)d.stride * 4);
-    if (e == cudaSuccess) e = cudaMemcpy(dm, mean, (size_t)dim * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(dsz, sizes.data(), (size_t)nsub * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(doff, offsets.data(), (size_t)nsub * 4, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { delete ds; return cuda_fail(e, "upload nvq"); }
-    d.bytes = db; d.params = dp; d.mean = dm; d.sub_sizes = dsz; d.sub_offsets = doff;
-    *out = ds;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(t_ctx.stream);
+    CK(e, "upload nvq");
+    *out = ds.release();
     return JV_OK;
 }
 
@@ -484,12 +472,15 @@ int jv_kmeans_assign_batch(const float *points, int64_t n, int dim, const float 
     NEED_INIT();
     if (!points || !centroids || !assignments_out || n <= 0 || dim <= 0 || k <= 0) return fail(JV_ERR_INVALID, "kmeans_assign: bad arguments");
     int rc;
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(0, (size_t)n * dim * 4)) || (rc = t_ctx.ensure(1, (size_t)n * 4)) || (rc = t_ctx.ensure(2, (size_t)k * dim * 4))) return rc;
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)n * dim * 4)) || (rc = grow(t_ctx.output, (size_t)n * 4)) || (rc = grow(t_ctx.aux, (size_t)k * dim * 4)))
+        return rc;
     cudaStream_t s = t_ctx.stream;
-    CK(cudaMemcpyAsync(t_ctx.dbuf[0], points, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D points");
-    CK(cudaMemcpyAsync(t_ctx.dbuf[2], centroids, (size_t)k * dim * 4, cudaMemcpyHostToDevice, s), "H2D centroids");
-    CK(launch_kmeans_assign((const float *)t_ctx.dbuf[0], n, dim, dim, (const float *)t_ctx.dbuf[2], k, (int32_t *)t_ctx.dbuf[1], s), "kmeans_assign");
-    CK(cudaMemcpyAsync(assignments_out, t_ctx.dbuf[1], (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H assignments");
+    float *dpoints = t_ctx.input.get<float>(), *dcen = t_ctx.aux.get<float>();
+    int32_t *dassign = t_ctx.output.get<int32_t>();
+    CK(cudaMemcpyAsync(dpoints, points, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D points");
+    CK(cudaMemcpyAsync(dcen, centroids, (size_t)k * dim * 4, cudaMemcpyHostToDevice, s), "H2D centroids");
+    CK(launch_kmeans_assign(dpoints, n, dim, dim, dcen, k, dassign, s), "kmeans_assign");
+    CK(cudaMemcpyAsync(assignments_out, dassign, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H assignments");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -542,19 +533,18 @@ int jv_query_begin(jv_dataset ds, const float *q, int metric, jv_query *out)
     int rc = check_metric(ds->d, metric);
     if (rc) return rc;
     if ((rc = t_ctx.init())) return rc;
-    jv_query h = new jv_query_s();
+    std::unique_ptr<jv_query_s> h(new jv_query_s());
     h->ds = ds;
     h->device = ds->device;
     h->metric = metric;
-    cudaError_t e = cudaMalloc((void **)&h->blob, (size_t)blob_floats(ds->d) * 4);
-    if (e != cudaSuccess) { delete h; return cuda_fail(e, "cudaMalloc(query)"); }
-    if ((rc = t_ctx.ensure(0, (size_t)ds->d.dim * 4))) { cudaFree(h->blob); delete h; return rc; }
+    CK(h->blob.alloc((size_t)blob_floats(ds->d) * 4), "cudaMalloc(query)");
+    if ((rc = grow(t_ctx.input, (size_t)ds->d.dim * 4))) return rc;
     cudaStream_t s = t_ctx.stream;
-    e = cudaMemcpyAsync(t_ctx.dbuf[0], q, (size_t)ds->d.dim * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = launch_prepare(ds->d, metric, (const float *)t_ctx.dbuf[0], 1, h->blob, s);
+    cudaError_t e = cudaMemcpyAsync(t_ctx.input.get(), q, (size_t)ds->d.dim * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = launch_prepare(ds->d, metric, t_ctx.input.get<float>(), 1, h->blob.get<float>(), s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { cudaFree(h->blob); delete h; return cuda_fail(e, "prepare query"); }
-    *out = h;
+    CK(e, "prepare query");
+    *out = h.release();
     return JV_OK;
 }
 
@@ -564,11 +554,13 @@ int jv_score_batch(jv_query q, const int32_t *ids, int n, float *scores_out)
     if (!q || (n > 0 && (!ids || !scores_out)) || n < 0) return fail(JV_ERR_INVALID, "score_batch: bad arguments");
     if (n == 0) return JV_OK;
     int rc;
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(1, (size_t)n * 4)) || (rc = t_ctx.ensure(2, (size_t)n * 4))) return rc;
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.aux, (size_t)n * 4)) || (rc = grow(t_ctx.output, (size_t)n * 4))) return rc;
     cudaStream_t s = t_ctx.stream;
-    CK(cudaMemcpyAsync(t_ctx.dbuf[1], ids, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D ids");
-    CK(launch_score_ragged(q->ds->d, q->metric, q->blob, 1, (const int32_t *)t_ctx.dbuf[1], nullptr, n, n, (float *)t_ctx.dbuf[2], s), "score_ragged");
-    CK(cudaMemcpyAsync(scores_out, t_ctx.dbuf[2], (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    int32_t *dids = t_ctx.aux.get<int32_t>();
+    float *dscores = t_ctx.output.get<float>();
+    CK(cudaMemcpyAsync(dids, ids, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D ids");
+    CK(launch_score_ragged(q->ds->d, q->metric, q->blob.get<float>(), 1, dids, nullptr, n, n, dscores, s), "score_ragged");
+    CK(cudaMemcpyAsync(scores_out, dscores, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -577,7 +569,7 @@ int jv_query_get_lut(jv_query q, float *lut_out)
 {
     ON_DEVICE_OF(q);
     if (!q || !lut_out || q->ds->d.kind != KIND_PQ) return fail(JV_ERR_INVALID, "get_lut: not a PQ query");
-    CK(cudaMemcpy(lut_out, q->blob, (size_t)q->ds->d.M * q->ds->d.k * 4, cudaMemcpyDeviceToHost), "D2H lut");
+    CK(cudaMemcpy(lut_out, q->blob.get(), (size_t)q->ds->d.M * q->ds->d.k * 4, cudaMemcpyDeviceToHost), "D2H lut");
     return JV_OK;
 }
 
@@ -585,7 +577,6 @@ int jv_query_end(jv_query q)
 {
     if (!q) return JV_OK;
     cudaSetDevice(q->device);
-    if (!q->pooled) cudaFree(q->blob);
     delete q;
     return JV_OK;
 }
@@ -605,18 +596,25 @@ int jv_score_multi(jv_dataset ds, int metric, const float *queries, int nq, cons
     }
     if (total == 0) return JV_OK;
     const size_t bf = (size_t)blob_floats(ds->d);
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(0, (size_t)nq * ds->d.dim * 4)) || (rc = t_ctx.ensure(1, (size_t)total * 4)) ||
-        (rc = t_ctx.ensure(2, (size_t)total * 4)) || (rc = t_ctx.ensure(3, (size_t)(nq + 1) * 4)) || (rc = t_ctx.ensure(4, (size_t)nq * bf * 4)))
+    int32_t *dids, *doff;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dids = c.take<int32_t>(total);
+        doff = c.take<int32_t>(nq + 1);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)nq * ds->d.dim * 4)) || (rc = grow(t_ctx.aux, carve(nullptr))) ||
+        (rc = grow(t_ctx.output, (size_t)total * 4)) || (rc = grow(t_ctx.blobs, (size_t)nq * bf * 4)))
         return rc;
+    carve(t_ctx.aux.get());
     cudaStream_t s = t_ctx.stream;
-    CK(cudaMemcpyAsync(t_ctx.dbuf[0], queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
-    CK(cudaMemcpyAsync(t_ctx.dbuf[1], ids, (size_t)total * 4, cudaMemcpyHostToDevice, s), "H2D ids");
-    CK(cudaMemcpyAsync(t_ctx.dbuf[3], offsets, (size_t)(nq + 1) * 4, cudaMemcpyHostToDevice, s), "H2D offsets");
-    CK(launch_prepare(ds->d, metric, (const float *)t_ctx.dbuf[0], nq, (float *)t_ctx.dbuf[4], s), "prepare");
-    CK(launch_score_ragged(ds->d, metric, (const float *)t_ctx.dbuf[4], nq, (const int32_t *)t_ctx.dbuf[1], (const int32_t *)t_ctx.dbuf[3], 0, maxc,
-                           (float *)t_ctx.dbuf[2], s),
-       "score_ragged");
-    CK(cudaMemcpyAsync(scores_out, t_ctx.dbuf[2], (size_t)total * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    float *dq = t_ctx.input.get<float>(), *dblobs = t_ctx.blobs.get<float>(), *dscores = t_ctx.output.get<float>();
+    CK(cudaMemcpyAsync(dq, queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+    CK(cudaMemcpyAsync(dids, ids, (size_t)total * 4, cudaMemcpyHostToDevice, s), "H2D ids");
+    CK(cudaMemcpyAsync(doff, offsets, (size_t)(nq + 1) * 4, cudaMemcpyHostToDevice, s), "H2D offsets");
+    CK(launch_prepare(ds->d, metric, dq, nq, dblobs, s), "prepare");
+    CK(launch_score_ragged(ds->d, metric, dblobs, nq, dids, doff, 0, maxc, dscores, s), "score_ragged");
+    CK(cudaMemcpyAsync(scores_out, dscores, (size_t)total * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -631,13 +629,14 @@ int jv_score_pairs(jv_dataset ds, int metric, const int32_t *a, const int32_t *b
         if (a[i] < 0 || a[i] >= ds->d.n || b[i] < 0 || b[i] >= ds->d.n) return fail(JV_ERR_INVALID, "score_pairs: node id out of range");
     int rc = check_metric(ds->d, metric);
     if (rc) return rc;
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(1, (size_t)n * 8)) || (rc = t_ctx.ensure(2, (size_t)n * 4))) return rc;
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.aux, (size_t)n * 8)) || (rc = grow(t_ctx.output, (size_t)n * 4))) return rc;
     cudaStream_t s = t_ctx.stream;
-    int32_t *da = (int32_t *)t_ctx.dbuf[1], *db = da + n;
+    int32_t *da = t_ctx.aux.get<int32_t>(), *db = da + n;
+    float *dscores = t_ctx.output.get<float>();
     CK(cudaMemcpyAsync(da, a, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D a");
     CK(cudaMemcpyAsync(db, b, (size_t)n * 4, cudaMemcpyHostToDevice, s), "H2D b");
-    CK(launch_score_pairs(ds->d, metric, da, db, n, (float *)t_ctx.dbuf[2], s), "score_pairs");
-    CK(cudaMemcpyAsync(scores_out, t_ctx.dbuf[2], (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    CK(launch_score_pairs(ds->d, metric, da, db, n, dscores, s), "score_pairs");
+    CK(cudaMemcpyAsync(scores_out, dscores, (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -652,12 +651,13 @@ static int topk_device_generic(jv_dataset ds, int metric, const float *queries_d
     const int chunk_max = (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)512 << 20) / (bf * 4)));
     for (int q0 = 0; q0 < nq; q0 += chunk_max) {
         const int cq = std::min(chunk_max, nq - q0);
-        if ((rc = t_ctx.ensure(4, (size_t)cq * bf * 4)) || (rc = t_ctx.ensure(2, topk_scratch_bytes(ds->d, cq, k))) || (rc = t_ctx.ensure(3, 64)))
+        if ((rc = grow(t_ctx.blobs, (size_t)cq * bf * 4)) || (rc = grow(t_ctx.topk_scratch, topk_scratch_bytes(ds->d, cq, k))) || (rc = grow(t_ctx.flag, 64)))
             return rc;
-        int *dflag = (int *)t_ctx.dbuf[3];
+        int *dflag = t_ctx.flag.get<int>();
+        float *dblobs = t_ctx.blobs.get<float>();
         CK(cudaMemsetAsync(dflag, 0, sizeof(int), s), "memset flag");
-        CK(launch_prepare(ds->d, metric, queries_dev + (size_t)q0 * ds->d.dim, cq, (float *)t_ctx.dbuf[4], s), "prepare");
-        CK(launch_topk_bruteforce(ds->d, metric, (const float *)t_ctx.dbuf[4], cq, k, t_ctx.dbuf[2], keys_dev + (size_t)q0 * k, dflag, s), "topk");
+        CK(launch_prepare(ds->d, metric, queries_dev + (size_t)q0 * ds->d.dim, cq, dblobs, s), "prepare");
+        CK(launch_topk_bruteforce(ds->d, metric, dblobs, cq, k, t_ctx.topk_scratch.get(), keys_dev + (size_t)q0 * k, dflag, s), "topk");
         if (id_base) CK(launch_key_rebase(keys_dev + (size_t)q0 * k, (long long)cq * k, (long long)id_base, s), "rebase");
         int flag = 0;
         CK(cudaMemcpyAsync(&flag, dflag, sizeof(int), cudaMemcpyDeviceToHost, s), "D2H flag");
@@ -670,12 +670,13 @@ static int topk_device_generic(jv_dataset ds, int metric, const float *queries_d
 constexpr int IMMA_QUERY_CHUNK = 4096;  // queries per bq_imma launch sequence (bounds the capture buffers: 64 KB per query)
 
 // BQ: the tensor-core contraction (bq_imma.cu), enqueued on `s` without any host synchronisation. status_dev receives the number of
-// queries the integer-threshold path left unresolved (0 in the normal case).
-static int topk_bq_imma_enqueue(jv_dataset ds, const float *queries_dev, int nq, int k, int64_t id_base, long long *keys_dev, int *status_dev, cudaStream_t s)
+// queries the integer-threshold path left unresolved (0 in the normal case). `buf` is in use until `s` has passed this work.
+static int topk_bq_imma_enqueue(jv_dataset ds, const float *queries_dev, int nq, int k, int64_t id_base, long long *keys_dev, int *status_dev,
+                                DeviceBuffer &buf, cudaStream_t s)
 {
     int rc;
     const int chunk = std::min(nq, IMMA_QUERY_CHUNK);
-    // slot 7: the launcher's scratch, then the status word of the chunks after the first (carved over nullptr: the slot's size)
+    // the launcher's scratch, then the status word of the chunks after the first (carved over nullptr: the buffer's size)
     void *scratch;
     int *tmp;
     auto carve = [&](void *base) {
@@ -684,8 +685,8 @@ static int topk_bq_imma_enqueue(jv_dataset ds, const float *queries_dev, int nq,
         tmp = c.take<int>(1);
         return c.bytes;
     };
-    if ((rc = t_ctx.ensure(7, carve(nullptr)))) return rc;
-    carve(t_ctx.dbuf[7]);
+    if ((rc = grow(buf, carve(nullptr)))) return rc;
+    carve(buf.get());
     for (int q0 = 0; q0 < nq; q0 += chunk) {
         const int cq = std::min(chunk, nq - q0);
         // one status word per call: chunks after the first accumulate through a scratch word
@@ -701,9 +702,9 @@ static int topk_device(jv_dataset ds, int metric, const float *queries_dev, int 
     const char *force = getenv("JV_BQ_BRUTEFORCE");  // "popc": keep the round-1 popcount kernels (A/B timing, fallback tests)
     if (bq_imma_supported(ds->d, k) && !(force && force[0] == 'p')) {
         int rc;
-        if ((rc = t_ctx.ensure(3, 64))) return rc;
-        int *dflag = (int *)t_ctx.dbuf[3];
-        if ((rc = topk_bq_imma_enqueue(ds, queries_dev, nq, k, id_base, keys_dev, dflag, t_ctx.stream))) return rc;
+        if ((rc = grow(t_ctx.flag, 64))) return rc;
+        int *dflag = t_ctx.flag.get<int>();
+        if ((rc = topk_bq_imma_enqueue(ds, queries_dev, nq, k, id_base, keys_dev, dflag, t_ctx.bq_scratch, t_ctx.stream))) return rc;
         int unresolved = 0;
         CK(cudaMemcpyAsync(&unresolved, dflag, sizeof(int), cudaMemcpyDeviceToHost, t_ctx.stream), "D2H status");
         CK(cudaStreamSynchronize(t_ctx.stream), "sync");
@@ -720,11 +721,11 @@ int jv_topk_bruteforce(jv_dataset ds, int metric, const float *queries, int nq, 
     if (k > 2048) return fail(JV_ERR_INVALID, "topk_bruteforce: k <= 2048");
     int rc = check_metric(ds->d, metric);
     if (rc) return rc;
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(0, (size_t)nq * ds->d.dim * 4)) || (rc = t_ctx.ensure(5, (size_t)nq * k * 8))) return rc;
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)nq * ds->d.dim * 4)) || (rc = grow(t_ctx.output, (size_t)nq * k * 8))) return rc;
     cudaStream_t s = t_ctx.stream;
-    CK(cudaMemcpyAsync(t_ctx.dbuf[0], queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
-    if ((rc = topk_device(ds, metric, (const float *)t_ctx.dbuf[0], nq, k, 0, (long long *)t_ctx.dbuf[5]))) return rc;
-    CK(cudaMemcpyAsync(keys_out, t_ctx.dbuf[5], (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s), "D2H keys");
+    CK(cudaMemcpyAsync(t_ctx.input.get(), queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+    if ((rc = topk_device(ds, metric, t_ctx.input.get<float>(), nq, k, 0, t_ctx.output.get<long long>()))) return rc;
+    CK(cudaMemcpyAsync(keys_out, t_ctx.output.get(), (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s), "D2H keys");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -759,7 +760,7 @@ int jv_topk_bruteforce_device_async(jv_dataset ds, int metric, const float *quer
     if (!bq_imma_supported(ds->d, k)) return fail(JV_ERR_UNSUPPORTED, "topk_bruteforce_device_async: BQ data sets (even word count, n >= 4096) only; use jv_topk_bruteforce_device");
     int rc;
     if ((rc = t_ctx.init())) return rc;
-    return topk_bq_imma_enqueue(ds, queries_device, nq, k, id_base, (long long *)keys_out_device, status_device, (cudaStream_t)cuda_stream);
+    return topk_bq_imma_enqueue(ds, queries_device, nq, k, id_base, (long long *)keys_out_device, status_device, t_ctx.bq_async, (cudaStream_t)cuda_stream);
 }
 
 int jv_topk_merge_device_async(const int64_t *keys_in_device, int nq, int parts, int k, int64_t *keys_out_device, void *cuda_stream)
@@ -775,15 +776,15 @@ static int bq_encode_impl(const float *rows_host, const float *rows_dev, int row
 {
     int rc;
     const int W = (dim + 63) / 64;
-    if ((rc = t_ctx.init()) || (rows_host && (rc = t_ctx.ensure(0, (size_t)n * dim * 4))) || (rc = t_ctx.ensure(1, (size_t)n * W * 8))) return rc;
+    if ((rc = t_ctx.init()) || (rows_host && (rc = grow(t_ctx.input, (size_t)n * dim * 4))) || (rc = grow(t_ctx.output, (size_t)n * W * 8))) return rc;
     cudaStream_t s = t_ctx.stream;
     if (rows_host) {
-        CK(cudaMemcpyAsync(t_ctx.dbuf[0], rows_host, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
-        rows_dev = (const float *)t_ctx.dbuf[0];
+        CK(cudaMemcpyAsync(t_ctx.input.get(), rows_host, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
+        rows_dev = t_ctx.input.get<float>();
         row_stride = dim;
     }
-    CK(launch_bq_encode(rows_dev, n, dim, row_stride, (unsigned long long *)t_ctx.dbuf[1], s), "bq_encode");
-    CK(cudaMemcpyAsync(words_out, t_ctx.dbuf[1], (size_t)n * W * 8, cudaMemcpyDeviceToHost, s), "D2H words");
+    CK(launch_bq_encode(rows_dev, n, dim, row_stride, t_ctx.output.get<unsigned long long>(), s), "bq_encode");
+    CK(cudaMemcpyAsync(words_out, t_ctx.output.get(), (size_t)n * W * 8, cudaMemcpyDeviceToHost, s), "D2H words");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -806,29 +807,33 @@ static int pq_encode_impl(const float *rows, const float *rows_dev, int row_stri
                           const float *centroid, uint8_t *codes_out)
 {
     int rc;
-    std::vector<int> sizes, offsets;
-    pq_layout(dim, M, sizes, offsets);
-    const size_t cb_bytes = (size_t)k * dim * 4;
-    const size_t aux = cb_bytes + (size_t)dim * 4 + (size_t)M * 8 + 64;
-    if ((rc = t_ctx.init()) || (rows && (rc = t_ctx.ensure(0, (size_t)n * dim * 4))) || (rc = t_ctx.ensure(1, (size_t)n * M)) || (rc = t_ctx.ensure(2, aux))) return rc;
+    float *dcb, *dcen;
+    int *dlay;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dcb = c.take<float>((size_t)k * dim);
+        dcen = c.take<float>(dim);
+        dlay = c.take<int>(2 * (size_t)M);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rows && (rc = grow(t_ctx.input, (size_t)n * dim * 4))) || (rc = grow(t_ctx.output, (size_t)n * M)) ||
+        (rc = grow(t_ctx.aux, carve(nullptr))))
+        return rc;
+    carve(t_ctx.aux.get());
     cudaStream_t s = t_ctx.stream;
-    char *a = (char *)t_ctx.dbuf[2];
-    float *dcb = (float *)a, *dcen = (float *)(a + cb_bytes);
-    int *dsz = (int *)(a + cb_bytes + (size_t)dim * 4), *doff = dsz + M;
     if (rows) {
-        CK(cudaMemcpyAsync(t_ctx.dbuf[0], rows, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
-        rows_dev = (const float *)t_ctx.dbuf[0];
+        CK(cudaMemcpyAsync(t_ctx.input.get(), rows, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
+        rows_dev = t_ctx.input.get<float>();
         row_stride = dim;
     }
-    CK(cudaMemcpyAsync(dcb, codebooks, cb_bytes, cudaMemcpyHostToDevice, s), "H2D codebooks");
+    CK(cudaMemcpyAsync(dcb, codebooks, (size_t)k * dim * 4, cudaMemcpyHostToDevice, s), "H2D codebooks");
     if (centroid) CK(cudaMemcpyAsync(dcen, centroid, (size_t)dim * 4, cudaMemcpyHostToDevice, s), "H2D centroid");
-    CK(cudaMemcpyAsync(dsz, sizes.data(), (size_t)M * 4, cudaMemcpyHostToDevice, s), "H2D sizes");
-    CK(cudaMemcpyAsync(doff, offsets.data(), (size_t)M * 4, cudaMemcpyHostToDevice, s), "H2D offsets");
+    CK(upload_layout(dim, M, dlay, s), "H2D layout");
     DataDesc d;
     memset(&d, 0, sizeof(d));
-    d.kind = KIND_PQ; d.dim = dim; d.n = n; d.M = M; d.k = k; d.codebooks = dcb; d.sub_sizes = dsz; d.sub_offsets = doff; d.centroid = centroid ? dcen : nullptr;
-    CK(launch_pq_encode(d, rows_dev, n, row_stride, (uint8_t *)t_ctx.dbuf[1], s), "pq_encode");
-    CK(cudaMemcpyAsync(codes_out, t_ctx.dbuf[1], (size_t)n * M, cudaMemcpyDeviceToHost, s), "D2H codes");
+    d.kind = KIND_PQ; d.dim = dim; d.n = n; d.M = M; d.k = k; d.codebooks = dcb; d.sub_sizes = dlay; d.sub_offsets = dlay + M; d.centroid = centroid ? dcen : nullptr;
+    CK(launch_pq_encode(d, rows_dev, n, row_stride, t_ctx.output.get<uint8_t>(), s), "pq_encode");
+    CK(cudaMemcpyAsync(codes_out, t_ctx.output.get(), (size_t)n * M, cudaMemcpyDeviceToHost, s), "D2H codes");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -852,27 +857,37 @@ static int nvq_encode_impl(const float *rows, const float *rows_dev, int row_str
                            float *params_out, uint8_t *bytes_out)
 {
     int rc;
-    std::vector<int> sizes, offsets;
-    pq_layout(dim, nsub, sizes, offsets);
-    const size_t aux = (size_t)dim * 4 + (size_t)nsub * 8 + 64;
-    if ((rc = t_ctx.init()) || (rows && (rc = t_ctx.ensure(0, (size_t)n * dim * 4))) || (rc = t_ctx.ensure(1, (size_t)n * dim)) ||
-        (rc = t_ctx.ensure(2, aux)) || (rc = t_ctx.ensure(3, (size_t)n * nsub * 16)))
+    float *dmean, *dparams;
+    int *dlay;
+    uint8_t *dbytes;
+    auto carve_aux = [&](void *base) {
+        Carver c(base);
+        dmean = c.take<float>(dim);
+        dlay = c.take<int>(2 * (size_t)nsub);
+        return c.bytes;
+    };
+    auto carve_out = [&](void *base) {
+        Carver c(base);
+        dbytes = c.take<uint8_t>((size_t)n * dim);
+        dparams = c.take<float>((size_t)n * nsub * 4);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rows && (rc = grow(t_ctx.input, (size_t)n * dim * 4))) || (rc = grow(t_ctx.aux, carve_aux(nullptr))) ||
+        (rc = grow(t_ctx.output, carve_out(nullptr))))
         return rc;
+    carve_aux(t_ctx.aux.get());
+    carve_out(t_ctx.output.get());
     cudaStream_t s = t_ctx.stream;
-    char *a = (char *)t_ctx.dbuf[2];
-    float *dmean = (float *)a;
-    int *dsz = (int *)(a + (size_t)dim * 4), *doff = dsz + nsub;
     if (rows) {
-        CK(cudaMemcpyAsync(t_ctx.dbuf[0], rows, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
-        rows_dev = (const float *)t_ctx.dbuf[0];
+        CK(cudaMemcpyAsync(t_ctx.input.get(), rows, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
+        rows_dev = t_ctx.input.get<float>();
         row_stride = dim;
     }
     CK(cudaMemcpyAsync(dmean, mean, (size_t)dim * 4, cudaMemcpyHostToDevice, s), "H2D mean");
-    CK(cudaMemcpyAsync(dsz, sizes.data(), (size_t)nsub * 4, cudaMemcpyHostToDevice, s), "H2D sizes");
-    CK(cudaMemcpyAsync(doff, offsets.data(), (size_t)nsub * 4, cudaMemcpyHostToDevice, s), "H2D offsets");
-    CK(launch_nvq_encode(rows_dev, n, row_stride, nsub, dsz, doff, dmean, learn, (float *)t_ctx.dbuf[3], (uint8_t *)t_ctx.dbuf[1], dim, s), "nvq_encode");
-    CK(cudaMemcpyAsync(params_out, t_ctx.dbuf[3], (size_t)n * nsub * 16, cudaMemcpyDeviceToHost, s), "D2H params");
-    CK(cudaMemcpyAsync(bytes_out, t_ctx.dbuf[1], (size_t)n * dim, cudaMemcpyDeviceToHost, s), "D2H bytes");
+    CK(upload_layout(dim, nsub, dlay, s), "H2D layout");
+    CK(launch_nvq_encode(rows_dev, n, row_stride, nsub, dlay, dlay + nsub, dmean, learn, dparams, dbytes, dim, s), "nvq_encode");
+    CK(cudaMemcpyAsync(params_out, dparams, (size_t)n * nsub * 16, cudaMemcpyDeviceToHost, s), "D2H params");
+    CK(cudaMemcpyAsync(bytes_out, dbytes, (size_t)n * dim, cudaMemcpyDeviceToHost, s), "D2H bytes");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -897,37 +912,17 @@ int jv_nvq_encode_dataset_resident(jv_dataset f32, int nsub, const float *mean, 
 {
     ON_DEVICE_OF(f32);
     if (f32->d.kind != KIND_F32 || !mean || !out || nsub <= 0 || nsub > f32->d.dim) return fail(JV_ERR_INVALID, "nvq_encode_dataset_resident: bad arguments");
+    std::unique_ptr<jv_dataset_s> ds;
+    uint8_t *db;
+    float *dp;
     int rc;
-    if ((rc = t_ctx.init())) return rc;
-    const int dim = f32->d.dim;
-    const int64_t n = f32->d.n;
-    jv_dataset ds = new jv_dataset_s();
-    ds->device = f32->device;
-    memset(&ds->d, 0, sizeof(DataDesc));
-    DataDesc &d = ds->d;
-    d.kind = KIND_NVQ; d.dim = dim; d.n = n; d.nsub = nsub; d.stride = round4(dim); d.byte_stride = round4(dim);
-    std::vector<int> sizes, offsets;
-    pq_layout(dim, nsub, sizes, offsets);
-    uint8_t *db = nullptr;
-    float *dp = nullptr, *dm = nullptr;
-    int *dsz = nullptr, *doff = nullptr;
-    if ((rc = ds->alloc((void **)&db, (size_t)n * d.byte_stride)) || (rc = ds->alloc((void **)&dp, (size_t)n * nsub * 16)) ||
-        (rc = ds->alloc((void **)&dm, (size_t)d.stride * 4)) || (rc = ds->alloc((void **)&dsz, (size_t)nsub * 4)) ||
-        (rc = ds->alloc((void **)&doff, (size_t)nsub * 4))) {
-        delete ds;
-        return rc;
-    }
+    if ((rc = t_ctx.init()) || (rc = nvq_dataset(f32->d.n, f32->d.dim, nsub, mean, t_ctx.stream, ds, &db, &dp))) return rc;
     cudaStream_t s = t_ctx.stream;
-    cudaError_t e = cudaMemsetAsync(dm, 0, (size_t)d.stride * 4, s);
-    if (e == cudaSuccess && d.byte_stride != dim) e = cudaMemsetAsync(db, 0, (size_t)n * d.byte_stride, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dm, mean, (size_t)dim * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dsz, sizes.data(), (size_t)nsub * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(doff, offsets.data(), (size_t)nsub * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = launch_nvq_encode(f32->d.rows, n, f32->d.stride, nsub, dsz, doff, dm, learn, dp, db, d.byte_stride, s);
+    cudaError_t e = ds->d.byte_stride != ds->d.dim ? cudaMemsetAsync(db, 0, (size_t)ds->d.n * ds->d.byte_stride, s) : cudaSuccess;
+    if (e == cudaSuccess) e = launch_nvq_encode(f32->d.rows, ds->d.n, f32->d.stride, nsub, ds->d.sub_sizes, ds->d.sub_offsets, ds->d.mean, learn, dp, db, ds->d.byte_stride, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { delete ds; return cuda_fail(e, "nvq_encode_dataset_resident"); }
-    d.bytes = db; d.params = dp; d.mean = dm; d.sub_sizes = dsz; d.sub_offsets = doff;
-    *out = ds;
+    CK(e, "nvq_encode_dataset_resident");
+    *out = ds.release();
     return JV_OK;
 }
 
@@ -940,22 +935,21 @@ int jv_graph_create(int32_t n, int degree, const int32_t *adj0, int32_t entry_no
     // one pass over data that is copied anyway: a neighbour id outside [-1, n) would be an illegal address inside the search kernel
     for (size_t i = 0, tot = (size_t)n * degree; i < tot; i++)
         if (adj0[i] < -1 || adj0[i] >= n) return fail(JV_ERR_INVALID, "graph_create: neighbour id out of range");
-    jv_graph g = new jv_graph_s();
+    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
     g->device = t_active;
     memset(&g->g, 0, sizeof(GraphDesc));
-    cudaError_t e = cudaMalloc((void **)&g->adj0, (size_t)n * degree * 4);
-    if (e == cudaSuccess) e = cudaMemcpy(g->adj0, adj0, (size_t)n * degree * 4, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { delete g; return cuda_fail(e, "upload adjacency"); }
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = entry_node; g->g.entry_level = 0; g->g.adj0 = g->adj0;
-    *out = g;
+    cudaError_t e = g->adj0.alloc((size_t)n * degree * 4);
+    if (e == cudaSuccess) e = cudaMemcpy(g->adj0.get(), adj0, (size_t)n * degree * 4, cudaMemcpyHostToDevice);
+    CK(e, "upload adjacency");
+    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = entry_node; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
+    *out = g.release();
     return JV_OK;
 }
 
 static int graph_rebuild_upper(jv_graph g)
 {
     const int L = (int)g->level_ids.size();
-    cudaFree(g->upper_row); cudaFree(g->upper_adj); cudaFree(g->upper_off);
-    g->upper_row = nullptr; g->upper_adj = nullptr; g->upper_off = nullptr;
+    g->upper_row.reset(); g->upper_adj.reset(); g->upper_off.reset();
     if (L == 0) return JV_OK;
     const int n = g->g.n, degree = g->g.degree;
     std::vector<int32_t> rows((size_t)L * n, -1);
@@ -968,13 +962,13 @@ static int graph_rebuild_upper(jv_graph g)
         adj.insert(adj.end(), g->level_adj[l].begin(), g->level_adj[l].end());
         o += (long long)g->level_ids[l].size();
     }
-    CK(cudaMalloc((void **)&g->upper_row, rows.size() * 4), "cudaMalloc(upper_row)");
-    CK(cudaMalloc((void **)&g->upper_adj, std::max<size_t>(adj.size(), 1) * 4), "cudaMalloc(upper_adj)");
-    CK(cudaMalloc((void **)&g->upper_off, (size_t)L * 8), "cudaMalloc(upper_off)");
-    CK(cudaMemcpy(g->upper_row, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice), "H2D upper_row");
-    CK(cudaMemcpy(g->upper_adj, adj.data(), adj.size() * 4, cudaMemcpyHostToDevice), "H2D upper_adj");
-    CK(cudaMemcpy(g->upper_off, offs.data(), (size_t)L * 8, cudaMemcpyHostToDevice), "H2D upper_off");
-    g->g.upper_row = g->upper_row; g->g.upper_adj = g->upper_adj; g->g.upper_off = g->upper_off;
+    CK(g->upper_row.alloc(rows.size() * 4), "cudaMalloc(upper_row)");
+    CK(g->upper_adj.alloc(std::max<size_t>(adj.size(), 1) * 4), "cudaMalloc(upper_adj)");
+    CK(g->upper_off.alloc((size_t)L * 8), "cudaMalloc(upper_off)");
+    CK(cudaMemcpy(g->upper_row.get(), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice), "H2D upper_row");
+    CK(cudaMemcpy(g->upper_adj.get(), adj.data(), adj.size() * 4, cudaMemcpyHostToDevice), "H2D upper_adj");
+    CK(cudaMemcpy(g->upper_off.get(), offs.data(), (size_t)L * 8, cudaMemcpyHostToDevice), "H2D upper_off");
+    g->g.upper_row = g->upper_row.get<int32_t>(); g->g.upper_adj = g->upper_adj.get<int32_t>(); g->g.upper_off = g->upper_off.get<long long>();
     g->g.levels = L + 1;
     g->g.entry_level = L;
     (void)degree;
@@ -1006,13 +1000,11 @@ int jv_graph_fuse_pq(jv_graph g, jv_dataset pq)
     int rc;
     if ((rc = t_ctx.init())) return rc;
     const int rec = (g->g.degree * (4 + pq->d.code_stride) + 15) & ~15;
-    cudaFree(g->fused);
-    g->fused = nullptr;
     g->g.fused = nullptr;
-    CK(cudaMalloc((void **)&g->fused, (size_t)g->g.n * rec), "cudaMalloc(fused records)");
-    CK(launch_fuse_pq(g->g, pq->d, g->fused, rec, t_ctx.stream), "fuse_pq");
+    CK(g->fused.alloc((size_t)g->g.n * rec), "cudaMalloc(fused records)");
+    CK(launch_fuse_pq(g->g, pq->d, g->fused.get<uint8_t>(), rec, t_ctx.stream), "fuse_pq");
     CK(cudaStreamSynchronize(t_ctx.stream), "fuse_pq");
-    g->g.fused = g->fused;
+    g->g.fused = g->fused.get<uint8_t>();
     g->g.fused_codes_of = pq->d.codes;
     g->g.fused_rec = rec;
     g->g.fused_code_stride = pq->d.code_stride;
@@ -1022,9 +1014,9 @@ int jv_graph_fuse_pq(jv_graph g, jv_dataset pq)
 int jv_graph_fused_download(jv_graph g, uint8_t *records_out, int *record_bytes)
 {
     ON_DEVICE_OF(g);
-    if (!g->fused) return fail(JV_ERR_INVALID, "graph_fused_download: jv_graph_fuse_pq has not been called");
+    if (!g->fused.get()) return fail(JV_ERR_INVALID, "graph_fused_download: jv_graph_fuse_pq has not been called");
     if (record_bytes) *record_bytes = g->g.fused_rec;
-    if (records_out) CK(cudaMemcpy(records_out, g->fused, (size_t)g->g.n * g->g.fused_rec, cudaMemcpyDeviceToHost), "D2H fused records");
+    if (records_out) CK(cudaMemcpy(records_out, g->fused.get(), (size_t)g->g.n * g->g.fused_rec, cudaMemcpyDeviceToHost), "D2H fused records");
     return JV_OK;
 }
 
@@ -1055,7 +1047,7 @@ int jv_graph_download(jv_graph g, int level, int32_t *node_ids_out, int32_t *adj
         if (count_out) *count_out = g->g.n;
         if (node_ids_out)
             for (int i = 0; i < g->g.n; i++) node_ids_out[i] = i;
-        if (adj_out) CK(cudaMemcpy(adj_out, g->adj0, (size_t)g->g.n * g->g.degree * 4, cudaMemcpyDeviceToHost), "D2H adjacency");
+        if (adj_out) CK(cudaMemcpy(adj_out, g->adj0.get(), (size_t)g->g.n * g->g.degree * 4, cudaMemcpyDeviceToHost), "D2H adjacency");
         return JV_OK;
     }
     const auto &ids = g->level_ids[level - 1];
@@ -1069,25 +1061,19 @@ int jv_graph_download(jv_graph g, int level, int32_t *node_ids_out, int32_t *adj
 static int ensure_sketch(jv_dataset ds, cudaStream_t s)
 {
     std::lock_guard<std::mutex> lk(ds->sketch_mu);
-    if (ds->sketch || ds->sketch_failed) return JV_OK;
+    if (ds->sketch.get() || ds->sketch_failed) return JV_OK;
     const int ss = sketch_stride(ds->d.stride);
-    int8_t *sk = nullptr;
-    float2 *meta = nullptr;
-    if (cudaMalloc(&sk, (size_t)ds->d.n * ss) != cudaSuccess || cudaMalloc(&meta, (size_t)ds->d.n * sizeof(float2)) != cudaSuccess) {
+    DeviceBuffer sk, meta;
+    if (sk.alloc((size_t)ds->d.n * ss) != cudaSuccess || meta.alloc((size_t)ds->d.n * sizeof(float2)) != cudaSuccess) {
         cudaGetLastError();  // out of memory: not an error of the search, which walks without the sketch
-        cudaFree(sk);
         ds->sketch_failed = true;
         return JV_OK;
     }
-    cudaError_t e = launch_row_sketch(ds->d.rows, ds->d.n, ds->d.stride, ss, sk, meta, s);
+    cudaError_t e = launch_row_sketch(ds->d.rows, ds->d.n, ds->d.stride, ss, sk.get<int8_t>(), meta.get<float2>(), s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-        cudaFree(sk);
-        cudaFree(meta);
-        CK(e, "row_sketch");
-    }
-    ds->sketch = sk;
-    ds->sketch_meta = meta;
+    CK(e, "row_sketch");
+    ds->sketch = std::move(sk);
+    ds->sketch_meta = std::move(meta);
     return JV_OK;
 }
 
@@ -1128,11 +1114,11 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
     if (search_uses_sketch(ad, metric, plan, nq) && (rc = ensure_sketch(approx, s))) return rc;
     if (ad.kind == KIND_F32) {
         std::lock_guard<std::mutex> lk(approx->sketch_mu);
-        ad.sketch = approx->sketch;
-        ad.sketch_meta = approx->sketch_meta;
+        ad.sketch = approx->sketch.get<int8_t>();
+        ad.sketch_meta = approx->sketch_meta.get<float2>();
         ad.sketch_stride = sketch_stride(ad.stride);
     }
-    // slot 3: counters, work counter, per-query overflow codes, retry index (carved over nullptr: the slot's size)
+    // counters, work counter, per-query overflow codes, retry index (carved over nullptr: the block's size)
     SearchCounters *dcnt;
     int *dwork;
     uint8_t *dover;
@@ -1145,26 +1131,37 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         dindex = c.take<int32_t>(nq);
         return c.bytes;
     };
-    if ((rc = t_ctx.ensure(5, search_scratch_bytes(plan))) || (rc = t_ctx.ensure(3, carve(nullptr)))) return rc;
-    carve(t_ctx.dbuf[3]);
+    if ((rc = grow(t_ctx.search_aux, carve(nullptr)))) return rc;
+    carve(t_ctx.search_aux.get());
     CK(cudaMemsetAsync(dcnt, 0, sizeof(SearchCounters), s), "memset counters");
-    CK(cudaEventRecord(t_ctx.ev0, s), "event");
-    CK(launch_search(g->g, ad, rr, metric, queries_dev, nq, topK, rerankK, plan, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover, nullptr, 0, filter, s),
-       "launch_search");
-    CK(cudaEventRecord(t_ctx.ev1, s), "event");
     SearchCounters hc;
-    CK(cudaMemcpyAsync(&hc, dcnt, sizeof(hc), cudaMemcpyDeviceToHost, s), "D2H counters");
-    CK(cudaStreamSynchronize(s), "search kernel");
     float ms = 0.f;
-    cudaEventElapsedTime(&ms, t_ctx.ev0, t_ctx.ev1);
     long long retried = 0;
     int cap = plan.visited_cap, lcap = plan.list_cap;
-    // queries whose visited table filled up (code 1) or whose candidate list could not hold a tie tail (code 2) are re-run with a
-    // 4x larger table / list: the result does not depend on either size, only whether the run completes does
-    for (int attempt = 0; hc.overflowed > 0 && attempt < 6; attempt++) {
+    std::vector<int32_t> idx;  // the queries an attempt after the first re-runs
+    for (int attempt = 0;; attempt++) {
+        const int cnt = attempt ? (int)idx.size() : nq;
+        if (attempt) {
+            CK(plan_search(approx->d, rr, g->g, topK, rerankK, cnt, cap, lcap, g_sm_count, &plan), "plan_search(retry)");
+            CK(cudaMemcpyAsync(dindex, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, s), "H2D retry index");
+            unsigned long long zero = 0;
+            CK(cudaMemcpyAsync(&dcnt->overflowed, &zero, sizeof(zero), cudaMemcpyHostToDevice, s), "reset overflow");
+        }
+        if ((rc = grow(t_ctx.search_scratch, search_scratch_bytes(plan)))) return rc;
+        CK(t_ctx.timer.start(s), "event");
+        CK(launch_search(g->g, ad, rr, metric, queries_dev, cnt, topK, rerankK, plan, t_ctx.search_scratch.get(), dwork, nodes_dev, scores_dev, dcnt, dover,
+                         attempt ? dindex : nullptr, 0, filter, s),
+           "launch_search");
+        CK(t_ctx.timer.stop(s), "event");
+        CK(cudaMemcpyAsync(&hc, dcnt, sizeof(hc), cudaMemcpyDeviceToHost, s), "D2H counters");
+        CK(cudaStreamSynchronize(s), "search kernel");
+        ms += t_ctx.timer.ms();
+        if (hc.overflowed == 0 || attempt == 6) break;
+        // queries whose visited table filled up (code 1) or whose candidate list could not hold a tie tail (code 2) are re-run with a
+        // 4x larger table / list: the result does not depend on either size, only whether the run completes does
         std::vector<uint8_t> hover(nq);
         CK(cudaMemcpy(hover.data(), dover, (size_t)nq, cudaMemcpyDeviceToHost), "D2H overflow flags");
-        std::vector<int32_t> idx;
+        idx.clear();
         bool need_table = false, need_list = false;
         for (int i = 0; i < nq; i++)
             if (hover[i]) {
@@ -1179,22 +1176,6 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
             if (lcap >= MAX_LIST_CAP) return fail(JV_ERR_OVERFLOW, "graph_search: more equal-score (or filtered-out) candidates than the longest candidate list holds");
             lcap = std::min(MAX_LIST_CAP, lcap * 4);
         }
-        SearchPlan p2;
-        CK(plan_search(approx->d, rr, g->g, topK, rerankK, (int)idx.size(), cap, lcap, g_sm_count, &p2), "plan_search(retry)");
-        if ((rc = t_ctx.ensure(5, search_scratch_bytes(p2)))) return rc;
-        CK(cudaMemcpyAsync(dindex, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, s), "H2D retry index");
-        unsigned long long zero = 0;
-        CK(cudaMemcpyAsync(&dcnt->overflowed, &zero, sizeof(zero), cudaMemcpyHostToDevice, s), "reset overflow");
-        CK(cudaEventRecord(t_ctx.ev0, s), "event");
-        CK(launch_search(g->g, ad, rr, metric, queries_dev, (int)idx.size(), topK, rerankK, p2, t_ctx.dbuf[5], dwork, nodes_dev, scores_dev, dcnt, dover,
-                         dindex, 0, filter, s),
-           "launch_search(retry)");
-        CK(cudaEventRecord(t_ctx.ev1, s), "event");
-        CK(cudaMemcpyAsync(&hc, dcnt, sizeof(hc), cudaMemcpyDeviceToHost, s), "D2H counters");
-        CK(cudaStreamSynchronize(s), "search kernel (retry)");
-        float ms2 = 0.f;
-        cudaEventElapsedTime(&ms2, t_ctx.ev0, t_ctx.ev1);
-        ms += ms2;
     }
     if (hc.overflowed > 0) return fail(JV_ERR_OVERFLOW, "graph_search: visited table / candidate list overflow after retries");
     if (stats) {
@@ -1225,10 +1206,10 @@ static int make_filter(const jv_search_options *opts, jv_graph g, int nq, bool b
         if (bits_on_device) f->accept_bits = opts->accept_bits;
         else {
             const size_t total = opts->accept_stride_words ? (size_t)opts->accept_stride_words * (size_t)(nq - 1) + words : words;
-            int rc = t_ctx.ensure(6, total * 4);
+            int rc = grow(t_ctx.accept_bits, total * 4);
             if (rc) return rc;
-            CK(cudaMemcpyAsync(t_ctx.dbuf[6], opts->accept_bits, total * 4, cudaMemcpyHostToDevice, t_ctx.stream), "H2D accept bits");
-            f->accept_bits = (const uint32_t *)t_ctx.dbuf[6];
+            CK(cudaMemcpyAsync(t_ctx.accept_bits.get(), opts->accept_bits, total * 4, cudaMemcpyHostToDevice, t_ctx.stream), "H2D accept bits");
+            f->accept_bits = t_ctx.accept_bits.get<uint32_t>();
         }
     }
     *use = f->accept_bits != nullptr || f->threshold > 0.f || f->rerank_floor > 0.f;
@@ -1262,7 +1243,17 @@ int jv_graph_search_batch_ex(jv_graph g, jv_dataset approx, jv_dataset reranker,
     if (!g || !approx || !queries || !nodes_out || !scores_out || nq <= 0 || topK < 1) return fail(JV_ERR_INVALID, "graph_search: bad arguments");
     int rc;
     const size_t qb = (size_t)nq * approx->d.dim * 4, ob = (size_t)nq * topK * 4;
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(0, qb)) || (rc = t_ctx.ensure(1, ob)) || (rc = t_ctx.ensure(2, ob))) return rc;
+    int32_t *dnodes;
+    float *dscores;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dnodes = c.take<int32_t>((size_t)nq * topK);
+        dscores = c.take<float>((size_t)nq * topK);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, qb)) || (rc = grow(t_ctx.output, carve(nullptr)))) return rc;
+    carve(t_ctx.output.get());
+    char *dq = t_ctx.input.get<char>();
     cudaStream_t s = t_ctx.stream;
     SearchFilter f;
     bool use;
@@ -1273,8 +1264,8 @@ int jv_graph_search_batch_ex(jv_graph g, jv_dataset approx, jv_dataset reranker,
     const char *ov = getenv("JV_SEARCH_OVERLAP");
     const bool overlap = qb >= ((size_t)1 << 20) && nq >= 64 && !(ov && ov[0] == '0');
     if (overlap) {
-        if ((rc = t_ctx.init_copy()) || (rc = t_ctx.ensure(7, 256))) return rc;
-        int *arrived = (int *)t_ctx.dbuf[7];
+        if ((rc = t_ctx.init_copy()) || (rc = grow(t_ctx.watermark, sizeof(int)))) return rc;
+        int *arrived = t_ctx.watermark.get<int>();
         CK(cudaMemsetAsync(arrived, 0, sizeof(int), s), "memset watermark");
         CK(cudaEventRecord(t_ctx.ev_copy, s), "event");
         cudaStream_t s2 = t_ctx.copy_stream;
@@ -1295,19 +1286,20 @@ int jv_graph_search_batch_ex(jv_graph g, jv_dataset approx, jv_dataset reranker,
             };
             const long long lo = bound(c), hi = bound(c + 1);
             if (hi <= lo) continue;
-            CK(cudaMemcpyAsync((char *)t_ctx.dbuf[0] + (size_t)lo * row, (const char *)queries + (size_t)lo * row, (size_t)(hi - lo) * row, cudaMemcpyHostToDevice, s2), "H2D queries");
-            t_ctx.marks_pinned[c] = (int)hi;
-            CK(cudaMemcpyAsync(arrived, &t_ctx.marks_pinned[c], sizeof(int), cudaMemcpyHostToDevice, s2), "H2D watermark");
+            CK(cudaMemcpyAsync(dq + (size_t)lo * row, (const char *)queries + (size_t)lo * row, (size_t)(hi - lo) * row, cudaMemcpyHostToDevice, s2), "H2D queries");
+            int *mark = t_ctx.marks.get<int>() + c;
+            *mark = (int)hi;
+            CK(cudaMemcpyAsync(arrived, mark, sizeof(int), cudaMemcpyHostToDevice, s2), "H2D watermark");
         }
         f.arrived = arrived;
-        rc = search_device(g, approx, reranker, metric, (const float *)t_ctx.dbuf[0], nq, topK, rerankK, &f, (int32_t *)t_ctx.dbuf[1], (float *)t_ctx.dbuf[2], stats);
+        rc = search_device(g, approx, reranker, metric, (const float *)dq, nq, topK, rerankK, &f, dnodes, dscores, stats);
     } else {
-        CK(cudaMemcpyAsync(t_ctx.dbuf[0], queries, qb, cudaMemcpyHostToDevice, s), "H2D queries");
-        rc = search_device(g, approx, reranker, metric, (const float *)t_ctx.dbuf[0], nq, topK, rerankK, use ? &f : nullptr, (int32_t *)t_ctx.dbuf[1], (float *)t_ctx.dbuf[2], stats);
+        CK(cudaMemcpyAsync(dq, queries, qb, cudaMemcpyHostToDevice, s), "H2D queries");
+        rc = search_device(g, approx, reranker, metric, (const float *)dq, nq, topK, rerankK, use ? &f : nullptr, dnodes, dscores, stats);
     }
     if (rc) return rc;
-    CK(cudaMemcpyAsync(nodes_out, t_ctx.dbuf[1], ob, cudaMemcpyDeviceToHost, s), "D2H nodes");
-    CK(cudaMemcpyAsync(scores_out, t_ctx.dbuf[2], ob, cudaMemcpyDeviceToHost, s), "D2H scores");
+    CK(cudaMemcpyAsync(nodes_out, dnodes, ob, cudaMemcpyDeviceToHost, s), "D2H nodes");
+    CK(cudaMemcpyAsync(scores_out, dscores, ob, cudaMemcpyDeviceToHost, s), "D2H scores");
     CK(cudaStreamSynchronize(s), "sync");
     return JV_OK;
 }
@@ -1359,27 +1351,24 @@ static int build_upper_levels(jv_graph g, jv_dataset f32, int metric, const Buil
     int entry = 0;
     assign_levels(n, degree, seed, members, &entry);
     g->g.entry_node = entry;
-    int rc;
     for (size_t l = 0; l < members.size(); l++) {
         const std::vector<int32_t> &ids = members[l];
         const int cnt = (int)ids.size();
         std::vector<int32_t> ladj((size_t)cnt * degree, -1);
         if (cnt > 1) {
-            jv_dataset_s sub;
-            sub.device = f32->device;
-            memset(&sub.d, 0, sizeof(DataDesc));
-            sub.d.kind = KIND_F32; sub.d.dim = f32->d.dim; sub.d.stride = f32->d.stride; sub.d.n = cnt;
-            float *drows = nullptr;
-            int32_t *dadj = nullptr, *dids = nullptr;
-            if ((rc = sub.alloc((void **)&drows, (size_t)cnt * sub.d.stride * 4)) || (rc = sub.alloc((void **)&dadj, (size_t)cnt * degree * 4)) ||
-                (rc = sub.alloc((void **)&dids, (size_t)cnt * 4)))
-                return rc;
-            cudaError_t e = cudaMemcpyAsync(dids, ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
-            if (e == cudaSuccess) e = launch_gather_rows(f32->d, dids, cnt, drows, s);
-            sub.d.rows = drows;
+            DataDesc sub;
+            memset(&sub, 0, sizeof(DataDesc));
+            sub.kind = KIND_F32; sub.dim = f32->d.dim; sub.stride = f32->d.stride; sub.n = cnt;
+            DeviceBuffer rows, adj, dids;  // the members' rows, their adjacency, their ids
+            cudaError_t e = rows.alloc((size_t)cnt * sub.stride * 4);
+            if (e == cudaSuccess) e = adj.alloc((size_t)cnt * degree * 4);
+            if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
+            if (e == cudaSuccess) e = launch_gather_rows(f32->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
+            sub.rows = rows.get<float>();
             BuildStats bs2;
-            if (e == cudaSuccess) e = build_graph_flat(sub.d, metric, bp, dadj, g_sm_count, &bs2, s);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(ladj.data(), dadj, ladj.size() * 4, cudaMemcpyDeviceToHost, s);
+            if (e == cudaSuccess) e = build_graph_flat(sub, metric, bp, adj.get<int32_t>(), g_sm_count, &bs2, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(ladj.data(), adj.get(), ladj.size() * 4, cudaMemcpyDeviceToHost, s);
             if (e == cudaSuccess) e = cudaStreamSynchronize(s);
             if (e != cudaSuccess) return cuda_fail(e, "build upper level");
             for (auto &x : ladj)
@@ -1402,30 +1391,24 @@ int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv
     BuildParams bp;
     if ((rc = build_params_check(params, &bp))) return rc;
     const int n = (int)f32->d.n, degree = params->degree;
-    jv_graph g = new jv_graph_s();
+    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
     g->device = f32->device;
     memset(&g->g, 0, sizeof(GraphDesc));
-    cudaError_t e = cudaMalloc((void **)&g->adj0, (size_t)n * degree * 4);
-    if (e != cudaSuccess) { delete g; return cuda_fail(e, "cudaMalloc(adjacency)"); }
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
-    cudaEventRecord(e0, s);
+    CK(g->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+    StreamTimer timer;
+    CK(timer.start(s), "event");
     BuildStats bs;
-    e = build_graph_flat(f32->d, metric, bp, g->adj0, g_sm_count, &bs, s);
+    cudaError_t e = build_graph_flat(f32->d, metric, bp, g->adj0.get<int32_t>(), g_sm_count, &bs, s);
     t_build_stats = bs;
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0;
+    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
     rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "build_graph_flat");
-    if (!rc && params->add_hierarchy && n > 1) rc = build_upper_levels(g, f32, metric, bp, params->seed, s);
-    cudaEventRecord(e1, s);  // the upper levels are part of the build and of its time
+    if (!rc && params->add_hierarchy && n > 1) rc = build_upper_levels(g.get(), f32, metric, bp, params->seed, s);
+    cudaError_t e1 = timer.stop(s);  // the upper levels are part of the build and of its time
     cudaStreamSynchronize(s);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    if (rc) { delete g; return rc; }
-    if (device_ms) *device_ms = ms;
-    *out = g;
+    if (rc) return rc;
+    CK(e1, "event");
+    if (device_ms) *device_ms = timer.ms();
+    *out = g.release();
     return JV_OK;
 }
 
@@ -1442,7 +1425,8 @@ struct jv_builder_s {
     BuildParams bp;
     GraphBuilder *B = nullptr;
     cudaStream_t stream = nullptr;
-    cudaEvent_t e0 = nullptr;
+    StreamTimer timer;  // jv_builder_create to jv_builder_finish
+    ~jv_builder_s() { builder_destroy(B); }
 };
 
 int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
@@ -1451,14 +1435,12 @@ int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params,
     if (!params || !out || f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "builder_create: needs an fp32 data set");
     int rc = check_metric(f32->d, metric);
     if (rc) return rc;
-    jv_builder b = new jv_builder_s();
+    std::unique_ptr<jv_builder_s> b(new jv_builder_s());
     b->device = f32->device; b->f32 = f32; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
-    if ((rc = build_params_check(params, &b->bp))) { delete b; return rc; }
-    cudaEventCreate(&b->e0);
-    cudaEventRecord(b->e0, b->stream);
-    cudaError_t e = builder_create(f32->d, metric, b->bp, g_sm_count, &b->B, b->stream);
-    if (e != cudaSuccess) { cudaEventDestroy(b->e0); delete b; return cuda_fail(e, "builder_create"); }
-    *out = b;
+    if ((rc = build_params_check(params, &b->bp))) return rc;
+    CK(b->timer.start(b->stream), "event");
+    CK(builder_create(f32->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
+    *out = b.release();
     return JV_OK;
 }
 
@@ -1535,26 +1517,20 @@ int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms)
     int rc;
     if ((rc = t_ctx.init())) return rc;
     const int n = (int)b->f32->d.n, degree = b->bp.degree;
-    jv_graph g = new jv_graph_s();
+    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
     g->device = b->device;
     memset(&g->g, 0, sizeof(GraphDesc));
-    cudaError_t e = cudaMalloc((void **)&g->adj0, (size_t)n * degree * 4);
-    if (e != cudaSuccess) { delete g; return cuda_fail(e, "cudaMalloc(adjacency)"); }
+    CK(g->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
     BuildStats bs;
-    e = builder_finish(b->B, g->adj0, &bs, b->stream);
+    cudaError_t e = builder_finish(b->B, g->adj0.get<int32_t>(), &bs, b->stream);
     t_build_stats = bs;
-    if (e != cudaSuccess) { delete g; return cuda_fail(e, "builder_finish"); }
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0;
-    if (b->params.add_hierarchy && n > 1 && (rc = build_upper_levels(g, b->f32, b->metric, b->bp, b->params.seed, b->stream))) { delete g; return rc; }
-    cudaEvent_t e1;
-    cudaEventCreate(&e1);
-    cudaEventRecord(e1, b->stream);
+    CK(e, "builder_finish");
+    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
+    if (b->params.add_hierarchy && n > 1 && (rc = build_upper_levels(g.get(), b->f32, b->metric, b->bp, b->params.seed, b->stream))) return rc;
+    CK(b->timer.stop(b->stream), "event");
     cudaStreamSynchronize(b->stream);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, b->e0, e1);
-    cudaEventDestroy(e1);
-    if (device_ms) *device_ms = ms;
-    *out = g;
+    if (device_ms) *device_ms = b->timer.ms();
+    *out = g.release();
     return JV_OK;
 }
 
@@ -1564,8 +1540,6 @@ int jv_builder_free(jv_builder b)
     cudaSetDevice(b->device);
     if (b->stream) cudaStreamSynchronize(b->stream);
     else cudaDeviceSynchronize();
-    builder_destroy(b->B);
-    if (b->e0) cudaEventDestroy(b->e0);
     delete b;
     return JV_OK;
 }
@@ -1594,38 +1568,35 @@ static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset f32, int met
         if (!bit_of(dead, v)) members.push_back(v);
     }
     std::sort(members.begin(), members.end());
-    int32_t *dmem = nullptr, *dids = nullptr, *dold = nullptr, *dnew = nullptr;
-    cudaError_t e = cudaMalloc((void **)&dmem, std::max<size_t>(members.size(), 1) * 4);
-    if (e == cudaSuccess && !members.empty()) e = cudaMemcpyAsync(dmem, members.data(), members.size() * 4, cudaMemcpyHostToDevice, s);
+    // level 0: g's adjacency is copied into ng's and repaired there; an upper level: its host rows are uploaded as old and new rows
+    DeviceBuffer dmem, dids, old_rows, new_rows;
+    int32_t *dold = g->adj0.get<int32_t>(), *dnew = ng->adj0.get<int32_t>();
+    cudaError_t e = dmem.alloc(std::max<size_t>(members.size(), 1) * 4);
+    if (e == cudaSuccess && !members.empty()) e = cudaMemcpyAsync(dmem.get(), members.data(), members.size() * 4, cudaMemcpyHostToDevice, s);
     if (level == 0) {
-        dold = g->adj0;
-        dnew = ng->adj0;
         if (e == cudaSuccess) e = cudaMemcpyAsync(dnew, dold, (size_t)n * degree * 4, cudaMemcpyDeviceToDevice, s);
     } else {
         const std::vector<int32_t> &adj = g->level_adj[level - 1];
-        if (e == cudaSuccess) e = cudaMalloc((void **)&dids, (size_t)rows * 4);
-        if (e == cudaSuccess) e = cudaMalloc((void **)&dold, adj.size() * 4);
-        if (e == cudaSuccess) e = cudaMalloc((void **)&dnew, adj.size() * 4);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(dids, ids->data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = dids.alloc((size_t)rows * 4);
+        if (e == cudaSuccess) e = old_rows.alloc(adj.size() * 4);
+        if (e == cudaSuccess) e = new_rows.alloc(adj.size() * 4);
+        dold = old_rows.get<int32_t>();
+        dnew = new_rows.get<int32_t>();
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids->data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(dold, adj.data(), adj.size() * 4, cudaMemcpyHostToDevice, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(dnew, adj.data(), adj.size() * 4, cudaMemcpyHostToDevice, s);
     }
-    const int32_t *rowmap = level ? g->upper_row + (size_t)(level - 1) * n : nullptr;
+    const int32_t *rowmap = level ? g->upper_row.get<int32_t>() + (size_t)(level - 1) * n : nullptr;
     if (e == cudaSuccess)
-        e = repair_level(f32->d, metric, alpha, degree, rows, dold, dnew, dids, rowmap, dead_dev, dmem, (int)members.size(), seed, level, g_sm_count, st, s);
+        e = repair_level(f32->d, metric, alpha, degree, rows, dold, dnew, dids.get<int32_t>(), rowmap, dead_dev, dmem.get<int32_t>(), (int)members.size(), seed,
+                         level, g_sm_count, st, s);
     if (e == cudaSuccess && level == 0) e = launch_clear_dead_rows(dnew, n, degree, dead_dev, s);
     if (e == cudaSuccess && level > 0) {
         adj_out->resize((size_t)rows * degree);
         e = cudaMemcpyAsync(adj_out->data(), dnew, adj_out->size() * 4, cudaMemcpyDeviceToHost, s);
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    else cudaStreamSynchronize(s);
-    cudaFree(dmem);
-    cudaFree(dids);
-    if (level > 0) {
-        cudaFree(dold);
-        cudaFree(dnew);
-    }
+    else cudaStreamSynchronize(s);  // the buffers above are freed on return
     return e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted");
 }
 
@@ -1655,28 +1626,27 @@ int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha,
         dead[w] |= h;
         gone += __builtin_popcount(dead[w]);
     }
-    jv_graph ng = new jv_graph_s();
+    std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
     ng->device = g->device;
     memset(&ng->g, 0, sizeof(GraphDesc));
     ng->g.n = n; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_node = -1; ng->g.entry_level = 0;
     ng->removed = dead;
-    uint32_t *dead_dev = nullptr;
+    DeviceBuffer dead_buf;
     RepairStats st;
     memset(&st, 0, sizeof(st));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
-    cudaEventRecord(e0, s);
-    cudaError_t e = cudaMalloc((void **)&ng->adj0, (size_t)n * degree * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&dead_dev, W * 4);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dead_dev, dead.data(), W * 4, cudaMemcpyHostToDevice, s);
+    StreamTimer timer;
+    CK(timer.start(s), "event");
+    cudaError_t e = ng->adj0.alloc((size_t)n * degree * 4);
+    if (e == cudaSuccess) e = dead_buf.alloc(W * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dead_buf.get(), dead.data(), W * 4, cudaMemcpyHostToDevice, s);
     rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted: allocation");
-    ng->g.adj0 = ng->adj0;
-    if (!rc) rc = remove_deleted_level(g, ng, f32, metric, alpha, seed, 0, dead, dead_dev, &st, nullptr, s);
+    ng->g.adj0 = ng->adj0.get<int32_t>();
+    const uint32_t *dead_dev = dead_buf.get<uint32_t>();
+    if (!rc) rc = remove_deleted_level(g, ng.get(), f32, metric, alpha, seed, 0, dead, dead_dev, &st, nullptr, s);
     // upper levels: repaired on the device like level 0, then their deleted members are dropped from the host copies
     for (int level = 1; !rc && level < g->g.levels; level++) {
         std::vector<int32_t> adj;
-        rc = remove_deleted_level(g, ng, f32, metric, alpha, seed, level, dead, dead_dev, &st, &adj, s);
+        rc = remove_deleted_level(g, ng.get(), f32, metric, alpha, seed, level, dead, dead_dev, &st, &adj, s);
         if (rc) break;
         const std::vector<int32_t> &ids = g->level_ids[level - 1];
         std::vector<int32_t> nids, nadj;
@@ -1704,24 +1674,19 @@ int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha,
                     if (!bit_of(dead, v)) { entry = v; break; }
         }
         ng->g.entry_node = entry;
-        rc = graph_rebuild_upper(ng);
+        rc = graph_rebuild_upper(ng.get());
     }
-    cudaEventRecord(e1, s);
+    timer.stop(s);
     cudaStreamSynchronize(s);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(dead_dev);
-    if (rc) { delete ng; return rc; }
+    if (rc) return rc;
     stats->live_nodes = (int32_t)(n - gone);
     stats->removed = (int32_t)(gone - holes);
     stats->repaired_rows = st.repaired_rows;
     stats->candidates = st.candidates;
     stats->max_candidates = st.max_candidates;
     stats->random_fallbacks = st.random_fallbacks;
-    stats->device_ms = ms;
-    *out = ng;
+    stats->device_ms = timer.ms();
+    *out = ng.release();
     return JV_OK;
 }
 
@@ -1733,38 +1698,26 @@ struct jv_query_batch_s {
     int device = 0;
     jv_dataset ds = nullptr;
     int metric = 0, nq = 0;
-    float *blobs = nullptr;        // [nq][blob_floats]
+    DeviceBuffer blobs;  // [nq][blob_floats]
     size_t blob_floats = 0;
-    // pinned + mapped staging (grown on demand)
-    int32_t *h_ids = nullptr, *h_off = nullptr;
-    float *h_scores = nullptr;
-    size_t cap_ids = 0, cap_off = 0;
-    int32_t *d_ids = nullptr, *d_off = nullptr;
-    float *d_scores = nullptr;
-    size_t dcap = 0;
+    // staging, grown on demand: pinned copies for pageable caller buffers, and the device side
+    PinnedBuffer h_ids, h_off, h_scores;
+    DeviceBuffer d_ids, d_off, d_scores;
     cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    StreamTimer timer;
     // single-hop path: mapped pinned ids / scores / completion flag the kernel reads and writes directly, a device-side CTA counter
-    int32_t *hop_ids = nullptr, *hop_ids_dev = nullptr;
-    float *hop_scores = nullptr, *hop_scores_dev = nullptr;
-    int *hop_flag = nullptr, *hop_flag_dev = nullptr, *hop_done = nullptr;
-    size_t hop_cap = 0;
+    PinnedBuffer hop_ids, hop_scores, hop_flag;
+    DeviceBuffer hop_done;
     int hop_seq = 0;
+    ~jv_query_batch_s()
+    {
+        cudaSetDevice(device);
+        if (stream) {
+            cudaStreamSynchronize(stream);
+            cudaStreamDestroy(stream);
+        }
+    }
 };
-
-static void query_batch_release(jv_query_batch_s *b)
-{
-    if (!b) return;
-    cudaSetDevice(b->device);
-    if (b->stream) cudaStreamSynchronize(b->stream);
-    cudaFree(b->blobs); cudaFree(b->d_ids); cudaFree(b->d_off); cudaFree(b->d_scores);
-    cudaFreeHost(b->h_ids); cudaFreeHost(b->h_off); cudaFreeHost(b->h_scores);
-    cudaFreeHost(b->hop_ids); cudaFreeHost(b->hop_scores); cudaFreeHost(b->hop_flag); cudaFree(b->hop_done);
-    if (b->ev0) cudaEventDestroy(b->ev0);
-    if (b->ev1) cudaEventDestroy(b->ev1);
-    if (b->stream) cudaStreamDestroy(b->stream);
-    delete b;
-}
 
 int jv_query_batch_begin(jv_dataset ds, int metric, const float *queries, int nq, jv_query_batch *out)
 {
@@ -1772,46 +1725,16 @@ int jv_query_batch_begin(jv_dataset ds, int metric, const float *queries, int nq
     if (!queries || !out || nq <= 0 || nq > 65535) return fail(JV_ERR_INVALID, "query_batch_begin: 1 <= nq <= 65535");
     int rc = check_metric(ds->d, metric);
     if (rc) return rc;
-    if ((rc = t_ctx.init()) || (rc = t_ctx.ensure(0, (size_t)nq * ds->d.dim * 4))) return rc;
-    jv_query_batch_s *b = new jv_query_batch_s();
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)nq * ds->d.dim * 4))) return rc;
+    std::unique_ptr<jv_query_batch_s> b(new jv_query_batch_s());
     b->device = ds->device; b->ds = ds; b->metric = metric; b->nq = nq; b->blob_floats = (size_t)blob_floats(ds->d);
-    cudaError_t e = cudaMalloc((void **)&b->blobs, (size_t)nq * b->blob_floats * 4);
+    cudaError_t e = b->blobs.alloc((size_t)nq * b->blob_floats * 4);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev0);
-    if (e == cudaSuccess) e = cudaEventCreate(&b->ev1);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(t_ctx.dbuf[0], queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, t_ctx.stream);
-    if (e == cudaSuccess) e = launch_prepare(ds->d, metric, (const float *)t_ctx.dbuf[0], nq, b->blobs, t_ctx.stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(t_ctx.input.get(), queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, t_ctx.stream);
+    if (e == cudaSuccess) e = launch_prepare(ds->d, metric, t_ctx.input.get<float>(), nq, b->blobs.get<float>(), t_ctx.stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(t_ctx.stream);
-    if (e != cudaSuccess) { query_batch_release(b); return cuda_fail(e, "query_batch_begin"); }
-    *out = b;
-    return JV_OK;
-}
-
-static int query_batch_staging(jv_query_batch_s *b, size_t total, size_t noff)
-{
-    if (total > b->cap_ids) {
-        cudaFreeHost(b->h_ids); cudaFreeHost(b->h_scores);
-        b->h_ids = nullptr; b->h_scores = nullptr; b->cap_ids = 0;
-        const size_t want = total + total / 2 + 256;
-        CK(cudaHostAlloc((void **)&b->h_ids, want * 4, cudaHostAllocMapped), "cudaHostAlloc(ids)");
-        CK(cudaHostAlloc((void **)&b->h_scores, want * 4, cudaHostAllocMapped), "cudaHostAlloc(scores)");
-        b->cap_ids = want;
-    }
-    if (noff > b->cap_off) {
-        cudaFreeHost(b->h_off);
-        b->h_off = nullptr; b->cap_off = 0;
-        CK(cudaHostAlloc((void **)&b->h_off, (noff + 64) * 4, cudaHostAllocMapped), "cudaHostAlloc(offsets)");
-        b->cap_off = noff + 64;
-    }
-    if (total > b->dcap) {
-        cudaFree(b->d_ids); cudaFree(b->d_scores); cudaFree(b->d_off);
-        b->d_ids = nullptr; b->d_scores = nullptr; b->d_off = nullptr; b->dcap = 0;
-        const size_t want = total + total / 2 + 256;
-        CK(cudaMalloc((void **)&b->d_ids, want * 4), "cudaMalloc(ids)");
-        CK(cudaMalloc((void **)&b->d_scores, want * 4), "cudaMalloc(scores)");
-        CK(cudaMalloc((void **)&b->d_off, ((size_t)b->nq + 64) * 4), "cudaMalloc(offsets)");
-        b->dcap = want;
-    }
+    CK(e, "query_batch_begin");
+    *out = b.release();
     return JV_OK;
 }
 
@@ -1829,8 +1752,13 @@ int jv_query_batch_score(jv_query_batch b, const int32_t *ids, const int32_t *of
     }
     if (device_ms) *device_ms = 0.0;
     if (total <= 0) return JV_OK;
-    int rc = query_batch_staging(b, (size_t)total, (size_t)nq + 1);
-    if (rc) return rc;
+    const size_t ib = (size_t)total * 4, ob = ((size_t)nq + 1) * 4;
+    CK(b->h_ids.grow(ib), "cudaHostAlloc(ids)");
+    CK(b->h_scores.grow(ib), "cudaHostAlloc(scores)");
+    CK(b->h_off.grow(ob), "cudaHostAlloc(offsets)");
+    CK(b->d_ids.grow(ib), "cudaMalloc(ids)");
+    CK(b->d_scores.grow(ib), "cudaMalloc(scores)");
+    CK(b->d_off.grow(ob), "cudaMalloc(offsets)");
     // caller buffers that are already pinned (jv_host_register / cudaHostAlloc) are copied from / to directly; pageable ones go
     // through the batch's own pinned staging so that the copies stay asynchronous and full speed
     auto pinned = [](const void *p) {
@@ -1839,22 +1767,19 @@ int jv_query_batch_score(jv_query_batch b, const int32_t *ids, const int32_t *of
         return a.type == cudaMemoryTypeHost;
     };
     const bool ids_pinned = pinned(ids), out_pinned = pinned(scores_out);
-    if (!ids_pinned) memcpy(b->h_ids, ids, (size_t)total * 4);
-    memcpy(b->h_off, offsets, ((size_t)nq + 1) * 4);
+    if (!ids_pinned) memcpy(b->h_ids.get(), ids, ib);
+    memcpy(b->h_off.get(), offsets, ob);
     cudaStream_t s = b->stream;
-    CK(cudaMemcpyAsync(b->d_ids, ids_pinned ? ids : b->h_ids, (size_t)total * 4, cudaMemcpyHostToDevice, s), "H2D ids");
-    CK(cudaMemcpyAsync(b->d_off, b->h_off, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, s), "H2D offsets");
-    CK(cudaEventRecord(b->ev0, s), "event");
-    CK(launch_score_ragged(b->ds->d, b->metric, b->blobs, nq, b->d_ids, b->d_off, 0, maxc, b->d_scores, s), "score_ragged");
-    CK(cudaEventRecord(b->ev1, s), "event");
-    CK(cudaMemcpyAsync(out_pinned ? scores_out : b->h_scores, b->d_scores, (size_t)total * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    CK(cudaMemcpyAsync(b->d_ids.get(), ids_pinned ? ids : b->h_ids.get(), ib, cudaMemcpyHostToDevice, s), "H2D ids");
+    CK(cudaMemcpyAsync(b->d_off.get(), b->h_off.get(), ob, cudaMemcpyHostToDevice, s), "H2D offsets");
+    CK(b->timer.start(s), "event");
+    CK(launch_score_ragged(b->ds->d, b->metric, b->blobs.get<float>(), nq, b->d_ids.get<int32_t>(), b->d_off.get<int32_t>(), 0, maxc, b->d_scores.get<float>(), s),
+       "score_ragged");
+    CK(b->timer.stop(s), "event");
+    CK(cudaMemcpyAsync(out_pinned ? scores_out : b->h_scores.get(), b->d_scores.get(), ib, cudaMemcpyDeviceToHost, s), "D2H scores");
     CK(cudaStreamSynchronize(s), "sync");
-    if (!out_pinned) memcpy(scores_out, b->h_scores, (size_t)total * 4);
-    if (device_ms) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, b->ev0, b->ev1);
-        *device_ms = ms;
-    }
+    if (!out_pinned) memcpy(scores_out, b->h_scores.get(), ib);
+    if (device_ms) *device_ms = b->timer.ms();
     return JV_OK;
 }
 
@@ -1866,31 +1791,24 @@ int jv_query_batch_score_one(jv_query_batch b, int query_index, const int32_t *i
     ON_DEVICE_OF(b);
     if (query_index < 0 || query_index >= b->nq || n < 0 || (n > 0 && (!ids || !scores_out))) return fail(JV_ERR_INVALID, "query_batch_score_one: bad arguments");
     if (n == 0) return JV_OK;
-    if ((size_t)n > b->hop_cap) {
-        CK(cudaStreamSynchronize(b->stream), "sync");
-        cudaFreeHost(b->hop_ids); cudaFreeHost(b->hop_scores);
-        b->hop_ids = nullptr; b->hop_scores = nullptr; b->hop_cap = 0;
-        const size_t want = (size_t)n + 1024;
-        CK(cudaHostAlloc((void **)&b->hop_ids, want * 4, cudaHostAllocMapped), "cudaHostAlloc(hop ids)");
-        CK(cudaHostAlloc((void **)&b->hop_scores, want * 4, cudaHostAllocMapped), "cudaHostAlloc(hop scores)");
-        CK(cudaHostGetDevicePointer((void **)&b->hop_ids_dev, b->hop_ids, 0), "cudaHostGetDevicePointer");
-        CK(cudaHostGetDevicePointer((void **)&b->hop_scores_dev, b->hop_scores, 0), "cudaHostGetDevicePointer");
-        if (!b->hop_flag) {
-            CK(cudaHostAlloc((void **)&b->hop_flag, 64, cudaHostAllocMapped), "cudaHostAlloc(hop flag)");
-            CK(cudaHostGetDevicePointer((void **)&b->hop_flag_dev, b->hop_flag, 0), "cudaHostGetDevicePointer");
-            *b->hop_flag = 0;
-            CK(cudaMalloc((void **)&b->hop_done, 64), "cudaMalloc(hop counter)");
-            CK(cudaMemset(b->hop_done, 0, 64), "memset");
-        }
-        b->hop_cap = want;
+    if ((size_t)n * 4 > b->hop_ids.capacity()) {
+        CK(cudaStreamSynchronize(b->stream), "sync");  // the previous hop's kernel is done with the blocks about to be replaced
+        CK(b->hop_ids.grow((size_t)n * 4), "cudaHostAlloc(hop ids)");
+        CK(b->hop_scores.grow((size_t)n * 4), "cudaHostAlloc(hop scores)");
     }
-    const float *blob = b->blobs + (size_t)query_index * b->blob_floats;
+    if (!b->hop_flag.get()) {
+        CK(b->hop_flag.grow(64), "cudaHostAlloc(hop flag)");
+        *b->hop_flag.get<int>() = 0;
+        CK(b->hop_done.alloc(64), "cudaMalloc(hop counter)");
+        CK(cudaMemset(b->hop_done.get(), 0, 64), "memset");
+    }
+    const float *blob = b->blobs.get<float>() + (size_t)query_index * b->blob_floats;
     if (n <= HOP_MAX_IDS) {
         // ids in the kernel parameters, every score word pre-set to a pattern no score can have and polled until it is overwritten
-        volatile uint32_t *sc = reinterpret_cast<volatile uint32_t *>(b->hop_scores);
+        volatile uint32_t *sc = b->hop_scores.get<volatile uint32_t>();
         for (int i = 0; i < n; i++) sc[i] = 0xffffffffu;
         __atomic_thread_fence(__ATOMIC_SEQ_CST);
-        CK(launch_score_hop(b->ds->d, b->metric, blob, ids, n, b->hop_scores_dev, b->stream), "score_hop");
+        CK(launch_score_hop(b->ds->d, b->metric, blob, ids, n, b->hop_scores.dev<float>(), b->stream), "score_hop");
         unsigned spins = 0;
         for (int i = 0; i < n; i++) {
             while (sc[i] == 0xffffffffu) {
@@ -1908,15 +1826,16 @@ int jv_query_batch_score_one(jv_query_batch b, int query_index, const int32_t *i
             }
         }
         __atomic_thread_fence(__ATOMIC_ACQUIRE);
-        memcpy(scores_out, b->hop_scores, (size_t)n * 4);
+        memcpy(scores_out, b->hop_scores.get(), (size_t)n * 4);
         return JV_OK;
     }
-    memcpy(b->hop_ids, ids, (size_t)n * 4);
+    memcpy(b->hop_ids.get(), ids, (size_t)n * 4);
     const int seq = ++b->hop_seq == 0 ? ++b->hop_seq : b->hop_seq;
     // one lane group per id and 4 ids per CTA: the hop's rows are fetched in one wave instead of one CTA walking them in turn
-    CK(launch_score_ragged(b->ds->d, b->metric, blob, 1, b->hop_ids_dev, nullptr, n, n, b->hop_scores_dev, b->stream, 4, b->hop_done, b->hop_flag_dev, seq),
+    CK(launch_score_ragged(b->ds->d, b->metric, blob, 1, b->hop_ids.dev<int32_t>(), nullptr, n, n, b->hop_scores.dev<float>(), b->stream, 4,
+                           b->hop_done.get<int>(), b->hop_flag.dev<int>(), seq),
        "score_ragged");
-    volatile int *flag = b->hop_flag;
+    volatile int *flag = b->hop_flag.get<volatile int>();
     for (unsigned spins = 1; *flag != seq; spins++) {
         if ((spins & 0x3fffu) == 0) {
             const cudaError_t e = cudaStreamQuery(b->stream);
@@ -1931,13 +1850,13 @@ int jv_query_batch_score_one(jv_query_batch b, int query_index, const int32_t *i
 #endif
     }
     __atomic_thread_fence(__ATOMIC_ACQUIRE);
-    memcpy(scores_out, b->hop_scores, (size_t)n * 4);
+    memcpy(scores_out, b->hop_scores.get(), (size_t)n * 4);
     return JV_OK;
 }
 
 int jv_query_batch_end(jv_query_batch b)
 {
-    query_batch_release(b);
+    delete b;
     return JV_OK;
 }
 
@@ -1955,6 +1874,7 @@ int jv_multi_free(jv_multi m)
         cudaSetDevice(m->devices[i]);
         delete m->ctx[i];
     }
+    if (!m->devices.empty()) cudaSetDevice(m->devices[0]);
     delete m;
     return JV_OK;
 }
@@ -2008,11 +1928,11 @@ int jv_multi_topk_bruteforce(jv_multi m, int metric, const float *queries, int n
         t_ctx_override = c0;
         cudaSetDevice(m->devices[0]);
         int rc = c0->init();
-        if (!rc) rc = c0->ensure(6, kb * parts + kb);
+        if (!rc) rc = grow(m->gathered, kb * parts + kb);
         t_ctx_override = nullptr;
         if (rc) return rc;
     }
-    long long *gathered = (long long *)c0->dbuf[6];
+    long long *gathered = m->gathered.get<long long>();
     auto work = [&](int i) {
         t_active = m->devices[i];
         t_ctx_override = m->ctx[i];
@@ -2020,11 +1940,11 @@ int jv_multi_topk_bruteforce(jv_multi m, int metric, const float *queries, int n
         int rc = JV_OK;
         do {
             if (cudaSetDevice(m->devices[i]) != cudaSuccess) { rc = fail(JV_ERR_CUDA, "cudaSetDevice"); break; }
-            if ((rc = c.init()) || (rc = c.ensure(0, qb)) || (rc = c.ensure(5, kb))) break;
-            if (cudaMemcpyAsync(c.dbuf[0], queries, qb, cudaMemcpyHostToDevice, c.stream) != cudaSuccess) { rc = fail(JV_ERR_CUDA, "H2D queries"); break; }
-            if ((rc = topk_device(m->shards[i], metric, (const float *)c.dbuf[0], nq, k, m->lo[i], (long long *)c.dbuf[5]))) break;
+            if ((rc = c.init()) || (rc = grow(c.input, qb)) || (rc = grow(c.output, kb))) break;
+            if (cudaMemcpyAsync(c.input.get(), queries, qb, cudaMemcpyHostToDevice, c.stream) != cudaSuccess) { rc = fail(JV_ERR_CUDA, "H2D queries"); break; }
+            if ((rc = topk_device(m->shards[i], metric, c.input.get<float>(), nq, k, m->lo[i], c.output.get<long long>()))) break;
             // shard keys -> the first device (NVLink peer copy; a plain device copy for shard 0)
-            cudaError_t e = cudaMemcpyPeerAsync(gathered + (size_t)i * nq * k, m->devices[0], c.dbuf[5], m->devices[i], kb, c.stream);
+            cudaError_t e = cudaMemcpyPeerAsync(gathered + (size_t)i * nq * k, m->devices[0], c.output.get(), m->devices[i], kb, c.stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(c.stream);
             if (e != cudaSuccess) rc = cuda_fail(e, "peer copy of shard keys");
         } while (0);

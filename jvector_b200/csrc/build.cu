@@ -19,10 +19,12 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <vector>
 
 #include <cub/cub.cuh>
 
+#include "host_mem.h"
 #include "kernels.h"
 
 namespace jv {
@@ -923,39 +925,28 @@ struct GraphBuilder {
     unsigned char *head_flag = nullptr, *node_flag = nullptr;
     SearchCounters *counters = nullptr;
     uint8_t *overflow = nullptr;
-    void *scratch = nullptr, *cub_tmp = nullptr;
-    size_t scratch_bytes = 0, cub_bytes = 0;
+    void *cub_tmp = nullptr;
+    size_t cub_bytes = 0;
     int32_t *own_rows = nullptr;  // single-GPU path: the slice buffers are the builder's own
     int *own_deg = nullptr;
-    int32_t *own_rp_rows = nullptr;
-    int *own_rp_deg = nullptr;
-    size_t own_rp_cap = 0;
+    std::vector<DeviceBuffer> mem;  // owns every block above
+    DeviceBuffer scratch;           // the insert searches' scratch, grown with the slice
     BuildStats st = {0, 0, 0, 0, 0};
     size_t psmem = 0;
     int prune_grid = 0;
 };
 
-static void builder_free(GraphBuilder *B)
-{
-    if (!B) return;
-    cudaFree(B->adj); cudaFree(B->res_nodes); cudaFree(B->list); cudaFree(B->head_target); cudaFree(B->iota); cudaFree(B->deg); cudaFree(B->mark);
-    cudaFree(B->list_count); cudaFree(B->work_counter); cudaFree(B->res_scores); cudaFree(B->dropped); cudaFree(B->pairs); cudaFree(B->pairs_sorted);
-    cudaFree(B->head_flag); cudaFree(B->node_flag); cudaFree(B->counters); cudaFree(B->overflow); cudaFree(B->scratch); cudaFree(B->cub_tmp);
-    cudaFree(B->own_rows); cudaFree(B->own_deg); cudaFree(B->own_rp_rows); cudaFree(B->own_rp_deg);
-    delete B;
-}
-
-void builder_destroy(GraphBuilder *B) { builder_free(B); }
+void builder_destroy(GraphBuilder *B) { delete B; }
 
 cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp, int sm_count, GraphBuilder **out, cudaStream_t s)
 {
     const int n = (int)d.n;
     if (d.kind != KIND_F32 || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
-    GraphBuilder *B = new GraphBuilder();
+    std::unique_ptr<GraphBuilder> B(new GraphBuilder());
     B->d = d; B->metric = metric; B->bp = bp; B->sm_count = sm_count; B->n = n; B->degree = bp.degree; B->beam = bp.beam;
     B->hard_max = (int)(bp.overflow * bp.degree);  // ConcurrentNeighborMap.java:300
     B->row_cap = std::max(2 * bp.degree, B->hard_max + 1);
-    if (B->row_cap > MAX_DEGREE) { delete B; return cudaErrorInvalidValue; }
+    if (B->row_cap > MAX_DEGREE) return cudaErrorInvalidValue;
     B->max_batch = bp.max_batch > 0 ? bp.max_batch : 16384;
     if (const char *e = getenv("JV_BUILD_BATCH_DIV")) B->batch_div = atoi(e) > 0 ? atoi(e) : 32;  // tuning knob (tools/build_quality.py)
     // in-progress window: as many concurrently inserting peers as still fit the 128-candidate Gram tile next to the beam
@@ -964,38 +955,32 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
     B->prune_grid = sm_count * 5;  // ~10 KB of shared memory per CTA: register-limited residency
     cudaError_t err = cudaSuccess;
     const size_t mb = (size_t)B->max_batch;
-#define ALLOC(ptr, bytes)                                                  \
-    do {                                                                   \
-        err = cudaMalloc((void **)&(ptr), (bytes));                        \
-        if (err != cudaSuccess) { builder_free(B); return err; }           \
-    } while (0)
-    ALLOC(B->adj, (size_t)n * B->row_cap * 4);
-    ALLOC(B->deg, (size_t)n * 4);
-    ALLOC(B->mark, (size_t)n * 4);
-    ALLOC(B->res_nodes, mb * B->beam * 4);
-    ALLOC(B->res_scores, mb * B->beam * 4);
-    ALLOC(B->list, (size_t)n * 4);
-    ALLOC(B->iota, (size_t)n * 4);
-    ALLOC(B->node_flag, (size_t)n);
-    ALLOC(B->list_count, 16);
-    ALLOC(B->work_counter, 16);
-    ALLOC(B->dropped, 16);
-    ALLOC(B->counters, sizeof(SearchCounters));
-    ALLOC(B->overflow, mb);
-    ALLOC(B->pairs, mb * B->degree * 8);
-    ALLOC(B->pairs_sorted, mb * B->degree * 8);
-    ALLOC(B->head_flag, mb * B->degree);
-    ALLOC(B->head_target, mb * B->degree * 4);
-    ALLOC(B->own_rows, mb * B->degree * 4);
-    ALLOC(B->own_deg, mb * 4);
-#undef ALLOC
+    auto &owned = B->mem;
+    JV_TRY(alloc_owned(owned, B->adj, (size_t)n * B->row_cap * 4));
+    JV_TRY(alloc_owned(owned, B->deg, (size_t)n * 4));
+    JV_TRY(alloc_owned(owned, B->mark, (size_t)n * 4));
+    JV_TRY(alloc_owned(owned, B->res_nodes, mb * B->beam * 4));
+    JV_TRY(alloc_owned(owned, B->res_scores, mb * B->beam * 4));
+    JV_TRY(alloc_owned(owned, B->list, (size_t)n * 4));
+    JV_TRY(alloc_owned(owned, B->iota, (size_t)n * 4));
+    JV_TRY(alloc_owned(owned, B->node_flag, (size_t)n));
+    JV_TRY(alloc_owned(owned, B->list_count, 16));
+    JV_TRY(alloc_owned(owned, B->work_counter, 16));
+    JV_TRY(alloc_owned(owned, B->dropped, 16));
+    JV_TRY(alloc_owned(owned, B->counters, sizeof(SearchCounters)));
+    JV_TRY(alloc_owned(owned, B->overflow, mb));
+    JV_TRY(alloc_owned(owned, B->pairs, mb * B->degree * 8));
+    JV_TRY(alloc_owned(owned, B->pairs_sorted, mb * B->degree * 8));
+    JV_TRY(alloc_owned(owned, B->head_flag, mb * B->degree));
+    JV_TRY(alloc_owned(owned, B->head_target, mb * B->degree * 4));
+    JV_TRY(alloc_owned(owned, B->own_rows, mb * B->degree * 4));
+    JV_TRY(alloc_owned(owned, B->own_deg, mb * 4));
     {
         size_t b1 = 0, b2 = 0;
         cub::DeviceRadixSort::SortKeys(nullptr, b1, B->pairs, B->pairs_sorted, (int)(mb * B->degree), 0, 64, s);
         cub::DeviceSelect::Flagged(nullptr, b2, B->iota, B->node_flag, B->list, B->list_count, n, s);
         B->cub_bytes = std::max(b1, b2) + 256;
-        err = cudaMalloc(&B->cub_tmp, B->cub_bytes);
-        if (err != cudaSuccess) { builder_free(B); return err; }
+        JV_TRY(alloc_owned(owned, B->cub_tmp, B->cub_bytes));
     }
     JV_TRY(cudaMemsetAsync(B->adj, 0xff, (size_t)n * B->row_cap * 4, s));
     JV_TRY(cudaMemsetAsync(B->deg, 0, (size_t)n * 4, s));
@@ -1005,8 +990,9 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
     JV_TRY(cudaMemsetAsync(B->counters, 0, sizeof(SearchCounters), s));
     iota_kernel<<<(n + 255) / 256, 256, 0, s>>>(B->iota, n);
     g_launches++;
-    *out = B;
-    return cudaGetLastError();
+    JV_TRY(cudaGetLastError());
+    *out = B.release();
+    return cudaSuccess;
 }
 
 // the next batch: 1/32 of what is already inserted, at most max_batch — every batch searches a graph that already holds 97 % of the
@@ -1044,18 +1030,11 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
     g.n = B->n; g.degree = B->row_cap; g.levels = 1; g.entry_node = 0; g.entry_level = 0; g.adj0 = B->adj;
     SearchPlan plan;
     JV_TRY(plan_search(B->d, nullptr, g, B->beam, B->beam, m, 0, 0, B->sm_count, &plan));
-    const size_t need = search_scratch_bytes(plan);
-    if (need > B->scratch_bytes) {
-        if (B->scratch) cudaFree(B->scratch);
-        B->scratch = nullptr;
-        B->scratch_bytes = 0;
-        JV_TRY(cudaMalloc(&B->scratch, need));
-        B->scratch_bytes = need;
-    }
+    JV_TRY(B->scratch.grow(search_scratch_bytes(plan)));
     SearchFilter lenient;
     memset(&lenient, 0, sizeof(lenient));
     lenient.lenient = 1;  // an insert search never fails the build: see SearchParams::lenient
-    JV_TRY(launch_search(g, B->d, nullptr, B->metric, B->d.rows + (size_t)(first + lo) * B->d.stride, m, B->beam, B->beam, plan, B->scratch, B->work_counter,
+    JV_TRY(launch_search(g, B->d, nullptr, B->metric, B->d.rows + (size_t)(first + lo) * B->d.stride, m, B->beam, B->beam, plan, B->scratch.get(), B->work_counter,
                          B->res_nodes, B->res_scores, B->counters, B->overflow, nullptr, B->d.stride, &lenient, s));
     PruneParams P = prune_params(B);
     P.mode = 0; P.node_base = first + lo; P.count = m; P.cand = B->res_nodes; P.cand_stride = B->beam;
@@ -1171,7 +1150,7 @@ cudaError_t build_graph_flat(const DataDesc &d, int metric, const BuildParams &b
     if (err == cudaSuccess) err = builder_reprune_slice(B, 0, 0, nullptr, nullptr, s);
     if (err == cudaSuccess) err = builder_finish(B, adj_out_dev, stats, s);
     else if (stats) *stats = B->st;
-    builder_free(B);
+    delete B;
     return err;
 }
 
@@ -1381,83 +1360,72 @@ static cudaError_t launch_repair_prune(const PruneParams &P, int tier, int grid,
     return launch_repair_prune_t<JV_METRIC_COSINE>(P, tier, grid, s);
 }
 
-cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new, const int32_t *ids_dev,
-                         const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev, int nmembers, uint64_t seed, int level,
-                         int sm_count, RepairStats *st, cudaStream_t s)
+// repair_level's work, enqueued on `s`; every block it allocates goes to `mem`
+static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new,
+                                        const int32_t *ids_dev, const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev,
+                                        int nmembers, uint64_t seed, int level, int sm_count, RepairStats *st, std::vector<DeviceBuffer> &mem,
+                                        cudaStream_t s)
 {
     cudaError_t err = cudaSuccess;
-    if (rows <= 0) return cudaSuccess;
-    if (degree < 1 || degree > 64) return cudaErrorInvalidValue;
-    unsigned char *flag = nullptr, *fallback = nullptr;
-    long long *cnt = nullptr, *off_all = nullptr, *cand_off = nullptr;
-    int32_t *iota = nullptr, *aff = nullptr, *cand = nullptr, *row_node = nullptr, *out_rows = nullptr, *tier_list = nullptr;
-    int *naff_dev = nullptr, *cand_cnt = nullptr, *out_deg = nullptr;
-    void *tmp = nullptr;
-    int naff = 0;
-    long long total = 0;
-    std::vector<int> hcnt;
-    std::vector<unsigned char> hfb;
-    std::vector<int32_t> tiers[REPAIR_TIERS];
-    std::vector<int32_t> hlist;
-    size_t tb = 0, t1 = 0, t2 = 0;
-#define R_TRY(x)                                 \
-    do {                                         \
-        err = (x);                               \
-        if (err != cudaSuccess) goto done;       \
-    } while (0)
-    R_TRY(cudaMalloc(&flag, (size_t)rows));
-    R_TRY(cudaMalloc(&cnt, (size_t)rows * 8));
-    R_TRY(cudaMalloc(&off_all, (size_t)rows * 8));
-    R_TRY(cudaMalloc(&iota, (size_t)rows * 4));
-    R_TRY(cudaMalloc(&aff, (size_t)rows * 4));
-    R_TRY(cudaMalloc(&naff_dev, 16));
+    unsigned char *flag, *fallback;
+    long long *cnt, *off_all, *cand_off;
+    int32_t *iota, *aff, *cand, *row_node, *out_rows, *tier_list;
+    int *naff_dev, *cand_cnt, *out_deg;
+    void *tmp;
+    JV_TRY(alloc_owned(mem, flag, (size_t)rows));
+    JV_TRY(alloc_owned(mem, cnt, (size_t)rows * 8));
+    JV_TRY(alloc_owned(mem, off_all, (size_t)rows * 8));
+    JV_TRY(alloc_owned(mem, iota, (size_t)rows * 4));
+    JV_TRY(alloc_owned(mem, aff, (size_t)rows * 4));
+    JV_TRY(alloc_owned(mem, naff_dev, 16));
     repair_count_kernel<<<(unsigned)(((long long)rows * 32 + 255) / 256), 256, 0, s>>>(adj_old, rows, degree, ids_dev, rowmap_dev, dead_dev, flag, cnt);
     g_launches++;
     iota_kernel<<<(rows + 255) / 256, 256, 0, s>>>(iota, rows);
     g_launches++;
-    R_TRY(cudaGetLastError());
+    JV_TRY(cudaGetLastError());
+    size_t t1 = 0, t2 = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, t1, cnt, off_all, rows, s);
     cub::DeviceSelect::Flagged(nullptr, t2, iota, flag, aff, naff_dev, rows, s);
-    tb = std::max(t1, t2) + 256;
-    R_TRY(cudaMalloc(&tmp, tb));
+    const size_t tb = std::max(t1, t2) + 256;
+    JV_TRY(alloc_owned(mem, tmp, tb));
     t1 = tb;
-    R_TRY(cub::DeviceScan::ExclusiveSum(tmp, t1, cnt, off_all, rows, s));
+    JV_TRY(cub::DeviceScan::ExclusiveSum(tmp, t1, cnt, off_all, rows, s));
     g_launches++;
     t2 = tb;
-    R_TRY(cub::DeviceSelect::Flagged(tmp, t2, iota, flag, aff, naff_dev, rows, s));
+    JV_TRY(cub::DeviceSelect::Flagged(tmp, t2, iota, flag, aff, naff_dev, rows, s));
     g_launches++;
-    {
-        long long last[2] = {0, 0};
-        R_TRY(cudaMemcpyAsync(&naff, naff_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
-        R_TRY(cudaMemcpyAsync(&last[0], off_all + rows - 1, 8, cudaMemcpyDeviceToHost, s));
-        R_TRY(cudaMemcpyAsync(&last[1], cnt + rows - 1, 8, cudaMemcpyDeviceToHost, s));
-        R_TRY(cudaStreamSynchronize(s));
-        total = last[0] + last[1];
-    }
-    if (naff == 0) goto done;
-    R_TRY(cudaMalloc(&cand, (size_t)std::max(total, 1ll) * 4));
-    R_TRY(cudaMalloc(&row_node, (size_t)naff * 4));
-    R_TRY(cudaMalloc(&cand_off, (size_t)naff * 8));
-    R_TRY(cudaMalloc(&cand_cnt, (size_t)naff * 4));
-    R_TRY(cudaMalloc(&fallback, (size_t)naff));
-    R_TRY(cudaMalloc(&out_rows, (size_t)naff * degree * 4));
-    R_TRY(cudaMalloc(&out_deg, (size_t)naff * 4));
-    R_TRY(cudaMalloc(&tier_list, (size_t)naff * 4));
+    int naff = 0;
+    long long last[2] = {0, 0};
+    JV_TRY(cudaMemcpyAsync(&naff, naff_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
+    JV_TRY(cudaMemcpyAsync(&last[0], off_all + rows - 1, 8, cudaMemcpyDeviceToHost, s));
+    JV_TRY(cudaMemcpyAsync(&last[1], cnt + rows - 1, 8, cudaMemcpyDeviceToHost, s));
+    JV_TRY(cudaStreamSynchronize(s));
+    const long long total = last[0] + last[1];
+    if (naff == 0) return cudaSuccess;
+    JV_TRY(alloc_owned(mem, cand, (size_t)std::max(total, 1ll) * 4));
+    JV_TRY(alloc_owned(mem, row_node, (size_t)naff * 4));
+    JV_TRY(alloc_owned(mem, cand_off, (size_t)naff * 8));
+    JV_TRY(alloc_owned(mem, cand_cnt, (size_t)naff * 4));
+    JV_TRY(alloc_owned(mem, fallback, (size_t)naff));
+    JV_TRY(alloc_owned(mem, out_rows, (size_t)naff * degree * 4));
+    JV_TRY(alloc_owned(mem, out_deg, (size_t)naff * 4));
+    JV_TRY(alloc_owned(mem, tier_list, (size_t)naff * 4));
     {
         int cap = 256;
         while (cap < degree * (degree + 2)) cap <<= 1;
         const size_t gsm = (size_t)cap * 4;
-        R_TRY(cudaFuncSetAttribute(repair_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm));
+        JV_TRY(cudaFuncSetAttribute(repair_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm));
         repair_gather_kernel<<<std::min(naff, sm_count * 8), 256, gsm, s>>>(adj_old, degree, ids_dev, rowmap_dev, dead_dev, aff, naff, off_all, cap, members_dev,
                                                                            nmembers, (unsigned long long)seed, level, cand, row_node, cand_off, cand_cnt, fallback);
         g_launches++;
-        R_TRY(cudaGetLastError());
+        JV_TRY(cudaGetLastError());
     }
-    hcnt.resize(naff);
-    hfb.resize(naff);
-    R_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)naff * 4, cudaMemcpyDeviceToHost, s));
-    R_TRY(cudaMemcpyAsync(hfb.data(), fallback, (size_t)naff, cudaMemcpyDeviceToHost, s));
-    R_TRY(cudaStreamSynchronize(s));
+    std::vector<int> hcnt(naff);
+    std::vector<unsigned char> hfb(naff);
+    JV_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)naff * 4, cudaMemcpyDeviceToHost, s));
+    JV_TRY(cudaMemcpyAsync(hfb.data(), fallback, (size_t)naff, cudaMemcpyDeviceToHost, s));
+    JV_TRY(cudaStreamSynchronize(s));
+    std::vector<int32_t> tiers[REPAIR_TIERS];
     for (int a = 0; a < naff; a++) {
         int t = 0;
         while (t < REPAIR_TIERS - 1 && hcnt[a] > REPAIR_TIER_MAX[t]) t++;
@@ -1468,8 +1436,9 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
         st->tier_rows[t]++;
     }
     st->repaired_rows += naff;
+    std::vector<int32_t> hlist;
     for (int t = 0; t < REPAIR_TIERS; t++) hlist.insert(hlist.end(), tiers[t].begin(), tiers[t].end());
-    R_TRY(cudaMemcpyAsync(tier_list, hlist.data(), (size_t)naff * 4, cudaMemcpyHostToDevice, s));
+    JV_TRY(cudaMemcpyAsync(tier_list, hlist.data(), (size_t)naff * 4, cudaMemcpyHostToDevice, s));
     {
         PruneParams P;
         memset(&P, 0, sizeof(P));
@@ -1482,20 +1451,26 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
             if (c == 0) continue;
             P.list = tier_list + first;
             P.count = c;
-            R_TRY(launch_repair_prune(P, t, std::min(c, sm_count * 5), s));
+            JV_TRY(launch_repair_prune(P, t, std::min(c, sm_count * 5), s));
             first += c;
         }
     }
     repair_scatter_kernel<<<(unsigned)(((long long)naff * degree + 255) / 256), 256, 0, s>>>(adj_new, degree, aff, naff, out_rows);
     g_launches++;
-    R_TRY(cudaGetLastError());
-    R_TRY(cudaStreamSynchronize(s));  // the scratch below is freed on return
-done:
-#undef R_TRY
-    if (err != cudaSuccess) cudaStreamSynchronize(s);
-    cudaFree(flag); cudaFree(cnt); cudaFree(off_all); cudaFree(iota); cudaFree(aff); cudaFree(naff_dev); cudaFree(tmp);
-    cudaFree(cand); cudaFree(row_node); cudaFree(cand_off); cudaFree(cand_cnt); cudaFree(fallback); cudaFree(out_rows); cudaFree(out_deg); cudaFree(tier_list);
-    return err;
+    return cudaGetLastError();
+}
+
+cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new, const int32_t *ids_dev,
+                         const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev, int nmembers, uint64_t seed, int level,
+                         int sm_count, RepairStats *st, cudaStream_t s)
+{
+    if (rows <= 0) return cudaSuccess;
+    if (degree < 1 || degree > 64) return cudaErrorInvalidValue;
+    std::vector<DeviceBuffer> mem;  // the scratch goes when this returns: the stream drains first, on success and on error
+    const cudaError_t err = repair_level_enqueue(d, metric, alpha, degree, rows, adj_old, adj_new, ids_dev, rowmap_dev, dead_dev, members_dev, nmembers,
+                                                 seed, level, sm_count, st, mem, s);
+    const cudaError_t drained = cudaStreamSynchronize(s);
+    return err != cudaSuccess ? err : drained;
 }
 
 }  // namespace jv
