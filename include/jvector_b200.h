@@ -295,7 +295,8 @@ typedef struct {
     uint64_t seed;
     int max_batch;     /* 0 = default (16384): nodes inserted per round; they play the reference's concurrently inserting threads */
     int concurrent_window; /* in-progress peers each insert sees besides its beam (getConcurrentCandidates,
-                              GraphIndexBuilder.java:823-837): -1 = default (what fits the 128-candidate prune tile, <= 32), 0 = none */
+                              GraphIndexBuilder.java:823-837): -1 = default (what fits the 128-candidate prune tile, <= 32), 0 = none;
+                              beam_width + concurrent_window <= 256 (the prune's candidate capacity), else JV_ERR_INVALID */
 } jv_build_params;
 JV_API int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv_graph *out, double *device_ms);
 /* The same build advanced batch by batch, for a build SHARDED over several GPUs (BASELINE config 5): every participant holds a
@@ -317,6 +318,10 @@ JV_API int jv_builder_apply_repruned(jv_builder b, int32_t count, const int32_t 
 /* cleanup(): the sorted list of rows longer than M (enforceDegree), to be re-pruned with the two calls above */
 JV_API int jv_builder_collect_over_degree(jv_builder b, int32_t *rows);
 JV_API int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms);
+/* counters so far (synchronises the builder's stream; valid before and after jv_builder_finish): batches applied, insert searches
+ * cut short by a full visited table or an oversized tie tail (0 = every insert search was exact), back-links dropped because the
+ * target's row was full */
+JV_API int jv_builder_stats(jv_builder b, int64_t *batches, int64_t *truncated_searches, int64_t *dropped_backlinks);
 JV_API int jv_builder_free(jv_builder b);
 /* counters of this thread's last jv_graph_build (level 0): vectors scored by the insert searches, batches, back-links dropped */
 JV_API int jv_graph_build_stats(int64_t *scored_vectors, int64_t *batches, int64_t *dropped_backlinks);

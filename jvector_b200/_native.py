@@ -104,7 +104,8 @@ SYMBOLS = [
     ("jv_builder_next_batch", _I, [_P, i32p, i32p]), ("jv_builder_insert_slice", _I, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     ("jv_builder_apply_new", _I, [_P, C.c_int32, C.c_int32, _P, _P, i32p]), ("jv_builder_reprune_slice", _I, [_P, C.c_int32, C.c_int32, _P, _P]),
     ("jv_builder_apply_repruned", _I, [_P, C.c_int32, _P, _P]), ("jv_builder_collect_over_degree", _I, [_P, i32p]),
-    ("jv_builder_finish", _I, [_P, C.POINTER(_P), C.POINTER(C.c_double)]), ("jv_builder_free", _I, [_P]),
+    ("jv_builder_finish", _I, [_P, C.POINTER(_P), C.POINTER(C.c_double)]), ("jv_builder_stats", _I, [_P, i64p, i64p, i64p]),
+    ("jv_builder_free", _I, [_P]),
     ("jv_device_malloc", _I, [C.POINTER(_P), _Z]), ("jv_device_free", _I, [_P]), ("jv_memcpy_h2d", _I, [_P, _P, _Z]),
     ("jv_memcpy_d2h", _I, [_P, _P, _Z]), ("jv_host_register", _I, [_P, _Z]), ("jv_host_unregister", _I, [_P]),
     ("jv_device_synchronize", _I, []), ("jv_kernel_launch_count", _L, []),

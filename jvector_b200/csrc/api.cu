@@ -1314,6 +1314,9 @@ static int build_params_check(const jv_build_params *params, BuildParams *bp)
 {
     if (params->degree < 1 || params->degree > 64 || params->beam_width < 1 || params->beam_width > 256 || params->overflow < 1.0f || params->alpha < 1.0f)
         return fail(JV_ERR_INVALID, "graph_build: need 1 <= degree <= 64, 1 <= beam <= 256, overflow >= 1, alpha >= 1");
+    // the prune holds at most 256 candidates: a wider beam + window would silently lose the last window peers
+    if (params->concurrent_window >= 0 && params->beam_width + params->concurrent_window > 256)
+        return fail(JV_ERR_INVALID, "graph_build: need beam + concurrent_window <= 256");
     bp->degree = params->degree; bp->beam = params->beam_width; bp->overflow = params->overflow; bp->alpha = params->alpha;
     bp->max_batch = params->max_batch; bp->window = params->concurrent_window;
     return JV_OK;
@@ -1531,6 +1534,17 @@ int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms)
     cudaStreamSynchronize(b->stream);
     if (device_ms) *device_ms = b->timer.ms();
     *out = g.release();
+    return JV_OK;
+}
+
+int jv_builder_stats(jv_builder b, int64_t *batches, int64_t *truncated_searches, int64_t *dropped_backlinks)
+{
+    ON_DEVICE_OF(b);
+    BuildStats bs;
+    CK(builder_stats(b->B, &bs, b->stream), "builder_stats");
+    if (batches) *batches = bs.batches;
+    if (truncated_searches) *truncated_searches = bs.truncated_searches;
+    if (dropped_backlinks) *dropped_backlinks = bs.dropped_backlinks;
     return JV_OK;
 }
 

@@ -10,8 +10,8 @@
 //   search  : graph_search_kernel (search.cu) over the batch, one CTA per inserted node, beam = efConstruction
 //   prune   : prune_kernel, one CTA per node: scores -> sort by the reference key -> retainDiverse restated over a running
 //             max-similarity per candidate, updated in bulk whenever a neighbour is selected (SURVEY §3.2 seam v)
-//   backlink: append u to adj[v] for every chosen v (atomic slot), then prune_kernel again over every v whose list
-//             passed overflow * M
+//   backlink: append u to adj[v] for every chosen v (sorted (v, u) pairs, slot deg_before[v] + rank; a pair past the row's
+//             capacity is dropped and counted), then prune_kernel again over every v whose list passed overflow * M
 // Batches grow geometrically (x 33/32, JV_BUILD_BATCH_DIV) up to max_batch so early nodes see a connected graph. Neighbour lists in the
 // reference are concurrency-order dependent, so parity is on scores and on the recall of the resulting graph
 // (SURVEY §8d C5), not on identical adjacency.
@@ -258,6 +258,18 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
 constexpr int GRAM_KC = 32;
 constexpr int GRAM_PITCH = 36;
 
+// floats [k, k + 4) of candidate `node` as the Gram product stages them. L2 takes x_node - x_v, the row translated by the pruned
+// node's own: distances do not change, and G_ii + G_jj - 2 G_ij then carries an error relative to the neighbourhood's size
+// (|x_i - x_v| + |x_j - x_v|)^2 instead of to |x|^2, which on rows sharing a large offset swamps the distances themselves.
+template <int METRIC>
+__device__ __forceinline__ float4 gram_row(const DataDesc &d, int32_t node, int v, int k)
+{
+    const float4 x = __ldg(reinterpret_cast<const float4 *>(d.rows + (size_t)node * d.stride + k));
+    if (METRIC != JV_METRIC_EUCLIDEAN) return x;
+    const float4 y = __ldg(reinterpret_cast<const float4 *>(d.rows + (size_t)v * d.stride + k));
+    return make_float4(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y), __fsub_rn(x.z, y.z), __fsub_rn(x.w, y.w));
+}
+
 template <int METRIC, int TILE>
 __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P)
 {
@@ -334,7 +346,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
         }
         __syncthreads();
 
-        // ---- Gram matrix of the candidate rows ----
+        // ---- Gram matrix of the candidate rows (L2: translated by v's row, see gram_row) ----
         float acc[NB][NB];
 #pragma unroll
         for (int a = 0; a < NB; a++)
@@ -346,7 +358,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
                 const int r = t / (GRAM_KC / 4), c4 = t - r * (GRAM_KC / 4);
                 float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
                 const int32_t node = ids[r];
-                if (node >= 0 && k0 + 4 * c4 < P.d.stride) val = __ldg(reinterpret_cast<const float4 *>(P.d.rows + (size_t)node * P.d.stride + k0) + c4);
+                if (node >= 0 && k0 + 4 * c4 < P.d.stride) val = gram_row<METRIC>(P.d, node, v, k0 + 4 * c4);
                 *reinterpret_cast<float4 *>(tileA + r * GRAM_PITCH + 4 * c4) = val;
             }
             __syncthreads();
@@ -585,16 +597,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
         }
         __syncthreads();
 
-        // ---- Gram matrix of the candidate rows on the tensor cores (3xTF32) ----
-        const float *rowp[PASSES];
+        // ---- Gram matrix of the candidate rows on the tensor cores (3xTF32; L2: translated by v's row, see gram_row) ----
+        int32_t rnode[PASSES];
 #pragma unroll
-        for (int j = 0; j < PASSES; j++) {
-            const int32_t node = ids[r0 + 32 * j];
-            rowp[j] = node >= 0 ? P.d.rows + (size_t)node * P.d.stride + 4 * c4 : nullptr;
-        }
+        for (int j = 0; j < PASSES; j++) rnode[j] = ids[r0 + 32 * j];
         float4 pre[PASSES];
 #pragma unroll
-        for (int j = 0; j < PASSES; j++) pre[j] = (rowp[j] && 4 * c4 < P.d.stride) ? __ldg(reinterpret_cast<const float4 *>(rowp[j])) : make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int j = 0; j < PASSES; j++) pre[j] = (rnode[j] >= 0 && 4 * c4 < P.d.stride) ? gram_row<METRIC>(P.d, rnode[j], v, 4 * c4) : make_float4(0.f, 0.f, 0.f, 0.f);
         for (int c = 0; c < nchunks; c++) {
             const int b = c & 1;
             if (c >= 2) {  // the MMAs of chunk c - 2 (both warpgroups) have read this buffer
@@ -619,7 +628,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
                 const int k1 = (c + 1) * 32 + 4 * c4;
 #pragma unroll
                 for (int j = 0; j < PASSES; j++)
-                    pre[j] = (rowp[j] && k1 < P.d.stride) ? __ldg(reinterpret_cast<const float4 *>(rowp[j] + (c + 1) * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    pre[j] = (rnode[j] >= 0 && k1 < P.d.stride) ? gram_row<METRIC>(P.d, rnode[j], v, k1) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
             fence_proxy_async();
             __syncthreads();
@@ -1110,13 +1119,10 @@ cudaError_t builder_list_count(GraphBuilder *B, int *count_host, cudaStream_t s)
     return cudaStreamSynchronize(s);
 }
 
-cudaError_t builder_finish(GraphBuilder *B, int32_t *adj_out_dev, BuildStats *stats, cudaStream_t s)
+// the counters so far: batches applied, insert searches cut short, back-links dropped at a full row (synchronises `s`)
+cudaError_t builder_stats(GraphBuilder *B, BuildStats *stats, cudaStream_t s)
 {
     cudaError_t err = cudaSuccess;
-    const long long total = (long long)B->n * B->degree;
-    compact_adj_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(B->adj, B->deg, B->n, B->row_cap, B->degree, adj_out_dev);
-    g_launches++;
-    JV_TRY(cudaGetLastError());
     SearchCounters hc;
     unsigned long long hd = 0;
     JV_TRY(cudaMemcpyAsync(&hc, B->counters, sizeof(hc), cudaMemcpyDeviceToHost, s));
@@ -1127,6 +1133,16 @@ cudaError_t builder_finish(GraphBuilder *B, int32_t *adj_out_dev, BuildStats *st
     B->st.truncated_searches = (long long)hc.overflowed;
     if (stats) *stats = B->st;
     return cudaSuccess;
+}
+
+cudaError_t builder_finish(GraphBuilder *B, int32_t *adj_out_dev, BuildStats *stats, cudaStream_t s)
+{
+    const long long total = (long long)B->n * B->degree;
+    compact_adj_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(B->adj, B->deg, B->n, B->row_cap, B->degree, adj_out_dev);
+    g_launches++;
+    const cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+    return builder_stats(B, stats, s);
 }
 
 int builder_row_cap(const GraphBuilder *B) { return B->row_cap; }

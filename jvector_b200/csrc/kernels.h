@@ -167,6 +167,7 @@ cudaError_t builder_reprune_slice(GraphBuilder *B, int lo, int hi, int32_t *rows
 cudaError_t builder_apply_repruned(GraphBuilder *B, int count, const int32_t *rows, const int *rdeg, cudaStream_t s);
 cudaError_t builder_collect_over_degree(GraphBuilder *B, cudaStream_t s);
 cudaError_t builder_list_count(GraphBuilder *B, int *count_host, cudaStream_t s);
+cudaError_t builder_stats(GraphBuilder *B, BuildStats *stats, cudaStream_t s);
 cudaError_t builder_finish(GraphBuilder *B, int32_t *adj_out_dev, BuildStats *stats, cudaStream_t s);
 int builder_row_cap(const GraphBuilder *B);
 int builder_degree(const GraphBuilder *B);

@@ -12,15 +12,56 @@ repair_random (the reference uses ThreadLocalRandom over all ids), and the new e
 the level's iteration order.
 
 Scores are exact (float64 over the fp32 rows). A row is flagged as a near tie when one of its decisions is too close to call in
-fp32: two adjacent sorted candidate scores, or a running maximum similarity and score(c) * alpha in the isDiverse test, equal
-within relative REL. Only on flagged rows may the device (fp32 keys, 3xTF32 Gram products) legitimately disagree. Given the
-device's own key scores (key_scores, the oracle's warp-order scorer) the candidate order is certain, and only isDiverse tests are
-flagged: at 10 % deleted and M = 16 that leaves about 0.5 % of the repaired rows flagged, at 40 % and M = 32 about 0.7 %."""
+fp32. Pair similarities (the isDiverse test) carry the proven bound of pair_bound: a test is a near tie when score(c) * alpha lies
+between the running maxima of (similarity - bound) and (similarity + bound). Without the device's key scores, two adjacent sorted
+candidate scores equal within relative REL are near ties too. Only on flagged rows may the device (fp32 keys, 3xTF32 Gram products)
+legitimately disagree. Given the device's own key scores (key_scores, the oracle's warp-order scorer) the candidate order is
+certain, and only isDiverse tests are flagged."""
 import numpy as np
 
 EUCLIDEAN, DOT_PRODUCT, COSINE = 0, 1, 2
 REL = 1e-5
+U = 2.0 ** -24  # fp32 unit round-off
+# 3xTF32 (prune_gram_tc_kernel): the dropped lo * lo product and the tf32 truncation of lo in the two cross products, each below
+# 2^-20 |x_k y_k| (|lo| < 2^-10 |x|): 3 * 2^-20 relative to |x| |y| over the whole sum
+TF32_SPLIT = 3 * 2.0 ** -20
 _M64 = (1 << 64) - 1
+
+
+def dot_gamma(stride):
+    """relative error of any fp32 dot product of depth below stride + 8, whatever the summation order (DESIGN §4.1), plus the
+    3xTF32 split of the tensor-core Gram product"""
+    return (stride + 8) * 2.0 ** -23 + TF32_SPLIT
+
+
+def pair_bound(metric, X, xv, stride):
+    """[nc][nc] bound on |device pair similarity - exact pair similarity| for the candidate rows X (float64) of the node whose
+    row is xv, for every prune tier (fp32 Gram product on the CUDA or the tensor cores, or the direct fp32 sum of prune_kernel).
+    DOT / COSINE: the dot product's error gamma |x_i| |x_j| through the score map. L2: gamma (|x_i - x_v| + |x_j - x_v|)^2 on the
+    squared distance, which bounds the direct sum (|x_i - x_j| <= |x_i - x_v| + |x_j - x_v|) and the Gram form over rows translated
+    by x_v (build.cu gram_row); it does not depend on how far the rows sit from the origin."""
+    g = dot_gamma(stride) + 4 * U  # + the rounding of the translation and of the final adds
+    if metric == EUCLIDEAN:
+        Y = X - xv
+        r = np.sqrt((Y * Y).sum(1))
+        dd = g * (r[:, None] + r[None, :]) ** 2
+        if np.array_equal(Y, np.round(Y)) and np.abs(Y).max(initial=0) < 2048:
+            # integer rows (SIFT): every product and partial sum is an integer below 2^24 while (r_i + r_j)^2 is, so the pair's
+            # squared distance is exact in fp32 on every tier (integers below 2^11 have no 3xTF32 lo part)
+            dd = np.where((r[:, None] + r[None, :]) ** 2 < 2.0 ** 24, 0.0, dd)
+        d = _sqdist(Y)
+        return dd / ((1.0 + d) * (1.0 + np.maximum(0.0, d - dd))) + 4 * U / (1.0 + d)
+    nrm = np.sqrt((X * X).sum(1))
+    if metric == DOT_PRODUCT:
+        return g * nrm[:, None] * nrm[None, :] / 2.0 + 2 * U * np.abs(1.0 + X @ X.T) + 4 * U
+    # cosine: g from the dot product, g / 2 from each squared norm under the square root, then the divide
+    return np.full((len(X), len(X)), (2 * g + 4 * U) / 2.0 + 4 * U)
+
+
+def _sqdist(Y):
+    """squared distances of the rows of Y (float64; translated by the pruned node's row, so the Gram form loses nothing)"""
+    n2 = (Y * Y).sum(1)
+    return np.maximum(0.0, n2[:, None] + n2[None, :] - 2.0 * (Y @ Y.T))
 
 
 def _mix(x):
@@ -47,11 +88,10 @@ def _scores(metric, x, Y):
     return (1.0 + (Y @ x) / np.sqrt((Y * Y).sum(1) * (x @ x))) / 2.0
 
 
-def _pairs(metric, Y):
-    G = Y @ Y.T
+def _pairs(metric, Y, xv):
     if metric == EUCLIDEAN:
-        d = np.diag(G)
-        return 1.0 / (1.0 + np.maximum(0.0, d[:, None] + d[None, :] - 2.0 * G))
+        return 1.0 / (1.0 + _sqdist(Y - xv))
+    G = Y @ Y.T
     if metric == DOT_PRODUCT:
         return (1.0 + G) / 2.0
     d = np.diag(G)
@@ -62,16 +102,19 @@ def retain_diverse(metric, data, v, cands, degree, alpha, key_scores=None):
     """retainDiverse with diverseBefore = 0 over the distinct `cands` of node v: (selected ids in score order, near-tie flag).
     key_scores(v, ids) -> float32: the candidates' scores against v with the device's exact bits (the oracle's warp-order
     scorer); then their order is certain and only the isDiverse tests can be near ties. Without it, exact float64 scores."""
-    c = np.array(sorted(set(int(x) for x in cands)), dtype=np.int64)
+    c = np.array(sorted(set(int(x) for x in cands) - {int(v)}), dtype=np.int64)
     if len(c) == 0:
         return [], False
     X = data[c].astype(np.float64)
-    s = _scores(metric, data[v].astype(np.float64), X) if key_scores is None else np.asarray(key_scores(v, c), np.float32)
+    xv = data[v].astype(np.float64)
+    s = _scores(metric, xv, X) if key_scores is None else np.asarray(key_scores(v, c), np.float32)
     order = np.lexsort((c, -s))  # score descending, then the lower id first
     c, s, X = c[order], s[order], X[order]
     flag = key_scores is None and any(_near(s[i], s[i + 1]) for i in range(len(s) - 1))
-    P = _pairs(metric, X)
+    P = _pairs(metric, X, xv)
+    B = pair_bound(metric, X, xv, (data.shape[1] + 3) & ~3)
     maxsim = np.full(len(c), -np.inf)
+    lo, hi = maxsim.copy(), maxsim.copy()  # running maxima of P - B and P + B: where the device's fp32 maximum can lie
     taken = np.zeros(len(c), bool)
     sel = []
     a = np.float32(1.0)
@@ -83,12 +126,14 @@ def retain_diverse(metric, data, v, cands, degree, alpha, key_scores=None):
             if taken[i]:
                 continue
             thr = float(np.float32(s[i]) * a) if key_scores is not None else s[i] * float(a)  # fp32 product, as __fmul_rn
-            if np.isfinite(maxsim[i]) and _near(maxsim[i], thr):
+            if lo[i] <= thr < hi[i]:
                 flag = True
             if not maxsim[i] > thr:
                 taken[i] = True
                 sel.append(i)
                 maxsim = np.maximum(maxsim, P[:, i])
+                lo = np.maximum(lo, P[:, i] - B[:, i])
+                hi = np.maximum(hi, P[:, i] + B[:, i])
         a = np.float32(a + np.float32(0.2))
     return [int(c[i]) for i in sorted(sel)], flag
 

@@ -860,7 +860,8 @@ def test_device_builder_quality_vs_reference_builder(jv, oracle):
         res = jv.GraphSearcher(g).search(vec, queries, o.DOT_PRODUCT, 10, 30)
         rec[name] = np.mean([len(set(res.nodes[i]) & set(gt[i])) / 10.0 for i in range(200)])
         rec[name + "_visited"] = res.visitedCount / 200.0
-    # the device build is not bit-reproducible run to run (back-link slots are claimed by atomics), so leave head-room
+    # the batched build is a different insert order from the sequential one (batches, in-progress window), so its graph is not the
+    # oracle's; its own rows are pinned step by step in tests/test_build_steps.py. Here only searchability, with head-room
     assert rec["dev"] >= rec["ref"] - 0.05, rec
     assert rec["dev_visited"] <= 1.35 * rec["ref_visited"], rec
     vec.close()

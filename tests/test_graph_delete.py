@@ -276,6 +276,26 @@ def test_device_equals_restatement(jv, oracle, latent_world, metric, hier):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("hier", [False, True])
+def test_device_equals_restatement_offset_rows(jv, oracle, hier):
+    # EUCLIDEAN rows sharing a large offset (100 + 0.1 x): distances of ~0.01 against |x|^2 ~ 6e5. The Gram tiers stage the rows
+    # translated by the pruned node's own, so the repair's decisions stay within the pair bound here too
+    rng = np.random.default_rng(61 + hier)
+    data = np.ascontiguousarray(100 + 0.1 * latent_rows(rng, 6000, 64), dtype=np.float32)
+    vec = jv.F32Vectors(data)
+    gi = jv.GraphIndexBuilder(o.EUCLIDEAN, M=16, beamWidth=60, alpha=1.2, addHierarchy=hier, seed=3).build(vec)
+    _, adj0 = gi.level(0)
+    upper, entry = _upper_of(gi), gi.info()["entry_node"]
+    deleted = rng.random(data.shape[0]) < 0.1
+    got = _remove(jv, o.EUCLIDEAN, gi, vec, deleted, seed=17)
+    res = dm.remove_deleted(data, o.EUCLIDEAN, adj0, entry, upper, deleted, seed=17, key_scores=warp_keys(oracle, o.EUCLIDEAN, data))
+    repaired, flagged = assert_matches_oracle(got, res, ("offset", hier))
+    assert flagged <= 0.01 * repaired, (flagged, repaired)
+    for h in (got, gi, vec):
+        h.close()
+
+
+@pytest.mark.gpu
 def test_device_large_candidate_sets(jv, oracle, latent_world):
     # 40 % deleted at degree 32: candidate sets past 256 take the high-capacity prune kernels, never a clipped set
     data, vec = latent_world
