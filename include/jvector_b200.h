@@ -350,6 +350,35 @@ JV_API int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float
                                    const uint32_t *deleted_bits /* host, bit (node & 31) of word (node >> 5) */,
                                    jv_graph *out, jv_remove_stats *stats);
 
+/* GraphIndexBuilder.addGraphNode (base:graph/GraphIndexBuilder.java:588-659) for a batch, on the device: nodes n0 .. n-1 of `f32`
+ * (n rows, n >= n0 = g's size) are inserted into g in id order, as a build inserts them: batches of inserted / 32 nodes, at most
+ * max_batch; beam search of the graph as it stands, robust prune of the beam and the in-progress window, sorted back-links,
+ * re-prune of overflowing rows, and the final over-degree cleanup over all n rows. Rows [0, n0) of `f32` must be g's own nodes
+ * (the call cannot check it): grow the data set by registering a longer one, or adopt a longer prefix of the same device buffer
+ * with jv_dataset_adopt_f32_device, which copies nothing.
+ * The result is a NEW graph of n nodes (`g` is not modified) without FusedPQ records. g's holes (jv_graph_remove_deleted) stay
+ * holes: the new graph remembers them, widened to n, so a later removal still counts them as gone.
+ * Level 0: g's rows seed the builder, each with its -1 slots squeezed out (entries keep their order); the insert searches walk
+ * level 0 from g's entry node (not down through the hierarchy). If g has no entry (every node removed), node n0 becomes the
+ * entry with an empty row.
+ * Upper levels (only when g has them): new node i takes draw i of the build's level draws for n nodes and `params->seed`, so a
+ * node's level does not depend on when it was added. A level of g that gains members is extended the same way (its old members'
+ * rows seed the builder, the inserts start at the entry); levels above g's top are built over their new members, and the lowest
+ * id of the new top level becomes the entry. params->add_hierarchy is ignored: the hierarchy follows g.
+ * params: degree must equal g's; beam_width, overflow, alpha, max_batch, concurrent_window and seed mean what they mean for a build.
+ * deleted_bits (optional, host, ceil(n0 / 32) words, the accept_bits layout): nodes marked deleted but not yet removed. The
+ * insert searches walk through them but never pick one as a neighbour of a new node (the liveNodes() filter of :630-632).
+ * n == n0 returns a copy of g. Errors: JV_ERR_INVALID for a null argument, a data set that is not fp32, n < n0, a device
+ * mismatch, a degree mismatch or a bad metric; JV_ERR_UNSUPPORTED for a degree above 64. jv_graph_build_stats then reports the
+ * level-0 insert; device_ms covers the whole call. */
+JV_API int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                              jv_graph *out, double *device_ms);
+/* The same add, step by step: a builder seeded from g exactly as jv_graph_add_nodes seeds it, driven by the jv_builder_* calls
+ * above (jv_builder_next_batch starts at node n0); jv_builder_finish extends the upper levels as jv_graph_add_nodes does. g is no
+ * longer read once this returns. */
+JV_API int jv_builder_create_from_graph(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                        void *cuda_stream, jv_builder *out);
+
 /* device-memory helpers for callers that keep queries/results in HBM (bench `value` leg) */
 JV_API int jv_device_malloc(void **out, size_t bytes);
 JV_API int jv_device_free(void *p);

@@ -430,19 +430,7 @@ class GraphIndexBuilder:
         Until this is called, a graph with marked nodes is searched with GraphSearcher.search(..., acceptOrds=~deleted): the marked
         nodes stay on the search paths but are never returned."""
         lib = nat.init()
-        n = graph.info()["n"]
-        d = np.asarray(deleted)
-        if d.dtype == bool:
-            if d.shape != (n,):
-                raise ValueError("deleted mask has shape %s, the graph has %d nodes" % (d.shape, n))
-            mask = d
-        else:
-            ids = d.astype(np.int64).ravel()
-            if ids.size and (ids.min() < 0 or ids.max() >= n):
-                raise ValueError("deleted ids outside [0, %d)" % n)
-            mask = np.zeros(n, bool)
-            mask[ids] = True
-        bits = pack_accept_bits(mask)
+        bits = _deleted_bits(deleted, graph.info()["n"])
         st = nat.RemoveStats()
         h = C.c_void_p()
         check(lib.jv_graph_remove_deleted(graph._h, vectors._h, int(self.vsf), float(self.params.alpha), int(self.params.seed),
@@ -450,3 +438,39 @@ class GraphIndexBuilder:
         out = GraphIndex(_handle=h)
         out.remove_stats = {name: getattr(st, name) for name, _ in nat.RemoveStats._fields_}
         return out
+
+    def addGraphNodes(self, graph, vectors, deleted=None):
+        """GraphIndexBuilder.addGraphNode for every node graph.size() .. vectors.size() - 1, on the device (jv_graph_add_nodes).
+
+        vectors: F32Vectors whose first rows are the graph's own nodes, followed by the new ones. Returns a NEW GraphIndex (`graph`
+        is left as it is), built from the graph's rows with this builder's parameters (M must equal the graph's degree); its holes
+        stay holes, the hierarchy follows the graph's (addHierarchy is ignored) and it has no FusedPQ records. deleted: nodes marked
+        deleted but not removed yet (a bool mask over the graph's nodes or an array of their ids): the new nodes never pick them as
+        neighbours. Sets scored_vectors / batches / dropped_backlinks / device_ms as build() does."""
+        lib = nat.init()
+        bits = _deleted_bits(deleted, graph.info()["n"]) if deleted is not None else None
+        h = C.c_void_p()
+        ms = C.c_double()
+        check(lib.jv_graph_add_nodes(graph._h, vectors._h, int(self.vsf), C.byref(self.params),
+                                     bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None, C.byref(h), C.byref(ms)))
+        self.device_ms = ms.value
+        s, b, d = C.c_int64(), C.c_int64(), C.c_int64()
+        lib.jv_graph_build_stats(C.byref(s), C.byref(b), C.byref(d))
+        self.scored_vectors, self.batches, self.dropped_backlinks = s.value, b.value, d.value
+        return GraphIndex(_handle=h)
+
+
+def _deleted_bits(deleted, n):
+    """a bool mask [n] or an array of node ids -> the accept_bits layout over n nodes, set = deleted"""
+    d = np.asarray(deleted)
+    if d.dtype == bool:
+        if d.shape != (n,):
+            raise ValueError("deleted mask has shape %s, the graph has %d nodes" % (d.shape, n))
+        mask = d
+    else:
+        ids = d.astype(np.int64).ravel()
+        if ids.size and (ids.min() < 0 or ids.max() >= n):
+            raise ValueError("deleted ids outside [0, %d)" % n)
+        mask = np.zeros(n, bool)
+        mask[ids] = True
+    return pack_accept_bits(mask)

@@ -1322,9 +1322,8 @@ static int build_params_check(const jv_build_params *params, BuildParams *bp)
     return JV_OK;
 }
 
-// HNSW-style levels (GraphIndexBuilder.java:562-575): level(node) = floor(-ln(U) / ln(M)); returns the members of every level >= 1
-// (ascending ids) and the entry node (the first node of the top level)
-static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vector<int32_t>> &members, int *entry)
+// HNSW-style levels (GraphIndexBuilder.java:562-575): level(node) = floor(-ln(U) / ln(M)), node i takes draw i of the generator
+static std::vector<int> draw_levels(int n, int degree, uint64_t seed)
 {
     uint64_t st = seed ? seed : 0x9E3779B97F4A7C15ull;
     auto next_u = [&st]() {
@@ -1333,11 +1332,16 @@ static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vec
     };
     const double ml = degree == 1 ? 1.0 : 1.0 / log((double)degree);
     std::vector<int> level(n);
+    for (int i = 0; i < n; i++) level[i] = (int)(-log(next_u()) * ml);
+    return level;
+}
+
+// the members of every level >= 1 (ascending ids) and the entry node (the first node of the top level)
+static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vector<int32_t>> &members, int *entry)
+{
+    const std::vector<int> level = draw_levels(n, degree, seed);
     int maxl = 0;
-    for (int i = 0; i < n; i++) {
-        level[i] = (int)(-log(next_u()) * ml);
-        maxl = std::max(maxl, level[i]);
-    }
+    for (int i = 0; i < n; i++) maxl = std::max(maxl, level[i]);
     *entry = 0;
     for (int i = 0; i < n; i++)
         if (level[i] == maxl) { *entry = i; break; }
@@ -1346,39 +1350,48 @@ static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vec
         for (int l = 1; l <= level[i]; l++) members[l - 1].push_back(i);
 }
 
-// every upper level is a Vamana graph over its members, built by the same device builder on the members' rows (one gather kernel)
+// one upper level: a Vamana graph over its members ids (local row r = node ids[r]), built by the device builder on the members'
+// rows (one gather kernel), from nothing or from `seed` (local rows). ladj: [ids.size()][degree] in node ids. Synchronises `s`.
+static int build_level(jv_dataset f32, int metric, const BuildParams &bp, const std::vector<int32_t> &ids, const BuilderSeed *seed,
+                       std::vector<int32_t> &ladj, cudaStream_t s)
+{
+    const int cnt = (int)ids.size(), degree = bp.degree;
+    ladj.assign((size_t)cnt * degree, -1);
+    if (cnt <= 1) return JV_OK;
+    DataDesc sub;
+    memset(&sub, 0, sizeof(DataDesc));
+    sub.kind = KIND_F32; sub.dim = f32->d.dim; sub.stride = f32->d.stride; sub.n = cnt;
+    DeviceBuffer rows, adj, dids;  // the members' rows, their adjacency, their ids
+    cudaError_t e = rows.alloc((size_t)cnt * sub.stride * 4);
+    if (e == cudaSuccess) e = adj.alloc((size_t)cnt * degree * 4);
+    if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = launch_gather_rows(f32->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
+    sub.rows = rows.get<float>();
+    BuildStats bs2;
+    if (e == cudaSuccess) e = build_graph_flat(sub, metric, bp, adj.get<int32_t>(), g_sm_count, &bs2, s, seed);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ladj.data(), adj.get(), ladj.size() * 4, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) return cuda_fail(e, "build upper level");
+    for (auto &x : ladj)
+        if (x >= 0) x = ids[x];
+    return JV_OK;
+}
+
+// every upper level is a Vamana graph over its members, built by the same device builder on the members' rows
 static int build_upper_levels(jv_graph g, jv_dataset f32, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
 {
-    const int n = (int)f32->d.n, degree = bp.degree;
+    const int n = (int)f32->d.n;
     std::vector<std::vector<int32_t>> members;
     int entry = 0;
-    assign_levels(n, degree, seed, members, &entry);
+    assign_levels(n, bp.degree, seed, members, &entry);
     g->g.entry_node = entry;
     for (size_t l = 0; l < members.size(); l++) {
-        const std::vector<int32_t> &ids = members[l];
-        const int cnt = (int)ids.size();
-        std::vector<int32_t> ladj((size_t)cnt * degree, -1);
-        if (cnt > 1) {
-            DataDesc sub;
-            memset(&sub, 0, sizeof(DataDesc));
-            sub.kind = KIND_F32; sub.dim = f32->d.dim; sub.stride = f32->d.stride; sub.n = cnt;
-            DeviceBuffer rows, adj, dids;  // the members' rows, their adjacency, their ids
-            cudaError_t e = rows.alloc((size_t)cnt * sub.stride * 4);
-            if (e == cudaSuccess) e = adj.alloc((size_t)cnt * degree * 4);
-            if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
-            if (e == cudaSuccess) e = launch_gather_rows(f32->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
-            sub.rows = rows.get<float>();
-            BuildStats bs2;
-            if (e == cudaSuccess) e = build_graph_flat(sub, metric, bp, adj.get<int32_t>(), g_sm_count, &bs2, s);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(ladj.data(), adj.get(), ladj.size() * 4, cudaMemcpyDeviceToHost, s);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-            if (e != cudaSuccess) return cuda_fail(e, "build upper level");
-            for (auto &x : ladj)
-                if (x >= 0) x = ids[x];
-        }
-        g->level_ids.push_back(ids);
-        g->level_adj.push_back(ladj);
+        std::vector<int32_t> ladj;
+        const int rc = build_level(f32, metric, bp, members[l], nullptr, ladj, s);
+        if (rc) return rc;
+        g->level_ids.push_back(members[l]);
+        g->level_adj.push_back(std::move(ladj));
     }
     return graph_rebuild_upper(g);
 }
@@ -1415,6 +1428,172 @@ int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv
     return JV_OK;
 }
 
+static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bits[(size_t)v >> 5] >> (v & 31)) & 1u; }
+
+// ------------------------------------------------------------------------------------------------ addGraphNode for a batch
+// Nodes [n0, n) of a data set go into a graph of n0 nodes (GraphIndexBuilder.addGraphNode, base:graph/GraphIndexBuilder.java:588-659,
+// for each of them): level 0 through a builder seeded with g's rows, then every upper level that gains members through a builder
+// seeded with that level's rows. GraphAdd is what the add keeps of g, so that g is no longer read once the builder exists.
+struct GraphAdd {
+    int32_t n0 = 0, entry = -1;
+    std::vector<std::vector<int32_t>> level_ids, level_adj;  // g's upper levels
+    std::vector<uint32_t> removed;                          // g's holes (jv_graph_remove_deleted)
+    std::vector<uint32_t> marks;                            // deleted_bits over the n0 old nodes; empty = none marked
+    DeviceBuffer upper_row;                                 // g's id -> row maps of its upper levels, [levels - 1][n0]
+};
+
+// the accept bits of an insert over `rows` builder rows: row r < nold is node ids[r] (ids == nullptr: node r) and is refused when
+// marked, the rows past nold are new nodes. Empty when nothing is marked: the insert searches then run unfiltered, as a build's do.
+static std::vector<uint32_t> add_accept_bits(const GraphAdd &A, const int32_t *ids, int nold, int rows)
+{
+    std::vector<uint32_t> bits;
+    if (A.marks.empty()) return bits;
+    bits.assign(((size_t)rows + 31) / 32, 0u);
+    for (int r = 0; r < rows; r++)
+        if (r >= nold || !bit_of(A.marks, ids ? ids[r] : r)) bits[(size_t)r >> 5] |= 1u << (r & 31);
+    return bits;
+}
+
+static int add_check(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, BuildParams *bp)
+{
+    if (!f32 || !params) return fail(JV_ERR_INVALID, "add_nodes: null argument");
+    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "add_nodes: needs an fp32 data set");
+    if (f32->device != g->device) return fail(JV_ERR_INVALID, "add_nodes: data set and graph live on different devices");
+    if (f32->d.n < g->g.n || f32->d.n > INT32_MAX) return fail(JV_ERR_INVALID, "add_nodes: the data set must hold the graph's nodes first");
+    int rc = check_metric(f32->d, metric);
+    if (rc) return rc;
+    if (g->g.degree > 64)
+        return fail(JV_ERR_UNSUPPORTED, "add_nodes: degree " + std::to_string(g->g.degree) + " > 64, the largest row the builder handles");
+    if (params->degree != g->g.degree) return fail(JV_ERR_INVALID, "add_nodes: params->degree differs from the graph's degree");
+    return build_params_check(params, bp);
+}
+
+// g's state into A and the seed of a level-0 builder over n rows (accept: the storage of its bits). Enqueues a copy of g's
+// upper_row and, through the seed, a read of g's adjacency on `s`.
+static int add_prepare(jv_graph g, const uint32_t *deleted_bits, int n, GraphAdd &A, std::vector<uint32_t> &accept, BuilderSeed *seed, cudaStream_t s)
+{
+    const int n0 = g->g.n;
+    A.n0 = n0; A.entry = g->g.entry_node; A.level_ids = g->level_ids; A.level_adj = g->level_adj; A.removed = g->removed;
+    if (deleted_bits) {
+        const size_t W0 = ((size_t)n0 + 31) / 32;
+        A.marks.assign(deleted_bits, deleted_bits + W0);
+        if (n0 & 31) A.marks[W0 - 1] &= (1u << (n0 & 31)) - 1u;
+    }
+    if (!A.level_ids.empty()) {
+        const size_t bytes = A.level_ids.size() * (size_t)n0 * 4;
+        CK(A.upper_row.alloc(bytes), "cudaMalloc(upper_row)");
+        CK(cudaMemcpyAsync(A.upper_row.get(), g->upper_row.get(), bytes, cudaMemcpyDeviceToDevice, s), "copy upper_row");
+    }
+    accept = add_accept_bits(A, nullptr, n0, n);
+    *seed = {g->adj0.get<int32_t>(), n0, g->g.degree, nullptr, A.entry, accept.empty() ? nullptr : accept.data()};
+    return JV_OK;
+}
+
+// the upper levels after an add. New node i joins the levels its draw i of draw_levels(n, M, seed) reaches, so a node's level does
+// not depend on when it was added. A level of g that gains members is extended by a builder seeded with its rows: local rows are the
+// old members in the level's order, then the new members ascending; the old rows are mapped to local rows through g's upper_row on
+// the device; the inserts start at the entry's row (the level's first row if the entry is not a member). A level above g's top is
+// built over its members, all new, and its lowest id becomes the entry.
+static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+{
+    const int n = (int)f32->d.n, n0 = A.n0, degree = bp.degree, L = (int)A.level_ids.size();
+    const std::vector<int> level = draw_levels(n, degree, seed);
+    int top = L;
+    for (int i = n0; i < n; i++) top = std::max(top, level[i]);
+    for (int l = 1; l <= top; l++) {
+        std::vector<int32_t> ids = l <= L ? A.level_ids[l - 1] : std::vector<int32_t>();
+        const int nold = (int)ids.size();
+        for (int i = n0; i < n; i++)
+            if (level[i] >= l) ids.push_back(i);
+        std::vector<int32_t> ladj;
+        int rc = JV_OK;
+        if (l > L) {
+            rc = build_level(f32, metric, bp, ids, nullptr, ladj, s);
+        } else if ((int)ids.size() == nold) {
+            ladj = A.level_adj[l - 1];
+        } else {
+            const std::vector<int32_t> &old = A.level_adj[l - 1];
+            DeviceBuffer rows;
+            cudaError_t e = rows.alloc(std::max<size_t>(old.size(), 1) * 4);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(rows.get(), old.data(), old.size() * 4, cudaMemcpyHostToDevice, s);
+            if (e != cudaSuccess) return cuda_fail(e, "add_nodes: upper level rows");
+            const int at = (int)(std::find(ids.begin(), ids.begin() + nold, A.entry) - ids.begin());
+            const std::vector<uint32_t> accept = add_accept_bits(A, ids.data(), nold, (int)ids.size());
+            const BuilderSeed sd = {rows.get<int32_t>(), nold, degree, A.upper_row.get<int32_t>() + (size_t)(l - 1) * n0, at < nold ? at : 0,
+                                    accept.empty() ? nullptr : accept.data()};
+            rc = build_level(f32, metric, bp, ids, &sd, ladj, s);
+        }
+        if (rc) return rc;
+        ng->level_ids.push_back(std::move(ids));
+        ng->level_adj.push_back(std::move(ladj));
+    }
+    if (top > L) ng->g.entry_node = ng->level_ids[top - 1][0];
+    return JV_OK;
+}
+
+// the new graph around its level-0 adjacency (already in ng->adj0): size, entry, holes widened to n, upper levels
+static int add_finish(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+{
+    const int n = (int)f32->d.n;
+    ng->g.n = n; ng->g.degree = bp.degree; ng->g.levels = 1; ng->g.entry_level = 0; ng->g.adj0 = ng->adj0.get<int32_t>();
+    ng->g.entry_node = A.entry >= 0 ? A.entry : n > A.n0 ? A.n0 : -1;  // an empty graph's first new node is its entry (build.cu)
+    if (!A.removed.empty()) {
+        ng->removed = A.removed;
+        ng->removed.resize(((size_t)n + 31) / 32, 0u);
+    }
+    if (!A.level_ids.empty()) {
+        const int rc = add_upper_levels(ng, A, f32, metric, bp, seed, s);
+        if (rc) return rc;
+    }
+    return graph_rebuild_upper(ng);
+}
+
+int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
+                       double *device_ms)
+{
+    ON_DEVICE_OF(g);
+    if (!out) return fail(JV_ERR_INVALID, "add_nodes: null argument");
+    BuildParams bp;
+    int rc = add_check(g, f32, metric, params, &bp);
+    if (rc) return rc;
+    if ((rc = t_ctx.init())) return rc;
+    cudaStream_t s = t_ctx.stream;
+    const int n0 = g->g.n, n = (int)f32->d.n, degree = g->g.degree;
+    std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
+    ng->device = g->device;
+    memset(&ng->g, 0, sizeof(GraphDesc));
+    StreamTimer timer;
+    CK(timer.start(s), "event");
+    CK(ng->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+    BuildStats bs = {0, 0, 0, 0, 0};
+    if (n == n0) {
+        // nothing to insert: a copy of g
+        CK(cudaMemcpyAsync(ng->adj0.get(), g->adj0.get(), (size_t)n * degree * 4, cudaMemcpyDeviceToDevice, s), "copy adjacency");
+        ng->g.n = n; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_node = g->g.entry_node; ng->g.entry_level = 0;
+        ng->g.adj0 = ng->adj0.get<int32_t>();
+        ng->level_ids = g->level_ids; ng->level_adj = g->level_adj; ng->removed = g->removed;
+        rc = graph_rebuild_upper(ng.get());
+    } else {
+        GraphAdd A;
+        std::vector<uint32_t> accept;
+        BuilderSeed seed;
+        rc = add_prepare(g, deleted_bits, n, A, accept, &seed, s);
+        if (!rc) {
+            const cudaError_t e = build_graph_flat(f32->d, metric, bp, ng->adj0.get<int32_t>(), g_sm_count, &bs, s, &seed);
+            rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_add_nodes");
+        }
+        if (!rc) rc = add_finish(ng.get(), A, f32, metric, bp, params->seed, s);
+    }
+    t_build_stats = bs;
+    const cudaError_t e1 = timer.stop(s);
+    cudaStreamSynchronize(s);
+    if (rc) return rc;
+    CK(e1, "event");
+    if (device_ms) *device_ms = timer.ms();
+    *out = ng.release();
+    return JV_OK;
+}
+
 // ---- the same build advanced batch by batch, for a build SHARDED over several GPUs (BASELINE config 5) ----------------------
 // Every rank holds a replica of the rows and of the adjacency. Per batch: each rank searches + prunes ITS slice of the batch
 // (jv_builder_insert_slice -> rows in a caller buffer), the slices are all-gathered by the caller (NCCL; jvector_b200/parallel.py),
@@ -1429,6 +1608,7 @@ struct jv_builder_s {
     GraphBuilder *B = nullptr;
     cudaStream_t stream = nullptr;
     StreamTimer timer;  // jv_builder_create to jv_builder_finish
+    std::unique_ptr<GraphAdd> add;  // jv_builder_create_from_graph: the graph the builder extends
     ~jv_builder_s() { builder_destroy(B); }
 };
 
@@ -1443,6 +1623,27 @@ int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params,
     if ((rc = build_params_check(params, &b->bp))) return rc;
     CK(b->timer.start(b->stream), "event");
     CK(builder_create(f32->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
+    *out = b.release();
+    return JV_OK;
+}
+
+int jv_builder_create_from_graph(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                 void *cuda_stream, jv_builder *out)
+{
+    ON_DEVICE_OF(g);
+    if (!out) return fail(JV_ERR_INVALID, "builder_create_from_graph: null argument");
+    BuildParams bp;
+    int rc = add_check(g, f32, metric, params, &bp);
+    if (rc) return rc;
+    std::unique_ptr<jv_builder_s> b(new jv_builder_s());
+    b->device = g->device; b->f32 = f32; b->metric = metric; b->params = *params; b->bp = bp; b->stream = (cudaStream_t)cuda_stream;
+    b->add.reset(new GraphAdd());
+    CK(b->timer.start(b->stream), "event");
+    std::vector<uint32_t> accept;
+    BuilderSeed seed;
+    if ((rc = add_prepare(g, deleted_bits, (int)f32->d.n, *b->add, accept, &seed, b->stream))) return rc;
+    CK(builder_create(f32->d, metric, bp, g_sm_count, &b->B, b->stream, &seed), "builder_create");
+    CK(cudaStreamSynchronize(b->stream), "builder_create_from_graph");  // g has been read: the caller may free it
     *out = b.release();
     return JV_OK;
 }
@@ -1529,7 +1730,9 @@ int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms)
     t_build_stats = bs;
     CK(e, "builder_finish");
     g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
-    if (b->params.add_hierarchy && n > 1 && (rc = build_upper_levels(g.get(), b->f32, b->metric, b->bp, b->params.seed, b->stream))) return rc;
+    if (b->add) rc = add_finish(g.get(), *b->add, b->f32, b->metric, b->bp, b->params.seed, b->stream);  // the hierarchy follows the graph
+    else if (b->params.add_hierarchy && n > 1) rc = build_upper_levels(g.get(), b->f32, b->metric, b->bp, b->params.seed, b->stream);
+    if (rc) return rc;
     CK(b->timer.stop(b->stream), "event");
     cudaStreamSynchronize(b->stream);
     if (device_ms) *device_ms = b->timer.ms();
@@ -1567,7 +1770,6 @@ int jv_graph_build_stats(int64_t *scored_vectors, int64_t *batches, int64_t *dro
 }
 
 // ------------------------------------------------------------------------------------------------ removeDeletedNodes
-static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bits[(size_t)v >> 5] >> (v & 31)) & 1u; }
 
 // one level of the repair on the device (repair_level, build.cu); level L >= 1 also hands back its repaired rows
 static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset f32, int metric, float alpha, uint64_t seed, int level, const std::vector<uint32_t> &dead,

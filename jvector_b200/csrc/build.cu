@@ -837,6 +837,27 @@ __global__ void __launch_bounds__(256) scatter_rows_kernel(int32_t *adj, int *de
     if (j == 0) deg[v] = rdeg[i];
 }
 
+// an existing graph's rows as the builder's first rows (BuilderSeed), one warp per row: the valid ids, mapped through row_map when
+// given, are compacted by ballot to the front of the row_cap-wide row in their order; the rest of the row stays -1
+__global__ void __launch_bounds__(256) seed_rows_kernel(const int32_t *__restrict__ rows, int count, int width, const int32_t *__restrict__ row_map,
+                                                        int32_t *adj, int *deg, int row_cap)
+{
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (warp >= count) return;
+    const int32_t *src = rows + (size_t)warp * width;
+    int32_t *dst = adj + (size_t)warp * row_cap;
+    int w = 0;
+    for (int j0 = 0; j0 < width; j0 += 32) {
+        int32_t id = j0 + lane < width ? src[j0 + lane] : -1;
+        if (id >= 0 && row_map) id = row_map[id];
+        const unsigned valid = __ballot_sync(FULL, id >= 0);
+        if (id >= 0) dst[w + __popc(valid & ((1u << lane) - 1u))] = id;
+        w += __popc(valid);
+    }
+    if (lane == 0) deg[warp] = w;
+}
+
 __global__ void __launch_bounds__(256) compact_adj_kernel(const int32_t *adj, const int *deg, int n, int row_cap, int degree, int32_t *out)
 {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -926,7 +947,9 @@ struct GraphBuilder {
     int metric = 0, sm_count = 0;
     BuildParams bp;
     int n = 0, degree = 0, beam = 0, hard_max = 0, row_cap = 0, max_batch = 0, window = 0, batch_div = 32;
-    int inserted = 1;  // node 0 is the entry point with an empty list
+    int inserted = 1;  // rows [0, inserted) are in the graph: a build starts with node 0, the entry point, and an empty list
+    int32_t entry = 0;  // where the insert searches start
+    uint32_t *accept = nullptr;  // rows an insert may pick (nullptr = all): bit (row & 31) of word (row >> 5)
     int32_t *adj = nullptr, *res_nodes = nullptr, *list = nullptr, *head_target = nullptr, *iota = nullptr;
     int *deg = nullptr, *mark = nullptr, *list_count = nullptr, *work_counter = nullptr;
     float *res_scores = nullptr;
@@ -947,15 +970,18 @@ struct GraphBuilder {
 
 void builder_destroy(GraphBuilder *B) { delete B; }
 
-cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp, int sm_count, GraphBuilder **out, cudaStream_t s)
+cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp, int sm_count, GraphBuilder **out, cudaStream_t s,
+                           const BuilderSeed *seed)
 {
     const int n = (int)d.n;
     if (d.kind != KIND_F32 || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
+    if (seed && (seed->count < 0 || seed->count > n || (seed->count > 0 && (!seed->rows_dev || seed->width < 1)) || seed->entry >= seed->count))
+        return cudaErrorInvalidValue;
     std::unique_ptr<GraphBuilder> B(new GraphBuilder());
     B->d = d; B->metric = metric; B->bp = bp; B->sm_count = sm_count; B->n = n; B->degree = bp.degree; B->beam = bp.beam;
     B->hard_max = (int)(bp.overflow * bp.degree);  // ConcurrentNeighborMap.java:300
     B->row_cap = std::max(2 * bp.degree, B->hard_max + 1);
-    if (B->row_cap > MAX_DEGREE) return cudaErrorInvalidValue;
+    if (B->row_cap > MAX_DEGREE || (seed && seed->width > B->row_cap)) return cudaErrorInvalidValue;
     B->max_batch = bp.max_batch > 0 ? bp.max_batch : 16384;
     if (const char *e = getenv("JV_BUILD_BATCH_DIV")) B->batch_div = atoi(e) > 0 ? atoi(e) : 32;  // tuning knob (tools/build_quality.py)
     // in-progress window: as many concurrently inserting peers as still fit the 128-candidate Gram tile next to the beam
@@ -1000,6 +1026,22 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
     iota_kernel<<<(n + 255) / 256, 256, 0, s>>>(B->iota, n);
     g_launches++;
     JV_TRY(cudaGetLastError());
+    if (seed) {
+        if (seed->count > 0) {
+            seed_rows_kernel<<<(unsigned)(((long long)seed->count * 32 + 255) / 256), 256, 0, s>>>(seed->rows_dev, seed->count, seed->width, seed->row_map_dev,
+                                                                                                  B->adj, B->deg, B->row_cap);
+            g_launches++;
+            JV_TRY(cudaGetLastError());
+        }
+        if (seed->accept) {
+            const size_t words = ((size_t)n + 31) / 32;
+            JV_TRY(alloc_owned(owned, B->accept, words * 4));
+            JV_TRY(cudaMemcpyAsync(B->accept, seed->accept, words * 4, cudaMemcpyHostToDevice, s));
+        }
+        // a graph without an entry (every node removed) takes its first new row as the entry, with an empty list
+        B->entry = seed->entry >= 0 ? seed->entry : seed->count;
+        B->inserted = std::min(n, seed->entry >= 0 ? seed->count : seed->count + 1);
+    }
     *out = B.release();
     return cudaSuccess;
 }
@@ -1036,13 +1078,14 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
     const int m = hi - lo;
     if (m <= 0) return cudaSuccess;
     GraphDesc g = {};
-    g.n = B->n; g.degree = B->row_cap; g.levels = 1; g.entry_node = 0; g.entry_level = 0; g.adj0 = B->adj;
+    g.n = B->n; g.degree = B->row_cap; g.levels = 1; g.entry_node = B->entry; g.entry_level = 0; g.adj0 = B->adj;
     SearchPlan plan;
     JV_TRY(plan_search(B->d, nullptr, g, B->beam, B->beam, m, 0, 0, B->sm_count, &plan));
     JV_TRY(B->scratch.grow(search_scratch_bytes(plan)));
     SearchFilter lenient;
     memset(&lenient, 0, sizeof(lenient));
     lenient.lenient = 1;  // an insert search never fails the build: see SearchParams::lenient
+    lenient.accept_bits = B->accept;  // an add into a graph with marked nodes walks through them but never links to them
     JV_TRY(launch_search(g, B->d, nullptr, B->metric, B->d.rows + (size_t)(first + lo) * B->d.stride, m, B->beam, B->beam, plan, B->scratch.get(), B->work_counter,
                          B->res_nodes, B->res_scores, B->counters, B->overflow, nullptr, B->d.stride, &lenient, s));
     PruneParams P = prune_params(B);
@@ -1149,12 +1192,13 @@ int builder_row_cap(const GraphBuilder *B) { return B->row_cap; }
 int builder_degree(const GraphBuilder *B) { return B->degree; }
 int builder_max_batch(const GraphBuilder *B) { return B->max_batch; }
 
-// the whole build on one GPU: no exchange, no host synchronisation between batches
+// the whole build on one GPU: no exchange, no host synchronisation between batches. The same loop extends a seeded builder (an
+// add into an existing graph): only the starting state differs.
 cudaError_t build_graph_flat(const DataDesc &d, int metric, const BuildParams &bp, int32_t *adj_out_dev, int sm_count,
-                             BuildStats *stats, cudaStream_t s)
+                             BuildStats *stats, cudaStream_t s, const BuilderSeed *seed)
 {
     GraphBuilder *B = nullptr;
-    cudaError_t err = builder_create(d, metric, bp, sm_count, &B, s);
+    cudaError_t err = builder_create(d, metric, bp, sm_count, &B, s, seed);
     if (err != cudaSuccess) return err;
     int first, count;
     while (err == cudaSuccess && builder_next_batch(B, &first, &count)) {

@@ -152,13 +152,27 @@ struct BuildStats {
     long long searched, pruned, dropped_backlinks, batches;
     long long truncated_searches;  // insert searches cut short by a full visited table / an oversized tie tail (pathological inputs)
 };
-// flat Vamana graph over rows [0, n) of an f32 data set; adj_out_dev [n][degree] (-1 padded); entry node is 0
+// The state a builder starts from (addGraphNode into an existing graph). Rows [0, count) are seeded from rows_dev [count][width]
+// (-1 = empty slot), their ids mapped through row_map_dev when given (an upper level's id -> row map); the valid entries move to
+// the front of each row, in their order. Rows [count, n) start empty and are inserted in order. The insert searches start at
+// `entry`; entry < 0 makes row `count` the entry with an empty row, as node 0 is for a build. accept (host, ceil(n / 32) words,
+// nullptr = every row): the rows an insert may pick as neighbours; the others are still walked through.
+// No seed = {nullptr, 0, 0, nullptr, -1, nullptr}: the build from nothing.
+struct BuilderSeed {
+    const int32_t *rows_dev;
+    int count, width;
+    const int32_t *row_map_dev;
+    int32_t entry;
+    const uint32_t *accept;
+};
+// flat Vamana graph over rows [0, n) of an f32 data set; adj_out_dev [n][degree] (-1 padded); entry node is 0 (or the seed's)
 cudaError_t build_graph_flat(const DataDesc &f32, int metric, const BuildParams &bp, int32_t *adj_out_dev, int sm_count,
-                             BuildStats *stats, cudaStream_t s);
+                             BuildStats *stats, cudaStream_t s, const BuilderSeed *seed = nullptr);
 // the same build advanced batch by batch; a sharded build calls the *_slice functions for its part of each batch and moves the
 // rows between the replicas itself (see build.cu)
 struct GraphBuilder;
-cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp, int sm_count, GraphBuilder **out, cudaStream_t s);
+cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp, int sm_count, GraphBuilder **out, cudaStream_t s,
+                           const BuilderSeed *seed = nullptr);
 void builder_destroy(GraphBuilder *B);
 bool builder_next_batch(GraphBuilder *B, int *first, int *count);
 cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, int hi, int32_t *rows_out, int *deg_out, cudaStream_t s);
