@@ -121,6 +121,10 @@ JV_API int jv_dataset_register_nvq(const uint8_t *bytes, const float *params, in
  * (A graph searched over them assumes unchanged rows already; so does the row sketch that the first DOT_PRODUCT graph search of a
  * batch larger than the GPU's resident CTAs derives from them: int8 codes + 8 bytes per row, built once, freed with the handle.) */
 JV_API int jv_dataset_adopt_f32_device(const float *rows_device, int64_t n, int dim, int row_stride, jv_dataset *out);
+/* the row sketch of an fp32 data set, as that search built it: codes_out [n][sketch_stride] int8 (sketch_stride = row stride
+ * rounded up to 8, padding codes 0), meta_out [n][2] = {scale, radius} per row. Builds nothing: JV_ERR_INVALID ("no row sketch")
+ * while no search has built one. codes_out / meta_out may be NULL (only *sketch_stride_out, and whether the sketch exists). */
+JV_API int jv_dataset_row_sketch_download(jv_dataset f32, int8_t *codes_out, float *meta_out, int *sketch_stride_out);
 JV_API int jv_dataset_device(jv_dataset ds);
 /* ImmutablePQVectors' code-vs-code scoring (base:quantization/ImmutablePQVectors.java:63-105): build the triangular
  * centroid-vs-centroid table of ProductQuantization.createCodebookPartialSums (ProductQuantization.java:609-628; 12.6 MB at M = 96,

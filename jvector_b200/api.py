@@ -68,6 +68,21 @@ class F32Vectors(_Vectors):
         check(lib.jv_dataset_register_f32(fp(rows), rows.shape[0], rows.shape[1], C.byref(h)))
         super().__init__(h, None)
 
+    def row_sketch(self):
+        """the int8 row sketch a DOT_PRODUCT graph search of a batch that fills the GPU builds (never built here):
+        (codes [n][sketch_stride] int8, meta [n][2] float32 = {scale, radius}), or None while no search has built it"""
+        lib = nat.load()
+        ss = C.c_int(0)
+        rc = lib.jv_dataset_row_sketch_download(self._h, None, None, C.byref(ss))
+        if rc != 0 and ss.value > 0:  # the stride is set for every fp32 data set: this one has no sketch yet
+            return None
+        check(rc)
+        n = self.size()
+        codes = np.empty((n, ss.value), np.int8)
+        meta = np.empty((n, 2), np.float32)
+        check(lib.jv_dataset_row_sketch_download(self._h, codes.ctypes.data, fp(meta), None))
+        return codes, meta
+
 
 class PQVectors(_Vectors):
     """base:quantization/PQVectors.java — codes [n][M] + codebooks (concatenated, codebook m = [k][size_m])."""

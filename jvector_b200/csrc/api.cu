@@ -1057,6 +1057,19 @@ int jv_graph_download(jv_graph g, int level, int32_t *node_ids_out, int32_t *adj
     return JV_OK;
 }
 
+int jv_dataset_row_sketch_download(jv_dataset f32, int8_t *codes_out, float *meta_out, int *sketch_stride_out)
+{
+    ON_DEVICE_OF(f32);
+    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "row_sketch_download: not an fp32 data set");
+    const int ss = sketch_stride(f32->d.stride);
+    if (sketch_stride_out) *sketch_stride_out = ss;
+    std::lock_guard<std::mutex> lk(f32->sketch_mu);
+    if (!f32->sketch.get()) return fail(JV_ERR_INVALID, "row_sketch_download: no row sketch");
+    if (codes_out) CK(cudaMemcpy(codes_out, f32->sketch.get(), (size_t)f32->d.n * ss, cudaMemcpyDeviceToHost), "D2H row sketch");
+    if (meta_out) CK(cudaMemcpy(meta_out, f32->sketch_meta.get(), (size_t)f32->d.n * sizeof(float2), cudaMemcpyDeviceToHost), "D2H row sketch meta");
+    return JV_OK;
+}
+
 // the fp32 row sketch of a data set (row_sketch_kernel), built once. Complete when this returns: another thread's stream may read it
 static int ensure_sketch(jv_dataset ds, cudaStream_t s)
 {

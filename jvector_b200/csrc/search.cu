@@ -334,7 +334,8 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
             // a new level: results + evicted are candidates again (setEntryPointsFromPreviousLayer), the result heap is empty
             for (int i = tid; i < size; i += SEARCH_THREADS) fcur[i] &= F_ACCEPTED;
             int sel = 0;
-            if (tid == 0) { s_posv[0] = 0; s_posv[1] = INT_MAX; s_n = 0; s_m = 0; s_hsize = 0; s_drop[0] = INT_MIN; s_drop[1] = INT_MIN; s_cnt = 0; }
+            // (the list is empty when every node an upper level expanded was refused: no entry point, nothing to walk)
+            if (tid == 0) { s_posv[0] = size > 0 ? 0 : INT_MAX; s_posv[1] = INT_MAX; s_n = 0; s_m = 0; s_hsize = 0; s_drop[0] = INT_MIN; s_drop[1] = INT_MIN; s_cnt = 0; }
             __syncthreads();
             for (;;) {
                 const int p = s_posv[sel];  // first unexpanded entry = the top of the candidate queue
@@ -346,10 +347,12 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 const float wsc = hs > 0 ? key_score(heap[1]) : 0.f;
                 if (hs >= K && csc < wsc) break;  // stopSearch (strict <: a tie with the worst result is still expanded)
                 const int node = key_node(ckey);
-                // addTopCandidate: 1 push, 2 replace the worst, 3 tie with the worst: not added, 0 not acceptable (level 0 only)
+                // addTopCandidate: 1 push, 2 replace the worst, 3 tie with the worst: not added, 0 not acceptable. searchOneLayer admits
+                // a node only if score >= threshold: at level 0 with acceptOrds and the caller's threshold (F_ACCEPTED), on upper levels
+                // with Bits.ALL and threshold 0, which refuses a DOT_PRODUCT score (1 + q.x) / 2 below 0 (GraphSearcher.java:273-278, 429)
                 int action = 0;
-                if (lvl > 0 || (fcur[p] & F_ACCEPTED)) action = hs < K ? 1 : (csc > wsc ? 2 : 3);
-                const int dead = (lvl > 0 && action == 3) ? p : -1;
+                if (lvl > 0 ? csc >= 0.f : (fcur[p] & F_ACCEPTED) != 0) action = hs < K ? 1 : (csc > wsc ? 2 : 3);
+                const int dead = (lvl > 0 && (action == 3 || action == 0)) ? p : -1;
                 if (tid == 0) { fcur[p] |= F_EXPANDED; s_posv[sel ^ 1] = INT_MAX; s_m = 0; }
                 expanded++;
                 if (lvl == 0) expanded_base++;
@@ -606,7 +609,8 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                         for (int jj = 0; jj < nm; jj++) c += (cand_keys[jj] > k);
                         if (c < LC) {
                             nxt[c] = k;
-                            fnxt[c] = P.filtered ? cand_acc[it - size] : F_ACCEPTED;
+                            // unfiltered (threshold 0, no acceptOrds): only a score below 0 is refused, and the key carries the score
+                            fnxt[c] = P.filtered ? cand_acc[it - size] : (key_score(k) >= 0.f ? F_ACCEPTED : 0);
                             mypos = min(mypos, c);
                             // a new candidate that lands at the very front is the likeliest next expansion: start pulling
                             // its adjacency row towards L2 now (128 B; reads only)
@@ -631,7 +635,9 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 const int dm = s_drop[sel];
                 if (dm != INT_MIN) {
                     bool ok;
-                    if (!P.filtered) ok = float_to_sortable(key_score(nxt[L - 1])) > dm;  // newsize == LC >= L here
+                    // unfiltered, the list is sorted by score: when its L-th entry scores >= 0 all L are accepted (newsize == LC >= L)
+                    const float sl = key_score(nxt[L - 1]);
+                    if (!P.filtered && sl >= 0.f) ok = float_to_sortable(sl) > dm;
                     else {
                         int c = 0;
                         for (int i = tid; i < newsize; i += SEARCH_THREADS)

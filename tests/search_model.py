@@ -88,9 +88,10 @@ def search(graph_levels, entry_node, score_fn, topK, rerankK, list_cap, rerank_f
                 break
             node = key_node(ckey)
             action = 0
-            if lvl > 0 or (lst[p][1] & F_ACCEPTED):
+            # searchOneLayer's score >= threshold: F_ACCEPTED at level 0, threshold 0 with Bits.ALL on upper levels
+            if (csc >= 0) if lvl > 0 else (lst[p][1] & F_ACCEPTED):
                 action = 1 if hs < K else (2 if csc > wsc else 3)
-            dead = p if (lvl > 0 and action == 3) else -1
+            dead = p if (lvl > 0 and action in (0, 3)) else -1
             lst[p][1] |= F_EXPANDED
             if action == 1:
                 heap.append(ckey)
@@ -106,7 +107,7 @@ def search(graph_levels, entry_node, score_fn, topK, rerankK, list_cap, rerank_f
                     continue
                 seen.add(f)
                 sc = score_fn(f)
-                cands.append([topk_key(sc, f), (F_ACCEPTED if accepted(f, sc) else 0) if filtered else F_ACCEPTED])
+                cands.append([topk_key(sc, f), F_ACCEPTED if accepted(f, sc) else 0])
                 visited += 1
             # merge: drop `dead`, keep the best LC, remember the best score that fell off
             merged = [e for i, e in enumerate(lst) if i != dead] + cands
@@ -116,7 +117,7 @@ def search(graph_levels, entry_node, score_fn, topK, rerankK, list_cap, rerank_f
             drop = [f2sortable(key_score(e[0])) for e in dropped if (not (e[1] & F_EXPANDED)) or lvl > 0]
             if drop:
                 dm = max(drop)
-                if not filtered:
+                if not filtered and key_score(merged[L - 1][0]) >= 0:
                     ok = f2sortable(key_score(merged[L - 1][0])) > dm
                 else:
                     ok = sum(1 for e in merged if (e[1] & F_ACCEPTED) and f2sortable(key_score(e[0])) > dm) >= L

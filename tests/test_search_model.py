@@ -65,7 +65,7 @@ def world(oracle):
 
 
 @pytest.mark.parametrize("hier", [False, True])
-@pytest.mark.parametrize("kind", ["bq", "f32"])
+@pytest.mark.parametrize("kind", ["bq", "f32", "f32x30"])
 def test_list_model_equals_two_heap_reference(oracle, world, hier, kind):
     w = world
     upper = w["upper"] if hier else None
@@ -79,13 +79,19 @@ def test_list_model_equals_two_heap_reference(oracle, world, hier, kind):
     cases = [dict(topK=10, rerankK=10), dict(topK=10, rerankK=40), dict(topK=1, rerankK=1), dict(topK=5, rerankK=25, rerank=True),
              dict(topK=10, rerankK=30, rerank=True, rerank_floor=0.55), dict(topK=10, rerankK=30, rerank=True, rerank_floor=2.0),
              dict(topK=10, rerankK=20, accept=accept), dict(topK=10, rerankK=20, accept=accept, threshold=0.52, rerank=True),
-             dict(topK=10, rerankK=20, threshold=0.6)]
+             dict(topK=10, rerankK=20, threshold=0.6), dict(topK=10, rerankK=20, accept=np.ones(n, bool))]
     for case in cases:
         topK, rerankK = case["topK"], case["rerankK"]
         thr, floor = case.get("threshold", 0.0), case.get("rerank_floor", 0.0)
         acc = case.get("accept")
         bits = _bits(acc) if acc is not None else None
-        for q in w["queries"]:
+        # f32x30: queries x 30, so about half the DOT_PRODUCT scores (1 + q.x) / 2 are below 0, which searchOneLayer refuses at
+        # threshold 0 on every level, with or without acceptOrds; the last query scores every node of the top level below 0
+        qs = w["queries"]
+        if kind == "f32x30":
+            top = w["data"][w["upper"][1][0]].sum(0)
+            qs = np.concatenate([qs * np.float32(30), (-30 * top / np.linalg.norm(top))[None].astype(np.float32)])
+        for q in qs:
             mk = (lambda: oracle.jvo_scorer_bq(wp(w["words"]), n, dim, fp(q))) if kind == "bq" else \
                  (lambda: oracle.jvo_scorer_f32(o.DOT_PRODUCT, fp(w["data"]), n, dim, fp(q)))
             sf = mk()
