@@ -303,6 +303,14 @@ typedef struct {
                               beam_width + concurrent_window <= 256 (the prune's candidate capacity), else JV_ERR_INVALID */
 } jv_build_params;
 JV_API int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv_graph *out, double *device_ms);
+/* The same build over PQ codes (BuildScoreProvider.pqBuildScoreProvider, for indexes whose fp32 rows do not fit in memory): the
+ * insert of node v searches with the query decode(c_v) over the codes (no rerank, topK = rerankK = beam_width), the prune's keys are
+ * the ADC scores under decode(c_v)'s LUT, and its pair similarities sum the centroid-pair table of the metric (ImmutablePQVectors'
+ * diversity; built and kept on the data set when it has none, as jv_dataset_pq_pair_table does). Everything else is jv_graph_build's.
+ * Errors: JV_ERR_INVALID for a null argument, a data set that is not PQ or a bad metric; JV_ERR_UNSUPPORTED for a degree above 64
+ * or a LUT the prune cannot hold in shared memory (M * k above ~56 K entries, e.g. M > 216 at k = 256). jv_graph_build_stats then
+ * reports this build. */
+JV_API int jv_graph_build_pq(jv_dataset pq, int metric, const jv_build_params *params, jv_graph *out, double *device_ms);
 /* The same build advanced batch by batch, for a build SHARDED over several GPUs (BASELINE config 5): every participant holds a
  * replica of the rows and of the adjacency; per batch each one searches + prunes ITS slice (jv_builder_insert_slice), the caller
  * all-gathers the slices (NCCL; jvector_b200/parallel.py sharded_build), every participant applies the whole batch — back-links in
@@ -311,6 +319,8 @@ JV_API int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *par
  * enqueued on `cuda_stream`. Slices are positions [lo, hi) of the batch (insert) or of the sorted overflow list (re-prune). */
 typedef struct jv_builder_s *jv_builder;
 JV_API int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out);
+/* the step-wise form of jv_graph_build_pq (same checks and errors); every other jv_builder_* call works on either kind */
+JV_API int jv_builder_create_pq(jv_dataset pq, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out);
 JV_API int jv_builder_info(jv_builder b, int *degree, int *row_cap, int *max_batch);
 JV_API int jv_builder_next_batch(jv_builder b, int32_t *first, int32_t *count); /* count = 0: every node is inserted */
 JV_API int jv_builder_insert_slice(jv_builder b, int32_t first, int32_t count, int32_t lo, int32_t hi,

@@ -166,6 +166,14 @@ public:
         check(jv_graph_build(v.handle(), (int)vsf_, &p_, &g, &deviceMs));
         return GraphIndex(g);
     }
+    /// the build over PQ codes (BuildScoreProvider.pqBuildScoreProvider): ADC scores of decode(c_v) for the inserts, the
+    /// centroid-pair table for the diversity test (built on v when it has none)
+    GraphIndex build(const PQVectors &v)
+    {
+        jv_graph g = nullptr;
+        check(jv_graph_build_pq(v.handle(), (int)vsf_, &p_, &g, &deviceMs));
+        return GraphIndex(g);
+    }
     /// markNodeDeleted + removeDeletedNodes (GraphIndexBuilder.java:678-799): a NEW graph without the nodes whose bit is set in
     /// deletedBits (bit node & 31 of word node >> 5), their neighbours' lists repaired on the device; `graph` is left as it is.
     /// Until then, search the marked graph with acceptOrds excluding them. Counters go to removeStats.

@@ -415,7 +415,8 @@ def pack_accept_bits(mask):
 
 
 class GraphIndexBuilder:
-    """base:graph/GraphIndexBuilder.java: (M, beamWidth, neighborOverflow, alpha, addHierarchy) over exact fp32 scores."""
+    """base:graph/GraphIndexBuilder.java: (M, beamWidth, neighborOverflow, alpha, addHierarchy) over exact fp32 scores, or over PQ
+    codes (BuildScoreProvider.pqBuildScoreProvider) when build() is given PQVectors."""
 
     def __init__(self, vsf, M=32, beamWidth=100, neighborOverflow=1.2, alpha=1.2, addHierarchy=False, seed=0, max_batch=0, concurrent_window=-1):
         self.vsf = vsf
@@ -423,10 +424,13 @@ class GraphIndexBuilder:
         self.device_ms = 0.0
 
     def build(self, vectors):
+        """F32Vectors: exact scores (jv_graph_build). PQVectors: the inserts walk the codes with decode(c_v) as the query and the
+        prune compares codes through the centroid-pair table (jv_graph_build_pq), which it builds on the data set if needed."""
         lib = nat.init()
         h = C.c_void_p()
         ms = C.c_double()
-        check(lib.jv_graph_build(vectors._h, int(self.vsf), C.byref(self.params), C.byref(h), C.byref(ms)))
+        fn = lib.jv_graph_build_pq if isinstance(vectors, PQVectors) else lib.jv_graph_build
+        check(fn(vectors._h, int(self.vsf), C.byref(self.params), C.byref(h), C.byref(ms)))
         self.device_ms = ms.value
         s, b, d = C.c_int64(), C.c_int64(), C.c_int64()
         lib.jv_graph_build_stats(C.byref(s), C.byref(b), C.byref(d))

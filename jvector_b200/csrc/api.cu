@@ -1365,22 +1365,30 @@ static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vec
 
 // one upper level: a Vamana graph over its members ids (local row r = node ids[r]), built by the device builder on the members'
 // rows (one gather kernel), from nothing or from `seed` (local rows). ladj: [ids.size()][degree] in node ids. Synchronises `s`.
-static int build_level(jv_dataset f32, int metric, const BuildParams &bp, const std::vector<int32_t> &ids, const BuilderSeed *seed,
+// A PQ data set (jv_graph_build_pq) gives the level its members' code rows; codebooks, centroid, magnitudes and pair tables are shared.
+static int build_level(jv_dataset ds, int metric, const BuildParams &bp, const std::vector<int32_t> &ids, const BuilderSeed *seed,
                        std::vector<int32_t> &ladj, cudaStream_t s)
 {
     const int cnt = (int)ids.size(), degree = bp.degree;
     ladj.assign((size_t)cnt * degree, -1);
     if (cnt <= 1) return JV_OK;
+    const bool pq = ds->d.kind == KIND_PQ;
     DataDesc sub;
     memset(&sub, 0, sizeof(DataDesc));
-    sub.kind = KIND_F32; sub.dim = f32->d.dim; sub.stride = f32->d.stride; sub.n = cnt;
-    DeviceBuffer rows, adj, dids;  // the members' rows, their adjacency, their ids
-    cudaError_t e = rows.alloc((size_t)cnt * sub.stride * 4);
+    if (pq) sub = ds->d;
+    sub.kind = ds->d.kind; sub.dim = ds->d.dim; sub.stride = ds->d.stride; sub.n = cnt;
+    DeviceBuffer rows, adj, dids;  // the members' rows (fp32 rows or code rows), their adjacency, their ids
+    cudaError_t e = rows.alloc(pq ? (size_t)cnt * sub.code_stride : (size_t)cnt * sub.stride * 4);
     if (e == cudaSuccess) e = adj.alloc((size_t)cnt * degree * 4);
     if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
     if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = launch_gather_rows(f32->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
-    sub.rows = rows.get<float>();
+    if (pq) {
+        if (e == cudaSuccess) e = launch_gather_codes(ds->d, dids.get<int32_t>(), cnt, rows.get<uint8_t>(), s);
+        sub.codes = rows.get<uint8_t>();
+    } else {
+        if (e == cudaSuccess) e = launch_gather_rows(ds->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
+        sub.rows = rows.get<float>();
+    }
     BuildStats bs2;
     if (e == cudaSuccess) e = build_graph_flat(sub, metric, bp, adj.get<int32_t>(), g_sm_count, &bs2, s, seed);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ladj.data(), adj.get(), ladj.size() * 4, cudaMemcpyDeviceToHost, s);
@@ -1392,21 +1400,49 @@ static int build_level(jv_dataset f32, int metric, const BuildParams &bp, const 
 }
 
 // every upper level is a Vamana graph over its members, built by the same device builder on the members' rows
-static int build_upper_levels(jv_graph g, jv_dataset f32, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+static int build_upper_levels(jv_graph g, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
 {
-    const int n = (int)f32->d.n;
+    const int n = (int)ds->d.n;
     std::vector<std::vector<int32_t>> members;
     int entry = 0;
     assign_levels(n, bp.degree, seed, members, &entry);
     g->g.entry_node = entry;
     for (size_t l = 0; l < members.size(); l++) {
         std::vector<int32_t> ladj;
-        const int rc = build_level(f32, metric, bp, members[l], nullptr, ladj, s);
+        const int rc = build_level(ds, metric, bp, members[l], nullptr, ladj, s);
         if (rc) return rc;
         g->level_ids.push_back(members[l]);
         g->level_adj.push_back(std::move(ladj));
     }
     return graph_rebuild_upper(g);
+}
+
+// the whole build over an fp32 or a PQ data set whose arguments have been checked: level 0, then the upper levels
+static int graph_build(jv_dataset ds, int metric, const jv_build_params *params, const BuildParams &bp, jv_graph *out, double *device_ms)
+{
+    int rc;
+    if ((rc = t_ctx.init())) return rc;
+    cudaStream_t s = t_ctx.stream;
+    const int n = (int)ds->d.n, degree = params->degree;
+    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
+    g->device = ds->device;
+    memset(&g->g, 0, sizeof(GraphDesc));
+    CK(g->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+    StreamTimer timer;
+    CK(timer.start(s), "event");
+    BuildStats bs;
+    cudaError_t e = build_graph_flat(ds->d, metric, bp, g->adj0.get<int32_t>(), g_sm_count, &bs, s);
+    t_build_stats = bs;
+    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
+    rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "build_graph_flat");
+    if (!rc && params->add_hierarchy && n > 1) rc = build_upper_levels(g.get(), ds, metric, bp, params->seed, s);
+    cudaError_t e1 = timer.stop(s);  // the upper levels are part of the build and of its time
+    cudaStreamSynchronize(s);
+    if (rc) return rc;
+    CK(e1, "event");
+    if (device_ms) *device_ms = timer.ms();
+    *out = g.release();
+    return JV_OK;
 }
 
 int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
@@ -1416,29 +1452,35 @@ int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv
     int rc = check_metric(f32->d, metric);
     if (rc) return rc;
     if ((rc = t_ctx.init())) return rc;
-    cudaStream_t s = t_ctx.stream;
     BuildParams bp;
     if ((rc = build_params_check(params, &bp))) return rc;
-    const int n = (int)f32->d.n, degree = params->degree;
-    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
-    g->device = f32->device;
-    memset(&g->g, 0, sizeof(GraphDesc));
-    CK(g->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
-    StreamTimer timer;
-    CK(timer.start(s), "event");
-    BuildStats bs;
-    cudaError_t e = build_graph_flat(f32->d, metric, bp, g->adj0.get<int32_t>(), g_sm_count, &bs, s);
-    t_build_stats = bs;
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
-    rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "build_graph_flat");
-    if (!rc && params->add_hierarchy && n > 1) rc = build_upper_levels(g.get(), f32, metric, bp, params->seed, s);
-    cudaError_t e1 = timer.stop(s);  // the upper levels are part of the build and of its time
-    cudaStreamSynchronize(s);
+    return graph_build(f32, metric, params, bp, out, device_ms);
+}
+
+// the checks of a build over PQ codes (pqBuildScoreProvider), and the centroid-pair table of the metric, built and kept on the data
+// set when it has none yet (as jv_dataset_pq_pair_table does)
+static int pq_build_check(jv_dataset pq, int metric, const jv_build_params *params, BuildParams *bp)
+{
+    if (pq->d.kind != KIND_PQ) return fail(JV_ERR_INVALID, "graph_build_pq: needs a PQ data set");
+    int rc = check_metric(pq->d, metric);
     if (rc) return rc;
-    CK(e1, "event");
-    if (device_ms) *device_ms = timer.ms();
-    *out = g.release();
-    return JV_OK;
+    if (params->degree > 64)
+        return fail(JV_ERR_UNSUPPORTED, "graph_build_pq: degree " + std::to_string(params->degree) + " > 64, the largest row the builder handles");
+    if ((rc = build_params_check(params, bp))) return rc;
+    if (!pq_prune_fits(pq->d))
+        return fail(JV_ERR_UNSUPPORTED, "graph_build_pq: a LUT of M * k = " + std::to_string(pq->d.M * pq->d.k) +
+                                            " entries does not fit the prune's shared memory next to its candidates (DESIGN §4.3c)");
+    return jv_dataset_pq_pair_table(pq, metric);
+}
+
+int jv_graph_build_pq(jv_dataset pq, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
+{
+    ON_DEVICE_OF(pq);
+    if (!params || !out) return fail(JV_ERR_INVALID, "graph_build_pq: null argument");
+    BuildParams bp;
+    const int rc = pq_build_check(pq, metric, params, &bp);
+    if (rc) return rc;
+    return graph_build(pq, metric, params, bp, out, device_ms);
 }
 
 static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bits[(size_t)v >> 5] >> (v & 31)) & 1u; }
@@ -1614,7 +1656,7 @@ int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_pa
 // re-pruned slice-wise and exchanged the same way. The device pointers are the caller's (e.g. torch tensors = the NCCL buffers).
 struct jv_builder_s {
     int device = 0;
-    jv_dataset f32 = nullptr;
+    jv_dataset data = nullptr;  // fp32 rows, or PQ codes (jv_builder_create_pq)
     int metric = 0;
     jv_build_params params;
     BuildParams bp;
@@ -1632,10 +1674,24 @@ int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params,
     int rc = check_metric(f32->d, metric);
     if (rc) return rc;
     std::unique_ptr<jv_builder_s> b(new jv_builder_s());
-    b->device = f32->device; b->f32 = f32; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
+    b->device = f32->device; b->data = f32; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
     if ((rc = build_params_check(params, &b->bp))) return rc;
     CK(b->timer.start(b->stream), "event");
     CK(builder_create(f32->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
+    *out = b.release();
+    return JV_OK;
+}
+
+int jv_builder_create_pq(jv_dataset pq, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
+{
+    ON_DEVICE_OF(pq);
+    if (!params || !out) return fail(JV_ERR_INVALID, "builder_create_pq: null argument");
+    std::unique_ptr<jv_builder_s> b(new jv_builder_s());
+    int rc = pq_build_check(pq, metric, params, &b->bp);
+    if (rc) return rc;
+    b->device = pq->device; b->data = pq; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
+    CK(b->timer.start(b->stream), "event");
+    CK(builder_create(pq->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
     *out = b.release();
     return JV_OK;
 }
@@ -1649,7 +1705,7 @@ int jv_builder_create_from_graph(jv_graph g, jv_dataset f32, int metric, const j
     int rc = add_check(g, f32, metric, params, &bp);
     if (rc) return rc;
     std::unique_ptr<jv_builder_s> b(new jv_builder_s());
-    b->device = g->device; b->f32 = f32; b->metric = metric; b->params = *params; b->bp = bp; b->stream = (cudaStream_t)cuda_stream;
+    b->device = g->device; b->data = f32; b->metric = metric; b->params = *params; b->bp = bp; b->stream = (cudaStream_t)cuda_stream;
     b->add.reset(new GraphAdd());
     CK(b->timer.start(b->stream), "event");
     std::vector<uint32_t> accept;
@@ -1733,7 +1789,7 @@ int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms)
     if (!out) return fail(JV_ERR_INVALID, "builder_finish: null");
     int rc;
     if ((rc = t_ctx.init())) return rc;
-    const int n = (int)b->f32->d.n, degree = b->bp.degree;
+    const int n = (int)b->data->d.n, degree = b->bp.degree;
     std::unique_ptr<jv_graph_s> g(new jv_graph_s());
     g->device = b->device;
     memset(&g->g, 0, sizeof(GraphDesc));
@@ -1743,8 +1799,8 @@ int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms)
     t_build_stats = bs;
     CK(e, "builder_finish");
     g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
-    if (b->add) rc = add_finish(g.get(), *b->add, b->f32, b->metric, b->bp, b->params.seed, b->stream);  // the hierarchy follows the graph
-    else if (b->params.add_hierarchy && n > 1) rc = build_upper_levels(g.get(), b->f32, b->metric, b->bp, b->params.seed, b->stream);
+    if (b->add) rc = add_finish(g.get(), *b->add, b->data, b->metric, b->bp, b->params.seed, b->stream);  // the hierarchy follows the graph
+    else if (b->params.add_hierarchy && n > 1) rc = build_upper_levels(g.get(), b->data, b->metric, b->bp, b->params.seed, b->stream);
     if (rc) return rc;
     CK(b->timer.stop(b->stream), "event");
     cudaStreamSynchronize(b->stream);

@@ -15,6 +15,8 @@
 // Batches grow geometrically (x 33/32, JV_BUILD_BATCH_DIV) up to max_batch so early nodes see a connected graph. Neighbour lists in the
 // reference are concurrency-order dependent, so parity is on scores and on the recall of the resulting graph
 // (SURVEY §8d C5), not on identical adjacency.
+// Over a PQ data set (BuildScoreProvider.pqBuildScoreProvider, DESIGN §4.3c) the same loop runs on the codes: the insert queries
+// are decode(c_u) (pq_decode_kernel), the walk is the PQ walk, and the prune is prune_kernel<.., KIND_PQ> (ADC keys, pair table).
 #include <limits.h>
 #include <string.h>
 
@@ -31,6 +33,9 @@ namespace jv {
 
 constexpr int PRUNE_THREADS = 256;
 constexpr int PRUNE_MAXC = 256;  // candidates per prune (beam or list capacity), power of two
+// the PQ prune keeps v's whole LUT in shared memory next to its candidate state (the opt-in limit less the kernel's static shared
+// memory): M * k up to ~56 K entries, M = 216 at k = 256
+constexpr int PRUNE_PQ_SMEM_MAX = 226 * 1024;
 
 struct PruneParams {
     DataDesc d;
@@ -80,6 +85,19 @@ __device__ __forceinline__ int32_t prune_candidate(const PruneParams &P, const i
     return w;
 }
 
+// decode(c_v) (ProductQuantization.decode, :454-471): per sub-space the codebook row, plus the global centroid when there is one —
+// one fp32 add per element. The walk and prepare_blob then subtract the centroid again, as PQDecoder.CachingDecoder does, so both
+// roundings are kept. Threads nt-strided over the sub-spaces; out[0, dim).
+__device__ __forceinline__ void pq_decode_row(const DataDesc &d, int v, float *out, int tid, int nt)
+{
+    const uint8_t *c = d.codes + (size_t)v * d.code_stride;
+    for (int m = tid; m < d.M; m += nt) {
+        const int sz = d.sub_sizes[m], off = d.sub_offsets[m];
+        const float *src = d.codebooks + (size_t)d.k * off + (size_t)c[m] * sz;
+        for (int j = 0; j < sz; j++) out[off + j] = d.centroid ? __fadd_rn(src[j], d.centroid[off + j]) : src[j];
+    }
+}
+
 // similarity score of candidate row `c` (global) against a cached row `srow` (shared or global), one warp
 template <int METRIC>
 __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const float4 *srow, int n4, int lane)
@@ -118,13 +136,18 @@ __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const f
 // sequence — and therefore the neighbour list — is exactly the reference loop's, including the alpha = 1.0, 1.2 passes.
 // MAXC: candidate capacity (power of two). The builder uses PRUNE_MAXC; the repair of deleted neighbours also instantiates
 // larger capacities so that no candidate set is ever clipped.
-template <int METRIC, int MAXC = PRUNE_MAXC>
+// KIND_PQ (pqBuildScoreProvider, §4.3c): v's query is decode(c_v) (pq_decode_row, into the row slot), its LUT is prepare_blob's, the
+// keys are score_pq's bits — the walk's — and the fold sums the centroid-pair table (pair_pq_table, ImmutablePQVectors' diversity).
+template <int METRIC, int MAXC = PRUNE_MAXC, int KIND = KIND_F32>
 __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    float *blob = reinterpret_cast<float *>(smem_raw);                       // stride + 4
-    float *newrow = blob + P.d.stride + 4;                                   // stride: the most recently selected row
-    long long *keys = reinterpret_cast<long long *>(newrow + P.d.stride);    // MAXC
+    // f32: blob stride + 4, newrow stride (the most recently selected row). PQ: blob = the LUT, newrow = decode(c_v) (dim rounded to 4)
+    const int blob_fl = KIND == KIND_PQ ? blob_floats(P.d) : P.d.stride + 4;
+    const int row_fl = KIND == KIND_PQ ? (P.d.dim + 3) & ~3 : P.d.stride;
+    float *blob = reinterpret_cast<float *>(smem_raw);
+    float *newrow = blob + blob_fl;
+    long long *keys = reinterpret_cast<long long *>(newrow + row_fl);        // MAXC
     float *maxsim = reinterpret_cast<float *>(keys + MAXC);                  // MAXC
     int32_t *sel_ids = reinterpret_cast<int32_t *>(maxsim + MAXC);           // 128
     uint8_t *state = reinterpret_cast<uint8_t *>(sel_ids + 128);             // MAXC: 0 eligible, 1 selected, 2 dropped
@@ -156,22 +179,35 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             ncs = nc = min(P.deg[v], P.row_cap);
         }
         nc = min(nc, MAXC);
-        prepare_blob(P.d, P.metric, P.d.rows + (size_t)v * P.d.stride, blob, red);
-        // exact scores of the candidates against v, as sortable keys (two rows per warp at a time)
-        for (int i = warp; i < MAXC; i += 2 * NW) {
-            const int i2 = i + NW;
-            const int32_t ca = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1, cb = i2 < nc ? prune_candidate(P, cand, ncs, v, i2) : -1;
-            const bool va = ca >= 0 && ca != v, vb = cb >= 0 && cb != v;
-            long long ka = KEY_MIN, kb = KEY_MIN;
-            if (va || vb) {
-                float sa, sb;
-                score_f32_pair<METRIC>(P.d, blob, va ? ca : cb, vb ? cb : ca, lane, sa, sb);
-                if (va) ka = topk_key(sa, ca);
-                if (vb) kb = topk_key(sb, cb);
+        if (KIND == KIND_PQ) {
+            pq_decode_row(P.d, v, newrow, tid, PRUNE_THREADS);
+            __syncthreads();
+            prepare_blob(P.d, P.metric, newrow, blob, red);
+            // the candidates' ADC scores under v's LUT as sortable keys: 8 lanes per candidate, the walk's scorer and bits
+            for (int i = tid >> 3; i < MAXC; i += PRUNE_THREADS / 8) {
+                const int32_t c = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1;
+                long long kc = KEY_MIN;
+                if (c >= 0 && c != v) kc = topk_key(score_pq<METRIC>(P.d, blob, c, lane & 7), c);
+                if ((lane & 7) == 0) keys[i] = kc;
             }
-            if (lane == 0) {
-                keys[i] = ka;
-                if (i2 < MAXC) keys[i2] = kb;
+        } else {
+            prepare_blob(P.d, P.metric, P.d.rows + (size_t)v * P.d.stride, blob, red);
+            // exact scores of the candidates against v, as sortable keys (two rows per warp at a time)
+            for (int i = warp; i < MAXC; i += 2 * NW) {
+                const int i2 = i + NW;
+                const int32_t ca = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1, cb = i2 < nc ? prune_candidate(P, cand, ncs, v, i2) : -1;
+                const bool va = ca >= 0 && ca != v, vb = cb >= 0 && cb != v;
+                long long ka = KEY_MIN, kb = KEY_MIN;
+                if (va || vb) {
+                    float sa, sb;
+                    score_f32_pair<METRIC>(P.d, blob, va ? ca : cb, vb ? cb : ca, lane, sa, sb);
+                    if (va) ka = topk_key(sa, ca);
+                    if (vb) kb = topk_key(sb, cb);
+                }
+                if (lane == 0) {
+                    keys[i] = ka;
+                    if (i2 < MAXC) keys[i2] = kb;
+                }
             }
         }
         __syncthreads();
@@ -209,7 +245,8 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
                 const int32_t c = key_node(keys[pick]);
                 const float4 *crow = reinterpret_cast<const float4 *>(P.d.rows + (size_t)c * P.d.stride);
                 if (tid == 0) { state[pick] = 1; sel_ids[nsel] = c; }
-                for (int t = tid; t < n4; t += PRUNE_THREADS) reinterpret_cast<float4 *>(newrow)[t] = __ldg(crow + t);
+                if (KIND != KIND_PQ)
+                    for (int t = tid; t < n4; t += PRUNE_THREADS) reinterpret_cast<float4 *>(newrow)[t] = __ldg(crow + t);
                 nsel++;
                 cursor = pick + 1;
                 __syncthreads();
@@ -217,8 +254,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
                 // fold the new neighbour into every still-eligible candidate's running maximum
                 for (int i = warp; i < nvalid; i += NW) {
                     if (state[i] != 0) continue;
-                    const float4 *row = reinterpret_cast<const float4 *>(P.d.rows + (size_t)key_node(keys[i]) * P.d.stride);
-                    const float ps = pair_rows<METRIC>(row, reinterpret_cast<const float4 *>(newrow), n4, lane);
+                    float ps;
+                    if (KIND == KIND_PQ) {
+                        ps = pair_pq_table<METRIC>(P.d, key_node(keys[i]), c, lane);
+                    } else {
+                        const float4 *row = reinterpret_cast<const float4 *>(P.d.rows + (size_t)key_node(keys[i]) * P.d.stride);
+                        ps = pair_rows<METRIC>(row, reinterpret_cast<const float4 *>(newrow), n4, lane);
+                    }
                     if (lane == 0) {
                         const float m = fmaxf(maxsim[i], ps);
                         maxsim[i] = m;
@@ -886,10 +928,66 @@ cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int 
     return cudaGetLastError();
 }
 
+// code rows [ids[i]] of a PQ data set gathered into a dense array (upper levels of a PQ build): one thread per 32-bit word
+__global__ void __launch_bounds__(256) gather_codes_kernel(const uint32_t *__restrict__ codes, int words, const int32_t *__restrict__ ids, int count,
+                                                           uint32_t *__restrict__ out)
+{
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)count * words) return;
+    const int i = (int)(idx / words), w = (int)(idx - (long long)i * words);
+    out[idx] = __ldg(codes + (size_t)ids[i] * words + w);
+}
+
+cudaError_t launch_gather_codes(const DataDesc &pq, const int32_t *ids_dev, int count, uint8_t *out_dev, cudaStream_t s)
+{
+    if (count <= 0) return cudaSuccess;
+    const int words = pq.code_stride >> 2;
+    const long long total = (long long)count * words;
+    gather_codes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint32_t *>(pq.codes), words, ids_dev, count,
+                                                                        reinterpret_cast<uint32_t *>(out_dev));
+    g_launches++;
+    return cudaGetLastError();
+}
+
+// the insert searches' queries of a PQ build: decode(c_u) for nodes first .. first + count - 1 -> out [count][dim], one CTA per node
+__global__ void __launch_bounds__(128) pq_decode_kernel(DataDesc d, int first, int count, float *out)
+{
+    for (int i = blockIdx.x; i < count; i += gridDim.x) pq_decode_row(d, first + i, out + (size_t)i * d.dim, threadIdx.x, blockDim.x);
+}
+
 static size_t prune_smem_bytes(const DataDesc &d, int maxc = PRUNE_MAXC)
 {
     size_t b = (size_t)(d.stride + 4) * 4 + (size_t)d.stride * 4 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
     return (b + 15) & ~(size_t)15;
+}
+
+// the PQ prune's shared memory: v's LUT, decode(c_v), then the candidate state of prune_kernel
+static size_t prune_pq_smem_bytes(const DataDesc &d, int maxc)
+{
+    size_t b = (size_t)blob_floats(d) * 4 + (size_t)((d.dim + 3) & ~3) * 4 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
+    return (b + 15) & ~(size_t)15;
+}
+
+bool pq_prune_fits(const DataDesc &pq) { return prune_pq_smem_bytes(pq, PRUNE_MAXC) <= (size_t)PRUNE_PQ_SMEM_MAX; }
+
+// PQ: no Gram tier (it would change the pair bits); the incremental kernel at the smallest capacity that holds the candidates
+template <int METRIC>
+static cudaError_t launch_prune_pq_t(const PruneParams &P, int grid, int ncmax, cudaStream_t s)
+{
+    cudaError_t e;
+#define JV_PQ_PRUNE_LAUNCH(MAXC)                                                                                                     \
+    do {                                                                                                                             \
+        const size_t sm_ = prune_pq_smem_bytes(P.d, MAXC);                                                                           \
+        if ((e = cudaFuncSetAttribute(prune_kernel<METRIC, MAXC, KIND_PQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_)) != cudaSuccess) \
+            return e;                                                                                                                \
+        prune_kernel<METRIC, MAXC, KIND_PQ><<<grid, PRUNE_THREADS, sm_, s>>>(P);                                                     \
+    } while (0)
+    if (ncmax <= 64) JV_PQ_PRUNE_LAUNCH(64);
+    else if (ncmax <= 128) JV_PQ_PRUNE_LAUNCH(128);
+    else JV_PQ_PRUNE_LAUNCH(256);
+#undef JV_PQ_PRUNE_LAUNCH
+    g_launches++;
+    return cudaGetLastError();
 }
 
 template <int METRIC>
@@ -897,6 +995,7 @@ static cudaError_t launch_prune_t(const PruneParams &P, int grid, size_t smem, c
 {
     // candidate sets that fit a tile go through the Gram-matrix kernel; anything larger keeps the incremental kernel
     const int ncmax = P.mode == 0 ? P.cand_stride + P.window : P.row_cap;
+    if (P.d.kind == KIND_PQ) return launch_prune_pq_t<METRIC>(P, grid, ncmax, s);
     cudaError_t e;
     // Gram products on the tensor cores (wgmma, 3xTF32) unless JV_PRUNE_GRAM=ffma asks for the CUDA-core kernel
     static const bool use_tc = !(getenv("JV_PRUNE_GRAM") && getenv("JV_PRUNE_GRAM")[0] == 'f');
@@ -961,6 +1060,7 @@ struct GraphBuilder {
     size_t cub_bytes = 0;
     int32_t *own_rows = nullptr;  // single-GPU path: the slice buffers are the builder's own
     int *own_deg = nullptr;
+    float *qdec = nullptr;        // PQ: the insert searches' queries decode(c_u), [max_batch][dim]
     std::vector<DeviceBuffer> mem;  // owns every block above
     DeviceBuffer scratch;           // the insert searches' scratch, grown with the slice
     BuildStats st = {0, 0, 0, 0, 0};
@@ -974,7 +1074,9 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
                            const BuilderSeed *seed)
 {
     const int n = (int)d.n;
-    if (d.kind != KIND_F32 || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
+    if ((d.kind != KIND_F32 && d.kind != KIND_PQ) || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
+    // PQ: a fresh build only, with the centroid-pair table of this metric (jv_dataset_pq_pair_table) and a LUT the prune can hold
+    if (d.kind == KIND_PQ && (seed || !d.pair_table[metric == JV_METRIC_EUCLIDEAN ? 0 : 1] || !pq_prune_fits(d))) return cudaErrorInvalidValue;
     if (seed && (seed->count < 0 || seed->count > n || (seed->count > 0 && (!seed->rows_dev || seed->width < 1)) || seed->entry >= seed->count))
         return cudaErrorInvalidValue;
     std::unique_ptr<GraphBuilder> B(new GraphBuilder());
@@ -1010,6 +1112,7 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
     JV_TRY(alloc_owned(owned, B->head_target, mb * B->degree * 4));
     JV_TRY(alloc_owned(owned, B->own_rows, mb * B->degree * 4));
     JV_TRY(alloc_owned(owned, B->own_deg, mb * 4));
+    if (d.kind == KIND_PQ) JV_TRY(alloc_owned(owned, B->qdec, mb * d.dim * 4));
     {
         size_t b1 = 0, b2 = 0;
         cub::DeviceRadixSort::SortKeys(nullptr, b1, B->pairs, B->pairs_sorted, (int)(mb * B->degree), 0, 64, s);
@@ -1086,8 +1189,18 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
     memset(&lenient, 0, sizeof(lenient));
     lenient.lenient = 1;  // an insert search never fails the build: see SearchParams::lenient
     lenient.accept_bits = B->accept;  // an add into a graph with marked nodes walks through them but never links to them
-    JV_TRY(launch_search(g, B->d, nullptr, B->metric, B->d.rows + (size_t)(first + lo) * B->d.stride, m, B->beam, B->beam, plan, B->scratch.get(), B->work_counter,
-                         B->res_nodes, B->res_scores, B->counters, B->overflow, nullptr, B->d.stride, &lenient, s));
+    const float *queries = B->d.rows + (size_t)(first + lo) * B->d.stride;
+    int query_stride = B->d.stride;
+    if (B->d.kind == KIND_PQ) {
+        // searchProviderFor over PQ: the walk scores with the codes only (no rerank), its query is decode(c_u)
+        pq_decode_kernel<<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, B->qdec);
+        g_launches++;
+        JV_TRY(cudaGetLastError());
+        queries = B->qdec;
+        query_stride = B->d.dim;
+    }
+    JV_TRY(launch_search(g, B->d, nullptr, B->metric, queries, m, B->beam, B->beam, plan, B->scratch.get(), B->work_counter,
+                         B->res_nodes, B->res_scores, B->counters, B->overflow, nullptr, query_stride, &lenient, s));
     PruneParams P = prune_params(B);
     P.mode = 0; P.node_base = first + lo; P.count = m; P.cand = B->res_nodes; P.cand_stride = B->beam;
     P.window = B->window; P.batch_first = first; P.batch_count = count;

@@ -165,7 +165,8 @@ struct BuilderSeed {
     int32_t entry;
     const uint32_t *accept;
 };
-// flat Vamana graph over rows [0, n) of an f32 data set; adj_out_dev [n][degree] (-1 padded); entry node is 0 (or the seed's)
+// flat Vamana graph over rows [0, n) of an f32 data set, or of a PQ data set that carries the metric's pair table and no seed
+// (pqBuildScoreProvider); adj_out_dev [n][degree] (-1 padded); entry node is 0 (or the seed's)
 cudaError_t build_graph_flat(const DataDesc &f32, int metric, const BuildParams &bp, int32_t *adj_out_dev, int sm_count,
                              BuildStats *stats, cudaStream_t s, const BuilderSeed *seed = nullptr);
 // the same build advanced batch by batch; a sharded build calls the *_slice functions for its part of each batch and moves the
@@ -187,6 +188,9 @@ int builder_row_cap(const GraphBuilder *B);
 int builder_degree(const GraphBuilder *B);
 int builder_max_batch(const GraphBuilder *B);
 cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s);
+// PQ build (pqBuildScoreProvider): code rows [ids[i]] into out_dev [count][code_stride]; whether the PQ prune holds the data set's LUT
+cudaError_t launch_gather_codes(const DataDesc &pq, const int32_t *ids_dev, int count, uint8_t *out_dev, cudaStream_t s);
+bool pq_prune_fits(const DataDesc &pq);
 
 // removeDeletedNodes on one level (see build.cu). rows: members of the level; row r is node ids_dev[r] (nullptr: node r, level 0);
 // rowmap_dev[node] = the node's row on this level (nullptr: identity). dead_dev: bitset of deleted nodes (bit node & 31 of word
