@@ -395,6 +395,15 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                             // the row is needed one barrier from now: start the DRAM -> L2 transfer of all of it at once (one
                             // UBLKPF per row; bytes in flight that occupy no registers and no shared memory)
                             if (KIND == KIND_F32 && P.row_prefetch == 1) bulk_prefetch_l2(P.approx.rows + (size_t)f * P.approx.stride, (unsigned)P.approx.stride * 4u);
+                            // a sketched walk (the condition of `sketched` below) reads this row's sketch and {s, r} first, one barrier
+                            // from now: request them (768 + 8 B at d = 768) so that the bound waits on L2, not DRAM. The full rows are
+                            // not prefetched: only the ~17 % the bound does not settle read them, and they would not fit in L2.
+                            if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && P.approx.sketch != nullptr) {
+                                const char *sk = reinterpret_cast<const char *>(P.approx.sketch) + (size_t)f * P.approx.sketch_stride;
+                                for (int o = 0; o < P.approx.sketch_stride; o += 128) prefetch_l2(sk + o);
+                                prefetch_l2(sk + P.approx.sketch_stride - 1);
+                                prefetch_l2(P.approx.sketch_meta + f);
+                            }
                             if (KIND == KIND_NVQ && P.row_prefetch == 1) {
                                 bulk_prefetch_l2(P.approx.bytes + (size_t)f * P.approx.byte_stride, (unsigned)P.approx.byte_stride);
                                 prefetch_l2(P.approx.params + (size_t)f * 4 * P.approx.nsub);  // {min, max, growthRate, midpoint} per sub-vector
@@ -1029,8 +1038,8 @@ size_t search_scratch_bytes(const SearchPlan &p) { return SearchScratch(p, nullp
 // a batch with more queries than resident CTAs fills the GPU: bandwidth bound rather than latency bound
 static bool fills_gpu(const SearchPlan &plan, int nq) { return nq > plan.ctas; }
 
-// fp32 DOT walks of such batches drop hopeless neighbours on the bound of their row sketch (sketch_bound_pair): HBM bound, half the
-// bytes per dropped row. A latency-bound batch reads the rows it prefetched anyway.
+// fp32 DOT walks of such batches drop hopeless neighbours on the bound of their row sketch (sketch_bound_pair): HBM bound, a quarter
+// of the bytes per dropped row, the sketch requested at gather time. A latency-bound batch reads the rows it prefetched anyway.
 bool search_uses_sketch(const DataDesc &approx, int metric, const SearchPlan &plan, int nq)
 {
     return approx.kind == KIND_F32 && metric == JV_METRIC_DOT && fills_gpu(plan, nq);

@@ -9,6 +9,11 @@ with tools/build_variant.sh) and reports
 for the fp16 sketch and for an int8 sketch with one scale per row; b is replayed on the host over a sample of the drops
 ({query, row, key of the list's last entry}). Predicted bytes per visited row = sketch + 8 + (1 - f b) 4 d, against 4 d + 8.
 
+For the two-tier int8 sketch (tests/row_bound_coarse.py) it also reports b1, the share of the drops the coarse half's bound catches,
+and b12, the share caught by the coarse or the int8 bound, and predicts (ss = sketch bytes per row)
+
+    (ss / 2 + 16) + 8 + (1 - f b1) ss / 2 + (1 - f b12) 4 d    against the one-tier ss + 8 + 8 + (1 - f b) 4 d.
+
     python tools/row_bound_stats.py [--out row_bound_stats.json]"""
 import argparse
 import json
@@ -35,6 +40,7 @@ os.environ["JV_B200_SO"] = VARIANT
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import bench  # noqa: E402
+import row_bound_coarse as rbc  # noqa: E402
 import row_bound_model as rb  # noqa: E402
 
 args = argparse.Namespace(impl="b200", n=a.n, dim=768, nq=a.nq, dist="latent", topk=10, gt_queries=500)
@@ -84,6 +90,16 @@ for name, enc, sketch_bytes in (("fp16", rb.encode_fp16, 2 * stride), ("int8", r
     pred = sketch_bytes + 8 + (1.0 - f * b) * 4 * stride
     out["formats"][name] = {"b": b, "sketch_bytes": sketch_bytes, "predicted_bytes_per_row": pred, "vs_today": pred / (4 * stride + 8),
                             "median_radius_over_norm": float(np.median(rad / np.maximum(np.linalg.norm(rows, axis=1), 1e-30)))}
+# the two-tier int8 sketch: the coarse half (high nibbles, c1 = 16 (c >> 4) + 8, radius r1) first, the int8 bound for what it keeps
+# (scale and caught are the int8 pass of the loop above)
+ss = rbc.sketch_stride(stride)
+c1, _, rad1 = rbc.encode_coarse(rows, stride)
+caught1 = rb.topk_key(rb.dot_score_up(rbc.upper_bound_raw(qs, c1, scale, rad1, stride)), smp["row"]) < smp["last_key"]
+b, b1, b12 = out["formats"]["int8"]["b"], float(caught1.mean()), float((caught1 | caught).mean())
+today = ss + 8 + 8 + (1.0 - f * b) * 4 * stride
+two = (ss / 2 + 16) + 8 + (1.0 - f * b1) * ss / 2 + (1.0 - f * b12) * 4 * stride
+out["int8_two_tier"] = {"b1": b1, "b12": b12, "b": b, "bytes_per_row_today": today, "predicted_bytes_per_row": two, "vs_today": two / today,
+                        "median_coarse_radius_over_norm": float(np.median(rad1 / np.maximum(np.linalg.norm(rows, axis=1), 1e-30)))}
 print(json.dumps(out, indent=1))
 if a.out:
     os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
