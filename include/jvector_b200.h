@@ -216,6 +216,37 @@ JV_API int jv_nvq_encode_dataset(jv_dataset f32, int nsub, const float *mean, in
 /* NVQ inline vectors without a host round trip: encode the resident fp32 rows into a NEW resident NVQ data set */
 JV_API int jv_nvq_encode_dataset_resident(jv_dataset f32, int nsub, const float *mean, int learn, jv_dataset *out);
 
+/* ---- PQ training: ProductQuantization.compute / refine with isotropic (UNWEIGHTED) loss, on the device ----
+ * The training rows are the resident rows of `f32` (an out-of-core index registers a sample), all of them, or, above the cap, a
+ * sample of `cap` rows drawn with Floyd's algorithm from `seed` and sorted. compute: optional global centring (the mean is an int64
+ * fixed-point sum, independent of thread order), k-means++ seeding (as an exponential race: the same distribution as the
+ * reference's inverse-CDF scan), then Lloyd as KMeansPlusPlusClusterer.cluster(lloyd_iterations, 0): each sub-space stops once at
+ * most 1 % of its rows change cluster; an empty cluster is reseeded to a random training row. refine: Lloyd only, from the given
+ * codebooks, on the rows minus `centroid`; 0 rounds returns the codebooks bit for bit. The result is a pure function of the rows
+ * and the parameters. Errors: JV_ERR_INVALID for a data set that is not fp32, M outside 1..dim, k outside 1..256, fewer training
+ * rows than k, a negative iteration count or cap, a null required pointer, globally_center with a NULL centroid_out;
+ * JV_ERR_OOM when the training buffers (about n_train * dim * 4 + n_train * M * 8 bytes) do not fit. */
+typedef struct {
+    int M;                  /* sub-spaces; sizes and offsets as ProductQuantization.getSubvectorSizesAndOffsets */
+    int k;                  /* clusterCount, 1..256 */
+    int globally_center;    /* compute only: subtract the training rows' mean first (the centroid is written to centroid_out) */
+    int lloyd_iterations;   /* K_MEANS_ITERATIONS (6) for compute, lloydsRounds for refine; >= 0 */
+    int64_t max_train_rows; /* 0 = MAX_PQ_TRAINING_SET_SIZE (128 000) */
+    uint64_t seed;
+} jv_pq_train_params;
+typedef struct {
+    int64_t train_rows;        /* rows trained on */
+    int32_t max_lloyd_updates; /* centroid updates of the sub-space that ran longest */
+    int64_t changed_last;      /* summed over sub-spaces: rows that changed cluster in the sub-space's last reassignment */
+    int64_t empty_reseeds;     /* empty clusters reseeded to a random training row */
+    int64_t seeding_fallbacks; /* seeding rounds in which every row already coincided with a chosen centroid */
+    double device_ms;
+} jv_pq_train_stats;
+JV_API int jv_pq_train(jv_dataset f32, const jv_pq_train_params *p, float *codebooks_out /* [k * dim], the jv_dataset_register_pq layout */,
+                       float *centroid_out /* [dim] or NULL */, jv_pq_train_stats *stats /* may be NULL */);
+JV_API int jv_pq_refine(jv_dataset f32, const jv_pq_train_params *p, const float *codebooks, const float *centroid /* or NULL */,
+                        float *codebooks_out, jv_pq_train_stats *stats /* may be NULL */);
+
 /* ---- graph: ImmutableGraphIndex adjacency in HBM + GraphSearcher traversal on the device ---- */
 /* adj0: [n][degree] int32, -1 padded (level 0). */
 JV_API int jv_graph_create(int32_t n, int degree, const int32_t *adj0, int32_t entry_node, jv_graph *out);

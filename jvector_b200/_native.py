@@ -41,6 +41,16 @@ class RemoveStats(C.Structure):
                 ("max_candidates", C.c_int32), ("random_fallbacks", C.c_int64), ("device_ms", C.c_double)]
 
 
+class PQTrainParams(C.Structure):
+    _fields_ = [("M", C.c_int), ("k", C.c_int), ("globally_center", C.c_int), ("lloyd_iterations", C.c_int), ("max_train_rows", C.c_int64),
+                ("seed", C.c_uint64)]
+
+
+class PQTrainStats(C.Structure):
+    _fields_ = [("train_rows", C.c_int64), ("max_lloyd_updates", C.c_int32), ("changed_last", C.c_int64), ("empty_reseeds", C.c_int64),
+                ("seeding_fallbacks", C.c_int64), ("device_ms", C.c_double)]
+
+
 # every symbol include/jvector_b200.h declares: (name, restype, argtypes)
 _F, _I, _Z, _P, _L = C.c_float, C.c_int, C.c_size_t, C.c_void_p, C.c_int64
 SYMBOLS = [
@@ -90,6 +100,8 @@ SYMBOLS = [
     ("jv_bq_encode_dataset", _I, [_P, u64p]), ("jv_pq_encode_dataset", _I, [_P, _I, _I, f32p, f32p, u8p]),
     ("jv_nvq_encode_dataset", _I, [_P, _I, f32p, _I, f32p, u8p]),
     ("jv_nvq_encode_dataset_resident", _I, [_P, _I, f32p, _I, C.POINTER(_P)]),
+    ("jv_pq_train", _I, [_P, C.POINTER(PQTrainParams), f32p, f32p, C.POINTER(PQTrainStats)]),
+    ("jv_pq_refine", _I, [_P, C.POINTER(PQTrainParams), f32p, f32p, f32p, C.POINTER(PQTrainStats)]),
     ("jv_graph_create", _I, [C.c_int32, _I, i32p, C.c_int32, C.POINTER(_P)]), ("jv_graph_add_level", _I, [_P, C.c_int32, i32p, i32p]),
     ("jv_graph_fuse_pq", _I, [_P, _P]), ("jv_graph_fused_download", _I, [_P, u8p, C.POINTER(_I)]),
     ("jv_graph_free", _I, [_P]), ("jv_graph_info", _I, [_P, i32p, C.POINTER(_I), C.POINTER(_I), i32p]),

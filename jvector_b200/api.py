@@ -110,6 +110,48 @@ class PQVectors(_Vectors):
         return out
 
 
+class ProductQuantization:
+    """base:quantization/ProductQuantization.java with isotropic (UNWEIGHTED) loss, trained on the device (jv_pq_train /
+    jv_pq_refine). codebooks: float32 [k * dim] (codebook m = [k][size_m] at k * offset_m); centroid: the global centroid or None."""
+
+    K_MEANS_ITERATIONS = 6
+
+    def __init__(self, codebooks, M, k, dim, centroid=None, stats=None):
+        self.codebooks, self.M, self.k, self.dim, self.centroid, self.stats = codebooks, M, k, dim, centroid, stats
+
+    @staticmethod
+    def _stats(st):
+        return {name: getattr(st, name) for name, _ in nat.PQTrainStats._fields_}
+
+    @classmethod
+    def compute(cls, vectors, M, clusterCount=256, globallyCenter=False, seed=0):
+        """ProductQuantization.compute over F32Vectors resident in HBM: at most 128 000 sampled training rows, k-means++ seeding,
+        K_MEANS_ITERATIONS Lloyd iterations with the reference's early stop. The result is a pure function of the rows and seed."""
+        lib = nat.init()
+        dim = vectors.dimension()
+        p = nat.PQTrainParams(M, clusterCount, 1 if globallyCenter else 0, cls.K_MEANS_ITERATIONS, 0, seed)
+        cb = np.empty(clusterCount * dim, np.float32)
+        cen = np.empty(dim, np.float32) if globallyCenter else None
+        st = nat.PQTrainStats()
+        check(lib.jv_pq_train(vectors._h, C.byref(p), fp(cb), fp(cen), C.byref(st)))
+        return cls(cb, M, clusterCount, dim, cen, cls._stats(st))
+
+    def refine(self, vectors, lloydsRounds=1, seed=0):
+        """ProductQuantization.refine: lloydsRounds Lloyd iterations from these codebooks over `vectors` (minus the centroid);
+        returns a new ProductQuantization with the same centroid."""
+        lib = nat.init()
+        p = nat.PQTrainParams(self.M, self.k, 0, lloydsRounds, 0, seed)
+        cb = np.empty_like(self.codebooks)
+        st = nat.PQTrainStats()
+        check(lib.jv_pq_refine(vectors._h, C.byref(p), fp(self.codebooks), fp(self.centroid), fp(cb), C.byref(st)))
+        return ProductQuantization(cb, self.M, self.k, self.dim, self.centroid, self._stats(st))
+
+    def encodeAll(self, vectors):
+        """ProductQuantization.encodeAll of resident F32Vectors into resident PQVectors"""
+        codes = pq_encode_all(vectors, self.codebooks, self.M, self.k, self.centroid)
+        return PQVectors(codes, self.codebooks, self.dim, self.k, self.centroid)
+
+
 def kmeans_assign(points, centroids):
     """KMeansPlusPlusClusterer.getNearestCluster for a batch of points (the Lloyd assignment step), one launch."""
     lib = nat.init()

@@ -853,6 +853,49 @@ int jv_pq_encode_dataset(jv_dataset f32, int M, int k, const float *codebooks, c
     return pq_encode_impl(nullptr, f32->d.rows, f32->d.stride, f32->d.n, f32->d.dim, M, k, codebooks, centroid, codes_out);
 }
 
+// ------------------------------------------------------------------------------------------------ PQ training
+constexpr int64_t MAX_PQ_TRAINING_SET_SIZE = 128000;  // ProductQuantization.java:64
+
+static int pq_train_impl(jv_dataset f32, const jv_pq_train_params *p, const float *codebooks, const float *centroid, float *codebooks_out,
+                         float *centroid_out, jv_pq_train_stats *stats)
+{
+    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "pq_train: needs an fp32 data set");
+    if (!p || !codebooks_out) return fail(JV_ERR_INVALID, "pq_train: null argument");
+    if (p->M < 1 || p->M > f32->d.dim) return fail(JV_ERR_INVALID, "pq_train: M must be in 1..dim");
+    if (p->k < 1 || p->k > 256) return fail(JV_ERR_INVALID, "pq_train: k must be in 1..256");
+    if (p->lloyd_iterations < 0 || p->max_train_rows < 0) return fail(JV_ERR_INVALID, "pq_train: negative iteration count or row cap");
+    const int64_t cap = p->max_train_rows ? p->max_train_rows : MAX_PQ_TRAINING_SET_SIZE;
+    if (std::min<int64_t>(f32->d.n, cap) < p->k) return fail(JV_ERR_INVALID, "pq_train: fewer training rows than clusters");
+    int rc;
+    if ((rc = t_ctx.init())) return rc;
+    const PqTrainArgs a = {p->M, p->k, p->globally_center, p->lloyd_iterations, (long long)cap, p->seed};
+    PqTrainStats st;
+    CK(pq_train(f32->d, a, codebooks, centroid, codebooks_out, centroid_out, &st, t_ctx.stream), "pq_train");
+    if (stats) {
+        stats->train_rows = st.train_rows;
+        stats->max_lloyd_updates = st.max_lloyd_updates;
+        stats->changed_last = st.changed_last;
+        stats->empty_reseeds = st.empty_reseeds;
+        stats->seeding_fallbacks = st.seeding_fallbacks;
+        stats->device_ms = st.device_ms;
+    }
+    return JV_OK;
+}
+
+int jv_pq_train(jv_dataset f32, const jv_pq_train_params *p, float *codebooks_out, float *centroid_out, jv_pq_train_stats *stats)
+{
+    ON_DEVICE_OF(f32);
+    if (p && p->globally_center && !centroid_out) return fail(JV_ERR_INVALID, "pq_train: globally_center needs centroid_out");
+    return pq_train_impl(f32, p, nullptr, nullptr, codebooks_out, centroid_out, stats);
+}
+
+int jv_pq_refine(jv_dataset f32, const jv_pq_train_params *p, const float *codebooks, const float *centroid, float *codebooks_out, jv_pq_train_stats *stats)
+{
+    ON_DEVICE_OF(f32);
+    if (!codebooks) return fail(JV_ERR_INVALID, "pq_refine: null codebooks");
+    return pq_train_impl(f32, p, codebooks, centroid, codebooks_out, nullptr, stats);
+}
+
 static int nvq_encode_impl(const float *rows, const float *rows_dev, int row_stride, int64_t n, int dim, int nsub, const float *mean, int learn,
                            float *params_out, uint8_t *bytes_out)
 {

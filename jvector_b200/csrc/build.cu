@@ -1372,19 +1372,6 @@ __global__ void __launch_bounds__(256) repair_count_kernel(const int32_t *__rest
     }
 }
 
-// the counter-based generator of the random fallback: a pure function of (seed, level, node, attempt)
-__host__ __device__ __forceinline__ uint64_t repair_mix(uint64_t x)
-{
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
-__host__ __device__ __forceinline__ uint64_t repair_random(uint64_t seed, int level, int node, int attempt)
-{
-    return repair_mix(repair_mix(repair_mix(seed ^ (uint64_t)(uint32_t)level) ^ (uint64_t)(uint32_t)node) ^ (uint64_t)(uint32_t)attempt);
-}
-
 __device__ __forceinline__ void bitonic_sort_asc_int(int32_t *keys, int n_pow2)
 {
     for (int k = 2; k <= n_pow2; k <<= 1) {
@@ -1450,7 +1437,7 @@ __global__ void __launch_bounds__(256) repair_gather_kernel(const int32_t *__res
             int32_t *pick = buf + degree * (degree + 1);
             int np = 0;
             for (int at = 0; at < 2 * degree && np < degree; at++) {
-                const int32_t k = members[repair_random(seed, level, v, at) % (uint64_t)nmembers];
+                const int32_t k = members[counter_random(seed, level, v, at) % (uint64_t)nmembers];
                 bool dup = k == v;
                 for (int p = 0; p < np && !dup; p++) dup = pick[p] == k;
                 if (!dup) pick[np++] = k;

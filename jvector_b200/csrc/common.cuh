@@ -186,4 +186,42 @@ __host__ __device__ __forceinline__ int next_pow2(int v)
     return p;
 }
 
+// The library's counter-based generator: a pure function of (seed, a, b, c), so a draw does not depend on thread order.
+// Callers: the removal's random fallback (seed, level, node, attempt) and PQ training (pq_train.cu).
+__host__ __device__ __forceinline__ uint64_t mix64(uint64_t x)
+{
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+__host__ __device__ __forceinline__ uint64_t counter_random(uint64_t seed, int a, int b, int c)
+{
+    return mix64(mix64(mix64(seed ^ (uint64_t)(uint32_t)a) ^ (uint64_t)(uint32_t)b) ^ (uint64_t)(uint32_t)c);
+}
+
+// -ln(u) for u in (0, 1] as a fixed sequence of round-to-nearest fp32 operations (no log intrinsic, no FMA), so a host model
+// repeats it bit for bit: u = m 2^e with m in [sqrt(1/2), sqrt(2)], ln m = 2 s (1 + z/3 + z^2/5 + z^3/7 + z^4/9) with
+// s = (m - 1) / (m + 1), z = s^2 (|s| <= 0.172: the truncated series is below 1e-9 relative). ln(1) gives +0.
+__device__ __forceinline__ float neg_ln_unit(float u)
+{
+    const int bits = __float_as_int(u);
+    int e = ((bits >> 23) & 0xff) - 127;
+    float m = __int_as_float((bits & 0x7fffff) | 0x3f800000);
+    if (m > __int_as_float(0x3fb504f3)) {  // fp32 sqrt(2)
+        m = __fmul_rn(m, 0.5f);
+        e += 1;
+    }
+    const float s = __fdiv_rn(__fsub_rn(m, 1.0f), __fadd_rn(m, 1.0f));
+    const float z = __fmul_rn(s, s);
+    float p = __int_as_float(0x3de38e39);                              // 1/9
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0x3e124925));        // 1/7
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0x3e4ccccd));        // 1/5
+    p = __fadd_rn(__fmul_rn(p, z), __int_as_float(0x3eaaaaab));        // 1/3
+    p = __fadd_rn(__fmul_rn(p, z), 1.0f);
+    const float ln_m = __fmul_rn(__fmul_rn(2.0f, s), p);
+    const float ln_u = __fadd_rn(__fmul_rn((float)e, __int_as_float(0x3f317218)), ln_m);  // fp32 ln(2)
+    return __fsub_rn(0.0f, ln_u);
+}
+
 }  // namespace jv

@@ -206,4 +206,25 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
                          int sm_count, RepairStats *st, cudaStream_t s);
 cudaError_t launch_clear_dead_rows(int32_t *adj_dev, int n, int degree, const uint32_t *dead_dev, cudaStream_t s);
 
+// ---- pq_train.cu: ProductQuantization.compute / refine (UNWEIGHTED) ----
+struct PqTrainArgs {
+    int M, k;
+    int globally_center;  // compute only
+    int iters;            // Lloyd iterations (>= 0)
+    long long cap;        // training rows at most (> 0)
+    uint64_t seed;
+};
+struct PqTrainStats {
+    long long train_rows;
+    int max_lloyd_updates;  // centroid updates of the sub-space that ran longest
+    long long changed_last;  // summed over sub-spaces: rows that moved in the sub-space's last reassignment
+    long long empty_reseeds, seeding_fallbacks;
+    double device_ms;
+};
+// init_codebooks == nullptr: compute (sample, optional centring, k-means++ seeding, Lloyd); otherwise refine from those host
+// codebooks, the training rows minus `centroid` (host, optional). Host outputs: codebooks_out [k * dim] (jv_dataset_register_pq
+// layout), centroid_out [dim] (compute with centring). Synchronises `s`.
+cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *init_codebooks, const float *centroid, float *codebooks_out,
+                     float *centroid_out, PqTrainStats *st, cudaStream_t s);
+
 }  // namespace jv
