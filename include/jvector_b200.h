@@ -424,6 +424,39 @@ JV_API int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_b
 JV_API int jv_builder_create_from_graph(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
                                         void *cuda_stream, jv_builder *out);
 
+/* ---- maintaining a graph over PQ codes (addGraphNode / removeDeletedNodes under BuildScoreProvider.pqBuildScoreProvider) ----
+ * The three calls below are jv_graph_add_nodes, jv_builder_create_from_graph and jv_graph_remove_deleted over a PQ data set, for
+ * an index whose fp32 rows do not fit in memory. Everything their contracts say that does not mention scores holds unchanged: the
+ * result is a NEW graph without FusedPQ records and the input is not modified; holes are carried (and widened by an add); the
+ * deleted_bits layout; n == n0 returns a copy; an add with no entry makes node n0 the entry; the level draws of new nodes and the
+ * extension of upper levels; how a removal picks its new entry, drops emptied levels, and answers searches when every node is gone;
+ * what jv_graph_build_stats and jv_remove_stats report.
+ * The scores are those of jv_graph_build_pq: the insert or repair of node v uses the query decode(c_v); keys are the ADC scores of
+ * the PQ walk under that query's LUT; pair similarities sum the metric's centroid-pair table (built and kept on the data set when
+ * it has none). An add into a one-node graph therefore gives the bytes of jv_graph_build_pq, and a node's row does not depend on
+ * whether the caller still held its fp32 vector when it was added.
+ * Rows [0, n0) of `pq` must be the graph's own nodes, encoded with the same codebooks (the calls cannot check it). A PQ data set
+ * does not grow in place: encode the new rows with jv_pq_encode_batch (nothing new is needed for that) and register the longer
+ * code array with jv_dataset_register_pq.
+ * The removal's prune runs at the smallest of 64 / 128 / 256 / 1024 / 2048 / 8192 candidate slots that holds a row's distinct
+ * candidates, and keeps the whole LUT of M * k floats in shared memory next to them (13 bytes per slot). A row gathers at most
+ * degree * (degree + 2) candidates, so a call needs the smallest capacity at or above that: 2048 slots up to degree 44, 8192
+ * above. When the LUT and that capacity do not fit in 226 KB together (e.g. degree 64 with M above ~118 at k = 256) the call is
+ * refused; no candidate set is ever clipped.
+ * Errors: JV_ERR_INVALID for a null argument, a data set that is not PQ, n < n0 (add) or n != g's size (remove), a device
+ * mismatch, a degree mismatch, a bad metric or alpha < 1; JV_ERR_UNSUPPORTED for a degree above 64, or a LUT the prune cannot hold
+ * at the capacity the call may need (add: the builder's 256 slots, as jv_graph_build_pq). Every check precedes the device work:
+ * a refused call has done none of it and leaves *out untouched. jv_graph_add_nodes, jv_builder_create_from_graph and
+ * jv_graph_remove_deleted keep answering JV_ERR_INVALID for a PQ data set. */
+JV_API int jv_graph_add_nodes_pq(jv_graph g, jv_dataset pq, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                 jv_graph *out, double *device_ms);
+/* the step-wise form, driven by the jv_builder_* calls like jv_builder_create_from_graph's builder */
+JV_API int jv_builder_create_from_graph_pq(jv_graph g, jv_dataset pq, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                           void *cuda_stream, jv_builder *out);
+JV_API int jv_graph_remove_deleted_pq(jv_graph g, jv_dataset pq, int metric, float alpha, uint64_t seed,
+                                      const uint32_t *deleted_bits /* host, bit (node & 31) of word (node >> 5) */,
+                                      jv_graph *out, jv_remove_stats *stats);
+
 /* device-memory helpers for callers that keep queries/results in HBM (bench `value` leg) */
 JV_API int jv_device_malloc(void **out, size_t bytes);
 JV_API int jv_device_free(void *p);

@@ -184,6 +184,14 @@ public:
         check(jv_graph_remove_deleted(graph.handle(), v.handle(), (int)vsf_, p_.alpha, p_.seed, deletedBits.data(), &g, &removeStats));
         return GraphIndex(g);
     }
+    /// removeDeletedNodes over the graph's PQ codes (jv_graph_remove_deleted_pq): the scores of build(const PQVectors &)
+    GraphIndex removeDeletedNodes(const GraphIndex &graph, const PQVectors &v, const std::vector<uint32_t> &deletedBits)
+    {
+        if ((int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "removeDeletedNodes: deletedBits shorter than the graph");
+        jv_graph g = nullptr;
+        check(jv_graph_remove_deleted_pq(graph.handle(), v.handle(), (int)vsf_, p_.alpha, p_.seed, deletedBits.data(), &g, &removeStats));
+        return GraphIndex(g);
+    }
     /// addGraphNode (GraphIndexBuilder.java:588-659) for nodes graph.size() .. v.size() - 1: a NEW graph (`graph` is left as it
     /// is); v's first rows must be graph's own nodes. deletedBits (optional, bit node & 31 of word node >> 5): marked nodes the new
     /// ones never pick as neighbours. The hierarchy follows graph's.
@@ -192,6 +200,14 @@ public:
         if (!deletedBits.empty() && (int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "addGraphNodes: deletedBits shorter than the graph");
         jv_graph g = nullptr;
         check(jv_graph_add_nodes(graph.handle(), v.handle(), (int)vsf_, &p_, deletedBits.empty() ? nullptr : deletedBits.data(), &g, &deviceMs));
+        return GraphIndex(g);
+    }
+    /// addGraphNodes over PQ codes (jv_graph_add_nodes_pq): v holds graph's nodes first, then the new rows' codes (same codebooks)
+    GraphIndex addGraphNodes(const GraphIndex &graph, const PQVectors &v, const std::vector<uint32_t> &deletedBits = {})
+    {
+        if (!deletedBits.empty() && (int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "addGraphNodes: deletedBits shorter than the graph");
+        jv_graph g = nullptr;
+        check(jv_graph_add_nodes_pq(graph.handle(), v.handle(), (int)vsf_, &p_, deletedBits.empty() ? nullptr : deletedBits.data(), &g, &deviceMs));
         return GraphIndex(g);
     }
     double deviceMs = 0;

@@ -458,7 +458,7 @@ def pack_accept_bits(mask):
 
 class GraphIndexBuilder:
     """base:graph/GraphIndexBuilder.java: (M, beamWidth, neighborOverflow, alpha, addHierarchy) over exact fp32 scores, or over PQ
-    codes (BuildScoreProvider.pqBuildScoreProvider) when build() is given PQVectors."""
+    codes (BuildScoreProvider.pqBuildScoreProvider) when build(), addGraphNodes() or removeDeletedNodes() is given PQVectors."""
 
     def __init__(self, vsf, M=32, beamWidth=100, neighborOverflow=1.2, alpha=1.2, addHierarchy=False, seed=0, max_batch=0, concurrent_window=-1):
         self.vsf = vsf
@@ -488,22 +488,29 @@ class GraphIndexBuilder:
         neighbours (random live members of its level, seeded by this builder's seed, when those offer none). The result carries
         `.remove_stats` (jv_remove_stats as a dict) and no FusedPQ records: call fuse_pq on it again if needed.
 
+        vectors: the graph's F32Vectors (exact scores, jv_graph_remove_deleted) or its PQVectors (jv_graph_remove_deleted_pq): the
+        repair of node v then scores with decode(c_v)'s ADC and the centroid-pair table, as build() over PQVectors does.
+
         Until this is called, a graph with marked nodes is searched with GraphSearcher.search(..., acceptOrds=~deleted): the marked
         nodes stay on the search paths but are never returned."""
         lib = nat.init()
         bits = _deleted_bits(deleted, graph.info()["n"])
         st = nat.RemoveStats()
         h = C.c_void_p()
-        check(lib.jv_graph_remove_deleted(graph._h, vectors._h, int(self.vsf), float(self.params.alpha), int(self.params.seed),
-                                          bits.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(h), C.byref(st)))
+        fn = lib.jv_graph_remove_deleted_pq if isinstance(vectors, PQVectors) else lib.jv_graph_remove_deleted
+        check(fn(graph._h, vectors._h, int(self.vsf), float(self.params.alpha), int(self.params.seed),
+                 bits.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(h), C.byref(st)))
         out = GraphIndex(_handle=h)
         out.remove_stats = {name: getattr(st, name) for name, _ in nat.RemoveStats._fields_}
         return out
 
     def addGraphNodes(self, graph, vectors, deleted=None):
-        """GraphIndexBuilder.addGraphNode for every node graph.size() .. vectors.size() - 1, on the device (jv_graph_add_nodes).
+        """GraphIndexBuilder.addGraphNode for every node graph.size() .. vectors.size() - 1, on the device (jv_graph_add_nodes, or
+        jv_graph_add_nodes_pq for PQVectors).
 
-        vectors: F32Vectors whose first rows are the graph's own nodes, followed by the new ones. Returns a NEW GraphIndex (`graph`
+        vectors: F32Vectors or PQVectors whose first rows are the graph's own nodes, followed by the new ones. A PQ data set grows
+        by encoding the new rows with the same codebooks (ProductQuantization.encodeAll) and wrapping the longer code array in new
+        PQVectors; the insert of node v then uses decode(c_v) as its query, as build() over PQVectors does. Returns a NEW GraphIndex (`graph`
         is left as it is), built from the graph's rows with this builder's parameters (M must equal the graph's degree); its holes
         stay holes, the hierarchy follows the graph's (addHierarchy is ignored) and it has no FusedPQ records. deleted: nodes marked
         deleted but not removed yet (a bool mask over the graph's nodes or an array of their ids): the new nodes never pick them as
@@ -512,8 +519,9 @@ class GraphIndexBuilder:
         bits = _deleted_bits(deleted, graph.info()["n"]) if deleted is not None else None
         h = C.c_void_p()
         ms = C.c_double()
-        check(lib.jv_graph_add_nodes(graph._h, vectors._h, int(self.vsf), C.byref(self.params),
-                                     bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None, C.byref(h), C.byref(ms)))
+        fn = lib.jv_graph_add_nodes_pq if isinstance(vectors, PQVectors) else lib.jv_graph_add_nodes
+        check(fn(graph._h, vectors._h, int(self.vsf), C.byref(self.params),
+                 bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None, C.byref(h), C.byref(ms)))
         self.device_ms = ms.value
         s, b, d = C.c_int64(), C.c_int64(), C.c_int64()
         lib.jv_graph_build_stats(C.byref(s), C.byref(b), C.byref(d))

@@ -1552,18 +1552,24 @@ static std::vector<uint32_t> add_accept_bits(const GraphAdd &A, const int32_t *i
     return bits;
 }
 
-static int add_check(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, BuildParams *bp)
+// the checks of an add over a data set of `kind` (KIND_F32: jv_graph_add_nodes, KIND_PQ: jv_graph_add_nodes_pq). Over PQ also those
+// of the PQ build: a LUT the prune can hold, and the metric's centroid-pair table, built and kept on the data set when it has none
+static int add_check(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, BuildParams *bp)
 {
-    if (!f32 || !params) return fail(JV_ERR_INVALID, "add_nodes: null argument");
-    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "add_nodes: needs an fp32 data set");
-    if (f32->device != g->device) return fail(JV_ERR_INVALID, "add_nodes: data set and graph live on different devices");
-    if (f32->d.n < g->g.n || f32->d.n > INT32_MAX) return fail(JV_ERR_INVALID, "add_nodes: the data set must hold the graph's nodes first");
-    int rc = check_metric(f32->d, metric);
+    if (!ds || !params) return fail(JV_ERR_INVALID, "add_nodes: null argument");
+    if (ds->d.kind != kind) return fail(JV_ERR_INVALID, kind == KIND_PQ ? "add_nodes_pq: needs a PQ data set" : "add_nodes: needs an fp32 data set");
+    if (ds->device != g->device) return fail(JV_ERR_INVALID, "add_nodes: data set and graph live on different devices");
+    if (ds->d.n < g->g.n || ds->d.n > INT32_MAX) return fail(JV_ERR_INVALID, "add_nodes: the data set must hold the graph's nodes first");
+    int rc = check_metric(ds->d, metric);
     if (rc) return rc;
     if (g->g.degree > 64)
         return fail(JV_ERR_UNSUPPORTED, "add_nodes: degree " + std::to_string(g->g.degree) + " > 64, the largest row the builder handles");
     if (params->degree != g->g.degree) return fail(JV_ERR_INVALID, "add_nodes: params->degree differs from the graph's degree");
-    return build_params_check(params, bp);
+    if ((rc = build_params_check(params, bp)) || kind != KIND_PQ) return rc;
+    if (!pq_prune_fits(ds->d))
+        return fail(JV_ERR_UNSUPPORTED, "add_nodes_pq: a LUT of M * k = " + std::to_string(ds->d.M * ds->d.k) +
+                                            " entries does not fit the prune's shared memory next to its candidates (DESIGN §4.3c)");
+    return jv_dataset_pq_pair_table(ds, metric);
 }
 
 // g's state into A and the seed of a level-0 builder over n rows (accept: the storage of its bits). Enqueues a copy of g's
@@ -1592,9 +1598,10 @@ static int add_prepare(jv_graph g, const uint32_t *deleted_bits, int n, GraphAdd
 // old members in the level's order, then the new members ascending; the old rows are mapped to local rows through g's upper_row on
 // the device; the inserts start at the entry's row (the level's first row if the entry is not a member). A level above g's top is
 // built over its members, all new, and its lowest id becomes the entry.
-static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+// Over a PQ data set build_level gathers the members' code rows instead of their fp32 rows; nothing else differs.
+static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
 {
-    const int n = (int)f32->d.n, n0 = A.n0, degree = bp.degree, L = (int)A.level_ids.size();
+    const int n = (int)ds->d.n, n0 = A.n0, degree = bp.degree, L = (int)A.level_ids.size();
     const std::vector<int> level = draw_levels(n, degree, seed);
     int top = L;
     for (int i = n0; i < n; i++) top = std::max(top, level[i]);
@@ -1606,7 +1613,7 @@ static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, i
         std::vector<int32_t> ladj;
         int rc = JV_OK;
         if (l > L) {
-            rc = build_level(f32, metric, bp, ids, nullptr, ladj, s);
+            rc = build_level(ds, metric, bp, ids, nullptr, ladj, s);
         } else if ((int)ids.size() == nold) {
             ladj = A.level_adj[l - 1];
         } else {
@@ -1619,7 +1626,7 @@ static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, i
             const std::vector<uint32_t> accept = add_accept_bits(A, ids.data(), nold, (int)ids.size());
             const BuilderSeed sd = {rows.get<int32_t>(), nold, degree, A.upper_row.get<int32_t>() + (size_t)(l - 1) * n0, at < nold ? at : 0,
                                     accept.empty() ? nullptr : accept.data()};
-            rc = build_level(f32, metric, bp, ids, &sd, ladj, s);
+            rc = build_level(ds, metric, bp, ids, &sd, ladj, s);
         }
         if (rc) return rc;
         ng->level_ids.push_back(std::move(ids));
@@ -1630,9 +1637,9 @@ static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, i
 }
 
 // the new graph around its level-0 adjacency (already in ng->adj0): size, entry, holes widened to n, upper levels
-static int add_finish(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+static int add_finish(jv_graph_s *ng, const GraphAdd &A, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
 {
-    const int n = (int)f32->d.n;
+    const int n = (int)ds->d.n;
     ng->g.n = n; ng->g.degree = bp.degree; ng->g.levels = 1; ng->g.entry_level = 0; ng->g.adj0 = ng->adj0.get<int32_t>();
     ng->g.entry_node = A.entry >= 0 ? A.entry : n > A.n0 ? A.n0 : -1;  // an empty graph's first new node is its entry (build.cu)
     if (!A.removed.empty()) {
@@ -1640,23 +1647,24 @@ static int add_finish(jv_graph_s *ng, const GraphAdd &A, jv_dataset f32, int met
         ng->removed.resize(((size_t)n + 31) / 32, 0u);
     }
     if (!A.level_ids.empty()) {
-        const int rc = add_upper_levels(ng, A, f32, metric, bp, seed, s);
+        const int rc = add_upper_levels(ng, A, ds, metric, bp, seed, s);
         if (rc) return rc;
     }
     return graph_rebuild_upper(ng);
 }
 
-int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
-                       double *device_ms)
+// jv_graph_add_nodes (kind = KIND_F32) and jv_graph_add_nodes_pq (KIND_PQ): the builder scores whatever kind of rows it is given
+static int graph_add_nodes(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
+                           double *device_ms)
 {
     ON_DEVICE_OF(g);
     if (!out) return fail(JV_ERR_INVALID, "add_nodes: null argument");
     BuildParams bp;
-    int rc = add_check(g, f32, metric, params, &bp);
+    int rc = add_check(g, ds, kind, metric, params, &bp);
     if (rc) return rc;
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
-    const int n0 = g->g.n, n = (int)f32->d.n, degree = g->g.degree;
+    const int n0 = g->g.n, n = (int)ds->d.n, degree = g->g.degree;
     std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
     ng->device = g->device;
     memset(&ng->g, 0, sizeof(GraphDesc));
@@ -1677,10 +1685,10 @@ int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_pa
         BuilderSeed seed;
         rc = add_prepare(g, deleted_bits, n, A, accept, &seed, s);
         if (!rc) {
-            const cudaError_t e = build_graph_flat(f32->d, metric, bp, ng->adj0.get<int32_t>(), g_sm_count, &bs, s, &seed);
+            const cudaError_t e = build_graph_flat(ds->d, metric, bp, ng->adj0.get<int32_t>(), g_sm_count, &bs, s, &seed);
             rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_add_nodes");
         }
-        if (!rc) rc = add_finish(ng.get(), A, f32, metric, bp, params->seed, s);
+        if (!rc) rc = add_finish(ng.get(), A, ds, metric, bp, params->seed, s);
     }
     t_build_stats = bs;
     const cudaError_t e1 = timer.stop(s);
@@ -1690,6 +1698,18 @@ int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_pa
     if (device_ms) *device_ms = timer.ms();
     *out = ng.release();
     return JV_OK;
+}
+
+int jv_graph_add_nodes(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
+                       double *device_ms)
+{
+    return graph_add_nodes(g, f32, KIND_F32, metric, params, deleted_bits, out, device_ms);
+}
+
+int jv_graph_add_nodes_pq(jv_graph g, jv_dataset pq, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
+                          double *device_ms)
+{
+    return graph_add_nodes(g, pq, KIND_PQ, metric, params, deleted_bits, out, device_ms);
 }
 
 // ---- the same build advanced batch by batch, for a build SHARDED over several GPUs (BASELINE config 5) ----------------------
@@ -1739,25 +1759,37 @@ int jv_builder_create_pq(jv_dataset pq, int metric, const jv_build_params *param
     return JV_OK;
 }
 
-int jv_builder_create_from_graph(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
-                                 void *cuda_stream, jv_builder *out)
+static int builder_from_graph(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                              void *cuda_stream, jv_builder *out)
 {
     ON_DEVICE_OF(g);
     if (!out) return fail(JV_ERR_INVALID, "builder_create_from_graph: null argument");
     BuildParams bp;
-    int rc = add_check(g, f32, metric, params, &bp);
+    int rc = add_check(g, ds, kind, metric, params, &bp);
     if (rc) return rc;
     std::unique_ptr<jv_builder_s> b(new jv_builder_s());
-    b->device = g->device; b->data = f32; b->metric = metric; b->params = *params; b->bp = bp; b->stream = (cudaStream_t)cuda_stream;
+    b->device = g->device; b->data = ds; b->metric = metric; b->params = *params; b->bp = bp; b->stream = (cudaStream_t)cuda_stream;
     b->add.reset(new GraphAdd());
     CK(b->timer.start(b->stream), "event");
     std::vector<uint32_t> accept;
     BuilderSeed seed;
-    if ((rc = add_prepare(g, deleted_bits, (int)f32->d.n, *b->add, accept, &seed, b->stream))) return rc;
-    CK(builder_create(f32->d, metric, bp, g_sm_count, &b->B, b->stream, &seed), "builder_create");
+    if ((rc = add_prepare(g, deleted_bits, (int)ds->d.n, *b->add, accept, &seed, b->stream))) return rc;
+    CK(builder_create(ds->d, metric, bp, g_sm_count, &b->B, b->stream, &seed), "builder_create");
     CK(cudaStreamSynchronize(b->stream), "builder_create_from_graph");  // g has been read: the caller may free it
     *out = b.release();
     return JV_OK;
+}
+
+int jv_builder_create_from_graph(jv_graph g, jv_dataset f32, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                 void *cuda_stream, jv_builder *out)
+{
+    return builder_from_graph(g, f32, KIND_F32, metric, params, deleted_bits, cuda_stream, out);
+}
+
+int jv_builder_create_from_graph_pq(jv_graph g, jv_dataset pq, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                    void *cuda_stream, jv_builder *out)
+{
+    return builder_from_graph(g, pq, KIND_PQ, metric, params, deleted_bits, cuda_stream, out);
 }
 
 int jv_builder_info(jv_builder b, int *degree, int *row_cap, int *max_batch)
@@ -1884,7 +1916,7 @@ int jv_graph_build_stats(int64_t *scored_vectors, int64_t *batches, int64_t *dro
 // ------------------------------------------------------------------------------------------------ removeDeletedNodes
 
 // one level of the repair on the device (repair_level, build.cu); level L >= 1 also hands back its repaired rows
-static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset f32, int metric, float alpha, uint64_t seed, int level, const std::vector<uint32_t> &dead,
+static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset ds, int metric, float alpha, uint64_t seed, int level, const std::vector<uint32_t> &dead,
                                 const uint32_t *dead_dev, RepairStats *st, std::vector<int32_t> *adj_out, cudaStream_t s)
 {
     const int n = g->g.n, degree = g->g.degree;
@@ -1916,7 +1948,7 @@ static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset f32, int met
     }
     const int32_t *rowmap = level ? g->upper_row.get<int32_t>() + (size_t)(level - 1) * n : nullptr;
     if (e == cudaSuccess)
-        e = repair_level(f32->d, metric, alpha, degree, rows, dold, dnew, dids.get<int32_t>(), rowmap, dead_dev, dmem.get<int32_t>(), (int)members.size(), seed,
+        e = repair_level(ds->d, metric, alpha, degree, rows, dold, dnew, dids.get<int32_t>(), rowmap, dead_dev, dmem.get<int32_t>(), (int)members.size(), seed,
                          level, g_sm_count, st, s);
     if (e == cudaSuccess && level == 0) e = launch_clear_dead_rows(dnew, n, degree, dead_dev, s);
     if (e == cudaSuccess && level > 0) {
@@ -1928,18 +1960,27 @@ static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset f32, int met
     return e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted");
 }
 
-int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
-                            jv_remove_stats *stats)
+// jv_graph_remove_deleted (kind = KIND_F32) and jv_graph_remove_deleted_pq (KIND_PQ): repair_level dispatches its prune by kind.
+// Every check comes before any device work, so a refused call has done none of it.
+static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
+                                jv_remove_stats *stats)
 {
     ON_DEVICE_OF(g);
-    if (!f32 || !deleted_bits || !out || !stats) return fail(JV_ERR_INVALID, "graph_remove_deleted: null argument");
-    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "graph_remove_deleted: needs the graph's fp32 data set");
-    if (f32->d.n != g->g.n || f32->device != g->device) return fail(JV_ERR_INVALID, "graph_remove_deleted: data set and graph differ in size or device");
+    if (!ds || !deleted_bits || !out || !stats) return fail(JV_ERR_INVALID, "graph_remove_deleted: null argument");
+    if (ds->d.kind != kind)
+        return fail(JV_ERR_INVALID, kind == KIND_PQ ? "graph_remove_deleted_pq: needs the graph's PQ data set" : "graph_remove_deleted: needs the graph's fp32 data set");
+    if (ds->d.n != g->g.n || ds->device != g->device) return fail(JV_ERR_INVALID, "graph_remove_deleted: data set and graph differ in size or device");
     if (!(alpha >= 1.0f)) return fail(JV_ERR_INVALID, "graph_remove_deleted: need alpha >= 1");
-    int rc = check_metric(f32->d, metric);
+    int rc = check_metric(ds->d, metric);
     if (rc) return rc;
     if (g->g.degree > 64)
         return fail(JV_ERR_UNSUPPORTED, "graph_remove_deleted: degree " + std::to_string(g->g.degree) + " > 64, the largest row the prune kernels handle");
+    if (kind == KIND_PQ) {
+        if (!pq_repair_fits(ds->d, g->g.degree))
+            return fail(JV_ERR_UNSUPPORTED, "graph_remove_deleted_pq: a LUT of M * k = " + std::to_string(ds->d.M * ds->d.k) + " entries does not fit the prune's shared memory next to the " +
+                                                std::to_string(g->g.degree * (g->g.degree + 2)) + " candidates a row of this degree can gather (DESIGN §4.3e)");
+        if ((rc = jv_dataset_pq_pair_table(ds, metric))) return rc;
+    }
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
     const int n = g->g.n, degree = g->g.degree;
@@ -1970,11 +2011,11 @@ int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha,
     rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted: allocation");
     ng->g.adj0 = ng->adj0.get<int32_t>();
     const uint32_t *dead_dev = dead_buf.get<uint32_t>();
-    if (!rc) rc = remove_deleted_level(g, ng.get(), f32, metric, alpha, seed, 0, dead, dead_dev, &st, nullptr, s);
+    if (!rc) rc = remove_deleted_level(g, ng.get(), ds, metric, alpha, seed, 0, dead, dead_dev, &st, nullptr, s);
     // upper levels: repaired on the device like level 0, then their deleted members are dropped from the host copies
     for (int level = 1; !rc && level < g->g.levels; level++) {
         std::vector<int32_t> adj;
-        rc = remove_deleted_level(g, ng.get(), f32, metric, alpha, seed, level, dead, dead_dev, &st, &adj, s);
+        rc = remove_deleted_level(g, ng.get(), ds, metric, alpha, seed, level, dead, dead_dev, &st, &adj, s);
         if (rc) break;
         const std::vector<int32_t> &ids = g->level_ids[level - 1];
         std::vector<int32_t> nids, nadj;
@@ -2016,6 +2057,18 @@ int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha,
     stats->device_ms = timer.ms();
     *out = ng.release();
     return JV_OK;
+}
+
+int jv_graph_remove_deleted(jv_graph g, jv_dataset f32, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
+                            jv_remove_stats *stats)
+{
+    return graph_remove_deleted(g, f32, KIND_F32, metric, alpha, seed, deleted_bits, out, stats);
+}
+
+int jv_graph_remove_deleted_pq(jv_graph g, jv_dataset pq, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
+                               jv_remove_stats *stats)
+{
+    return graph_remove_deleted(g, pq, KIND_PQ, metric, alpha, seed, deleted_bits, out, stats);
 }
 
 // ------------------------------------------------------------------------------------------------ query batches (host-driven seam)

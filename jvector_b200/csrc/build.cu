@@ -138,9 +138,13 @@ __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const f
 // larger capacities so that no candidate set is ever clipped.
 // KIND_PQ (pqBuildScoreProvider, §4.3c): v's query is decode(c_v) (pq_decode_row, into the row slot), its LUT is prepare_blob's, the
 // keys are score_pq's bits — the walk's — and the fold sums the centroid-pair table (pair_pq_table, ImmutablePQVectors' diversity).
+// The PQ capacities above PRUNE_MAXC (the repair's upper tiers, §4.3e) work on the power of two that holds the row's own candidates
+// instead of on MAXC — the key pass, the sort and the state reset shrink with it; a sort of KEY_MIN pads changes no result — and
+// write the selected row with one thread per neighbour.
 template <int METRIC, int MAXC = PRUNE_MAXC, int KIND = KIND_F32>
 __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
 {
+    constexpr bool BOUNDED = KIND == KIND_PQ && MAXC > PRUNE_MAXC;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     // f32: blob stride + 4, newrow stride (the most recently selected row). PQ: blob = the LUT, newrow = decode(c_v) (dim rounded to 4)
     const int blob_fl = KIND == KIND_PQ ? blob_floats(P.d) : P.d.stride + 4;
@@ -179,12 +183,15 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             ncs = nc = min(P.deg[v], P.row_cap);
         }
         nc = min(nc, MAXC);
+        int cap = MAXC;
+        if (BOUNDED)
+            for (cap = PRUNE_MAXC; cap < nc;) cap <<= 1;
         if (KIND == KIND_PQ) {
             pq_decode_row(P.d, v, newrow, tid, PRUNE_THREADS);
             __syncthreads();
             prepare_blob(P.d, P.metric, newrow, blob, red);
             // the candidates' ADC scores under v's LUT as sortable keys: 8 lanes per candidate, the walk's scorer and bits
-            for (int i = tid >> 3; i < MAXC; i += PRUNE_THREADS / 8) {
+            for (int i = tid >> 3; i < cap; i += PRUNE_THREADS / 8) {
                 const int32_t c = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1;
                 long long kc = KEY_MIN;
                 if (c >= 0 && c != v) kc = topk_key(score_pq<METRIC>(P.d, blob, c, lane & 7), c);
@@ -211,11 +218,11 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             }
         }
         __syncthreads();
-        bitonic_sort_desc(keys, MAXC);
+        bitonic_sort_desc(keys, cap);
         // valid keys form a prefix (KEY_MIN sorts last); duplicates are adjacent after the sort and are dropped
         int nvalid;
         {
-            int lo = 0, hi = MAXC;
+            int lo = 0, hi = cap;
             while (lo < hi) {
                 const int mid = (lo + hi) >> 1;
                 if (keys[mid] != KEY_MIN) lo = mid + 1;
@@ -223,7 +230,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             }
             nvalid = lo;
         }
-        for (int i = tid; i < MAXC; i += PRUNE_THREADS) {
+        for (int i = tid; i < cap; i += PRUNE_THREADS) {
             maxsim[i] = -3.0e38f;
             state[i] = (i < nvalid && !(i > 0 && keys[i - 1] == keys[i])) ? 0 : 2;
         }
@@ -244,7 +251,11 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
                 if (pick == INT_MAX) break;
                 const int32_t c = key_node(keys[pick]);
                 const float4 *crow = reinterpret_cast<const float4 *>(P.d.rows + (size_t)c * P.d.stride);
-                if (tid == 0) { state[pick] = 1; sel_ids[nsel] = c; }
+                if (tid == 0) {
+                    state[pick] = 1;
+                    sel_ids[nsel] = c;
+                    if (BOUNDED) sel_ids[64 + nsel] = pick;  // degree <= 64: the second half holds the picks' sorted positions
+                }
                 if (KIND != KIND_PQ)
                     for (int t = tid; t < n4; t += PRUNE_THREADS) reinterpret_cast<float4 *>(newrow)[t] = __ldg(crow + t);
                 nsel++;
@@ -273,7 +284,27 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
         }
         // the selected neighbours, in score order (NodeArray.retain keeps the sorted order)
         __syncthreads();
-        if (tid == 0) {
+        if (BOUNDED) {
+            // thread t places pick t at its rank among the picks' sorted positions instead of one thread scanning nvalid states
+            const int oi = P.mode == 2 ? a : P.out_base + it;
+            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
+            const int width = P.out_rows ? P.out_stride : P.row_cap;
+            for (int t = tid; t < width; t += PRUNE_THREADS) {
+                if (t < nsel) {
+                    int rank = 0;
+                    for (int j = 0; j < nsel; j++) rank += sel_ids[64 + j] < sel_ids[64 + t];
+                    row[rank] = sel_ids[t];
+                } else {
+                    row[t] = -1;
+                }
+            }
+            if (tid == 0) {
+                if (P.out_rows) P.out_deg[oi] = nsel;
+                else P.deg[v] = nsel;
+                if (P.mode == 1 && P.mark) P.mark[v] = 0;
+            }
+        }
+        if (!BOUNDED && tid == 0) {
             int w = 0;
             const int oi = P.mode == 2 ? a : P.out_base + it;
             int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
@@ -1075,8 +1106,8 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
 {
     const int n = (int)d.n;
     if ((d.kind != KIND_F32 && d.kind != KIND_PQ) || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
-    // PQ: a fresh build only, with the centroid-pair table of this metric (jv_dataset_pq_pair_table) and a LUT the prune can hold
-    if (d.kind == KIND_PQ && (seed || !d.pair_table[metric == JV_METRIC_EUCLIDEAN ? 0 : 1] || !pq_prune_fits(d))) return cudaErrorInvalidValue;
+    // PQ: with the centroid-pair table of this metric (jv_dataset_pq_pair_table) and a LUT the prune can hold
+    if (d.kind == KIND_PQ && (!d.pair_table[metric == JV_METRIC_EUCLIDEAN ? 0 : 1] || !pq_prune_fits(d))) return cudaErrorInvalidValue;
     if (seed && (seed->count < 0 || seed->count > n || (seed->count > 0 && (!seed->rows_dev || seed->width < 1)) || seed->entry >= seed->count))
         return cudaErrorInvalidValue;
     std::unique_ptr<GraphBuilder> B(new GraphBuilder());
@@ -1332,7 +1363,8 @@ cudaError_t build_graph_flat(const DataDesc &d, int metric, const BuildParams &b
 //   count  : one warp per row flags the live rows that name a deleted node and sizes their candidate segment
 //   gather : one CTA per flagged row writes its live neighbours, the live 2-hop ids through its deleted neighbours (the FreshDiskANN
 //            rule, :705-721) — or, when there are no such ids, random live members of the level (:743-759) — sorted and deduplicated
-//   prune  : the builder's prune kernels (mode 2, ragged candidates, out of place), dispatched by candidate count so no set is clipped
+//   prune  : the builder's prune kernels (mode 2, ragged candidates, out of place), dispatched by candidate count so no set is clipped;
+//            over a PQ data set the PQ prune at every tier, with the scores of the PQ build (query decode(c_v), ADC keys, pair table)
 //   scatter: the pruned rows replace the old ones in the output adjacency
 // Nothing depends on timing: compaction and offsets come from cub scans, the dedup from a sort, and the prune is deterministic.
 // ------------------------------------------------------------------------------------------------
@@ -1490,6 +1522,21 @@ cudaError_t launch_clear_dead_rows(int32_t *adj_dev, int n, int degree, const ui
 // the prune tiers of the repair: TILE-candidate Gram kernels on the tensor cores, then the incremental kernel at growing capacity
 constexpr int REPAIR_TIERS = 5;
 constexpr int REPAIR_TIER_MAX[REPAIR_TIERS] = {64, 128, 256, 1024, 8192};
+// over a PQ data set (§4.3e) there is no Gram tier — it would change the pair bits — and every tier is prune_kernel<.., KIND_PQ>. The
+// candidate state (13 B per slot) shares the CTA's shared memory with the whole LUT, so 2048 sits between 1024 and 8192: a degree-32
+// row has at most 32 * 34 = 1088 candidates and never pays for 8192 slots (106 KB)
+constexpr int PQ_REPAIR_TIERS = 6;
+constexpr int PQ_REPAIR_TIER_MAX[PQ_REPAIR_TIERS] = {64, 128, 256, 1024, 2048, 8192};
+static_assert(PQ_REPAIR_TIERS <= (int)(sizeof(RepairStats::tier_rows) / sizeof(long long)), "RepairStats::tier_rows holds every tier");
+
+// whether the repair of a degree-`degree` graph over `pq` can run: a row gathers up to degree * (degree + 2) candidates, and the tier
+// that holds them must fit next to the LUT
+bool pq_repair_fits(const DataDesc &pq, int degree)
+{
+    int t = 0;
+    while (t < PQ_REPAIR_TIERS - 1 && degree * (degree + 2) > PQ_REPAIR_TIER_MAX[t]) t++;
+    return prune_pq_smem_bytes(pq, PQ_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
+}
 
 template <int METRIC>
 static cudaError_t launch_repair_prune_t(const PruneParams &P, int tier, int grid, cudaStream_t s)
@@ -1501,12 +1548,23 @@ static cudaError_t launch_repair_prune_t(const PruneParams &P, int tier, int gri
         if ((e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_)) != cudaSuccess) return e; \
         KERNEL<<<grid, PRUNE_THREADS, sm_, s>>>(P);                                                                     \
     } while (0)
-    switch (tier) {
-    case 0: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 64>), gram_tc_smem_bytes<64>(P.d)); break;
-    case 1: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 128>), gram_tc_smem_bytes<128>(P.d)); break;
-    case 2: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 256>), prune_smem_bytes(P.d, 256)); break;
-    case 3: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 1024>), prune_smem_bytes(P.d, 1024)); break;
-    default: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 8192>), prune_smem_bytes(P.d, 8192)); break;
+    if (P.d.kind == KIND_PQ) {
+        switch (tier) {
+        case 0: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 64, KIND_PQ>), prune_pq_smem_bytes(P.d, 64)); break;
+        case 1: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 128, KIND_PQ>), prune_pq_smem_bytes(P.d, 128)); break;
+        case 2: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 256, KIND_PQ>), prune_pq_smem_bytes(P.d, 256)); break;
+        case 3: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 1024, KIND_PQ>), prune_pq_smem_bytes(P.d, 1024)); break;
+        case 4: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 2048, KIND_PQ>), prune_pq_smem_bytes(P.d, 2048)); break;
+        default: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 8192, KIND_PQ>), prune_pq_smem_bytes(P.d, 8192)); break;
+        }
+    } else {
+        switch (tier) {
+        case 0: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 64>), gram_tc_smem_bytes<64>(P.d)); break;
+        case 1: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 128>), gram_tc_smem_bytes<128>(P.d)); break;
+        case 2: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 256>), prune_smem_bytes(P.d, 256)); break;
+        case 3: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 1024>), prune_smem_bytes(P.d, 1024)); break;
+        default: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 8192>), prune_smem_bytes(P.d, 8192)); break;
+        }
     }
 #undef JV_PRUNE_LAUNCH
     g_launches++;
@@ -1585,10 +1643,12 @@ static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alp
     JV_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)naff * 4, cudaMemcpyDeviceToHost, s));
     JV_TRY(cudaMemcpyAsync(hfb.data(), fallback, (size_t)naff, cudaMemcpyDeviceToHost, s));
     JV_TRY(cudaStreamSynchronize(s));
-    std::vector<int32_t> tiers[REPAIR_TIERS];
+    const int ntiers = d.kind == KIND_PQ ? PQ_REPAIR_TIERS : REPAIR_TIERS;
+    const int *tier_max = d.kind == KIND_PQ ? PQ_REPAIR_TIER_MAX : REPAIR_TIER_MAX;
+    std::vector<int32_t> tiers[PQ_REPAIR_TIERS];
     for (int a = 0; a < naff; a++) {
         int t = 0;
-        while (t < REPAIR_TIERS - 1 && hcnt[a] > REPAIR_TIER_MAX[t]) t++;
+        while (t < ntiers - 1 && hcnt[a] > tier_max[t]) t++;
         tiers[t].push_back(a);
         st->candidates += hcnt[a];
         st->max_candidates = std::max(st->max_candidates, hcnt[a]);
@@ -1597,7 +1657,7 @@ static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alp
     }
     st->repaired_rows += naff;
     std::vector<int32_t> hlist;
-    for (int t = 0; t < REPAIR_TIERS; t++) hlist.insert(hlist.end(), tiers[t].begin(), tiers[t].end());
+    for (int t = 0; t < ntiers; t++) hlist.insert(hlist.end(), tiers[t].begin(), tiers[t].end());
     JV_TRY(cudaMemcpyAsync(tier_list, hlist.data(), (size_t)naff * 4, cudaMemcpyHostToDevice, s));
     {
         PruneParams P;
@@ -1606,7 +1666,7 @@ static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alp
         P.cand = cand; P.row_node = row_node; P.cand_off = cand_off; P.cand_cnt = cand_cnt;
         P.out_rows = out_rows; P.out_deg = out_deg; P.out_stride = degree;
         int first = 0;
-        for (int t = 0; t < REPAIR_TIERS; t++) {
+        for (int t = 0; t < ntiers; t++) {
             const int c = (int)tiers[t].size();
             if (c == 0) continue;
             P.list = tier_list + first;
@@ -1625,7 +1685,8 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
                          int sm_count, RepairStats *st, cudaStream_t s)
 {
     if (rows <= 0) return cudaSuccess;
-    if (degree < 1 || degree > 64) return cudaErrorInvalidValue;
+    if (degree < 1 || degree > 64 || (d.kind != KIND_F32 && d.kind != KIND_PQ)) return cudaErrorInvalidValue;
+    if (d.kind == KIND_PQ && (!d.pair_table[metric == JV_METRIC_EUCLIDEAN ? 0 : 1] || !pq_repair_fits(d, degree))) return cudaErrorInvalidValue;
     std::vector<DeviceBuffer> mem;  // the scratch goes when this returns: the stream drains first, on success and on error
     const cudaError_t err = repair_level_enqueue(d, metric, alpha, degree, rows, adj_old, adj_new, ids_dev, rowmap_dev, dead_dev, members_dev, nmembers,
                                                  seed, level, sm_count, st, mem, s);
