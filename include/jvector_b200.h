@@ -247,6 +247,38 @@ JV_API int jv_pq_train(jv_dataset f32, const jv_pq_train_params *p, float *codeb
 JV_API int jv_pq_refine(jv_dataset f32, const jv_pq_train_params *p, const float *codebooks, const float *centroid /* or NULL */,
                         float *codebooks_out, jv_pq_train_stats *stats /* may be NULL */);
 
+/* ---- PQ with an anisotropic threshold T (ProductQuantization with anisotropicThreshold > UNWEIGHTED = -1), on the device ----
+ * Training: jv_pq_train's steps, then KMeansPlusPlusClusterer's anisotropic rounds per sub-space: centroids from a per-cluster
+ * d_s x d_s Gauss-Jordan solve in the reference's order (the outer-product sums are int64 fixed point, independent of thread order),
+ * rows reassigned by the weighted parallel / perpendicular loss, the same 1 % early stop, pcm from T and the sub-space's size.
+ * compute runs lloyd_iterations Lloyd rounds and then lloyd_iterations anisotropic rounds; refine runs lloyd_iterations anisotropic
+ * rounds only, from the unweighted nearest-centroid assignment. Encoding: the reference's coordinate descent over sub-spaces
+ * (at most 10 sweeps, pcm from T and dim), one row at a time, for every row ever encoded with such a PQ.
+ * T == -1 gives exactly the bytes and counters of jv_pq_train / jv_pq_refine / jv_pq_encode_*. Errors, all before any device work,
+ * leaving the outputs untouched: JV_ERR_INVALID for T NaN, below -1 or at least 1, and whatever the unweighted call rejects;
+ * JV_ERR_UNSUPPORTED from the training calls when T > -1 and a sub-space is wider than 64 floats (ceil(dim / M) > 64).
+ * Anisotropic codebooks and codes register with jv_dataset_register_pq like any others: search, build, add and remove are unchanged. */
+typedef struct {
+    jv_pq_train_stats lloyd;          /* the unweighted phase, as jv_pq_train reports it; lloyd.device_ms covers the whole call */
+    int32_t max_anisotropic_updates;  /* anisotropic rounds of the sub-space that ran longest */
+    int64_t changed_last_anisotropic; /* summed over sub-spaces: rows moved by each one's last anisotropic reassignment */
+    int64_t anisotropic_reseeds;      /* empty clusters reseeded to a random training row in the anisotropic rounds */
+} jv_pq_anisotropic_stats;
+JV_API int jv_pq_train_anisotropic(jv_dataset f32, const jv_pq_train_params *p, float anisotropic_threshold,
+                                   float *codebooks_out, float *centroid_out, jv_pq_anisotropic_stats *stats /* may be NULL */);
+JV_API int jv_pq_refine_anisotropic(jv_dataset f32, const jv_pq_train_params *p, float anisotropic_threshold, const float *codebooks,
+                                    const float *centroid /* or NULL */, float *codebooks_out, jv_pq_anisotropic_stats *stats /* may be NULL */);
+typedef struct {
+    int64_t rows_moved; /* rows whose code left its minimum-residual start */
+    int64_t moves;      /* coordinate-descent moves in all */
+    int32_t max_sweeps; /* sweeps of the row that ran longest (0 when T == -1) */
+    double device_ms;   /* the call's work on the device stream, copies included */
+} jv_pq_encode_stats;
+JV_API int jv_pq_encode_batch_anisotropic(const float *rows, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid,
+                                          float anisotropic_threshold, uint8_t *codes_out, jv_pq_encode_stats *stats /* may be NULL */);
+JV_API int jv_pq_encode_dataset_anisotropic(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid,
+                                            float anisotropic_threshold, uint8_t *codes_out, jv_pq_encode_stats *stats /* may be NULL */);
+
 /* ---- graph: ImmutableGraphIndex adjacency in HBM + GraphSearcher traversal on the device ---- */
 /* adj0: [n][degree] int32, -1 padded (level 0). */
 JV_API int jv_graph_create(int32_t n, int degree, const int32_t *adj0, int32_t entry_node, jv_graph *out);

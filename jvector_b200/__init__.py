@@ -13,9 +13,9 @@ mirror of the reference's interface for that path, used by the tests and the ben
 from . import api
 from .api import (BQVectors, F32Vectors, GraphIndex, GraphIndexBuilder, GraphSearcher, NVQVectors, PQVectors, ProductQuantization, QueryBatch,
                   ScoreFunction, SearchResult, VectorSimilarityFunction, bq_encode_all, kmeans_assign, nvq_encode_all, nvq_encode_resident,
-                  pack_accept_bits, pq_encode_all, score_multi, topk_bruteforce)
+                  pack_accept_bits, pq_encode_all, pq_encode_all_anisotropic, score_multi, topk_bruteforce)
 from ._native import JVectorB200Error, init, load
 
 __all__ = ["VectorSimilarityFunction", "F32Vectors", "PQVectors", "BQVectors", "NVQVectors", "ProductQuantization", "ScoreFunction", "GraphIndex",
            "GraphSearcher", "GraphIndexBuilder", "SearchResult", "score_multi", "topk_bruteforce", "bq_encode_all",
-           "pq_encode_all", "nvq_encode_all", "nvq_encode_resident", "QueryBatch", "kmeans_assign", "pack_accept_bits", "JVectorB200Error", "init", "load"]
+           "pq_encode_all", "pq_encode_all_anisotropic", "nvq_encode_all", "nvq_encode_resident", "QueryBatch", "kmeans_assign", "pack_accept_bits", "JVectorB200Error", "init", "load"]

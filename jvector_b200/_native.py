@@ -51,6 +51,15 @@ class PQTrainStats(C.Structure):
                 ("seeding_fallbacks", C.c_int64), ("device_ms", C.c_double)]
 
 
+class PQAnisotropicStats(C.Structure):
+    _fields_ = [("lloyd", PQTrainStats), ("max_anisotropic_updates", C.c_int32), ("changed_last_anisotropic", C.c_int64),
+                ("anisotropic_reseeds", C.c_int64)]
+
+
+class PQEncodeStats(C.Structure):
+    _fields_ = [("rows_moved", C.c_int64), ("moves", C.c_int64), ("max_sweeps", C.c_int32), ("device_ms", C.c_double)]
+
+
 # every symbol include/jvector_b200.h declares: (name, restype, argtypes)
 _F, _I, _Z, _P, _L = C.c_float, C.c_int, C.c_size_t, C.c_void_p, C.c_int64
 SYMBOLS = [
@@ -102,6 +111,10 @@ SYMBOLS = [
     ("jv_nvq_encode_dataset_resident", _I, [_P, _I, f32p, _I, C.POINTER(_P)]),
     ("jv_pq_train", _I, [_P, C.POINTER(PQTrainParams), f32p, f32p, C.POINTER(PQTrainStats)]),
     ("jv_pq_refine", _I, [_P, C.POINTER(PQTrainParams), f32p, f32p, f32p, C.POINTER(PQTrainStats)]),
+    ("jv_pq_train_anisotropic", _I, [_P, C.POINTER(PQTrainParams), _F, f32p, f32p, C.POINTER(PQAnisotropicStats)]),
+    ("jv_pq_refine_anisotropic", _I, [_P, C.POINTER(PQTrainParams), _F, f32p, f32p, f32p, C.POINTER(PQAnisotropicStats)]),
+    ("jv_pq_encode_batch_anisotropic", _I, [f32p, _L, _I, _I, _I, f32p, f32p, _F, u8p, C.POINTER(PQEncodeStats)]),
+    ("jv_pq_encode_dataset_anisotropic", _I, [_P, _I, _I, f32p, f32p, _F, u8p, C.POINTER(PQEncodeStats)]),
     ("jv_graph_create", _I, [C.c_int32, _I, i32p, C.c_int32, C.POINTER(_P)]), ("jv_graph_add_level", _I, [_P, C.c_int32, i32p, i32p]),
     ("jv_graph_fuse_pq", _I, [_P, _P]), ("jv_graph_fused_download", _I, [_P, u8p, C.POINTER(_I)]),
     ("jv_graph_free", _I, [_P]), ("jv_graph_info", _I, [_P, i32p, C.POINTER(_I), C.POINTER(_I), i32p]),

@@ -111,44 +111,68 @@ class PQVectors(_Vectors):
 
 
 class ProductQuantization:
-    """base:quantization/ProductQuantization.java with isotropic (UNWEIGHTED) loss, trained on the device (jv_pq_train /
-    jv_pq_refine). codebooks: float32 [k * dim] (codebook m = [k][size_m] at k * offset_m); centroid: the global centroid or None."""
+    """base:quantization/ProductQuantization.java, trained on the device (jv_pq_train / jv_pq_refine, or their _anisotropic forms
+    when anisotropicThreshold > UNWEIGHTED). codebooks: float32 [k * dim] (codebook m = [k][size_m] at k * offset_m); centroid: the
+    global centroid or None; anisotropicThreshold: the T the codebooks were trained or refined with, which encodeAll also uses."""
 
     K_MEANS_ITERATIONS = 6
+    UNWEIGHTED = -1.0
 
-    def __init__(self, codebooks, M, k, dim, centroid=None, stats=None):
+    def __init__(self, codebooks, M, k, dim, centroid=None, stats=None, anisotropicThreshold=UNWEIGHTED):
         self.codebooks, self.M, self.k, self.dim, self.centroid, self.stats = codebooks, M, k, dim, centroid, stats
+        self.anisotropicThreshold = float(anisotropicThreshold)
 
     @staticmethod
     def _stats(st):
         return {name: getattr(st, name) for name, _ in nat.PQTrainStats._fields_}
 
     @classmethod
-    def compute(cls, vectors, M, clusterCount=256, globallyCenter=False, seed=0):
+    def _astats(cls, st):
+        out = cls._stats(st.lloyd)
+        out.update({name: getattr(st, name) for name, _ in nat.PQAnisotropicStats._fields_[1:]})
+        return out
+
+    @classmethod
+    def compute(cls, vectors, M, clusterCount=256, globallyCenter=False, seed=0, anisotropicThreshold=UNWEIGHTED):
         """ProductQuantization.compute over F32Vectors resident in HBM: at most 128 000 sampled training rows, k-means++ seeding,
-        K_MEANS_ITERATIONS Lloyd iterations with the reference's early stop. The result is a pure function of the rows and seed."""
+        K_MEANS_ITERATIONS Lloyd iterations with the reference's early stop, then (anisotropicThreshold > UNWEIGHTED) as many
+        anisotropic rounds. The result is a pure function of the rows, the seed and the threshold."""
         lib = nat.init()
         dim = vectors.dimension()
         p = nat.PQTrainParams(M, clusterCount, 1 if globallyCenter else 0, cls.K_MEANS_ITERATIONS, 0, seed)
         cb = np.empty(clusterCount * dim, np.float32)
         cen = np.empty(dim, np.float32) if globallyCenter else None
-        st = nat.PQTrainStats()
-        check(lib.jv_pq_train(vectors._h, C.byref(p), fp(cb), fp(cen), C.byref(st)))
-        return cls(cb, M, clusterCount, dim, cen, cls._stats(st))
+        if anisotropicThreshold == cls.UNWEIGHTED:
+            st = nat.PQTrainStats()
+            check(lib.jv_pq_train(vectors._h, C.byref(p), fp(cb), fp(cen), C.byref(st)))
+            return cls(cb, M, clusterCount, dim, cen, cls._stats(st))
+        st = nat.PQAnisotropicStats()
+        check(lib.jv_pq_train_anisotropic(vectors._h, C.byref(p), anisotropicThreshold, fp(cb), fp(cen), C.byref(st)))
+        return cls(cb, M, clusterCount, dim, cen, cls._astats(st), anisotropicThreshold)
 
-    def refine(self, vectors, lloydsRounds=1, seed=0):
-        """ProductQuantization.refine: lloydsRounds Lloyd iterations from these codebooks over `vectors` (minus the centroid);
-        returns a new ProductQuantization with the same centroid."""
+    def refine(self, vectors, lloydsRounds=1, seed=0, anisotropicThreshold=UNWEIGHTED):
+        """ProductQuantization.refine: lloydsRounds Lloyd iterations (anisotropic rounds when anisotropicThreshold > UNWEIGHTED)
+        from these codebooks over `vectors` (minus the centroid); returns a new ProductQuantization with the same centroid and
+        the threshold it was refined with."""
         lib = nat.init()
         p = nat.PQTrainParams(self.M, self.k, 0, lloydsRounds, 0, seed)
         cb = np.empty_like(self.codebooks)
-        st = nat.PQTrainStats()
-        check(lib.jv_pq_refine(vectors._h, C.byref(p), fp(self.codebooks), fp(self.centroid), fp(cb), C.byref(st)))
-        return ProductQuantization(cb, self.M, self.k, self.dim, self.centroid, self._stats(st))
+        if anisotropicThreshold == self.UNWEIGHTED:
+            st = nat.PQTrainStats()
+            check(lib.jv_pq_refine(vectors._h, C.byref(p), fp(self.codebooks), fp(self.centroid), fp(cb), C.byref(st)))
+            return ProductQuantization(cb, self.M, self.k, self.dim, self.centroid, self._stats(st))
+        st = nat.PQAnisotropicStats()
+        check(lib.jv_pq_refine_anisotropic(vectors._h, C.byref(p), anisotropicThreshold, fp(self.codebooks), fp(self.centroid), fp(cb),
+                                           C.byref(st)))
+        return ProductQuantization(cb, self.M, self.k, self.dim, self.centroid, self._astats(st), anisotropicThreshold)
 
     def encodeAll(self, vectors):
-        """ProductQuantization.encodeAll of resident F32Vectors into resident PQVectors"""
-        codes = pq_encode_all(vectors, self.codebooks, self.M, self.k, self.centroid)
+        """ProductQuantization.encodeAll of resident F32Vectors into resident PQVectors (the anisotropic encoder when the
+        threshold is above UNWEIGHTED)"""
+        if self.anisotropicThreshold > self.UNWEIGHTED:
+            codes = pq_encode_all_anisotropic(vectors, self.codebooks, self.M, self.k, self.centroid, self.anisotropicThreshold)[0]
+        else:
+            codes = pq_encode_all(vectors, self.codebooks, self.M, self.k, self.centroid)
         return PQVectors(codes, self.codebooks, self.dim, self.k, self.centroid)
 
 
@@ -319,6 +343,24 @@ def pq_encode_all(rows, codebooks, M, k=256, centroid=None):
     out = np.empty((rows.shape[0], M), dtype=np.uint8)
     check(lib.jv_pq_encode_batch(fp(rows), rows.shape[0], rows.shape[1], M, k, fp(codebooks), fp(cen), bp(out)))
     return out
+
+
+def pq_encode_all_anisotropic(rows, codebooks, M, k, centroid, anisotropicThreshold):
+    """ProductQuantization.encodeAll with an anisotropic threshold (encodeAnisotropic for T > -1). rows: a host array, or
+    F32Vectors resident in HBM. Returns (codes [n][M] uint8, stats dict: rows_moved, moves, max_sweeps, device_ms)."""
+    lib = nat.init()
+    codebooks = c32(codebooks).reshape(-1)
+    cen = c32(centroid) if centroid is not None else None
+    st = nat.PQEncodeStats()
+    if isinstance(rows, _Vectors):
+        out = np.empty((rows.size(), M), dtype=np.uint8)
+        check(lib.jv_pq_encode_dataset_anisotropic(rows._h, M, k, fp(codebooks), fp(cen), anisotropicThreshold, bp(out), C.byref(st)))
+    else:
+        rows = c32(rows)
+        out = np.empty((rows.shape[0], M), dtype=np.uint8)
+        check(lib.jv_pq_encode_batch_anisotropic(fp(rows), rows.shape[0], rows.shape[1], M, k, fp(codebooks), fp(cen), anisotropicThreshold,
+                                                 bp(out), C.byref(st)))
+    return out, {name: getattr(st, name) for name, _ in nat.PQEncodeStats._fields_}
 
 
 def nvq_encode_all(rows, mean, nsub, learn=True):

@@ -803,17 +803,26 @@ int jv_bq_encode_dataset(jv_dataset f32, uint64_t *words_out)
     return bq_encode_impl(nullptr, f32->d.rows, f32->d.stride, f32->d.n, f32->d.dim, words_out);
 }
 
+// ProductQuantization.anisotropicThreshold: UNWEIGHTED (-1) <= T < 1, not NaN (KMeansPlusPlusClusterer.java:86-92)
+static bool bad_threshold(float t) { return !(t >= -1.f && t < 1.f); }
+
+// threshold > -1: the anisotropic encoder (ProductQuantization.encodeAnisotropic); stats (optional) also times the stream's work
 static int pq_encode_impl(const float *rows, const float *rows_dev, int row_stride, int64_t n, int dim, int M, int k, const float *codebooks,
-                          const float *centroid, uint8_t *codes_out)
+                          const float *centroid, uint8_t *codes_out, float threshold = -1.f, jv_pq_encode_stats *stats = nullptr)
 {
     int rc;
+    const bool aniso = threshold > -1.f;
     float *dcb, *dcen;
     int *dlay;
+    unsigned long long *dstats;
+    void *dscratch;
     auto carve = [&](void *base) {
         Carver c(base);
         dcb = c.take<float>((size_t)k * dim);
         dcen = c.take<float>(dim);
         dlay = c.take<int>(2 * (size_t)M);
+        dstats = c.take<unsigned long long>(aniso ? 3 : 0);
+        dscratch = c.take<char>(aniso ? pq_encode_aniso_scratch(dim, M, k) : 0);
         return c.bytes;
     };
     if ((rc = t_ctx.init()) || (rows && (rc = grow(t_ctx.input, (size_t)n * dim * 4))) || (rc = grow(t_ctx.output, (size_t)n * M)) ||
@@ -821,6 +830,8 @@ static int pq_encode_impl(const float *rows, const float *rows_dev, int row_stri
         return rc;
     carve(t_ctx.aux.get());
     cudaStream_t s = t_ctx.stream;
+    StreamTimer timer;
+    if (stats) CK(timer.start(s), "timer");
     if (rows) {
         CK(cudaMemcpyAsync(t_ctx.input.get(), rows, (size_t)n * dim * 4, cudaMemcpyHostToDevice, s), "H2D rows");
         rows_dev = t_ctx.input.get<float>();
@@ -832,32 +843,72 @@ static int pq_encode_impl(const float *rows, const float *rows_dev, int row_stri
     DataDesc d;
     memset(&d, 0, sizeof(d));
     d.kind = KIND_PQ; d.dim = dim; d.n = n; d.M = M; d.k = k; d.codebooks = dcb; d.sub_sizes = dlay; d.sub_offsets = dlay + M; d.centroid = centroid ? dcen : nullptr;
-    CK(launch_pq_encode(d, rows_dev, n, row_stride, t_ctx.output.get<uint8_t>(), s), "pq_encode");
+    if (aniso)
+        CK(launch_pq_encode_aniso(d, rows_dev, n, row_stride, pq_parallel_cost_multiplier(threshold, dim), dscratch, dstats, t_ctx.output.get<uint8_t>(), s),
+           "pq_encode_aniso");
+    else
+        CK(launch_pq_encode(d, rows_dev, n, row_stride, t_ctx.output.get<uint8_t>(), s), "pq_encode");
     CK(cudaMemcpyAsync(codes_out, t_ctx.output.get(), (size_t)n * M, cudaMemcpyDeviceToHost, s), "D2H codes");
+    unsigned long long counters[3] = {0, 0, 0};
+    if (stats && aniso) CK(cudaMemcpyAsync(counters, dstats, sizeof(counters), cudaMemcpyDeviceToHost, s), "D2H stats");
+    if (stats) CK(timer.stop(s), "timer");
     CK(cudaStreamSynchronize(s), "sync");
+    if (stats) {
+        stats->rows_moved = (int64_t)counters[0];
+        stats->moves = (int64_t)counters[1];
+        stats->max_sweeps = (int32_t)counters[2];
+        stats->device_ms = timer.ms();
+    }
     return JV_OK;
 }
 
-int jv_pq_encode_batch(const float *rows, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid, uint8_t *codes_out)
+static int pq_encode_batch_entry(const float *rows, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid, uint8_t *codes_out,
+                                 float threshold, jv_pq_encode_stats *stats)
 {
     NEED_INIT();
     if (!rows || !codebooks || !codes_out || n <= 0 || dim <= 0 || M <= 0 || M > dim || k <= 0 || k > 256) return fail(JV_ERR_INVALID, "pq_encode: bad arguments");
-    return pq_encode_impl(rows, nullptr, 0, n, dim, M, k, codebooks, centroid, codes_out);
+    if (bad_threshold(threshold)) return fail(JV_ERR_INVALID, "pq_encode: anisotropic threshold outside [-1, 1)");
+    return pq_encode_impl(rows, nullptr, 0, n, dim, M, k, codebooks, centroid, codes_out, threshold, stats);
 }
 
-int jv_pq_encode_dataset(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, uint8_t *codes_out)
+static int pq_encode_dataset_entry(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, uint8_t *codes_out, float threshold,
+                                   jv_pq_encode_stats *stats)
 {
     ON_DEVICE_OF(f32);
     if (!f32 || f32->d.kind != KIND_F32 || !codebooks || !codes_out || M <= 0 || M > f32->d.dim || k <= 0 || k > 256)
         return fail(JV_ERR_INVALID, "pq_encode_dataset: bad arguments");
-    return pq_encode_impl(nullptr, f32->d.rows, f32->d.stride, f32->d.n, f32->d.dim, M, k, codebooks, centroid, codes_out);
+    if (bad_threshold(threshold)) return fail(JV_ERR_INVALID, "pq_encode_dataset: anisotropic threshold outside [-1, 1)");
+    return pq_encode_impl(nullptr, f32->d.rows, f32->d.stride, f32->d.n, f32->d.dim, M, k, codebooks, centroid, codes_out, threshold, stats);
+}
+
+int jv_pq_encode_batch(const float *rows, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid, uint8_t *codes_out)
+{
+    return pq_encode_batch_entry(rows, n, dim, M, k, codebooks, centroid, codes_out, -1.f, nullptr);
+}
+
+int jv_pq_encode_dataset(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, uint8_t *codes_out)
+{
+    return pq_encode_dataset_entry(f32, M, k, codebooks, centroid, codes_out, -1.f, nullptr);
+}
+
+int jv_pq_encode_batch_anisotropic(const float *rows, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid,
+                                   float anisotropic_threshold, uint8_t *codes_out, jv_pq_encode_stats *stats)
+{
+    return pq_encode_batch_entry(rows, n, dim, M, k, codebooks, centroid, codes_out, anisotropic_threshold, stats);
+}
+
+int jv_pq_encode_dataset_anisotropic(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, float anisotropic_threshold,
+                                     uint8_t *codes_out, jv_pq_encode_stats *stats)
+{
+    return pq_encode_dataset_entry(f32, M, k, codebooks, centroid, codes_out, anisotropic_threshold, stats);
 }
 
 // ------------------------------------------------------------------------------------------------ PQ training
 constexpr int64_t MAX_PQ_TRAINING_SET_SIZE = 128000;  // ProductQuantization.java:64
 
+// threshold > -1 adds the anisotropic rounds: lloyd_iterations of them after compute's Lloyd, or in place of refine's
 static int pq_train_impl(jv_dataset f32, const jv_pq_train_params *p, const float *codebooks, const float *centroid, float *codebooks_out,
-                         float *centroid_out, jv_pq_train_stats *stats)
+                         float *centroid_out, jv_pq_train_stats *stats, float threshold = -1.f, jv_pq_anisotropic_stats *astats = nullptr)
 {
     if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "pq_train: needs an fp32 data set");
     if (!p || !codebooks_out) return fail(JV_ERR_INVALID, "pq_train: null argument");
@@ -866,9 +917,12 @@ static int pq_train_impl(jv_dataset f32, const jv_pq_train_params *p, const floa
     if (p->lloyd_iterations < 0 || p->max_train_rows < 0) return fail(JV_ERR_INVALID, "pq_train: negative iteration count or row cap");
     const int64_t cap = p->max_train_rows ? p->max_train_rows : MAX_PQ_TRAINING_SET_SIZE;
     if (std::min<int64_t>(f32->d.n, cap) < p->k) return fail(JV_ERR_INVALID, "pq_train: fewer training rows than clusters");
+    const bool aniso = threshold > -1.f;
+    if (aniso && (f32->d.dim + p->M - 1) / p->M > 64) return fail(JV_ERR_UNSUPPORTED, "pq_train: anisotropic sub-spaces above 64 floats");
     int rc;
     if ((rc = t_ctx.init())) return rc;
-    const PqTrainArgs a = {p->M, p->k, p->globally_center, p->lloyd_iterations, (long long)cap, p->seed};
+    const int lloyd = aniso && codebooks ? 0 : p->lloyd_iterations;  // refine: anisotropic rounds only (ProductQuantization.refine)
+    const PqTrainArgs a = {p->M, p->k, p->globally_center, lloyd, (long long)cap, p->seed, aniso ? p->lloyd_iterations : 0, threshold};
     PqTrainStats st;
     CK(pq_train(f32->d, a, codebooks, centroid, codebooks_out, centroid_out, &st, t_ctx.stream), "pq_train");
     if (stats) {
@@ -878,6 +932,11 @@ static int pq_train_impl(jv_dataset f32, const jv_pq_train_params *p, const floa
         stats->empty_reseeds = st.empty_reseeds;
         stats->seeding_fallbacks = st.seeding_fallbacks;
         stats->device_ms = st.device_ms;
+    }
+    if (astats) {
+        astats->max_anisotropic_updates = st.aniso_updates;
+        astats->changed_last_anisotropic = st.aniso_changed_last;
+        astats->anisotropic_reseeds = st.aniso_reseeds;
     }
     return JV_OK;
 }
@@ -894,6 +953,44 @@ int jv_pq_refine(jv_dataset f32, const jv_pq_train_params *p, const float *codeb
     ON_DEVICE_OF(f32);
     if (!codebooks) return fail(JV_ERR_INVALID, "pq_refine: null codebooks");
     return pq_train_impl(f32, p, codebooks, centroid, codebooks_out, nullptr, stats);
+}
+
+static void unweighted_stats(jv_pq_anisotropic_stats *stats, const jv_pq_train_stats &st)
+{
+    stats->lloyd = st;
+    stats->max_anisotropic_updates = 0;
+    stats->changed_last_anisotropic = 0;
+    stats->anisotropic_reseeds = 0;
+}
+
+int jv_pq_train_anisotropic(jv_dataset f32, const jv_pq_train_params *p, float anisotropic_threshold, float *codebooks_out, float *centroid_out,
+                            jv_pq_anisotropic_stats *stats)
+{
+    ON_DEVICE_OF(f32);
+    if (bad_threshold(anisotropic_threshold)) return fail(JV_ERR_INVALID, "pq_train: anisotropic threshold outside [-1, 1)");
+    jv_pq_train_stats st;
+    if (anisotropic_threshold == -1.f) {
+        const int rc = jv_pq_train(f32, p, codebooks_out, centroid_out, stats ? &st : nullptr);
+        if (rc == JV_OK && stats) unweighted_stats(stats, st);
+        return rc;
+    }
+    if (p && p->globally_center && !centroid_out) return fail(JV_ERR_INVALID, "pq_train: globally_center needs centroid_out");
+    return pq_train_impl(f32, p, nullptr, nullptr, codebooks_out, centroid_out, stats ? &stats->lloyd : nullptr, anisotropic_threshold, stats);
+}
+
+int jv_pq_refine_anisotropic(jv_dataset f32, const jv_pq_train_params *p, float anisotropic_threshold, const float *codebooks, const float *centroid,
+                             float *codebooks_out, jv_pq_anisotropic_stats *stats)
+{
+    ON_DEVICE_OF(f32);
+    if (bad_threshold(anisotropic_threshold)) return fail(JV_ERR_INVALID, "pq_refine: anisotropic threshold outside [-1, 1)");
+    jv_pq_train_stats st;
+    if (anisotropic_threshold == -1.f) {
+        const int rc = jv_pq_refine(f32, p, codebooks, centroid, codebooks_out, stats ? &st : nullptr);
+        if (rc == JV_OK && stats) unweighted_stats(stats, st);
+        return rc;
+    }
+    if (!codebooks) return fail(JV_ERR_INVALID, "pq_refine: null codebooks");
+    return pq_train_impl(f32, p, codebooks, centroid, codebooks_out, nullptr, stats ? &stats->lloyd : nullptr, anisotropic_threshold, stats);
 }
 
 static int nvq_encode_impl(const float *rows, const float *rows_dev, int row_stride, int64_t n, int dim, int nsub, const float *mean, int learn,

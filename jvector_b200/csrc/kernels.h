@@ -1,5 +1,6 @@
 // kernels.h — host-callable launchers of the sm_90a kernels (internal; the public surface is include/jvector_b200.h)
 #pragma once
+#include <algorithm>
 #include <atomic>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -217,18 +218,39 @@ struct PqTrainArgs {
     int iters;            // Lloyd iterations (>= 0)
     long long cap;        // training rows at most (> 0)
     uint64_t seed;
+    int aniso_iters;      // anisotropic rounds after Lloyd (0: none, UNWEIGHTED)
+    float threshold;      // the anisotropic threshold T, -1 < T < 1 (aniso_iters > 0 only); sub-spaces of at most 64 floats
 };
 struct PqTrainStats {
     long long train_rows;
     int max_lloyd_updates;  // centroid updates of the sub-space that ran longest
     long long changed_last;  // summed over sub-spaces: rows that moved in the sub-space's last reassignment
     long long empty_reseeds, seeding_fallbacks;
+    int aniso_updates;  // the same three for the anisotropic rounds
+    long long aniso_changed_last, aniso_reseeds;
     double device_ms;
 };
+// KMeansPlusPlusClusterer.computeParallelCostMultiplier (base:quantization/KMeansPlusPlusClusterer.java:116-124), in double
+inline float pq_parallel_cost_multiplier(double threshold, int dimensions)
+{
+    const double par = threshold * threshold, perp = (1 - par) / (dimensions - 1);
+    return (float)std::max(1.0, par / perp);
+}
 // init_codebooks == nullptr: compute (sample, optional centring, k-means++ seeding, Lloyd); otherwise refine from those host
 // codebooks, the training rows minus `centroid` (host, optional). Host outputs: codebooks_out [k * dim] (jv_dataset_register_pq
 // layout), centroid_out [dim] (compute with centring). Synchronises `s`.
 cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *init_codebooks, const float *centroid, float *codebooks_out,
                      float *centroid_out, PqTrainStats *st, cudaStream_t s);
 
+// ---- pq_encode_aniso.cu: ProductQuantization.encodeAnisotropic ----
+struct PqEncodeStats {
+    long long rows_moved, moves;  // rows whose code left its minimum-residual start; coordinate-descent moves in all
+    int max_sweeps;               // sweeps of the row that ran longest (the last one changes nothing, or it is the 10th)
+};
+// pq: KIND_PQ descriptor with device codebooks, layout and optional centroid (its n is unused); rows_dev [n] rows of row_stride
+// floats; pcm = pq_parallel_cost_multiplier(T, dim). scratch: pq_encode_aniso_scratch(dim, M, k) bytes. codes_dev [n][M].
+// Does not synchronise; stats_dev: 3 uint64 counters, zeroed by the call.
+size_t pq_encode_aniso_scratch(int dim, int M, int k);
+cudaError_t launch_pq_encode_aniso(const DataDesc &pq, const float *rows_dev, long long n, int row_stride, float pcm, void *scratch,
+                                   unsigned long long *stats_dev, uint8_t *codes_dev, cudaStream_t s);
 }  // namespace jv

@@ -10,6 +10,11 @@
 //   4. Lloyd    KMeansPlusPlusClusterer.cluster(iterations, 0): initial assignment; then per iteration centroid update (fixed-point
 //               sums per (sub-space, cluster), empty clusters reseeded), reassignment, and a sub-space stops once
 //               changed <= 0.01 n_train.
+//   5. anisotropic (T > UNWEIGHTED only) KMeansPlusPlusClusterer.cluster(.., anisotropicIterations), from the assignment step 4
+//               left: per round, for every active sub-space, the fixed-point means and counts of step 4, int64 fixed-point sums of
+//               fl(fl(x_a x_b) * fl(1 / |x|^2)) per (cluster, a <= b), one Gauss-Jordan solve per (sub-space, cluster) in the
+//               reference's order (Matrix.invert, then the row-wise product with the mean), then the weighted reassignment;
+//               a sub-space stops once changed <= 0.01 n_train. pcm uses the sub-space's own size, as the reference does.
 #include <algorithm>
 #include <unordered_set>
 #include <vector>
@@ -21,6 +26,10 @@ namespace jv {
 namespace {
 
 constexpr int TAG_RESEED = 0x40000000;  // first counter of the empty-cluster reseed draws: sub-space | TAG_RESEED
+constexpr int TAG_ARESEED = 0x20000000; // the same for the anisotropic rounds: sub-space | TAG_ARESEED never equals a Lloyd,
+                                        // seeding (sub-space < 2^29) or sampling counter
+constexpr int ANISO_MAX_SUB = 64;       // largest sub-space the anisotropic solve holds in shared memory (N x 2N floats)
+constexpr int PAIR_TILE = 512;          // (a, b) pairs per outer-product block at most
 constexpr int TAG_SAMPLE = 0x7fffffff;  // first counter of Floyd's draws
 constexpr int SAMPLE_ROWS = 256;        // training rows per block of the gather / column passes
 constexpr int TILE_FLOATS = 12288;      // centroid floats per shared-memory tile of the assignment (48 KB)
@@ -307,6 +316,215 @@ __global__ void pq_train_finalize_kernel(const float *__restrict__ train, long l
     } else cent[q] = from_fixed(sums[q], fixed_exp(colmax[off + t], nt), cnt);
 }
 
+// step 5: |x|^2 of every (sub-space = grid.y, training row), accumulated in order, and fl(1 / |x|^2) where |x|^2 > 0 (else 0)
+__global__ void __launch_bounds__(256) pq_train_norm_kernel(const float *__restrict__ train, long long nt, int dim, int M, float *__restrict__ xn,
+                                                            float *__restrict__ rinv)
+{
+    const int m = blockIdx.y;
+    int sz, off;
+    sub_layout(dim, M, m, sz, off);
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nt) return;
+    const float *x = train + (size_t)nt * off + (size_t)j * sz;
+    float s = 0.f;
+    for (int t = 0; t < sz; t++) s = __fadd_rn(s, __fmul_rn(x[t], x[t]));
+    xn[(size_t)m * nt + j] = s;
+    rinv[(size_t)m * nt + j] = s > 0.f ? __fdiv_rn(1.f, s) : 0.f;
+}
+
+// the upper-triangle pair index of (a, b), a <= b < n, rows in order
+__device__ __forceinline__ int pair_index(int a, int b, int n) { return a * n - a * (a - 1) / 2 + (b - a); }
+
+// step 5, outer-product sums: int64 fixed point of fl(fl(x_a x_b) * rinv) for the pairs [p0, p0 + ptile) of sub-space grid.z, summed
+// per cluster over UPDATE_ROWS rows (grid.x) in shared memory, then added to osum [M][k][npair_max]. |term| < 2, so one exponent
+// (fixed_exp of 1.0f) serves every term; rows with |x|^2 = 0 add nothing (KMeansPlusPlusClusterer skips them).
+__global__ void __launch_bounds__(256) pq_train_outer_kernel(const float *__restrict__ train, long long nt, int dim, int M, int k, int ptile, int npmax,
+                                                             const int32_t *__restrict__ assign, const int *__restrict__ active,
+                                                             const float *__restrict__ rinv, long long *__restrict__ osum)
+{
+    __shared__ long long s_sum[SUM_TILE];
+    __shared__ unsigned char s_a[PAIR_TILE], s_b[PAIR_TILE];
+    const int m = blockIdx.z;
+    if (!active[m]) return;
+    int sz, off;
+    sub_layout(dim, M, m, sz, off);
+    const int np = sz * (sz + 1) / 2, p0 = blockIdx.y * ptile;
+    if (p0 >= np) return;
+    const int pl = min(ptile, np - p0);
+    for (int q = threadIdx.x; q < k * pl; q += blockDim.x) s_sum[q] = 0;
+    for (int p = threadIdx.x; p < pl; p += blockDim.x) {
+        int a = 0, r = p0 + p;
+        while (r >= sz - a) { r -= sz - a; a++; }
+        s_a[p] = (unsigned char)a;
+        s_b[p] = (unsigned char)(a + r);
+    }
+    __syncthreads();
+    const int e = fixed_exp(0x3f800000u, nt);
+    const long long i0 = (long long)blockIdx.x * UPDATE_ROWS, i1 = min(nt, i0 + UPDATE_ROWS);
+    const int32_t *as = assign + (size_t)m * nt;
+    const float *ri = rinv + (size_t)m * nt;
+    const float *x = train + (size_t)nt * off;
+    for (long long q = threadIdx.x; q < (i1 - i0) * pl; q += blockDim.x) {
+        const long long i = i0 + q / pl;
+        const int p = (int)(q % pl);
+        const float r = ri[i];
+        if (r == 0.f) continue;
+        const float *xi = x + (size_t)i * sz;
+        const float term = __fmul_rn(__fmul_rn(xi[s_a[p]], xi[s_b[p]]), r);
+        atomicAdd((unsigned long long *)&s_sum[as[i] * pl + p], (unsigned long long)to_fixed(term, e));
+    }
+    __syncthreads();
+    for (int q = threadIdx.x; q < k * pl; q += blockDim.x) {
+        const long long v = s_sum[q];
+        if (v) atomicAdd((unsigned long long *)&osum[((size_t)m * k + q / pl) * npmax + p0 + q % pl], (unsigned long long)v);
+    }
+}
+
+// step 5, the new centroid of (cluster = grid.x, sub-space = grid.y) (KMeansPlusPlusClusterer.updateCentroidsAnisotropic):
+//   A = fl(S * fl(fl(1 - ocm) / |L|)) (+ ocm on the diagonal), S the outer-product sums, ocm = fl(1 / pcm);
+//   c = invert(A) * mean, Matrix.invert's Gauss-Jordan (largest |pivot|, the first row on a tie; the pivot row times fl(1 / pivot);
+//   every other row plus fl(-factor * pivot row)), then row-wise dot products accumulated in order. Every element sees the same
+//   sequence of roundings whichever thread applies it. Columns left of the pivot are never read again and are not updated.
+//   An empty cluster takes training row counter_random(seed, m | TAG_ARESEED, round, cluster) % n_train.
+__global__ void __launch_bounds__(256) pq_train_solve_kernel(const float *__restrict__ train, long long nt, int dim, int M, int k, int npmax,
+                                                             const int *__restrict__ active, const long long *__restrict__ sums,
+                                                             const int *__restrict__ counts, const unsigned *__restrict__ colmax,
+                                                             const long long *__restrict__ osum, float pcm_big, float pcm_small, uint64_t seed, int round,
+                                                             float *__restrict__ cent, unsigned long long *__restrict__ reseeds)
+{
+    __shared__ float a[ANISO_MAX_SUB * 2 * ANISO_MAX_SUB];
+    __shared__ float mean[ANISO_MAX_SUB], fac[ANISO_MAX_SUB];
+    __shared__ int s_piv;
+    const int c = blockIdx.x, m = blockIdx.y;
+    if (!active[m]) return;
+    int N, off;
+    sub_layout(dim, M, m, N, off);
+    const int W = 2 * N;
+    float *dst = cent + (size_t)k * off + (size_t)c * N;
+    const int cnt = counts[(size_t)m * k + c];
+    if (cnt == 0) {
+        const long long r = (long long)(counter_random(seed, m | TAG_ARESEED, round, c) % (uint64_t)nt);
+        for (int t = threadIdx.x; t < N; t += blockDim.x) dst[t] = train[(size_t)nt * off + (size_t)r * N + t];
+        if (threadIdx.x == 0) atomicAdd(reseeds, 1ull);
+        return;
+    }
+    const float pcm = m < dim % M ? pcm_big : pcm_small;
+    const float ocm = __fdiv_rn(1.f, pcm);
+    const float scale = __fdiv_rn(__fsub_rn(1.f, ocm), (float)cnt);
+    const int eo = fixed_exp(0x3f800000u, nt);
+    const long long *os = osum + ((size_t)m * k + c) * npmax;
+    for (int t = threadIdx.x; t < N; t += blockDim.x) mean[t] = from_fixed(sums[(size_t)k * off + (size_t)c * N + t], fixed_exp(colmax[off + t], nt), cnt);
+    for (int q = threadIdx.x; q < N * N; q += blockDim.x) {
+        const int i = q / N, j = q - i * N;
+        const float S = __double2float_rn(__dmul_rn(__ll2double_rn(os[pair_index(min(i, j), max(i, j), N)]), pow2(-eo)));
+        float v = __fmul_rn(S, scale);
+        if (i == j) v = __fadd_rn(v, ocm);
+        a[i * W + j] = v;
+        a[i * W + N + j] = i == j ? 1.f : 0.f;
+    }
+    __syncthreads();
+    for (int i = 0; i < N; i++) {
+        if (threadIdx.x == 0) {
+            int mr = i;
+            for (int r = i + 1; r < N; r++)
+                if (fabsf(a[r * W + i]) > fabsf(a[mr * W + i])) mr = r;
+            s_piv = mr;
+        }
+        __syncthreads();
+        const int mr = s_piv;
+        if (mr != i)
+            for (int j = i + threadIdx.x; j < W; j += blockDim.x) {
+                const float t = a[i * W + j];
+                a[i * W + j] = a[mr * W + j];
+                a[mr * W + j] = t;
+            }
+        __syncthreads();
+        const float rp = __fdiv_rn(1.f, a[i * W + i]);
+        for (int r = threadIdx.x; r < N; r += blockDim.x) fac[r] = a[r * W + i];
+        __syncthreads();
+        for (int j = i + 1 + threadIdx.x; j < W; j += blockDim.x) a[i * W + j] = __fmul_rn(a[i * W + j], rp);
+        __syncthreads();
+        const int cols = W - i - 1;
+        for (int q = threadIdx.x; q < (N - 1) * cols; q += blockDim.x) {
+            int r = q / cols;
+            const int j = i + 1 + (q - r * cols);
+            r += r >= i;
+            a[r * W + j] = __fadd_rn(a[r * W + j], __fmul_rn(-fac[r], a[i * W + j]));
+        }
+        __syncthreads();
+    }
+    for (int t = threadIdx.x; t < N; t += blockDim.x) {
+        float s = 0.f;
+        for (int u = 0; u < N; u++) s = __fadd_rn(s, __fmul_rn(a[t * W + N + u], mean[u]));
+        dst[t] = s;
+    }
+}
+
+// step 5, weighted reassignment (KMeansPlusPlusClusterer.updateAssignedPointsAnisotropic): argmin over c of
+//   fl(fl(pcm * fl(e * e)) + fl(fl(fl(|c|^2 - fl(2 dot)) + |x|^2) - fl(e * e))),  dot = c.x in order, e = fl(dot - |x|^2),
+// starting from the current cluster at Float.MAX_VALUE, first minimum wins. Centroid tiles and their |c|^2 in shared memory.
+template <bool REG>
+__global__ void __launch_bounds__(256) pq_train_assign_aniso_kernel(const float *__restrict__ train, long long nt, int dim, int M, int k,
+                                                                    const float *__restrict__ cent, const int *__restrict__ active,
+                                                                    const float *__restrict__ xn, float pcm_big, float pcm_small,
+                                                                    int32_t *__restrict__ assign, unsigned long long *__restrict__ changed)
+{
+    extern __shared__ float s_cent[];
+    const int m = blockIdx.y;
+    if (!active[m]) return;
+    int sz, off;
+    sub_layout(dim, M, m, sz, off);
+    const float pcm = m < dim % M ? pcm_big : pcm_small;
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool valid = j < nt;
+    const float *x = train + (size_t)nt * off + (size_t)(valid ? j : 0) * sz;
+    float xr[REG ? REG_X : 1];
+    if (REG) {
+#pragma unroll
+        for (int t = 0; t < REG_X; t++) xr[t] = valid && t < sz ? x[t] : 0.f;
+    }
+    const float xx = valid ? xn[(size_t)m * nt + j] : 0.f;
+    const float *cb = cent + (size_t)k * off;
+    const int ct = TILE_FLOATS / (sz + 1);
+    float *s_norm = s_cent + (size_t)ct * sz;
+    int32_t *a = assign + (size_t)m * nt + (valid ? j : 0);
+    const int old = valid ? *a : 0;
+    float best = 3.402823466e+38f;  // Float.MAX_VALUE
+    int bi = old;
+    for (int c0 = 0; c0 < k; c0 += ct) {
+        const int c1 = min(k, c0 + ct);
+        __syncthreads();
+        for (int q = threadIdx.x; q < (c1 - c0) * sz; q += blockDim.x) s_cent[q] = cb[(size_t)c0 * sz + q];
+        __syncthreads();
+        for (int c = threadIdx.x; c < c1 - c0; c += blockDim.x) {
+            float s = 0.f;
+            for (int t = 0; t < sz; t++) s = __fadd_rn(s, __fmul_rn(s_cent[c * sz + t], s_cent[c * sz + t]));
+            s_norm[c] = s;
+        }
+        __syncthreads();
+        if (!valid) continue;
+        for (int c = c0; c < c1; c++) {
+            const float *cen = s_cent + (size_t)(c - c0) * sz;
+            float dot = 0.f;
+            if (REG) {
+#pragma unroll
+                for (int t = 0; t < REG_X; t++)
+                    if (t < sz) dot = __fadd_rn(dot, __fmul_rn(cen[t], xr[t]));
+            } else
+                for (int t = 0; t < sz; t++) dot = __fadd_rn(dot, __fmul_rn(cen[t], x[t]));
+            const float e = __fsub_rn(dot, xx);
+            const float resid = __fadd_rn(__fsub_rn(s_norm[c - c0], __fmul_rn(2.f, dot)), xx);
+            const float par = __fmul_rn(e, e);
+            const float d = __fadd_rn(__fmul_rn(pcm, par), __fsub_rn(resid, par));
+            if (d < best) { best = d; bi = c; }
+        }
+    }
+    const bool moved = valid && bi != old;
+    if (valid) *a = bi;
+    const unsigned b = __ballot_sync(FULL, moved);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(changed + m, (unsigned long long)__popc(b));
+}
+
 #define LAUNCHED()                                  \
     do {                                            \
         g_launches++;                               \
@@ -346,9 +564,11 @@ cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *ini
     const long long nt = ord.empty() ? n : (long long)ord.size();
     const bool seeding = init_codebooks == nullptr;
     const bool center = seeding ? p.globally_center != 0 : centroid != nullptr;
+    const bool aniso = p.aniso_iters > 0;
+    const int szmax = (dim + M - 1) / M, npmax = aniso ? szmax * (szmax + 1) / 2 : 0;
     int32_t *d_ord, *d_assign, *d_counts, *d_active;
-    float *d_train, *d_D, *d_cent, *d_mean;
-    long long *d_sums, *d_csum;
+    float *d_train, *d_D, *d_cent, *d_mean, *d_xn, *d_rinv;
+    long long *d_sums, *d_csum, *d_osum;
     unsigned long long *d_best, *d_ebest, *d_changed, *d_counters;
     unsigned *d_colmax;
     auto carve = [&](void *base) {
@@ -367,7 +587,10 @@ cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *ini
         d_mean = c.take<float>(dim);
         d_changed = c.take<unsigned long long>(M);
         d_active = c.take<int32_t>(M);
-        d_counters = c.take<unsigned long long>(2);  // seeding fallbacks, empty reseeds
+        d_counters = c.take<unsigned long long>(3);  // seeding fallbacks, empty reseeds, anisotropic reseeds
+        d_xn = c.take<float>(aniso ? (size_t)nt * M : 0);
+        d_rinv = c.take<float>(aniso ? (size_t)nt * M : 0);
+        d_osum = c.take<long long>((size_t)M * k * npmax);
         return c.bytes;
     };
     DeviceBuffer mem;
@@ -380,7 +603,7 @@ cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *ini
     TRY(timer.start(s));
     TRY(cudaMemsetAsync(d_colmax, 0, 2 * (size_t)dim * 4, s));
     TRY(cudaMemsetAsync(d_csum, 0, (size_t)dim * 8, s));
-    TRY(cudaMemsetAsync(d_counters, 0, 16, s));
+    TRY(cudaMemsetAsync(d_counters, 0, 24, s));
     if (!ord.empty()) TRY(cudaMemcpyAsync(d_ord, ord.data(), ord.size() * 4, cudaMemcpyHostToDevice, s));
     const int32_t *ordp = ord.empty() ? nullptr : d_ord;
     const dim3 col_grid((dim + 127) / 128, (unsigned)((nt + SAMPLE_ROWS - 1) / SAMPLE_ROWS));
@@ -395,7 +618,6 @@ cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *ini
     pq_train_gather_kernel<<<col_grid, 128, 0, s>>>(f32.rows, f32.stride, ordp, nt, dim, M, center ? d_mean : nullptr, d_train, d_colmax);
     LAUNCHED();
 
-    const int szmax = (dim + M - 1) / M;
     const dim3 row_grid((unsigned)((nt + 255) / 256), M);
     if (seeding) {
         TRY(cudaMemsetAsync(d_best, 0xff, 2 * (size_t)k * M * 8, s));
@@ -445,10 +667,51 @@ cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *ini
             if ((double)changed[m] <= 0.01 * (double)nt) active[m] = 0;
         }
     }
-    unsigned long long counters[2];
+    // anisotropic rounds (KMeansPlusPlusClusterer.cluster(.., aniso_iters)) for every sub-space, from the assignment above
+    std::vector<int> aupdates(M, 0);
+    std::vector<long long> alast(M, 0);
+    if (aniso) {
+        const float pcm_big = pq_parallel_cost_multiplier(p.threshold, szmax), pcm_small = pq_parallel_cost_multiplier(p.threshold, dim / M);
+        pq_train_norm_kernel<<<row_grid, 256, 0, s>>>(d_train, nt, dim, M, d_xn, d_rinv);
+        LAUNCHED();
+        const int ptile = std::max(1, std::min({npmax, SUM_TILE / k, PAIR_TILE}));
+        const dim3 outer_grid(upd_grid.x, (unsigned)((npmax + ptile - 1) / ptile), M);
+        std::fill(active.begin(), active.end(), 1);
+        for (int r = 0; r < p.aniso_iters; r++) {
+            if (std::find(active.begin(), active.end(), 1) == active.end()) break;
+            TRY(cudaMemcpyAsync(d_active, active.data(), (size_t)M * 4, cudaMemcpyHostToDevice, s));
+            TRY(cudaMemsetAsync(d_sums, 0, (size_t)k * dim * 8, s));
+            TRY(cudaMemsetAsync(d_counts, 0, (size_t)M * k * 4, s));
+            TRY(cudaMemsetAsync(d_osum, 0, (size_t)M * k * npmax * 8, s));
+            TRY(cudaMemsetAsync(d_changed, 0, (size_t)M * 8, s));
+            pq_train_update_kernel<<<upd_grid, 256, 0, s>>>(d_train, nt, dim, M, k, tlen, d_assign, d_active, d_colmax, d_sums, d_counts);
+            LAUNCHED();
+            pq_train_outer_kernel<<<outer_grid, 256, 0, s>>>(d_train, nt, dim, M, k, ptile, npmax, d_assign, d_active, d_rinv, d_osum);
+            LAUNCHED();
+            pq_train_solve_kernel<<<dim3(k, M), 256, 0, s>>>(d_train, nt, dim, M, k, npmax, d_active, d_sums, d_counts, d_colmax, d_osum, pcm_big, pcm_small,
+                                                             p.seed, r, d_cent, d_counters + 2);
+            LAUNCHED();
+            if (szmax <= REG_X)
+                pq_train_assign_aniso_kernel<true><<<row_grid, 256, assign_smem, s>>>(d_train, nt, dim, M, k, d_cent, d_active, d_xn, pcm_big, pcm_small,
+                                                                                      d_assign, d_changed);
+            else
+                pq_train_assign_aniso_kernel<false><<<row_grid, 256, assign_smem, s>>>(d_train, nt, dim, M, k, d_cent, d_active, d_xn, pcm_big, pcm_small,
+                                                                                       d_assign, d_changed);
+            LAUNCHED();
+            TRY(cudaMemcpyAsync(changed.data(), d_changed, (size_t)M * 8, cudaMemcpyDeviceToHost, s));
+            TRY(cudaStreamSynchronize(s));
+            for (int m = 0; m < M; m++) {
+                if (!active[m]) continue;
+                aupdates[m]++;
+                alast[m] = (long long)changed[m];
+                if ((double)changed[m] <= 0.01 * (double)nt) active[m] = 0;
+            }
+        }
+    }
+    unsigned long long counters[3];
     TRY(cudaMemcpyAsync(codebooks_out, d_cent, (size_t)k * dim * 4, cudaMemcpyDeviceToHost, s));
     if (seeding && center && centroid_out) TRY(cudaMemcpyAsync(centroid_out, d_mean, (size_t)dim * 4, cudaMemcpyDeviceToHost, s));
-    TRY(cudaMemcpyAsync(counters, d_counters, 16, cudaMemcpyDeviceToHost, s));
+    TRY(cudaMemcpyAsync(counters, d_counters, 24, cudaMemcpyDeviceToHost, s));
     TRY(timer.stop(s));
     TRY(cudaStreamSynchronize(s));
     st->train_rows = nt;
@@ -457,6 +720,10 @@ cudaError_t pq_train(const DataDesc &f32, const PqTrainArgs &p, const float *ini
     for (long long c : last) st->changed_last += c;
     st->seeding_fallbacks = (long long)counters[0];
     st->empty_reseeds = (long long)counters[1];
+    st->aniso_updates = *std::max_element(aupdates.begin(), aupdates.end());
+    st->aniso_changed_last = 0;
+    for (long long c : alast) st->aniso_changed_last += c;
+    st->aniso_reseeds = (long long)counters[2];
     st->device_ms = timer.ms();
     return cudaSuccess;
 }
