@@ -489,6 +489,39 @@ JV_API int jv_graph_remove_deleted_pq(jv_graph g, jv_dataset pq, int metric, flo
                                       const uint32_t *deleted_bits /* host, bit (node & 31) of word (node >> 5) */,
                                       jv_graph *out, jv_remove_stats *stats);
 
+/* ---- building and maintaining a graph over BQ codes (BuildScoreProvider.bqBuildScoreProvider) ----
+ * jv_graph_build, jv_builder_create, jv_graph_add_nodes, jv_builder_create_from_graph and jv_graph_remove_deleted over a BQ data
+ * set, for an index that keeps only its binary codes (ceil(dim / 64) * 8 bytes per node: 192 B at 1536 dims, against 6 144 B of fp32
+ * rows). Everything their contracts say that does not mention scores holds unchanged, as for the PQ calls above: batches, window,
+ * back-links, re-prunes and cleanup; the level draws and upper levels; the add's seeding, entry rule and deleted_bits; the removal's
+ * candidate gathering, random fallback, entry rule and holes; what jv_graph_build_stats and jv_remove_stats report.
+ * The scores are BQVectors': the insert or repair of node v searches with its own code c_v as the query (the BQ walk, no rerank,
+ * topK = rerankK = beam_width), the prune's keys are 1 - hd(c_v, c_u) / dim — the walk's own scores — and its pair similarities
+ * 1 - hd(c_a, c_b) / dim. No score depends on the metric: it is checked as every call checks it, and the three metrics give the same
+ * bytes. An add into a one-node graph gives the bytes of jv_graph_build_bq.
+ * Rows [0, n0) of `bq` must be the graph's own nodes (the calls cannot check it). A BQ data set does not grow in place: encode the
+ * new rows with jv_bq_encode_batch and register the longer word array with jv_dataset_register_bq.
+ * No row may set a bit past dim in its last word (BinaryQuantization.encode and jv_bq_encode_* never do): the walk's query, re-encoded
+ * from c_v, has those bits clear while the pair scores read the raw words. The calls check every row, with one small reduction before
+ * any other device work.
+ * The removal's prune runs at the smallest of 64 / 128 / 256 / 1024 / 2048 / 8192 candidate slots that holds a row's distinct
+ * candidates; every degree up to 64 fits, so no candidate set is ever clipped and no call is refused for shared memory.
+ * Errors: JV_ERR_INVALID for a null argument, a data set that is not BQ, a row with bits set past dim, n < n0 (add) or n != g's size
+ * (remove), a device mismatch, a degree mismatch, a bad metric or alpha < 1; JV_ERR_UNSUPPORTED for a degree above 64. Every check
+ * precedes the device work: a refused call has done none of it and leaves *out untouched. The fp32 and PQ calls keep refusing a BQ
+ * data set with the codes they return for it. */
+JV_API int jv_graph_build_bq(jv_dataset bq, int metric, const jv_build_params *params, jv_graph *out, double *device_ms);
+/* the step-wise form of jv_graph_build_bq (same checks and errors); every other jv_builder_* call works on it unchanged */
+JV_API int jv_builder_create_bq(jv_dataset bq, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out);
+JV_API int jv_graph_add_nodes_bq(jv_graph g, jv_dataset bq, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                 jv_graph *out, double *device_ms);
+/* the step-wise form of jv_graph_add_nodes_bq, driven by the jv_builder_* calls like jv_builder_create_from_graph's builder */
+JV_API int jv_builder_create_from_graph_bq(jv_graph g, jv_dataset bq, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                           void *cuda_stream, jv_builder *out);
+JV_API int jv_graph_remove_deleted_bq(jv_graph g, jv_dataset bq, int metric, float alpha, uint64_t seed,
+                                      const uint32_t *deleted_bits /* host, bit (node & 31) of word (node >> 5) */,
+                                      jv_graph *out, jv_remove_stats *stats);
+
 /* device-memory helpers for callers that keep queries/results in HBM (bench `value` leg) */
 JV_API int jv_device_malloc(void **out, size_t bytes);
 JV_API int jv_device_free(void *p);

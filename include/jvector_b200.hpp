@@ -174,6 +174,13 @@ public:
         check(jv_graph_build_pq(v.handle(), (int)vsf_, &p_, &g, &deviceMs));
         return GraphIndex(g);
     }
+    /// the build over BQ codes (BuildScoreProvider.bqBuildScoreProvider): every score is 1 - hamming / dim, whatever vsf is
+    GraphIndex build(const BQVectors &v)
+    {
+        jv_graph g = nullptr;
+        check(jv_graph_build_bq(v.handle(), (int)vsf_, &p_, &g, &deviceMs));
+        return GraphIndex(g);
+    }
     /// markNodeDeleted + removeDeletedNodes (GraphIndexBuilder.java:678-799): a NEW graph without the nodes whose bit is set in
     /// deletedBits (bit node & 31 of word node >> 5), their neighbours' lists repaired on the device; `graph` is left as it is.
     /// Until then, search the marked graph with acceptOrds excluding them. Counters go to removeStats.
@@ -192,6 +199,14 @@ public:
         check(jv_graph_remove_deleted_pq(graph.handle(), v.handle(), (int)vsf_, p_.alpha, p_.seed, deletedBits.data(), &g, &removeStats));
         return GraphIndex(g);
     }
+    /// removeDeletedNodes over the graph's BQ codes (jv_graph_remove_deleted_bq): the scores of build(const BQVectors &)
+    GraphIndex removeDeletedNodes(const GraphIndex &graph, const BQVectors &v, const std::vector<uint32_t> &deletedBits)
+    {
+        if ((int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "removeDeletedNodes: deletedBits shorter than the graph");
+        jv_graph g = nullptr;
+        check(jv_graph_remove_deleted_bq(graph.handle(), v.handle(), (int)vsf_, p_.alpha, p_.seed, deletedBits.data(), &g, &removeStats));
+        return GraphIndex(g);
+    }
     /// addGraphNode (GraphIndexBuilder.java:588-659) for nodes graph.size() .. v.size() - 1: a NEW graph (`graph` is left as it
     /// is); v's first rows must be graph's own nodes. deletedBits (optional, bit node & 31 of word node >> 5): marked nodes the new
     /// ones never pick as neighbours. The hierarchy follows graph's.
@@ -208,6 +223,14 @@ public:
         if (!deletedBits.empty() && (int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "addGraphNodes: deletedBits shorter than the graph");
         jv_graph g = nullptr;
         check(jv_graph_add_nodes_pq(graph.handle(), v.handle(), (int)vsf_, &p_, deletedBits.empty() ? nullptr : deletedBits.data(), &g, &deviceMs));
+        return GraphIndex(g);
+    }
+    /// addGraphNodes over BQ codes (jv_graph_add_nodes_bq): v holds graph's nodes first, then the new rows' words
+    GraphIndex addGraphNodes(const GraphIndex &graph, const BQVectors &v, const std::vector<uint32_t> &deletedBits = {})
+    {
+        if (!deletedBits.empty() && (int64_t)deletedBits.size() * 32 < (int64_t)graph.size()) throw Error(JV_ERR_INVALID, "addGraphNodes: deletedBits shorter than the graph");
+        jv_graph g = nullptr;
+        check(jv_graph_add_nodes_bq(graph.handle(), v.handle(), (int)vsf_, &p_, deletedBits.empty() ? nullptr : deletedBits.data(), &g, &deviceMs));
         return GraphIndex(g);
     }
     double deviceMs = 0;

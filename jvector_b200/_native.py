@@ -133,6 +133,11 @@ SYMBOLS = [
     ("jv_graph_remove_deleted_pq", _I, [_P, _P, _I, _F, C.c_uint64, C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(RemoveStats)]),
     ("jv_graph_add_nodes_pq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_builder_create_from_graph_pq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), _P, C.POINTER(_P)]),
+    ("jv_graph_build_bq", _I, [_P, _I, C.POINTER(BuildParams), C.POINTER(_P), C.POINTER(C.c_double)]),
+    ("jv_builder_create_bq", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]),
+    ("jv_graph_remove_deleted_bq", _I, [_P, _P, _I, _F, C.c_uint64, C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(RemoveStats)]),
+    ("jv_graph_add_nodes_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(C.c_double)]),
+    ("jv_builder_create_from_graph_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), _P, C.POINTER(_P)]),
     ("jv_builder_create", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]), ("jv_builder_info", _I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     ("jv_builder_next_batch", _I, [_P, i32p, i32p]), ("jv_builder_insert_slice", _I, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     ("jv_builder_apply_new", _I, [_P, C.c_int32, C.c_int32, _P, _P, i32p]), ("jv_builder_reprune_slice", _I, [_P, C.c_int32, C.c_int32, _P, _P]),

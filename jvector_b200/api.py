@@ -498,9 +498,15 @@ def pack_accept_bits(mask):
     return np.ascontiguousarray(np.packbits(m, axis=-1, bitorder="little").view(np.uint32))
 
 
+def _by_kind(vectors, f32, pq, bq):
+    """the entry point of the kind of `vectors`: fp32 rows, PQ codes or BQ codes"""
+    return pq if isinstance(vectors, PQVectors) else bq if isinstance(vectors, BQVectors) else f32
+
+
 class GraphIndexBuilder:
-    """base:graph/GraphIndexBuilder.java: (M, beamWidth, neighborOverflow, alpha, addHierarchy) over exact fp32 scores, or over PQ
-    codes (BuildScoreProvider.pqBuildScoreProvider) when build(), addGraphNodes() or removeDeletedNodes() is given PQVectors."""
+    """base:graph/GraphIndexBuilder.java: (M, beamWidth, neighborOverflow, alpha, addHierarchy) over exact fp32 scores, over PQ
+    codes (BuildScoreProvider.pqBuildScoreProvider) when build(), addGraphNodes() or removeDeletedNodes() is given PQVectors, or over
+    BQ codes (BuildScoreProvider.bqBuildScoreProvider) when they are given BQVectors."""
 
     def __init__(self, vsf, M=32, beamWidth=100, neighborOverflow=1.2, alpha=1.2, addHierarchy=False, seed=0, max_batch=0, concurrent_window=-1):
         self.vsf = vsf
@@ -509,11 +515,13 @@ class GraphIndexBuilder:
 
     def build(self, vectors):
         """F32Vectors: exact scores (jv_graph_build). PQVectors: the inserts walk the codes with decode(c_v) as the query and the
-        prune compares codes through the centroid-pair table (jv_graph_build_pq), which it builds on the data set if needed."""
+        prune compares codes through the centroid-pair table (jv_graph_build_pq), which it builds on the data set if needed.
+        BQVectors: the inserts walk the codes with c_v as the query and every score is 1 - hamming / dim (jv_graph_build_bq), whatever
+        the similarity function."""
         lib = nat.init()
         h = C.c_void_p()
         ms = C.c_double()
-        fn = lib.jv_graph_build_pq if isinstance(vectors, PQVectors) else lib.jv_graph_build
+        fn = _by_kind(vectors, lib.jv_graph_build, lib.jv_graph_build_pq, lib.jv_graph_build_bq)
         check(fn(vectors._h, int(self.vsf), C.byref(self.params), C.byref(h), C.byref(ms)))
         self.device_ms = ms.value
         s, b, d = C.c_int64(), C.c_int64(), C.c_int64()
@@ -531,7 +539,8 @@ class GraphIndexBuilder:
         `.remove_stats` (jv_remove_stats as a dict) and no FusedPQ records: call fuse_pq on it again if needed.
 
         vectors: the graph's F32Vectors (exact scores, jv_graph_remove_deleted) or its PQVectors (jv_graph_remove_deleted_pq): the
-        repair of node v then scores with decode(c_v)'s ADC and the centroid-pair table, as build() over PQVectors does.
+        repair of node v then scores with decode(c_v)'s ADC and the centroid-pair table, as build() over PQVectors does. Or its
+        BQVectors (jv_graph_remove_deleted_bq): Hamming scores, as build() over BQVectors uses.
 
         Until this is called, a graph with marked nodes is searched with GraphSearcher.search(..., acceptOrds=~deleted): the marked
         nodes stay on the search paths but are never returned."""
@@ -539,7 +548,7 @@ class GraphIndexBuilder:
         bits = _deleted_bits(deleted, graph.info()["n"])
         st = nat.RemoveStats()
         h = C.c_void_p()
-        fn = lib.jv_graph_remove_deleted_pq if isinstance(vectors, PQVectors) else lib.jv_graph_remove_deleted
+        fn = _by_kind(vectors, lib.jv_graph_remove_deleted, lib.jv_graph_remove_deleted_pq, lib.jv_graph_remove_deleted_bq)
         check(fn(graph._h, vectors._h, int(self.vsf), float(self.params.alpha), int(self.params.seed),
                  bits.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(h), C.byref(st)))
         out = GraphIndex(_handle=h)
@@ -548,11 +557,12 @@ class GraphIndexBuilder:
 
     def addGraphNodes(self, graph, vectors, deleted=None):
         """GraphIndexBuilder.addGraphNode for every node graph.size() .. vectors.size() - 1, on the device (jv_graph_add_nodes, or
-        jv_graph_add_nodes_pq for PQVectors).
+        jv_graph_add_nodes_pq for PQVectors, jv_graph_add_nodes_bq for BQVectors).
 
-        vectors: F32Vectors or PQVectors whose first rows are the graph's own nodes, followed by the new ones. A PQ data set grows
-        by encoding the new rows with the same codebooks (ProductQuantization.encodeAll) and wrapping the longer code array in new
-        PQVectors; the insert of node v then uses decode(c_v) as its query, as build() over PQVectors does. Returns a NEW GraphIndex (`graph`
+        vectors: F32Vectors, PQVectors or BQVectors whose first rows are the graph's own nodes, followed by the new ones. A PQ data set
+        grows by encoding the new rows with the same codebooks (ProductQuantization.encodeAll) and wrapping the longer code array in new
+        PQVectors; the insert of node v then uses decode(c_v) as its query, as build() over PQVectors does. A BQ data set grows by
+        encoding the new rows (bq_encode_all) and wrapping the longer word array in new BQVectors. Returns a NEW GraphIndex (`graph`
         is left as it is), built from the graph's rows with this builder's parameters (M must equal the graph's degree); its holes
         stay holes, the hierarchy follows the graph's (addHierarchy is ignored) and it has no FusedPQ records. deleted: nodes marked
         deleted but not removed yet (a bool mask over the graph's nodes or an array of their ids): the new nodes never pick them as
@@ -561,7 +571,7 @@ class GraphIndexBuilder:
         bits = _deleted_bits(deleted, graph.info()["n"]) if deleted is not None else None
         h = C.c_void_p()
         ms = C.c_double()
-        fn = lib.jv_graph_add_nodes_pq if isinstance(vectors, PQVectors) else lib.jv_graph_add_nodes
+        fn = _by_kind(vectors, lib.jv_graph_add_nodes, lib.jv_graph_add_nodes_pq, lib.jv_graph_add_nodes_bq)
         check(fn(graph._h, vectors._h, int(self.vsf), C.byref(self.params),
                  bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None, C.byref(h), C.byref(ms)))
         self.device_ms = ms.value

@@ -1506,25 +1506,27 @@ static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vec
 // one upper level: a Vamana graph over its members ids (local row r = node ids[r]), built by the device builder on the members'
 // rows (one gather kernel), from nothing or from `seed` (local rows). ladj: [ids.size()][degree] in node ids. Synchronises `s`.
 // A PQ data set (jv_graph_build_pq) gives the level its members' code rows; codebooks, centroid, magnitudes and pair tables are shared.
+// A BQ data set (jv_graph_build_bq) gives it their word rows.
 static int build_level(jv_dataset ds, int metric, const BuildParams &bp, const std::vector<int32_t> &ids, const BuilderSeed *seed,
                        std::vector<int32_t> &ladj, cudaStream_t s)
 {
     const int cnt = (int)ids.size(), degree = bp.degree;
     ladj.assign((size_t)cnt * degree, -1);
     if (cnt <= 1) return JV_OK;
-    const bool pq = ds->d.kind == KIND_PQ;
+    const bool codes = ds->d.kind == KIND_PQ || ds->d.kind == KIND_BQ;
     DataDesc sub;
     memset(&sub, 0, sizeof(DataDesc));
-    if (pq) sub = ds->d;
+    if (codes) sub = ds->d;
     sub.kind = ds->d.kind; sub.dim = ds->d.dim; sub.stride = ds->d.stride; sub.n = cnt;
-    DeviceBuffer rows, adj, dids;  // the members' rows (fp32 rows or code rows), their adjacency, their ids
-    cudaError_t e = rows.alloc(pq ? (size_t)cnt * sub.code_stride : (size_t)cnt * sub.stride * 4);
+    DeviceBuffer rows, adj, dids;  // the members' rows (fp32 rows, code rows or word rows), their adjacency, their ids
+    cudaError_t e = rows.alloc(codes ? (size_t)cnt * code_row_bytes(sub) : (size_t)cnt * sub.stride * 4);
     if (e == cudaSuccess) e = adj.alloc((size_t)cnt * degree * 4);
     if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
     if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
-    if (pq) {
-        if (e == cudaSuccess) e = launch_gather_codes(ds->d, dids.get<int32_t>(), cnt, rows.get<uint8_t>(), s);
-        sub.codes = rows.get<uint8_t>();
+    if (codes) {
+        if (e == cudaSuccess) e = launch_gather_codes(ds->d, dids.get<int32_t>(), cnt, rows.get(), s);
+        if (sub.kind == KIND_BQ) sub.words = rows.get<unsigned long long>();
+        else sub.codes = rows.get<uint8_t>();
     } else {
         if (e == cudaSuccess) e = launch_gather_rows(ds->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
         sub.rows = rows.get<float>();
@@ -1557,7 +1559,7 @@ static int build_upper_levels(jv_graph g, jv_dataset ds, int metric, const Build
     return graph_rebuild_upper(g);
 }
 
-// the whole build over an fp32 or a PQ data set whose arguments have been checked: level 0, then the upper levels
+// the whole build over an fp32, a PQ or a BQ data set whose arguments have been checked: level 0, then the upper levels
 static int graph_build(jv_dataset ds, int metric, const jv_build_params *params, const BuildParams &bp, jv_graph *out, double *device_ms)
 {
     int rc;
@@ -1623,6 +1625,41 @@ int jv_graph_build_pq(jv_dataset pq, int metric, const jv_build_params *params, 
     return graph_build(pq, metric, params, bp, out, device_ms);
 }
 
+// a BQ data set whose rows set a bit past dim: the walk re-encodes its query with those bits clear while the prune's pair scores
+// read the raw words, so the two would disagree on Hamming distances. BinaryQuantization.encode and jv_bq_encode_* never set them.
+// One reduction over the last word of every row, the first device work of the call.
+static int bq_padding_check(jv_dataset bq, const char *who)
+{
+    int rc;
+    if ((rc = t_ctx.init())) return rc;
+    bool set = false;
+    CK(bq_padding_set(bq->d, &set, t_ctx.stream), "bq padding check");
+    if (set) return fail(JV_ERR_INVALID, std::string(who) + ": a row of the BQ data set has bits set past dim " + std::to_string(bq->d.dim));
+    return JV_OK;
+}
+
+// the checks of a build over BQ codes (bqBuildScoreProvider). The metric is checked as every call checks it, and no score uses it.
+static int bq_build_check(jv_dataset bq, int metric, const jv_build_params *params, BuildParams *bp)
+{
+    if (bq->d.kind != KIND_BQ) return fail(JV_ERR_INVALID, "graph_build_bq: needs a BQ data set");
+    int rc = check_metric(bq->d, metric);
+    if (rc) return rc;
+    if (params->degree > 64)
+        return fail(JV_ERR_UNSUPPORTED, "graph_build_bq: degree " + std::to_string(params->degree) + " > 64, the largest row the builder handles");
+    if ((rc = build_params_check(params, bp))) return rc;
+    return bq_padding_check(bq, "graph_build_bq");
+}
+
+int jv_graph_build_bq(jv_dataset bq, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
+{
+    ON_DEVICE_OF(bq);
+    if (!params || !out) return fail(JV_ERR_INVALID, "graph_build_bq: null argument");
+    BuildParams bp;
+    const int rc = bq_build_check(bq, metric, params, &bp);
+    if (rc) return rc;
+    return graph_build(bq, metric, params, bp, out, device_ms);
+}
+
 static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bits[(size_t)v >> 5] >> (v & 31)) & 1u; }
 
 // ------------------------------------------------------------------------------------------------ addGraphNode for a batch
@@ -1649,12 +1686,14 @@ static std::vector<uint32_t> add_accept_bits(const GraphAdd &A, const int32_t *i
     return bits;
 }
 
-// the checks of an add over a data set of `kind` (KIND_F32: jv_graph_add_nodes, KIND_PQ: jv_graph_add_nodes_pq). Over PQ also those
-// of the PQ build: a LUT the prune can hold, and the metric's centroid-pair table, built and kept on the data set when it has none
+// the checks of an add over a data set of `kind` (KIND_F32: jv_graph_add_nodes, KIND_PQ: jv_graph_add_nodes_pq, KIND_BQ:
+// jv_graph_add_nodes_bq). Over PQ also those of the PQ build: a LUT the prune can hold, and the metric's centroid-pair table, built and
+// kept on the data set when it has none. Over BQ also the BQ build's: no bit set past dim.
 static int add_check(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, BuildParams *bp)
 {
     if (!ds || !params) return fail(JV_ERR_INVALID, "add_nodes: null argument");
-    if (ds->d.kind != kind) return fail(JV_ERR_INVALID, kind == KIND_PQ ? "add_nodes_pq: needs a PQ data set" : "add_nodes: needs an fp32 data set");
+    if (ds->d.kind != kind)
+        return fail(JV_ERR_INVALID, kind == KIND_PQ ? "add_nodes_pq: needs a PQ data set" : kind == KIND_BQ ? "add_nodes_bq: needs a BQ data set" : "add_nodes: needs an fp32 data set");
     if (ds->device != g->device) return fail(JV_ERR_INVALID, "add_nodes: data set and graph live on different devices");
     if (ds->d.n < g->g.n || ds->d.n > INT32_MAX) return fail(JV_ERR_INVALID, "add_nodes: the data set must hold the graph's nodes first");
     int rc = check_metric(ds->d, metric);
@@ -1662,7 +1701,8 @@ static int add_check(jv_graph g, jv_dataset ds, int kind, int metric, const jv_b
     if (g->g.degree > 64)
         return fail(JV_ERR_UNSUPPORTED, "add_nodes: degree " + std::to_string(g->g.degree) + " > 64, the largest row the builder handles");
     if (params->degree != g->g.degree) return fail(JV_ERR_INVALID, "add_nodes: params->degree differs from the graph's degree");
-    if ((rc = build_params_check(params, bp)) || kind != KIND_PQ) return rc;
+    if ((rc = build_params_check(params, bp)) || kind == KIND_F32) return rc;
+    if (kind == KIND_BQ) return bq_padding_check(ds, "add_nodes_bq");
     if (!pq_prune_fits(ds->d))
         return fail(JV_ERR_UNSUPPORTED, "add_nodes_pq: a LUT of M * k = " + std::to_string(ds->d.M * ds->d.k) +
                                             " entries does not fit the prune's shared memory next to its candidates (DESIGN §4.3c)");
@@ -1750,7 +1790,8 @@ static int add_finish(jv_graph_s *ng, const GraphAdd &A, jv_dataset ds, int metr
     return graph_rebuild_upper(ng);
 }
 
-// jv_graph_add_nodes (kind = KIND_F32) and jv_graph_add_nodes_pq (KIND_PQ): the builder scores whatever kind of rows it is given
+// jv_graph_add_nodes (kind = KIND_F32), jv_graph_add_nodes_pq (KIND_PQ) and jv_graph_add_nodes_bq (KIND_BQ): the builder scores
+// whatever kind of rows it is given
 static int graph_add_nodes(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
                            double *device_ms)
 {
@@ -1809,6 +1850,12 @@ int jv_graph_add_nodes_pq(jv_graph g, jv_dataset pq, int metric, const jv_build_
     return graph_add_nodes(g, pq, KIND_PQ, metric, params, deleted_bits, out, device_ms);
 }
 
+int jv_graph_add_nodes_bq(jv_graph g, jv_dataset bq, int metric, const jv_build_params *params, const uint32_t *deleted_bits, jv_graph *out,
+                          double *device_ms)
+{
+    return graph_add_nodes(g, bq, KIND_BQ, metric, params, deleted_bits, out, device_ms);
+}
+
 // ---- the same build advanced batch by batch, for a build SHARDED over several GPUs (BASELINE config 5) ----------------------
 // Every rank holds a replica of the rows and of the adjacency. Per batch: each rank searches + prunes ITS slice of the batch
 // (jv_builder_insert_slice -> rows in a caller buffer), the slices are all-gathered by the caller (NCCL; jvector_b200/parallel.py),
@@ -1816,7 +1863,7 @@ int jv_graph_add_nodes_pq(jv_graph g, jv_dataset pq, int metric, const jv_build_
 // re-pruned slice-wise and exchanged the same way. The device pointers are the caller's (e.g. torch tensors = the NCCL buffers).
 struct jv_builder_s {
     int device = 0;
-    jv_dataset data = nullptr;  // fp32 rows, or PQ codes (jv_builder_create_pq)
+    jv_dataset data = nullptr;  // fp32 rows, PQ codes (jv_builder_create_pq) or BQ words (jv_builder_create_bq)
     int metric = 0;
     jv_build_params params;
     BuildParams bp;
@@ -1856,6 +1903,20 @@ int jv_builder_create_pq(jv_dataset pq, int metric, const jv_build_params *param
     return JV_OK;
 }
 
+int jv_builder_create_bq(jv_dataset bq, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
+{
+    ON_DEVICE_OF(bq);
+    if (!params || !out) return fail(JV_ERR_INVALID, "builder_create_bq: null argument");
+    std::unique_ptr<jv_builder_s> b(new jv_builder_s());
+    int rc = bq_build_check(bq, metric, params, &b->bp);
+    if (rc) return rc;
+    b->device = bq->device; b->data = bq; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
+    CK(b->timer.start(b->stream), "event");
+    CK(builder_create(bq->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
+    *out = b.release();
+    return JV_OK;
+}
+
 static int builder_from_graph(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
                               void *cuda_stream, jv_builder *out)
 {
@@ -1887,6 +1948,12 @@ int jv_builder_create_from_graph_pq(jv_graph g, jv_dataset pq, int metric, const
                                     void *cuda_stream, jv_builder *out)
 {
     return builder_from_graph(g, pq, KIND_PQ, metric, params, deleted_bits, cuda_stream, out);
+}
+
+int jv_builder_create_from_graph_bq(jv_graph g, jv_dataset bq, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
+                                    void *cuda_stream, jv_builder *out)
+{
+    return builder_from_graph(g, bq, KIND_BQ, metric, params, deleted_bits, cuda_stream, out);
 }
 
 int jv_builder_info(jv_builder b, int *degree, int *row_cap, int *max_batch)
@@ -2057,15 +2124,17 @@ static int remove_deleted_level(jv_graph g, jv_graph ng, jv_dataset ds, int metr
     return e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted");
 }
 
-// jv_graph_remove_deleted (kind = KIND_F32) and jv_graph_remove_deleted_pq (KIND_PQ): repair_level dispatches its prune by kind.
-// Every check comes before any device work, so a refused call has done none of it.
+// jv_graph_remove_deleted (kind = KIND_F32), jv_graph_remove_deleted_pq (KIND_PQ) and jv_graph_remove_deleted_bq (KIND_BQ): repair_level
+// dispatches its prune by kind. Every check comes before any device work, so a refused call has done none of it.
 static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
                                 jv_remove_stats *stats)
 {
     ON_DEVICE_OF(g);
     if (!ds || !deleted_bits || !out || !stats) return fail(JV_ERR_INVALID, "graph_remove_deleted: null argument");
     if (ds->d.kind != kind)
-        return fail(JV_ERR_INVALID, kind == KIND_PQ ? "graph_remove_deleted_pq: needs the graph's PQ data set" : "graph_remove_deleted: needs the graph's fp32 data set");
+        return fail(JV_ERR_INVALID, kind == KIND_PQ   ? "graph_remove_deleted_pq: needs the graph's PQ data set"
+                                    : kind == KIND_BQ ? "graph_remove_deleted_bq: needs the graph's BQ data set"
+                                                      : "graph_remove_deleted: needs the graph's fp32 data set");
     if (ds->d.n != g->g.n || ds->device != g->device) return fail(JV_ERR_INVALID, "graph_remove_deleted: data set and graph differ in size or device");
     if (!(alpha >= 1.0f)) return fail(JV_ERR_INVALID, "graph_remove_deleted: need alpha >= 1");
     int rc = check_metric(ds->d, metric);
@@ -2078,6 +2147,7 @@ static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric,
                                                 std::to_string(g->g.degree * (g->g.degree + 2)) + " candidates a row of this degree can gather (DESIGN §4.3e)");
         if ((rc = jv_dataset_pq_pair_table(ds, metric))) return rc;
     }
+    if (kind == KIND_BQ && (rc = bq_padding_check(ds, "graph_remove_deleted_bq"))) return rc;
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
     const int n = g->g.n, degree = g->g.degree;
@@ -2166,6 +2236,12 @@ int jv_graph_remove_deleted_pq(jv_graph g, jv_dataset pq, int metric, float alph
                                jv_remove_stats *stats)
 {
     return graph_remove_deleted(g, pq, KIND_PQ, metric, alpha, seed, deleted_bits, out, stats);
+}
+
+int jv_graph_remove_deleted_bq(jv_graph g, jv_dataset bq, int metric, float alpha, uint64_t seed, const uint32_t *deleted_bits, jv_graph *out,
+                               jv_remove_stats *stats)
+{
+    return graph_remove_deleted(g, bq, KIND_BQ, metric, alpha, seed, deleted_bits, out, stats);
 }
 
 // ------------------------------------------------------------------------------------------------ query batches (host-driven seam)

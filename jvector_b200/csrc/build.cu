@@ -17,6 +17,8 @@
 // (SURVEY §8d C5), not on identical adjacency.
 // Over a PQ data set (BuildScoreProvider.pqBuildScoreProvider, DESIGN §4.3c) the same loop runs on the codes: the insert queries
 // are decode(c_u) (pq_decode_kernel), the walk is the PQ walk, and the prune is prune_kernel<.., KIND_PQ> (ADC keys, pair table).
+// Over a BQ data set (BuildScoreProvider.bqBuildScoreProvider, DESIGN §4.3g) the insert queries are c_u as +-1 (bq_decode_kernel), the
+// walk is the BQ walk, and the prune is prune_kernel<.., KIND_BQ> (Hamming keys and pair scores).
 #include <limits.h>
 #include <string.h>
 
@@ -127,6 +129,18 @@ __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const f
     return score_map(METRIC, s);
 }
 
+// one BQ word row as floats in shared memory (2 W, rounded to 4 so that what follows stays 16-byte aligned)
+__host__ __device__ inline int bq_row_floats(const DataDesc &d) { return (2 * d.W + 3) & ~3; }
+
+// BQVectors.similarityBetween (BQVectors.java:116-118) of candidate row `a` (global) against a cached word row `srow` (shared), one warp
+__device__ __forceinline__ float pair_bq_row(const DataDesc &d, int a, const unsigned long long *srow, int lane)
+{
+    const unsigned long long *x = d.words + (size_t)a * d.W;
+    int hd = 0;
+    for (int i = lane; i < d.W; i += 32) hd += __popcll(__ldg(x + i) ^ srow[i]);
+    return bq_score_from_hd(group_sum_int<32>(hd), d.dim);
+}
+
 // retainDiverse (VamanaDiversityProvider.java:45-95), restated so that the pair scores can be produced in bulk:
 //   isDiverse(c) at alpha  <=>  max over the selected s of sim(c, s)  <=  score(c) * alpha.
 // Keep M[c] = that running maximum. Selecting a candidate s updates M[c] for every still-eligible c in parallel (one warp
@@ -141,14 +155,18 @@ __device__ __forceinline__ float pair_rows(const float4 *__restrict__ c, const f
 // The PQ capacities above PRUNE_MAXC (the repair's upper tiers, §4.3e) work on the power of two that holds the row's own candidates
 // instead of on MAXC — the key pass, the sort and the state reset shrink with it; a sort of KEY_MIN pads changes no result — and
 // write the selected row with one thread per neighbour.
+// KIND_BQ (bqBuildScoreProvider, §4.3g): the blob is v's own words c_v, the keys are score_bq's bits under it — the walk's, whose query
+// decodes to c_v — and the fold is the Hamming score of two word rows (pair_bq_row). No score depends on the metric, so one METRIC
+// instantiation serves all three. Its capacities above PRUNE_MAXC are bounded like PQ's.
 template <int METRIC, int MAXC = PRUNE_MAXC, int KIND = KIND_F32>
 __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
 {
-    constexpr bool BOUNDED = KIND == KIND_PQ && MAXC > PRUNE_MAXC;
+    constexpr bool BOUNDED = (KIND == KIND_PQ || KIND == KIND_BQ) && MAXC > PRUNE_MAXC;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    // f32: blob stride + 4, newrow stride (the most recently selected row). PQ: blob = the LUT, newrow = decode(c_v) (dim rounded to 4)
-    const int blob_fl = KIND == KIND_PQ ? blob_floats(P.d) : P.d.stride + 4;
-    const int row_fl = KIND == KIND_PQ ? (P.d.dim + 3) & ~3 : P.d.stride;
+    // f32: blob stride + 4, newrow stride (the most recently selected row). PQ: blob = the LUT, newrow = decode(c_v) (dim rounded to 4).
+    // BQ: blob = c_v, newrow = the selected row's words (2 W floats each, rounded to 4)
+    const int blob_fl = KIND == KIND_PQ ? blob_floats(P.d) : KIND == KIND_BQ ? bq_row_floats(P.d) : P.d.stride + 4;
+    const int row_fl = KIND == KIND_PQ ? (P.d.dim + 3) & ~3 : KIND == KIND_BQ ? bq_row_floats(P.d) : P.d.stride;
     float *blob = reinterpret_cast<float *>(smem_raw);
     float *newrow = blob + blob_fl;
     long long *keys = reinterpret_cast<long long *>(newrow + row_fl);        // MAXC
@@ -186,7 +204,19 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
         int cap = MAXC;
         if (BOUNDED)
             for (cap = PRUNE_MAXC; cap < nc;) cap <<= 1;
-        if (KIND == KIND_PQ) {
+        // (if constexpr: the fp32 and PQ instantiations compile exactly as they did before the BQ branches existed)
+        if constexpr (KIND == KIND_BQ) {
+            const uint32_t *cv = reinterpret_cast<const uint32_t *>(P.d.words + (size_t)v * P.d.W);
+            for (int t = tid; t < 2 * P.d.W; t += PRUNE_THREADS) reinterpret_cast<uint32_t *>(blob)[t] = __ldg(cv + t);
+            __syncthreads();
+            // the candidates' Hamming scores under c_v as sortable keys: 8 lanes per candidate, the walk's scorer and bits
+            for (int i = tid >> 3; i < cap; i += PRUNE_THREADS / 8) {
+                const int32_t c = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1;
+                long long kc = KEY_MIN;
+                if (c >= 0 && c != v) kc = topk_key(score_bq(P.d, blob, c, lane & 7), c);
+                if ((lane & 7) == 0) keys[i] = kc;
+            }
+        } else if (KIND == KIND_PQ) {
             pq_decode_row(P.d, v, newrow, tid, PRUNE_THREADS);
             __syncthreads();
             prepare_blob(P.d, P.metric, newrow, blob, red);
@@ -256,7 +286,10 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
                     sel_ids[nsel] = c;
                     if (BOUNDED) sel_ids[64 + nsel] = pick;  // degree <= 64: the second half holds the picks' sorted positions
                 }
-                if (KIND != KIND_PQ)
+                if constexpr (KIND == KIND_BQ) {
+                    const uint32_t *cw = reinterpret_cast<const uint32_t *>(P.d.words + (size_t)c * P.d.W);
+                    for (int t = tid; t < 2 * P.d.W; t += PRUNE_THREADS) reinterpret_cast<uint32_t *>(newrow)[t] = __ldg(cw + t);
+                } else if (KIND != KIND_PQ)
                     for (int t = tid; t < n4; t += PRUNE_THREADS) reinterpret_cast<float4 *>(newrow)[t] = __ldg(crow + t);
                 nsel++;
                 cursor = pick + 1;
@@ -266,7 +299,9 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
                 for (int i = warp; i < nvalid; i += NW) {
                     if (state[i] != 0) continue;
                     float ps;
-                    if (KIND == KIND_PQ) {
+                    if constexpr (KIND == KIND_BQ) {
+                        ps = pair_bq_row(P.d, key_node(keys[i]), reinterpret_cast<const unsigned long long *>(newrow), lane);
+                    } else if (KIND == KIND_PQ) {
                         ps = pair_pq_table<METRIC>(P.d, key_node(keys[i]), c, lane);
                     } else {
                         const float4 *row = reinterpret_cast<const float4 *>(P.d.rows + (size_t)key_node(keys[i]) * P.d.stride);
@@ -959,7 +994,8 @@ cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int 
     return cudaGetLastError();
 }
 
-// code rows [ids[i]] of a PQ data set gathered into a dense array (upper levels of a PQ build): one thread per 32-bit word
+// fixed-size rows [ids[i]] of a code array (PQ code rows, BQ word rows) gathered into a dense one (upper levels of a PQ or BQ build):
+// one thread per 32-bit word
 __global__ void __launch_bounds__(256) gather_codes_kernel(const uint32_t *__restrict__ codes, int words, const int32_t *__restrict__ ids, int count,
                                                            uint32_t *__restrict__ out)
 {
@@ -969,12 +1005,15 @@ __global__ void __launch_bounds__(256) gather_codes_kernel(const uint32_t *__res
     out[idx] = __ldg(codes + (size_t)ids[i] * words + w);
 }
 
-cudaError_t launch_gather_codes(const DataDesc &pq, const int32_t *ids_dev, int count, uint8_t *out_dev, cudaStream_t s)
+int code_row_bytes(const DataDesc &d) { return d.kind == KIND_BQ ? 8 * d.W : d.code_stride; }
+
+cudaError_t launch_gather_codes(const DataDesc &d, const int32_t *ids_dev, int count, void *out_dev, cudaStream_t s)
 {
     if (count <= 0) return cudaSuccess;
-    const int words = pq.code_stride >> 2;
+    const int words = code_row_bytes(d) >> 2;
+    const void *src = d.kind == KIND_BQ ? static_cast<const void *>(d.words) : static_cast<const void *>(d.codes);
     const long long total = (long long)count * words;
-    gather_codes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint32_t *>(pq.codes), words, ids_dev, count,
+    gather_codes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint32_t *>(src), words, ids_dev, count,
                                                                         reinterpret_cast<uint32_t *>(out_dev));
     g_launches++;
     return cudaGetLastError();
@@ -984,6 +1023,45 @@ cudaError_t launch_gather_codes(const DataDesc &pq, const int32_t *ids_dev, int 
 __global__ void __launch_bounds__(128) pq_decode_kernel(DataDesc d, int first, int count, float *out)
 {
     for (int i = blockIdx.x; i < count; i += gridDim.x) pq_decode_row(d, first + i, out + (size_t)i * d.dim, threadIdx.x, blockDim.x);
+}
+
+// the insert searches' queries of a BQ build: c_u as fp32, +1 where bit j is set and -1 where it is clear, j < dim. The BQ walk
+// re-encodes them (prepare_blob: v > 0) to exactly c_u when c_u has no bit set past dim (bq_padding_set).
+__global__ void __launch_bounds__(128) bq_decode_kernel(DataDesc d, int first, int count, float *out)
+{
+    for (int i = blockIdx.x; i < count; i += gridDim.x) {
+        const unsigned long long *w = d.words + (size_t)(first + i) * d.W;
+        for (int j = threadIdx.x; j < d.dim; j += blockDim.x) out[(size_t)i * d.dim + j] = (__ldg(w + (j >> 6)) >> (j & 63)) & 1ull ? 1.0f : -1.0f;
+    }
+}
+
+// whether some row of a BQ data set has a bit set past dim in its last word: one thread per row, the flags OR-ed into *any
+__global__ void __launch_bounds__(256) bq_padding_kernel(const unsigned long long *__restrict__ words, long long n, int W, unsigned long long pad_mask, int *any)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool set = r < n && (__ldg(words + (size_t)r * W + W - 1) & pad_mask) != 0;
+    if (__syncthreads_or(set) && threadIdx.x == 0) atomicOr(any, 1);
+}
+
+cudaError_t bq_padding_set(const DataDesc &bq, bool *set, cudaStream_t s)
+{
+    *set = false;
+    if ((bq.dim & 63) == 0) return cudaSuccess;
+    const unsigned long long pad_mask = ~0ull << (bq.dim & 63);
+    DeviceBuffer flag;
+    int h = 0;
+    cudaError_t e = flag.alloc(sizeof(int));
+    if (e == cudaSuccess) e = cudaMemsetAsync(flag.get(), 0, sizeof(int), s);
+    if (e == cudaSuccess) {
+        bq_padding_kernel<<<(unsigned)((bq.n + 255) / 256), 256, 0, s>>>(bq.words, bq.n, bq.W, pad_mask, flag.get<int>());
+        g_launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&h, flag.get(), sizeof(int), cudaMemcpyDeviceToHost, s);
+    const cudaError_t drained = cudaStreamSynchronize(s);  // the flag goes when this returns
+    if (e != cudaSuccess) return e;
+    *set = h != 0;
+    return drained;
 }
 
 static size_t prune_smem_bytes(const DataDesc &d, int maxc = PRUNE_MAXC)
@@ -1000,6 +1078,26 @@ static size_t prune_pq_smem_bytes(const DataDesc &d, int maxc)
 }
 
 bool pq_prune_fits(const DataDesc &pq) { return prune_pq_smem_bytes(pq, PRUNE_MAXC) <= (size_t)PRUNE_PQ_SMEM_MAX; }
+
+// the BQ prune's shared memory: c_v and the selected row's words, then the candidate state (13 B per slot). At most 2 * 128 words
+// (dim 8192) and 8192 slots: 111 KB, so every call fits
+static size_t prune_bq_smem_bytes(const DataDesc &d, int maxc)
+{
+    size_t b = (size_t)bq_row_floats(d) * 4 * 2 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
+    return (b + 15) & ~(size_t)15;
+}
+
+// the one BQ prune instantiation (its scores do not depend on the metric) at capacity MAXC
+template <int MAXC>
+static cudaError_t launch_prune_bq(const PruneParams &P, int grid, cudaStream_t s)
+{
+    const size_t sm = prune_bq_smem_bytes(P.d, MAXC);
+    const cudaError_t e = cudaFuncSetAttribute(prune_kernel<JV_METRIC_DOT, MAXC, KIND_BQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    if (e != cudaSuccess) return e;
+    prune_kernel<JV_METRIC_DOT, MAXC, KIND_BQ><<<grid, PRUNE_THREADS, sm, s>>>(P);
+    g_launches++;
+    return cudaGetLastError();
+}
 
 // PQ: no Gram tier (it would change the pair bits); the incremental kernel at the smallest capacity that holds the candidates
 template <int METRIC>
@@ -1056,6 +1154,13 @@ static cudaError_t launch_prune_t(const PruneParams &P, int grid, size_t smem, c
 
 static cudaError_t launch_prune(const PruneParams &P, int grid, size_t smem, cudaStream_t s)
 {
+    if (P.d.kind == KIND_BQ) {
+        // BQ: no Gram tier, every metric on the one instantiation, at the smallest capacity that holds the candidates
+        const int ncmax = P.mode == 0 ? P.cand_stride + P.window : P.row_cap;
+        if (ncmax <= 64) return launch_prune_bq<64>(P, grid, s);
+        if (ncmax <= 128) return launch_prune_bq<128>(P, grid, s);
+        return launch_prune_bq<256>(P, grid, s);
+    }
     if (P.metric == JV_METRIC_EUCLIDEAN) return launch_prune_t<JV_METRIC_EUCLIDEAN>(P, grid, smem, s);
     if (P.metric == JV_METRIC_DOT) return launch_prune_t<JV_METRIC_DOT>(P, grid, smem, s);
     return launch_prune_t<JV_METRIC_COSINE>(P, grid, smem, s);
@@ -1091,7 +1196,7 @@ struct GraphBuilder {
     size_t cub_bytes = 0;
     int32_t *own_rows = nullptr;  // single-GPU path: the slice buffers are the builder's own
     int *own_deg = nullptr;
-    float *qdec = nullptr;        // PQ: the insert searches' queries decode(c_u), [max_batch][dim]
+    float *qdec = nullptr;        // PQ / BQ: the insert searches' queries decode(c_u) / c_u as +-1, [max_batch][dim]
     std::vector<DeviceBuffer> mem;  // owns every block above
     DeviceBuffer scratch;           // the insert searches' scratch, grown with the slice
     BuildStats st = {0, 0, 0, 0, 0};
@@ -1105,7 +1210,7 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
                            const BuilderSeed *seed)
 {
     const int n = (int)d.n;
-    if ((d.kind != KIND_F32 && d.kind != KIND_PQ) || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
+    if ((d.kind != KIND_F32 && d.kind != KIND_PQ && d.kind != KIND_BQ) || bp.degree < 1 || bp.degree > 64 || bp.beam < 1 || bp.beam > PRUNE_MAXC) return cudaErrorInvalidValue;
     // PQ: with the centroid-pair table of this metric (jv_dataset_pq_pair_table) and a LUT the prune can hold
     if (d.kind == KIND_PQ && (!d.pair_table[metric == JV_METRIC_EUCLIDEAN ? 0 : 1] || !pq_prune_fits(d))) return cudaErrorInvalidValue;
     if (seed && (seed->count < 0 || seed->count > n || (seed->count > 0 && (!seed->rows_dev || seed->width < 1)) || seed->entry >= seed->count))
@@ -1143,7 +1248,7 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
     JV_TRY(alloc_owned(owned, B->head_target, mb * B->degree * 4));
     JV_TRY(alloc_owned(owned, B->own_rows, mb * B->degree * 4));
     JV_TRY(alloc_owned(owned, B->own_deg, mb * 4));
-    if (d.kind == KIND_PQ) JV_TRY(alloc_owned(owned, B->qdec, mb * d.dim * 4));
+    if (d.kind == KIND_PQ || d.kind == KIND_BQ) JV_TRY(alloc_owned(owned, B->qdec, mb * d.dim * 4));
     {
         size_t b1 = 0, b2 = 0;
         cub::DeviceRadixSort::SortKeys(nullptr, b1, B->pairs, B->pairs_sorted, (int)(mb * B->degree), 0, 64, s);
@@ -1225,6 +1330,13 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
     if (B->d.kind == KIND_PQ) {
         // searchProviderFor over PQ: the walk scores with the codes only (no rerank), its query is decode(c_u)
         pq_decode_kernel<<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, B->qdec);
+        g_launches++;
+        JV_TRY(cudaGetLastError());
+        queries = B->qdec;
+        query_stride = B->d.dim;
+    } else if (B->d.kind == KIND_BQ) {
+        // searchProviderFor over BQ: the walk scores with the words only (no rerank), its query encodes to c_u
+        bq_decode_kernel<<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, B->qdec);
         g_launches++;
         JV_TRY(cudaGetLastError());
         queries = B->qdec;
@@ -1364,7 +1476,8 @@ cudaError_t build_graph_flat(const DataDesc &d, int metric, const BuildParams &b
 //   gather : one CTA per flagged row writes its live neighbours, the live 2-hop ids through its deleted neighbours (the FreshDiskANN
 //            rule, :705-721) — or, when there are no such ids, random live members of the level (:743-759) — sorted and deduplicated
 //   prune  : the builder's prune kernels (mode 2, ragged candidates, out of place), dispatched by candidate count so no set is clipped;
-//            over a PQ data set the PQ prune at every tier, with the scores of the PQ build (query decode(c_v), ADC keys, pair table)
+//            over a PQ data set the PQ prune at every tier, with the scores of the PQ build (query decode(c_v), ADC keys, pair table);
+//            over a BQ data set the BQ prune at every tier, with Hamming scores
 //   scatter: the pruned rows replace the old ones in the output adjacency
 // Nothing depends on timing: compaction and offsets come from cub scans, the dedup from a sort, and the prune is deterministic.
 // ------------------------------------------------------------------------------------------------
@@ -1522,20 +1635,20 @@ cudaError_t launch_clear_dead_rows(int32_t *adj_dev, int n, int degree, const ui
 // the prune tiers of the repair: TILE-candidate Gram kernels on the tensor cores, then the incremental kernel at growing capacity
 constexpr int REPAIR_TIERS = 5;
 constexpr int REPAIR_TIER_MAX[REPAIR_TIERS] = {64, 128, 256, 1024, 8192};
-// over a PQ data set (§4.3e) there is no Gram tier — it would change the pair bits — and every tier is prune_kernel<.., KIND_PQ>. The
-// candidate state (13 B per slot) shares the CTA's shared memory with the whole LUT, so 2048 sits between 1024 and 8192: a degree-32
-// row has at most 32 * 34 = 1088 candidates and never pays for 8192 slots (106 KB)
-constexpr int PQ_REPAIR_TIERS = 6;
-constexpr int PQ_REPAIR_TIER_MAX[PQ_REPAIR_TIERS] = {64, 128, 256, 1024, 2048, 8192};
-static_assert(PQ_REPAIR_TIERS <= (int)(sizeof(RepairStats::tier_rows) / sizeof(long long)), "RepairStats::tier_rows holds every tier");
+// over a PQ data set (§4.3e) or a BQ data set (§4.3g) there is no Gram tier — it would change the pair bits — and every tier is
+// prune_kernel<.., KIND_PQ> or <.., KIND_BQ>. The candidate state (13 B per slot) shares the CTA's shared memory with the whole LUT
+// (PQ), so 2048 sits between 1024 and 8192: a degree-32 row has at most 32 * 34 = 1088 candidates and never pays for 8192 slots (106 KB)
+constexpr int CODE_REPAIR_TIERS = 6;
+constexpr int CODE_REPAIR_TIER_MAX[CODE_REPAIR_TIERS] = {64, 128, 256, 1024, 2048, 8192};
+static_assert(CODE_REPAIR_TIERS <= (int)(sizeof(RepairStats::tier_rows) / sizeof(long long)), "RepairStats::tier_rows holds every tier");
 
 // whether the repair of a degree-`degree` graph over `pq` can run: a row gathers up to degree * (degree + 2) candidates, and the tier
 // that holds them must fit next to the LUT
 bool pq_repair_fits(const DataDesc &pq, int degree)
 {
     int t = 0;
-    while (t < PQ_REPAIR_TIERS - 1 && degree * (degree + 2) > PQ_REPAIR_TIER_MAX[t]) t++;
-    return prune_pq_smem_bytes(pq, PQ_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
+    while (t < CODE_REPAIR_TIERS - 1 && degree * (degree + 2) > CODE_REPAIR_TIER_MAX[t]) t++;
+    return prune_pq_smem_bytes(pq, CODE_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
 }
 
 template <int METRIC>
@@ -1573,6 +1686,16 @@ static cudaError_t launch_repair_prune_t(const PruneParams &P, int tier, int gri
 
 static cudaError_t launch_repair_prune(const PruneParams &P, int tier, int grid, cudaStream_t s)
 {
+    if (P.d.kind == KIND_BQ) {
+        switch (tier) {
+        case 0: return launch_prune_bq<64>(P, grid, s);
+        case 1: return launch_prune_bq<128>(P, grid, s);
+        case 2: return launch_prune_bq<256>(P, grid, s);
+        case 3: return launch_prune_bq<1024>(P, grid, s);
+        case 4: return launch_prune_bq<2048>(P, grid, s);
+        default: return launch_prune_bq<8192>(P, grid, s);
+        }
+    }
     if (P.metric == JV_METRIC_EUCLIDEAN) return launch_repair_prune_t<JV_METRIC_EUCLIDEAN>(P, tier, grid, s);
     if (P.metric == JV_METRIC_DOT) return launch_repair_prune_t<JV_METRIC_DOT>(P, tier, grid, s);
     return launch_repair_prune_t<JV_METRIC_COSINE>(P, tier, grid, s);
@@ -1643,9 +1766,10 @@ static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alp
     JV_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)naff * 4, cudaMemcpyDeviceToHost, s));
     JV_TRY(cudaMemcpyAsync(hfb.data(), fallback, (size_t)naff, cudaMemcpyDeviceToHost, s));
     JV_TRY(cudaStreamSynchronize(s));
-    const int ntiers = d.kind == KIND_PQ ? PQ_REPAIR_TIERS : REPAIR_TIERS;
-    const int *tier_max = d.kind == KIND_PQ ? PQ_REPAIR_TIER_MAX : REPAIR_TIER_MAX;
-    std::vector<int32_t> tiers[PQ_REPAIR_TIERS];
+    const bool codes = d.kind == KIND_PQ || d.kind == KIND_BQ;
+    const int ntiers = codes ? CODE_REPAIR_TIERS : REPAIR_TIERS;
+    const int *tier_max = codes ? CODE_REPAIR_TIER_MAX : REPAIR_TIER_MAX;
+    std::vector<int32_t> tiers[CODE_REPAIR_TIERS];
     for (int a = 0; a < naff; a++) {
         int t = 0;
         while (t < ntiers - 1 && hcnt[a] > tier_max[t]) t++;
@@ -1685,7 +1809,7 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
                          int sm_count, RepairStats *st, cudaStream_t s)
 {
     if (rows <= 0) return cudaSuccess;
-    if (degree < 1 || degree > 64 || (d.kind != KIND_F32 && d.kind != KIND_PQ)) return cudaErrorInvalidValue;
+    if (degree < 1 || degree > 64 || (d.kind != KIND_F32 && d.kind != KIND_PQ && d.kind != KIND_BQ)) return cudaErrorInvalidValue;
     if (d.kind == KIND_PQ && (!d.pair_table[metric == JV_METRIC_EUCLIDEAN ? 0 : 1] || !pq_repair_fits(d, degree))) return cudaErrorInvalidValue;
     std::vector<DeviceBuffer> mem;  // the scratch goes when this returns: the stream drains first, on success and on error
     const cudaError_t err = repair_level_enqueue(d, metric, alpha, degree, rows, adj_old, adj_new, ids_dev, rowmap_dev, dead_dev, members_dev, nmembers,

@@ -166,8 +166,8 @@ struct BuilderSeed {
     int32_t entry;
     const uint32_t *accept;
 };
-// flat Vamana graph over rows [0, n) of an f32 data set, or of a PQ data set that carries the metric's pair table
-// (pqBuildScoreProvider); adj_out_dev [n][degree] (-1 padded); entry node is 0 (or the seed's)
+// flat Vamana graph over rows [0, n) of an f32 data set, of a PQ data set that carries the metric's pair table
+// (pqBuildScoreProvider), or of a BQ data set (bqBuildScoreProvider); adj_out_dev [n][degree] (-1 padded); entry node is 0 (or the seed's)
 cudaError_t build_graph_flat(const DataDesc &f32, int metric, const BuildParams &bp, int32_t *adj_out_dev, int sm_count,
                              BuildStats *stats, cudaStream_t s, const BuilderSeed *seed = nullptr);
 // the same build advanced batch by batch; a sharded build calls the *_slice functions for its part of each batch and moves the
@@ -189,21 +189,25 @@ int builder_row_cap(const GraphBuilder *B);
 int builder_degree(const GraphBuilder *B);
 int builder_max_batch(const GraphBuilder *B);
 cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s);
-// PQ build (pqBuildScoreProvider): code rows [ids[i]] into out_dev [count][code_stride]; whether the PQ prune holds the data set's LUT
-cudaError_t launch_gather_codes(const DataDesc &pq, const int32_t *ids_dev, int count, uint8_t *out_dev, cudaStream_t s);
+// PQ / BQ build (pqBuildScoreProvider, bqBuildScoreProvider): the fixed-size rows [ids[i]] of the code array (PQ code rows, BQ word rows,
+// code_row_bytes each) into out_dev [count][code_row_bytes]; whether the PQ prune holds the data set's LUT
+int code_row_bytes(const DataDesc &d);
+cudaError_t launch_gather_codes(const DataDesc &d, const int32_t *ids_dev, int count, void *out_dev, cudaStream_t s);
 bool pq_prune_fits(const DataDesc &pq);
+// whether some row of a BQ data set has a bit set past dim (one reduction over the last word of every row; synchronises `s`)
+cudaError_t bq_padding_set(const DataDesc &bq, bool *set, cudaStream_t s);
 // whether the repair's PQ prune holds the LUT next to the largest candidate set a degree-`degree` row can gather
 bool pq_repair_fits(const DataDesc &pq, int degree);
 
-// removeDeletedNodes on one level (see build.cu), over an fp32 data set or a PQ data set that carries the metric's pair table and
-// passes pq_repair_fits. rows: members of the level; row r is node ids_dev[r] (nullptr: node r, level 0);
+// removeDeletedNodes on one level (see build.cu), over an fp32 data set, a PQ data set that carries the metric's pair table and
+// passes pq_repair_fits, or a BQ data set. rows: members of the level; row r is node ids_dev[r] (nullptr: node r, level 0);
 // rowmap_dev[node] = the node's row on this level (nullptr: identity). dead_dev: bitset of deleted nodes (bit node & 31 of word
 // node >> 5). members_dev: the level's live members, ascending (random fallback). adj_new must hold a copy of adj_old: the repaired
 // rows are written into it, every other row is left as it is. Synchronises `s`.
 struct RepairStats {
     long long repaired_rows, candidates, random_fallbacks;
     int max_candidates;
-    // fp32: rows pruned with <= 64, <= 128, <= 256, <= 1024, more candidates; PQ: <= 64, <= 128, <= 256, <= 1024, <= 2048, more
+    // fp32: rows pruned with <= 64, <= 128, <= 256, <= 1024, more candidates; PQ, BQ: <= 64, <= 128, <= 256, <= 1024, <= 2048, more
     long long tier_rows[6];
 };
 cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new, const int32_t *ids_dev,

@@ -173,21 +173,21 @@ def sharded_build(dist, vectors, vsf, M=32, beamWidth=100, neighborOverflow=1.2,
     runs the beam searches + robust prunes of ITS slice (jv_builder_insert_slice), ONE all-gather moves the new rows, every rank
     applies the whole batch (sorted back-links: the replicas stay bit-identical), then the rows that passed overflow * M are re-pruned
     slice-wise and all-gathered the same way. NCCL calls and kernels share torch's current stream. dist = None: one rank (the
-    same code path, no collective). `vectors` may be PQVectors instead (pqBuildScoreProvider: jv_builder_create_pq). Returns
-    (GraphIndex, device_ms, exchanged_bytes)."""
+    same code path, no collective). `vectors` may be PQVectors instead (pqBuildScoreProvider: jv_builder_create_pq) or BQVectors
+    (bqBuildScoreProvider: jv_builder_create_bq). Returns (GraphIndex, device_ms, exchanged_bytes)."""
     import ctypes as C
 
     import torch
 
     from . import _native as nat
-    from .api import GraphIndex, PQVectors
+    from .api import BQVectors, GraphIndex, PQVectors
     lib = nat.init()
     world = dist.get_world_size() if dist is not None and dist.is_initialized() else 1
     rank = dist.get_rank() if world > 1 else 0
     params = nat.BuildParams(M, beamWidth, neighborOverflow, alpha, 1 if addHierarchy else 0, seed, max_batch, concurrent_window)
     st = torch.cuda.current_stream().cuda_stream
     b = C.c_void_p()
-    create = lib.jv_builder_create_pq if isinstance(vectors, PQVectors) else lib.jv_builder_create
+    create = lib.jv_builder_create_pq if isinstance(vectors, PQVectors) else lib.jv_builder_create_bq if isinstance(vectors, BQVectors) else lib.jv_builder_create
     nat.check(create(vectors._h, int(vsf), C.byref(params), C.c_void_p(st), C.byref(b)))
     deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
     nat.check(lib.jv_builder_info(b, C.byref(deg_), C.byref(cap_), C.byref(mb_)))
