@@ -4,6 +4,7 @@ bench.py's cpu_baseline / --impl reference legs."""
 import ctypes as C
 import os
 import subprocess
+from fractions import Fraction
 
 import numpy as np
 
@@ -279,6 +280,72 @@ def train_pq_numpy(rng, data, M, k=256, iters=6):
             cent[nz] = sums[nz] / cnt[nz, None]
         out[k * offsets[m]: k * (offsets[m] + sizes[m])] = cent.reshape(-1)
     return out, sizes, offsets
+
+
+# ---------------------------------------------------------------------------------------------
+# exact fp32 restatements of the PQ kernels' fused chains (the oracle's own tables use separate multiply and add)
+# ---------------------------------------------------------------------------------------------
+def fma_f32(a, b, c):
+    """fmaf(a, b, c) elementwise with one rounding. The float64 product of two floats is exact and the float64 sum rounds once;
+    rounding that sum to float32 again gives fmaf's answer unless the sum is exactly halfway between two floats, and those entries
+    are decided on the exact rational value."""
+    a, b, c = np.broadcast_arrays(np.asarray(a, np.float32), np.asarray(b, np.float32), np.asarray(c, np.float32))
+    s = a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64)
+    r = s.astype(np.float32)
+    up, dn = np.nextafter(r, np.float32(np.inf)), np.nextafter(r, np.float32(-np.inf))
+    half_up = (r.astype(np.float64) + up.astype(np.float64)) / 2
+    half_dn = (r.astype(np.float64) + dn.astype(np.float64)) / 2
+    for i in zip(*np.nonzero(np.isfinite(s) & ((s == half_up) | (s == half_dn)))):
+        exact = Fraction(float(a[i])) * Fraction(float(b[i])) + Fraction(float(c[i]))
+        mid = Fraction(float(s[i]))
+        if exact != mid:  # off the midpoint: the float on exact's side of it
+            other = up[i] if s[i] == half_up[i] else dn[i]
+            lo, hi = sorted((r[i], other))
+            r[i] = hi if exact > mid else lo
+    return r
+
+
+def pq_lut_exact(codebooks, dim, M, k, centroid, q, metric):
+    """prepare_blob's PQ partial sums (scorers.cuh): entry m * k + c is one sequential fmaf chain over sub-space m of
+    (centroid_c - q') squared (EUCLIDEAN) or centroid_c * q' (otherwise), q' = q - global centroid rounded once"""
+    sizes, offsets = pq_layout(dim, M)
+    q = np.asarray(q, np.float32)
+    qc = (q - np.asarray(centroid, np.float32)).astype(np.float32) if centroid is not None else q
+    out = np.empty(M * k, np.float32)
+    for m in range(M):
+        sz, off = int(sizes[m]), int(offsets[m])
+        cb = np.asarray(codebooks, np.float32)[k * off:k * (off + sz)].reshape(k, sz)
+        s = np.zeros(k, np.float32)
+        for j in range(sz):
+            if metric == EUCLIDEAN:
+                df = (cb[:, j] - qc[off + j]).astype(np.float32)
+                s = fma_f32(df, df, s)
+            else:
+                s = fma_f32(cb[:, j], qc[off + j], s)
+        out[m * k:(m + 1) * k] = s
+    return out
+
+
+def pq_pair_table_exact(codebooks, dim, M, k, metric):
+    """pq_pair_table_kernel (kernels_batch.cu): per sub-space the upper triangle i <= j in row order, each entry one sequential
+    fmaf chain of (x - y) squared (EUCLIDEAN) or x * y (otherwise) over centroids x = i, y = j"""
+    sizes, offsets = pq_layout(dim, M)
+    iu, ju = np.triu_indices(k)
+    block = k * (k + 1) // 2
+    out = np.empty(M * block, np.float32)
+    for m in range(M):
+        sz, off = int(sizes[m]), int(offsets[m])
+        cb = np.asarray(codebooks, np.float32)[k * off:k * (off + sz)].reshape(k, sz)
+        x, y = cb[iu], cb[ju]
+        s = np.zeros(block, np.float32)
+        for j in range(sz):
+            if metric == EUCLIDEAN:
+                df = (x[:, j] - y[:, j]).astype(np.float32)
+                s = fma_f32(df, df, s)
+            else:
+                s = fma_f32(x[:, j], y[:, j], s)
+        out[m * block:(m + 1) * block] = s
+    return out
 
 
 def encode_pq(L, codebooks, sizes, offsets, M, k, centroid, data):

@@ -203,23 +203,41 @@ MODEL_CASES = [
 ]
 
 
+def exact_table(pqv, codebooks, dim, k, metric):
+    """the centroid-pair table of the metric computed on the host (pq_pair_table_kernel's fmaf chains), asserted equal to the one the
+    device holds, bit for bit: the models then score pairs with a table that does not come from the device"""
+    table = o.pq_pair_table_exact(codebooks, dim, pqv.M, k, metric)
+    got = pqv.pair_table(metric)
+    bad = np.flatnonzero(got.view(np.int32) != table.view(np.int32))
+    assert len(bad) == 0, ("device pair table differs from the host's", dim, pqv.M, k, metric, len(bad), bad[:5].tolist())
+    return table
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", MODEL_CASES, ids=[c[0] for c in MODEL_CASES])
 def test_device_pq_build_equals_model(jv, oracle, case):
+    cid, dim, Mq, centroid, metric, M, beam, window, max_batch, hier, n = case
+    _, codes, codebooks, cen = real_pq_world(cid, n, dim, Mq, centroid)
+    pqv = jv.PQVectors(codes, codebooks, dim, 256, cen)
+    drive_build_pq(jv, oracle, pqv, (codes, codebooks, cen, dim, 256), metric, M, beam, window, max_batch, hier, cid)
+    pqv.close()
+
+
+def drive_build_pq(jv, oracle, pqv, world, metric, M, beam, window, max_batch, hier, cid):
+    """the build over pqv driven step by step (jv_builder_create_pq + jv_builder_*): each batch's inserted rows, overflow list and
+    re-pruned rows equal PQBuildModel's exactly, then the counters, the finished adjacency and the upper levels"""
     import torch
 
     from jvector_b200 import _native as nat
-    cid, dim, Mq, centroid, metric, M, beam, window, max_batch, hier, n = case
-    k = 256
-    _, codes, codebooks, cen = real_pq_world(cid, n, dim, Mq, centroid)
+    codes, codebooks, cen, dim, k = world
+    n = codes.shape[0]
     lib = nat.init()
-    pqv = jv.PQVectors(codes, codebooks, dim, k, cen)
     seed = 3
     params = nat.BuildParams(M, beam, 1.2, 1.2, int(hier), seed, max_batch, window)
     st = torch.cuda.current_stream().cuda_stream
     b = C.c_void_p()
     nat.check(lib.jv_builder_create_pq(pqv._h, metric, C.byref(params), C.c_void_p(st), C.byref(b)))
-    table = pqv.pair_table(metric)  # the table the builder made, as the device holds it
+    table = exact_table(pqv, codebooks, dim, k, metric)  # the builder made the device's table
     kw = dict(M=M, beam=beam, overflow=1.2, alpha=1.2, max_batch=max_batch, window=window)
     model = pm.PQBuildModel(oracle, codes, codebooks, k, dim, cen, table, metric, **kw)
     deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
@@ -281,7 +299,6 @@ def test_device_pq_build_equals_model(jv, oracle, case):
             gids, gadj = gi.level(lv)
             assert np.array_equal(gids, ids) and np.array_equal(gadj, want_adj), (cid, "level", lv)
     gi.close()
-    pqv.close()
 
 
 @pytest.mark.gpu

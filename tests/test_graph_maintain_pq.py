@@ -20,7 +20,7 @@ import oracle_lib as o
 import pq_build_model as pm
 import pq_maintain_model as mm
 from oracle_lib import fp, ip
-from test_graph_build_pq import assert_same_graph, host_table, lossless_world, real_pq_world
+from test_graph_build_pq import assert_same_graph, exact_table, host_table, lossless_world, real_pq_world
 
 METRICS = (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)
 
@@ -220,7 +220,7 @@ def drive_add_pq(jv, oracle, pqv, world, g, metric, M, beam, window, max_batch, 
     st = torch.cuda.current_stream().cuda_stream
     b = C.c_void_p()
     nat.check(lib.jv_builder_create_from_graph_pq(g._h, pqv._h, metric, C.byref(params), _bptr(bits), C.c_void_p(st), C.byref(b)))
-    table = pqv.pair_table(metric)
+    table = exact_table(pqv, codebooks, dim, k, metric)
     kw = dict(M=M, beam=beam, overflow=1.2, alpha=1.2, max_batch=max_batch, window=window)
     accept = None if marks is None else np.concatenate([~marks, np.ones(n - n0, bool)])
     model = mm.SeededPQBuildModel(oracle, codes, codebooks, k, dim, cen, table, metric, levels0[0][1], entry0, accept, **kw)
@@ -389,7 +389,7 @@ def test_pq_removal_equals_model(jv, oracle, case):
     deleted[entry] = kill_entry
     got, again = b.removeDeletedNodes(g, pqv, deleted), b.removeDeletedNodes(g, pqv, deleted)
     assert_same_graph(got, again, (cid, "two calls"))
-    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, pqv.pair_table(metric), metric, M)
+    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, metric), metric, M)
     res = model.remove_deleted(levels[0][1], entry, levels[1:], deleted, seed=17)
     hit = assert_removal_matches_model(got, res, cid)
     print(cid, "rows per tier", hit.tolist(), got.remove_stats)
@@ -432,7 +432,7 @@ def test_pq_removal_hits_every_tier_on_a_made_graph(jv, oracle):
     g = jv.GraphIndex(adj, 0)
     b = _builder(jv, o.DOT_PRODUCT, M, seed=5)
     got = b.removeDeletedNodes(g, pqv, deleted)
-    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, pqv.pair_table(o.DOT_PRODUCT), o.DOT_PRODUCT, M)
+    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, o.DOT_PRODUCT), o.DOT_PRODUCT, M)
     res = model.remove_deleted(adj, 0, [], deleted, seed=5)
     hit = assert_removal_matches_model(got, res, "made graph")
     print("made graph: rows per tier", hit.tolist(), got.remove_stats)
@@ -453,7 +453,7 @@ def test_pq_removal_fallback_and_everything_deleted(jv, oracle):
     deleted = np.ones(n, bool)
     deleted[rng.choice(n, 50, replace=False)] = False
     got = b.removeDeletedNodes(g, pqv, deleted)
-    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, pqv.pair_table(o.EUCLIDEAN), o.EUCLIDEAN, M)
+    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, o.EUCLIDEAN), o.EUCLIDEAN, M)
     res = model.remove_deleted(levels[0][1], entry, levels[1:], deleted, seed=12)
     assert_removal_matches_model(got, res, "fallback")
     assert got.remove_stats["random_fallbacks"] > 0
