@@ -1587,77 +1587,68 @@ static int graph_build(jv_dataset ds, int metric, const jv_build_params *params,
     return JV_OK;
 }
 
-int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
+// the requirements of a build, add or removal over a data set of `kind` (fp32 rows, PQ codes: pqBuildScoreProvider, BQ words:
+// bqBuildScoreProvider), in this order: the kind; the metric (checked as every call checks it; no BQ score uses it); a row the
+// builder and the prune handle (the graph's degree for an add or a removal, params->degree for a build over codes; an fp32 build
+// leaves it to build_params_check); with params (build and add) the build parameters; over PQ a LUT the prune holds next to its
+// candidates (the builder's, or with params == nullptr the removal's tier), then the metric's centroid-pair table, built and kept
+// on the data set when it has none (as jv_dataset_pq_pair_table does); over BQ no bit set past dim. Every refusal comes before any
+// device work except the BQ padding check, one reduction over the last word of every row (bq_padding_set).
+static int provider_check(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, BuildParams *bp, const char *who)
 {
-    ON_DEVICE_OF(f32);
-    if (!f32 || !params || !out || f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "graph_build: needs an fp32 data set");
-    int rc = check_metric(f32->d, metric);
+    const std::string w(who);
+    if (ds->d.kind != kind)
+        return fail(JV_ERR_INVALID, w + (kind == KIND_PQ ? ": needs a PQ data set" : kind == KIND_BQ ? ": needs a BQ data set" : ": needs an fp32 data set"));
+    int rc = check_metric(ds->d, metric);
     if (rc) return rc;
-    if ((rc = t_ctx.init())) return rc;
-    BuildParams bp;
-    if ((rc = build_params_check(params, &bp))) return rc;
-    return graph_build(f32, metric, params, bp, out, device_ms);
+    const int degree = g ? g->g.degree : params->degree;
+    if (degree > 64 && (g || kind != KIND_F32))
+        return fail(JV_ERR_UNSUPPORTED, w + ": degree " + std::to_string(degree) + " > 64, the largest row the builder and the prune handle");
+    if (params) {
+        if (g && params->degree != degree) return fail(JV_ERR_INVALID, w + ": params->degree differs from the graph's degree");
+        if ((rc = build_params_check(params, bp))) return rc;
+    }
+    if (kind == KIND_PQ) {
+        if (!(params ? pq_prune_fits(ds->d) : pq_repair_fits(ds->d, degree)))
+            return fail(JV_ERR_UNSUPPORTED, w + ": a LUT of M * k = " + std::to_string(ds->d.M * ds->d.k) +
+                                                " entries does not fit the prune's shared memory next to its candidates (DESIGN §4.3c, §4.3e)");
+        return jv_dataset_pq_pair_table(ds, metric);
+    }
+    if (kind == KIND_BQ) {
+        // the walk re-encodes its query with the bits past dim clear while the prune's pair scores read the raw words, so the two
+        // would disagree on Hamming distances. BinaryQuantization.encode and jv_bq_encode_* never set them.
+        if ((rc = t_ctx.init())) return rc;
+        bool set = false;
+        CK(bq_padding_set(ds->d, &set, t_ctx.stream), "bq padding check");
+        if (set) return fail(JV_ERR_INVALID, w + ": a row of the BQ data set has bits set past dim " + std::to_string(ds->d.dim));
+    }
+    return JV_OK;
 }
 
-// the checks of a build over PQ codes (pqBuildScoreProvider), and the centroid-pair table of the metric, built and kept on the data
-// set when it has none yet (as jv_dataset_pq_pair_table does)
-static int pq_build_check(jv_dataset pq, int metric, const jv_build_params *params, BuildParams *bp)
+// jv_graph_build (kind = KIND_F32), jv_graph_build_pq (KIND_PQ) and jv_graph_build_bq (KIND_BQ)
+static int graph_build_of(jv_dataset ds, int kind, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
 {
-    if (pq->d.kind != KIND_PQ) return fail(JV_ERR_INVALID, "graph_build_pq: needs a PQ data set");
-    int rc = check_metric(pq->d, metric);
+    ON_DEVICE_OF(ds);
+    if (!params || !out) return fail(JV_ERR_INVALID, "graph_build: null argument");
+    BuildParams bp;
+    const int rc = provider_check(nullptr, ds, kind, metric, params, &bp, "graph_build");
     if (rc) return rc;
-    if (params->degree > 64)
-        return fail(JV_ERR_UNSUPPORTED, "graph_build_pq: degree " + std::to_string(params->degree) + " > 64, the largest row the builder handles");
-    if ((rc = build_params_check(params, bp))) return rc;
-    if (!pq_prune_fits(pq->d))
-        return fail(JV_ERR_UNSUPPORTED, "graph_build_pq: a LUT of M * k = " + std::to_string(pq->d.M * pq->d.k) +
-                                            " entries does not fit the prune's shared memory next to its candidates (DESIGN §4.3c)");
-    return jv_dataset_pq_pair_table(pq, metric);
+    return graph_build(ds, metric, params, bp, out, device_ms);
+}
+
+int jv_graph_build(jv_dataset f32, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
+{
+    return graph_build_of(f32, KIND_F32, metric, params, out, device_ms);
 }
 
 int jv_graph_build_pq(jv_dataset pq, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
 {
-    ON_DEVICE_OF(pq);
-    if (!params || !out) return fail(JV_ERR_INVALID, "graph_build_pq: null argument");
-    BuildParams bp;
-    const int rc = pq_build_check(pq, metric, params, &bp);
-    if (rc) return rc;
-    return graph_build(pq, metric, params, bp, out, device_ms);
-}
-
-// a BQ data set whose rows set a bit past dim: the walk re-encodes its query with those bits clear while the prune's pair scores
-// read the raw words, so the two would disagree on Hamming distances. BinaryQuantization.encode and jv_bq_encode_* never set them.
-// One reduction over the last word of every row, the first device work of the call.
-static int bq_padding_check(jv_dataset bq, const char *who)
-{
-    int rc;
-    if ((rc = t_ctx.init())) return rc;
-    bool set = false;
-    CK(bq_padding_set(bq->d, &set, t_ctx.stream), "bq padding check");
-    if (set) return fail(JV_ERR_INVALID, std::string(who) + ": a row of the BQ data set has bits set past dim " + std::to_string(bq->d.dim));
-    return JV_OK;
-}
-
-// the checks of a build over BQ codes (bqBuildScoreProvider). The metric is checked as every call checks it, and no score uses it.
-static int bq_build_check(jv_dataset bq, int metric, const jv_build_params *params, BuildParams *bp)
-{
-    if (bq->d.kind != KIND_BQ) return fail(JV_ERR_INVALID, "graph_build_bq: needs a BQ data set");
-    int rc = check_metric(bq->d, metric);
-    if (rc) return rc;
-    if (params->degree > 64)
-        return fail(JV_ERR_UNSUPPORTED, "graph_build_bq: degree " + std::to_string(params->degree) + " > 64, the largest row the builder handles");
-    if ((rc = build_params_check(params, bp))) return rc;
-    return bq_padding_check(bq, "graph_build_bq");
+    return graph_build_of(pq, KIND_PQ, metric, params, out, device_ms);
 }
 
 int jv_graph_build_bq(jv_dataset bq, int metric, const jv_build_params *params, jv_graph *out, double *device_ms)
 {
-    ON_DEVICE_OF(bq);
-    if (!params || !out) return fail(JV_ERR_INVALID, "graph_build_bq: null argument");
-    BuildParams bp;
-    const int rc = bq_build_check(bq, metric, params, &bp);
-    if (rc) return rc;
-    return graph_build(bq, metric, params, bp, out, device_ms);
+    return graph_build_of(bq, KIND_BQ, metric, params, out, device_ms);
 }
 
 static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bits[(size_t)v >> 5] >> (v & 31)) & 1u; }
@@ -1687,26 +1678,13 @@ static std::vector<uint32_t> add_accept_bits(const GraphAdd &A, const int32_t *i
 }
 
 // the checks of an add over a data set of `kind` (KIND_F32: jv_graph_add_nodes, KIND_PQ: jv_graph_add_nodes_pq, KIND_BQ:
-// jv_graph_add_nodes_bq). Over PQ also those of the PQ build: a LUT the prune can hold, and the metric's centroid-pair table, built and
-// kept on the data set when it has none. Over BQ also the BQ build's: no bit set past dim.
+// jv_graph_add_nodes_bq)
 static int add_check(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, BuildParams *bp)
 {
     if (!ds || !params) return fail(JV_ERR_INVALID, "add_nodes: null argument");
-    if (ds->d.kind != kind)
-        return fail(JV_ERR_INVALID, kind == KIND_PQ ? "add_nodes_pq: needs a PQ data set" : kind == KIND_BQ ? "add_nodes_bq: needs a BQ data set" : "add_nodes: needs an fp32 data set");
     if (ds->device != g->device) return fail(JV_ERR_INVALID, "add_nodes: data set and graph live on different devices");
     if (ds->d.n < g->g.n || ds->d.n > INT32_MAX) return fail(JV_ERR_INVALID, "add_nodes: the data set must hold the graph's nodes first");
-    int rc = check_metric(ds->d, metric);
-    if (rc) return rc;
-    if (g->g.degree > 64)
-        return fail(JV_ERR_UNSUPPORTED, "add_nodes: degree " + std::to_string(g->g.degree) + " > 64, the largest row the builder handles");
-    if (params->degree != g->g.degree) return fail(JV_ERR_INVALID, "add_nodes: params->degree differs from the graph's degree");
-    if ((rc = build_params_check(params, bp)) || kind == KIND_F32) return rc;
-    if (kind == KIND_BQ) return bq_padding_check(ds, "add_nodes_bq");
-    if (!pq_prune_fits(ds->d))
-        return fail(JV_ERR_UNSUPPORTED, "add_nodes_pq: a LUT of M * k = " + std::to_string(ds->d.M * ds->d.k) +
-                                            " entries does not fit the prune's shared memory next to its candidates (DESIGN §4.3c)");
-    return jv_dataset_pq_pair_table(ds, metric);
+    return provider_check(g, ds, kind, metric, params, bp, "add_nodes");
 }
 
 // g's state into A and the seed of a level-0 builder over n rows (accept: the storage of its bits). Enqueues a copy of g's
@@ -1874,47 +1852,34 @@ struct jv_builder_s {
     ~jv_builder_s() { builder_destroy(B); }
 };
 
-int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
+// jv_builder_create (kind = KIND_F32), jv_builder_create_pq (KIND_PQ) and jv_builder_create_bq (KIND_BQ)
+static int builder_of(jv_dataset ds, int kind, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
 {
-    ON_DEVICE_OF(f32);
-    if (!params || !out || f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "builder_create: needs an fp32 data set");
-    int rc = check_metric(f32->d, metric);
-    if (rc) return rc;
+    ON_DEVICE_OF(ds);
+    if (!params || !out) return fail(JV_ERR_INVALID, "builder_create: null argument");
     std::unique_ptr<jv_builder_s> b(new jv_builder_s());
-    b->device = f32->device; b->data = f32; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
-    if ((rc = build_params_check(params, &b->bp))) return rc;
+    const int rc = provider_check(nullptr, ds, kind, metric, params, &b->bp, "builder_create");
+    if (rc) return rc;
+    b->device = ds->device; b->data = ds; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
     CK(b->timer.start(b->stream), "event");
-    CK(builder_create(f32->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
+    CK(builder_create(ds->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
     *out = b.release();
     return JV_OK;
+}
+
+int jv_builder_create(jv_dataset f32, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
+{
+    return builder_of(f32, KIND_F32, metric, params, cuda_stream, out);
 }
 
 int jv_builder_create_pq(jv_dataset pq, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
 {
-    ON_DEVICE_OF(pq);
-    if (!params || !out) return fail(JV_ERR_INVALID, "builder_create_pq: null argument");
-    std::unique_ptr<jv_builder_s> b(new jv_builder_s());
-    int rc = pq_build_check(pq, metric, params, &b->bp);
-    if (rc) return rc;
-    b->device = pq->device; b->data = pq; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
-    CK(b->timer.start(b->stream), "event");
-    CK(builder_create(pq->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
-    *out = b.release();
-    return JV_OK;
+    return builder_of(pq, KIND_PQ, metric, params, cuda_stream, out);
 }
 
 int jv_builder_create_bq(jv_dataset bq, int metric, const jv_build_params *params, void *cuda_stream, jv_builder *out)
 {
-    ON_DEVICE_OF(bq);
-    if (!params || !out) return fail(JV_ERR_INVALID, "builder_create_bq: null argument");
-    std::unique_ptr<jv_builder_s> b(new jv_builder_s());
-    int rc = bq_build_check(bq, metric, params, &b->bp);
-    if (rc) return rc;
-    b->device = bq->device; b->data = bq; b->metric = metric; b->params = *params; b->stream = (cudaStream_t)cuda_stream;
-    CK(b->timer.start(b->stream), "event");
-    CK(builder_create(bq->d, metric, b->bp, g_sm_count, &b->B, b->stream), "builder_create");
-    *out = b.release();
-    return JV_OK;
+    return builder_of(bq, KIND_BQ, metric, params, cuda_stream, out);
 }
 
 static int builder_from_graph(jv_graph g, jv_dataset ds, int kind, int metric, const jv_build_params *params, const uint32_t *deleted_bits,
@@ -2131,24 +2096,10 @@ static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric,
 {
     ON_DEVICE_OF(g);
     if (!ds || !deleted_bits || !out || !stats) return fail(JV_ERR_INVALID, "graph_remove_deleted: null argument");
-    if (ds->d.kind != kind)
-        return fail(JV_ERR_INVALID, kind == KIND_PQ   ? "graph_remove_deleted_pq: needs the graph's PQ data set"
-                                    : kind == KIND_BQ ? "graph_remove_deleted_bq: needs the graph's BQ data set"
-                                                      : "graph_remove_deleted: needs the graph's fp32 data set");
     if (ds->d.n != g->g.n || ds->device != g->device) return fail(JV_ERR_INVALID, "graph_remove_deleted: data set and graph differ in size or device");
     if (!(alpha >= 1.0f)) return fail(JV_ERR_INVALID, "graph_remove_deleted: need alpha >= 1");
-    int rc = check_metric(ds->d, metric);
-    if (rc) return rc;
-    if (g->g.degree > 64)
-        return fail(JV_ERR_UNSUPPORTED, "graph_remove_deleted: degree " + std::to_string(g->g.degree) + " > 64, the largest row the prune kernels handle");
-    if (kind == KIND_PQ) {
-        if (!pq_repair_fits(ds->d, g->g.degree))
-            return fail(JV_ERR_UNSUPPORTED, "graph_remove_deleted_pq: a LUT of M * k = " + std::to_string(ds->d.M * ds->d.k) + " entries does not fit the prune's shared memory next to the " +
-                                                std::to_string(g->g.degree * (g->g.degree + 2)) + " candidates a row of this degree can gather (DESIGN §4.3e)");
-        if ((rc = jv_dataset_pq_pair_table(ds, metric))) return rc;
-    }
-    if (kind == KIND_BQ && (rc = bq_padding_check(ds, "graph_remove_deleted_bq"))) return rc;
-    if ((rc = t_ctx.init())) return rc;
+    int rc = provider_check(g, ds, kind, metric, nullptr, nullptr, "graph_remove_deleted");
+    if (rc || (rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
     const int n = g->g.n, degree = g->g.degree;
     const size_t W = ((size_t)n + 31) / 32;

@@ -1064,106 +1064,85 @@ cudaError_t bq_padding_set(const DataDesc &bq, bool *set, cudaStream_t s)
     return drained;
 }
 
-static size_t prune_smem_bytes(const DataDesc &d, int maxc = PRUNE_MAXC)
+// the prune's shared memory at capacity maxc: the query block of d's kind, then the candidate state of prune_kernel (13 B per slot).
+// fp32: the staged row and v's row. PQ: v's LUT and decode(c_v). BQ: c_v and the selected row's words; at most 2 * 128 words
+// (dim 8192) and 8192 slots make 111 KB, so every BQ call fits
+static size_t prune_smem_bytes(const DataDesc &d, int maxc)
 {
-    size_t b = (size_t)(d.stride + 4) * 4 + (size_t)d.stride * 4 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
+    size_t b;
+    switch (d.kind) {
+    case KIND_PQ: b = (size_t)blob_floats(d) * 4 + (size_t)((d.dim + 3) & ~3) * 4; break;
+    case KIND_BQ: b = (size_t)bq_row_floats(d) * 4 * 2; break;
+    default: b = (size_t)(d.stride + 4) * 4 + (size_t)d.stride * 4; break;
+    }
+    b += (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
     return (b + 15) & ~(size_t)15;
 }
 
-// the PQ prune's shared memory: v's LUT, decode(c_v), then the candidate state of prune_kernel
-static size_t prune_pq_smem_bytes(const DataDesc &d, int maxc)
-{
-    size_t b = (size_t)blob_floats(d) * 4 + (size_t)((d.dim + 3) & ~3) * 4 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
-    return (b + 15) & ~(size_t)15;
-}
+bool pq_prune_fits(const DataDesc &pq) { return prune_smem_bytes(pq, PRUNE_MAXC) <= (size_t)PRUNE_PQ_SMEM_MAX; }
 
-bool pq_prune_fits(const DataDesc &pq) { return prune_pq_smem_bytes(pq, PRUNE_MAXC) <= (size_t)PRUNE_PQ_SMEM_MAX; }
-
-// the BQ prune's shared memory: c_v and the selected row's words, then the candidate state (13 B per slot). At most 2 * 128 words
-// (dim 8192) and 8192 slots: 111 KB, so every call fits
-static size_t prune_bq_smem_bytes(const DataDesc &d, int maxc)
+template <typename Kernel>
+static cudaError_t launch_prune_kernel(Kernel kernel, size_t smem, const PruneParams &P, int grid, cudaStream_t s)
 {
-    size_t b = (size_t)bq_row_floats(d) * 4 * 2 + (size_t)maxc * 8 + (size_t)maxc * 4 + 128 * 4 + maxc;
-    return (b + 15) & ~(size_t)15;
-}
-
-// the one BQ prune instantiation (its scores do not depend on the metric) at capacity MAXC
-template <int MAXC>
-static cudaError_t launch_prune_bq(const PruneParams &P, int grid, cudaStream_t s)
-{
-    const size_t sm = prune_bq_smem_bytes(P.d, MAXC);
-    const cudaError_t e = cudaFuncSetAttribute(prune_kernel<JV_METRIC_DOT, MAXC, KIND_BQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    prune_kernel<JV_METRIC_DOT, MAXC, KIND_BQ><<<grid, PRUNE_THREADS, sm, s>>>(P);
+    kernel<<<grid, PRUNE_THREADS, smem, s>>>(P);
     g_launches++;
     return cudaGetLastError();
 }
 
-// PQ: no Gram tier (it would change the pair bits); the incremental kernel at the smallest capacity that holds the candidates
-template <int METRIC>
-static cudaError_t launch_prune_pq_t(const PruneParams &P, int grid, int ncmax, cudaStream_t s)
+// PQ and BQ: prune_kernel at the capacity, with no Gram tier (it would change the pair bits)
+template <int METRIC, int KIND>
+static cudaError_t launch_code_prune(const PruneParams &P, int maxc, int grid, cudaStream_t s)
 {
-    cudaError_t e;
-#define JV_PQ_PRUNE_LAUNCH(MAXC)                                                                                                     \
-    do {                                                                                                                             \
-        const size_t sm_ = prune_pq_smem_bytes(P.d, MAXC);                                                                           \
-        if ((e = cudaFuncSetAttribute(prune_kernel<METRIC, MAXC, KIND_PQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_)) != cudaSuccess) \
-            return e;                                                                                                                \
-        prune_kernel<METRIC, MAXC, KIND_PQ><<<grid, PRUNE_THREADS, sm_, s>>>(P);                                                     \
-    } while (0)
-    if (ncmax <= 64) JV_PQ_PRUNE_LAUNCH(64);
-    else if (ncmax <= 128) JV_PQ_PRUNE_LAUNCH(128);
-    else JV_PQ_PRUNE_LAUNCH(256);
-#undef JV_PQ_PRUNE_LAUNCH
-    g_launches++;
-    return cudaGetLastError();
+#define JV_CODE_PRUNE(MAXC) launch_prune_kernel(prune_kernel<METRIC, MAXC, KIND>, prune_smem_bytes(P.d, MAXC), P, grid, s)
+    switch (maxc) {
+    case 64: return JV_CODE_PRUNE(64);
+    case 128: return JV_CODE_PRUNE(128);
+    case 256: return JV_CODE_PRUNE(256);
+    case 1024: return JV_CODE_PRUNE(1024);
+    case 2048: return JV_CODE_PRUNE(2048);
+    default: return JV_CODE_PRUNE(8192);
+    }
+#undef JV_CODE_PRUNE
 }
 
+// fp32: candidate sets that fit a tile go through a Gram-matrix kernel, on the tensor cores (wgmma, 3xTF32) or the CUDA cores;
+// anything larger keeps the incremental kernel
 template <int METRIC>
-static cudaError_t launch_prune_t(const PruneParams &P, int grid, size_t smem, cudaStream_t s)
+static cudaError_t launch_prune_t(const PruneParams &P, int maxc, bool tc, int grid, cudaStream_t s)
 {
-    // candidate sets that fit a tile go through the Gram-matrix kernel; anything larger keeps the incremental kernel
-    const int ncmax = P.mode == 0 ? P.cand_stride + P.window : P.row_cap;
-    if (P.d.kind == KIND_PQ) return launch_prune_pq_t<METRIC>(P, grid, ncmax, s);
-    cudaError_t e;
-    // Gram products on the tensor cores (wgmma, 3xTF32) unless JV_PRUNE_GRAM=ffma asks for the CUDA-core kernel
+    if (P.d.kind == KIND_PQ) return launch_code_prune<METRIC, KIND_PQ>(P, maxc, grid, s);
+    if (maxc <= 64)
+        return tc ? launch_prune_kernel(prune_gram_tc_kernel<METRIC, 64>, gram_tc_smem_bytes<64>(P.d), P, grid, s)
+                  : launch_prune_kernel(prune_gram_kernel<METRIC, 64>, gram_smem_bytes<64>(P.d), P, grid, s);
+    if (maxc <= 128)
+        return tc ? launch_prune_kernel(prune_gram_tc_kernel<METRIC, 128>, gram_tc_smem_bytes<128>(P.d), P, grid, s)
+                  : launch_prune_kernel(prune_gram_kernel<METRIC, 128>, gram_smem_bytes<128>(P.d), P, grid, s);
+    switch (maxc) {
+    case 256: return launch_prune_kernel(prune_kernel<METRIC, 256>, prune_smem_bytes(P.d, 256), P, grid, s);
+    case 1024: return launch_prune_kernel(prune_kernel<METRIC, 1024>, prune_smem_bytes(P.d, 1024), P, grid, s);
+    default: return launch_prune_kernel(prune_kernel<METRIC, 8192>, prune_smem_bytes(P.d, 8192), P, grid, s);
+    }
+}
+
+// the prune of P.d's kind under P.metric at capacity maxc, the smallest of the caller's tiers that holds its candidates (the
+// builder: 64, 128 or 256; the repair: its tier table). tc picks the tensor-core Gram kernels for fp32 up to 128 candidates. BQ
+// scores do not depend on the metric: one instantiation serves all three
+static cudaError_t launch_prune(const PruneParams &P, int maxc, bool tc, int grid, cudaStream_t s)
+{
+    if (P.d.kind == KIND_BQ) return launch_code_prune<JV_METRIC_DOT, KIND_BQ>(P, maxc, grid, s);
+    if (P.metric == JV_METRIC_EUCLIDEAN) return launch_prune_t<JV_METRIC_EUCLIDEAN>(P, maxc, tc, grid, s);
+    if (P.metric == JV_METRIC_DOT) return launch_prune_t<JV_METRIC_DOT>(P, maxc, tc, grid, s);
+    return launch_prune_t<JV_METRIC_COSINE>(P, maxc, tc, grid, s);
+}
+
+// the builder's prune: the Gram kernels on the tensor cores unless JV_PRUNE_GRAM=ffma asks for the CUDA-core ones
+static cudaError_t launch_build_prune(const PruneParams &P, int grid, cudaStream_t s)
+{
     static const bool use_tc = !(getenv("JV_PRUNE_GRAM") && getenv("JV_PRUNE_GRAM")[0] == 'f');
-    if (ncmax <= 64 && use_tc) {
-        const size_t gs = gram_tc_smem_bytes<64>(P.d);
-        if ((e = cudaFuncSetAttribute(prune_gram_tc_kernel<METRIC, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gs)) != cudaSuccess) return e;
-        prune_gram_tc_kernel<METRIC, 64><<<grid, PRUNE_THREADS, gs, s>>>(P);
-    } else if (ncmax <= 128 && use_tc) {
-        const size_t gs = gram_tc_smem_bytes<128>(P.d);
-        if ((e = cudaFuncSetAttribute(prune_gram_tc_kernel<METRIC, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gs)) != cudaSuccess) return e;
-        prune_gram_tc_kernel<METRIC, 128><<<grid, PRUNE_THREADS, gs, s>>>(P);
-    } else if (ncmax <= 64) {
-        const size_t gs = gram_smem_bytes<64>(P.d);
-        if ((e = cudaFuncSetAttribute(prune_gram_kernel<METRIC, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gs)) != cudaSuccess) return e;
-        prune_gram_kernel<METRIC, 64><<<grid, PRUNE_THREADS, gs, s>>>(P);
-    } else if (ncmax <= 128) {
-        const size_t gs = gram_smem_bytes<128>(P.d);
-        if ((e = cudaFuncSetAttribute(prune_gram_kernel<METRIC, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gs)) != cudaSuccess) return e;
-        prune_gram_kernel<METRIC, 128><<<grid, PRUNE_THREADS, gs, s>>>(P);
-    } else {
-        if ((e = cudaFuncSetAttribute(prune_kernel<METRIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
-        prune_kernel<METRIC><<<grid, PRUNE_THREADS, smem, s>>>(P);
-    }
-    g_launches++;
-    return cudaGetLastError();
-}
-
-static cudaError_t launch_prune(const PruneParams &P, int grid, size_t smem, cudaStream_t s)
-{
-    if (P.d.kind == KIND_BQ) {
-        // BQ: no Gram tier, every metric on the one instantiation, at the smallest capacity that holds the candidates
-        const int ncmax = P.mode == 0 ? P.cand_stride + P.window : P.row_cap;
-        if (ncmax <= 64) return launch_prune_bq<64>(P, grid, s);
-        if (ncmax <= 128) return launch_prune_bq<128>(P, grid, s);
-        return launch_prune_bq<256>(P, grid, s);
-    }
-    if (P.metric == JV_METRIC_EUCLIDEAN) return launch_prune_t<JV_METRIC_EUCLIDEAN>(P, grid, smem, s);
-    if (P.metric == JV_METRIC_DOT) return launch_prune_t<JV_METRIC_DOT>(P, grid, smem, s);
-    return launch_prune_t<JV_METRIC_COSINE>(P, grid, smem, s);
+    const int ncmax = P.mode == 0 ? P.cand_stride + P.window : P.row_cap;
+    return launch_prune(P, ncmax <= 64 ? 64 : ncmax <= 128 ? 128 : 256, use_tc, grid, s);
 }
 
 #define JV_TRY(x)                      \
@@ -1200,7 +1179,6 @@ struct GraphBuilder {
     std::vector<DeviceBuffer> mem;  // owns every block above
     DeviceBuffer scratch;           // the insert searches' scratch, grown with the slice
     BuildStats st = {0, 0, 0, 0, 0};
-    size_t psmem = 0;
     int prune_grid = 0;
 };
 
@@ -1224,7 +1202,6 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
     if (const char *e = getenv("JV_BUILD_BATCH_DIV")) B->batch_div = atoi(e) > 0 ? atoi(e) : 32;  // tuning knob (tools/build_quality.py)
     // in-progress window: as many concurrently inserting peers as still fit the 128-candidate Gram tile next to the beam
     B->window = bp.window >= 0 ? bp.window : std::max(0, std::min(32, 128 - bp.beam));
-    B->psmem = prune_smem_bytes(d);
     B->prune_grid = sm_count * 5;  // ~10 KB of shared memory per CTA: register-limited residency
     cudaError_t err = cudaSuccess;
     const size_t mb = (size_t)B->max_batch;
@@ -1348,7 +1325,7 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
     P.mode = 0; P.node_base = first + lo; P.count = m; P.cand = B->res_nodes; P.cand_stride = B->beam;
     P.window = B->window; P.batch_first = first; P.batch_count = count;
     P.out_rows = rows_out; P.out_deg = deg_out; P.out_stride = B->degree; P.out_base = lo;
-    JV_TRY(launch_prune(P, m < B->prune_grid ? m : B->prune_grid, B->psmem, s));
+    JV_TRY(launch_build_prune(P, m < B->prune_grid ? m : B->prune_grid, s));
     return cudaSuccess;
 }
 
@@ -1384,11 +1361,11 @@ cudaError_t builder_reprune_slice(GraphBuilder *B, int lo, int hi, int32_t *rows
     P.mode = 1; P.list = B->list;
     if (!rows_out) {
         P.count_ptr = B->list_count;
-        return launch_prune(P, B->prune_grid, B->psmem, s);
+        return launch_build_prune(P, B->prune_grid, s);
     }
     if (hi <= lo) return cudaSuccess;
     P.count = hi - lo; P.list_base = lo; P.out_rows = rows_out; P.out_deg = deg_out; P.out_stride = B->row_cap; P.out_base = lo;
-    return launch_prune(P, std::min(hi - lo, B->prune_grid), B->psmem, s);
+    return launch_build_prune(P, std::min(hi - lo, B->prune_grid), s);
 }
 
 cudaError_t builder_apply_repruned(GraphBuilder *B, int count, const int32_t *rows, const int *rdeg, cudaStream_t s)
@@ -1648,57 +1625,7 @@ bool pq_repair_fits(const DataDesc &pq, int degree)
 {
     int t = 0;
     while (t < CODE_REPAIR_TIERS - 1 && degree * (degree + 2) > CODE_REPAIR_TIER_MAX[t]) t++;
-    return prune_pq_smem_bytes(pq, CODE_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
-}
-
-template <int METRIC>
-static cudaError_t launch_repair_prune_t(const PruneParams &P, int tier, int grid, cudaStream_t s)
-{
-    cudaError_t e;
-#define JV_PRUNE_LAUNCH(KERNEL, SMEM)                                                                                   \
-    do {                                                                                                                \
-        const size_t sm_ = (SMEM);                                                                                      \
-        if ((e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_)) != cudaSuccess) return e; \
-        KERNEL<<<grid, PRUNE_THREADS, sm_, s>>>(P);                                                                     \
-    } while (0)
-    if (P.d.kind == KIND_PQ) {
-        switch (tier) {
-        case 0: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 64, KIND_PQ>), prune_pq_smem_bytes(P.d, 64)); break;
-        case 1: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 128, KIND_PQ>), prune_pq_smem_bytes(P.d, 128)); break;
-        case 2: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 256, KIND_PQ>), prune_pq_smem_bytes(P.d, 256)); break;
-        case 3: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 1024, KIND_PQ>), prune_pq_smem_bytes(P.d, 1024)); break;
-        case 4: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 2048, KIND_PQ>), prune_pq_smem_bytes(P.d, 2048)); break;
-        default: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 8192, KIND_PQ>), prune_pq_smem_bytes(P.d, 8192)); break;
-        }
-    } else {
-        switch (tier) {
-        case 0: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 64>), gram_tc_smem_bytes<64>(P.d)); break;
-        case 1: JV_PRUNE_LAUNCH((prune_gram_tc_kernel<METRIC, 128>), gram_tc_smem_bytes<128>(P.d)); break;
-        case 2: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 256>), prune_smem_bytes(P.d, 256)); break;
-        case 3: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 1024>), prune_smem_bytes(P.d, 1024)); break;
-        default: JV_PRUNE_LAUNCH((prune_kernel<METRIC, 8192>), prune_smem_bytes(P.d, 8192)); break;
-        }
-    }
-#undef JV_PRUNE_LAUNCH
-    g_launches++;
-    return cudaGetLastError();
-}
-
-static cudaError_t launch_repair_prune(const PruneParams &P, int tier, int grid, cudaStream_t s)
-{
-    if (P.d.kind == KIND_BQ) {
-        switch (tier) {
-        case 0: return launch_prune_bq<64>(P, grid, s);
-        case 1: return launch_prune_bq<128>(P, grid, s);
-        case 2: return launch_prune_bq<256>(P, grid, s);
-        case 3: return launch_prune_bq<1024>(P, grid, s);
-        case 4: return launch_prune_bq<2048>(P, grid, s);
-        default: return launch_prune_bq<8192>(P, grid, s);
-        }
-    }
-    if (P.metric == JV_METRIC_EUCLIDEAN) return launch_repair_prune_t<JV_METRIC_EUCLIDEAN>(P, tier, grid, s);
-    if (P.metric == JV_METRIC_DOT) return launch_repair_prune_t<JV_METRIC_DOT>(P, tier, grid, s);
-    return launch_repair_prune_t<JV_METRIC_COSINE>(P, tier, grid, s);
+    return prune_smem_bytes(pq, CODE_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
 }
 
 // repair_level's work, enqueued on `s`; every block it allocates goes to `mem`
@@ -1795,7 +1722,7 @@ static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alp
             if (c == 0) continue;
             P.list = tier_list + first;
             P.count = c;
-            JV_TRY(launch_repair_prune(P, t, std::min(c, sm_count * 5), s));
+            JV_TRY(launch_prune(P, tier_max[t], true, std::min(c, sm_count * 5), s));
             first += c;
         }
     }

@@ -138,11 +138,24 @@ def retain_diverse(metric, data, v, cands, degree, alpha, key_scores=None):
     return [int(c[i]) for i in sorted(sel)], flag
 
 
-def remove_deleted(data, metric, adj0, entry, upper, deleted, alpha=1.2, seed=0, holes=None, key_scores=None):
+# the capacities of the removal's prune over PQ or BQ codes (build.cu CODE_REPAIR_TIER_MAX): a row runs at the smallest that holds
+# its candidates
+CODE_REPAIR_TIERS = (64, 128, 256, 1024, 2048, 8192)
+
+
+def repair_tier(ncand):
+    return next(t for t, cap in enumerate(CODE_REPAIR_TIERS) if ncand <= cap or cap == CODE_REPAIR_TIERS[-1])
+
+
+def remove_deleted(data, metric, adj0, entry, upper, deleted, alpha=1.2, seed=0, holes=None, key_scores=None, prune=None):
     """adj0 [n][degree]; upper: list of (ids, adj [count][degree], global ids) for levels 1..; deleted, holes: bool [n].
-    key_scores: see retain_diverse.
+    key_scores: see retain_diverse. prune(v, cands, degree, alpha) -> (selected ids, near-tie flag): the row prune, by default
+    retain_diverse over data (graph_model's score providers give the PQ and BQ ones).
     Returns {"adj0", "upper", "entry", "levels", "rows"}: rows[level][node] = {"flag", "fallback", "cands"} for every repaired row."""
     data = np.asarray(data, dtype=np.float32)
+    if prune is None:
+        def prune(v, cands, degree, alpha):
+            return retain_diverse(metric, data, v, cands, degree, alpha, key_scores)
     n, degree = adj0.shape
     dead = np.asarray(deleted, bool).copy()
     if holes is not None:
@@ -180,7 +193,7 @@ def remove_deleted(data, metric, adj0, entry, upper, deleted, alpha=1.2, seed=0,
                         picks.append(k)
                 two = set(picks)
             cands = set(live) | two
-            sel, flag = retain_diverse(metric, data, v, cands, degree, alpha, key_scores)
+            sel, flag = prune(v, cands, degree, alpha)
             new[r] = sel + [-1] * (degree - len(sel))
             info[v] = {"flag": flag, "fallback": fallback, "cands": cands}
         rows_info.append(info)

@@ -1,4 +1,4 @@
-"""The device graph build checked batch by batch, row for row, against its host restatement (tests/build_model.py).
+"""The device graph build checked batch by batch, row for row, against its host restatement (tests/graph_model.py).
 
 CPU: the restatement reproduces the reference's testDiversity lists; the pair bound of delete_model.pair_bound holds for a numpy
 emulation of the Gram product's arithmetic, and the untranslated L2 Gram form breaks it on rows that share a large offset.
@@ -14,8 +14,8 @@ import time
 import numpy as np
 import pytest
 
-import build_model as bm
 import delete_model as dm
+import graph_model as gm
 import oracle_lib as o
 
 METRICS = (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)
@@ -32,7 +32,7 @@ def test_model_reproduces_golden_diversity_lists(oracle):
                 5: {0: [1, 2], 1: [0, 3, 4], 2: [0], 3: [1, 4], 4: [1, 3]},
                 6: {0: [1, 2], 1: [0, 3, 4, 5], 2: [0], 3: [1, 4], 4: [1, 3, 5], 5: [1, 4]}}
     for n, want in expected.items():
-        m = bm.BuildModel(oracle, vec[:n], o.DOT_PRODUCT, 4, 10, overflow=1.0, alpha=1.0, window=0)
+        m = gm.BuildModel(gm.F32Scores(oracle, vec[:n], o.DOT_PRODUCT), 4, 10, overflow=1.0, alpha=1.0, window=0)
         assert m.next_batch() == (1, 1)  # below 32 inserted nodes every batch holds one
         adj, flagged = m.build()
         assert flagged == 0
@@ -42,15 +42,15 @@ def test_model_reproduces_golden_diversity_lists(oracle):
 
 def test_window_candidates():
     # prune_candidate: W = 4 around u = 10 in batch [8, 13): 8, 9, 11, 12 (u skipped); clipped at the batch's ends
-    assert bm.window_candidates(10, 4, 8, 5) == [8, 9, 11, 12]
-    assert bm.window_candidates(8, 4, 8, 5) == [9, 10]
-    assert bm.window_candidates(9, 3, 8, 5) == [8, 10, 11]
-    assert bm.window_candidates(5, 0, 0, 10) == []
-    assert bm.default_window(100) == 28 and bm.default_window(30) == 32 and bm.default_window(200) == 0
+    assert gm.window_candidates(10, 4, 8, 5) == [8, 9, 11, 12]
+    assert gm.window_candidates(8, 4, 8, 5) == [9, 10]
+    assert gm.window_candidates(9, 3, 8, 5) == [8, 10, 11]
+    assert gm.window_candidates(5, 0, 0, 10) == []
+    assert gm.default_window(100) == 28 and gm.default_window(30) == 32 and gm.default_window(200) == 0
 
 
 def test_assign_levels_distribution():
-    members, entry = bm.assign_levels(20000, 16, 7)
+    members, entry = gm.assign_levels(20000, 16, 7)
     assert len(members) >= 2 and entry in set(members[-1].tolist())
     assert abs(len(members[0]) / 20000 - 1 / 16) < 0.01  # P(level >= 1) = 1 / M
     for a, b in zip(members, members[1:]):
@@ -180,106 +180,18 @@ CASES = [
 FFMA_CASES = ("tc64_dot", "tc128_cos_d100", "offset_l2")
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _compare(got, gdeg, want, wdeg, flags, what):
-    """rows the model did not flag must be equal; returns (rows, flagged, differing)"""
-    differ = (got != want).any(1) | (gdeg != wdeg)
-    bad = np.flatnonzero(differ & ~flags)
-    assert len(bad) == 0, (what, "rows differ", bad[:5].tolist(), got[bad[:1]].tolist(), want[bad[:1]].tolist())
-    return len(flags), int(flags.sum()), int(differ.sum())
-
-
 def run_case(jv, oracle, sift, case):
-    import torch
-
+    import builder_driver as bd
     from jvector_b200 import _native as nat
     cid, wname, metric, M, beam, window, alpha, overflow, max_batch, hier = case
     data = world(wname, sift)
-    n = data.shape[0]
-    lib = nat.init()
     vec = jv.F32Vectors(data)
-    seed = 3
-    params = nat.BuildParams(M, beam, overflow, alpha, int(hier), seed, max_batch, window)
-    st = torch.cuda.current_stream().cuda_stream
-    b = C.c_void_p()
-    nat.check(lib.jv_builder_create(vec._h, metric, C.byref(params), C.c_void_p(st), C.byref(b)))
-    model = bm.BuildModel(oracle, data, metric, M, beam, overflow=overflow, alpha=alpha, max_batch=max_batch, window=window)
-    deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
-    nat.check(lib.jv_builder_info(b, C.byref(deg_), C.byref(cap_), C.byref(mb_)))
-    assert (deg_.value, cap_.value) == (M, model.row_cap)
-    rows_t = torch.empty((mb_.value, M), dtype=torch.int32, device="cuda")
-    rdeg_t = torch.empty(mb_.value, dtype=torch.int32, device="cuda")
-    tally = {"insert": [0, 0, 0], "reprune": [0, 0, 0]}
-
-    def add(kind, r):
-        tally[kind] = [a + x for a, x in zip(tally[kind], r)]
-
-    def reprune_round(L, lst, what):
-        assert L == len(lst), (what, "rows to re-prune", L, len(lst))
-        if L == 0:
-            return
-        rp = torch.empty((L, model.row_cap), dtype=torch.int32, device="cuda")
-        rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-        nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-        got, gdeg = rp.cpu().numpy(), rpd.cpu().numpy()
-        want, wdeg, flags = model.reprune_rows(lst)
-        add("reprune", _compare(got, gdeg, want, wdeg, flags, what))
-        model.apply_repruned(lst, got, gdeg)  # the mirror adopts the device's rows: a flagged near tie cannot cascade
-        nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
-
-    first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-    batches = 0
-    try:
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            f, c = first.value, count.value
-            if c == 0:
-                assert model.next_batch() is None
-                break
-            assert (f, c) == model.next_batch()
-            # every other batch in two slices: rows land at out_base + i, nodes are node_base + i
-            for lo, hi in ([(0, c // 2), (c // 2, c)] if batches % 2 else [(0, c)]):
-                nat.check(lib.jv_builder_insert_slice(b, f, c, lo, hi, _ptr(rows_t), _ptr(rdeg_t)))
-            got, gdeg = rows_t[:c].cpu().numpy(), rdeg_t[:c].cpu().numpy()
-            want, wdeg, flags = model.insert_rows(f, c)
-            add("insert", _compare(got, gdeg, want, wdeg, flags, (cid, "batch", batches, f, c)))
-            nat.check(lib.jv_builder_apply_new(b, f, c, _ptr(rows_t), _ptr(rdeg_t), C.byref(L)))
-            lst = model.apply_new(f, c, got, gdeg)
-            reprune_round(L.value, lst, (cid, "batch", batches))
-            batches += 1
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune_round(L.value, model.over_degree(), (cid, "cleanup"))
-        s_b, s_t, s_d = C.c_int64(), C.c_int64(), C.c_int64()
-        nat.check(lib.jv_builder_stats(b, C.byref(s_b), C.byref(s_t), C.byref(s_d)))
-        g = C.c_void_p()
-        ms = C.c_double()
-        nat.check(lib.jv_builder_finish(b, C.byref(g), C.byref(ms)))
-    finally:
-        lib.jv_builder_free(b)
-    gi = jv.GraphIndex(_handle=g)
-    assert (s_b.value, s_t.value, s_d.value) == (batches, 0, model.dropped), (cid, s_b.value, s_t.value, s_d.value, model.dropped)
-    _, adj = gi.level(0)
-    assert np.array_equal(adj, model.compact()), (cid, "finished adjacency")
-    upper_checked = upper_flagged = 0
-    if hier:
-        members, entry = bm.assign_levels(n, M, seed)
-        inf = gi.info()
-        assert inf["entry_node"] == entry and inf["levels"] == 1 + len(members), (cid, inf, entry, len(members))
-        for lv, (ids, want_adj, flagged) in enumerate(bm.upper_levels(oracle, data, metric, members, M=M, beam=beam, overflow=overflow,
-                                                                      alpha=alpha, max_batch=max_batch, window=window), 1):
-            gids, gadj = gi.level(lv)
-            assert np.array_equal(gids, ids), (cid, "members of level", lv)
-            if flagged == 0:  # a level the model built without a near tie has one correct adjacency
-                assert np.array_equal(gadj, want_adj), (cid, "level", lv)
-                upper_checked += 1
-            else:
-                upper_flagged += 1
+    params = nat.BuildParams(M, beam, overflow, alpha, int(hier), 3, max_batch, window)
+    gi, tally, batches, dropped, (upper_checked, upper_flagged) = bd.drive_build(nat.init(), vec, metric, params,
+                                                                                 lambda: gm.F32Scores(oracle, data, metric), cid)
     gi.close()
     vec.close()
-    return tally, model.dropped, batches, upper_checked, upper_flagged
+    return tally, dropped, batches, upper_checked, upper_flagged
 
 
 def _budget(case, kind):
@@ -287,7 +199,7 @@ def _budget(case, kind):
     isDiverse tests), 3 % past the 128-candidate tier. The proven pair bound grows with the depth of the dot product, so at
     stride 768 it is ten times the stride-64 one and flags proportionally more rows"""
     cid, wname, _, _, beam, window, *_ = case
-    w = bm.default_window(beam) if window < 0 else window
+    w = gm.default_window(beam) if window < 0 else window
     frac = (0.03 if beam + w > 128 else 0.02) if kind == "insert" else 0.01
     if wname.startswith("dup"):
         # a node whose exact duplicate d is selected first meets sim(c, d) = score(c) for every other candidate c: an exact tie at

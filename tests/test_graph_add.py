@@ -1,5 +1,5 @@
 """addGraphNode for a batch (jv_graph_add_nodes / jv_builder_create_from_graph), checked against the seeded host restatement of the
-builder (tests/add_model.py SeededBuildModel, extend_levels).
+builder (tests/graph_model.py BuildModel with a graph's rows, extend_levels).
 
 CPU: the seeded model, chained one node per call, reproduces the reference's testDiversity lists; new nodes take the tail of the
 build's level draws; both entry points report a missing device.
@@ -13,11 +13,11 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import add_model as am
-import build_model as bm
+import builder_driver as bd
+import graph_model as gm
 import oracle_lib as o
 from oracle_lib import fp, ip
-from test_build_steps import CASES, _budget, _compare, latent_rows, world
+from test_build_steps import CASES, _budget, latent_rows, world
 
 METRICS = (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)
 
@@ -33,10 +33,10 @@ def test_seeded_model_chain_reproduces_golden_diversity_lists(oracle):
                 5: {0: [1, 2], 1: [0, 3, 4], 2: [0], 3: [1, 4], 4: [1, 3]},
                 6: {0: [1, 2], 1: [0, 3, 4, 5], 2: [0], 3: [1, 4], 4: [1, 3, 5], 5: [1, 4]}}
     kw = dict(M=4, beam=10, overflow=1.0, alpha=1.0, window=0)
-    adj, flagged = bm.BuildModel(oracle, vec[:3], o.DOT_PRODUCT, **kw).build()
+    adj, flagged = gm.BuildModel(gm.F32Scores(oracle, vec[:3], o.DOT_PRODUCT), **kw).build()
     for n, want in expected.items():
         if n > 3:
-            m = am.SeededBuildModel(oracle, vec[:n], o.DOT_PRODUCT, adj, 0, **kw)
+            m = gm.BuildModel(gm.F32Scores(oracle, vec[:n], o.DOT_PRODUCT), rows=adj, entry=0, **kw)
             assert m.next_batch() == (n - 1, 1)
             adj, flagged = m.build()
         assert flagged == 0
@@ -47,21 +47,22 @@ def test_seeded_model_chain_reproduces_golden_diversity_lists(oracle):
 def test_seeded_model_squeezes_rows_and_starts_at_the_entry(oracle):
     data = o.random_unit_vectors(np.random.default_rng(3), 40, 8)
     rows = np.array([[-1, 2, -1, 1], [0, -1, -1, -1], [-1, -1, -1, -1]], np.int32)
-    m = am.SeededBuildModel(oracle, data, o.DOT_PRODUCT, rows, 1, M=4, beam=10)
+    scores = gm.F32Scores(oracle, data, o.DOT_PRODUCT)
+    m = gm.BuildModel(scores, M=4, beam=10, rows=rows, entry=1)
     assert m.adj[0, :3].tolist() == [2, 1, -1] and m.deg[:3].tolist() == [2, 1, 0]
     assert (m.entry, m.inserted, m.next_batch()) == (1, 3, (3, 1))
-    empty = am.SeededBuildModel(oracle, data, o.DOT_PRODUCT, rows, -1, M=4, beam=10)
+    empty = gm.BuildModel(scores, M=4, beam=10, rows=rows, entry=-1)
     assert (empty.entry, empty.inserted) == (3, 4)  # no entry: the first new node is the entry, as node 0 is for a build
 
 
 def test_new_nodes_take_the_tail_of_the_level_draws():
     n0, n, M, seed = 7000, 20000, 16, 5
-    members, _ = bm.assign_levels(n, M, seed)
-    fresh = am.added_levels(n0, n, M, seed)
+    members, _ = gm.assign_levels(n, M, seed)
+    fresh = gm.added_levels(n0, n, M, seed)
     assert len(fresh) == len(members) or (len(fresh) < len(members) and all(not (m >= n0).any() for m in members[len(fresh):]))
     for lv, ids in enumerate(fresh):
         assert np.array_equal(ids, members[lv][members[lv] >= n0]), lv
-    old, _ = bm.assign_levels(n0, M, seed)  # the build of the first n0 rows drew the same levels for them
+    old, _ = gm.assign_levels(n0, M, seed)  # the build of the first n0 rows drew the same levels for them
     for lv, ids in enumerate(old):
         assert np.array_equal(ids, members[lv][members[lv] < n0]), lv
 
@@ -88,133 +89,15 @@ def jv():
     return jvector_b200
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _levels(gi):
-    return [gi.level(lv) for lv in range(gi.info()["levels"])]
-
-
-def _same_graph(a, b):
-    if a.info() != b.info():
-        return False
-    return all(np.array_equal(x[0], y[0]) and x[1].tobytes() == y[1].tobytes() for x, y in zip(_levels(a), _levels(b)))
-
-
-def _bits(mask):
-    from jvector_b200.api import pack_accept_bits
-    return pack_accept_bits(mask) if mask is not None else None
-
-
-def _bptr(bits):
-    return bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None
-
-
 def drive_add(jv, oracle, vec, data, g, case, marks=None):
-    """the add of rows [n0, n) to g driven step by step (jv_builder_create_from_graph + jv_builder_*), each batch's inserted rows,
-    overflow list and re-pruned rows compared with the seeded model's, the mirror then adopting the device's rows. At the end the
-    adjacency, dropped back-links, upper levels and entry equal the model's, and the one-call add gives the same bytes (twice).
+    """the add of rows [n0, n) to g driven step by step against the seeded model (builder_driver.drive_add), on whole batches.
     Returns (graph, tally, batches, dropped, upper levels checked)"""
-    import torch
-
     from jvector_b200 import _native as nat
     cid, _, metric, M, beam, window, alpha, overflow, max_batch, _ = case
-    seed = 3
-    lib = nat.init()
-    n, n0 = data.shape[0], g.info()["n"]
-    entry0 = g.info()["entry_node"]
-    levels0 = _levels(g)
-    params = nat.BuildParams(M, beam, overflow, alpha, 0, seed, max_batch, window)
-    bits = _bits(marks)
-    kw = dict(M=M, beam=beam, overflow=overflow, alpha=alpha, max_batch=max_batch, window=window)
-    accept = None if marks is None else np.concatenate([~marks, np.ones(n - n0, bool)])
-    model = am.SeededBuildModel(oracle, data, metric, levels0[0][1], entry0, accept, **kw)
-    st = torch.cuda.current_stream().cuda_stream
-    b = C.c_void_p()
-    nat.check(lib.jv_builder_create_from_graph(g._h, vec._h, metric, C.byref(params), _bptr(bits), C.c_void_p(st), C.byref(b)))
-    rows_t = torch.empty((model.max_batch, M), dtype=torch.int32, device="cuda")
-    rdeg_t = torch.empty(model.max_batch, dtype=torch.int32, device="cuda")
-    tally = {"insert": [0, 0, 0], "reprune": [0, 0, 0]}
-
-    def add(kind, r):
-        tally[kind] = [a + x for a, x in zip(tally[kind], r)]
-
-    def reprune_round(L, lst, what):
-        assert L == len(lst), (what, "rows to re-prune", L, len(lst))
-        if L == 0:
-            return
-        rp = torch.empty((L, model.row_cap), dtype=torch.int32, device="cuda")
-        rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-        nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-        got, gdeg = rp.cpu().numpy(), rpd.cpu().numpy()
-        want, wdeg, flags = model.reprune_rows(lst)
-        add("reprune", _compare(got, gdeg, want, wdeg, flags, what))
-        model.apply_repruned(lst, got, gdeg)
-        nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
-
-    first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-    batches = 0
-    try:
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            f, c = first.value, count.value
-            if c == 0:
-                assert model.next_batch() is None
-                break
-            assert (f, c) == model.next_batch()
-            nat.check(lib.jv_builder_insert_slice(b, f, c, 0, c, _ptr(rows_t), _ptr(rdeg_t)))
-            got, gdeg = rows_t[:c].cpu().numpy(), rdeg_t[:c].cpu().numpy()
-            want, wdeg, flags = model.insert_rows(f, c)
-            add("insert", _compare(got, gdeg, want, wdeg, flags, (cid, "batch", batches, f, c)))
-            nat.check(lib.jv_builder_apply_new(b, f, c, _ptr(rows_t), _ptr(rdeg_t), C.byref(L)))
-            lst = model.apply_new(f, c, got, gdeg)
-            reprune_round(L.value, lst, (cid, "batch", batches))
-            batches += 1
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune_round(L.value, model.over_degree(), (cid, "cleanup"))
-        s_b, s_t, s_d = C.c_int64(), C.c_int64(), C.c_int64()
-        nat.check(lib.jv_builder_stats(b, C.byref(s_b), C.byref(s_t), C.byref(s_d)))
-        h = C.c_void_p()
-        nat.check(lib.jv_builder_finish(b, C.byref(h), None))
-    finally:
-        lib.jv_builder_free(b)
-    gi = jv.GraphIndex(_handle=h)
-    assert (s_b.value, s_t.value, s_d.value) == (batches, 0, model.dropped), (cid, s_b.value, s_t.value, s_d.value, model.dropped)
-    adj = gi.level(0)[1]
-    assert np.array_equal(adj, model.compact()), (cid, "finished adjacency")
-    inf = gi.info()
-    upper_checked = 0
-    if len(levels0) > 1:
-        want_levels, want_entry = am.extend_levels(oracle, data, metric, levels0[1:], entry0, n0, seed, marks, **kw)
-        assert inf["entry_node"] == want_entry and inf["levels"] == 1 + len(want_levels), (cid, inf, want_entry, len(want_levels))
-        for lv, (ids, want_adj, flagged) in enumerate(want_levels, 1):
-            gids, gadj = gi.level(lv)
-            assert np.array_equal(gids, ids), (cid, "members of level", lv)
-            if flagged == 0:
-                assert np.array_equal(gadj, want_adj), (cid, "level", lv)
-                upper_checked += 1
-    else:
-        assert inf["levels"] == 1 and inf["entry_node"] == model.entry, (cid, inf, model.entry)
-    # the one-call form: the same bytes, and the same again on a second call
-    ms = C.c_double()
-    one = []
-    for _ in range(2):
-        h1 = C.c_void_p()
-        nat.check(lib.jv_graph_add_nodes(g._h, vec._h, metric, C.byref(params), _bptr(bits), C.byref(h1), C.byref(ms)))
-        one.append(jv.GraphIndex(_handle=h1))
-    assert _same_graph(gi, one[0]) and _same_graph(one[0], one[1]), (cid, "step-wise and one-call adds differ")
-    sv, nb, nd = C.c_int64(), C.c_int64(), C.c_int64()
-    lib.jv_graph_build_stats(C.byref(sv), C.byref(nb), C.byref(nd))
-    assert (nb.value, nd.value) == (batches, model.dropped) and ms.value > 0
-    for x in one:
-        x.close()
-    if marks is not None:
-        marked = np.concatenate([marks, np.zeros(n - n0, bool)])
-        for lv, (ids, ladj) in enumerate(_levels(gi)):
-            new_rows = ladj[ids >= n0]
-            assert not marked[new_rows[new_rows >= 0]].any(), (cid, "a new row names a marked node on level", lv)
-    return gi, tally, batches, model.dropped, upper_checked
+    params = nat.BuildParams(M, beam, overflow, alpha, 0, 3, max_batch, window)
+    gi, tally, batches, dropped, (up, _) = bd.drive_add(nat.init(), g, vec, metric, params, marks, lambda: gm.F32Scores(oracle, data, metric),
+                                                        cid, slices=1)
+    return gi, tally, batches, dropped, up
 
 
 def check_budgets(case, tally):
@@ -272,11 +155,11 @@ def test_add_to_device_build_equals_model(jv, oracle, cid, metric, frac, hier):
     n0 = int(frac * data.shape[0])
     small, vec = jv.F32Vectors(data[:n0]), jv.F32Vectors(data)
     g = _build(jv, small, case, hier)
-    before = _levels(g)
+    before = bd.levels(g)
     gi, tally, batches, dropped, up = drive_add(jv, oracle, vec, data, g, case)
     print("%s: %d batches, dropped %d, insert %s, re-prune %s, upper levels checked %d" % (cid, batches, dropped, tally["insert"], tally["reprune"], up))
     check_budgets(case, tally)
-    after = _levels(g)  # the input graph is untouched
+    after = bd.levels(g)  # the input graph is untouched
     assert all(np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) for a, b in zip(before, after)) and len(before) == len(after)
     for h in (g, gi, small, vec):
         h.close()
@@ -325,12 +208,13 @@ def test_zero_new_nodes_copies_the_graph(jv):
     b = jv.GraphIndexBuilder(o.DOT_PRODUCT, M=16, beamWidth=60)
     g = _build(jv, vec, case, True)
     same = b.addGraphNodes(g, vec)
-    assert _same_graph(g, same) and g.info()["levels"] > 1
+    bd.assert_same_graph(g, same, "n == n0")
+    assert g.info()["levels"] > 1
     adj = g.level(0)[1].copy()
     adj[::3, 1] = -1
     holes = jv.GraphIndex(adj, g.info()["entry_node"], [g.level(lv) for lv in range(1, g.info()["levels"])])
     copy = b.addGraphNodes(holes, vec)  # rows with empty slots mid-row come back as they were
-    assert _same_graph(holes, copy)
+    bd.assert_same_graph(holes, copy, "empty slots mid-row")
     for h in (g, same, holes, copy, vec):
         h.close()
 
@@ -347,7 +231,7 @@ def test_search_on_the_added_graph_equals_oracle(jv, oracle):
     g = b.build(small)
     gi = b.addGraphNodes(g, vec)
     res = jv.GraphSearcher(gi).search(vec, queries, metric, 10, 40)
-    levels = _levels(gi)
+    levels = bd.levels(gi)
     og = o.make_graph(np.ascontiguousarray(levels[0][1]), gi.info()["entry_node"],
                       [(i, np.ascontiguousarray(a)) for i, a in levels[1:]] or None)
     tot = np.zeros(3, np.int64)

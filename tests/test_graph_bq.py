@@ -12,9 +12,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import add_model as am
-import bq_build_model as qm
-import build_model as bm
+import builder_driver as bd
+import delete_model as dm
+import graph_model as gm
 import oracle_lib as o
 from oracle_lib import fp
 
@@ -54,19 +54,19 @@ def latent_world(name, n, dim):
 def test_model_pair_scores_are_hamming_scores(oracle, dim):
     rng = np.random.default_rng(dim)
     _, words = latent_world("pairs%d" % dim, 40, dim)
-    got = qm.pair_scores(words, dim, np.arange(40), np.arange(40))
+    got = gm.bq_pair_scores(words, dim, np.arange(40), np.arange(40))
     W = words.shape[1]
     hd = np.array([[sum(bin(int(a) ^ int(b)).count("1") for a, b in zip(words[i], words[j])) for j in range(40)] for i in range(40)])
     assert np.array_equal(got, (np.float32(1) - hd.astype(np.float32) / np.float32(dim)).astype(np.float32))
     for i in range(40):
         for j in range(40):
-            want = oracle.jvo_bq_score(qm.wp(words[i]), qm.wp(words[j]), W, dim)
+            want = oracle.jvo_bq_score(gm.wp(words[i]), gm.wp(words[j]), W, dim)
             assert np.float32(want).view(np.int32) == got[i, j].view(np.int32), (i, j)
     # the insert query decodes to exactly c_v, padding clear
     back = np.zeros_like(words)
-    q = qm.decode(words, dim)
+    q = gm.bq_decode(words, dim)
     for v in range(len(words)):
-        oracle.jvo_bq_encode(fp(q[v]), dim, qm.wp(back[v]))
+        oracle.jvo_bq_encode(fp(q[v]), dim, gm.wp(back[v]))
     assert np.array_equal(back, words) and set(np.unique(q)) == {-1.0, 1.0}
     del rng
 
@@ -77,8 +77,8 @@ def test_lossless_world_bq_model_equals_fp32_dot_model(oracle, dim):
     n = 300
     rows, words = lossless_world(rng, n, dim)
     kw = dict(M=8, beam=40, max_batch=0, window=-1)
-    bq = qm.BQBuildModel(oracle, words, dim, o.DOT_PRODUCT, **kw)
-    f32 = bm.BuildModel(oracle, rows, o.DOT_PRODUCT, **kw)
+    bq = gm.BuildModel(gm.BQScores(oracle, words, dim, o.DOT_PRODUCT), **kw)
+    f32 = gm.BuildModel(gm.F32Scores(oracle, rows, o.DOT_PRODUCT), **kw)
     # in lock step, both adopting the BQ model's rows: no row may differ
     while (nb := bq.next_batch()) is not None:
         assert nb == f32.next_batch()
@@ -100,7 +100,7 @@ def test_lossless_world_bq_model_equals_fp32_dot_model(oracle, dim):
 
 
 def test_repair_tiers_of_the_model():
-    assert [qm.repair_tier(c) for c in (1, 64, 65, 128, 256, 257, 1024, 1025, 2048, 2049, 4224)] == [0, 0, 1, 1, 2, 3, 3, 4, 4, 5, 5]
+    assert [dm.repair_tier(c) for c in (1, 64, 65, 128, 256, 257, 1024, 1025, 2048, 2049, 4224)] == [0, 0, 1, 1, 2, 3, 3, 4, 4, 5, 5]
 
 
 def test_bq_graph_entry_points_without_device():
@@ -183,130 +183,6 @@ def jv():
     return jvector_b200
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _bptr(bits):
-    return bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None
-
-
-def _levels(gi):
-    return [gi.level(lv) for lv in range(gi.info()["levels"])]
-
-
-def assert_same_graph(a, b, what):
-    ia, ib = a.info(), b.info()
-    assert ia == ib, (what, ia, ib)
-    for lv, ((ids_a, adj_a), (ids_b, adj_b)) in enumerate(zip(_levels(a), _levels(b))):
-        assert np.array_equal(ids_a, ids_b) and np.array_equal(adj_a, adj_b), (what, "level", lv)
-
-
-def _builder(jv, metric, M, beam=60, hier=False, seed=3, **kw):
-    return jv.GraphIndexBuilder(metric, M=M, beamWidth=beam, neighborOverflow=1.2, alpha=1.2, addHierarchy=hier, seed=seed, **kw)
-
-
-def drive(jv, lib, b, model, cid):
-    """a created builder driven batch by batch against `model` (a BQBuildModel or SeededBQBuildModel in the builder's state): every
-    batch's inserted rows, overflow list and re-pruned rows equal the model's. Returns (GraphIndex, (batches, truncated, dropped))."""
-    import torch
-
-    from jvector_b200 import _native as nat
-    deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
-    nat.check(lib.jv_builder_info(b, C.byref(deg_), C.byref(cap_), C.byref(mb_)))
-    assert (deg_.value, cap_.value) == (model.degree, model.row_cap)
-    rows_t = torch.empty((mb_.value, model.degree), dtype=torch.int32, device="cuda")
-    rdeg_t = torch.empty(mb_.value, dtype=torch.int32, device="cuda")
-
-    def reprune_round(L, lst, what):
-        assert L == len(lst), (what, "rows to re-prune", L, len(lst))
-        if L == 0:
-            return
-        rp = torch.empty((L, model.row_cap), dtype=torch.int32, device="cuda")
-        rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-        nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-        got, gdeg = rp.cpu().numpy(), rpd.cpu().numpy()
-        want, wdeg, _ = model.reprune_rows(lst)
-        bad = np.flatnonzero((got != want).any(1) | (gdeg != wdeg))
-        assert len(bad) == 0, (what, "re-pruned rows differ", [lst[i] for i in bad[:5]], got[bad[:1]].tolist(), want[bad[:1]].tolist())
-        model.apply_repruned(lst, got, gdeg)
-        nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
-
-    first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-    batches = 0
-    try:
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            f, c = first.value, count.value
-            if c == 0:
-                assert model.next_batch() is None
-                break
-            assert (f, c) == model.next_batch()
-            for lo, hi in ([(0, c // 2), (c // 2, c)] if batches % 2 else [(0, c)]):
-                nat.check(lib.jv_builder_insert_slice(b, f, c, lo, hi, _ptr(rows_t), _ptr(rdeg_t)))
-            got, gdeg = rows_t[:c].cpu().numpy(), rdeg_t[:c].cpu().numpy()
-            want, wdeg, _ = model.insert_rows(f, c)
-            bad = np.flatnonzero((got != want).any(1) | (gdeg != wdeg))
-            assert len(bad) == 0, (cid, "batch", batches, "rows differ", (f + bad[:5]).tolist(), got[bad[:1]].tolist(), want[bad[:1]].tolist())
-            nat.check(lib.jv_builder_apply_new(b, f, c, _ptr(rows_t), _ptr(rdeg_t), C.byref(L)))
-            reprune_round(L.value, model.apply_new(f, c, got, gdeg), (cid, "batch", batches))
-            batches += 1
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune_round(L.value, model.over_degree(), (cid, "cleanup"))
-        s = [C.c_int64() for _ in range(3)]
-        nat.check(lib.jv_builder_stats(b, *[C.byref(x) for x in s]))
-        h = C.c_void_p()
-        nat.check(lib.jv_builder_finish(b, C.byref(h), None))
-    finally:
-        lib.jv_builder_free(b)
-    gi = jv.GraphIndex(_handle=h)
-    stats = tuple(x.value for x in s)
-    assert stats == (batches, 0, model.dropped), (cid, stats, model.dropped)
-    assert np.array_equal(gi.level(0)[1], model.compact()), (cid, "finished adjacency")
-    return gi, stats
-
-
-def step_build(jv, vectors, metric, params, bq):
-    """jv_builder_create(_bq) + jv_builder_* the way sharded_build drives them on one GPU: (GraphIndex, (batches, truncated, dropped))"""
-    import torch
-
-    from jvector_b200 import _native as nat
-    lib = nat.init()
-    st = torch.cuda.current_stream().cuda_stream
-    b = C.c_void_p()
-    nat.check((lib.jv_builder_create_bq if bq else lib.jv_builder_create)(vectors._h, metric, C.byref(params), C.c_void_p(st), C.byref(b)))
-    try:
-        deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
-        nat.check(lib.jv_builder_info(b, C.byref(deg_), C.byref(cap_), C.byref(mb_)))
-        rows = torch.empty((mb_.value, deg_.value), dtype=torch.int32, device="cuda")
-        rdeg = torch.empty(mb_.value, dtype=torch.int32, device="cuda")
-        first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-
-        def reprune(L):
-            if L:
-                rp = torch.empty((L, cap_.value), dtype=torch.int32, device="cuda")
-                rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-                nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-                nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
-
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            if count.value == 0:
-                break
-            nat.check(lib.jv_builder_insert_slice(b, first.value, count.value, 0, count.value, _ptr(rows), _ptr(rdeg)))
-            nat.check(lib.jv_builder_apply_new(b, first.value, count.value, _ptr(rows), _ptr(rdeg), C.byref(L)))
-            reprune(L.value)
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune(L.value)
-        s = [C.c_int64() for _ in range(3)]
-        nat.check(lib.jv_builder_stats(b, *[C.byref(x) for x in s]))
-        g = C.c_void_p()
-        nat.check(lib.jv_builder_finish(b, C.byref(g), None))
-    finally:
-        lib.jv_builder_free(b)
-    return jv.GraphIndex(_handle=g), tuple(x.value for x in s)
-
-
 # (dim, n, degree, beam, hierarchy, max_batch, window). At 64 dimensions there are 65 scores: beam 16 over 1000 rows keeps the nodes
 # tied at a beam's last score within the fp32 walk's tie tail (rerankK + 28 entries)
 LOSSLESS = [(64, 1000, 8, 16, True, 0, -1), (256, 3000, 16, 60, False, 64, 60), (1024, 4000, 16, 100, True, 0, -1)]
@@ -322,14 +198,14 @@ def test_lossless_world_byte_equal_to_fp32_dot_build(jv, case):
     assert np.array_equal(jv.bq_encode_all(rows), words)
     params = nat.BuildParams(M, beam, 1.2, 1.2, int(hier), 5, max_batch, window)
     bqv, f32 = jv.BQVectors(words, dim), jv.F32Vectors(rows)
-    g_f32, s_f32 = step_build(jv, f32, o.DOT_PRODUCT, params, False)
+    g_f32, s_f32 = bd.step_build(f32, o.DOT_PRODUCT, params)
     assert s_f32[1] == 0, s_f32
     for metric in METRICS:
-        g_bq, s_bq = step_build(jv, bqv, metric, params, True)
+        g_bq, s_bq = bd.step_build(bqv, metric, params, "_bq")
         assert s_bq == s_f32, (metric, s_bq, s_f32)
-        assert_same_graph(g_bq, g_f32, ("lossless step-wise", metric))
-        one = _builder(jv, metric, M, beam=beam, hier=hier, seed=5, max_batch=max_batch, concurrent_window=window).build(bqv)
-        assert_same_graph(one, g_f32, ("lossless one call", metric))
+        bd.assert_same_graph(g_bq, g_f32, ("lossless step-wise", metric))
+        one = bd.builder(jv, metric, M, beam=beam, hier=hier, seed=5, max_batch=max_batch, concurrent_window=window).build(bqv)
+        bd.assert_same_graph(one, g_f32, ("lossless one call", metric))
         g_bq.close(), one.close()
     g_f32.close(), bqv.close(), f32.close()
 
@@ -345,29 +221,14 @@ MODEL_CASES = [
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", MODEL_CASES, ids=[c[0] for c in MODEL_CASES])
 def test_device_bq_build_equals_model(jv, oracle, case):
-    import torch
-
     from jvector_b200 import _native as nat
     cid, dim, metric, M, beam, window, max_batch, hier, n = case
     _, words = latent_world(cid, n, dim)
-    lib = nat.init()
     bqv = jv.BQVectors(words, dim)
-    seed = 3
-    params = nat.BuildParams(M, beam, 1.2, 1.2, int(hier), seed, max_batch, window)
-    kw = dict(M=M, beam=beam, overflow=1.2, alpha=1.2, max_batch=max_batch, window=window)
-    b = C.c_void_p()
-    nat.check(lib.jv_builder_create_bq(bqv._h, metric, C.byref(params), C.c_void_p(torch.cuda.current_stream().cuda_stream), C.byref(b)))
-    gi, stats = drive(jv, lib, b, qm.BQBuildModel(oracle, words, dim, metric, **kw), cid)
-    assert stats[1] == 0
-    if hier:
-        members, entry = bm.assign_levels(n, M, seed)
-        inf = gi.info()
-        assert inf["entry_node"] == entry and inf["levels"] == 1 + len(members), (cid, inf, entry)
-        for lv, (ids, want_adj) in enumerate(qm.upper_levels(oracle, words, dim, metric, members, **kw), 1):
-            gids, gadj = gi.level(lv)
-            assert np.array_equal(gids, ids) and np.array_equal(gadj, want_adj), (cid, "level", lv)
-    one = _builder(jv, metric, M, beam=beam, hier=hier, seed=seed, max_batch=max_batch, concurrent_window=window).build(bqv)
-    assert_same_graph(one, gi, (cid, "one call vs step-wise"))
+    params = nat.BuildParams(M, beam, 1.2, 1.2, int(hier), 3, max_batch, window)
+    gi = bd.drive_build(nat.init(), bqv, metric, params, lambda: gm.BQScores(oracle, words, dim, metric), cid, "_bq")[0]
+    one = bd.builder(jv, metric, M, beam=beam, hier=hier, seed=3, max_batch=max_batch, concurrent_window=window).build(bqv)
+    bd.assert_same_graph(one, gi, (cid, "one call vs step-wise"))
     for h in (gi, one, bqv):
         h.close()
 
@@ -378,18 +239,18 @@ def test_bq_builds_reproduce_and_ignore_the_metric(jv):
     from jvector_b200 import parallel
     _, words = latent_world("repro", 6000, 100)
     bqv = jv.BQVectors(words, 100)
-    b = _builder(jv, o.DOT_PRODUCT, 16, beam=80, hier=True, seed=9)
+    b = bd.builder(jv, o.DOT_PRODUCT, 16, beam=80, hier=True, seed=9)
     one, two = b.build(bqv), b.build(bqv)
     assert b.batches > 0 and b.scored_vectors > 0
-    assert_same_graph(one, two, "two calls")
-    steps, stats = step_build(jv, bqv, o.DOT_PRODUCT, nat.BuildParams(16, 80, 1.2, 1.2, 1, 9, 0, -1), True)
+    bd.assert_same_graph(one, two, "two calls")
+    steps, stats = bd.step_build(bqv, o.DOT_PRODUCT, nat.BuildParams(16, 80, 1.2, 1.2, 1, 9, 0, -1), "_bq")
     assert stats[0] == b.batches and stats[2] == b.dropped_backlinks
-    assert_same_graph(one, steps, "one call vs step-wise")
+    bd.assert_same_graph(one, steps, "one call vs step-wise")
     sharded, _, _ = parallel.sharded_build(None, bqv, o.DOT_PRODUCT, M=16, beamWidth=80, addHierarchy=True, seed=9)
-    assert_same_graph(one, sharded, "sharded_build")
+    bd.assert_same_graph(one, sharded, "sharded_build")
     for metric in (o.EUCLIDEAN, o.COSINE):
-        other = _builder(jv, metric, 16, beam=80, hier=True, seed=9).build(bqv)
-        assert_same_graph(one, other, ("metric", metric))
+        other = bd.builder(jv, metric, 16, beam=80, hier=True, seed=9).build(bqv)
+        bd.assert_same_graph(one, other, ("metric", metric))
         other.close()
     for g in (one, two, steps, sharded, bqv):
         g.close()
@@ -401,63 +262,19 @@ def test_add_to_one_node_graph_is_the_bq_build(jv, hier):
     n, dim, M = 3000, 100, 16
     _, words = latent_world("anchor", n, dim)
     bqv = jv.BQVectors(words, dim)
-    seed = next(s for s in range(1, 400) if am.level_draws(n, M, s)[0] >= 1) if hier else 3
-    b = _builder(jv, o.COSINE, M, hier=hier, seed=seed)
+    seed = next(s for s in range(1, 400) if gm.level_draws(n, M, s)[0] >= 1) if hier else 3
+    b = bd.builder(jv, o.COSINE, M, hier=hier, seed=seed)
     built = b.build(bqv)
     want = (b.batches, b.dropped_backlinks)
     empty = np.full((1, M), -1, np.int32)
-    tops = int(am.level_draws(n, M, seed)[0]) if hier else 0
+    tops = int(gm.level_draws(n, M, seed)[0]) if hier else 0
     one = jv.GraphIndex(empty, 0, [(np.zeros(1, np.int32), empty)] * tops)
     added = b.addGraphNodes(one, bqv)
     assert (b.batches, b.dropped_backlinks) == want
-    assert_same_graph(added, built, ("one-node add", hier))
+    bd.assert_same_graph(added, built, ("one-node add", hier))
     assert built.info()["levels"] > 1 or not hier
     for h in (built, one, added, bqv):
         h.close()
-
-
-def drive_add(jv, oracle, bqv, words, dim, g, metric, M, beam, marks, cid):
-    """the add of word rows [n0, n) to g, step by step against SeededBQBuildModel, then its upper levels and entry; the one-call add
-    gives the same bytes, at every metric"""
-    import torch
-
-    from jvector_b200 import _native as nat
-    seed = 3
-    lib = nat.init()
-    n, n0 = words.shape[0], g.info()["n"]
-    entry0, levels0 = g.info()["entry_node"], _levels(g)
-    params = nat.BuildParams(M, beam, 1.2, 1.2, 0, seed, 0, -1)
-    from jvector_b200.api import pack_accept_bits
-    bits = None if marks is None else pack_accept_bits(marks)
-    b = C.c_void_p()
-    nat.check(lib.jv_builder_create_from_graph_bq(g._h, bqv._h, metric, C.byref(params), _bptr(bits), C.c_void_p(torch.cuda.current_stream().cuda_stream),
-                                                  C.byref(b)))
-    kw = dict(M=M, beam=beam, overflow=1.2, alpha=1.2, max_batch=0, window=-1)
-    accept = None if marks is None else np.concatenate([~marks, np.ones(n - n0, bool)])
-    model = qm.SeededBQBuildModel(oracle, words, dim, metric, levels0[0][1], entry0, accept, **kw)
-    gi, _ = drive(jv, lib, b, model, cid)
-    inf = gi.info()
-    if len(levels0) > 1:
-        want_levels, want_entry = qm.extend_levels(oracle, words, dim, metric, levels0[1:], entry0, n0, seed, marks, **kw)
-        assert inf["entry_node"] == want_entry and inf["levels"] == 1 + len(want_levels), (cid, inf, want_entry, len(want_levels))
-        for lv, (ids, want_adj) in enumerate(want_levels, 1):
-            gids, gadj = gi.level(lv)
-            assert np.array_equal(gids, ids) and np.array_equal(gadj, want_adj), (cid, "level", lv)
-    else:
-        assert inf["levels"] == 1 and inf["entry_node"] == model.entry, (cid, inf, model.entry)
-    ms = C.c_double()
-    for m in METRICS:
-        h1 = C.c_void_p()
-        nat.check(lib.jv_graph_add_nodes_bq(g._h, bqv._h, m, C.byref(params), _bptr(bits), C.byref(h1), C.byref(ms)))
-        one = jv.GraphIndex(_handle=h1)
-        assert_same_graph(gi, one, (cid, "step-wise vs one call", m))
-        one.close()
-    if marks is not None:
-        marked = np.concatenate([marks, np.zeros(n - n0, bool)])
-        for lv, (ids, ladj) in enumerate(_levels(gi)):
-            new_rows = ladj[ids >= n0]
-            assert not marked[new_rows[new_rows >= 0]].any(), (cid, "a new row names a marked node on level", lv)
-    return gi
 
 
 # (id, dim, metric, degree, beam, hierarchy, n0, n, origin of the graph)
@@ -472,11 +289,12 @@ ADD_CASES = [
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", ADD_CASES, ids=[c[0] for c in ADD_CASES])
 def test_stepwise_bq_add_equals_model(jv, oracle, case):
+    from jvector_b200 import _native as nat
     cid, dim, metric, M, beam, hier, n0, n, origin = case
     rng = np.random.default_rng(sum(map(ord, cid)))
     _, words = latent_world(cid, n, dim)
     small, bqv = jv.BQVectors(words[:n0], dim), jv.BQVectors(words, dim)
-    b = _builder(jv, metric, M, beam=beam, hier=hier)
+    b = bd.builder(jv, metric, M, beam=beam, hier=hier)
     g = b.build(small)
     marks = None
     if origin == "marked":
@@ -486,30 +304,15 @@ def test_stepwise_bq_add_equals_model(jv, oracle, case):
     elif origin == "all_removed":
         g = b.removeDeletedNodes(g, small, np.ones(n0, bool))
         assert g.info()["entry_node"] == -1
-    before = _levels(g)
-    gi = drive_add(jv, oracle, bqv, words, dim, g, metric, M, beam, marks, cid)
+    before = bd.levels(g)
+    params = nat.BuildParams(M, beam, 1.2, 1.2, 0, 3, 0, -1)
+    gi = bd.drive_add(nat.init(), g, bqv, metric, params, marks, lambda: gm.BQScores(oracle, words, dim, metric), cid, "_bq", METRICS)[0]
     if origin == "all_removed":
         assert gi.info()["entry_node"] == n0
-    after = _levels(g)
+    after = bd.levels(g)
     assert len(before) == len(after) and all(np.array_equal(a[0], c[0]) and np.array_equal(a[1], c[1]) for a, c in zip(before, after))
     for h in (g, gi, small, bqv):
         h.close()
-
-
-def assert_removal_matches_model(gi, res, what):
-    inf = gi.info()
-    assert inf["entry_node"] == res["entry"] and inf["levels"] == res["levels"], (what, inf, res["entry"], res["levels"])
-    want = [(np.arange(res["adj0"].shape[0], dtype=np.int32), res["adj0"])] + list(res["upper"])
-    for L, ((dids, dadj), (wids, wadj)) in enumerate(zip(_levels(gi), want)):
-        assert np.array_equal(dids, wids), (what, "members of level", L)
-        bad = np.flatnonzero((dadj != wadj).any(1))
-        assert len(bad) == 0, (what, "level", L, "rows differ", wids[bad[:5]].tolist(), dadj[bad[:1]].tolist(), wadj[bad[:1]].tolist())
-    cands = [len(r["cands"] - {v}) for lv in res["rows"] for v, r in lv.items()]
-    st = gi.remove_stats
-    assert st["repaired_rows"] == len(cands) and st["candidates"] == sum(cands) and st["max_candidates"] == max(cands, default=0), (what, st)
-    assert st["random_fallbacks"] == sum(r["fallback"] for lv in res["rows"] for r in lv.values()), (what, st)
-    assert st["live_nodes"] == (~res["dead"]).sum()
-    return np.bincount([qm.repair_tier(c) for c in cands], minlength=len(qm.REPAIR_TIERS))
 
 
 # (id, dim, metric, degree, hierarchy, n, deleted fraction, entry deleted)
@@ -527,18 +330,19 @@ def test_bq_removal_equals_model(jv, oracle, case):
     rng = np.random.default_rng(sum(map(ord, cid)))
     _, words = latent_world(cid, n, dim)
     bqv = jv.BQVectors(words, dim)
-    b = _builder(jv, metric, M, hier=hier, seed=17)
+    b = bd.builder(jv, metric, M, hier=hier, seed=17)
     g = b.build(bqv)
-    levels, entry = _levels(g), g.info()["entry_node"]
+    levels, entry = bd.levels(g), g.info()["entry_node"]
     deleted = rng.random(n) < frac
     deleted[entry] = kill_entry
     got = b.removeDeletedNodes(g, bqv, deleted)
     for m in METRICS:  # the same bytes at every metric, and from a second call
-        again = _builder(jv, m, M, hier=hier, seed=17).removeDeletedNodes(g, bqv, deleted)
-        assert_same_graph(got, again, (cid, "metric", m))
+        again = bd.builder(jv, m, M, hier=hier, seed=17).removeDeletedNodes(g, bqv, deleted)
+        bd.assert_same_graph(got, again, (cid, "metric", m))
         again.close()
-    res = qm.BQRepairModel(oracle, words, dim, metric, M).remove_deleted(levels[0][1], entry, levels[1:], deleted, seed=17)
-    hit = assert_removal_matches_model(got, res, cid)
+    bqs = gm.BQScores(oracle, words, dim, metric)
+    res = dm.remove_deleted(bqs.queries, metric, levels[0][1], entry, levels[1:], deleted, seed=17, prune=bqs.prune)
+    hit = bd.assert_removal_matches_model(got, res, cid)
     print(cid, "rows per tier", hit.tolist(), got.remove_stats)
     assert got.remove_stats["removed"] == deleted.sum() and (not kill_entry or got.info()["entry_node"] != entry)
     for h in (g, got, bqv):
@@ -573,9 +377,10 @@ def test_bq_removal_hits_every_tier_on_a_made_graph(jv, oracle):
             adj[j] = pick(j, M, pool)
     deleted[rng.choice(np.flatnonzero(~deleted[100:]) + 100, 60, replace=False)] = True
     g = jv.GraphIndex(adj, 0)
-    got = _builder(jv, o.EUCLIDEAN, M, seed=5).removeDeletedNodes(g, bqv, deleted)
-    res = qm.BQRepairModel(oracle, words, dim, o.EUCLIDEAN, M).remove_deleted(adj, 0, [], deleted, seed=5)
-    hit = assert_removal_matches_model(got, res, "made graph")
+    got = bd.builder(jv, o.EUCLIDEAN, M, seed=5).removeDeletedNodes(g, bqv, deleted)
+    bqs = gm.BQScores(oracle, words, dim, o.EUCLIDEAN)
+    res = dm.remove_deleted(bqs.queries, o.EUCLIDEAN, adj, 0, [], deleted, seed=5, prune=bqs.prune)
+    hit = bd.assert_removal_matches_model(got, res, "made graph")
     print("made graph: rows per tier", hit.tolist(), got.remove_stats)
     assert (hit > 0).all() and got.remove_stats["max_candidates"] > 2048, hit.tolist()
     for h in (g, got, bqv):
@@ -588,22 +393,24 @@ def test_bq_remove_add_remove_keeps_holes_and_equals_models(jv, oracle):
     n0, n, dim, M = 1600, 1800, 100, 16
     _, words = latent_world("holes", n, dim)
     small, bqv = jv.BQVectors(words[:n0], dim), jv.BQVectors(words, dim)
-    b = _builder(jv, o.DOT_PRODUCT, M, hier=True, seed=4)
+    b = bd.builder(jv, o.DOT_PRODUCT, M, hier=True, seed=4)
     g = b.build(small)
     first = rng.random(n0) < 0.1
     rep = b.removeDeletedNodes(g, small, first)
-    lv = _levels(g)
-    res = qm.BQRepairModel(oracle, words[:n0], dim, o.DOT_PRODUCT, M).remove_deleted(lv[0][1], g.info()["entry_node"], lv[1:], first, seed=4)
-    assert_removal_matches_model(rep, res, "first removal")
+    lv = bd.levels(g)
+    bqs = gm.BQScores(oracle, words[:n0], dim, o.DOT_PRODUCT)
+    res = dm.remove_deleted(bqs.queries, o.DOT_PRODUCT, lv[0][1], g.info()["entry_node"], lv[1:], first, seed=4, prune=bqs.prune)
+    bd.assert_removal_matches_model(rep, res, "first removal")
     grown = b.addGraphNodes(rep, bqv)
     wide = np.concatenate([first, np.zeros(n - n0, bool)])
     assert grown.info()["n"] == n and not np.isin(grown.level(0)[1], np.flatnonzero(first)).any()
     second = (rng.random(n) < 0.05) & ~wide
     again = b.removeDeletedNodes(grown, bqv, second | wide)
-    lv = _levels(grown)
-    res = qm.BQRepairModel(oracle, words, dim, o.DOT_PRODUCT, M).remove_deleted(lv[0][1], grown.info()["entry_node"], lv[1:], second | wide,
-                                                                               seed=4, holes=wide)
-    assert_removal_matches_model(again, res, "second removal")
+    lv = bd.levels(grown)
+    bqs = gm.BQScores(oracle, words, dim, o.DOT_PRODUCT)
+    res = dm.remove_deleted(bqs.queries, o.DOT_PRODUCT, lv[0][1], grown.info()["entry_node"], lv[1:], second | wide, seed=4, holes=wide,
+                            prune=bqs.prune)
+    bd.assert_removal_matches_model(again, res, "second removal")
     assert again.remove_stats["removed"] == second.sum(), (again.remove_stats, second.sum())
     assert again.remove_stats["live_nodes"] == n - first.sum() - second.sum()
     for h in (g, rep, grown, again, small, bqv):
@@ -636,7 +443,7 @@ def test_bq_graph_recall_near_fp32_graph(jv):
     truth, _, _ = jv.topk_bruteforce(f32, vsf, queries, 10)
     recall = {}
     for name, vec in (("fp32", f32), ("bq", bqv)):
-        g = _builder(jv, vsf, 16, beam=100, hier=True, seed=9).build(vec)
+        g = bd.builder(jv, vsf, 16, beam=100, hier=True, seed=9).build(vec)
         s = jv.GraphSearcher(g)
         recall[(name, "f32_walk")] = _recall(s.search(f32, queries, vsf, 10, 100).nodes, truth)
         recall[(name, "bq_walk")] = _recall(s.search(bqv, queries, vsf, 10, 100, reranker=f32).nodes, truth)
@@ -662,7 +469,7 @@ def test_bq_graph_errors(jv):
     full = jv.GraphIndex(np.full((300, 8), -1, np.int32), 0)
     params = nat.BuildParams(8, 30, 1.2, 1.2, 0, 0, 0, -1)
     out, ms, st = C.c_void_p(), C.c_double(), nat.RemoveStats()
-    none = np.zeros(10, np.uint32)
+    none = np.zeros(300, bool)
 
     def build(ds, metric=1, p=params, o_=C.byref(out)):
         a = lib.jv_graph_build_bq(ds, metric, C.byref(p) if p is not None else None, o_, C.byref(ms))
@@ -677,7 +484,7 @@ def test_bq_graph_errors(jv):
         return a
 
     def remove(graph, ds, metric=1, alpha=1.2, bits=none, o_=C.byref(out), st_=C.byref(st)):
-        return lib.jv_graph_remove_deleted_bq(graph, ds, metric, alpha, 0, _bptr(bits), o_, st_)
+        return lib.jv_graph_remove_deleted_bq(graph, ds, metric, alpha, 0, bd.bits(bits), o_, st_)
 
     launches = lib.jv_kernel_launch_count()
     assert build(None) == -2 and build(bqv._h, p=None) == -2 and build(bqv._h, o_=None) == -2
@@ -708,10 +515,10 @@ def test_bq_graph_errors(jv):
     assert lib.jv_builder_create_pq(bqv._h, 1, C.byref(params), None, C.byref(out)) == -2
     assert lib.jv_graph_add_nodes(g._h, bqv._h, 1, C.byref(params), None, C.byref(out), C.byref(ms)) == -2
     assert lib.jv_builder_create_from_graph(g._h, bqv._h, 1, C.byref(params), None, None, C.byref(out)) == -2
-    assert lib.jv_graph_remove_deleted(full._h, bqv._h, 1, 1.2, 0, _bptr(none), C.byref(out), C.byref(st)) == -2
+    assert lib.jv_graph_remove_deleted(full._h, bqv._h, 1, 1.2, 0, bd.bits(none), C.byref(out), C.byref(st)) == -2
     assert lib.jv_graph_add_nodes_pq(g._h, bqv._h, 1, C.byref(params), None, C.byref(out), C.byref(ms)) == -2
     assert lib.jv_builder_create_from_graph_pq(g._h, bqv._h, 1, C.byref(params), None, None, C.byref(out)) == -2
-    assert lib.jv_graph_remove_deleted_pq(full._h, bqv._h, 1, 1.2, 0, _bptr(none), C.byref(out), C.byref(st)) == -2
+    assert lib.jv_graph_remove_deleted_pq(full._h, bqv._h, 1, 1.2, 0, bd.bits(none), C.byref(out), C.byref(st)) == -2
     assert out.value is None
     # the same words without the stray bit build
     assert lib.jv_graph_build_bq(bqv._h, 1, C.byref(params), C.byref(out), C.byref(ms)) == 0

@@ -11,9 +11,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import build_model as bm
+import builder_driver as bd
+import graph_model as gm
 import oracle_lib as o
-import pq_build_model as pm
 from oracle_lib import bp, fp
 
 METRICS = (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)
@@ -26,7 +26,7 @@ def lossless_world(rng, n, dim, M, k, centroid):
     codes = rng.integers(0, k, (n, M)).astype(np.uint8)
     cen = rng.integers(-3, 4, dim).astype(np.float32) if centroid else None
     sizes, offsets = o.pq_layout(dim, M)
-    return codes, codebooks, cen, pm.decode(codes, codebooks, sizes, offsets, k, None)
+    return codes, codebooks, cen, gm.decode(codes, codebooks, sizes, offsets, k, None)
 
 
 def host_table(codebooks, dim, M, k, metric):
@@ -45,7 +45,7 @@ def test_model_pair_scores_match_oracle_diversity(oracle, metric):
     codebooks = rng.random(k * dim).astype(np.float32)  # positive entries: no cancellation, the two orders agree to a few ulps
     codes = rng.integers(0, k, (40, M)).astype(np.uint8)
     table = host_table(codebooks, dim, M, k, metric)
-    got = pm.pair_scores(metric, table, k, codes, codes)
+    got = gm.pair_scores(metric, table, k, codes, codes)
     for i in range(len(codes)):
         for j in range(len(codes)):
             want = oracle.jvo_pq_diversity_table(metric, fp(table), M, k, bp(codes[i]), bp(codes[j]))
@@ -59,8 +59,8 @@ def test_lossless_world_pq_model_equals_fp32_model(oracle, metric, centroid):
     n, dim, M, k = 500, 32, 8, 64
     codes, codebooks, cen, rows = lossless_world(rng, n, dim, M, k, centroid)
     kw = dict(M=8, beam=40, max_batch=0, window=-1)
-    pq = pm.PQBuildModel(oracle, codes, codebooks, k, dim, cen, host_table(codebooks, dim, M, k, metric), metric, **kw)
-    f32 = bm.BuildModel(oracle, rows, metric, **kw)
+    pq = gm.BuildModel(gm.PQScores(oracle, codes, codebooks, k, dim, cen, host_table(codebooks, dim, M, k, metric), metric), **kw)
+    f32 = gm.BuildModel(gm.F32Scores(oracle, rows, metric), **kw)
     # the two models in lock step, both adopting the PQ model's rows. The fp32 model scores pairs in float64: on integer rows an
     # isDiverse test whose pair distance equals the candidate's own distance is an exact tie, which fp32 (the device, the PQ model)
     # decides one way and float64 may decide the other; the fp32 model flags every such test, and only flagged rows may differ
@@ -100,64 +100,6 @@ def jv():
     return jvector_b200
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def step_build(jv, vectors, metric, params, pq):
-    """the builder driven the way sharded_build drives it on one GPU: (GraphIndex, (batches, truncated, dropped))"""
-    import torch
-
-    from jvector_b200 import _native as nat
-    lib = nat.init()
-    st = torch.cuda.current_stream().cuda_stream
-    b = C.c_void_p()
-    nat.check((lib.jv_builder_create_pq if pq else lib.jv_builder_create)(vectors._h, metric, C.byref(params), C.c_void_p(st), C.byref(b)))
-    try:
-        deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
-        nat.check(lib.jv_builder_info(b, C.byref(deg_), C.byref(cap_), C.byref(mb_)))
-        rows = torch.empty((mb_.value, deg_.value), dtype=torch.int32, device="cuda")
-        rdeg = torch.empty(mb_.value, dtype=torch.int32, device="cuda")
-        first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-
-        def reprune(L):
-            if L:
-                rp = torch.empty((L, cap_.value), dtype=torch.int32, device="cuda")
-                rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-                nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-                nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
-
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            if count.value == 0:
-                break
-            nat.check(lib.jv_builder_insert_slice(b, first.value, count.value, 0, count.value, _ptr(rows), _ptr(rdeg)))
-            nat.check(lib.jv_builder_apply_new(b, first.value, count.value, _ptr(rows), _ptr(rdeg), C.byref(L)))
-            reprune(L.value)
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune(L.value)
-        s = [C.c_int64() for _ in range(3)]
-        nat.check(lib.jv_builder_stats(b, *[C.byref(x) for x in s]))
-        g = C.c_void_p()
-        nat.check(lib.jv_builder_finish(b, C.byref(g), None))
-    finally:
-        lib.jv_builder_free(b)
-    return jv.GraphIndex(_handle=g), tuple(x.value for x in s)
-
-
-def graph_bytes(gi):
-    inf = gi.info()
-    return inf, [gi.level(lv) for lv in range(inf["levels"])]
-
-
-def assert_same_graph(a, b, what):
-    ia, la = graph_bytes(a)
-    ib, lb = graph_bytes(b)
-    assert ia == ib, (what, ia, ib)
-    for lv, ((ids_a, adj_a), (ids_b, adj_b)) in enumerate(zip(la, lb)):
-        assert np.array_equal(ids_a, ids_b) and np.array_equal(adj_a, adj_b), (what, "level", lv)
-
-
 # (metric, hierarchy, max_batch, window, centroid): the default schedule and 64-node batches with beam + window = 160
 LOSSLESS = [(o.EUCLIDEAN, False, 0, -1, True), (o.DOT_PRODUCT, True, 0, -1, False),
             (o.EUCLIDEAN, True, 64, 60, False), (o.DOT_PRODUCT, False, 64, 60, True)]
@@ -174,10 +116,10 @@ def test_lossless_world_byte_equal_to_fp32_build(jv, case):
     params = nat.BuildParams(16, 100, 1.2, 1.2, int(hier), 5, max_batch, window)
     pqv = jv.PQVectors(codes, codebooks, dim, k, cen)
     f32 = jv.F32Vectors(rows)
-    g_pq, s_pq = step_build(jv, pqv, metric, params, True)
-    g_f32, s_f32 = step_build(jv, f32, metric, params, False)
+    g_pq, s_pq = bd.step_build(pqv, metric, params, "_pq")
+    g_f32, s_f32 = bd.step_build(f32, metric, params)
     assert s_pq == s_f32 and s_pq[1] == 0, (s_pq, s_f32)
-    assert_same_graph(g_pq, g_f32, "lossless")
+    bd.assert_same_graph(g_pq, g_f32, "lossless")
     g_pq.close(), g_f32.close(), pqv.close(), f32.close()
 
 
@@ -224,81 +166,16 @@ def test_device_pq_build_equals_model(jv, oracle, case):
 
 
 def drive_build_pq(jv, oracle, pqv, world, metric, M, beam, window, max_batch, hier, cid):
-    """the build over pqv driven step by step (jv_builder_create_pq + jv_builder_*): each batch's inserted rows, overflow list and
-    re-pruned rows equal PQBuildModel's exactly, then the counters, the finished adjacency and the upper levels"""
-    import torch
-
+    """the build over pqv driven step by step (jv_builder_create_pq + jv_builder_*) against the PQ model over a pair table computed
+    on the host: every row equals the model's exactly"""
     from jvector_b200 import _native as nat
     codes, codebooks, cen, dim, k = world
-    n = codes.shape[0]
-    lib = nat.init()
-    seed = 3
-    params = nat.BuildParams(M, beam, 1.2, 1.2, int(hier), seed, max_batch, window)
-    st = torch.cuda.current_stream().cuda_stream
-    b = C.c_void_p()
-    nat.check(lib.jv_builder_create_pq(pqv._h, metric, C.byref(params), C.c_void_p(st), C.byref(b)))
-    table = exact_table(pqv, codebooks, dim, k, metric)  # the builder made the device's table
-    kw = dict(M=M, beam=beam, overflow=1.2, alpha=1.2, max_batch=max_batch, window=window)
-    model = pm.PQBuildModel(oracle, codes, codebooks, k, dim, cen, table, metric, **kw)
-    deg_, cap_, mb_ = C.c_int(), C.c_int(), C.c_int()
-    nat.check(lib.jv_builder_info(b, C.byref(deg_), C.byref(cap_), C.byref(mb_)))
-    assert (deg_.value, cap_.value) == (M, model.row_cap)
-    rows_t = torch.empty((mb_.value, M), dtype=torch.int32, device="cuda")
-    rdeg_t = torch.empty(mb_.value, dtype=torch.int32, device="cuda")
+    params = nat.BuildParams(M, beam, 1.2, 1.2, int(hier), 3, max_batch, window)
 
-    def reprune_round(L, lst, what):
-        assert L == len(lst), (what, "rows to re-prune", L, len(lst))
-        if L == 0:
-            return
-        rp = torch.empty((L, model.row_cap), dtype=torch.int32, device="cuda")
-        rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-        nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-        got, gdeg = rp.cpu().numpy(), rpd.cpu().numpy()
-        want, wdeg, _ = model.reprune_rows(lst)
-        bad = np.flatnonzero((got != want).any(1) | (gdeg != wdeg))
-        assert len(bad) == 0, (what, "re-pruned rows differ", [lst[i] for i in bad[:5]], got[bad[:1]].tolist(), want[bad[:1]].tolist())
-        model.apply_repruned(lst, got, gdeg)
-        nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
+    def scores():  # the builder made the device's table
+        return gm.PQScores(oracle, codes, codebooks, k, dim, cen, exact_table(pqv, codebooks, dim, k, metric), metric)
 
-    first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-    batches = 0
-    try:
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            f, c = first.value, count.value
-            if c == 0:
-                assert model.next_batch() is None
-                break
-            assert (f, c) == model.next_batch()
-            for lo, hi in ([(0, c // 2), (c // 2, c)] if batches % 2 else [(0, c)]):
-                nat.check(lib.jv_builder_insert_slice(b, f, c, lo, hi, _ptr(rows_t), _ptr(rdeg_t)))
-            got, gdeg = rows_t[:c].cpu().numpy(), rdeg_t[:c].cpu().numpy()
-            want, wdeg, _ = model.insert_rows(f, c)
-            bad = np.flatnonzero((got != want).any(1) | (gdeg != wdeg))
-            assert len(bad) == 0, (cid, "batch", batches, "rows differ", (f + bad[:5]).tolist(), got[bad[:1]].tolist(), want[bad[:1]].tolist())
-            nat.check(lib.jv_builder_apply_new(b, f, c, _ptr(rows_t), _ptr(rdeg_t), C.byref(L)))
-            reprune_round(L.value, model.apply_new(f, c, got, gdeg), (cid, "batch", batches))
-            batches += 1
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune_round(L.value, model.over_degree(), (cid, "cleanup"))
-        s = [C.c_int64() for _ in range(3)]
-        nat.check(lib.jv_builder_stats(b, *[C.byref(x) for x in s]))
-        g = C.c_void_p()
-        nat.check(lib.jv_builder_finish(b, C.byref(g), None))
-    finally:
-        lib.jv_builder_free(b)
-    gi = jv.GraphIndex(_handle=g)
-    assert tuple(x.value for x in s) == (batches, 0, model.dropped), (cid, [x.value for x in s], model.dropped)
-    _, adj = gi.level(0)
-    assert np.array_equal(adj, model.compact()), (cid, "finished adjacency")
-    if hier:
-        members, entry = bm.assign_levels(n, M, seed)
-        inf = gi.info()
-        assert inf["entry_node"] == entry and inf["levels"] == 1 + len(members), (cid, inf, entry)
-        for lv, (ids, want_adj) in enumerate(pm.upper_levels(oracle, codes, codebooks, k, dim, cen, table, metric, members, **kw), 1):
-            gids, gadj = gi.level(lv)
-            assert np.array_equal(gids, ids) and np.array_equal(gadj, want_adj), (cid, "level", lv)
-    gi.close()
+    bd.drive_build(nat.init(), pqv, metric, params, scores, cid, "_pq")[0].close()
 
 
 @pytest.mark.gpu
@@ -310,12 +187,12 @@ def test_pq_builds_reproduce(jv):
     b = jv.GraphIndexBuilder(o.DOT_PRODUCT, M=16, beamWidth=80, addHierarchy=True, seed=9)
     one, two = b.build(pqv), b.build(pqv)
     assert b.batches > 0 and b.scored_vectors > 0
-    assert_same_graph(one, two, "two calls")
-    steps, stats = step_build(jv, pqv, o.DOT_PRODUCT, nat.BuildParams(16, 80, 1.2, 1.2, 1, 9, 0, -1), True)
+    bd.assert_same_graph(one, two, "two calls")
+    steps, stats = bd.step_build(pqv, o.DOT_PRODUCT, nat.BuildParams(16, 80, 1.2, 1.2, 1, 9, 0, -1), "_pq")
     assert stats[0] == b.batches and stats[2] == b.dropped_backlinks
-    assert_same_graph(one, steps, "one call vs step-wise")
+    bd.assert_same_graph(one, steps, "one call vs step-wise")
     sharded, _, _ = parallel.sharded_build(None, pqv, o.DOT_PRODUCT, M=16, beamWidth=80, addHierarchy=True, seed=9)
-    assert_same_graph(one, sharded, "sharded_build")
+    bd.assert_same_graph(one, sharded, "sharded_build")
     for g in (one, two, steps, sharded):
         g.close()
     pqv.close()

@@ -14,13 +14,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import add_model as am
+import builder_driver as bd
 import delete_model as dm
+import graph_model as gm
 import oracle_lib as o
-import pq_build_model as pm
-import pq_maintain_model as mm
 from oracle_lib import fp, ip
-from test_graph_build_pq import assert_same_graph, exact_table, host_table, lossless_world, real_pq_world
+from test_graph_build_pq import exact_table, host_table, lossless_world, real_pq_world
 
 METRICS = (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)
 
@@ -39,11 +38,12 @@ def test_lossless_world_seeded_pq_model_equals_seeded_fp32_model(oracle, metric,
     codes, codebooks, cen, rows = lossless_world(rng, n, dim, M, k, centroid)
     table = host_table(codebooks, dim, M, k, metric)
     kw = dict(M=8, beam=40, max_batch=0, window=-1)
-    seed_adj, _ = pm.PQBuildModel(oracle, codes[:n0], codebooks, k, dim, cen, table, metric, **kw).build()
+    pqs = gm.PQScores(oracle, codes, codebooks, k, dim, cen, table, metric)
+    seed_adj, _ = gm.BuildModel(pqs.subset(np.arange(n0)), **kw).build()
     marks = rng.random(n0) < 0.05
     accept = np.concatenate([~marks, np.ones(n - n0, bool)])
-    pq = mm.SeededPQBuildModel(oracle, codes, codebooks, k, dim, cen, table, metric, seed_adj, 7, accept, **kw)
-    f32 = am.SeededBuildModel(oracle, rows, metric, seed_adj, 7, accept, **kw)
+    pq = gm.BuildModel(pqs, rows=seed_adj, entry=7, accept=accept, **kw)
+    f32 = gm.BuildModel(gm.F32Scores(oracle, rows, metric), rows=seed_adj, entry=7, accept=accept, **kw)
     assert pq.next_batch() == (n0, n0 // 32)
     # in lock step, both adopting the PQ model's rows; the fp32 model scores pairs in float64 and flags the isDiverse tests that
     # are exact ties on integer rows: only flagged rows may differ (test_graph_build_pq's lossless test)
@@ -83,14 +83,14 @@ def test_lossless_world_pq_repair_model_equals_delete_model(oracle, metric, cent
     codes, codebooks, cen, rows = lossless_world(rng, n, dim, M, k, centroid)
     table = host_table(codebooks, dim, M, k, metric)
     kw = dict(M=degree, beam=40, max_batch=0, window=-1)
-    adj0, _ = pm.PQBuildModel(oracle, codes, codebooks, k, dim, cen, table, metric, **kw).build()
+    pqs = gm.PQScores(oracle, codes, codebooks, k, dim, cen, table, metric)
+    adj0, _ = gm.BuildModel(pqs, **kw).build()
     ids = np.arange(0, n, 6, dtype=np.int32)
-    upper = [(i, a) for i, a in pm.upper_levels(oracle, codes, codebooks, k, dim, cen, table, metric, [ids], **kw)]
-    model = mm.PQRepairModel(oracle, codes, codebooks, k, dim, cen, table, metric, degree)
+    upper = [(i, a) for i, a, _ in gm.upper_levels(pqs, [ids], **kw)]
     for frac, kill_entry in ((0.05, False), (0.4, True)):
         deleted = rng.random(n) < frac
         deleted[0] = kill_entry
-        got = model.remove_deleted(adj0, 0, upper, deleted, seed=9)
+        got = dm.remove_deleted(pqs.queries, metric, adj0, 0, upper, deleted, seed=9, prune=pqs.prune)
         want = dm.remove_deleted(rows, metric, adj0, 0, upper, deleted, seed=9, key_scores=warp_keys(oracle, metric, rows))
         assert (got["entry"], got["levels"]) == (want["entry"], want["levels"])
         differ = repaired = 0
@@ -108,7 +108,7 @@ def test_lossless_world_pq_repair_model_equals_delete_model(oracle, metric, cent
 
 
 def test_repair_tiers_of_the_model():
-    assert [mm.repair_tier(c) for c in (1, 64, 65, 128, 256, 257, 1024, 1025, 2048, 2049, 4224)] == [0, 0, 1, 1, 2, 3, 3, 4, 4, 5, 5]
+    assert [dm.repair_tier(c) for c in (1, 64, 65, 128, 256, 257, 1024, 1025, 2048, 2049, 4224)] == [0, 0, 1, 1, 2, 3, 3, 4, 4, 5, 5]
 
 
 def test_pq_maintenance_entry_points_without_device():
@@ -133,27 +133,6 @@ def jv():
     return jvector_b200
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _levels(gi):
-    return [gi.level(lv) for lv in range(gi.info()["levels"])]
-
-
-def _bits(mask):
-    from jvector_b200.api import pack_accept_bits
-    return pack_accept_bits(mask) if mask is not None else None
-
-
-def _bptr(bits):
-    return bits.ctypes.data_as(C.POINTER(C.c_uint32)) if bits is not None else None
-
-
-def _builder(jv, metric, M, beam=60, hier=False, seed=3, **kw):
-    return jv.GraphIndexBuilder(metric, M=M, beamWidth=beam, neighborOverflow=1.2, alpha=1.2, addHierarchy=hier, seed=seed, **kw)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("metric", METRICS)
 @pytest.mark.parametrize("hier", (False, True), ids=("flat", "hier"))
@@ -162,16 +141,16 @@ def test_add_to_one_node_graph_is_the_pq_build(jv, metric, hier):
     _, codes, codebooks, cen = real_pq_world("anchor%d" % metric, n, dim, Mq, metric != o.DOT_PRODUCT)
     pqv = jv.PQVectors(codes, codebooks, dim, 256, cen)
     # a seed whose draw puts node 0 on level 1 or higher: the one-node graph then has the levels an add extends
-    seed = next(s for s in range(1, 400) if am.level_draws(n, M, s)[0] >= 1) if hier else 3
-    b = _builder(jv, metric, M, hier=hier, seed=seed)
+    seed = next(s for s in range(1, 400) if gm.level_draws(n, M, s)[0] >= 1) if hier else 3
+    b = bd.builder(jv, metric, M, hier=hier, seed=seed)
     built = b.build(pqv)
     want = (b.batches, b.dropped_backlinks)
     empty = np.full((1, M), -1, np.int32)
-    tops = int(am.level_draws(n, M, seed)[0]) if hier else 0
+    tops = int(gm.level_draws(n, M, seed)[0]) if hier else 0
     one = jv.GraphIndex(empty, 0, [(np.zeros(1, np.int32), empty)] * tops)
     added = b.addGraphNodes(one, pqv)
     assert (b.batches, b.dropped_backlinks) == want
-    assert_same_graph(added, built, ("one-node add", metric, hier))
+    bd.assert_same_graph(added, built, ("one-node add", metric, hier))
     assert built.info()["levels"] > 1 or not hier
     for h in (built, one, added, pqv):
         h.close()
@@ -184,15 +163,15 @@ def test_lossless_world_bytes_equal_the_fp32_calls(jv, metric, centroid):
     n0, n, dim, M, k = 7000, 8000, 32, 8, 256
     codes, codebooks, cen, rows = lossless_world(rng, n, dim, M, k, centroid)
     pqv, f32, f32_small = jv.PQVectors(codes, codebooks, dim, k, cen), jv.F32Vectors(rows), jv.F32Vectors(rows[:n0])
-    b = _builder(jv, metric, 16, beam=100, hier=True, seed=5)
+    b = bd.builder(jv, metric, 16, beam=100, hier=True, seed=5)
     g = b.build(f32_small)
     marks = rng.random(n0) < 0.03
     a_pq, a_f32 = b.addGraphNodes(g, pqv, marks), b.addGraphNodes(g, f32, marks)
-    assert_same_graph(a_pq, a_f32, "lossless add")
+    bd.assert_same_graph(a_pq, a_f32, "lossless add")
     deleted = rng.random(n) < 0.1
     deleted[a_pq.info()["entry_node"]] = True
     r_pq, r_f32 = b.removeDeletedNodes(a_pq, pqv, deleted), b.removeDeletedNodes(a_f32, f32, deleted)
-    assert_same_graph(r_pq, r_f32, "lossless removal")
+    bd.assert_same_graph(r_pq, r_f32, "lossless removal")
     assert r_pq.remove_stats["repaired_rows"] == r_f32.remove_stats["repaired_rows"] > 0
     assert r_pq.remove_stats["candidates"] == r_f32.remove_stats["candidates"]
     # the holes are the same too: a second removal of nothing counts them as gone in both
@@ -204,100 +183,17 @@ def test_lossless_world_bytes_equal_the_fp32_calls(jv, metric, centroid):
 
 
 def drive_add_pq(jv, oracle, pqv, world, g, metric, M, beam, window, max_batch, marks, cid):
-    """the add of code rows [n0, n) to g driven step by step (jv_builder_create_from_graph_pq + jv_builder_*): each batch's inserted
-    rows, overflow list and re-pruned rows equal the seeded PQ model's exactly; then the adjacency, counters, upper levels and entry;
-    then the one-call add gives the same bytes, twice"""
-    import torch
-
+    """the add of code rows [n0, n) to g driven step by step (jv_builder_create_from_graph_pq + jv_builder_*) against the seeded PQ
+    model over a pair table computed on the host: every row equals the model's exactly; then the one-call add gives the same bytes"""
     from jvector_b200 import _native as nat
     codes, codebooks, cen, dim, k = world
-    seed = 3
-    lib = nat.init()
-    n, n0 = codes.shape[0], g.info()["n"]
-    entry0, levels0 = g.info()["entry_node"], _levels(g)
-    params = nat.BuildParams(M, beam, 1.2, 1.2, 0, seed, max_batch, window)
-    bits = _bits(marks)
-    st = torch.cuda.current_stream().cuda_stream
-    b = C.c_void_p()
-    nat.check(lib.jv_builder_create_from_graph_pq(g._h, pqv._h, metric, C.byref(params), _bptr(bits), C.c_void_p(st), C.byref(b)))
-    table = exact_table(pqv, codebooks, dim, k, metric)
-    kw = dict(M=M, beam=beam, overflow=1.2, alpha=1.2, max_batch=max_batch, window=window)
-    accept = None if marks is None else np.concatenate([~marks, np.ones(n - n0, bool)])
-    model = mm.SeededPQBuildModel(oracle, codes, codebooks, k, dim, cen, table, metric, levels0[0][1], entry0, accept, **kw)
-    rows_t = torch.empty((model.max_batch, M), dtype=torch.int32, device="cuda")
-    rdeg_t = torch.empty(model.max_batch, dtype=torch.int32, device="cuda")
+    params = nat.BuildParams(M, beam, 1.2, 1.2, 0, 3, max_batch, window)
 
-    def reprune_round(L, lst, what):
-        assert L == len(lst), (what, "rows to re-prune", L, len(lst))
-        if L == 0:
-            return
-        rp = torch.empty((L, model.row_cap), dtype=torch.int32, device="cuda")
-        rpd = torch.empty(L, dtype=torch.int32, device="cuda")
-        nat.check(lib.jv_builder_reprune_slice(b, 0, L, _ptr(rp), _ptr(rpd)))
-        got, gdeg = rp.cpu().numpy(), rpd.cpu().numpy()
-        want, wdeg, _ = model.reprune_rows(lst)
-        bad = np.flatnonzero((got != want).any(1) | (gdeg != wdeg))
-        assert len(bad) == 0, (what, "re-pruned rows differ", [lst[i] for i in bad[:5]])
-        model.apply_repruned(lst, got, gdeg)
-        nat.check(lib.jv_builder_apply_repruned(b, L, _ptr(rp), _ptr(rpd)))
+    def scores():  # the builder made the device's table
+        return gm.PQScores(oracle, codes, codebooks, k, dim, cen, exact_table(pqv, codebooks, dim, k, metric), metric)
 
-    first, count, L = C.c_int32(), C.c_int32(), C.c_int32()
-    batches = 0
-    try:
-        while True:
-            nat.check(lib.jv_builder_next_batch(b, C.byref(first), C.byref(count)))
-            f, c = first.value, count.value
-            if c == 0:
-                assert model.next_batch() is None
-                break
-            assert (f, c) == model.next_batch()
-            for lo, hi in ([(0, c // 2), (c // 2, c)] if batches % 2 else [(0, c)]):
-                nat.check(lib.jv_builder_insert_slice(b, f, c, lo, hi, _ptr(rows_t), _ptr(rdeg_t)))
-            got, gdeg = rows_t[:c].cpu().numpy(), rdeg_t[:c].cpu().numpy()
-            want, wdeg, _ = model.insert_rows(f, c)
-            bad = np.flatnonzero((got != want).any(1) | (gdeg != wdeg))
-            assert len(bad) == 0, (cid, "batch", batches, "rows differ", (f + bad[:5]).tolist(), got[bad[:1]].tolist(), want[bad[:1]].tolist())
-            nat.check(lib.jv_builder_apply_new(b, f, c, _ptr(rows_t), _ptr(rdeg_t), C.byref(L)))
-            reprune_round(L.value, model.apply_new(f, c, got, gdeg), (cid, "batch", batches))
-            batches += 1
-        nat.check(lib.jv_builder_collect_over_degree(b, C.byref(L)))
-        reprune_round(L.value, model.over_degree(), (cid, "cleanup"))
-        s = [C.c_int64() for _ in range(3)]
-        nat.check(lib.jv_builder_stats(b, *[C.byref(x) for x in s]))
-        h = C.c_void_p()
-        nat.check(lib.jv_builder_finish(b, C.byref(h), None))
-    finally:
-        lib.jv_builder_free(b)
-    gi = jv.GraphIndex(_handle=h)
-    assert batches > 0 and tuple(x.value for x in s) == (batches, 0, model.dropped), (cid, [x.value for x in s], model.dropped)
-    assert np.array_equal(gi.level(0)[1], model.compact()), (cid, "finished adjacency")
-    inf = gi.info()
-    if len(levels0) > 1:
-        want_levels, want_entry = mm.extend_levels(oracle, codes, codebooks, k, dim, cen, table, metric, levels0[1:], entry0, n0, seed, marks, **kw)
-        assert inf["entry_node"] == want_entry and inf["levels"] == 1 + len(want_levels), (cid, inf, want_entry, len(want_levels))
-        for lv, (ids, want_adj) in enumerate(want_levels, 1):
-            gids, gadj = gi.level(lv)
-            assert np.array_equal(gids, ids) and np.array_equal(gadj, want_adj), (cid, "level", lv)
-    else:
-        assert inf["levels"] == 1 and inf["entry_node"] == model.entry, (cid, inf, model.entry)
-    ms = C.c_double()
-    one = []
-    for _ in range(2):
-        h1 = C.c_void_p()
-        nat.check(lib.jv_graph_add_nodes_pq(g._h, pqv._h, metric, C.byref(params), _bptr(bits), C.byref(h1), C.byref(ms)))
-        one.append(jv.GraphIndex(_handle=h1))
-    assert_same_graph(gi, one[0], (cid, "step-wise vs one call"))
-    assert_same_graph(one[0], one[1], (cid, "two calls"))
-    sv, nb, nd = C.c_int64(), C.c_int64(), C.c_int64()
-    lib.jv_graph_build_stats(C.byref(sv), C.byref(nb), C.byref(nd))
-    assert (nb.value, nd.value) == (batches, model.dropped) and sv.value > 0 and ms.value > 0
-    for x in one:
-        x.close()
-    if marks is not None:
-        marked = np.concatenate([marks, np.zeros(n - n0, bool)])
-        for lv, (ids, ladj) in enumerate(_levels(gi)):
-            new_rows = ladj[ids >= n0]
-            assert not marked[new_rows[new_rows >= 0]].any(), (cid, "a new row names a marked node on level", lv)
+    gi, _, batches, _, _ = bd.drive_add(nat.init(), g, pqv, metric, params, marks, scores, cid, "_pq")
+    assert batches > 0
     return gi
 
 
@@ -318,7 +214,7 @@ def test_stepwise_pq_add_equals_model(jv, oracle, case):
     rng = np.random.default_rng(sum(map(ord, cid)))
     _, codes, codebooks, cen = real_pq_world(cid, n, dim, Mq, centroid)
     small, pqv = jv.PQVectors(codes[:n0], codebooks, dim, 256, cen), jv.PQVectors(codes, codebooks, dim, 256, cen)
-    b = _builder(jv, metric, M, beam=beam, hier=hier, max_batch=max_batch, concurrent_window=window)
+    b = bd.builder(jv, metric, M, beam=beam, hier=hier, max_batch=max_batch, concurrent_window=window)
     g = b.build(small)
     marks = None
     if origin == "marked":
@@ -328,11 +224,11 @@ def test_stepwise_pq_add_equals_model(jv, oracle, case):
     elif origin == "all_removed":
         g = b.removeDeletedNodes(g, small, np.ones(n0, bool))
         assert g.info()["entry_node"] == -1
-    before = _levels(g)
+    before = bd.levels(g)
     gi = drive_add_pq(jv, oracle, pqv, (codes, codebooks, cen, dim, 256), g, metric, M, beam, window, max_batch, marks, cid)
     if origin == "all_removed":
         assert gi.info()["entry_node"] == n0
-    after = _levels(g)  # the input graph is untouched
+    after = bd.levels(g)  # the input graph is untouched
     assert len(before) == len(after) and all(np.array_equal(a[0], c[0]) and np.array_equal(a[1], c[1]) for a, c in zip(before, after))
     for h in (g, gi, small, pqv):
         h.close()
@@ -342,28 +238,12 @@ def test_stepwise_pq_add_equals_model(jv, oracle, case):
 def test_zero_new_rows_copies_the_graph(jv):
     _, codes, codebooks, cen = real_pq_world("zero", 1200, 32, 8, True)
     pqv = jv.PQVectors(codes, codebooks, 32, 256, cen)
-    b = _builder(jv, o.DOT_PRODUCT, 16, hier=True)
+    b = bd.builder(jv, o.DOT_PRODUCT, 16, hier=True)
     g = b.build(pqv)
     same = b.addGraphNodes(g, pqv)
-    assert_same_graph(g, same, "n == n0")
+    bd.assert_same_graph(g, same, "n == n0")
     for h in (g, same, pqv):
         h.close()
-
-
-def assert_removal_matches_model(gi, res, what):
-    inf = gi.info()
-    assert inf["entry_node"] == res["entry"] and inf["levels"] == res["levels"], (what, inf, res["entry"], res["levels"])
-    want = [(np.arange(res["adj0"].shape[0], dtype=np.int32), res["adj0"])] + list(res["upper"])
-    for L, ((dids, dadj), (wids, wadj)) in enumerate(zip(_levels(gi), want)):
-        assert np.array_equal(dids, wids), (what, "members of level", L)
-        bad = np.flatnonzero((dadj != wadj).any(1))
-        assert len(bad) == 0, (what, "level", L, "rows differ", wids[bad[:5]].tolist(), dadj[bad[:1]].tolist(), wadj[bad[:1]].tolist())
-    cands = [len(r["cands"] - {v}) for lv in res["rows"] for v, r in lv.items()]
-    st = gi.remove_stats
-    assert st["repaired_rows"] == len(cands) and st["candidates"] == sum(cands) and st["max_candidates"] == max(cands, default=0), (what, st)
-    assert st["random_fallbacks"] == sum(r["fallback"] for lv in res["rows"] for r in lv.values()), (what, st)
-    assert st["live_nodes"] == (~res["dead"]).sum()
-    return np.bincount([mm.repair_tier(c) for c in cands], minlength=len(mm.PQ_REPAIR_TIERS))
 
 
 # (id, dim, PQ M, centroid, metric, degree, hierarchy, n, deleted fraction, entry deleted, tiers that must be hit)
@@ -382,20 +262,20 @@ def test_pq_removal_equals_model(jv, oracle, case):
     rng = np.random.default_rng(sum(map(ord, cid)))
     _, codes, codebooks, cen = real_pq_world(cid, n, dim, Mq, centroid)
     pqv = jv.PQVectors(codes, codebooks, dim, 256, cen)
-    b = _builder(jv, metric, M, hier=hier, seed=17)
+    b = bd.builder(jv, metric, M, hier=hier, seed=17)
     g = b.build(pqv)
-    levels, entry = _levels(g), g.info()["entry_node"]
+    levels, entry = bd.levels(g), g.info()["entry_node"]
     deleted = rng.random(n) < frac
     deleted[entry] = kill_entry
     got, again = b.removeDeletedNodes(g, pqv, deleted), b.removeDeletedNodes(g, pqv, deleted)
-    assert_same_graph(got, again, (cid, "two calls"))
-    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, metric), metric, M)
-    res = model.remove_deleted(levels[0][1], entry, levels[1:], deleted, seed=17)
-    hit = assert_removal_matches_model(got, res, cid)
+    bd.assert_same_graph(got, again, (cid, "two calls"))
+    pqs = gm.PQScores(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, metric), metric)
+    res = dm.remove_deleted(pqs.queries, metric, levels[0][1], entry, levels[1:], deleted, seed=17, prune=pqs.prune)
+    hit = bd.assert_removal_matches_model(got, res, cid)
     print(cid, "rows per tier", hit.tolist(), got.remove_stats)
     assert all(hit[t] > 0 for t in tiers), (cid, hit.tolist(), tiers)
     assert got.remove_stats["removed"] == deleted.sum() and (not kill_entry or got.info()["entry_node"] != entry)
-    after = _levels(g)
+    after = bd.levels(g)
     assert all(np.array_equal(a[0], c[0]) and np.array_equal(a[1], c[1]) for a, c in zip(levels, after))
     for h in (g, got, again, pqv):
         h.close()
@@ -430,11 +310,11 @@ def test_pq_removal_hits_every_tier_on_a_made_graph(jv, oracle):
             adj[j] = pick(j, M, pool)
     deleted[rng.choice(np.flatnonzero(~deleted[100:]) + 100, 60, replace=False)] = True  # ordinary nodes
     g = jv.GraphIndex(adj, 0)
-    b = _builder(jv, o.DOT_PRODUCT, M, seed=5)
+    b = bd.builder(jv, o.DOT_PRODUCT, M, seed=5)
     got = b.removeDeletedNodes(g, pqv, deleted)
-    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, o.DOT_PRODUCT), o.DOT_PRODUCT, M)
-    res = model.remove_deleted(adj, 0, [], deleted, seed=5)
-    hit = assert_removal_matches_model(got, res, "made graph")
+    pqs = gm.PQScores(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, o.DOT_PRODUCT), o.DOT_PRODUCT)
+    res = dm.remove_deleted(pqs.queries, o.DOT_PRODUCT, adj, 0, [], deleted, seed=5, prune=pqs.prune)
+    hit = bd.assert_removal_matches_model(got, res, "made graph")
     print("made graph: rows per tier", hit.tolist(), got.remove_stats)
     assert (hit > 0).all() and got.remove_stats["max_candidates"] > 2048, hit.tolist()
     for h in (g, got, pqv):
@@ -447,20 +327,20 @@ def test_pq_removal_fallback_and_everything_deleted(jv, oracle):
     n, dim, Mq, M = 2000, 32, 8, 16
     _, codes, codebooks, cen = real_pq_world("fallback", n, dim, Mq, False)
     pqv = jv.PQVectors(codes, codebooks, dim, 256, cen)
-    b = _builder(jv, o.EUCLIDEAN, M, beam=40, hier=True, seed=12)
+    b = bd.builder(jv, o.EUCLIDEAN, M, beam=40, hier=True, seed=12)
     g = b.build(pqv)
-    levels, entry = _levels(g), g.info()["entry_node"]
+    levels, entry = bd.levels(g), g.info()["entry_node"]
     deleted = np.ones(n, bool)
     deleted[rng.choice(n, 50, replace=False)] = False
     got = b.removeDeletedNodes(g, pqv, deleted)
-    model = mm.PQRepairModel(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, o.EUCLIDEAN), o.EUCLIDEAN, M)
-    res = model.remove_deleted(levels[0][1], entry, levels[1:], deleted, seed=12)
-    assert_removal_matches_model(got, res, "fallback")
+    pqs = gm.PQScores(oracle, codes, codebooks, 256, dim, cen, exact_table(pqv, codebooks, dim, 256, o.EUCLIDEAN), o.EUCLIDEAN)
+    res = dm.remove_deleted(pqs.queries, o.EUCLIDEAN, levels[0][1], entry, levels[1:], deleted, seed=12, prune=pqs.prune)
+    bd.assert_removal_matches_model(got, res, "fallback")
     assert got.remove_stats["random_fallbacks"] > 0
     empty = b.removeDeletedNodes(g, pqv, np.ones(n, bool))
     inf = empty.info()
     assert inf["entry_node"] == -1 and inf["levels"] == 1 and empty.remove_stats["live_nodes"] == 0 and (empty.level(0)[1] == -1).all()
-    r = jv.GraphSearcher(empty).search(pqv, pm.decode(codes[:4], codebooks, *o.pq_layout(dim, Mq), 256, cen), o.EUCLIDEAN, 5, 10)
+    r = jv.GraphSearcher(empty).search(pqv, gm.decode(codes[:4], codebooks, *o.pq_layout(dim, Mq), 256, cen), o.EUCLIDEAN, 5, 10)
     assert (r.nodes == -1).all() and (r.scores == 0).all()
     for h in (g, got, empty, pqv):
         h.close()
@@ -472,7 +352,7 @@ def test_pq_remove_add_remove_keeps_holes(jv):
     n0, n, dim = 3600, 4000, 32
     _, codes, codebooks, cen = real_pq_world("holes", n, dim, 8, True)
     small, pqv = jv.PQVectors(codes[:n0], codebooks, dim, 256, cen), jv.PQVectors(codes, codebooks, dim, 256, cen)
-    b = _builder(jv, o.DOT_PRODUCT, 16, hier=True, seed=4)
+    b = bd.builder(jv, o.DOT_PRODUCT, 16, hier=True, seed=4)
     g = b.build(small)
     first = rng.random(n0) < 0.1
     rep = b.removeDeletedNodes(g, small, first)
@@ -504,7 +384,7 @@ def test_maintained_pq_graph_recall(jv):
     codes = jv.pq_encode_all(base, codebooks, M)
     vsf = o.DOT_PRODUCT
     f32, pqv = jv.F32Vectors(base), jv.PQVectors(codes, codebooks, dim)
-    b = _builder(jv, vsf, 16, beam=100, hier=True, seed=9)
+    b = bd.builder(jv, vsf, 16, beam=100, hier=True, seed=9)
 
     def walk(g, pq_set, rerank, **kw):
         return jv.GraphSearcher(g).search(pq_set, queries, vsf, 10, 100, reranker=rerank, **kw).nodes
@@ -542,7 +422,7 @@ def test_fused_pq_walk_on_maintained_pq_graph(jv, oracle):
     cb, sizes, offsets = o.train_pq_numpy(rng, data[:1500], M, k, iters=2)
     codes = o.encode_pq(oracle, cb, sizes, offsets, M, k, None, data)
     small, pqv, vec = jv.PQVectors(codes[:n0], cb, dim, k), jv.PQVectors(codes, cb, dim, k), jv.F32Vectors(data)
-    b = _builder(jv, o.DOT_PRODUCT, 16, beam=40, hier=True, seed=6)
+    b = bd.builder(jv, o.DOT_PRODUCT, 16, beam=40, hier=True, seed=6)
     g = b.build(small)
     grown = b.addGraphNodes(g, pqv)
     rep = b.removeDeletedNodes(grown, pqv, rng.random(n) < 0.1)
@@ -583,7 +463,7 @@ def test_pq_maintenance_errors(jv):
     full = jv.GraphIndex(np.full((300, 8), -1, np.int32), 0)
     params = nat.BuildParams(8, 30, 1.2, 1.2, 0, 0, 0, -1)
     out, ms, st = C.c_void_p(), C.c_double(), nat.RemoveStats()
-    none = np.zeros(10, np.uint32)
+    none = np.zeros(300, bool)
 
     def add(graph, ds, metric=1, p=params, o_=C.byref(out)):
         a = lib.jv_graph_add_nodes_pq(graph, ds, metric, C.byref(p) if p is not None else None, None, o_, C.byref(ms))
@@ -592,7 +472,7 @@ def test_pq_maintenance_errors(jv):
         return a
 
     def remove(graph, ds, metric=1, alpha=1.2, bits=none, o_=C.byref(out), st_=C.byref(st)):
-        return lib.jv_graph_remove_deleted_pq(graph, ds, metric, alpha, 0, _bptr(bits), o_, st_)
+        return lib.jv_graph_remove_deleted_pq(graph, ds, metric, alpha, 0, bd.bits(bits), o_, st_)
 
     assert add(None, pqv._h) == -2 and add(g._h, None) == -2 and add(g._h, pqv._h, p=None) == -2 and add(g._h, pqv._h, o_=None) == -2
     assert add(g._h, f32._h) == -2  # not PQ
@@ -623,7 +503,7 @@ def test_pq_maintenance_errors(jv):
     # the fp32 entry points still refuse a PQ data set
     assert lib.jv_graph_add_nodes(g._h, pqv._h, 1, C.byref(params), None, C.byref(out), C.byref(ms)) == -2
     assert lib.jv_builder_create_from_graph(g._h, pqv._h, 1, C.byref(params), None, None, C.byref(out)) == -2
-    assert lib.jv_graph_remove_deleted(full._h, pqv._h, 1, 1.2, 0, _bptr(none), C.byref(out), C.byref(st)) == -2
+    assert lib.jv_graph_remove_deleted(full._h, pqv._h, 1, 1.2, 0, bd.bits(none), C.byref(out), C.byref(st)) == -2
     assert out.value is None
     for h in (pqv, short, f32, g, full, wide, wide_full, m128, deg64, deg32, big):
         h.close()

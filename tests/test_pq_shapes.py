@@ -16,9 +16,8 @@ from fractions import Fraction
 import numpy as np
 import pytest
 
+import graph_model as gm
 import oracle_lib as o
-import pq_build_model as pm
-import pq_maintain_model as mm
 from oracle_lib import bp, fp, ip
 
 METRICS = (o.EUCLIDEAN, o.DOT_PRODUCT, o.COSINE)
@@ -165,7 +164,7 @@ def test_host_pair_table_against_oracle(oracle, shape):
             g, t = got[m * block:(m + 1) * block], want[m * block:(m + 1) * block]
             assert (np.abs(g - terms.sum(1)) <= bound).all() and (np.abs(g.astype(np.float64) - t) <= 2 * bound).all(), (shape, metric, m)
             if metric == o.EUCLIDEAN and k >= 3:
-                assert g[pm.tri_index(0, k - 1, k)] == 0  # duplicated centroids
+                assert g[gm.tri_index(0, k - 1, k)] == 0  # duplicated centroids
 
 
 def tri_invert(t, k):
@@ -180,11 +179,11 @@ def tri_invert(t, k):
 
 
 def test_triangular_index_for_every_k():
-    # tri_index (scorers.cuh, pq_build_model) and the kernel's inversion agree with the row-order upper triangle at every k
+    # tri_index (scorers.cuh, graph_model) and the kernel's inversion agree with the row-order upper triangle at every k
     for k in range(1, 257):
         iu, ju = np.triu_indices(k)
         t = np.arange(len(iu))
-        assert np.array_equal(pm.tri_index(iu, ju, k), t) and np.array_equal(pm.tri_index(ju, iu, k), t), k
+        assert np.array_equal(gm.tri_index(iu, ju, k), t) and np.array_equal(gm.tri_index(ju, iu, k), t), k
         i, j = tri_invert(t, k)
         assert np.array_equal(i, iu) and np.array_equal(j, ju), k
 
@@ -202,7 +201,7 @@ def test_oracle_encode_ties_and_model_pair_scores(oracle, shape):
     a, b = rng.integers(0, N, 40), rng.integers(0, N, 40)
     for metric in METRICS:
         table = o.pq_pair_table_exact(w["cb"], dim, M, k, metric)
-        got = np.diagonal(pm.pair_scores(metric, table, k, codes[a], codes[b]))
+        got = np.diagonal(gm.pair_scores(metric, table, k, codes[a], codes[b]))
         want = np.array([oracle.jvo_pq_diversity_table(metric, fp(table), M, k, bp(codes[x]), bp(codes[y])) for x, y in zip(a, b)], F32)
         bound = diversity_bound(metric, table, k, codes[a], codes[b])
         assert (np.abs(got.astype(np.float64) - want) <= bound).all(), (shape, metric, np.abs(got - want).max(), bound.min())
@@ -218,7 +217,7 @@ def diversity_bound(metric, table, k, ca, cb):
     T = np.asarray(table, F32).reshape(M, -1).astype(np.float64)
 
     def entries(x, y):
-        return np.stack([T[m][pm.tri_index(x[:, m], y[:, m], k)] for m in range(M)], 1)
+        return np.stack([T[m][gm.tri_index(x[:, m], y[:, m], k)] for m in range(M)], 1)
 
     t = entries(ca, cb)
     s, e = t.sum(1), 2 * (M + 5) * u * np.abs(t).sum(1)  # e: the two orders' sums, apart
@@ -293,7 +292,7 @@ def check_pairs(jv, oracle, pqv, codes, cb, dim, M, k, cen, a, b, what):
         pqv.build_pair_table(metric)
         bits_equal(pqv.pair_table(metric), table, what + (metric, "pair table"))
         got = pqv.diversity_scores(a, b, metric)
-        want = np.diagonal(pm.pair_scores(metric, table, k, codes[a], codes[b]))
+        want = np.diagonal(gm.pair_scores(metric, table, k, codes[a], codes[b]))
         bits_equal(got, want, what + (metric, "pair_pq_table"))
         bits_equal(direct, want, what + (metric, "pair_pq"))
         seq = np.array([oracle.jvo_pq_diversity_table(metric, fp(table), M, k, bp(codes[x]), bp(codes[y])) for x, y in zip(a, b)], F32)
@@ -393,8 +392,10 @@ NB = 1500
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", MAINTAIN, ids=[c[0] for c in MAINTAIN])
 def test_build_add_remove_equal_the_models(jv, oracle, case):
+    import builder_driver as bd
+    import delete_model as dm
     from test_graph_build_pq import drive_build_pq, exact_table
-    from test_graph_maintain_pq import _builder, _levels, assert_removal_matches_model, drive_add_pq
+    from test_graph_maintain_pq import drive_add_pq
     shape, metric, degree, beam, hier = case
     w = host_world(shape)
     dim, M, k, cen, codes, cb = w["dim"], w["M"], w["k"], w["cen"], w["codes"][:NB], w["cb"]
@@ -405,17 +406,17 @@ def test_build_add_remove_equal_the_models(jv, oracle, case):
     # an add of 300 rows into a graph built over the first 1200
     n0 = NB - 300
     small = jv.PQVectors(codes[:n0], cb, dim, k, cen)
-    b = _builder(jv, metric, degree, beam=beam, hier=hier)
+    b = bd.builder(jv, metric, degree, beam=beam, hier=hier)
     g = b.build(small)
     gi = drive_add_pq(jv, oracle, pqv, world, g, metric, degree, beam, -1, 0, None, shape)
     # a removal of about 10 % of the added graph's nodes
     rng = np.random.default_rng(k)
-    levels, entry = _levels(gi), gi.info()["entry_node"]
+    levels, entry = bd.levels(gi), gi.info()["entry_node"]
     deleted = rng.random(NB) < 0.1
     got = b.removeDeletedNodes(gi, pqv, deleted)
-    model = mm.PQRepairModel(oracle, codes, cb, k, dim, cen, exact_table(pqv, cb, dim, k, metric), metric, degree)
-    res = model.remove_deleted(levels[0][1], entry, levels[1:], deleted, seed=3)
-    hit = assert_removal_matches_model(got, res, shape)
+    pqs = gm.PQScores(oracle, codes, cb, k, dim, cen, exact_table(pqv, cb, dim, k, metric), metric)
+    res = dm.remove_deleted(pqs.queries, metric, levels[0][1], entry, levels[1:], deleted, seed=3, prune=pqs.prune)
+    hit = bd.assert_removal_matches_model(got, res, shape)
     assert (hit > 0).sum() >= 2, (shape, hit.tolist())
     for h in (g, gi, got, small, pqv):
         h.close()
