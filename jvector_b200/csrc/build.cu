@@ -141,13 +141,135 @@ __device__ __forceinline__ float pair_bq_row(const DataDesc &d, int a, const uns
     return bq_score_from_hd(group_sum_int<32>(hd), d.dim);
 }
 
+// ------------------------------------------------------------------------------------------------
+// The steps the prune kernels share. Per row: the row's candidates (PruneRow), their keys against v (prune_keys_f32; prune_kernel
+// has its own passes over codes), the sort and state reset, the selection (prune_select_gram over a Gram matrix; prune_kernel folds
+// one selected row at a time) and the write-out (prune_write_row; prune_kernel's bounded tiers write with one thread per neighbour).
+// The sort and prune_kernel's next-pick scan stay written out in each kernel: as shared functions they change the register
+// allocation of the BQ and Gram instantiations, and the BQ ones already spill.
+// ------------------------------------------------------------------------------------------------
+
+// row `it` of a launch: node v, its candidates cand[0, ncs) followed (mode 0) by the in-progress window, nc of them in all up to
+// the kernel's capacity; a is the repaired row's slot (mode 2)
+struct PruneRow {
+    int a, v, nc, ncs;
+    const int32_t *cand;
+    __device__ __forceinline__ PruneRow(const PruneParams &P, int it, int cap)
+    {
+        a = P.mode == 2 ? P.list[it] : 0;
+        v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
+        if (P.mode == 0) {
+            cand = P.cand + (size_t)it * P.cand_stride;
+            ncs = P.cand_stride;
+            nc = ncs + P.window;
+        } else if (P.mode == 2) {
+            cand = P.cand + P.cand_off[a];
+            ncs = nc = P.cand_cnt[a];
+        } else {
+            cand = P.adj + (size_t)v * P.row_cap;
+            ncs = nc = min(P.deg[v], P.row_cap);
+        }
+        nc = min(nc, cap);
+    }
+};
+
+// the last alpha the reference loop reaches: 1.0, 1.2, ... while <= alpha + 1e-6
+__device__ __forceinline__ float prune_alpha_max(float alpha)
+{
+    float alpha_max = 1.0f;
+    for (float a = 1.0f; a <= alpha + 1e-6f; a += 0.2f) alpha_max = a;
+    return alpha_max;
+}
+
+// exact fp32 scores of the row's candidates against v (blob: prepare_blob of v's row) as sortable keys in keys[0, CAP), two rows
+// per warp at a time; KEY_MIN for an empty slot and for v itself
+template <int METRIC, int CAP>
+__device__ __forceinline__ void prune_keys_f32(const PruneParams &P, const PruneRow &r, const float *blob, long long *keys, int warp, int lane)
+{
+    constexpr int NW = PRUNE_THREADS / 32;
+    for (int i = warp; i < CAP; i += 2 * NW) {
+        const int i2 = i + NW;
+        const int32_t ca = i < r.nc ? prune_candidate(P, r.cand, r.ncs, r.v, i) : -1, cb = (i2 < CAP && i2 < r.nc) ? prune_candidate(P, r.cand, r.ncs, r.v, i2) : -1;
+        const bool va = ca >= 0 && ca != r.v, vb = cb >= 0 && cb != r.v;
+        long long ka = KEY_MIN, kb = KEY_MIN;
+        if (va || vb) {
+            float sa, sb;
+            score_f32_pair<METRIC>(P.d, blob, va ? ca : cb, vb ? cb : ca, lane, sa, sb);
+            if (va) ka = topk_key(sa, ca);
+            if (vb) kb = topk_key(sb, cb);
+        }
+        if (lane == 0) {
+            keys[i] = ka;
+            if (i2 < CAP) keys[i2] = kb;
+        }
+    }
+}
+
 // retainDiverse (VamanaDiversityProvider.java:45-95), restated so that the pair scores can be produced in bulk:
 //   isDiverse(c) at alpha  <=>  max over the selected s of sim(c, s)  <=  score(c) * alpha.
-// Keep M[c] = that running maximum. Selecting a candidate s updates M[c] for every still-eligible c in parallel (one warp
-// per candidate, the new row cached in shared memory); the sequential part of the reference loop shrinks to "find the next
-// c at or after the cursor with M[c] <= score(c) * alpha", a flag scan. A candidate whose M[c] already exceeds
-// score(c) * alpha_max can never be selected in any pass (M only grows) and is dropped from further updates. The selection
-// sequence — and therefore the neighbour list — is exactly the reference loop's, including the alpha = 1.0, 1.2 passes.
+// Keep M[c] = that running maximum (maxsim). Selecting a candidate s updates M[c] for every still-eligible c in parallel (the
+// kernel's fold); the sequential part of the reference loop shrinks to "find the next c at or after the cursor with
+// M[c] <= score(c) * alpha", a flag scan (prune_next). A candidate whose M[c] already exceeds score(c) * alpha_max can never be
+// selected in any pass (M only grows) and is dropped from further updates. The selection sequence — and therefore the neighbour
+// list — is exactly the reference loop's, including the alpha = 1.0, 1.2 passes.
+
+// the next eligible candidate at or after the cursor that is diverse at alpha, INT_MAX if there is none; ends on a barrier
+__device__ __forceinline__ int prune_next(const long long *keys, const float *maxsim, const uint8_t *state, int cursor, int nvalid, float alpha,
+                                          int *s_next)
+{
+    if (threadIdx.x == 0) *s_next = INT_MAX;
+    __syncthreads();
+    for (int i = cursor + threadIdx.x; i < nvalid; i += PRUNE_THREADS)
+        if (state[i] == 0 && !(maxsim[i] > __fmul_rn(key_score(keys[i]), alpha))) { atomicMin(s_next, i); break; }
+    __syncthreads();
+    return *s_next;
+}
+
+// the selection over a precomputed similarity matrix C (pitch CP, row i = sorted candidate i): the fold reads column `pick`
+template <int CP>
+__device__ __forceinline__ void prune_select_gram(const PruneParams &P, const float *C, const long long *keys, float *maxsim, uint8_t *state,
+                                                  int nvalid, float alpha_max, int *s_next)
+{
+    int nsel = 0;
+    float currentAlpha = 1.0f;
+    while (currentAlpha <= P.alpha + 1e-6f && nsel < P.degree) {
+        int cursor = 0;
+        while (nsel < P.degree) {
+            const int pick = prune_next(keys, maxsim, state, cursor, nvalid, currentAlpha, s_next);
+            if (pick == INT_MAX) break;
+            nsel++;
+            cursor = pick + 1;
+            for (int i = threadIdx.x; i < nvalid; i += PRUNE_THREADS) {
+                if (i == pick) state[i] = 1;
+                else if (state[i] == 0) {
+                    const float m = fmaxf(maxsim[i], C[i * CP + pick]);
+                    maxsim[i] = m;
+                    if (m > __fmul_rn(key_score(keys[i]), alpha_max)) state[i] = 2;
+                }
+            }
+            __syncthreads();
+        }
+        currentAlpha += 0.2f;
+    }
+}
+
+// the selected neighbours (state 1) in score order (NodeArray.retain keeps the sorted order), -1 padded, to out_rows[oi] (a sharded
+// build's slice, or the repair's row a) or in place to v's adjacency row; node_of(i) is the node of sorted candidate i. One thread.
+template <typename NodeOf>
+__device__ __forceinline__ void prune_write_row(const PruneParams &P, const PruneRow &r, int it, const uint8_t *state, int nvalid, NodeOf node_of)
+{
+    int w = 0;
+    const int oi = P.mode == 2 ? r.a : P.out_base + it;
+    int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)r.v * P.row_cap;
+    const int width = P.out_rows ? P.out_stride : P.row_cap;
+    for (int i = 0; i < nvalid; i++)
+        if (state[i] == 1) row[w++] = node_of(i);
+    for (int i = w; i < width; i++) row[i] = -1;
+    if (P.out_rows) P.out_deg[oi] = w;
+    else P.deg[r.v] = w;
+    if (P.mode == 1 && P.mark) P.mark[r.v] = 0;
+}
+
 // MAXC: candidate capacity (power of two). The builder uses PRUNE_MAXC; the repair of deleted neighbours also instantiates
 // larger capacities so that no candidate set is ever clipped.
 // KIND_PQ (pqBuildScoreProvider, §4.3c): v's query is decode(c_v) (pq_decode_row, into the row slot), its LUT is prepare_blob's, the
@@ -180,30 +302,14 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
     constexpr int NW = PRUNE_THREADS / 32;
     const int total = P.count_ptr ? *P.count_ptr : P.count;
     const int n4 = P.d.stride >> 2;
-    // the last alpha the reference loop reaches: 1.0, 1.2, ... while <= alpha + 1e-6
-    float alpha_max = 1.0f;
-    for (float a = 1.0f; a <= P.alpha + 1e-6f; a += 0.2f) alpha_max = a;
+    const float alpha_max = prune_alpha_max(P.alpha);
 
     for (int it = blockIdx.x; it < total; it += gridDim.x) {
-        const int a = P.mode == 2 ? P.list[it] : 0;
-        const int v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
-        const int32_t *cand;
-        int nc, ncs;
-        if (P.mode == 0) {
-            cand = P.cand + (size_t)it * P.cand_stride;
-            ncs = P.cand_stride;
-            nc = ncs + P.window;
-        } else if (P.mode == 2) {
-            cand = P.cand + P.cand_off[a];
-            ncs = nc = P.cand_cnt[a];
-        } else {
-            cand = P.adj + (size_t)v * P.row_cap;
-            ncs = nc = min(P.deg[v], P.row_cap);
-        }
-        nc = min(nc, MAXC);
+        const PruneRow r(P, it, MAXC);
+        const int v = r.v;
         int cap = MAXC;
         if (BOUNDED)
-            for (cap = PRUNE_MAXC; cap < nc;) cap <<= 1;
+            for (cap = PRUNE_MAXC; cap < r.nc;) cap <<= 1;
         // (if constexpr: the fp32 and PQ instantiations compile exactly as they did before the BQ branches existed)
         if constexpr (KIND == KIND_BQ) {
             const uint32_t *cv = reinterpret_cast<const uint32_t *>(P.d.words + (size_t)v * P.d.W);
@@ -211,7 +317,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             __syncthreads();
             // the candidates' Hamming scores under c_v as sortable keys: 8 lanes per candidate, the walk's scorer and bits
             for (int i = tid >> 3; i < cap; i += PRUNE_THREADS / 8) {
-                const int32_t c = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1;
+                const int32_t c = i < r.nc ? prune_candidate(P, r.cand, r.ncs, v, i) : -1;
                 long long kc = KEY_MIN;
                 if (c >= 0 && c != v) kc = topk_key(score_bq(P.d, blob, c, lane & 7), c);
                 if ((lane & 7) == 0) keys[i] = kc;
@@ -222,30 +328,14 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             prepare_blob(P.d, P.metric, newrow, blob, red);
             // the candidates' ADC scores under v's LUT as sortable keys: 8 lanes per candidate, the walk's scorer and bits
             for (int i = tid >> 3; i < cap; i += PRUNE_THREADS / 8) {
-                const int32_t c = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1;
+                const int32_t c = i < r.nc ? prune_candidate(P, r.cand, r.ncs, v, i) : -1;
                 long long kc = KEY_MIN;
                 if (c >= 0 && c != v) kc = topk_key(score_pq<METRIC>(P.d, blob, c, lane & 7), c);
                 if ((lane & 7) == 0) keys[i] = kc;
             }
         } else {
             prepare_blob(P.d, P.metric, P.d.rows + (size_t)v * P.d.stride, blob, red);
-            // exact scores of the candidates against v, as sortable keys (two rows per warp at a time)
-            for (int i = warp; i < MAXC; i += 2 * NW) {
-                const int i2 = i + NW;
-                const int32_t ca = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1, cb = i2 < nc ? prune_candidate(P, cand, ncs, v, i2) : -1;
-                const bool va = ca >= 0 && ca != v, vb = cb >= 0 && cb != v;
-                long long ka = KEY_MIN, kb = KEY_MIN;
-                if (va || vb) {
-                    float sa, sb;
-                    score_f32_pair<METRIC>(P.d, blob, va ? ca : cb, vb ? cb : ca, lane, sa, sb);
-                    if (va) ka = topk_key(sa, ca);
-                    if (vb) kb = topk_key(sb, cb);
-                }
-                if (lane == 0) {
-                    keys[i] = ka;
-                    if (i2 < MAXC) keys[i2] = kb;
-                }
-            }
+            prune_keys_f32<METRIC, MAXC>(P, r, blob, keys, warp, lane);
         }
         __syncthreads();
         bitonic_sort_desc(keys, cap);
@@ -266,6 +356,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
         }
         __syncthreads();
 
+        // the selection; the fold scores each still-eligible candidate against the new neighbour, one warp per candidate
         int nsel = 0;
         float currentAlpha = 1.0f;
         while (currentAlpha <= P.alpha + 1e-6f && nsel < P.degree) {
@@ -317,11 +408,10 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
             }
             currentAlpha += 0.2f;
         }
-        // the selected neighbours, in score order (NodeArray.retain keeps the sorted order)
         __syncthreads();
         if (BOUNDED) {
             // thread t places pick t at its rank among the picks' sorted positions instead of one thread scanning nvalid states
-            const int oi = P.mode == 2 ? a : P.out_base + it;
+            const int oi = P.mode == 2 ? r.a : P.out_base + it;
             int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
             const int width = P.out_rows ? P.out_stride : P.row_cap;
             for (int t = tid; t < width; t += PRUNE_THREADS) {
@@ -339,18 +429,7 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_kernel(PruneParams P)
                 if (P.mode == 1 && P.mark) P.mark[v] = 0;
             }
         }
-        if (!BOUNDED && tid == 0) {
-            int w = 0;
-            const int oi = P.mode == 2 ? a : P.out_base + it;
-            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
-            const int width = P.out_rows ? P.out_stride : P.row_cap;
-            for (int i = 0; i < nvalid; i++)
-                if (state[i] == 1) row[w++] = key_node(keys[i]);
-            for (int i = w; i < width; i++) row[i] = -1;
-            if (P.out_rows) P.out_deg[oi] = w;
-            else P.deg[v] = w;
-            if (P.mode == 1 && P.mark) P.mark[v] = 0;
-        }
+        if (!BOUNDED && tid == 0) prune_write_row(P, r, it, state, nvalid, [&](int i) { return key_node(keys[i]); });
         __syncthreads();
     }
 }
@@ -378,6 +457,18 @@ __device__ __forceinline__ float4 gram_row(const DataDesc &d, int32_t node, int 
     return make_float4(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y), __fsub_rn(x.z, y.z), __fsub_rn(x.w, y.w));
 }
 
+// a Gram entry (the dot product of candidates i and j, diagonal entries di, dj) as the reference's similarity score; L2 and cosine
+// need the diagonal, DOT ignores it
+template <int METRIC>
+__device__ __forceinline__ float gram_score(float dotv, float di, float dj)
+{
+    float raw;
+    if (METRIC == JV_METRIC_EUCLIDEAN) raw = fmaxf(0.f, __fadd_rn(__fadd_rn(di, dj), -2.0f * dotv));
+    else if (METRIC == JV_METRIC_COSINE) raw = __fdiv_rn(dotv, __fsqrt_rn(__fmul_rn(di, dj)));
+    else raw = dotv;
+    return score_map(METRIC, raw);
+}
+
 template <int METRIC, int TILE>
 __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P)
 {
@@ -396,47 +487,17 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int ty = tid >> 4, tx = tid & 15;
-    constexpr int NW = PRUNE_THREADS / 32;
     const int total = P.count_ptr ? *P.count_ptr : P.count;
-    float alpha_max = 1.0f;
-    for (float a = 1.0f; a <= P.alpha + 1e-6f; a += 0.2f) alpha_max = a;
+    const float alpha_max = prune_alpha_max(P.alpha);
 
     for (int it = blockIdx.x; it < total; it += gridDim.x) {
-        const int a = P.mode == 2 ? P.list[it] : 0;
-        const int v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
-        const int32_t *cand;
-        int nc, ncs;
-        if (P.mode == 0) {
-            cand = P.cand + (size_t)it * P.cand_stride;
-            ncs = P.cand_stride;
-            nc = ncs + P.window;
-        } else if (P.mode == 2) {
-            cand = P.cand + P.cand_off[a];
-            ncs = nc = P.cand_cnt[a];
-        } else {
-            cand = P.adj + (size_t)v * P.row_cap;
-            ncs = nc = min(P.deg[v], P.row_cap);
-        }
-        nc = min(nc, TILE);
+        const PruneRow r(P, it, TILE);
+        const int v = r.v;
         prepare_blob(P.d, P.metric, P.d.rows + (size_t)v * P.d.stride, blob, red);
-        for (int i = warp; i < TILE; i += 2 * NW) {
-            const int i2 = i + NW;
-            const int32_t ca = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1, cb = (i2 < TILE && i2 < nc) ? prune_candidate(P, cand, ncs, v, i2) : -1;
-            const bool va = ca >= 0 && ca != v, vb = cb >= 0 && cb != v;
-            long long ka = KEY_MIN, kb = KEY_MIN;
-            if (va || vb) {
-                float sa, sb;
-                score_f32_pair<METRIC>(P.d, blob, va ? ca : cb, vb ? cb : ca, lane, sa, sb);
-                if (va) ka = topk_key(sa, ca);
-                if (vb) kb = topk_key(sb, cb);
-            }
-            if (lane == 0) {
-                keys[i] = ka;
-                if (i2 < TILE) keys[i2] = kb;
-            }
-        }
+        prune_keys_f32<METRIC, TILE>(P, r, blob, keys, warp, lane);
         __syncthreads();
         bitonic_sort_desc(keys, TILE);
+        // valid keys form a prefix (KEY_MIN sorts last); duplicates are adjacent after the sort and are dropped
         int nvalid;
         {
             int lo = 0, hi = TILE;
@@ -495,70 +556,23 @@ __global__ void __launch_bounds__(PRUNE_THREADS) prune_gram_kernel(PruneParams P
             for (int b = 0; b < NB; b++) C[(ty + 16 * a) * CP + tx + 16 * b] = acc[a][b];
         __syncthreads();
         // raw dot products -> the reference's similarity scores (needs the diagonal for L2 / cosine)
+        float diag_r[NB] = {}, diag_c[NB] = {};  // DOT reads no diagonal
         if (METRIC != JV_METRIC_DOT) {
-            float diag_r[NB], diag_c[NB];
 #pragma unroll
             for (int a = 0; a < NB; a++) diag_r[a] = C[(ty + 16 * a) * CP + ty + 16 * a];
 #pragma unroll
             for (int b = 0; b < NB; b++) diag_c[b] = C[(tx + 16 * b) * CP + tx + 16 * b];
             __syncthreads();
-#pragma unroll
-            for (int a = 0; a < NB; a++)
-#pragma unroll
-                for (int b = 0; b < NB; b++) {
-                    float raw;
-                    if (METRIC == JV_METRIC_EUCLIDEAN) raw = fmaxf(0.f, __fadd_rn(__fadd_rn(diag_r[a], diag_c[b]), -2.0f * acc[a][b]));
-                    else raw = __fdiv_rn(acc[a][b], __fsqrt_rn(__fmul_rn(diag_r[a], diag_c[b])));
-                    C[(ty + 16 * a) * CP + tx + 16 * b] = score_map(METRIC, raw);
-                }
-        } else {
-#pragma unroll
-            for (int a = 0; a < NB; a++)
-#pragma unroll
-                for (int b = 0; b < NB; b++) C[(ty + 16 * a) * CP + tx + 16 * b] = score_map(METRIC, acc[a][b]);
         }
+#pragma unroll
+        for (int a = 0; a < NB; a++)
+#pragma unroll
+            for (int b = 0; b < NB; b++) C[(ty + 16 * a) * CP + tx + 16 * b] = gram_score<METRIC>(acc[a][b], diag_r[a], diag_c[b]);
         __syncthreads();
 
-        // ---- the sequential selection, now over shared memory only ----
-        int nsel = 0;
-        float currentAlpha = 1.0f;
-        while (currentAlpha <= P.alpha + 1e-6f && nsel < P.degree) {
-            int cursor = 0;
-            while (nsel < P.degree) {
-                if (tid == 0) s_next = INT_MAX;
-                __syncthreads();
-                for (int i = cursor + tid; i < nvalid; i += PRUNE_THREADS)
-                    if (state[i] == 0 && !(maxsim[i] > __fmul_rn(key_score(keys[i]), currentAlpha))) { atomicMin(&s_next, i); break; }
-                __syncthreads();
-                const int pick = s_next;
-                if (pick == INT_MAX) break;
-                nsel++;
-                cursor = pick + 1;
-                for (int i = tid; i < nvalid; i += PRUNE_THREADS) {
-                    if (i == pick) state[i] = 1;
-                    else if (state[i] == 0) {
-                        const float m = fmaxf(maxsim[i], C[i * CP + pick]);
-                        maxsim[i] = m;
-                        if (m > __fmul_rn(key_score(keys[i]), alpha_max)) state[i] = 2;
-                    }
-                }
-                __syncthreads();
-            }
-            currentAlpha += 0.2f;
-        }
+        prune_select_gram<CP>(P, C, keys, maxsim, state, nvalid, alpha_max, &s_next);
         __syncthreads();
-        if (tid == 0) {
-            int w = 0;
-            const int oi = P.mode == 2 ? a : P.out_base + it;
-            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
-            const int width = P.out_rows ? P.out_stride : P.row_cap;
-            for (int i = 0; i < nvalid; i++)
-                if (state[i] == 1) row[w++] = ids[i];
-            for (int i = w; i < width; i++) row[i] = -1;
-            if (P.out_rows) P.out_deg[oi] = w;
-            else P.deg[v] = w;
-            if (P.mode == 1 && P.mark) P.mark[v] = 0;
-        }
+        if (tid == 0) prune_write_row(P, r, it, state, nvalid, [&](int i) { return ids[i]; });
         __syncthreads();
     }
 }
@@ -640,10 +654,8 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
     __shared__ int s_next;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr int NW = PRUNE_THREADS / 32;
     const int total = P.count_ptr ? *P.count_ptr : P.count;
-    float alpha_max = 1.0f;
-    for (float a = 1.0f; a <= P.alpha + 1e-6f; a += 0.2f) alpha_max = a;
+    const float alpha_max = prune_alpha_max(P.alpha);
 
     // warpgroup wg computes columns [wg N, wg N + N) of every 64-row block of the Gram matrix
     constexpr int N = TILE / 2, MB = TILE / 64, R = N / 2;
@@ -653,41 +665,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
     const int c4 = tid & 7, r0 = tid >> 3;
 
     for (int it = blockIdx.x; it < total; it += gridDim.x) {
-        const int a = P.mode == 2 ? P.list[it] : 0;
-        const int v = P.mode == 0 ? P.node_base + it : P.mode == 2 ? P.row_node[a] : P.list[P.list_base + it];
-        const int32_t *cand;
-        int nc, ncs;
-        if (P.mode == 0) {
-            cand = P.cand + (size_t)it * P.cand_stride;
-            ncs = P.cand_stride;
-            nc = ncs + P.window;
-        } else if (P.mode == 2) {
-            cand = P.cand + P.cand_off[a];
-            ncs = nc = P.cand_cnt[a];
-        } else {
-            cand = P.adj + (size_t)v * P.row_cap;
-            ncs = nc = min(P.deg[v], P.row_cap);
-        }
-        nc = min(nc, TILE);
+        const PruneRow r(P, it, TILE);
+        const int v = r.v;
         prepare_blob(P.d, P.metric, P.d.rows + (size_t)v * P.d.stride, blob, red);
-        for (int i = warp; i < TILE; i += 2 * NW) {
-            const int i2 = i + NW;
-            const int32_t ca = i < nc ? prune_candidate(P, cand, ncs, v, i) : -1, cb = (i2 < TILE && i2 < nc) ? prune_candidate(P, cand, ncs, v, i2) : -1;
-            const bool va = ca >= 0 && ca != v, vb = cb >= 0 && cb != v;
-            long long ka = KEY_MIN, kb = KEY_MIN;
-            if (va || vb) {
-                float sa, sb;
-                score_f32_pair<METRIC>(P.d, blob, va ? ca : cb, vb ? cb : ca, lane, sa, sb);
-                if (va) ka = topk_key(sa, ca);
-                if (vb) kb = topk_key(sb, cb);
-            }
-            if (lane == 0) {
-                keys[i] = ka;
-                if (i2 < TILE) keys[i2] = kb;
-            }
-        }
+        prune_keys_f32<METRIC, TILE>(P, r, blob, keys, warp, lane);
         __syncthreads();
         bitonic_sort_desc(keys, TILE);
+        // valid keys form a prefix (KEY_MIN sorts last); duplicates are adjacent after the sort and are dropped
         int nvalid;
         {
             int lo = 0, hi = TILE;
@@ -783,55 +767,13 @@ __global__ void __launch_bounds__(PRUNE_THREADS, TILE == 128 ? 2 : 3) prune_gram
         }
         for (int idx = tid; idx < TILE * TILE; idx += PRUNE_THREADS) {
             const int i = idx / TILE, j = idx - i * TILE;
-            const float dotv = C[i * CP + j];
-            float raw;
-            if (METRIC == JV_METRIC_EUCLIDEAN) raw = fmaxf(0.f, __fadd_rn(__fadd_rn(diag[i], diag[j]), -2.0f * dotv));
-            else if (METRIC == JV_METRIC_COSINE) raw = __fdiv_rn(dotv, __fsqrt_rn(__fmul_rn(diag[i], diag[j])));
-            else raw = dotv;
-            C[i * CP + j] = score_map(METRIC, raw);
+            C[i * CP + j] = gram_score<METRIC>(C[i * CP + j], diag[i], diag[j]);
         }
         __syncthreads();
 
-        // ---- the sequential selection, over shared memory only ----
-        int nsel = 0;
-        float currentAlpha = 1.0f;
-        while (currentAlpha <= P.alpha + 1e-6f && nsel < P.degree) {
-            int cursor = 0;
-            while (nsel < P.degree) {
-                if (tid == 0) s_next = INT_MAX;
-                __syncthreads();
-                for (int i = cursor + tid; i < nvalid; i += PRUNE_THREADS)
-                    if (state[i] == 0 && !(maxsim[i] > __fmul_rn(key_score(keys[i]), currentAlpha))) { atomicMin(&s_next, i); break; }
-                __syncthreads();
-                const int pick = s_next;
-                if (pick == INT_MAX) break;
-                nsel++;
-                cursor = pick + 1;
-                for (int i = tid; i < nvalid; i += PRUNE_THREADS) {
-                    if (i == pick) state[i] = 1;
-                    else if (state[i] == 0) {
-                        const float m = fmaxf(maxsim[i], C[i * CP + pick]);
-                        maxsim[i] = m;
-                        if (m > __fmul_rn(key_score(keys[i]), alpha_max)) state[i] = 2;
-                    }
-                }
-                __syncthreads();
-            }
-            currentAlpha += 0.2f;
-        }
+        prune_select_gram<CP>(P, C, keys, maxsim, state, nvalid, alpha_max, &s_next);
         __syncthreads();
-        if (tid == 0) {
-            int w = 0;
-            const int oi = P.mode == 2 ? a : P.out_base + it;
-            int32_t *row = P.out_rows ? P.out_rows + (size_t)oi * P.out_stride : P.adj + (size_t)v * P.row_cap;
-            const int width = P.out_rows ? P.out_stride : P.row_cap;
-            for (int i = 0; i < nvalid; i++)
-                if (state[i] == 1) row[w++] = ids[i];
-            for (int i = w; i < width; i++) row[i] = -1;
-            if (P.out_rows) P.out_deg[oi] = w;
-            else P.deg[v] = w;
-            if (P.mode == 1 && P.mark) P.mark[v] = 0;
-        }
+        if (tid == 0) prune_write_row(P, r, it, state, nvalid, [&](int i) { return ids[i]; });
         __syncthreads();
     }
 }
