@@ -522,6 +522,42 @@ JV_API int jv_graph_remove_deleted_bq(jv_graph g, jv_dataset bq, int metric, flo
                                       const uint32_t *deleted_bits /* host, bit (node & 31) of word (node >> 5) */,
                                       jv_graph *out, jv_remove_stats *stats);
 
+/* ---- merging graphs: OnDiskGraphIndexCompactor's per-node work (graph/disk/OnDiskGraphIndexCompactor.java) on the device ----
+ * S source graphs over fp32 rows become one graph over their live nodes, renumbered by each source's old_to_new. With
+ * searchTopK = max(2, ceil(degree / S) * 4), every live node v of source s at level L gets as candidates its live neighbours at L
+ * in s and, from every other source t that has a level L, the searchTopK best live members of t's level L: a search of t's graph
+ * with v's row as the query (level 0), or a greedy descent from t's entry to level L + 1 and a beam of searchTopK on level L (upper
+ * levels). When t has at most searchTopK live members at L, they are all candidates and no search runs (the set an exhaustive search
+ * returns). Exact fp32 scores under `metric` order the candidates (equal scores: the lower new id first) and retainDiverse at
+ * `alpha` picks the row, as the builder's prune does.
+ * The new graph has a level L for every level some source has that keeps a live member; v sits at L iff it does in its source. Its
+ * entry is the entry of the first source, in source order, whose top level is the merged top level and whose entry is live,
+ * otherwise the lowest new id of the top level. It has no holes and no FusedPQ records. rows_out is a new fp32 data set of the live
+ * rows in new-id order, the rows a search of the new graph needs. The sources are not modified.
+ * Errors, all before any device work (a refused call leaves *graph_out and *rows_out as they were): JV_ERR_INVALID for a null
+ * argument, nsources < 1, rows that are not fp32 or do not match their graph's size, unequal dims, degrees or devices, a bad
+ * metric, alpha < 1, no live node, or new ids of the live nodes that are not exactly [0, live nodes); JV_ERR_UNSUPPORTED for a
+ * degree above 64, or degree + (S - 1) * searchTopK above 8192 (more than 2033 sources at degree 64). JV_ERR_OVERFLOW when a search overflows its candidate list even after retries; what the call allocated is freed. */
+typedef struct {
+    jv_graph graph;            /* source graph; its holes (jv_graph_remove_deleted) count as dead */
+    jv_dataset rows;           /* its fp32 rows (row i = node i); all sources on one device, with one dim */
+    const uint32_t *live_bits; /* host, bit (node & 31) of word (node >> 5) over the graph's n; NULL = every node but holes live */
+    const int32_t *old_to_new; /* host [n]; read for live nodes only */
+} jv_compact_source;
+typedef struct {
+    int32_t nodes;          /* live nodes merged = the new graph's size */
+    int levels;             /* levels of the new graph */
+    int search_top_k;       /* the searchTopK used */
+    int64_t searches;       /* (query, other source, level) searches run */
+    int64_t exhaustive;     /* (query, other source, level) pairs answered by the whole live membership instead */
+    int64_t candidates;     /* summed over all rows of all levels */
+    int32_t max_candidates; /* largest candidate set of one row */
+    int64_t visited;        /* summed visited counts of the searches */
+    double device_ms;
+} jv_compact_stats;
+JV_API int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric, float alpha, jv_graph *graph_out, jv_dataset *rows_out,
+                            jv_compact_stats *stats);
+
 /* device-memory helpers for callers that keep queries/results in HBM (bench `value` leg) */
 JV_API int jv_device_malloc(void **out, size_t bytes);
 JV_API int jv_device_free(void *p);

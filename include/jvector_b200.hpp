@@ -59,6 +59,7 @@ protected:
 
 struct F32Vectors : Vectors {
     F32Vectors(const float *rows, int64_t n, int dim) { check(jv_dataset_register_f32(rows, n, dim, &h_)); }
+    explicit F32Vectors(jv_dataset h) { h_ = h; }
 };
 struct PQVectors : Vectors {
     PQVectors(const uint8_t *codes, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid = nullptr)
@@ -239,6 +240,39 @@ public:
 private:
     VectorSimilarityFunction vsf_;
     jv_build_params p_;
+};
+
+/// OnDiskGraphIndexCompactor's merge (jv_graph_compact): sources[i] is graph i with its rows, liveBits[i] its live nodes (bit
+/// node & 31 of word node >> 5; empty = every node but holes) and remappers[i] its old id -> new id map. compact() returns the
+/// merged graph and its rows in new-id order; the counters go to stats.
+class GraphIndexCompactor {
+public:
+    GraphIndexCompactor(std::vector<std::pair<const GraphIndex *, const F32Vectors *>> sources, std::vector<std::vector<uint32_t>> liveBits,
+                        std::vector<std::vector<int32_t>> remappers, VectorSimilarityFunction vsf, float alpha = 1.2f)
+        : sources_(std::move(sources)), live_(std::move(liveBits)), maps_(std::move(remappers)), vsf_(vsf), alpha_(alpha) {}
+    std::pair<GraphIndex, F32Vectors> compact()
+    {
+        if (live_.size() != sources_.size() || maps_.size() != sources_.size()) throw Error(JV_ERR_INVALID, "compact: one live set and one map per source");
+        std::vector<jv_compact_source> src(sources_.size());
+        for (size_t i = 0; i < sources_.size(); i++) {
+            const int32_t n = sources_[i].first->size();
+            if ((int64_t)maps_[i].size() < n || (!live_[i].empty() && (int64_t)live_[i].size() * 32 < n))
+                throw Error(JV_ERR_INVALID, "compact: a live set or a map shorter than its graph");
+            src[i] = {sources_[i].first->handle(), sources_[i].second->handle(), live_[i].empty() ? nullptr : live_[i].data(), maps_[i].data()};
+        }
+        jv_graph g = nullptr;
+        jv_dataset rows = nullptr;
+        check(jv_graph_compact(src.data(), (int)src.size(), (int)vsf_, alpha_, &g, &rows, &stats));
+        return {GraphIndex(g), F32Vectors(rows)};
+    }
+    jv_compact_stats stats = {};
+
+private:
+    std::vector<std::pair<const GraphIndex *, const F32Vectors *>> sources_;
+    std::vector<std::vector<uint32_t>> live_;
+    std::vector<std::vector<int32_t>> maps_;
+    VectorSimilarityFunction vsf_;
+    float alpha_;
 };
 
 }  // namespace jv

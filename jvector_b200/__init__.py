@@ -9,13 +9,14 @@ mirror of the reference's interface for that path, used by the tests and the ben
   ScoreFunction (similarityTo / similarityToBatch)  base:graph/similarity/ScoreFunction.java
   GraphIndex, GraphSearcher.search              base:graph/GraphSearcher.java:222
   GraphIndexBuilder.build                       base:graph/GraphIndexBuilder.java:436
+  GraphIndexCompactor.compact                   graph/disk/OnDiskGraphIndexCompactor.java (the per-node merge, not the file)
 """
 from . import api
-from .api import (BQVectors, F32Vectors, GraphIndex, GraphIndexBuilder, GraphSearcher, NVQVectors, PQVectors, ProductQuantization, QueryBatch,
-                  ScoreFunction, SearchResult, VectorSimilarityFunction, bq_encode_all, kmeans_assign, nvq_encode_all, nvq_encode_resident,
+from .api import (BQVectors, F32Vectors, GraphIndex, GraphIndexBuilder, GraphIndexCompactor, GraphSearcher, NVQVectors, PQVectors,
+                  ProductQuantization, QueryBatch, ScoreFunction, SearchResult, VectorSimilarityFunction, bq_encode_all, kmeans_assign, nvq_encode_all, nvq_encode_resident,
                   pack_accept_bits, pq_encode_all, pq_encode_all_anisotropic, score_multi, topk_bruteforce)
 from ._native import JVectorB200Error, init, load
 
 __all__ = ["VectorSimilarityFunction", "F32Vectors", "PQVectors", "BQVectors", "NVQVectors", "ProductQuantization", "ScoreFunction", "GraphIndex",
-           "GraphSearcher", "GraphIndexBuilder", "SearchResult", "score_multi", "topk_bruteforce", "bq_encode_all",
+           "GraphSearcher", "GraphIndexBuilder", "GraphIndexCompactor", "SearchResult", "score_multi", "topk_bruteforce", "bq_encode_all",
            "pq_encode_all", "pq_encode_all_anisotropic", "nvq_encode_all", "nvq_encode_resident", "QueryBatch", "kmeans_assign", "pack_accept_bits", "JVectorB200Error", "init", "load"]

@@ -41,6 +41,15 @@ class RemoveStats(C.Structure):
                 ("max_candidates", C.c_int32), ("random_fallbacks", C.c_int64), ("device_ms", C.c_double)]
 
 
+class CompactSource(C.Structure):
+    _fields_ = [("graph", C.c_void_p), ("rows", C.c_void_p), ("live_bits", C.POINTER(C.c_uint32)), ("old_to_new", i32p)]
+
+
+class CompactStats(C.Structure):
+    _fields_ = [("nodes", C.c_int32), ("levels", C.c_int), ("search_top_k", C.c_int), ("searches", C.c_int64), ("exhaustive", C.c_int64),
+                ("candidates", C.c_int64), ("max_candidates", C.c_int32), ("visited", C.c_int64), ("device_ms", C.c_double)]
+
+
 class PQTrainParams(C.Structure):
     _fields_ = [("M", C.c_int), ("k", C.c_int), ("globally_center", C.c_int), ("lloyd_iterations", C.c_int), ("max_train_rows", C.c_int64),
                 ("seed", C.c_uint64)]
@@ -138,6 +147,7 @@ SYMBOLS = [
     ("jv_graph_remove_deleted_bq", _I, [_P, _P, _I, _F, C.c_uint64, C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(RemoveStats)]),
     ("jv_graph_add_nodes_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_builder_create_from_graph_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), _P, C.POINTER(_P)]),
+    ("jv_graph_compact", _I, [C.POINTER(CompactSource), _I, _I, _F, C.POINTER(_P), C.POINTER(_P), C.POINTER(CompactStats)]),
     ("jv_builder_create", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]), ("jv_builder_info", _I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     ("jv_builder_next_batch", _I, [_P, i32p, i32p]), ("jv_builder_insert_slice", _I, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     ("jv_builder_apply_new", _I, [_P, C.c_int32, C.c_int32, _P, _P, i32p]), ("jv_builder_reprune_slice", _I, [_P, C.c_int32, C.c_int32, _P, _P]),

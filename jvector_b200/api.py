@@ -581,6 +581,58 @@ class GraphIndexBuilder:
         return GraphIndex(_handle=h)
 
 
+class GraphIndexCompactor:
+    """graph/disk/OnDiskGraphIndexCompactor.java's merge on the device (jv_graph_compact): several graphs over fp32 rows become one
+    graph over their live nodes, with the compactor's candidates (each node's live neighbours in its own source, the searchTopK best
+    live members of every other source) and the builder's robust prune at alpha.
+
+    sources: a list of (GraphIndex, F32Vectors), all with one dimension and degree. liveNodes: per source a bool mask over its nodes,
+    or None; None (the whole list or an entry) means every node but the source's holes. remappers: per source an int array mapping
+    old ids to new ids (read for live nodes, which must map onto exactly [0, live nodes)), or None: the sources in order, each one's
+    live nodes in id order (a source with holes from removeDeletedNodes then needs a live mask that leaves them out). compact() returns (GraphIndex, F32Vectors): the merged graph and its rows in new-id order. The sources
+    are left as they are; `.stats` holds jv_compact_stats as a dict after compact()."""
+
+    def __init__(self, sources, liveNodes, remappers, vsf, alpha=1.2):
+        self.sources, self.vsf, self.alpha = list(sources), vsf, float(alpha)
+        sizes = [g.info()["n"] for g, _ in self.sources]
+        live = liveNodes if liveNodes is not None else [None] * len(sizes)
+        if len(live) != len(sizes):
+            raise ValueError("one live mask per source")
+        self.live = [None if m is None else np.asarray(m, bool) for m in live]
+        for m, n in zip(self.live, sizes):
+            if m is not None and m.shape != (n,):
+                raise ValueError("live mask has shape %s, its graph has %d nodes" % (m.shape, n))
+        if remappers is None:
+            remappers, base = [], 0
+            for m, n in zip(self.live, sizes):
+                alive = np.ones(n, bool) if m is None else m
+                r = np.full(n, -1, np.int32)
+                r[alive] = base + np.arange(int(alive.sum()), dtype=np.int32)
+                remappers.append(r)
+                base += int(alive.sum())
+        if len(remappers) != len(sizes):
+            raise ValueError("one remapper per source")
+        self.remappers = [np.ascontiguousarray(r, dtype=np.int32) for r in remappers]
+        for r, n in zip(self.remappers, sizes):
+            if r.shape != (n,):
+                raise ValueError("remapper has shape %s, its graph has %d nodes" % (r.shape, n))
+        self.stats = None
+
+    def compact(self):
+        lib = nat.init()
+        bits = [None if m is None else pack_accept_bits(m) for m in self.live]
+        src = (nat.CompactSource * len(self.sources))()
+        for i, ((g, v), b, r) in enumerate(zip(self.sources, bits, self.remappers)):
+            src[i] = nat.CompactSource(g._h, v._h, b.ctypes.data_as(C.POINTER(C.c_uint32)) if b is not None else None, ip(r))
+        st = nat.CompactStats()
+        gh, rh = C.c_void_p(), C.c_void_p()
+        check(lib.jv_graph_compact(src, len(self.sources), int(self.vsf), self.alpha, C.byref(gh), C.byref(rh), C.byref(st)))
+        self.stats = {name: getattr(st, name) for name, _ in nat.CompactStats._fields_}
+        rows = F32Vectors.__new__(F32Vectors)
+        _Vectors.__init__(rows, rh, None)
+        return GraphIndex(_handle=gh), rows
+
+
 def _deleted_bits(deleted, n):
     """a bool mask [n] or an array of node ids -> the accept_bits layout over n nodes, set = deleted"""
     d = np.asarray(deleted)

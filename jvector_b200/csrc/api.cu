@@ -1230,8 +1230,9 @@ static int ensure_sketch(jv_dataset ds, cudaStream_t s)
     return JV_OK;
 }
 
+// query_stride: floats between two queries (0: dim)
 static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int metric, const float *queries_dev, int nq, int topK, int rerankK,
-                         const SearchFilter *filter, int32_t *nodes_dev, float *scores_dev, jv_search_stats *stats)
+                         const SearchFilter *filter, int32_t *nodes_dev, float *scores_dev, jv_search_stats *stats, int query_stride = 0)
 {
     if (!g || !approx || !queries_dev || !nodes_dev || !scores_dev || nq <= 0) return fail(JV_ERR_INVALID, "graph_search: bad arguments");
     if (topK < 1 || rerankK < topK) return fail(JV_ERR_INVALID, "graph_search: need 1 <= topK <= rerankK");
@@ -1303,7 +1304,7 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         if ((rc = grow(t_ctx.search_scratch, search_scratch_bytes(plan)))) return rc;
         CK(t_ctx.timer.start(s), "event");
         CK(launch_search(g->g, ad, rr, metric, queries_dev, cnt, topK, rerankK, plan, t_ctx.search_scratch.get(), dwork, nodes_dev, scores_dev, dcnt, dover,
-                         attempt ? dindex : nullptr, 0, filter, s),
+                         attempt ? dindex : nullptr, query_stride, filter, s),
            "launch_search");
         CK(t_ctx.timer.stop(s), "event");
         CK(cudaMemcpyAsync(&hc, dcnt, sizeof(hc), cudaMemcpyDeviceToHost, s), "D2H counters");
@@ -2193,6 +2194,366 @@ int jv_graph_remove_deleted_bq(jv_graph g, jv_dataset bq, int metric, float alph
                                jv_remove_stats *stats)
 {
     return graph_remove_deleted(g, bq, KIND_BQ, metric, alpha, seed, deleted_bits, out, stats);
+}
+
+// ------------------------------------------------------------------------------------------------ OnDiskGraphIndexCompactor
+// Merging S graphs into one (DESIGN §4.3h): per level, the live members of every source are the rows, source by source. Every other
+// source t is searched once per level for all of them (the search kernel over t, or over t's sub-hierarchy from level L up), the
+// assembly kernel writes each row's candidates under their new ids and the repair's ragged prune picks its neighbours.
+
+// one source as the compaction sees it: the new id of every live node (-1: dead or a hole), and per level its live members in the
+// level's order with their rows in the level's adjacency
+struct CompactSource {
+    jv_graph g;
+    jv_dataset ds;
+    std::vector<int32_t> map;
+    std::vector<std::vector<int32_t>> live, live_row;
+};
+
+// source t's level L (>= 1) and everything above it as a graph of its own: node p is t's p-th member of level L, its rows are the
+// members' rows (gathered on `s`); the search of it descends from t's entry exactly as a search of t would down to level L
+static int compact_sub_hierarchy(const CompactSource &t, int L, std::unique_ptr<jv_graph_s> &sg, std::unique_ptr<jv_dataset_s> &sd, cudaStream_t s)
+{
+    const jv_graph_s &g = *t.g;
+    const std::vector<int32_t> &ids = g.level_ids[L - 1];
+    const int m = (int)ids.size(), degree = g.g.degree;
+    std::vector<int32_t> pos(g.g.n, -1);
+    for (int p = 0; p < m; p++) pos[ids[p]] = p;
+    auto remap = [&](const std::vector<int32_t> &a) {
+        std::vector<int32_t> r(a.size());
+        for (size_t i = 0; i < a.size(); i++) r[i] = a[i] >= 0 ? pos[a[i]] : -1;
+        return r;
+    };
+    sd.reset(new jv_dataset_s());
+    sd->device = t.ds->device;
+    memset(&sd->d, 0, sizeof(DataDesc));
+    sd->d.kind = KIND_F32; sd->d.dim = t.ds->d.dim; sd->d.stride = t.ds->d.stride; sd->d.n = m;
+    float *rows;
+    int32_t *dids;
+    int rc = sd->alloc(&rows, (size_t)m * sd->d.stride * 4);
+    if (rc || (rc = sd->alloc(&dids, (size_t)m * 4))) return rc;
+    sd->d.rows = rows;
+    CK(cudaMemcpyAsync(dids, ids.data(), (size_t)m * 4, cudaMemcpyHostToDevice, s), "H2D members");
+    CK(launch_gather_rows(t.ds->d, dids, m, rows, s), "gather member rows");
+    sg.reset(new jv_graph_s());
+    sg->device = g.device;
+    memset(&sg->g, 0, sizeof(GraphDesc));
+    const std::vector<int32_t> adj = remap(g.level_adj[L - 1]);
+    CK(sg->adj0.alloc((size_t)m * degree * 4), "cudaMalloc(sub-hierarchy)");
+    CK(cudaMemcpy(sg->adj0.get(), adj.data(), adj.size() * 4, cudaMemcpyHostToDevice), "H2D sub-hierarchy");
+    sg->g.n = m; sg->g.degree = degree; sg->g.levels = 1; sg->g.entry_node = pos[g.g.entry_node]; sg->g.entry_level = 0;
+    sg->g.adj0 = sg->adj0.get<int32_t>();
+    for (size_t l = L; l < g.level_ids.size(); l++) {
+        sg->level_ids.push_back(remap(g.level_ids[l]));
+        sg->level_adj.push_back(remap(g.level_adj[l]));
+    }
+    return graph_rebuild_upper(sg.get());
+}
+
+// the searchTopK best live members of source t at level `level` for every row of the level that belongs to another source, into
+// res [queries][K] (t's node ids, or member positions above level 0). qids: the queries' new ids (their rows in `merged`)
+static int compact_search(const CompactSource &t, int level, jv_dataset merged, int metric, int K, const std::vector<int32_t> &qids, int32_t *res,
+                          jv_compact_stats *stats, cudaStream_t s)
+{
+    constexpr int QUERY_CHUNK = 1 << 18;  // queries per search call: bounds the search's scratch and the gathered query rows
+    std::unique_ptr<jv_graph_s> sg;
+    std::unique_ptr<jv_dataset_s> sd;
+    jv_graph g = t.g;
+    jv_dataset ds = t.ds;
+    int rc;
+    if (level > 0) {
+        if ((rc = compact_sub_hierarchy(t, level, sg, sd, s))) return rc;
+        g = sg.get();
+        ds = sd.get();
+    }
+    // accept bits: the live nodes of the searched graph (acceptOrds = live_t)
+    const int n = g->g.n;
+    std::vector<uint32_t> bits(((size_t)n + 31) / 32, 0u);
+    for (size_t p = 0; p < t.live_row[level].size(); p++) {
+        const int v = t.live_row[level][p];
+        bits[v >> 5] |= 1u << (v & 31);
+    }
+    const int nq = (int)qids.size(), chunk = std::min(nq, QUERY_CHUNK), stride = merged->d.stride;
+    std::vector<DeviceBuffer> mem;
+    uint32_t *dbits;
+    int32_t *dq;
+    float *qrows, *scores;
+    CK(alloc_owned(mem, dbits, bits.size() * 4), "cudaMalloc(accept bits)");
+    CK(alloc_owned(mem, dq, (size_t)nq * 4), "cudaMalloc(query ids)");
+    CK(alloc_owned(mem, qrows, (size_t)chunk * stride * 4), "cudaMalloc(query rows)");
+    CK(alloc_owned(mem, scores, (size_t)chunk * K * 4), "cudaMalloc(search scores)");
+    CK(cudaMemcpyAsync(dbits, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, s), "H2D accept bits");
+    CK(cudaMemcpyAsync(dq, qids.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, s), "H2D query ids");
+    SearchFilter f;
+    memset(&f, 0, sizeof(f));
+    f.accept_bits = dbits;
+    for (int q0 = 0; q0 < nq; q0 += chunk) {
+        const int c = std::min(chunk, nq - q0);
+        CK(launch_gather_rows(merged->d, dq + q0, c, qrows, s), "gather query rows");
+        jv_search_stats st;
+        if ((rc = search_device(g, ds, nullptr, metric, qrows, c, K, K, &f, res + (size_t)q0 * K, scores, &st, stride))) return rc;
+        stats->searches += c;
+        stats->visited += st.visited;
+    }
+    return JV_OK;
+}
+
+// one level of the merge: the rows of every source's live members, their candidates and their pruned neighbours. Level 0 scatters
+// the rows into ng's adjacency; an upper level hands back its members (ascending new ids) and their rows.
+static int compact_level(const std::vector<CompactSource> &src, int level, int K, jv_dataset merged, int metric, float alpha, jv_graph_s *ng,
+                         const std::vector<const int32_t *> &maps_dev, std::vector<int32_t> *ids_out, std::vector<int32_t> *adj_out,
+                         jv_compact_stats *stats, cudaStream_t s)
+{
+    const int S = (int)src.size(), degree = ng->g.degree;
+    std::vector<long long> start(S + 1, 0);
+    std::vector<int32_t> row_node;
+    for (int i = 0; i < S; i++) {
+        start[i + 1] = start[i] + (long long)src[i].live[level].size();
+        for (int32_t v : src[i].live[level]) row_node.push_back(src[i].map[v]);
+    }
+    const int rows = (int)start[S];
+    const int cand_stride = degree + (S - 1) * K;
+    std::vector<DeviceBuffer> mem;  // the level's scratch: every return below comes after the stream has drained
+    int32_t *drow_node, *cand, *out_rows;
+    long long *cand_off;
+    int *cand_cnt;
+    CompactTarget *dtargets;
+    cudaError_t e = alloc_owned(mem, drow_node, (size_t)rows * 4);
+    if (e == cudaSuccess) e = alloc_owned(mem, cand, (size_t)rows * cand_stride * 4);
+    if (e == cudaSuccess) e = alloc_owned(mem, cand_off, (size_t)rows * 8);
+    if (e == cudaSuccess) e = alloc_owned(mem, cand_cnt, (size_t)rows * 4);
+    if (e == cudaSuccess) e = alloc_owned(mem, out_rows, (size_t)rows * degree * 4);
+    if (e == cudaSuccess) e = alloc_owned(mem, dtargets, (size_t)S * sizeof(CompactTarget));
+    if (e == cudaSuccess) e = cudaMemcpyAsync(drow_node, row_node.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s);
+    CK(e, "graph_compact: level scratch");
+    // per other source: its search results for the rows of every other source, in source order, or its whole live membership
+    std::vector<CompactTarget> target(S, CompactTarget{nullptr, nullptr, nullptr, 0});
+    std::vector<const int32_t *> pos_map(S, nullptr);
+    int rc = JV_OK;
+    for (int t = 0; t < S && !rc; t++) {
+        const long long cnt = start[t + 1] - start[t], nq = rows - cnt;
+        if (src[t].g->g.levels <= level || nq == 0) continue;
+        if (cnt <= K) {
+            target[t].list = drow_node + start[t];
+            target[t].count = (int)cnt;
+            stats->exhaustive += nq;
+            continue;
+        }
+        std::vector<int32_t> qids(row_node.begin(), row_node.begin() + start[t]);
+        qids.insert(qids.end(), row_node.begin() + start[t + 1], row_node.end());
+        int32_t *res, *map = nullptr;
+        if ((e = alloc_owned(mem, res, (size_t)nq * K * 4)) != cudaSuccess) { rc = cuda_fail(e, "cudaMalloc(search results)"); break; }
+        if (level == 0) map = const_cast<int32_t *>(maps_dev[t]);
+        else {
+            // member position -> new id (-1: dead)
+            const std::vector<int32_t> &ids = src[t].g->level_ids[level - 1];
+            std::vector<int32_t> hm(ids.size());
+            for (size_t p = 0; p < ids.size(); p++) hm[p] = src[t].map[ids[p]];
+            e = alloc_owned(mem, map, hm.size() * 4);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(map, hm.data(), hm.size() * 4, cudaMemcpyHostToDevice, s);
+            if (e != cudaSuccess) { rc = cuda_fail(e, "graph_compact: member map"); break; }
+        }
+        rc = compact_search(src[t], level, merged, metric, K, qids, res, stats, s);
+        target[t].res = res;
+        target[t].map = map;
+    }
+    // the candidate segments, source block by source block
+    for (int i = 0; i < S && !rc; i++) {
+        const int cnt = (int)(start[i + 1] - start[i]);
+        if (cnt == 0) continue;
+        std::vector<CompactTarget> tg(S, CompactTarget{nullptr, nullptr, nullptr, 0});
+        for (int t = 0; t < S; t++) {
+            if (t == i) continue;
+            tg[t] = target[t];
+            if (tg[t].res) tg[t].res += (size_t)(start[i] - (i > t ? start[t + 1] - start[t] : 0)) * K;  // this block's first query of t
+        }
+        const jv_graph_s &g = *src[i].g;
+        const int32_t *own_adj = g.adj0.get<int32_t>(), *own_row;
+        int32_t *dadj, *drow;
+        e = alloc_owned(mem, drow, (size_t)cnt * 4);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(drow, src[i].live_row[level].data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess && level > 0) {
+            const std::vector<int32_t> &a = g.level_adj[level - 1];
+            e = alloc_owned(mem, dadj, a.size() * 4);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(dadj, a.data(), a.size() * 4, cudaMemcpyHostToDevice, s);
+            own_adj = dadj;
+        }
+        own_row = drow;
+        // the targets' device copy is read by the launch below before the next block's copy is enqueued behind it on `s`
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dtargets, tg.data(), (size_t)S * sizeof(CompactTarget), cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess)
+            e = launch_compact_assemble(cnt, degree, K, own_adj, own_row, maps_dev[i], dtargets, S, start[i], cand_stride, cand, cand_off + start[i],
+                                        cand_cnt + start[i], s);
+        if (e != cudaSuccess) rc = cuda_fail(e, "graph_compact: candidates");
+    }
+    std::vector<int> hcnt(rows);
+    if (!rc) {
+        e = cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)rows * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) e = prune_ragged_rows(merged->d, metric, alpha, degree, rows, cand, drow_node, cand_off, cand_cnt, hcnt, out_rows, g_sm_count, s);
+        if (e == cudaSuccess && level == 0) e = launch_scatter_rows(ng->adj0.get<int32_t>(), degree, drow_node, rows, out_rows, s);
+        std::vector<int32_t> hrows;
+        if (e == cudaSuccess && level > 0) {
+            hrows.resize((size_t)rows * degree);
+            e = cudaMemcpyAsync(hrows.data(), out_rows, hrows.size() * 4, cudaMemcpyDeviceToHost, s);
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) rc = cuda_fail(e, "graph_compact: prune");
+        for (int a = 0; a < rows && !rc; a++) {
+            stats->candidates += hcnt[a];
+            stats->max_candidates = std::max(stats->max_candidates, hcnt[a]);
+        }
+        if (!rc && level > 0) {
+            std::vector<int32_t> order(rows);
+            for (int a = 0; a < rows; a++) order[a] = a;
+            std::sort(order.begin(), order.end(), [&](int x, int y) { return row_node[x] < row_node[y]; });
+            ids_out->resize(rows);
+            adj_out->resize((size_t)rows * degree);
+            for (int r = 0; r < rows; r++) {
+                (*ids_out)[r] = row_node[order[r]];
+                std::copy_n(hrows.begin() + (size_t)order[r] * degree, degree, adj_out->begin() + (size_t)r * degree);
+            }
+        }
+    }
+    cudaStreamSynchronize(s);  // the level's scratch goes on return
+    return rc;
+}
+
+int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric, float alpha, jv_graph *graph_out, jv_dataset *rows_out,
+                     jv_compact_stats *stats)
+{
+    if (!sources || nsources < 1 || !graph_out || !rows_out || !stats) return fail(JV_ERR_INVALID, "graph_compact: null argument or no source");
+    for (int i = 0; i < nsources; i++)
+        if (!sources[i].graph || !sources[i].rows || !sources[i].old_to_new) return fail(JV_ERR_INVALID, "graph_compact: null argument");
+    ON_DEVICE_OF(sources[0].graph);
+    const int S = nsources, degree = sources[0].graph->g.degree, dim = sources[0].rows->d.dim;
+    for (int i = 0; i < S; i++) {
+        const jv_compact_source &c = sources[i];
+        if (c.rows->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "graph_compact: the sources' rows must be fp32");
+        if (c.rows->d.n != c.graph->g.n) return fail(JV_ERR_INVALID, "graph_compact: a source's rows and graph differ in size");
+        if (c.rows->d.dim != dim || c.graph->g.degree != degree || c.graph->device != t_active || c.rows->device != t_active)
+            return fail(JV_ERR_INVALID, "graph_compact: the sources differ in dim, degree or device");
+    }
+    int rc = check_metric(sources[0].rows->d, metric);
+    if (rc) return rc;
+    if (!(alpha >= 1.0f)) return fail(JV_ERR_INVALID, "graph_compact: need alpha >= 1");
+    // the live nodes (holes are dead) and their new ids, which must be exactly [0, live nodes)
+    std::vector<CompactSource> src(S);
+    long long total = 0;
+    int levels = 0;
+    for (int i = 0; i < S; i++) {
+        CompactSource &c = src[i];
+        c.g = sources[i].graph;
+        c.ds = sources[i].rows;
+        const int n = c.g->g.n;
+        c.map.assign(n, -1);
+        for (int v = 0; v < n; v++) {
+            const bool hole = !c.g->removed.empty() && bit_of(c.g->removed, v);
+            const bool live = !hole && (!sources[i].live_bits || ((sources[i].live_bits[v >> 5] >> (v & 31)) & 1u));
+            if (!live) continue;
+            c.map[v] = sources[i].old_to_new[v];
+            if (c.map[v] < 0) return fail(JV_ERR_INVALID, "graph_compact: a live node has a negative new id");
+            total++;
+        }
+        levels = std::max(levels, c.g->g.levels);
+    }
+    if (total == 0 || total > 0x7fffffffLL) return fail(JV_ERR_INVALID, "graph_compact: no live node, or more than 2^31 - 1");
+    std::vector<uint8_t> seen(total, 0);
+    for (const CompactSource &c : src)
+        for (int32_t x : c.map) {
+            if (x < 0) continue;
+            if (x >= total || seen[x]) return fail(JV_ERR_INVALID, "graph_compact: the new ids of the live nodes must be exactly [0, live nodes)");
+            seen[x] = 1;
+        }
+    if (degree > 64) return fail(JV_ERR_UNSUPPORTED, "graph_compact: degree above 64");
+    const int K = std::max(2, (degree + S - 1) / S * 4);
+    // a row's candidates must fit the prune's largest tier (8192): true for every S up to 2033 at degree 64
+    if (degree + (long long)(S - 1) * K > 8192) return fail(JV_ERR_UNSUPPORTED, "graph_compact: too many sources for one row's candidates");
+    for (CompactSource &c : src) {
+        c.live.resize(levels);  // a level the source does not have has no member
+        c.live_row.resize(levels);
+        for (int L = 0; L < c.g->g.levels; L++) {
+            const int cnt = L ? (int)c.g->level_ids[L - 1].size() : c.g->g.n;
+            for (int r = 0; r < cnt; r++) {
+                const int v = L ? c.g->level_ids[L - 1][r] : r;
+                if (c.map[v] < 0) continue;
+                c.live[L].push_back(v);
+                c.live_row[L].push_back(r);
+            }
+        }
+    }
+    if ((rc = t_ctx.init())) return rc;
+    cudaStream_t s = t_ctx.stream;
+    memset(stats, 0, sizeof(*stats));
+    std::unique_ptr<jv_dataset_s> nd(new jv_dataset_s());
+    nd->device = t_active;
+    memset(&nd->d, 0, sizeof(DataDesc));
+    nd->d.kind = KIND_F32; nd->d.dim = dim; nd->d.n = total; nd->d.stride = round4(dim);
+    std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
+    ng->device = t_active;
+    memset(&ng->g, 0, sizeof(GraphDesc));
+    ng->g.n = (int32_t)total; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_level = 0;
+    float *rows = nullptr;
+    if ((rc = nd->alloc(&rows, (size_t)total * nd->d.stride * 4))) return rc;
+    nd->d.rows = rows;
+    CK(ng->adj0.alloc((size_t)total * degree * 4), "cudaMalloc(adjacency)");
+    ng->g.adj0 = ng->adj0.get<int32_t>();
+    StreamTimer timer;
+    CK(timer.start(s), "event");
+    // every source's old -> new map on the device, and its live rows scattered to their new ids
+    std::vector<DeviceBuffer> mem;
+    std::vector<const int32_t *> maps_dev(S);
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < S && e == cudaSuccess; i++) {
+        const CompactSource &c = src[i];
+        const size_t cnt = c.live[0].size();
+        int32_t *dmap, *dold, *dnew;
+        std::vector<int32_t> hnew(cnt);
+        for (size_t j = 0; j < cnt; j++) hnew[j] = c.map[c.live[0][j]];
+        e = alloc_owned(mem, dmap, c.map.size() * 4);
+        if (e == cudaSuccess) e = alloc_owned(mem, dold, std::max<size_t>(cnt, 1) * 4);
+        if (e == cudaSuccess) e = alloc_owned(mem, dnew, std::max<size_t>(cnt, 1) * 4);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dmap, c.map.data(), c.map.size() * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dold, c.live[0].data(), cnt * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dnew, hnew.data(), cnt * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = launch_gather_rows(c.ds->d, dold, (int)cnt, rows, s, dnew);
+        maps_dev[i] = dmap;
+    }
+    if (e != cudaSuccess) rc = cuda_fail(e, "graph_compact: merged rows");
+    stats->search_top_k = K;
+    int nlev = 0;
+    for (int L = 0; L < levels && !rc; L++) {
+        long long members = 0;
+        for (const CompactSource &c : src) members += (long long)c.live[L].size();
+        if (members == 0) break;  // levels without a live member are dropped, and every level above one is empty too
+        if (L == 0) rc = compact_level(src, 0, K, nd.get(), metric, alpha, ng.get(), maps_dev, nullptr, nullptr, stats, s);
+        else {
+            std::vector<int32_t> ids, adj;
+            rc = compact_level(src, L, K, nd.get(), metric, alpha, ng.get(), maps_dev, &ids, &adj, stats, s);
+            ng->level_ids.push_back(std::move(ids));
+            ng->level_adj.push_back(std::move(adj));
+        }
+        nlev = L + 1;
+    }
+    timer.stop(s);
+    cudaStreamSynchronize(s);
+    if (rc) return rc;
+    // entry: the first source whose top level is the merged top level and whose entry is live, else the top level's lowest new id
+    int32_t entry = -1;
+    for (const CompactSource &c : src)
+        if (c.g->g.levels == nlev && c.g->g.entry_node >= 0 && c.map[c.g->g.entry_node] >= 0) {
+            entry = c.map[c.g->g.entry_node];
+            break;
+        }
+    if (entry < 0) entry = nlev > 1 ? ng->level_ids.back().front() : 0;
+    ng->g.entry_node = entry;
+    if ((rc = graph_rebuild_upper(ng.get()))) return rc;
+    stats->nodes = (int32_t)total;
+    stats->levels = ng->g.levels;
+    stats->device_ms = timer.ms();
+    *graph_out = ng.release();
+    *rows_out = nd.release();
+    return JV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ query batches (host-driven seam)

@@ -916,22 +916,24 @@ __global__ void __launch_bounds__(256) compact_adj_kernel(const int32_t *adj, co
     out[idx] = j < min(deg[v], degree) ? adj[(size_t)v * row_cap + j] : -1;
 }
 
-// rows [ids[i]] of a data set gathered into a dense one (upper levels of the hierarchy, repair pass): one warp per row
-__global__ void __launch_bounds__(256) gather_rows_kernel(const float *__restrict__ rows, int stride, const int32_t *__restrict__ ids, int count, float *__restrict__ out)
+// rows [ids[i]] of a data set gathered into a dense one (upper levels of the hierarchy, repair pass), or scattered to rows
+// [out_ids[i]] of another (the merged rows of a compaction): one warp per row
+__global__ void __launch_bounds__(256) gather_rows_kernel(const float *__restrict__ rows, int stride, const int32_t *__restrict__ ids, int count,
+                                                          const int32_t *__restrict__ out_ids, float *__restrict__ out)
 {
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (warp >= count) return;
     const float4 *src = reinterpret_cast<const float4 *>(rows + (size_t)ids[warp] * stride);
-    float4 *dst = reinterpret_cast<float4 *>(out + (size_t)warp * stride);
+    float4 *dst = reinterpret_cast<float4 *>(out + (size_t)(out_ids ? out_ids[warp] : warp) * stride);
     for (int i = lane; i < (stride >> 2); i += 32) dst[i] = ldg_stream(src + i);
 }
 
-cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s)
+cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s, const int32_t *out_ids_dev)
 {
     if (count <= 0) return cudaSuccess;
     const long long blocks = ((long long)count * 32 + 255) / 256;
-    gather_rows_kernel<<<(unsigned)blocks, 256, 0, s>>>(f32.rows, f32.stride, ids_dev, count, out_dev);
+    gather_rows_kernel<<<(unsigned)blocks, 256, 0, s>>>(f32.rows, f32.stride, ids_dev, count, out_ids_dev, out_dev);
     g_launches++;
     return cudaGetLastError();
 }
@@ -1570,6 +1572,51 @@ bool pq_repair_fits(const DataDesc &pq, int degree)
     return prune_smem_bytes(pq, CODE_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
 }
 
+// the prune of ragged candidate rows (mode 2, out of place), each row at the smallest tier that holds its candidates: the repair's
+// and the compaction's. tier_list: device scratch [rows]; tier_rows (optional) counts the rows of every tier
+static cudaError_t prune_ragged_enqueue(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *cand, const int32_t *row_node,
+                                        const long long *cand_off, const int *cand_cnt, const std::vector<int> &hcnt, int32_t *out_rows, int *out_deg,
+                                        int32_t *tier_list, int sm_count, long long *tier_rows, cudaStream_t s)
+{
+    cudaError_t err = cudaSuccess;
+    const bool codes = d.kind == KIND_PQ || d.kind == KIND_BQ;
+    const int ntiers = codes ? CODE_REPAIR_TIERS : REPAIR_TIERS;
+    const int *tier_max = codes ? CODE_REPAIR_TIER_MAX : REPAIR_TIER_MAX;
+    std::vector<int32_t> tiers[CODE_REPAIR_TIERS];
+    for (int a = 0; a < rows; a++) {
+        int t = 0;
+        while (t < ntiers - 1 && hcnt[a] > tier_max[t]) t++;
+        tiers[t].push_back(a);
+        if (tier_rows) tier_rows[t]++;
+    }
+    std::vector<int32_t> hlist;
+    for (int t = 0; t < ntiers; t++) hlist.insert(hlist.end(), tiers[t].begin(), tiers[t].end());
+    JV_TRY(cudaMemcpyAsync(tier_list, hlist.data(), (size_t)rows * 4, cudaMemcpyHostToDevice, s));
+    PruneParams P;
+    memset(&P, 0, sizeof(P));
+    P.d = d; P.metric = metric; P.degree = degree; P.row_cap = degree; P.alpha = alpha; P.mode = 2;
+    P.cand = cand; P.row_node = row_node; P.cand_off = cand_off; P.cand_cnt = cand_cnt;
+    P.out_rows = out_rows; P.out_deg = out_deg; P.out_stride = degree;
+    int first = 0;
+    for (int t = 0; t < ntiers; t++) {
+        const int c = (int)tiers[t].size();
+        if (c == 0) continue;
+        P.list = tier_list + first;
+        P.count = c;
+        JV_TRY(launch_prune(P, tier_max[t], true, std::min(c, sm_count * 5), s));
+        first += c;
+    }
+    return cudaSuccess;
+}
+
+cudaError_t launch_scatter_rows(int32_t *adj_dev, int degree, const int32_t *rows_of_dev, int count, const int32_t *rows_dev, cudaStream_t s)
+{
+    if (count <= 0) return cudaSuccess;
+    repair_scatter_kernel<<<(unsigned)(((long long)count * degree + 255) / 256), 256, 0, s>>>(adj_dev, degree, rows_of_dev, count, rows_dev);
+    g_launches++;
+    return cudaGetLastError();
+}
+
 // repair_level's work, enqueued on `s`; every block it allocates goes to `mem`
 static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new,
                                         const int32_t *ids_dev, const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev,
@@ -1635,42 +1682,15 @@ static cudaError_t repair_level_enqueue(const DataDesc &d, int metric, float alp
     JV_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)naff * 4, cudaMemcpyDeviceToHost, s));
     JV_TRY(cudaMemcpyAsync(hfb.data(), fallback, (size_t)naff, cudaMemcpyDeviceToHost, s));
     JV_TRY(cudaStreamSynchronize(s));
-    const bool codes = d.kind == KIND_PQ || d.kind == KIND_BQ;
-    const int ntiers = codes ? CODE_REPAIR_TIERS : REPAIR_TIERS;
-    const int *tier_max = codes ? CODE_REPAIR_TIER_MAX : REPAIR_TIER_MAX;
-    std::vector<int32_t> tiers[CODE_REPAIR_TIERS];
     for (int a = 0; a < naff; a++) {
-        int t = 0;
-        while (t < ntiers - 1 && hcnt[a] > tier_max[t]) t++;
-        tiers[t].push_back(a);
         st->candidates += hcnt[a];
         st->max_candidates = std::max(st->max_candidates, hcnt[a]);
         st->random_fallbacks += hfb[a];
-        st->tier_rows[t]++;
     }
     st->repaired_rows += naff;
-    std::vector<int32_t> hlist;
-    for (int t = 0; t < ntiers; t++) hlist.insert(hlist.end(), tiers[t].begin(), tiers[t].end());
-    JV_TRY(cudaMemcpyAsync(tier_list, hlist.data(), (size_t)naff * 4, cudaMemcpyHostToDevice, s));
-    {
-        PruneParams P;
-        memset(&P, 0, sizeof(P));
-        P.d = d; P.metric = metric; P.degree = degree; P.row_cap = degree; P.alpha = alpha; P.mode = 2;
-        P.cand = cand; P.row_node = row_node; P.cand_off = cand_off; P.cand_cnt = cand_cnt;
-        P.out_rows = out_rows; P.out_deg = out_deg; P.out_stride = degree;
-        int first = 0;
-        for (int t = 0; t < ntiers; t++) {
-            const int c = (int)tiers[t].size();
-            if (c == 0) continue;
-            P.list = tier_list + first;
-            P.count = c;
-            JV_TRY(launch_prune(P, tier_max[t], true, std::min(c, sm_count * 5), s));
-            first += c;
-        }
-    }
-    repair_scatter_kernel<<<(unsigned)(((long long)naff * degree + 255) / 256), 256, 0, s>>>(adj_new, degree, aff, naff, out_rows);
-    g_launches++;
-    return cudaGetLastError();
+    JV_TRY(prune_ragged_enqueue(d, metric, alpha, degree, naff, cand, row_node, cand_off, cand_cnt, hcnt, out_rows, out_deg, tier_list, sm_count,
+                                st->tier_rows, s));
+    return launch_scatter_rows(adj_new, degree, aff, naff, out_rows, s);
 }
 
 cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *adj_old, int32_t *adj_new, const int32_t *ids_dev,
@@ -1683,6 +1703,81 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
     std::vector<DeviceBuffer> mem;  // the scratch goes when this returns: the stream drains first, on success and on error
     const cudaError_t err = repair_level_enqueue(d, metric, alpha, degree, rows, adj_old, adj_new, ids_dev, rowmap_dev, dead_dev, members_dev, nmembers,
                                                  seed, level, sm_count, st, mem, s);
+    const cudaError_t drained = cudaStreamSynchronize(s);
+    return err != cudaSuccess ? err : drained;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Compaction (OnDiskGraphIndexCompactor's per-node work, DESIGN §4.3h). The searches into the other sources run in api.cu (the search
+// kernel over each source, or over a source's sub-hierarchy for an upper level); here every merged row of a level gets its candidate
+// segment and the repair's ragged prune picks its neighbours. The candidates are the node's live neighbours in its own source and,
+// per other source, the search results or that source's whole live membership of the level, each under its new id. Distinct
+// sources map to distinct new ids, so no segment holds an id twice and none needs a dedup. One warp per row; the ballot compaction
+// keeps the order of its inputs, so the segment is a pure function of them.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) compact_assemble_kernel(int rows, int degree, int K, const int32_t *__restrict__ own_adj,
+                                                               const int32_t *__restrict__ own_row, const int32_t *__restrict__ old_to_new,
+                                                               const CompactTarget *__restrict__ targets, int ntargets, long long row0, int cand_stride,
+                                                               int32_t *__restrict__ cand, long long *__restrict__ cand_off, int *__restrict__ cand_cnt)
+{
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (warp >= rows) return;
+    const int i = (int)warp;
+    const long long off = (row0 + i) * cand_stride;
+    int32_t *seg = cand + off;
+    int w = 0;
+    // every lane offers one id (-1: none); the kept ones are appended in lane order
+    auto put = [&](int32_t id) {
+        const unsigned b = __ballot_sync(FULL, id >= 0);
+        if (id >= 0) seg[w + __popc(b & ((1u << lane) - 1u))] = id;
+        w += __popc(b);
+    };
+    const int32_t *row = own_adj + (size_t)own_row[i] * degree;
+    for (int j0 = 0; j0 < degree; j0 += 32) {
+        const int32_t nb = j0 + lane < degree ? row[j0 + lane] : -1;
+        put(nb >= 0 ? old_to_new[nb] : -1);
+    }
+    for (int t = 0; t < ntargets; t++) {
+        const CompactTarget T = targets[t];
+        if (T.res) {
+            const int32_t *r = T.res + (size_t)i * K;
+            for (int j0 = 0; j0 < K; j0 += 32) {
+                const int32_t p = j0 + lane < K ? r[j0 + lane] : -1;
+                put(p >= 0 ? T.map[p] : -1);
+            }
+        } else {
+            for (int j0 = 0; j0 < T.count; j0 += 32) put(j0 + lane < T.count ? T.list[j0 + lane] : -1);
+        }
+    }
+    if (lane == 0) {
+        cand_off[i] = off;
+        cand_cnt[i] = w;
+    }
+}
+
+cudaError_t launch_compact_assemble(int rows, int degree, int K, const int32_t *own_adj, const int32_t *own_row, const int32_t *old_to_new,
+                                    const CompactTarget *targets_dev, int ntargets, long long row0, int cand_stride, int32_t *cand, long long *cand_off,
+                                    int *cand_cnt, cudaStream_t s)
+{
+    if (rows <= 0) return cudaSuccess;
+    compact_assemble_kernel<<<(unsigned)(((long long)rows * 32 + 255) / 256), 256, 0, s>>>(rows, degree, K, own_adj, own_row, old_to_new, targets_dev,
+                                                                                          ntargets, row0, cand_stride, cand, cand_off, cand_cnt);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t prune_ragged_rows(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *cand, const int32_t *row_node,
+                              const long long *cand_off, const int *cand_cnt, const std::vector<int> &hcnt, int32_t *out_rows, int sm_count, cudaStream_t s)
+{
+    if (rows <= 0) return cudaSuccess;
+    if (degree < 1 || degree > 64 || d.kind != KIND_F32) return cudaErrorInvalidValue;
+    std::vector<DeviceBuffer> mem;  // the scratch goes when this returns: the stream drains first, on success and on error
+    cudaError_t err = cudaSuccess;
+    int *out_deg = nullptr;
+    int32_t *tier_list = nullptr;
+    if ((err = alloc_owned(mem, out_deg, (size_t)rows * 4)) == cudaSuccess && (err = alloc_owned(mem, tier_list, (size_t)rows * 4)) == cudaSuccess)
+        err = prune_ragged_enqueue(d, metric, alpha, degree, rows, cand, row_node, cand_off, cand_cnt, hcnt, out_rows, out_deg, tier_list, sm_count, nullptr, s);
     const cudaError_t drained = cudaStreamSynchronize(s);
     return err != cudaSuccess ? err : drained;
 }

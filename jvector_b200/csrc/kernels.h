@@ -4,6 +4,7 @@
 #include <atomic>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <vector>
 
 #include "scorers.cuh"
 
@@ -188,7 +189,8 @@ cudaError_t builder_finish(GraphBuilder *B, int32_t *adj_out_dev, BuildStats *st
 int builder_row_cap(const GraphBuilder *B);
 int builder_degree(const GraphBuilder *B);
 int builder_max_batch(const GraphBuilder *B);
-cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s);
+// rows [ids[i]] of an fp32 data set into out_dev [count][stride], or into rows out_ids_dev[i] of out_dev when that is given
+cudaError_t launch_gather_rows(const DataDesc &f32, const int32_t *ids_dev, int count, float *out_dev, cudaStream_t s, const int32_t *out_ids_dev = nullptr);
 // PQ / BQ build (pqBuildScoreProvider, bqBuildScoreProvider): the fixed-size rows [ids[i]] of the code array (PQ code rows, BQ word rows,
 // code_row_bytes each) into out_dev [count][code_row_bytes]; whether the PQ prune holds the data set's LUT
 int code_row_bytes(const DataDesc &d);
@@ -214,6 +216,26 @@ cudaError_t repair_level(const DataDesc &d, int metric, float alpha, int degree,
                          const int32_t *rowmap_dev, const uint32_t *dead_dev, const int32_t *members_dev, int nmembers, uint64_t seed, int level,
                          int sm_count, RepairStats *st, cudaStream_t s);
 cudaError_t launch_clear_dead_rows(int32_t *adj_dev, int n, int degree, const uint32_t *dead_dev, cudaStream_t s);
+
+// OnDiskGraphIndexCompactor's per-node work on one level (DESIGN §4.3h, build.cu "Compaction"). The level's rows are handed over one
+// source at a time: row i of a source block is the source's live member own_row[i] of its level adjacency own_adj; its candidates
+// are its live neighbours mapped through old_to_new (-1 = dead), then, per other source t, targets[t]'s candidates: the search
+// results res[i * K ..] mapped through map (-1 = dead or padding), or, when res is null, the `count` new ids of list for every row.
+// The candidate segment of block row i goes to cand[(row0 + i) * cand_stride ..], its count to cand_cnt[i], its offset to cand_off[i].
+struct CompactTarget {
+    const int32_t *res, *map, *list;
+    int count;
+};
+cudaError_t launch_compact_assemble(int rows, int degree, int K, const int32_t *own_adj, const int32_t *own_row, const int32_t *old_to_new,
+                                    const CompactTarget *targets_dev, int ntargets, long long row0, int cand_stride, int32_t *cand, long long *cand_off,
+                                    int *cand_cnt, cudaStream_t s);
+// the builder's prune over `rows` ragged candidate rows (the repair's tiers, mode 2, out of place): row a is node row_node[a] of d,
+// its candidates cand[cand_off[a] .. + cand_cnt[a]) (hcnt: the same counts on the host); the selected rows go to out_rows
+// [rows][degree], -1 padded. Synchronises `s`.
+cudaError_t prune_ragged_rows(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *cand, const int32_t *row_node,
+                              const long long *cand_off, const int *cand_cnt, const std::vector<int> &hcnt, int32_t *out_rows, int sm_count, cudaStream_t s);
+// adj_dev[rows_of[a] * degree ..] = rows_dev[a * degree ..] for a < count
+cudaError_t launch_scatter_rows(int32_t *adj_dev, int degree, const int32_t *rows_of_dev, int count, const int32_t *rows_dev, cudaStream_t s);
 
 // ---- pq_train.cu: ProductQuantization.compute / refine (UNWEIGHTED) ----
 struct PqTrainArgs {
