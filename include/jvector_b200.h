@@ -125,6 +125,18 @@ JV_API int jv_dataset_adopt_f32_device(const float *rows_device, int64_t n, int 
  * rounded up to 8, padding codes 0), meta_out [n][2] = {scale, radius} per row. Builds nothing: JV_ERR_INVALID ("no row sketch")
  * while no search has built one. codes_out / meta_out may be NULL (only *sketch_stride_out, and whether the sketch exists). */
 JV_API int jv_dataset_row_sketch_download(jv_dataset f32, int8_t *codes_out, float *meta_out, int *sketch_stride_out);
+/* The low-rank rows of an fp32 data set, built with its row sketch when the rows lie close to a rank-32 subspace: basis [rank][stride]
+   fp32, rows [n][48] bytes = rank int8 codes then float {t, rho, beta, ||x||} (DESIGN §4.1). JV_ERR_INVALID when there are none;
+   rank_out is set either way. Either output may be NULL. */
+JV_API int jv_dataset_lowrank_download(jv_dataset f32, float *basis_out, uint8_t *rows_out, int *rank_out);
+/* A graph's edge records for the low-rank bound: [n][degree][48] bytes, slot t of node v = the low-rank row of its t-th level-0
+   neighbour (zeros for an empty slot). Built by the first sketched search; JV_ERR_INVALID when there are none. */
+JV_API int jv_graph_edge_records_download(jv_graph g, uint8_t *out);
+/* New neighbours the calling thread's last graph search settled on edge records (they are part of jv_search_stats.visited). */
+JV_API int64_t jv_search_last_settled(void);
+/* The low-rank bound as a DOT_PRODUCT score of rows[i] against queries[i] (both [n][dim]) for basis [dim][32] (column j = basis
+   vector j), computed by the device functions the search uses; records_out (may be NULL): the rows' [n][48]-byte records. */
+JV_API int jv_lowrank_bound_pairs(const float *basis, int dim, const float *rows, const float *queries, int64_t n, uint8_t *records_out, float *bounds_out);
 JV_API int jv_dataset_device(jv_dataset ds);
 /* ImmutablePQVectors' code-vs-code scoring (base:quantization/ImmutablePQVectors.java:63-105): build the triangular
  * centroid-vs-centroid table of ProductQuantization.createCodebookPartialSums (ProductQuantization.java:609-628; 12.6 MB at M = 96,

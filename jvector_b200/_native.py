@@ -97,6 +97,10 @@ SYMBOLS = [
     ("jv_dataset_register_nvq", _I, [u8p, f32p, _L, _I, _I, f32p, C.POINTER(_P)]),
     ("jv_dataset_adopt_f32_device", _I, [_P, _L, _I, _I, C.POINTER(_P)]), ("jv_dataset_device", _I, [_P]),
     ("jv_dataset_row_sketch_download", _I, [_P, _P, f32p, C.POINTER(_I)]),
+    ("jv_dataset_lowrank_download", _I, [_P, f32p, _P, C.POINTER(_I)]),
+    ("jv_graph_edge_records_download", _I, [_P, _P]),
+    ("jv_search_last_settled", _L, []),
+    ("jv_lowrank_bound_pairs", _I, [f32p, _I, f32p, f32p, C.c_int64, _P, f32p]),
     ("jv_dataset_pq_pair_table", _I, [_P, _I]), ("jv_dataset_pq_pair_table_download", _I, [_P, _I, f32p]),
     ("jv_dataset_free", _I, [_P]), ("jv_dataset_size", _L, [_P]), ("jv_dataset_dim", _I, [_P]), ("jv_dataset_device_bytes", _L, [_P]),
     ("jv_query_begin", _I, [_P, f32p, _I, C.POINTER(_P)]), ("jv_score_batch", _I, [_P, i32p, _I, f32p]), ("jv_query_end", _I, [_P]),

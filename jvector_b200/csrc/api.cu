@@ -6,6 +6,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
+#include <cmath>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -180,6 +182,11 @@ struct jv_dataset_s {
     // Not part of `d`: only the search kernel's fp32 DOT walks read it, the builder and the batch scorers never see it
     DeviceBuffer sketch, sketch_meta;
     bool sketch_failed = false;  // the allocation failed once: walk without it from then on
+    // low-rank rows (lowrank_rows_kernel) and their basis, built with the sketch (ensure_lowrank); lr_id names this build for the
+    // graphs' edge records (0: none). lr_off: the data set does not get them (too wide, too far from a rank-LR_K subspace, or out of memory)
+    DeviceBuffer lr_basis, lr_rows;
+    uint64_t lr_id = 0;
+    bool lr_off = false;
     std::mutex sketch_mu;
     template <typename T>
     int alloc(T **p, size_t n)
@@ -205,6 +212,13 @@ struct jv_graph_s {
     std::vector<std::vector<int32_t>> level_ids;  // host copies, level >= 1
     std::vector<std::vector<int32_t>> level_adj;
     std::vector<uint32_t> removed;  // ids taken out by jv_graph_remove_deleted (holes), bit (id & 31) of word (id >> 5); empty = none
+    // edge records of the low-rank bound (launch_edge_records) for the data set whose lr_id is edge_rec_of; built by the first
+    // sketched search over that data set, freed with the graph
+    // (shared: a search holds its records until its kernels are done, so a concurrent search over another data set that replaces
+    // them cannot free them under it)
+    std::shared_ptr<DeviceBuffer> edge_rec;
+    uint64_t edge_rec_of = 0;
+    std::mutex edge_mu;
 };
 
 struct jv_multi_s {
@@ -1210,7 +1224,172 @@ int jv_dataset_row_sketch_download(jv_dataset f32, int8_t *codes_out, float *met
     return JV_OK;
 }
 
-// the fp32 row sketch of a data set (row_sketch_kernel), built once. Complete when this returns: another thread's stream may read it
+static thread_local int64_t t_last_settled = 0;
+int64_t jv_search_last_settled(void) { return t_last_settled; }
+
+int jv_lowrank_bound_pairs(const float *basis, int dim, const float *rows, const float *queries, int64_t n, uint8_t *records_out, float *bounds_out)
+{
+    if (!basis || !rows || !queries || dim <= 0 || n <= 0 || !bounds_out) return fail(JV_ERR_INVALID, "lowrank_bound_pairs: bad arguments");
+    int rc = t_ctx.init();
+    if (rc) return rc;
+    cudaStream_t s = t_ctx.stream;
+    const int stride = (dim + 3) & ~3;
+    if (lowrank_warps(stride) == 0) return fail(JV_ERR_UNSUPPORTED, "lowrank_bound_pairs: rows too wide");
+    DeviceBuffer B, X, Q, R, O;
+    CK(B.alloc((size_t)LR_K * stride * 4), "cudaMalloc");
+    CK(X.alloc((size_t)n * stride * 4), "cudaMalloc");
+    CK(Q.alloc((size_t)n * stride * 4), "cudaMalloc");
+    CK(R.alloc((size_t)n * LR_SLOT), "cudaMalloc");
+    CK(O.alloc((size_t)n * 4), "cudaMalloc");
+    // basis: [dim][LR_K] row-major on the host (column j = basis vector j), stored [LR_K][stride] on the device
+    std::vector<float> bt((size_t)LR_K * stride, 0.f);
+    for (int i = 0; i < dim; i++)
+        for (int j = 0; j < LR_K; j++) bt[(size_t)j * stride + i] = basis[(size_t)i * LR_K + j];
+    CK(cudaMemsetAsync(X.get(), 0, (size_t)n * stride * 4, s), "memset");
+    CK(cudaMemsetAsync(Q.get(), 0, (size_t)n * stride * 4, s), "memset");
+    CK(cudaMemcpyAsync(B.get(), bt.data(), bt.size() * 4, cudaMemcpyHostToDevice, s), "H2D basis");
+    CK(cudaMemcpy2DAsync(X.get(), (size_t)stride * 4, rows, (size_t)dim * 4, (size_t)dim * 4, n, cudaMemcpyHostToDevice, s), "H2D rows");
+    CK(cudaMemcpy2DAsync(Q.get(), (size_t)stride * 4, queries, (size_t)dim * 4, (size_t)dim * 4, n, cudaMemcpyHostToDevice, s), "H2D queries");
+    CK(launch_lowrank_rows(X.get<float>(), n, stride, B.get<float>(), R.get<uint8_t>(), s), "lowrank_rows");
+    CK(launch_lowrank_bound_pairs(B.get<float>(), dim, stride, Q.get<float>(), R.get<uint8_t>(), n, O.get<float>(), s), "lowrank_bound_pairs");
+    if (records_out) CK(cudaMemcpyAsync(records_out, R.get(), (size_t)n * LR_SLOT, cudaMemcpyDeviceToHost, s), "D2H records");
+    CK(cudaMemcpyAsync(bounds_out, O.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, s), "D2H bounds");
+    CK(cudaStreamSynchronize(s), "lowrank_bound_pairs");
+    return JV_OK;
+}
+
+int jv_dataset_lowrank_download(jv_dataset f32, float *basis_out, uint8_t *rows_out, int *rank_out)
+{
+    ON_DEVICE_OF(f32);
+    if (f32->d.kind != KIND_F32) return fail(JV_ERR_INVALID, "lowrank_download: not an fp32 data set");
+    if (rank_out) *rank_out = LR_K;
+    std::lock_guard<std::mutex> lk(f32->sketch_mu);
+    if (!f32->lr_rows.get()) return fail(JV_ERR_INVALID, f32->lr_off ? "lowrank_download: the data set has no low-rank rows" : "lowrank_download: no sketched search has run");
+    if (basis_out) CK(cudaMemcpy(basis_out, f32->lr_basis.get(), (size_t)LR_K * f32->d.stride * 4, cudaMemcpyDeviceToHost), "D2H low-rank basis");
+    if (rows_out) CK(cudaMemcpy(rows_out, f32->lr_rows.get(), (size_t)f32->d.n * LR_SLOT, cudaMemcpyDeviceToHost), "D2H low-rank rows");
+    return JV_OK;
+}
+
+int jv_graph_edge_records_download(jv_graph g, uint8_t *out)
+{
+    ON_DEVICE_OF(g);
+    std::lock_guard<std::mutex> lk(g->edge_mu);
+    if (!g->edge_rec) return fail(JV_ERR_INVALID, "edge_records_download: no edge records");
+    if (out) CK(cudaMemcpy(out, g->edge_rec->get(), (size_t)g->g.n * g->g.degree * LR_SLOT, cudaMemcpyDeviceToHost), "D2H edge records");
+    return JV_OK;
+}
+
+// modified Gram-Schmidt over the LR_K columns (rows of v, `stride` apart) in double; a column that vanishes becomes 0
+static void orthonormalise(std::vector<double> &v, int stride)
+{
+    for (int j = 0; j < LR_K; j++) {
+        double *vj = v.data() + (size_t)j * stride;
+        for (int i = 0; i < j; i++) {
+            const double *vi = v.data() + (size_t)i * stride;
+            double d = 0.0;
+            for (int x = 0; x < stride; x++) d += vi[x] * vj[x];
+            for (int x = 0; x < stride; x++) vj[x] -= d * vi[x];
+        }
+        double nn = 0.0;
+        for (int x = 0; x < stride; x++) nn += vj[x] * vj[x];
+        nn = std::sqrt(nn);
+        for (int x = 0; x < stride; x++) vj[x] = nn > 1e-300 ? vj[x] / nn : 0.0;
+    }
+}
+
+// The low-rank rows of a data set (scorers.cuh lowrank_bound), caller holds sketch_mu. The basis: LR_BASIS_ITERS steps of subspace
+// iteration over LR_BASIS_ROWS evenly spaced rows, started from the first LR_K of them. The bound only pays where the rows lie close
+// to a rank-LR_K subspace: if the median rho / ||x|| over the sampled rows exceeds LR_MAX_RESIDUAL the data set gets none (an
+// isotropic data set would read the edge records and settle almost nothing on them).
+constexpr int LR_BASIS_ROWS = 4096, LR_BASIS_ITERS = 4;
+constexpr double LR_MAX_RESIDUAL = 0.5;
+static int ensure_lowrank(jv_dataset ds, cudaStream_t s)
+{
+    static std::atomic<uint64_t> next_id{1};
+    const int stride = ds->d.stride;
+    const long long n = ds->d.n;
+    const int S = (int)std::min<long long>(n, LR_BASIS_ROWS);
+    const long long step = std::max<long long>(1, n / LR_BASIS_ROWS);
+    DeviceBuffer V, Z, Y, B, rows;
+    if (n < LR_K || lowrank_warps(stride) == 0 || V.alloc((size_t)LR_K * stride * 8) != cudaSuccess || Y.alloc((size_t)LR_K * stride * 8) != cudaSuccess ||
+        Z.alloc((size_t)S * LR_K * 8) != cudaSuccess || B.alloc((size_t)LR_K * stride * 4) != cudaSuccess || rows.alloc((size_t)n * LR_SLOT) != cudaSuccess) {
+        cudaGetLastError();  // out of memory (or too few rows): the walk keeps the sketch alone
+        ds->lr_off = true;
+        return JV_OK;
+    }
+    // every copy and kernel below runs on `s` (a non-blocking stream: the legacy default stream would not order against it), and the
+    // host waits for `s` before it reads or rewrites a host buffer the stream uses
+    std::vector<float> x0((size_t)LR_K * stride);
+    CK(cudaMemcpy2DAsync(x0.data(), (size_t)stride * 4, ds->d.rows, (size_t)step * stride * 4, (size_t)stride * 4, LR_K, cudaMemcpyDeviceToHost, s), "D2H basis rows");
+    CK(cudaStreamSynchronize(s), "D2H basis rows");
+    std::vector<double> v(x0.begin(), x0.end());
+    orthonormalise(v, stride);
+    for (int it = 0; it < LR_BASIS_ITERS; it++) {
+        CK(cudaMemcpyAsync(V.get(), v.data(), v.size() * 8, cudaMemcpyHostToDevice, s), "H2D basis");
+        CK(launch_lowrank_iteration(ds->d.rows, stride, step, S, V.get<double>(), Z.get<double>(), Y.get<double>(), s), "lowrank_iteration");
+        CK(cudaMemcpyAsync(v.data(), Y.get(), v.size() * 8, cudaMemcpyDeviceToHost, s), "D2H basis");
+        CK(cudaStreamSynchronize(s), "lowrank_iteration");
+        orthonormalise(v, stride);
+    }
+    std::vector<float> bf(v.begin(), v.end());
+    CK(cudaMemcpyAsync(B.get(), bf.data(), bf.size() * 4, cudaMemcpyHostToDevice, s), "H2D basis");
+    cudaError_t e = launch_lowrank_rows(ds->d.rows, n, stride, B.get<float>(), rows.get<uint8_t>(), s);
+    std::vector<float4> meta(S);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(meta.data(), 16, rows.get<uint8_t>() + LR_K, (size_t)step * LR_SLOT, 16, S, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    CK(e, "lowrank_rows");
+    std::vector<double> ratio;
+    for (const float4 &m : meta)
+        if (m.w > 0.f) ratio.push_back((double)m.y / m.w);
+    if (ratio.empty()) {
+        ds->lr_off = true;
+        return JV_OK;
+    }
+    std::nth_element(ratio.begin(), ratio.begin() + ratio.size() / 2, ratio.end());
+    if (ratio[ratio.size() / 2] > LR_MAX_RESIDUAL) {
+        ds->lr_off = true;
+        return JV_OK;
+    }
+    ds->lr_basis = std::move(B);
+    ds->lr_rows = std::move(rows);
+    ds->lr_id = next_id++;
+    return JV_OK;
+}
+
+// the edge records of graph g for data set ds's low-rank rows, built once per (graph, data set build). *out: the records (empty when
+// there are none), which the caller holds until its kernels have finished
+static int ensure_edge_records(jv_graph g, jv_dataset ds, cudaStream_t s, std::shared_ptr<DeviceBuffer> *out)
+{
+    out->reset();
+    uint64_t id;
+    const uint8_t *lr;
+    {
+        std::lock_guard<std::mutex> lk(ds->sketch_mu);
+        id = ds->lr_id;
+        lr = ds->lr_rows.get<uint8_t>();
+    }
+    if (!id || g->g.n <= 0) return JV_OK;
+    std::lock_guard<std::mutex> lk(g->edge_mu);
+    if (g->edge_rec_of != id) {
+        g->edge_rec.reset();  // freed here unless a running search still holds it (then when that search ends)
+        g->edge_rec_of = 0;
+        auto rec = std::make_shared<DeviceBuffer>();
+        if (rec->alloc((size_t)g->g.n * g->g.degree * LR_SLOT) != cudaSuccess) {
+            cudaGetLastError();  // out of memory: the walk keeps the sketch alone
+            return JV_OK;
+        }
+        cudaError_t e = launch_edge_records(g->g.adj0, g->g.n, g->g.degree, lr, rec->get<uint8_t>(), s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        CK(e, "edge_records");
+        g->edge_rec = std::move(rec);
+        g->edge_rec_of = id;
+    }
+    *out = g->edge_rec;
+    return JV_OK;
+}
+
+// the fp32 row sketch of a data set (row_sketch_kernel), built once, and its low-rank rows (ensure_lowrank). Complete when this
+// returns: another thread's stream may read them
 static int ensure_sketch(jv_dataset ds, cudaStream_t s)
 {
     std::lock_guard<std::mutex> lk(ds->sketch_mu);
@@ -1227,7 +1406,7 @@ static int ensure_sketch(jv_dataset ds, cudaStream_t s)
     CK(e, "row_sketch");
     ds->sketch = std::move(sk);
     ds->sketch_meta = std::move(meta);
-    return JV_OK;
+    return ensure_lowrank(ds, s);
 }
 
 // query_stride: floats between two queries (0: dim)
@@ -1271,7 +1450,13 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         ad.sketch = approx->sketch.get<int8_t>();
         ad.sketch_meta = approx->sketch_meta.get<float2>();
         ad.sketch_stride = sketch_stride(ad.stride);
+        ad.lr_basis = approx->lr_basis.get<float>();
     }
+    // a sketched walk over a data set with low-rank rows settles most hopeless neighbours at gather time on the graph's edge records
+    GraphDesc gd = g->g;
+    std::shared_ptr<DeviceBuffer> edge_rec;  // held until this function returns: every path out of it has synchronised `s`
+    if (ad.sketch && ad.lr_basis && search_uses_sketch(ad, metric, plan, nq) && (rc = ensure_edge_records(g, approx, s, &edge_rec))) return rc;
+    gd.edge_rec = edge_rec ? edge_rec->get<uint8_t>() : nullptr;
     // counters, work counter, per-query overflow codes, retry index (carved over nullptr: the block's size)
     SearchCounters *dcnt;
     int *dwork;
@@ -1303,7 +1488,7 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         }
         if ((rc = grow(t_ctx.search_scratch, search_scratch_bytes(plan)))) return rc;
         CK(t_ctx.timer.start(s), "event");
-        CK(launch_search(g->g, ad, rr, metric, queries_dev, cnt, topK, rerankK, plan, t_ctx.search_scratch.get(), dwork, nodes_dev, scores_dev, dcnt, dover,
+        CK(launch_search(gd, ad, rr, metric, queries_dev, cnt, topK, rerankK, plan, t_ctx.search_scratch.get(), dwork, nodes_dev, scores_dev, dcnt, dover,
                          attempt ? dindex : nullptr, query_stride, filter, s),
            "launch_search");
         CK(t_ctx.timer.stop(s), "event");
@@ -1337,6 +1522,9 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         stats->expanded = (int64_t)hc.expanded;
         stats->expanded_base = (int64_t)hc.expanded_base;
         stats->reranked = (int64_t)hc.reranked;
+    }
+    t_last_settled = (int64_t)hc.settled;
+    if (stats) {
         stats->retried = retried;
         stats->device_ms = ms;
     }

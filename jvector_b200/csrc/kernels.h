@@ -44,10 +44,14 @@ struct GraphDesc {
     const uint8_t *fused_codes_of;  // the PQ code array the records were packed from (identity of the data set they belong to)
     int fused_rec;                  // bytes per record (multiple of 16)
     int fused_code_stride;
+    // low-rank edge bound (scorers.cuh lowrank_bound): [n][degree][LR_SLOT], slot t = the low-rank row of adj0[v][t]. Set per search
+    // (api.cu search_device) for a sketched walk over the data set the records were built from; nullptr otherwise
+    const uint8_t *edge_rec;
 };
 
 struct SearchCounters {  // device-side totals
     unsigned long long visited, expanded, expanded_base, reranked, overflowed;
+    unsigned long long settled;  // new neighbours settled on their edge record (part of `visited`)
 };
 
 // ---- kernels_batch.cu ----
@@ -79,6 +83,16 @@ cudaError_t launch_topk_merge_strided(const long long *keys_in_dev, int nq, int 
 
 // int8 row sketch + {scale, radius} per row of an fp32 data set (the search kernel's sketch bound, see sketch_bound_pair)
 cudaError_t launch_row_sketch(const float *rows_dev, long long n, int stride, int sketch_stride, int8_t *sketch_dev, float2 *meta_dev, cudaStream_t s);
+// the low-rank edge bound (scorers.cuh lowrank_bound): one subspace-iteration step Y = X^T (X V) over the rows s * step, s < S
+// (V, Y: [LR_K][stride] float64, Z: [S][LR_K] scratch); every row's codes and {t, rho, beta, xn} ([n][LR_SLOT]; nothing is launched for
+// rows too wide to stage, lowrank_warps(stride) == 0); a graph's edge records ([n][degree][LR_SLOT], the rows of adj0's ids)
+cudaError_t launch_lowrank_iteration(const float *rows_dev, int stride, long long step, int S, const double *V_dev, double *Z_dev, double *Y_dev, cudaStream_t s);
+int lowrank_warps(int stride);
+cudaError_t launch_lowrank_rows(const float *rows_dev, long long n, int stride, const float *B_dev, uint8_t *out_dev, cudaStream_t s);
+// the low-rank bound as a DOT_PRODUCT score of row i against query i (rows_dev, queries_dev: [n][stride] zero padded), with the
+// records of those rows in records_dev ([n][LR_SLOT], launch_lowrank_rows): one CTA per pair, the search kernel's device functions
+cudaError_t launch_lowrank_bound_pairs(const float *B_dev, int dim, int stride, const float *queries_dev, const uint8_t *records_dev, long long n, float *out_dev, cudaStream_t s);
+cudaError_t launch_edge_records(const int32_t *adj0_dev, long long n, int degree, const uint8_t *lr_rows_dev, uint8_t *rec_dev, cudaStream_t s);
 cudaError_t launch_bq_encode(const float *rows_dev, long long n, int dim, int row_stride, unsigned long long *words_dev, cudaStream_t s);
 cudaError_t launch_pq_encode(const DataDesc &pq, const float *rows_dev, long long n, int row_stride, uint8_t *codes_dev, cudaStream_t s);
 cudaError_t launch_pq_self_magnitudes(const DataDesc &pq, float *mag_dev, cudaStream_t s);

@@ -782,6 +782,181 @@ cudaError_t launch_row_sketch(const float *rows_dev, long long n, int stride, in
     return cudaGetLastError();
 }
 
+// Basis of the low-rank edge bound (scorers.cuh lowrank_bound): subspace iteration V <- orth(X^T (X V)) over the rows s * step,
+// s < S, in float64; the orthonormalisation of the LR_K columns runs on the host (api.cu ensure_lowrank). Z = X V: one warp per
+// sampled row. Y = X^T Z: one thread per (column j, coordinate i).
+__global__ void __launch_bounds__(256) lowrank_project_kernel(const float *__restrict__ rows, int stride, long long step, int S, const double *__restrict__ V,
+                                                              double *__restrict__ Z)
+{
+    const int sr = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (sr >= S) return;
+    const float *x = rows + (size_t)sr * step * stride;
+    for (int j = 0; j < LR_K; j++) {
+        double a = 0.0;
+        for (int i = lane; i < stride; i += 32) a = fma((double)x[i], V[(size_t)j * stride + i], a);
+        for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+        if (lane == 0) Z[(size_t)sr * LR_K + j] = a;
+    }
+}
+
+__global__ void __launch_bounds__(256) lowrank_gram_kernel(const float *__restrict__ rows, int stride, long long step, int S, const double *__restrict__ Z,
+                                                           double *__restrict__ Y)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y;
+    if (i >= stride) return;
+    double a = 0.0;
+    for (int sr = 0; sr < S; sr++) a = fma((double)rows[(size_t)sr * step * stride + i], Z[(size_t)sr * LR_K + j], a);
+    Y[(size_t)j * stride + i] = a;
+}
+
+cudaError_t launch_lowrank_iteration(const float *rows_dev, int stride, long long step, int S, const double *V_dev, double *Z_dev, double *Y_dev, cudaStream_t s)
+{
+    lowrank_project_kernel<<<(unsigned)((S * 32 + 255) / 256), 256, 0, s>>>(rows_dev, stride, step, S, V_dev, Z_dev);
+    lowrank_gram_kernel<<<dim3((unsigned)((stride + 127) / 128), LR_K), 128, 0, s>>>(rows_dev, stride, step, S, Z_dev, Y_dev);
+    g_launches += 2;
+    return cudaGetLastError();
+}
+
+// Low-rank rows (scorers.cuh lowrank_bound): one warp per row, float64 throughout. a = B^T x, t = max|a_j| / 127 rounded to fp32,
+// c = round(a / t) in [-127, 127] (0 when t = 0), w = x - t B c with each w_i within lr_g64(LR_K + 2) A_i, A_i = |x_i| + t sum_j |B_ij c_j|,
+// so rho = ||w~|| + g ||A|| >= ||w||; |(B^T w)_j| <= |(B^T w~)_j| + lr_g64(stride + LR_K + 2) sum_i |B_ij| (|w~_i| + A_i) gives beta.
+// Out: [n][LR_SLOT] = LR_K int8 codes, then {t, rho, beta, xn} rounded up. w~ and A are staged in shared memory, 2 stride doubles
+// per warp.
+__global__ void lowrank_rows_kernel(const float *__restrict__ rows, long long n, int stride, const float *__restrict__ B, uint8_t *__restrict__ out)
+{
+    extern __shared__ double lr_stage[];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + wib;
+    if (r >= n) return;
+    double *ws = lr_stage + (size_t)wib * 2 * stride, *as = ws + stride;
+    const float *x = rows + r * stride;
+    double aj = 0.0;  // lane j: a_j
+    for (int j = 0; j < LR_K; j++) {
+        double a = 0.0;
+        for (int i = lane; i < stride; i += 32) a = fma((double)__ldg(B + (size_t)j * stride + i), (double)x[i], a);
+        for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(FULL, a, o);
+        if (lane == j) aj = a;
+    }
+    double amax = fabs(aj);
+    for (int o = 16; o; o >>= 1) amax = fmax(amax, __shfl_xor_sync(FULL, amax, o));
+    const float t = (float)(amax / 127.0);
+    const int cj = t > 0.f ? (int)fmin(127.0, fmax(-127.0, rint(aj / (double)t))) : 0;
+    out[r * LR_SLOT + lane] = (uint8_t)(int8_t)cj;
+    double w2 = 0.0, a2 = 0.0, x2 = 0.0;
+    for (int i0 = 0; i0 < stride; i0 += 32) {  // every lane runs every step: the code shuffles below name the whole warp
+        const int i = i0 + lane;
+        double v = 0.0, av = 0.0;
+        for (int j = 0; j < LR_K; j++) {
+            const double c = (double)__shfl_sync(FULL, cj, j);
+            const double bc = i < stride ? (double)__ldg(B + (size_t)j * stride + i) * c : 0.0;
+            v += bc;
+            av += fabs(bc);
+        }
+        if (i >= stride) continue;
+        const double xi = (double)x[i];
+        const double w = xi - (double)t * v, A = fabs(xi) + (double)t * av;
+        ws[i] = w;
+        as[i] = A;
+        w2 = fma(w, w, w2);
+        a2 = fma(A, A, a2);
+        x2 = fma(xi, xi, x2);
+    }
+    __syncwarp();
+    double bj = 0.0;  // lane j: |(B^T w~)_j| + its error bound
+    const double gb = lr_g64(stride + LR_K + 2);
+    for (int j = 0; j < LR_K; j++) {
+        double bw = 0.0, ab = 0.0;
+        for (int i = lane; i < stride; i += 32) {
+            const double b = (double)__ldg(B + (size_t)j * stride + i);
+            bw = fma(b, ws[i], bw);
+            ab = fma(fabs(b), fabs(ws[i]) + as[i], ab);
+        }
+        for (int o = 16; o; o >>= 1) {
+            bw += __shfl_xor_sync(FULL, bw, o);
+            ab += __shfl_xor_sync(FULL, ab, o);
+        }
+        if (lane == j) bj = fabs(bw) + gb * ab;
+    }
+    double b2 = bj * bj;
+    for (int o = 16; o; o >>= 1) {
+        b2 += __shfl_xor_sync(FULL, b2, o);
+        w2 += __shfl_xor_sync(FULL, w2, o);
+        a2 += __shfl_xor_sync(FULL, a2, o);
+        x2 += __shfl_xor_sync(FULL, x2, o);
+    }
+    if (lane == 0) {
+        const float rho = __double2float_ru((sqrt(w2 * LR_PAD) + lr_g64(LR_K + 2) * sqrt(a2 * LR_PAD)) * LR_PAD);
+        const float beta = __double2float_ru(sqrt(b2 * LR_PAD) * LR_PAD), xn = __double2float_ru(sqrt(x2 * LR_PAD) * LR_PAD);
+        *reinterpret_cast<float4 *>(out + r * LR_SLOT + LR_K) = make_float4(t, rho, beta, xn);
+    }
+}
+
+// rows per block of lowrank_rows_kernel for rows of `stride` floats (0: the staging does not fit in shared memory)
+int lowrank_warps(int stride)
+{
+    const long long per = 16ll * stride;
+    return per > 200 * 1024 ? 0 : (int)std::min(4ll, (200 * 1024) / per);
+}
+
+cudaError_t launch_lowrank_rows(const float *rows_dev, long long n, int stride, const float *B_dev, uint8_t *out_dev, cudaStream_t s)
+{
+    const int w = lowrank_warps(stride);
+    if (w == 0 || n <= 0) return cudaSuccess;
+    const size_t smem = (size_t)w * 16 * stride;
+    cudaError_t e = cudaFuncSetAttribute(lowrank_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    lowrank_rows_kernel<<<(unsigned)((n + w - 1) / w), 32 * w, smem, s>>>(rows_dev, n, stride, B_dev, out_dev);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(128) lowrank_bound_pairs_kernel(DataDesc d, const float *__restrict__ queries, const uint8_t *__restrict__ records, float *__restrict__ out)
+{
+    extern __shared__ __align__(16) float pair_blob[];
+    __shared__ float red[36], lr[LR_QUERY];
+    const long long i = blockIdx.x;
+    prepare_blob<128>(d, JV_METRIC_DOT, queries + i * d.stride, pair_blob, red);
+    prepare_lowrank<128>(d.lr_basis, d.stride, pair_blob, lr);
+    if (threadIdx.x == 0) {
+        const uint4 *e = reinterpret_cast<const uint4 *>(records + i * LR_SLOT);
+        out[i] = lowrank_bound(d, pair_blob, lr, e[0], e[1], *reinterpret_cast<const float4 *>(e + 2));
+    }
+}
+
+cudaError_t launch_lowrank_bound_pairs(const float *B_dev, int dim, int stride, const float *queries_dev, const uint8_t *records_dev, long long n, float *out_dev, cudaStream_t s)
+{
+    if (n <= 0) return cudaSuccess;
+    DataDesc d;
+    memset(&d, 0, sizeof(d));
+    d.kind = KIND_F32;
+    d.dim = dim;
+    d.stride = stride;
+    d.n = n;
+    d.lr_basis = B_dev;
+    lowrank_bound_pairs_kernel<<<(unsigned)n, 128, (size_t)(stride + 4) * 4, s>>>(d, queries_dev, records_dev, out_dev);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+// a graph's edge records: slot t of node v = the low-rank row of adj0[v][t] (zeros for an empty slot), 16 bytes per thread
+__global__ void __launch_bounds__(256) edge_records_kernel(const int32_t *__restrict__ adj0, long long slots, const uint4 *__restrict__ lr_rows, uint4 *__restrict__ rec)
+{
+    constexpr int P = LR_SLOT / 16;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= slots * P) return;
+    const int32_t f = __ldg(adj0 + i / P);
+    rec[i] = f >= 0 ? __ldg(lr_rows + (size_t)f * P + i % P) : make_uint4(0, 0, 0, 0);
+}
+
+cudaError_t launch_edge_records(const int32_t *adj0_dev, long long n, int degree, const uint8_t *lr_rows_dev, uint8_t *rec_dev, cudaStream_t s)
+{
+    const long long items = n * degree * (LR_SLOT / 16);
+    if (items <= 0) return cudaSuccess;
+    edge_records_kernel<<<(unsigned)((items + 255) / 256), 256, 0, s>>>(adj0_dev, n * degree, reinterpret_cast<const uint4 *>(lr_rows_dev), reinterpret_cast<uint4 *>(rec_dev));
+    g_launches++;
+    return cudaGetLastError();
+}
+
 // ProductQuantization.encode (ProductQuantization.java:507-520): code[m] = argmin_c ||v[off_m..] - centroid_{m,c}||^2, first
 // minimum wins. One warp per (row, subspace); lanes stride over the k centroids, then an arg-min shuffle that prefers
 // the smaller index on ties.

@@ -28,6 +28,9 @@ struct DataDesc {
     const int8_t *sketch;
     const float2 *sketch_meta;
     int sketch_stride;
+    // the basis of the low-rank edge bound (lowrank_bound), [LR_K][stride] fp32, zero padded: set with the sketch when the data set
+    // has low-rank rows (api.cu ensure_lowrank); nullptr elsewhere
+    const float *lr_basis;
     // pq: codes [n][code_stride] u8 (code_stride = M rounded up to 4), codebooks concatenated, codebook m at k*sub_offsets[m]
     const uint8_t *codes;
     int M, k, code_stride;
@@ -344,6 +347,102 @@ __device__ __forceinline__ void sketch_bound_pair(const DataDesc &d, const float
     const float ub = __fadd_ru(__fmaf_ru(qn, mb.y, __fmul_ru(sb, mb.x)), __fmaf_ru(kd, mb.x, kd));
     outA = score_map(JV_METRIC_DOT, ua);
     outB = score_map(JV_METRIC_DOT, ub);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Low-rank edge bound (DESIGN §4.1). B = lr_basis, any fp32 LR_K x d matrix taken as exact reals. A row x is stored as LR_K int8
+// codes c and {t, rho, beta, xn} (lowrank_rows_kernel, 48 B: one slot of a graph's edge record): a = B^T x, t = max|a_j| / 127,
+// c = round(a / t), w = x - t B c, rho >= ||w||, beta >= ||B^T w||, xn >= ||x||. A query keeps u = fl(B^T q), e_j >= gk |u_j| + eps_j
+// with eps_j >= |(B^T q)_j - u_j|, sigma >= ||q - B u|| and nu >= ||u|| (prepare_lowrank). Exactly
+//   q . x = t (u . c) + t (B^T q - u) . c + (q - B u) . w + u . (B^T w)
+//        <= t fl(u . c) + t (sum_j |c_j| e_j + kdk) + sigma rho + nu beta,
+// gk = (LR_K + 8) 2^-23 and kdk = (LR_K + 512) 2^-149 bounding the rounding and underflow of fl(u . c); the warp-order exact score
+// adds at most gamma ||q|| ||x|| + kd (sketch_bound_pair).
+// ------------------------------------------------------------------------------------------------
+constexpr int LR_K = 32;      // basis columns
+constexpr int LR_SLOT = 48;   // bytes per row: LR_K codes + {t, rho, beta, xn}
+constexpr int LR_QUERY = 2 * LR_K + 2;  // floats per prepared query: u, e, sigma, nu
+
+// float64 sums of up to n products: the absolute error is at most (n + 8) 2^-53 of the sum of the absolute terms. LR_PAD covers the
+// float64 rounding of a sum of squares of non-negative terms (depth < 2^16) and of a square root
+__host__ __device__ inline double lr_g64(int n) { return (double)(n + 8) * 0x1p-53; }
+constexpr double LR_PAD = 1.0 + 0x1p-36;
+
+// whole CTA of NT threads, after prepare_blob: q = blob (the fp32 query, zero padded to stride), basis = DataDesc::lr_basis ->
+// lr[LR_QUERY] in shared memory. Once per query: kept out of line so that its float64 registers do not weigh on the walk's.
+template <int NT>
+__device__ __noinline__ void prepare_lowrank(const float *basis, int stride, const float *q, float *lr)
+{
+    __shared__ double redd[2 * (NT / 32)];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float g = __fmul_rn((float)(stride + 8), 0x1p-23f), kd = __fmul_rn((float)(stride + 512), 0x1p-149f);
+    const float gk = (float)(LR_K + 8) * 0x1p-23f;
+    for (int j = warp; j < LR_K; j += NT / 32) {
+        const float *b = basis + (size_t)j * stride;
+        float s = 0.f, a = 0.f;  // fl(B_j . q) in any order (depth < stride + 8); sum |B_ij q_i| rounded upward
+        for (int i = lane; i < stride; i += 32) {
+            const float bv = __ldg(b + i), qv = q[i];
+            s = fmaf(bv, qv, s);
+            a = __fmaf_ru(fabsf(bv), fabsf(qv), a);
+        }
+        s = group_sum<32>(s);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a = __fadd_ru(a, __shfl_xor_sync(FULL, a, o));
+        if (lane == 0) {
+            lr[j] = s;
+            lr[LR_K + j] = __fmaf_ru(gk, fabsf(s), __fmaf_ru(g, a, kd));
+        }
+    }
+    __syncthreads();
+    // sigma: r_i = q_i - sum_j B_ij u_j in float64, within lr_g64(LR_K + 2) of A_i = |q_i| + sum_j |B_ij u_j|
+    double r2 = 0.0, a2 = 0.0;
+    for (int i = tid; i < stride; i += NT) {
+        double r = (double)q[i], a = fabs(r);
+        for (int j = 0; j < LR_K; j++) {
+            const double bu = (double)__ldg(basis + (size_t)j * stride + i) * (double)lr[j];
+            r -= bu;
+            a += fabs(bu);
+        }
+        r2 = fma(r, r, r2);
+        a2 = fma(a, a, a2);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        r2 += __shfl_xor_sync(FULL, r2, o);
+        a2 += __shfl_xor_sync(FULL, a2, o);
+    }
+    if (lane == 0) { redd[warp] = r2; redd[NT / 32 + warp] = a2; }
+    __syncthreads();
+    if (tid == 0) {
+        double R = 0.0, A = 0.0, U = 0.0;
+        for (int w = 0; w < NT / 32; w++) { R += redd[w]; A += redd[NT / 32 + w]; }
+        for (int j = 0; j < LR_K; j++) U = fma((double)lr[j], (double)lr[j], U);
+        lr[2 * LR_K] = __double2float_ru((sqrt(R * LR_PAD) + lr_g64(LR_K + 2) * sqrt(A * LR_PAD)) * LR_PAD);
+        lr[2 * LR_K + 1] = __double2float_ru(sqrt(U * LR_PAD) * LR_PAD);
+    }
+    __syncthreads();
+}
+
+// the bound of one row from its 48-byte slot (codes in c0, c1; {t, rho, beta, xn} in m), as a DOT_PRODUCT score (score_map is
+// monotone, so it stays >= score_f32's). Returns +inf when the bound is not finite.
+__device__ __forceinline__ float lowrank_bound(const DataDesc &d, const float *blob, const float *lr, uint4 c0, uint4 c1, float4 m)
+{
+    const unsigned w[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+    float s = 0.f, e = 0.f;
+#pragma unroll
+    for (int j = 0; j < LR_K; j++) {
+        const float c = (float)(int8_t)(w[j >> 2] >> (8 * (j & 3)));
+        s = fmaf(lr[j], c, s);
+        e = __fmaf_ru(fabsf(c), lr[LR_K + j], e);
+    }
+    const float kdk = (float)(LR_K + 512) * 0x1p-149f;
+    const float kd = __fmul_rn((float)(d.stride + 512), 0x1p-149f), g = __fmul_rn((float)(d.stride + 8), 0x1p-23f);
+    float rest = __fmaf_ru(m.x, __fadd_ru(e, kdk), kd);
+    rest = __fmaf_ru(lr[2 * LR_K], m.y, rest);
+    rest = __fmaf_ru(lr[2 * LR_K + 1], m.z, rest);
+    rest = __fmaf_ru(__fmul_ru(g, blob[d.stride + 1]), m.w, rest);
+    const float raw = __fadd_ru(__fmul_ru(m.x, s), rest);
+    return raw <= 3.4028235e38f ? score_map(JV_METRIC_DOT, raw) : __int_as_float(0x7f800000);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -226,7 +226,8 @@ constexpr uint8_t F_ACCEPTED = 2;  // acceptOrds.get(node) && score >= threshold
 // nothing else limits residency) and 4 (64 registers; the modes whose shared-memory LUT part allows at most 4-5 CTAs anyway).
 // VSM: the visited set lives in shared memory (a template parameter, not a run-time flag: the two forms must not cost each other
 // registers — the fp32 walk lost 15 % when they shared one instantiation).
-template <int KIND, int METRIC, int MINB, bool VSM>
+// EDGE: the fp32 DOT walk over a graph with edge records (P.g.edge_rec, launch_search), a separate instantiation for the same reason
+template <int KIND, int METRIC, int MINB, bool VSM, bool EDGE = false>
 __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search_kernel(SearchParams P)
 {
     constexpr int SEARCH_THREADS = SearchThreads<KIND>::value;
@@ -257,6 +258,9 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
     __shared__ long long s_nk;  // key of the second unexpanded entry behind the one being expanded (see JV_EMIT)
     __shared__ float red[36];
     __shared__ int s_q, s_n, s_m, s_hsize, s_cnt;
+    __shared__ int s_settled;  // new neighbours of this hop settled on their edge record (counted as visited, never candidates)
+    __shared__ unsigned long long s_settled_total;  // over this CTA's queries (thread 0 only), added to counters->settled at exit
+    __shared__ float s_lr[LR_QUERY];  // the query's low-rank terms (prepare_lowrank)
     __shared__ int s_drop[2];  // best sortable score that fell off the list, double-buffered like s_posv
     __shared__ int s_posv[2];
 
@@ -267,6 +271,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
     const int vis_limit = 3 << (P.vis_slots_log > 2 ? P.vis_slots_log - 2 : 0);  // shared-memory table: at most 3/4 full
     int32_t *table = P.visited_tables + (size_t)blockIdx.x * P.visited_cap;
     const int degree = P.g.degree;
+    if (EDGE && tid == 0) s_settled_total = 0;
 
     for (;;) {
         if (tid == 0) {
@@ -285,7 +290,10 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         }
         __syncthreads();
         const int wq = s_q;
-        if (wq >= P.nq) break;
+        if (wq >= P.nq) {
+            if (EDGE && tid == 0 && s_settled_total) atomicAdd(&P.counters->settled, s_settled_total);
+            break;
+        }
         const int qi = P.query_index ? P.query_index[wq] : wq;
         const float *q = P.queries + (size_t)qi * P.query_stride;
         const uint32_t *acc = P.accept_bits ? P.accept_bits + (size_t)qi * P.accept_stride : nullptr;
@@ -295,6 +303,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         JV_T(t_q0);
         prepare_blob<SEARCH_THREADS>(P.approx, P.metric, q, blobA, red, blobH, splitm);
         if (P.has_rerank) prepare_blob<SEARCH_THREADS>(P.rerank, P.metric, q, blobR, red);
+        if (EDGE) prepare_lowrank<SEARCH_THREADS>(P.approx.lr_basis, P.approx.stride, blobA, s_lr);
         if (vsm) {
             int4 *t4 = reinterpret_cast<int4 *>(vis);
             const int4 z = make_int4(0, 0, 0, 0);
@@ -336,6 +345,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
             int sel = 0;
             // (the list is empty when every node an upper level expanded was refused: no entry point, nothing to walk)
             if (tid == 0) { s_posv[0] = size > 0 ? 0 : INT_MAX; s_posv[1] = INT_MAX; s_n = 0; s_m = 0; s_hsize = 0; s_drop[0] = INT_MIN; s_drop[1] = INT_MIN; s_cnt = 0; }
+            if (EDGE && tid == 0) s_settled = 0;
             __syncthreads();
             for (;;) {
                 const int p = s_posv[sel];  // first unexpanded entry = the top of the candidate queue
@@ -384,11 +394,26 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                         if (o < P.g.fused_rec) prefetch_l2(rec + o);
                     }
                 }
+                // sketched DOT walk over a graph with edge records (the condition of `sketched` below): a new neighbour whose low-rank
+                // bound (lowrank_bound), read from slot t of the expanded node's record together with its id, falls under the list's
+                // last key would be dropped by the scoring phase whatever its exact score. It is settled here: its bound goes into
+                // s_drop (>= the exact score, like the sketch bound), it is counted as visited and takes no candidate slot.
+                const bool edge_tier = EDGE && lvl == 0 && size == LC;
                 // processNeighbors: score a neighbour only if visited.add() says it is new (OnHeapGraphIndex.java:478)
                 if (nb)
                     for (int t = tid; t < degree; t += SEARCH_THREADS) {
                         const int32_t f = __ldg(nb + t);
                         if (f >= 0 && (vsm ? visited_insert_smem(vis, P.vis_idmask, P.vis_rlog, f, &s_vfail) : visited_insert(table, vmask, P.visited_shift, f))) {
+                            if (edge_tier) {
+                                // (the record was requested towards L2 with the adjacency row, by the speculation below one or more hops ago)
+                                const uint4 *e = reinterpret_cast<const uint4 *>(P.g.edge_rec + ((size_t)node * degree + t) * LR_SLOT);
+                                const float ub = lowrank_bound(P.approx, blobA, s_lr, __ldg(e), __ldg(e + 1), __ldg(reinterpret_cast<const float4 *>(e + 2)));
+                                if (topk_key(ub, f) < cur[LC - 1]) {
+                                    atomicAdd(&s_settled, 1);
+                                    atomicMax(&s_drop[sel], float_to_sortable(ub));
+                                    continue;
+                                }
+                            }
                             const int slot = atomicAdd(&s_n, 1);
                             cand_ids[slot] = f;
                             if (KIND == KIND_PQ) cand_slot[slot] = (uint8_t)t;
@@ -419,7 +444,11 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     // pops are most likely the unexpanded entries right behind p, and their rows then come from L2 instead of DRAM
                     if (tid >= 32 && tid < 36) {
                         const int pp = p + (tid - 31);
-                        if (pp < size && !(fcur[pp] & F_EXPANDED)) prefetch_l2(P.g.adj0 + (size_t)key_node(cur[pp]) * degree);
+                        if (pp < size && !(fcur[pp] & F_EXPANDED)) {
+                            prefetch_l2(P.g.adj0 + (size_t)key_node(cur[pp]) * degree);
+                            // and their edge records (degree x 48 B), so that a hop's record reads wait on L2 like its adjacency row
+                            if (edge_tier) bulk_prefetch_l2(P.g.edge_rec + (size_t)key_node(cur[pp]) * degree * LR_SLOT, (unsigned)(degree * LR_SLOT));
+                        }
                     }
                 }
                 if (lvl == 0 && P.early_pf && tid == 36) {
@@ -476,6 +505,12 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 if (tid == 0) { s_drop[sel ^ 1] = INT_MIN; s_cnt = 0; }
                 const int n = s_n;
                 table_cnt += n;
+                if (EDGE) {
+                    const int ns = s_settled;
+                    table_cnt += ns;
+                    visited += ns;
+                    if (tid == 0) s_settled_total += (unsigned)ns;
+                }
                 if (vsm ? (table_cnt > vis_limit || s_vfail) : (table_cnt * 2 > P.visited_cap)) {
                     if (P.lenient) truncated = true;
                     else failed = 1;
@@ -626,13 +661,18 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                             if (c < 2 && lvl == 0) {
                                 if (KIND == KIND_PQ && P.g.fused) prefetch_l2(P.g.fused + (size_t)key_node(k) * P.g.fused_rec);
                                 else prefetch_l2(P.g.adj0 + (size_t)key_node(k) * degree);
+                                if (EDGE && size == LC)
+                                    bulk_prefetch_l2(P.g.edge_rec + (size_t)key_node(k) * degree * LR_SLOT, (unsigned)(degree * LR_SLOT));
                             }
                         } else mydrop = max(mydrop, float_to_sortable(key_score(k)));
                     }
                 }
                 if (mypos != INT_MAX) atomicMin(&s_posv[sel ^ 1], mypos);
                 if (mydrop != INT_MIN) atomicMax(&s_drop[sel], mydrop);
-                if (tid == 0) s_n = 0;
+                if (tid == 0) {
+                    s_n = 0;
+                    if (EDGE) s_settled = 0;
+                }
                 __syncthreads();
                 JV_T(t_i3);
                 JV_ACC(3, t_i2, t_i3);
@@ -1111,6 +1151,7 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
 #ifdef JV_ROW_BOUND_STATS
     P.approx.sketch = nullptr;  // the drop statistics describe the walk that reads every row
 #endif
+    if (!P.approx.sketch || !P.approx.lr_basis || approx.kind != KIND_F32 || metric != JV_METRIC_DOT) P.g.edge_rec = nullptr;
     P.pq_rows = plan.pq_rows;
     {
         // on for the latency-bound walks (PQ / BQ: c3 12.0 -> 11.5 ms); off where HBM is already saturated and a wasted adjacency
@@ -1139,7 +1180,19 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
         e = cudaFuncSetAttribute(graph_search_kernel<K, M, B, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
         if (e == cudaSuccess) graph_search_kernel<K, M, B, V><<<plan.ctas, SearchThreads<K>::value, plan.smem_bytes, s>>>(P);               \
     } while (0)
-    JV_SEARCH_DISPATCH(approx.kind, metric, plan.pq_wide != 0, plan.vis_slots_log != 0, CALL);
+#define CALL_EDGE(B, V)                                                                                                                \
+    do {                                                                                                                              \
+        e = cudaFuncSetAttribute(graph_search_kernel<KIND_F32, JV_METRIC_DOT, B, V, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
+        if (e == cudaSuccess) graph_search_kernel<KIND_F32, JV_METRIC_DOT, B, V, true><<<plan.ctas, SearchThreads<KIND_F32>::value, plan.smem_bytes, s>>>(P); \
+    } while (0)
+    if (P.g.edge_rec) {
+        if (plan.vis_slots_log != 0) {
+            if (plan.pq_wide) CALL_EDGE(MINB_ROWS_WIDE, true);
+            else CALL_EDGE(MINB_ROWS, true);
+        } else if (plan.pq_wide) CALL_EDGE(MINB_ROWS_WIDE, false);
+        else CALL_EDGE(MINB_ROWS, false);
+    } else JV_SEARCH_DISPATCH(approx.kind, metric, plan.pq_wide != 0, plan.vis_slots_log != 0, CALL);
+#undef CALL_EDGE
 #undef CALL
     if (e != cudaSuccess) return e;
     g_launches++;

@@ -14,6 +14,13 @@ and b12, the share caught by the coarse or the int8 bound, and predicts (ss = sk
 
     (ss / 2 + 16) + 8 + (1 - f b1) ss / 2 + (1 - f b12) 4 d    against the one-tier ss + 8 + 8 + (1 - f b) 4 d.
 
+For the low-rank edge bound (tests/row_bound_lowrank.py, a basis fitted on --basis-rows sampled rows) at each k of --ranks it reports
+b1, the share of the drops that bound catches before the sketch is read, and predicts
+
+    rec + (1 - f b1) (ss + 16) + (1 - f b) 4 d,   rec = degree (k + 16) / (new rows per hop),
+
+where rec counts the whole edge record of every expanded node (its k + 16 B slots stored with the adjacency row).
+
     python tools/row_bound_stats.py [--out row_bound_stats.json]"""
 import argparse
 import json
@@ -31,6 +38,8 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--n", type=int, default=1_000_000)
 ap.add_argument("--nq", type=int, default=10_000)
 ap.add_argument("--max-samples", type=int, default=100_000)
+ap.add_argument("--ranks", default="16,32,64")
+ap.add_argument("--basis-rows", type=int, default=4096)
 ap.add_argument("--out", default="")
 a = ap.parse_args()
 
@@ -41,6 +50,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import bench  # noqa: E402
 import row_bound_coarse as rbc  # noqa: E402
+import row_bound_lowrank as rl  # noqa: E402
 import row_bound_model as rb  # noqa: E402
 
 args = argparse.Namespace(impl="b200", n=a.n, dim=768, nq=a.nq, dist="latent", topk=10, gt_queries=500)
@@ -100,6 +110,23 @@ today = ss + 8 + 8 + (1.0 - f * b) * 4 * stride
 two = (ss / 2 + 16) + 8 + (1.0 - f * b1) * ss / 2 + (1.0 - f * b12) * 4 * stride
 out["int8_two_tier"] = {"b1": b1, "b12": b12, "b": b, "bytes_per_row_today": today, "predicted_bytes_per_row": two, "vs_today": two / today,
                         "median_coarse_radius_over_norm": float(np.median(rad1 / np.maximum(np.linalg.norm(rows, axis=1), 1e-30)))}
+# the low-rank edge bound: settled at gather time from the expanded node's record; the others read the sketch as today
+deg = w.gi.info()["degree"]
+new_per_hop = r.visitedCount / max(r.expandedCountBaseLayer, 1)
+xs = w.base_dev[torch.from_numpy(rl.sample_rows(a.n, a.basis_rows)).cuda()].cpu().numpy()
+out["lowrank"] = {"degree": deg, "visited_per_expanded_base": new_per_hop, "bytes_per_row_today": today, "ranks": {}}
+for k in (int(v) for v in a.ranks.split(",")):
+    B = rl.basis(xs, k)
+    codes, t, rho, beta, xn = rl.encode_rows(rows, B)
+    ubl = rl.upper_bound_raw(qs, B, codes, t, rho, beta, xn, stride)
+    caughtl = rb.topk_key(rb.dot_score_up(ubl), smp["row"]) < smp["last_key"]
+    b1l = float(caughtl.mean())
+    rec = deg * (k + 16) / new_per_hop
+    pred = rec + (1.0 - f * b1l) * (ss + 16) + (1.0 - f * b) * 4 * stride
+    _, _, sig, _ = rl.prepare_query(qs[:2000], B)
+    out["lowrank"]["ranks"][str(k)] = {"b1": b1l, "b1_not_caught_by_int8": float((caughtl & ~caught).mean()), "record_bytes_per_new_row": rec,
+                                       "predicted_bytes_per_row": pred, "vs_today": pred / today, "median_rho": float(np.median(rho)),
+                                       "median_sigma": float(np.median(sig)), "median_beta": float(np.median(beta))}
 print(json.dumps(out, indent=1))
 if a.out:
     os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
