@@ -173,7 +173,7 @@ cudaError_t upload_padded(void *dev, const void *host, size_t n, size_t row_byte
 }  // namespace
 
 struct jv_dataset_s {
-    int device = 0;
+    int device = t_active;
     bool borrowed_rows = false;  // jv_dataset_adopt_f32_device: rows belong to the caller
     DataDesc d;
     std::vector<DeviceBuffer> allocs;
@@ -188,12 +188,30 @@ struct jv_dataset_s {
     uint64_t lr_id = 0;
     bool lr_off = false;
     std::mutex sketch_mu;
+    // an empty data set of n rows of `kind` on the active device: every other field of `d` is zero
+    jv_dataset_s(int kind, long long n, int dim)
+    {
+        memset(&d, 0, sizeof(DataDesc));
+        d.kind = kind;
+        d.dim = dim;
+        d.n = n;
+    }
     template <typename T>
     int alloc(T **p, size_t n)
     {
         CK(alloc_owned(allocs, *p, n ? n : 16), "cudaMalloc(dataset)");
         bytes += n;
         return JV_OK;
+    }
+    // the fp32 row layout (DataDesc::rows): every row zero padded to a multiple of 4 floats
+    static int f32_stride(int dim) { return round4(dim); }
+    // fp32 rows [n][f32_stride(dim)], d.rows pointing at them, for the caller to fill (padding included)
+    int alloc_rows(float **rows)
+    {
+        d.stride = f32_stride(d.dim);
+        const int rc = alloc(rows, (size_t)d.n * d.stride * sizeof(float));
+        d.rows = *rows;
+        return rc;
     }
 };
 
@@ -204,13 +222,16 @@ struct jv_query_s {
     DeviceBuffer blob;
 };
 
+// the upper levels of a graph, level l >= 1 at [l - 1]: its members (node ids), or their rows ([members][degree] node ids, -1 = empty)
+using Levels = std::vector<std::vector<int32_t>>;
+
+// Only create, set_levels and jv_graph_fuse_pq write `g`.
 struct jv_graph_s {
-    int device = 0;
+    int device = t_active;
     GraphDesc g;
     DeviceBuffer fused;  // FusedPQ records
     DeviceBuffer adj0, upper_row, upper_adj, upper_off;
-    std::vector<std::vector<int32_t>> level_ids;  // host copies, level >= 1
-    std::vector<std::vector<int32_t>> level_adj;
+    Levels level_ids, level_adj;  // host copies of the upper levels
     std::vector<uint32_t> removed;  // ids taken out by jv_graph_remove_deleted (holes), bit (id & 31) of word (id >> 5); empty = none
     // edge records of the low-rank bound (launch_edge_records) for the data set whose lr_id is edge_rec_of; built by the first
     // sketched search over that data set, freed with the graph
@@ -219,6 +240,19 @@ struct jv_graph_s {
     std::shared_ptr<DeviceBuffer> edge_rec;
     uint64_t edge_rec_of = 0;
     std::mutex edge_mu;
+    // a graph of n nodes with `degree` neighbour slots each on the active device, into `out`: adj0 allocated for the caller to
+    // fill, level 0 only and no entry until set_levels
+    static int create(int32_t n, int degree, std::unique_ptr<jv_graph_s> &out)
+    {
+        std::unique_ptr<jv_graph_s> h(new jv_graph_s());
+        memset(&h->g, 0, sizeof(GraphDesc));
+        h->g.n = n; h->g.degree = degree; h->g.levels = 1; h->g.entry_level = 0; h->g.entry_node = -1;
+        CK(h->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+        h->g.adj0 = h->adj0.get<int32_t>();
+        out = std::move(h);
+        return JV_OK;
+    }
+    int set_levels(Levels ids, Levels adj, int32_t entry);
 };
 
 struct jv_multi_s {
@@ -346,18 +380,11 @@ int jv_dataset_register_f32(const float *rows, int64_t n, int dim, jv_dataset *o
 {
     NEED_INIT();
     if (!rows || !out || n <= 0 || dim <= 0 || n > 0x7fffffffLL) return fail(JV_ERR_INVALID, "register_f32: bad arguments");
-    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s());
-    ds->device = t_active;
-    memset(&ds->d, 0, sizeof(DataDesc));
-    ds->d.kind = KIND_F32;
-    ds->d.dim = dim;
-    ds->d.n = n;
-    ds->d.stride = round4(dim);
+    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s(KIND_F32, n, dim));
     float *dev = nullptr;
-    int rc = ds->alloc(&dev, (size_t)n * ds->d.stride * sizeof(float));
+    int rc = ds->alloc_rows(&dev);
     if (rc) return rc;
     CK(upload_padded(dev, rows, (size_t)n, (size_t)dim * 4, (size_t)ds->d.stride * 4), "upload rows");
-    ds->d.rows = dev;
     *out = ds.release();
     return JV_OK;
 }
@@ -367,11 +394,9 @@ int jv_dataset_register_pq(const uint8_t *codes, int64_t n, int dim, int M, int 
     NEED_INIT();
     if (!codes || !codebooks || !out || n <= 0 || dim <= 0 || M <= 0 || M > dim || k <= 0 || k > 256 || n > 0x7fffffffLL)
         return fail(JV_ERR_INVALID, "register_pq: bad arguments");
-    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s());
-    ds->device = t_active;
-    memset(&ds->d, 0, sizeof(DataDesc));
+    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s(KIND_PQ, n, dim));
     DataDesc &d = ds->d;
-    d.kind = KIND_PQ; d.dim = dim; d.n = n; d.M = M; d.k = k; d.code_stride = round4(M);
+    d.M = M; d.k = k; d.code_stride = round4(M);
     uint8_t *dcodes = nullptr;
     float *dcb = nullptr, *dcen = nullptr, *dmag = nullptr;
     int *dlay = nullptr;
@@ -396,10 +421,8 @@ int jv_dataset_register_bq(const uint64_t *words, int64_t n, int dim, jv_dataset
 {
     NEED_INIT();
     if (!words || !out || n <= 0 || dim <= 0 || n > 0x7fffffffLL) return fail(JV_ERR_INVALID, "register_bq: bad arguments");
-    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s());
-    ds->device = t_active;
-    memset(&ds->d, 0, sizeof(DataDesc));
-    ds->d.kind = KIND_BQ; ds->d.dim = dim; ds->d.n = n; ds->d.W = (dim + 63) / 64;
+    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s(KIND_BQ, n, dim));
+    ds->d.W = (dim + 63) / 64;
     unsigned long long *dw = nullptr;
     int rc = ds->alloc(&dw, (size_t)n * ds->d.W * 8);
     if (rc) return rc;
@@ -414,11 +437,9 @@ int jv_dataset_register_bq(const uint64_t *words, int64_t n, int dim, jv_dataset
 static int nvq_dataset(int64_t n, int dim, int nsub, const float *mean, cudaStream_t s, std::unique_ptr<jv_dataset_s> &ds, uint8_t **bytes_dev,
                        float **params_dev)
 {
-    ds.reset(new jv_dataset_s());
-    ds->device = t_active;
-    memset(&ds->d, 0, sizeof(DataDesc));
+    ds.reset(new jv_dataset_s(KIND_NVQ, n, dim));
     DataDesc &d = ds->d;
-    d.kind = KIND_NVQ; d.dim = dim; d.n = n; d.nsub = nsub; d.stride = round4(dim); d.byte_stride = round4(dim);
+    d.nsub = nsub; d.stride = round4(dim); d.byte_stride = round4(dim);
     float *dm = nullptr;
     int *dlay = nullptr;
     int rc;
@@ -504,14 +525,9 @@ int jv_dataset_adopt_f32_device(const float *rows_device, int64_t n, int dim, in
     NEED_INIT();
     if (!rows_device || !out || n <= 0 || dim <= 0 || n > 0x7fffffffLL || row_stride < dim || (row_stride & 3) || ((uintptr_t)rows_device & 15))
         return fail(JV_ERR_INVALID, "adopt_f32_device: need 16-byte aligned rows and a row stride that is a multiple of 4 floats >= dim");
-    if (row_stride != round4(dim)) return fail(JV_ERR_INVALID, "adopt_f32_device: row_stride must equal dim rounded up to 4 (padding floats must be zero)");
-    jv_dataset ds = new jv_dataset_s();
-    ds->device = t_active;
+    if (row_stride != jv_dataset_s::f32_stride(dim)) return fail(JV_ERR_INVALID, "adopt_f32_device: row_stride must equal dim rounded up to 4 (padding floats must be zero)");
+    jv_dataset ds = new jv_dataset_s(KIND_F32, n, dim);
     ds->borrowed_rows = true;
-    memset(&ds->d, 0, sizeof(DataDesc));
-    ds->d.kind = KIND_F32;
-    ds->d.dim = dim;
-    ds->d.n = n;
     ds->d.stride = row_stride;
     ds->d.rows = rows_device;
     *out = ds;
@@ -1089,43 +1105,44 @@ int jv_graph_create(int32_t n, int degree, const int32_t *adj0, int32_t entry_no
     // one pass over data that is copied anyway: a neighbour id outside [-1, n) would be an illegal address inside the search kernel
     for (size_t i = 0, tot = (size_t)n * degree; i < tot; i++)
         if (adj0[i] < -1 || adj0[i] >= n) return fail(JV_ERR_INVALID, "graph_create: neighbour id out of range");
-    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
-    g->device = t_active;
-    memset(&g->g, 0, sizeof(GraphDesc));
-    cudaError_t e = g->adj0.alloc((size_t)n * degree * 4);
-    if (e == cudaSuccess) e = cudaMemcpy(g->adj0.get(), adj0, (size_t)n * degree * 4, cudaMemcpyHostToDevice);
-    CK(e, "upload adjacency");
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = entry_node; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
+    std::unique_ptr<jv_graph_s> g;
+    int rc = jv_graph_s::create(n, degree, g);
+    if (rc) return rc;
+    CK(cudaMemcpy(g->adj0.get(), adj0, (size_t)n * degree * 4, cudaMemcpyHostToDevice), "upload adjacency");
+    if ((rc = g->set_levels({}, {}, entry_node))) return rc;
     *out = g.release();
     return JV_OK;
 }
 
-static int graph_rebuild_upper(jv_graph g)
+// the whole hierarchy: the upper levels (none: level 0 only) on the host and on the device, and the entry node, which belongs to the
+// top level. The device copies are made before anything is replaced, so a failure leaves the graph as it was.
+int jv_graph_s::set_levels(Levels ids, Levels adj, int32_t entry)
 {
-    const int L = (int)g->level_ids.size();
-    g->upper_row.reset(); g->upper_adj.reset(); g->upper_off.reset();
-    if (L == 0) return JV_OK;
-    const int n = g->g.n, degree = g->g.degree;
-    std::vector<int32_t> rows((size_t)L * n, -1);
-    std::vector<long long> offs(L);
-    std::vector<int32_t> adj;
-    long long o = 0;
-    for (int l = 0; l < L; l++) {
-        offs[l] = o;
-        for (size_t i = 0; i < g->level_ids[l].size(); i++) rows[(size_t)l * n + g->level_ids[l][i]] = (int32_t)i;
-        adj.insert(adj.end(), g->level_adj[l].begin(), g->level_adj[l].end());
-        o += (long long)g->level_ids[l].size();
+    const int L = (int)ids.size(), n = g.n;
+    DeviceBuffer row, cat, off;  // upper_row, upper_adj, upper_off to be
+    if (L > 0) {
+        std::vector<int32_t> rows((size_t)L * n, -1), adjs;
+        std::vector<long long> offs(L);
+        long long o = 0;
+        for (int l = 0; l < L; l++) {
+            offs[l] = o;
+            for (size_t i = 0; i < ids[l].size(); i++) rows[(size_t)l * n + ids[l][i]] = (int32_t)i;
+            adjs.insert(adjs.end(), adj[l].begin(), adj[l].end());
+            o += (long long)ids[l].size();
+        }
+        CK(row.alloc(rows.size() * 4), "cudaMalloc(upper_row)");
+        CK(cat.alloc(std::max<size_t>(adjs.size(), 1) * 4), "cudaMalloc(upper_adj)");
+        CK(off.alloc((size_t)L * 8), "cudaMalloc(upper_off)");
+        CK(cudaMemcpy(row.get(), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice), "H2D upper_row");
+        CK(cudaMemcpy(cat.get(), adjs.data(), adjs.size() * 4, cudaMemcpyHostToDevice), "H2D upper_adj");
+        CK(cudaMemcpy(off.get(), offs.data(), (size_t)L * 8, cudaMemcpyHostToDevice), "H2D upper_off");
     }
-    CK(g->upper_row.alloc(rows.size() * 4), "cudaMalloc(upper_row)");
-    CK(g->upper_adj.alloc(std::max<size_t>(adj.size(), 1) * 4), "cudaMalloc(upper_adj)");
-    CK(g->upper_off.alloc((size_t)L * 8), "cudaMalloc(upper_off)");
-    CK(cudaMemcpy(g->upper_row.get(), rows.data(), rows.size() * 4, cudaMemcpyHostToDevice), "H2D upper_row");
-    CK(cudaMemcpy(g->upper_adj.get(), adj.data(), adj.size() * 4, cudaMemcpyHostToDevice), "H2D upper_adj");
-    CK(cudaMemcpy(g->upper_off.get(), offs.data(), (size_t)L * 8, cudaMemcpyHostToDevice), "H2D upper_off");
-    g->g.upper_row = g->upper_row.get<int32_t>(); g->g.upper_adj = g->upper_adj.get<int32_t>(); g->g.upper_off = g->upper_off.get<long long>();
-    g->g.levels = L + 1;
-    g->g.entry_level = L;
-    (void)degree;
+    // the old device copies go with the locals
+    std::swap(upper_row, row); std::swap(upper_adj, cat); std::swap(upper_off, off);
+    level_ids = std::move(ids);
+    level_adj = std::move(adj);
+    g.levels = L + 1; g.entry_level = L; g.entry_node = entry;
+    g.upper_row = upper_row.get<int32_t>(); g.upper_adj = upper_adj.get<int32_t>(); g.upper_off = upper_off.get<long long>();
     return JV_OK;
 }
 
@@ -1141,9 +1158,10 @@ int jv_graph_add_level(jv_graph g, int32_t count, const int32_t *node_ids, const
         if (node_ids[i] == g->g.entry_node) has_entry = true;
     }
     if (!has_entry) return fail(JV_ERR_INVALID, "graph_add_level: the entry node must belong to every level");
-    g->level_ids.emplace_back(node_ids, node_ids + count);
-    g->level_adj.emplace_back(adj, adj + (size_t)count * g->g.degree);
-    return graph_rebuild_upper(g);
+    Levels ids = g->level_ids, rows = g->level_adj;
+    ids.emplace_back(node_ids, node_ids + count);
+    rows.emplace_back(adj, adj + (size_t)count * g->g.degree);
+    return g->set_levels(std::move(ids), std::move(rows), g->g.entry_node);
 }
 
 int jv_graph_fuse_pq(jv_graph g, jv_dataset pq)
@@ -1730,22 +1748,20 @@ static int build_level(jv_dataset ds, int metric, const BuildParams &bp, const s
     return JV_OK;
 }
 
-// every upper level is a Vamana graph over its members, built by the same device builder on the members' rows
-static int build_upper_levels(jv_graph g, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+// the hierarchy of a build: every upper level is a Vamana graph over its members, built by the same device builder on the members'
+// rows. Without one (hierarchy false, or a single node) the build's entry is node 0.
+static int build_upper_levels(jv_graph g, jv_dataset ds, int metric, const BuildParams &bp, bool hierarchy, uint64_t seed, cudaStream_t s)
 {
     const int n = (int)ds->d.n;
-    std::vector<std::vector<int32_t>> members;
+    Levels members, adj;
     int entry = 0;
-    assign_levels(n, bp.degree, seed, members, &entry);
-    g->g.entry_node = entry;
-    for (size_t l = 0; l < members.size(); l++) {
-        std::vector<int32_t> ladj;
-        const int rc = build_level(ds, metric, bp, members[l], nullptr, ladj, s);
+    if (hierarchy && n > 1) assign_levels(n, bp.degree, seed, members, &entry);
+    for (const std::vector<int32_t> &ids : members) {
+        adj.emplace_back();
+        const int rc = build_level(ds, metric, bp, ids, nullptr, adj.back(), s);
         if (rc) return rc;
-        g->level_ids.push_back(members[l]);
-        g->level_adj.push_back(std::move(ladj));
     }
-    return graph_rebuild_upper(g);
+    return g->set_levels(std::move(members), std::move(adj), entry);
 }
 
 // the whole build over an fp32, a PQ or a BQ data set whose arguments have been checked: level 0, then the upper levels
@@ -1754,19 +1770,15 @@ static int graph_build(jv_dataset ds, int metric, const jv_build_params *params,
     int rc;
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
-    const int n = (int)ds->d.n, degree = params->degree;
-    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
-    g->device = ds->device;
-    memset(&g->g, 0, sizeof(GraphDesc));
-    CK(g->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+    std::unique_ptr<jv_graph_s> g;
+    if ((rc = jv_graph_s::create((int32_t)ds->d.n, params->degree, g))) return rc;
     StreamTimer timer;
     CK(timer.start(s), "event");
     BuildStats bs;
     cudaError_t e = build_graph_flat(ds->d, metric, bp, g->adj0.get<int32_t>(), g_sm_count, &bs, s);
     t_build_stats = bs;
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
     rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "build_graph_flat");
-    if (!rc && params->add_hierarchy && n > 1) rc = build_upper_levels(g.get(), ds, metric, bp, params->seed, s);
+    if (!rc) rc = build_upper_levels(g.get(), ds, metric, bp, params->add_hierarchy, params->seed, s);
     cudaError_t e1 = timer.stop(s);  // the upper levels are part of the build and of its time
     cudaStreamSynchronize(s);
     if (rc) return rc;
@@ -1848,7 +1860,7 @@ static inline bool bit_of(const std::vector<uint32_t> &bits, int v) { return (bi
 // seeded with that level's rows. GraphAdd is what the add keeps of g, so that g is no longer read once the builder exists.
 struct GraphAdd {
     int32_t n0 = 0, entry = -1;
-    std::vector<std::vector<int32_t>> level_ids, level_adj;  // g's upper levels
+    Levels level_ids, level_adj;                            // g's upper levels
     std::vector<uint32_t> removed;                          // g's holes (jv_graph_remove_deleted)
     std::vector<uint32_t> marks;                            // deleted_bits over the n0 old nodes; empty = none marked
     DeviceBuffer upper_row;                                 // g's id -> row maps of its upper levels, [levels - 1][n0]
@@ -1903,7 +1915,8 @@ static int add_prepare(jv_graph g, const uint32_t *deleted_bits, int n, GraphAdd
 // the device; the inserts start at the entry's row (the level's first row if the entry is not a member). A level above g's top is
 // built over its members, all new, and its lowest id becomes the entry.
 // Over a PQ data set build_level gathers the members' code rows instead of their fp32 rows; nothing else differs.
-static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
+static int add_upper_levels(const GraphAdd &A, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, Levels &level_ids, Levels &level_adj,
+                            int32_t *entry, cudaStream_t s)
 {
     const int n = (int)ds->d.n, n0 = A.n0, degree = bp.degree, L = (int)A.level_ids.size();
     const std::vector<int> level = draw_levels(n, degree, seed);
@@ -1933,28 +1946,28 @@ static int add_upper_levels(jv_graph_s *ng, const GraphAdd &A, jv_dataset ds, in
             rc = build_level(ds, metric, bp, ids, &sd, ladj, s);
         }
         if (rc) return rc;
-        ng->level_ids.push_back(std::move(ids));
-        ng->level_adj.push_back(std::move(ladj));
+        level_ids.push_back(std::move(ids));
+        level_adj.push_back(std::move(ladj));
     }
-    if (top > L) ng->g.entry_node = ng->level_ids[top - 1][0];
+    if (top > L) *entry = level_ids[top - 1][0];
     return JV_OK;
 }
 
-// the new graph around its level-0 adjacency (already in ng->adj0): size, entry, holes widened to n, upper levels
+// the new graph around its level-0 adjacency (already in ng->adj0, ng sized to the data set): holes widened to n, upper levels, entry
 static int add_finish(jv_graph_s *ng, const GraphAdd &A, jv_dataset ds, int metric, const BuildParams &bp, uint64_t seed, cudaStream_t s)
 {
     const int n = (int)ds->d.n;
-    ng->g.n = n; ng->g.degree = bp.degree; ng->g.levels = 1; ng->g.entry_level = 0; ng->g.adj0 = ng->adj0.get<int32_t>();
-    ng->g.entry_node = A.entry >= 0 ? A.entry : n > A.n0 ? A.n0 : -1;  // an empty graph's first new node is its entry (build.cu)
+    int32_t entry = A.entry >= 0 ? A.entry : n > A.n0 ? A.n0 : -1;  // an empty graph's first new node is its entry (build.cu)
     if (!A.removed.empty()) {
         ng->removed = A.removed;
         ng->removed.resize(((size_t)n + 31) / 32, 0u);
     }
+    Levels ids, adj;
     if (!A.level_ids.empty()) {
-        const int rc = add_upper_levels(ng, A, ds, metric, bp, seed, s);
+        const int rc = add_upper_levels(A, ds, metric, bp, seed, ids, adj, &entry, s);
         if (rc) return rc;
     }
-    return graph_rebuild_upper(ng);
+    return ng->set_levels(std::move(ids), std::move(adj), entry);
 }
 
 // jv_graph_add_nodes (kind = KIND_F32), jv_graph_add_nodes_pq (KIND_PQ) and jv_graph_add_nodes_bq (KIND_BQ): the builder scores
@@ -1970,20 +1983,16 @@ static int graph_add_nodes(jv_graph g, jv_dataset ds, int kind, int metric, cons
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
     const int n0 = g->g.n, n = (int)ds->d.n, degree = g->g.degree;
-    std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
-    ng->device = g->device;
-    memset(&ng->g, 0, sizeof(GraphDesc));
     StreamTimer timer;
     CK(timer.start(s), "event");
-    CK(ng->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+    std::unique_ptr<jv_graph_s> ng;
+    if ((rc = jv_graph_s::create(n, degree, ng))) return rc;
     BuildStats bs = {0, 0, 0, 0, 0};
     if (n == n0) {
         // nothing to insert: a copy of g
         CK(cudaMemcpyAsync(ng->adj0.get(), g->adj0.get(), (size_t)n * degree * 4, cudaMemcpyDeviceToDevice, s), "copy adjacency");
-        ng->g.n = n; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_node = g->g.entry_node; ng->g.entry_level = 0;
-        ng->g.adj0 = ng->adj0.get<int32_t>();
-        ng->level_ids = g->level_ids; ng->level_adj = g->level_adj; ng->removed = g->removed;
-        rc = graph_rebuild_upper(ng.get());
+        ng->removed = g->removed;
+        rc = ng->set_levels(g->level_ids, g->level_adj, g->g.entry_node);
     } else {
         GraphAdd A;
         std::vector<uint32_t> accept;
@@ -2182,18 +2191,14 @@ int jv_builder_finish(jv_builder b, jv_graph *out, double *device_ms)
     if (!out) return fail(JV_ERR_INVALID, "builder_finish: null");
     int rc;
     if ((rc = t_ctx.init())) return rc;
-    const int n = (int)b->data->d.n, degree = b->bp.degree;
-    std::unique_ptr<jv_graph_s> g(new jv_graph_s());
-    g->device = b->device;
-    memset(&g->g, 0, sizeof(GraphDesc));
-    CK(g->adj0.alloc((size_t)n * degree * 4), "cudaMalloc(adjacency)");
+    std::unique_ptr<jv_graph_s> g;
+    if ((rc = jv_graph_s::create((int32_t)b->data->d.n, b->bp.degree, g))) return rc;
     BuildStats bs;
     cudaError_t e = builder_finish(b->B, g->adj0.get<int32_t>(), &bs, b->stream);
     t_build_stats = bs;
     CK(e, "builder_finish");
-    g->g.n = n; g->g.degree = degree; g->g.levels = 1; g->g.entry_node = 0; g->g.entry_level = 0; g->g.adj0 = g->adj0.get<int32_t>();
     if (b->add) rc = add_finish(g.get(), *b->add, b->data, b->metric, b->bp, b->params.seed, b->stream);  // the hierarchy follows the graph
-    else if (b->params.add_hierarchy && n > 1) rc = build_upper_levels(g.get(), b->data, b->metric, b->bp, b->params.seed, b->stream);
+    else rc = build_upper_levels(g.get(), b->data, b->metric, b->bp, b->params.add_hierarchy, b->params.seed, b->stream);
     if (rc) return rc;
     CK(b->timer.stop(b->stream), "event");
     cudaStreamSynchronize(b->stream);
@@ -2302,24 +2307,21 @@ static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric,
         dead[w] |= h;
         gone += __builtin_popcount(dead[w]);
     }
-    std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
-    ng->device = g->device;
-    memset(&ng->g, 0, sizeof(GraphDesc));
-    ng->g.n = n; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_node = -1; ng->g.entry_level = 0;
-    ng->removed = dead;
     DeviceBuffer dead_buf;
     RepairStats st;
     memset(&st, 0, sizeof(st));
     StreamTimer timer;
     CK(timer.start(s), "event");
-    cudaError_t e = ng->adj0.alloc((size_t)n * degree * 4);
-    if (e == cudaSuccess) e = dead_buf.alloc(W * 4);
+    std::unique_ptr<jv_graph_s> ng;
+    if ((rc = jv_graph_s::create(n, degree, ng))) return rc;
+    ng->removed = dead;
+    cudaError_t e = dead_buf.alloc(W * 4);
     if (e == cudaSuccess) e = cudaMemcpyAsync(dead_buf.get(), dead.data(), W * 4, cudaMemcpyHostToDevice, s);
     rc = e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_remove_deleted: allocation");
-    ng->g.adj0 = ng->adj0.get<int32_t>();
     const uint32_t *dead_dev = dead_buf.get<uint32_t>();
     if (!rc) rc = remove_deleted_level(g, ng.get(), ds, metric, alpha, seed, 0, dead, dead_dev, &st, nullptr, s);
     // upper levels: repaired on the device like level 0, then their deleted members are dropped from the host copies
+    Levels level_ids, level_adj;
     for (int level = 1; !rc && level < g->g.levels; level++) {
         std::vector<int32_t> adj;
         rc = remove_deleted_level(g, ng.get(), ds, metric, alpha, seed, level, dead, dead_dev, &st, &adj, s);
@@ -2331,8 +2333,8 @@ static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric,
             nids.push_back(ids[r]);
             nadj.insert(nadj.end(), adj.begin() + r * degree, adj.begin() + (r + 1) * degree);
         }
-        ng->level_ids.push_back(std::move(nids));
-        ng->level_adj.push_back(std::move(nadj));
+        level_ids.push_back(std::move(nids));
+        level_adj.push_back(std::move(nadj));
     }
     if (!rc) {
         // entry (GraphIndexBuilder.java:769-786): kept while it lives; otherwise the lowest live id of the highest level that still has a
@@ -2340,17 +2342,16 @@ static int graph_remove_deleted(jv_graph g, jv_dataset ds, int kind, int metric,
         int entry = g->g.entry_node;
         if (entry < 0 || bit_of(dead, entry)) {
             entry = -1;
-            int top = (int)ng->level_ids.size();
-            while (top > 0 && ng->level_ids[top - 1].empty()) top--;
-            ng->level_ids.resize(top);
-            ng->level_adj.resize(top);
-            if (top > 0) entry = *std::min_element(ng->level_ids[top - 1].begin(), ng->level_ids[top - 1].end());
+            int top = (int)level_ids.size();
+            while (top > 0 && level_ids[top - 1].empty()) top--;
+            level_ids.resize(top);
+            level_adj.resize(top);
+            if (top > 0) entry = *std::min_element(level_ids[top - 1].begin(), level_ids[top - 1].end());
             else
                 for (int v = 0; v < n; v++)
                     if (!bit_of(dead, v)) { entry = v; break; }
         }
-        ng->g.entry_node = entry;
-        rc = graph_rebuild_upper(ng.get());
+        rc = ng->set_levels(std::move(level_ids), std::move(level_adj), entry);
     }
     timer.stop(s);
     cudaStreamSynchronize(s);
@@ -2412,30 +2413,22 @@ static int compact_sub_hierarchy(const CompactSource &t, int L, std::unique_ptr<
         for (size_t i = 0; i < a.size(); i++) r[i] = a[i] >= 0 ? pos[a[i]] : -1;
         return r;
     };
-    sd.reset(new jv_dataset_s());
-    sd->device = t.ds->device;
-    memset(&sd->d, 0, sizeof(DataDesc));
-    sd->d.kind = KIND_F32; sd->d.dim = t.ds->d.dim; sd->d.stride = t.ds->d.stride; sd->d.n = m;
+    sd.reset(new jv_dataset_s(KIND_F32, m, t.ds->d.dim));
     float *rows;
     int32_t *dids;
-    int rc = sd->alloc(&rows, (size_t)m * sd->d.stride * 4);
+    int rc = sd->alloc_rows(&rows);
     if (rc || (rc = sd->alloc(&dids, (size_t)m * 4))) return rc;
-    sd->d.rows = rows;
     CK(cudaMemcpyAsync(dids, ids.data(), (size_t)m * 4, cudaMemcpyHostToDevice, s), "H2D members");
     CK(launch_gather_rows(t.ds->d, dids, m, rows, s), "gather member rows");
-    sg.reset(new jv_graph_s());
-    sg->device = g.device;
-    memset(&sg->g, 0, sizeof(GraphDesc));
     const std::vector<int32_t> adj = remap(g.level_adj[L - 1]);
-    CK(sg->adj0.alloc((size_t)m * degree * 4), "cudaMalloc(sub-hierarchy)");
+    if ((rc = jv_graph_s::create(m, degree, sg))) return rc;
     CK(cudaMemcpy(sg->adj0.get(), adj.data(), adj.size() * 4, cudaMemcpyHostToDevice), "H2D sub-hierarchy");
-    sg->g.n = m; sg->g.degree = degree; sg->g.levels = 1; sg->g.entry_node = pos[g.g.entry_node]; sg->g.entry_level = 0;
-    sg->g.adj0 = sg->adj0.get<int32_t>();
+    Levels up_ids, up_adj;
     for (size_t l = L; l < g.level_ids.size(); l++) {
-        sg->level_ids.push_back(remap(g.level_ids[l]));
-        sg->level_adj.push_back(remap(g.level_adj[l]));
+        up_ids.push_back(remap(g.level_ids[l]));
+        up_adj.push_back(remap(g.level_adj[l]));
     }
-    return graph_rebuild_upper(sg.get());
+    return sg->set_levels(std::move(up_ids), std::move(up_adj), pos[g.g.entry_node]);
 }
 
 // the searchTopK best live members of source t at level `level` for every row of the level that belongs to another source, into
@@ -2673,19 +2666,11 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
     memset(stats, 0, sizeof(*stats));
-    std::unique_ptr<jv_dataset_s> nd(new jv_dataset_s());
-    nd->device = t_active;
-    memset(&nd->d, 0, sizeof(DataDesc));
-    nd->d.kind = KIND_F32; nd->d.dim = dim; nd->d.n = total; nd->d.stride = round4(dim);
-    std::unique_ptr<jv_graph_s> ng(new jv_graph_s());
-    ng->device = t_active;
-    memset(&ng->g, 0, sizeof(GraphDesc));
-    ng->g.n = (int32_t)total; ng->g.degree = degree; ng->g.levels = 1; ng->g.entry_level = 0;
+    std::unique_ptr<jv_dataset_s> nd(new jv_dataset_s(KIND_F32, total, dim));
     float *rows = nullptr;
-    if ((rc = nd->alloc(&rows, (size_t)total * nd->d.stride * 4))) return rc;
-    nd->d.rows = rows;
-    CK(ng->adj0.alloc((size_t)total * degree * 4), "cudaMalloc(adjacency)");
-    ng->g.adj0 = ng->adj0.get<int32_t>();
+    if ((rc = nd->alloc_rows(&rows))) return rc;
+    std::unique_ptr<jv_graph_s> ng;
+    if ((rc = jv_graph_s::create((int32_t)total, degree, ng))) return rc;
     StreamTimer timer;
     CK(timer.start(s), "event");
     // every source's old -> new map on the device, and its live rows scattered to their new ids
@@ -2710,16 +2695,16 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
     if (e != cudaSuccess) rc = cuda_fail(e, "graph_compact: merged rows");
     stats->search_top_k = K;
     int nlev = 0;
+    Levels level_ids, level_adj;
     for (int L = 0; L < levels && !rc; L++) {
         long long members = 0;
         for (const CompactSource &c : src) members += (long long)c.live[L].size();
         if (members == 0) break;  // levels without a live member are dropped, and every level above one is empty too
         if (L == 0) rc = compact_level(src, 0, K, nd.get(), metric, alpha, ng.get(), maps_dev, nullptr, nullptr, stats, s);
         else {
-            std::vector<int32_t> ids, adj;
-            rc = compact_level(src, L, K, nd.get(), metric, alpha, ng.get(), maps_dev, &ids, &adj, stats, s);
-            ng->level_ids.push_back(std::move(ids));
-            ng->level_adj.push_back(std::move(adj));
+            level_ids.emplace_back();
+            level_adj.emplace_back();
+            rc = compact_level(src, L, K, nd.get(), metric, alpha, ng.get(), maps_dev, &level_ids.back(), &level_adj.back(), stats, s);
         }
         nlev = L + 1;
     }
@@ -2733,9 +2718,8 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
             entry = c.map[c.g->g.entry_node];
             break;
         }
-    if (entry < 0) entry = nlev > 1 ? ng->level_ids.back().front() : 0;
-    ng->g.entry_node = entry;
-    if ((rc = graph_rebuild_upper(ng.get()))) return rc;
+    if (entry < 0) entry = nlev > 1 ? level_ids.back().front() : 0;
+    if ((rc = ng->set_levels(std::move(level_ids), std::move(level_adj), entry))) return rc;
     stats->nodes = (int32_t)total;
     stats->levels = ng->g.levels;
     stats->device_ms = timer.ms();
