@@ -137,6 +137,11 @@ JV_API int64_t jv_search_last_settled(void);
 /* The low-rank bound as a DOT_PRODUCT score of rows[i] against queries[i] (both [n][dim]) for basis [dim][32] (column j = basis
    vector j), computed by the device functions the search uses; records_out (may be NULL): the rows' [n][48]-byte records. */
 JV_API int jv_lowrank_bound_pairs(const float *basis, int dim, const float *rows, const float *queries, int64_t n, uint8_t *records_out, float *bounds_out);
+/* The graph search with the refine pass's exclusion (host pointers): query q walks through node exclude_ids[q] (-1: none) but never
+   returns it, as acceptOrds without that one node would. No reranker, no threshold. counters_out (may be NULL): visited, expanded,
+   expanded_base, reranked. */
+JV_API int jv_graph_search_exclude(jv_graph g, jv_dataset approx, int metric, const float *queries, int nq, int topK, int rerankK,
+                                   const int32_t *exclude_ids, int32_t *nodes_out, float *scores_out, int64_t *counters_out);
 JV_API int jv_dataset_device(jv_dataset ds);
 /* ImmutablePQVectors' code-vs-code scoring (base:quantization/ImmutablePQVectors.java:63-105): build the triangular
  * centroid-vs-centroid table of ProductQuantization.createCodebookPartialSums (ProductQuantization.java:609-628; 12.6 MB at M = 96,
@@ -569,6 +574,39 @@ typedef struct {
 } jv_compact_stats;
 JV_API int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric, float alpha, jv_graph *graph_out, jv_dataset *rows_out,
                             jv_compact_stats *stats);
+
+/* The refinement pass on the device (DESIGN §4.3i). Returns a NEW graph in *out; g is untouched, its holes stay holes, and the entry
+ * and the level membership are unchanged. The result has no FusedPQ records. ds holds g's rows (ds's n = g's n, same device).
+ * JV_REFINE_BUILDER: GraphIndexBuilder.cleanup's improveConnections, over fp32, PQ or BQ data sets with the scores their builds use.
+ *   Only a graph with upper levels is refined (a flat graph comes back as a copy): at level 0 every member of level 1, at each level
+ *   L >= 1 every member of L, each with a non-empty row there. Per level the nodes go in ascending batches of params->max_batch (0:
+ *   16384); each batch searches the level as the previous batches left it (level 0 from the entry, without descending; an upper level
+ *   as a graph of its own), beam params->beam_width, excluding the node itself; its candidates are its current row plus the results
+ *   not in it; the robust prune at params->alpha picks M; back-links follow (a row that already names the node is left as it is), rows
+ *   past params->overflow * M are re-pruned, and after the last batch every row longer than M is.
+ * JV_REFINE_COMPACTOR: OnDiskGraphIndexCompactor's refine pass, fp32 only. Level 0 only: the members of level 1, or every live node
+ *   when g is flat; beam 8 M; every search reads g as it is and the rows replace the old ones at the end, with no back-links;
+ *   params->alpha is the compactor's alpha. params->beam_width, overflow and max_batch still have to be valid.
+ * params->degree must equal g's degree; params->add_hierarchy, seed and concurrent_window are not read.
+ * Errors, all before any device work (a refused call leaves *out untouched): JV_ERR_INVALID for a null argument, a data set whose kind
+ * the mode does not take, a size or device mismatch, a degree that differs from g's, bad build parameters, a bad metric or mode;
+ * JV_ERR_UNSUPPORTED for a degree above 64, or a PQ LUT the prune cannot hold next to the candidates. */
+#define JV_REFINE_BUILDER 0
+#define JV_REFINE_COMPACTOR 1
+#define JV_REFINE_MAX_LEVELS 64
+typedef struct {
+    int levels;                                   /* levels refined: g's levels (builder form), 1 (compactor form), 0 for a copy */
+    int64_t nodes_refined[JV_REFINE_MAX_LEVELS];  /* per level; levels past the last entry are counted in it */
+    int64_t candidates;                           /* candidates scored, summed over all refined nodes */
+    int32_t max_candidates;                       /* the largest candidate set of one node */
+    int64_t rows_changed;                         /* rows, over all levels, whose contents differ from g's */
+    int64_t backlinks_added, backlinks_dropped;   /* builder form: back-links written, and dropped at a full row */
+    int64_t rows_repruned;                        /* builder form: rows re-pruned past overflow * M and by the final cleanup */
+    double device_ms;                             /* stream time of the refine's device work (searches, candidates, prunes, back-links,
+                                                     re-prunes), summed between the host's waits for each batch's counts; the
+                                                     host's work (node lists, the upper levels' rows and id mapping) is not in it */
+} jv_refine_stats;
+JV_API int jv_graph_refine(jv_graph g, jv_dataset ds, int metric, const jv_build_params *params, int mode, jv_graph *out, jv_refine_stats *stats);
 
 /* device-memory helpers for callers that keep queries/results in HBM (bench `value` leg) */
 JV_API int jv_device_malloc(void **out, size_t bytes);

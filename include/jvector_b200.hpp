@@ -234,8 +234,17 @@ public:
         check(jv_graph_add_nodes_bq(graph.handle(), v.handle(), (int)vsf_, &p_, deletedBits.empty() ? nullptr : deletedBits.data(), &g, &deviceMs));
         return GraphIndex(g);
     }
+    /// cleanup()'s improveConnections (jv_graph_refine, JV_REFINE_BUILDER): a NEW graph; the counters go to refineStats
+    template <typename V>
+    GraphIndex refine(const GraphIndex &graph, const V &v)
+    {
+        jv_graph g = nullptr;
+        check(jv_graph_refine(graph.handle(), v.handle(), (int)vsf_, &p_, JV_REFINE_BUILDER, &g, &refineStats));
+        return GraphIndex(g);
+    }
     double deviceMs = 0;
     jv_remove_stats removeStats = {};
+    jv_refine_stats refineStats = {};
 
 private:
     VectorSimilarityFunction vsf_;
@@ -263,9 +272,18 @@ public:
         jv_graph g = nullptr;
         jv_dataset rows = nullptr;
         check(jv_graph_compact(src.data(), (int)src.size(), (int)vsf_, alpha_, &g, &rows, &stats));
-        return {GraphIndex(g), F32Vectors(rows)};
+        GraphIndex merged(g);
+        F32Vectors merged_rows(rows);
+        if (!refine_) return {std::move(merged), std::move(merged_rows)};
+        // the compactor's refine pass (jv_graph_refine, JV_REFINE_COMPACTOR) at alpha; beam, overflow and batch are only validated
+        jv_build_params p = {merged.maxDegree(), 100, 1.2f, alpha_, 0, 0, 0, -1};
+        jv_graph r = nullptr;
+        check(jv_graph_refine(merged.handle(), merged_rows.handle(), (int)vsf_, &p, JV_REFINE_COMPACTOR, &r, &refineStats));
+        return {GraphIndex(r), std::move(merged_rows)};
     }
+    void setRefineAfterCompaction(bool refine) { refine_ = refine; }
     jv_compact_stats stats = {};
+    jv_refine_stats refineStats = {};
 
 private:
     std::vector<std::pair<const GraphIndex *, const F32Vectors *>> sources_;
@@ -273,6 +291,7 @@ private:
     std::vector<std::vector<int32_t>> maps_;
     VectorSimilarityFunction vsf_;
     float alpha_;
+    bool refine_ = false;
 };
 
 }  // namespace jv

@@ -9,6 +9,7 @@ mirror of the reference's interface for that path, used by the tests and the ben
   ScoreFunction (similarityTo / similarityToBatch)  base:graph/similarity/ScoreFunction.java
   GraphIndex, GraphSearcher.search              base:graph/GraphSearcher.java:222
   GraphIndexBuilder.build                       base:graph/GraphIndexBuilder.java:436
+  GraphIndexBuilder.refine                      base:graph/GraphIndexBuilder.java:472-538 (cleanup's improveConnections)
   GraphIndexCompactor.compact                   graph/disk/OnDiskGraphIndexCompactor.java (the per-node merge, not the file)
 """
 from . import api

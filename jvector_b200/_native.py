@@ -50,6 +50,15 @@ class CompactStats(C.Structure):
                 ("candidates", C.c_int64), ("max_candidates", C.c_int32), ("visited", C.c_int64), ("device_ms", C.c_double)]
 
 
+class RefineStats(C.Structure):
+    _fields_ = [("levels", C.c_int), ("nodes_refined", C.c_int64 * 64), ("candidates", C.c_int64), ("max_candidates", C.c_int32),
+                ("rows_changed", C.c_int64), ("backlinks_added", C.c_int64), ("backlinks_dropped", C.c_int64), ("rows_repruned", C.c_int64),
+                ("device_ms", C.c_double)]
+
+
+REFINE_BUILDER, REFINE_COMPACTOR = 0, 1
+
+
 class PQTrainParams(C.Structure):
     _fields_ = [("M", C.c_int), ("k", C.c_int), ("globally_center", C.c_int), ("lloyd_iterations", C.c_int), ("max_train_rows", C.c_int64),
                 ("seed", C.c_uint64)]
@@ -101,6 +110,7 @@ SYMBOLS = [
     ("jv_graph_edge_records_download", _I, [_P, _P]),
     ("jv_search_last_settled", _L, []),
     ("jv_lowrank_bound_pairs", _I, [f32p, _I, f32p, f32p, C.c_int64, _P, f32p]),
+    ("jv_graph_search_exclude", _I, [_P, _P, _I, f32p, _I, _I, _I, i32p, i32p, f32p, i64p]),
     ("jv_dataset_pq_pair_table", _I, [_P, _I]), ("jv_dataset_pq_pair_table_download", _I, [_P, _I, f32p]),
     ("jv_dataset_free", _I, [_P]), ("jv_dataset_size", _L, [_P]), ("jv_dataset_dim", _I, [_P]), ("jv_dataset_device_bytes", _L, [_P]),
     ("jv_query_begin", _I, [_P, f32p, _I, C.POINTER(_P)]), ("jv_score_batch", _I, [_P, i32p, _I, f32p]), ("jv_query_end", _I, [_P]),
@@ -152,6 +162,7 @@ SYMBOLS = [
     ("jv_graph_add_nodes_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_builder_create_from_graph_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), _P, C.POINTER(_P)]),
     ("jv_graph_compact", _I, [C.POINTER(CompactSource), _I, _I, _F, C.POINTER(_P), C.POINTER(_P), C.POINTER(CompactStats)]),
+    ("jv_graph_refine", _I, [_P, _P, _I, C.POINTER(BuildParams), _I, C.POINTER(_P), C.POINTER(RefineStats)]),
     ("jv_builder_create", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]), ("jv_builder_info", _I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     ("jv_builder_next_batch", _I, [_P, i32p, i32p]), ("jv_builder_insert_slice", _I, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     ("jv_builder_apply_new", _I, [_P, C.c_int32, C.c_int32, _P, _P, i32p]), ("jv_builder_reprune_slice", _I, [_P, C.c_int32, C.c_int32, _P, _P]),

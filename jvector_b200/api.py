@@ -508,9 +508,13 @@ class GraphIndexBuilder:
     codes (BuildScoreProvider.pqBuildScoreProvider) when build(), addGraphNodes() or removeDeletedNodes() is given PQVectors, or over
     BQ codes (BuildScoreProvider.bqBuildScoreProvider) when they are given BQVectors."""
 
-    def __init__(self, vsf, M=32, beamWidth=100, neighborOverflow=1.2, alpha=1.2, addHierarchy=False, seed=0, max_batch=0, concurrent_window=-1):
+    def __init__(self, vsf, M=32, beamWidth=100, neighborOverflow=1.2, alpha=1.2, addHierarchy=False, seed=0, max_batch=0, concurrent_window=-1,
+                 refineFinalGraph=False):
+        """refineFinalGraph: build() ends with refine() of its graph, as the reference's cleanup() does. The reference's default is true;
+        here it is False, so that a build gives the graph it always gave unless the refine is asked for."""
         self.vsf = vsf
         self.params = nat.BuildParams(M, beamWidth, neighborOverflow, alpha, 1 if addHierarchy else 0, seed, max_batch, concurrent_window)
+        self.refineFinalGraph = bool(refineFinalGraph)
         self.device_ms = 0.0
 
     def build(self, vectors):
@@ -527,7 +531,22 @@ class GraphIndexBuilder:
         s, b, d = C.c_int64(), C.c_int64(), C.c_int64()
         lib.jv_graph_build_stats(C.byref(s), C.byref(b), C.byref(d))
         self.scored_vectors, self.batches, self.dropped_backlinks = s.value, b.value, d.value
-        return GraphIndex(_handle=h)
+        g = GraphIndex(_handle=h)
+        if not self.refineFinalGraph:
+            return g
+        try:
+            return self.refine(g, vectors)
+        finally:
+            g.close()
+
+    def refine(self, graph, vectors):
+        """GraphIndexBuilder.cleanup's improveConnections on the device (jv_graph_refine, JV_REFINE_BUILDER): the step a caller runs
+        after addGraphNodes or removeDeletedNodes. Every member of level 1 is refined at level 0 and every member of a level L >= 1 at L:
+        a search of the level excluding the node, its row merged with the results, the robust prune at alpha, back-links, and the
+        re-prune of rows past neighborOverflow * M; at the end every row is cut to M. A graph without upper levels comes back as a copy.
+        vectors: the graph's F32Vectors, PQVectors or BQVectors, scored as build() scores them. Returns a NEW GraphIndex (`graph` is left
+        as it is, its holes, entry and levels are kept) carrying `.refine_stats` (jv_refine_stats as a dict) and no FusedPQ records."""
+        return _refine(graph, vectors, self.vsf, self.params, nat.REFINE_BUILDER)
 
     def removeDeletedNodes(self, graph, vectors, deleted):
         """GraphIndexBuilder.markNodeDeleted + cleanup's removeDeletedNodes (GraphIndexBuilder.java:689-799) on the device.
@@ -592,8 +611,9 @@ class GraphIndexCompactor:
     live nodes in id order (a source with holes from removeDeletedNodes then needs a live mask that leaves them out). compact() returns (GraphIndex, F32Vectors): the merged graph and its rows in new-id order. The sources
     are left as they are; `.stats` holds jv_compact_stats as a dict after compact()."""
 
-    def __init__(self, sources, liveNodes, remappers, vsf, alpha=1.2):
+    def __init__(self, sources, liveNodes, remappers, vsf, alpha=1.2, refineAfterCompaction=False):
         self.sources, self.vsf, self.alpha = list(sources), vsf, float(alpha)
+        self.refineAfterCompaction = bool(refineAfterCompaction)
         sizes = [g.info()["n"] for g, _ in self.sources]
         live = liveNodes if liveNodes is not None else [None] * len(sizes)
         if len(live) != len(sizes):
@@ -617,6 +637,13 @@ class GraphIndexCompactor:
             if r.shape != (n,):
                 raise ValueError("remapper has shape %s, its graph has %d nodes" % (r.shape, n))
         self.stats = None
+        self.refine_stats = None
+
+    def setRefineAfterCompaction(self, refine):
+        """whether compact() ends with the compactor's refine pass (jv_graph_refine, JV_REFINE_COMPACTOR) over the merged graph: each
+        member of level 1, or each node when the merged graph is flat, gets its level-0 row re-pruned at alpha over its row and a beam
+        of 8 M from a search of the merged graph that excludes it; all rows are replaced at the end, without back-links"""
+        self.refineAfterCompaction = bool(refine)
 
     def compact(self):
         lib = nat.init()
@@ -630,7 +657,30 @@ class GraphIndexCompactor:
         self.stats = {name: getattr(st, name) for name, _ in nat.CompactStats._fields_}
         rows = F32Vectors.__new__(F32Vectors)
         _Vectors.__init__(rows, rh, None)
-        return GraphIndex(_handle=gh), rows
+        g = GraphIndex(_handle=gh)
+        if self.refineAfterCompaction:
+            params = nat.BuildParams(g.info()["degree"], 100, 1.2, self.alpha, 0, 0, 0, -1)
+            try:
+                refined = _refine(g, rows, self.vsf, params, nat.REFINE_COMPACTOR)
+            except BaseException:
+                rows.close()
+                raise
+            finally:
+                g.close()
+            self.refine_stats, g = refined.refine_stats, refined
+        return g, rows
+
+
+def _refine(graph, vectors, vsf, params, mode):
+    """jv_graph_refine: a new GraphIndex carrying .refine_stats"""
+    lib = nat.init()
+    st = nat.RefineStats()
+    h = C.c_void_p()
+    check(lib.jv_graph_refine(graph._h, vectors._h, int(vsf), C.byref(params), mode, C.byref(h), C.byref(st)))
+    out = GraphIndex(_handle=h)
+    out.refine_stats = {name: getattr(st, name) for name, _ in nat.RefineStats._fields_}
+    out.refine_stats["nodes_refined"] = list(st.nodes_refined)[:max(st.levels, 1)]
+    return out
 
 
 def _deleted_bits(deleted, n):

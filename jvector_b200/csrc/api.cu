@@ -1670,6 +1670,45 @@ int jv_graph_search_batch(jv_graph g, jv_dataset approx, jv_dataset reranker, in
     return jv_graph_search_batch_ex(g, approx, reranker, metric, queries, nq, topK, rerankK, nullptr, nodes_out, scores_out, stats);
 }
 
+int jv_graph_search_exclude(jv_graph g, jv_dataset approx, int metric, const float *queries, int nq, int topK, int rerankK,
+                            const int32_t *exclude_ids, int32_t *nodes_out, float *scores_out, int64_t *counters_out)
+{
+    ON_DEVICE_OF(g);
+    if (!approx || !queries || !exclude_ids || !nodes_out || !scores_out || nq <= 0 || topK < 1) return fail(JV_ERR_INVALID, "search_exclude: bad arguments");
+    for (int i = 0; i < nq; i++)
+        if (exclude_ids[i] < -1 || exclude_ids[i] >= g->g.n) return fail(JV_ERR_INVALID, "search_exclude: excluded id out of range");
+    int rc;
+    int32_t *dnodes, *dex;
+    float *dscores;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dnodes = c.take<int32_t>((size_t)nq * topK);
+        dscores = c.take<float>((size_t)nq * topK);
+        dex = c.take<int32_t>(nq);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)nq * approx->d.dim * 4)) || (rc = grow(t_ctx.output, carve(nullptr)))) return rc;
+    carve(t_ctx.output.get());
+    cudaStream_t s = t_ctx.stream;
+    CK(cudaMemcpyAsync(t_ctx.input.get(), queries, (size_t)nq * approx->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+    CK(cudaMemcpyAsync(dex, exclude_ids, (size_t)nq * 4, cudaMemcpyHostToDevice, s), "H2D excluded ids");
+    SearchFilter f;
+    memset(&f, 0, sizeof(f));
+    f.exclude_ids = dex;
+    jv_search_stats st;
+    if ((rc = search_device(g, approx, nullptr, metric, t_ctx.input.get<float>(), nq, topK, rerankK, &f, dnodes, dscores, &st))) return rc;
+    CK(cudaMemcpyAsync(nodes_out, dnodes, (size_t)nq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H nodes");
+    CK(cudaMemcpyAsync(scores_out, dscores, (size_t)nq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    CK(cudaStreamSynchronize(s), "sync");
+    if (counters_out) {
+        counters_out[0] = st.visited;
+        counters_out[1] = st.expanded;
+        counters_out[2] = st.expanded_base;
+        counters_out[3] = st.reranked;
+    }
+    return JV_OK;
+}
+
 static int build_params_check(const jv_build_params *params, BuildParams *bp)
 {
     if (params->degree < 1 || params->degree > 64 || params->beam_width < 1 || params->beam_width > 256 || params->overflow < 1.0f || params->alpha < 1.0f)
@@ -1714,30 +1753,39 @@ static void assign_levels(int n, int degree, uint64_t seed, std::vector<std::vec
 // rows (one gather kernel), from nothing or from `seed` (local rows). ladj: [ids.size()][degree] in node ids. Synchronises `s`.
 // A PQ data set (jv_graph_build_pq) gives the level its members' code rows; codebooks, centroid, magnitudes and pair tables are shared.
 // A BQ data set (jv_graph_build_bq) gives it their word rows.
+// the members ids of a level as a data set of their own, local row r = node ids[r] (one gather kernel on `s`): their fp32 rows, code
+// rows or word rows in `rows`, the ids in `dids`; codebooks, centroid, magnitudes and pair tables are shared with ds
+static cudaError_t gather_level(jv_dataset ds, const std::vector<int32_t> &ids, DeviceBuffer &rows, DeviceBuffer &dids, DataDesc *sub, cudaStream_t s)
+{
+    const int cnt = (int)ids.size();
+    const bool codes = ds->d.kind == KIND_PQ || ds->d.kind == KIND_BQ;
+    memset(sub, 0, sizeof(DataDesc));
+    if (codes) *sub = ds->d;
+    sub->kind = ds->d.kind; sub->dim = ds->d.dim; sub->stride = ds->d.stride; sub->n = cnt;
+    cudaError_t e = rows.alloc(codes ? (size_t)cnt * code_row_bytes(*sub) : (size_t)cnt * sub->stride * 4);
+    if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
+    if (codes) {
+        if (e == cudaSuccess) e = launch_gather_codes(ds->d, dids.get<int32_t>(), cnt, rows.get(), s);
+        if (sub->kind == KIND_BQ) sub->words = rows.get<unsigned long long>();
+        else sub->codes = rows.get<uint8_t>();
+    } else {
+        if (e == cudaSuccess) e = launch_gather_rows(ds->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
+        sub->rows = rows.get<float>();
+    }
+    return e;
+}
+
 static int build_level(jv_dataset ds, int metric, const BuildParams &bp, const std::vector<int32_t> &ids, const BuilderSeed *seed,
                        std::vector<int32_t> &ladj, cudaStream_t s)
 {
     const int cnt = (int)ids.size(), degree = bp.degree;
     ladj.assign((size_t)cnt * degree, -1);
     if (cnt <= 1) return JV_OK;
-    const bool codes = ds->d.kind == KIND_PQ || ds->d.kind == KIND_BQ;
     DataDesc sub;
-    memset(&sub, 0, sizeof(DataDesc));
-    if (codes) sub = ds->d;
-    sub.kind = ds->d.kind; sub.dim = ds->d.dim; sub.stride = ds->d.stride; sub.n = cnt;
     DeviceBuffer rows, adj, dids;  // the members' rows (fp32 rows, code rows or word rows), their adjacency, their ids
-    cudaError_t e = rows.alloc(codes ? (size_t)cnt * code_row_bytes(sub) : (size_t)cnt * sub.stride * 4);
+    cudaError_t e = gather_level(ds, ids, rows, dids, &sub, s);
     if (e == cudaSuccess) e = adj.alloc((size_t)cnt * degree * 4);
-    if (e == cudaSuccess) e = dids.alloc((size_t)cnt * 4);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dids.get(), ids.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s);
-    if (codes) {
-        if (e == cudaSuccess) e = launch_gather_codes(ds->d, dids.get<int32_t>(), cnt, rows.get(), s);
-        if (sub.kind == KIND_BQ) sub.words = rows.get<unsigned long long>();
-        else sub.codes = rows.get<uint8_t>();
-    } else {
-        if (e == cudaSuccess) e = launch_gather_rows(ds->d, dids.get<int32_t>(), cnt, rows.get<float>(), s);
-        sub.rows = rows.get<float>();
-    }
     BuildStats bs2;
     if (e == cudaSuccess) e = build_graph_flat(sub, metric, bp, adj.get<int32_t>(), g_sm_count, &bs2, s, seed);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ladj.data(), adj.get(), ladj.size() * 4, cudaMemcpyDeviceToHost, s);
@@ -2725,6 +2773,127 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
     stats->device_ms = timer.ms();
     *graph_out = ng.release();
     *rows_out = nd.release();
+    return JV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ refinement (DESIGN §4.3i)
+// One level of jv_graph_refine through refine_level (build.cu). Level 0 reads g's adjacency and writes ng's; an upper level is a graph
+// of its own over its members' rows (gather_level, as build_level builds it), its rows mapped to local ids and back, into *adj_out.
+// nodes: the rows of the level to refine, ascending.
+static int refine_graph_level(jv_graph g, jv_graph_s *ng, jv_dataset ds, int metric, const BuildParams &bp, int beam, bool compactor, int level,
+                              const std::vector<int32_t> &nodes, RefineStats *st, std::vector<int32_t> *adj_out, cudaStream_t s)
+{
+    const int n = g->g.n, degree = g->g.degree;
+    cudaError_t e;
+    if (nodes.empty()) {  // nothing to refine: the level as it was
+        if (level > 0) *adj_out = g->level_adj[level - 1];
+        else CK(cudaMemcpyAsync(ng->adj0.get(), g->adj0.get(), (size_t)n * degree * 4, cudaMemcpyDeviceToDevice, s), "copy adjacency");
+        return JV_OK;
+    }
+    if (level == 0) {
+        e = refine_level(ds->d, metric, bp, beam, compactor, g->adj0.get<int32_t>(), degree, g->g.entry_node, nodes, ng->adj0.get<int32_t>(), g_sm_count, st, s);
+        return e == cudaSuccess ? JV_OK : cuda_fail(e, "graph_refine");
+    }
+    const std::vector<int32_t> &ids = g->level_ids[level - 1];
+    const int cnt = (int)ids.size();
+    std::vector<int32_t> pos(n, -1);
+    for (int r = 0; r < cnt; r++) pos[ids[r]] = r;
+    std::vector<int32_t> local(g->level_adj[level - 1]);
+    for (int32_t &x : local) x = x >= 0 ? pos[x] : -1;
+    DataDesc sub;
+    DeviceBuffer rows, dids, din, dout;
+    e = gather_level(ds, ids, rows, dids, &sub, s);
+    if (e == cudaSuccess) e = din.alloc(local.size() * 4);
+    if (e == cudaSuccess) e = dout.alloc(local.size() * 4);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(din.get(), local.data(), local.size() * 4, cudaMemcpyHostToDevice, s);
+    const int32_t entry = pos[g->g.entry_node] >= 0 ? pos[g->g.entry_node] : 0;
+    if (e == cudaSuccess) e = refine_level(sub, metric, bp, beam, compactor, din.get<int32_t>(), degree, entry, nodes, dout.get<int32_t>(), g_sm_count, st, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(local.data(), dout.get(), local.size() * 4, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    else cudaStreamSynchronize(s);  // the buffers above are freed on return
+    if (e != cudaSuccess) return cuda_fail(e, "graph_refine");
+    adj_out->resize(local.size());
+    for (size_t i = 0; i < local.size(); i++) (*adj_out)[i] = local[i] >= 0 ? ids[local[i]] : -1;
+    return JV_OK;
+}
+
+int jv_graph_refine(jv_graph g, jv_dataset ds, int metric, const jv_build_params *params, int mode, jv_graph *out, jv_refine_stats *stats)
+{
+    ON_DEVICE_OF(g);
+    if (!ds || !params || !out || !stats) return fail(JV_ERR_INVALID, "graph_refine: null argument");
+    if (mode != JV_REFINE_BUILDER && mode != JV_REFINE_COMPACTOR) return fail(JV_ERR_INVALID, "graph_refine: unknown mode");
+    if (ds->d.n != g->g.n || ds->device != g->device) return fail(JV_ERR_INVALID, "graph_refine: data set and graph differ in size or device");
+    const bool compactor = mode == JV_REFINE_COMPACTOR;
+    const int kind = ds->d.kind;
+    if (compactor ? kind != KIND_F32 : (kind != KIND_F32 && kind != KIND_PQ && kind != KIND_BQ))
+        return fail(JV_ERR_INVALID, compactor ? "graph_refine: the compactor form takes fp32 rows" : "graph_refine: needs fp32 rows, PQ codes or BQ codes");
+    int rc = check_metric(ds->d, metric);
+    if (rc) return rc;
+    const int degree = g->g.degree;
+    if (params->degree != degree) return fail(JV_ERR_INVALID, "graph_refine: params->degree differs from the graph's degree");
+    if (degree > 64) return fail(JV_ERR_UNSUPPORTED, "graph_refine: degree above 64");
+    BuildParams bp;
+    if ((rc = build_params_check(params, &bp))) return rc;
+    // the compactor's beam: 2 * max(M, max(2, 4 M)) (OnDiskGraphIndexCompactor)
+    const int beam = compactor ? 8 * degree : bp.beam;
+    const int row_cap = std::max(2 * degree, (int)(bp.overflow * degree) + 1);
+    if (row_cap > MAX_DEGREE) return fail(JV_ERR_INVALID, "graph_refine: overflow * degree above the widest row");
+    if (kind == KIND_PQ && !pq_ragged_fits(ds->d, row_cap + beam))
+        return fail(JV_ERR_UNSUPPORTED, "graph_refine: the PQ LUT does not fit the prune's shared memory next to the candidates");
+    if ((rc = provider_check(g, ds, kind, metric, params, &bp, "graph_refine"))) return rc;
+    if ((rc = t_ctx.init())) return rc;
+    cudaStream_t s = t_ctx.stream;
+    const int n = g->g.n, levels = g->g.levels;
+    memset(stats, 0, sizeof(*stats));
+    RefineStats st;
+    memset(&st, 0, sizeof(st));
+    std::unique_ptr<jv_graph_s> ng;
+    if ((rc = jv_graph_s::create(n, degree, ng))) return rc;
+    ng->removed = g->removed;
+    Levels level_adj = g->level_adj;
+    // builder form: refined only when there are upper levels (maxLevel > 0); compactor form: level 0 whenever there is an entry
+    const bool run = g->g.entry_node >= 0 && (compactor || levels > 1);
+    if (!run) CK(cudaMemcpyAsync(ng->adj0.get(), g->adj0.get(), (size_t)n * degree * 4, cudaMemcpyDeviceToDevice, s), "copy adjacency");
+    std::vector<int32_t> adj0;
+    if (run && !compactor) {
+        adj0.resize((size_t)n * degree);
+        CK(cudaMemcpyAsync(adj0.data(), g->adj0.get(), adj0.size() * 4, cudaMemcpyDeviceToHost, s), "D2H adjacency");
+        CK(cudaStreamSynchronize(s), "D2H adjacency");
+    }
+    auto empty_row = [&](const int32_t *row) { return std::all_of(row, row + degree, [](int32_t x) { return x < 0; }); };
+    const int refined_levels = run ? (compactor ? 1 : levels) : 0;
+    for (int L = 0; L < refined_levels && !rc; L++) {
+        std::vector<int32_t> nodes;
+        if (L == 0) {
+            if (levels > 1) {
+                for (int32_t v : g->level_ids[0])
+                    if (compactor || !empty_row(adj0.data() + (size_t)v * degree)) nodes.push_back(v);
+            } else {
+                for (int v = 0; v < n; v++)
+                    if (g->removed.empty() || !bit_of(g->removed, v)) nodes.push_back(v);
+            }
+            std::sort(nodes.begin(), nodes.end());
+        } else {
+            const std::vector<int32_t> &a = g->level_adj[L - 1];
+            for (int r = 0; r < (int)g->level_ids[L - 1].size(); r++)
+                if (!empty_row(a.data() + (size_t)r * degree)) nodes.push_back(r);
+        }
+        const long long before = st.nodes;
+        rc = refine_graph_level(g, ng.get(), ds, metric, bp, beam, compactor, L, nodes, &st, L ? &level_adj[L - 1] : nullptr, s);
+        stats->nodes_refined[std::min(L, JV_REFINE_MAX_LEVELS - 1)] += st.nodes - before;
+    }
+    if (!rc) rc = ng->set_levels(g->level_ids, std::move(level_adj), g->g.entry_node);
+    cudaStreamSynchronize(s);
+    if (rc) return rc;
+    stats->levels = refined_levels;
+    stats->candidates = st.candidates;
+    stats->max_candidates = st.max_candidates;
+    stats->rows_changed = st.rows_changed;
+    stats->backlinks_added = st.backlinks_added;
+    stats->backlinks_dropped = st.backlinks_dropped;
+    stats->rows_repruned = st.rows_repruned;
+    stats->device_ms = st.device_ms;
+    *out = ng.release();
     return JV_OK;
 }
 

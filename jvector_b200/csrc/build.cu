@@ -791,23 +791,48 @@ static size_t gram_smem_bytes(const DataDesc &d)
 // inside t's segment), so every replica of a sharded build applies a batch to bit-identical adjacency (atomics would order the
 // appends by timing, and which back-link a full row drops would differ between replicas).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) apply_rows_kernel(int32_t *adj, int *deg, int row_cap, int degree, int first, int count, const int32_t *rows,
-                                                         const int *rdeg, unsigned long long *pairs)
+// position of node t in the ascending list ids[0, count), -1 if absent
+__device__ __forceinline__ int batch_pos(const int32_t *ids, int count, int32_t t)
+{
+    int lo = 0, hi = count;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (ids[mid] < t) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < count && ids[lo] == t ? lo : -1;
+}
+
+// row i of a batch replaces node u's row: u = first + i (an insert), or with IDS u = ids[i] (a refine, ids ascending). (IDS is a
+// template parameter so that the inserts' form compiles as it did without the id list.)
+template <bool IDS>
+__global__ void __launch_bounds__(256) apply_rows_kernel(int32_t *adj, int *deg, int row_cap, int degree, int first, int count, const int32_t *ids,
+                                                         const int32_t *rows, const int *rdeg, unsigned long long *pairs)
 {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= count * row_cap) return;
     const int i = idx / row_cap, j = idx - i * row_cap;
-    const int u = first + i;
+    const int u = IDS ? ids[i] : first + i;
     const int32_t t = j < degree ? rows[(size_t)i * degree + j] : -1;
     adj[(size_t)u * row_cap + j] = t;
     if (j == 0) deg[u] = rdeg[i];
     if (j < degree) {
         bool link = t >= 0;
-        if (link && t >= first && t < first + count) {
-            // t was inserted in this very batch and may have chosen u itself (both sit in each other's in-progress window): then u is
-            // already in t's row and the back-link would duplicate it (NodeArray.insertSorted refuses duplicates)
-            const int32_t *trow = rows + (size_t)(t - first) * degree;
-            for (int x = 0; x < degree; x++)
+        if constexpr (!IDS) {
+            if (link && t >= first && t < first + count) {
+                // t was inserted in this very batch and may have chosen u itself (both sit in each other's in-progress window): then u is
+                // already in t's row and the back-link would duplicate it (NodeArray.insertSorted refuses duplicates)
+                const int32_t *trow = rows + (size_t)(t - first) * degree;
+                for (int x = 0; x < degree; x++)
+                    if (trow[x] == u) { link = false; break; }
+            }
+        } else if (link) {
+            // a refine: a row that already names u takes no back-link (ConcurrentNeighborMap.java:305-309, a no-op) — t's new row when t
+            // is in the batch, else its current one, which this launch does not write
+            const int tp = batch_pos(ids, count, t);
+            const int32_t *trow = tp >= 0 ? rows + (size_t)tp * degree : adj + (size_t)t * row_cap;
+            const int w = tp >= 0 ? degree : row_cap;
+            for (int x = 0; x < w; x++)
                 if (trow[x] == u) { link = false; break; }
         }
         pairs[(size_t)i * degree + j] = link ? (((unsigned long long)(unsigned)t << 32) | (unsigned)u) : ~0ull;  // ~0 sorts last
@@ -963,18 +988,22 @@ cudaError_t launch_gather_codes(const DataDesc &d, const int32_t *ids_dev, int c
     return cudaGetLastError();
 }
 
-// the insert searches' queries of a PQ build: decode(c_u) for nodes first .. first + count - 1 -> out [count][dim], one CTA per node
-__global__ void __launch_bounds__(128) pq_decode_kernel(DataDesc d, int first, int count, float *out)
+// the insert searches' queries of a PQ build: decode(c_u) for nodes first .. first + count - 1 (IDS, a refine's: nodes ids[i]) -> out
+// [count][dim], one CTA per node. (IDS is a template parameter so that the build's form compiles as it did without the id list.)
+template <bool IDS>
+__global__ void __launch_bounds__(128) pq_decode_kernel(DataDesc d, int first, int count, const int32_t *ids, float *out)
 {
-    for (int i = blockIdx.x; i < count; i += gridDim.x) pq_decode_row(d, first + i, out + (size_t)i * d.dim, threadIdx.x, blockDim.x);
+    for (int i = blockIdx.x; i < count; i += gridDim.x) pq_decode_row(d, IDS ? ids[i] : first + i, out + (size_t)i * d.dim, threadIdx.x, blockDim.x);
 }
 
 // the insert searches' queries of a BQ build: c_u as fp32, +1 where bit j is set and -1 where it is clear, j < dim. The BQ walk
 // re-encodes them (prepare_blob: v > 0) to exactly c_u when c_u has no bit set past dim (bq_padding_set).
-__global__ void __launch_bounds__(128) bq_decode_kernel(DataDesc d, int first, int count, float *out)
+// (IDS, a refine's: nodes ids[i], as pq_decode_kernel)
+template <bool IDS>
+__global__ void __launch_bounds__(128) bq_decode_kernel(DataDesc d, int first, int count, const int32_t *ids, float *out)
 {
     for (int i = blockIdx.x; i < count; i += gridDim.x) {
-        const unsigned long long *w = d.words + (size_t)(first + i) * d.W;
+        const unsigned long long *w = d.words + (size_t)(IDS ? ids[i] : first + i) * d.W;
         for (int j = threadIdx.x; j < d.dim; j += blockDim.x) out[(size_t)i * d.dim + j] = (__ldg(w + (j >> 6)) >> (j & 63)) & 1ull ? 1.0f : -1.0f;
     }
 }
@@ -1250,14 +1279,14 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
     int query_stride = B->d.stride;
     if (B->d.kind == KIND_PQ) {
         // searchProviderFor over PQ: the walk scores with the codes only (no rerank), its query is decode(c_u)
-        pq_decode_kernel<<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, B->qdec);
+        pq_decode_kernel<false><<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, nullptr, B->qdec);
         g_launches++;
         JV_TRY(cudaGetLastError());
         queries = B->qdec;
         query_stride = B->d.dim;
     } else if (B->d.kind == KIND_BQ) {
         // searchProviderFor over BQ: the walk scores with the words only (no rerank), its query encodes to c_u
-        bq_decode_kernel<<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, B->qdec);
+        bq_decode_kernel<false><<<std::min(m, B->sm_count * 16), 128, 0, s>>>(B->d, first + lo, m, nullptr, B->qdec);
         g_launches++;
         JV_TRY(cudaGetLastError());
         queries = B->qdec;
@@ -1275,12 +1304,15 @@ cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, 
 
 // the whole batch's rows (this rank's own slice + the gathered ones): write them, back-link them deterministically, and leave
 // the SORTED list of rows that passed overflow * M in B->list (count in B->list_count[0])
-cudaError_t builder_apply_new(GraphBuilder *B, int first, int count, const int32_t *rows, const int *rdeg, cudaStream_t s)
+// ids (device, ascending): the batch is those nodes' rows replaced (a refine) rather than nodes [first, first + count) inserted
+cudaError_t builder_apply_new(GraphBuilder *B, int first, int count, const int32_t *rows, const int *rdeg, cudaStream_t s, const int32_t *ids)
 {
     cudaError_t err = cudaSuccess;
     if (!rows) { rows = B->own_rows; rdeg = B->own_deg; }
     const int npairs = count * B->degree;
-    apply_rows_kernel<<<(count * B->row_cap + 255) / 256, 256, 0, s>>>(B->adj, B->deg, B->row_cap, B->degree, first, count, rows, rdeg, B->pairs);
+    const unsigned blocks = (count * B->row_cap + 255) / 256;
+    if (ids) apply_rows_kernel<true><<<blocks, 256, 0, s>>>(B->adj, B->deg, B->row_cap, B->degree, first, count, ids, rows, rdeg, B->pairs);
+    else apply_rows_kernel<false><<<blocks, 256, 0, s>>>(B->adj, B->deg, B->row_cap, B->degree, first, count, nullptr, rows, rdeg, B->pairs);
     g_launches++;
     size_t tb = B->cub_bytes;
     JV_TRY(cub::DeviceRadixSort::SortKeys(B->cub_tmp, tb, B->pairs, B->pairs_sorted, npairs, 0, 64, s));
@@ -1292,7 +1324,7 @@ cudaError_t builder_apply_new(GraphBuilder *B, int first, int count, const int32
     tb = B->cub_bytes;
     JV_TRY(cub::DeviceSelect::Flagged(B->cub_tmp, tb, B->head_target, B->head_flag, B->list, B->list_count, npairs, s));  // sorted by target: heads are
     g_launches++;
-    B->inserted = first + count;
+    if (!ids) B->inserted = first + count;
     B->st.batches++;
     return cudaGetLastError();
 }
@@ -1565,10 +1597,13 @@ static_assert(CODE_REPAIR_TIERS <= (int)(sizeof(RepairStats::tier_rows) / sizeof
 
 // whether the repair of a degree-`degree` graph over `pq` can run: a row gathers up to degree * (degree + 2) candidates, and the tier
 // that holds them must fit next to the LUT
-bool pq_repair_fits(const DataDesc &pq, int degree)
+bool pq_repair_fits(const DataDesc &pq, int degree) { return pq_ragged_fits(pq, degree * (degree + 2)); }
+
+// whether the ragged prune's PQ tier that holds max_cands candidates fits next to the LUT
+bool pq_ragged_fits(const DataDesc &pq, int max_cands)
 {
     int t = 0;
-    while (t < CODE_REPAIR_TIERS - 1 && degree * (degree + 2) > CODE_REPAIR_TIER_MAX[t]) t++;
+    while (t < CODE_REPAIR_TIERS - 1 && max_cands > CODE_REPAIR_TIER_MAX[t]) t++;
     return prune_smem_bytes(pq, CODE_REPAIR_TIER_MAX[t]) <= (size_t)PRUNE_PQ_SMEM_MAX;
 }
 
@@ -1779,6 +1814,203 @@ cudaError_t prune_ragged_rows(const DataDesc &d, int metric, float alpha, int de
     if ((err = alloc_owned(mem, out_deg, (size_t)rows * 4)) == cudaSuccess && (err = alloc_owned(mem, tier_list, (size_t)rows * 4)) == cudaSuccess)
         err = prune_ragged_enqueue(d, metric, alpha, degree, rows, cand, row_node, cand_off, cand_cnt, hcnt, out_rows, out_deg, tier_list, sm_count, nullptr, s);
     const cudaError_t drained = cudaStreamSynchronize(s);
+    return err != cudaSuccess ? err : drained;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Refinement (GraphIndexBuilder.cleanup's improveConnections, OnDiskGraphIndexCompactor's refine pass; DESIGN §4.3i), one level at a
+// time. The level's rows seed a GraphBuilder; the nodes to refine go through it in ascending batches of at most max_batch:
+//   search  : graph_search_kernel over the level from its entry, the node's own row (decode(c_v), c_v as +-1) as the query and the
+//             node itself walked through but never accepted (SearchFilter::exclude_ids), topK = rerankK = beam
+//   assemble: refine_assemble_kernel, one warp per node: its current row, then the results that are not in it
+//   prune   : the ragged prune (prune_ragged_enqueue) to M, which sorts the candidates by the top-k key
+//   builder form  : the batch's rows are applied with their back-links (builder_apply_new over the id list, a link into a row that
+//                   already names the node skipped), the rows that passed overflow * M are re-pruned, so the next batch searches the
+//                   level as this one left it; after the last batch every row longer than M is re-pruned
+//   compactor form: every search reads the level as it was given; the rows replace the old ones at the end, with no back-links
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) refine_assemble_kernel(int rows, const int32_t *__restrict__ ids, const int32_t *__restrict__ adj,
+                                                              const int *__restrict__ deg, int row_cap, const int32_t *__restrict__ res, int K,
+                                                              int cand_stride, int32_t *__restrict__ cand, long long *__restrict__ cand_off,
+                                                              int *__restrict__ cand_cnt)
+{
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (warp >= rows) return;
+    const int i = (int)warp;
+    const int32_t *row = adj + (size_t)ids[i] * row_cap;
+    const int d = min(deg[ids[i]], row_cap);
+    int32_t *seg = cand + (size_t)i * cand_stride;
+    int w = 0;
+    // every lane offers one id (-1: none); the kept ones are appended in lane order
+    auto put = [&](int32_t id) {
+        const unsigned b = __ballot_sync(FULL, id >= 0);
+        if (id >= 0) seg[w + __popc(b & ((1u << lane) - 1u))] = id;
+        w += __popc(b);
+    };
+    for (int j0 = 0; j0 < d; j0 += 32) put(j0 + lane < d ? row[j0 + lane] : -1);
+    for (int j0 = 0; j0 < K; j0 += 32) {
+        int32_t id = j0 + lane < K ? res[(size_t)i * K + j0 + lane] : -1;
+        for (int x = 0; x < d && id >= 0; x++)
+            if (row[x] == id) id = -1;
+        put(id);
+    }
+    if (lane == 0) {
+        cand_off[i] = (long long)i * cand_stride;
+        cand_cnt[i] = w;
+    }
+}
+
+// the back-link pairs of a batch that were not skipped: the sorted pairs end in ~0 entries
+__global__ void count_links_kernel(const unsigned long long *pairs_sorted, int npairs, unsigned long long *count)
+{
+    atomicAdd(count, (unsigned long long)lower_bound_u64(pairs_sorted, npairs, ~0ull));
+}
+
+// rows of a [n][degree] adjacency that differ from those of b, one thread per row
+__global__ void __launch_bounds__(256) count_changed_rows_kernel(const int32_t *a, const int32_t *b, int n, int degree, unsigned long long *count)
+{
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    bool changed = false;
+    if (v < n)
+        for (int j = 0; j < degree && !changed; j++) changed = a[(size_t)v * degree + j] != b[(size_t)v * degree + j];
+    const unsigned m = __ballot_sync(FULL, changed);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(count, (unsigned long long)__popc(m));
+}
+
+static cudaError_t refine_level_enqueue(const DataDesc &d, int metric, const BuildParams &bp, int beam, bool compactor, const int32_t *adj_in,
+                                        int degree, int32_t entry, const std::vector<int32_t> &nodes, int32_t *adj_out, int sm_count, RefineStats *st,
+                                        GraphBuilder **Bp, std::vector<DeviceBuffer> &mem, cudaStream_t s)
+{
+    cudaError_t err = cudaSuccess;
+    const int n = (int)d.n, nn = (int)nodes.size();
+    // the builder holds the level's rows, degrees, back-link and re-prune state; its own insert buffers go unused
+    BuildParams cp = bp;
+    cp.beam = std::min(beam, PRUNE_MAXC);
+    cp.window = 0;
+    const BuilderSeed seed = {adj_in, n, degree, nullptr, entry, nullptr};
+    JV_TRY(builder_create(d, metric, cp, sm_count, Bp, s, &seed));
+    GraphBuilder *B = *Bp;
+    const int mb = std::min(B->max_batch, std::max(nn, 1)), row_cap = B->row_cap, cand_stride = row_cap + beam;
+    const bool codes = d.kind == KIND_PQ || d.kind == KIND_BQ;
+    int32_t *list, *res, *cand, *out_rows, *tier_list;
+    float *qrows = B->qdec, *scores;
+    long long *cand_off;
+    int *cand_cnt, *out_deg;
+    unsigned long long *counts;  // back-links kept, rows changed
+    JV_TRY(alloc_owned(mem, list, (size_t)std::max(nn, 1) * 4));
+    if (!codes) JV_TRY(alloc_owned(mem, qrows, (size_t)mb * d.stride * 4));
+    JV_TRY(alloc_owned(mem, res, (size_t)mb * beam * 4));
+    JV_TRY(alloc_owned(mem, scores, (size_t)mb * beam * 4));
+    JV_TRY(alloc_owned(mem, cand, (size_t)mb * cand_stride * 4));
+    JV_TRY(alloc_owned(mem, cand_off, (size_t)mb * 8));
+    JV_TRY(alloc_owned(mem, cand_cnt, (size_t)mb * 4));
+    JV_TRY(alloc_owned(mem, tier_list, (size_t)mb * 4));
+    // compactor form: every refined row is kept until the end
+    JV_TRY(alloc_owned(mem, out_rows, (size_t)(compactor ? std::max(nn, 1) : mb) * degree * 4));
+    JV_TRY(alloc_owned(mem, out_deg, (size_t)(compactor ? std::max(nn, 1) : mb) * 4));
+    JV_TRY(alloc_owned(mem, counts, 16));
+    // st->device_ms: the stream time of the device work, lap by lap between the host's waits (the batch's candidate counts, the
+    // re-prune list's length); the allocations above and the host's work while the stream is idle are outside it
+    StreamTimer timer;
+    auto lap_end = [&]() -> cudaError_t {
+        cudaError_t e = timer.stop(s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) st->device_ms += timer.ms();
+        return e;
+    };
+    JV_TRY(timer.start(s));
+    JV_TRY(cudaMemsetAsync(counts, 0, 16, s));
+    if (nn > 0) JV_TRY(cudaMemcpyAsync(list, nodes.data(), (size_t)nn * 4, cudaMemcpyHostToDevice, s));
+    GraphDesc g = {};
+    g.n = n; g.degree = row_cap; g.levels = 1; g.entry_node = B->entry; g.entry_level = 0; g.adj0 = B->adj;
+    SearchFilter f;
+    memset(&f, 0, sizeof(f));
+    f.lenient = 1;  // as an insert search: a full visited table ends the walk with what it has
+    std::vector<int> hcnt;
+    for (int b0 = 0; b0 < nn; b0 += mb) {
+        const int m = std::min(mb, nn - b0);
+        const int32_t *ids = list + b0;
+        int query_stride = d.stride;
+        if (d.kind == KIND_PQ) pq_decode_kernel<true><<<std::min(m, sm_count * 16), 128, 0, s>>>(d, 0, m, ids, qrows);
+        else if (d.kind == KIND_BQ) bq_decode_kernel<true><<<std::min(m, sm_count * 16), 128, 0, s>>>(d, 0, m, ids, qrows);
+        if (codes) {
+            g_launches++;
+            JV_TRY(cudaGetLastError());
+            query_stride = d.dim;
+        } else {
+            JV_TRY(launch_gather_rows(d, ids, m, qrows, s));
+        }
+        SearchPlan plan;
+        JV_TRY(plan_search(d, nullptr, g, beam, beam, m, 0, 0, sm_count, &plan));
+        JV_TRY(B->scratch.grow(search_scratch_bytes(plan)));
+        f.exclude_ids = ids;
+        JV_TRY(launch_search(g, d, nullptr, metric, qrows, m, beam, beam, plan, B->scratch.get(), B->work_counter, res, scores, B->counters, B->overflow,
+                             nullptr, query_stride, &f, s));
+        refine_assemble_kernel<<<(unsigned)(((long long)m * 32 + 255) / 256), 256, 0, s>>>(m, ids, B->adj, B->deg, row_cap, res, beam, cand_stride, cand,
+                                                                                         cand_off, cand_cnt);
+        g_launches++;
+        JV_TRY(cudaGetLastError());
+        hcnt.resize(m);
+        JV_TRY(cudaMemcpyAsync(hcnt.data(), cand_cnt, (size_t)m * 4, cudaMemcpyDeviceToHost, s));
+        JV_TRY(lap_end());
+        JV_TRY(timer.start(s));
+        for (int a = 0; a < m; a++) {
+            st->candidates += hcnt[a];
+            st->max_candidates = std::max(st->max_candidates, hcnt[a]);
+        }
+        int32_t *rows = compactor ? out_rows + (size_t)b0 * degree : out_rows;
+        int *rdeg = compactor ? out_deg + b0 : out_deg;
+        JV_TRY(prune_ragged_enqueue(d, metric, bp.alpha, degree, m, cand, ids, cand_off, cand_cnt, hcnt, rows, rdeg, tier_list, sm_count, nullptr, s));
+        if (compactor) continue;
+        JV_TRY(builder_apply_new(B, 0, m, rows, rdeg, s, ids));
+        count_links_kernel<<<1, 1, 0, s>>>(B->pairs_sorted, m * degree, counts);
+        g_launches++;
+        int over = 0;
+        JV_TRY(lap_end());
+        JV_TRY(builder_list_count(B, &over, s));
+        JV_TRY(timer.start(s));
+        st->rows_repruned += over;
+        JV_TRY(builder_reprune_slice(B, 0, 0, nullptr, nullptr, s));
+    }
+    st->nodes += nn;
+    if (!compactor) {
+        int over = 0;
+        JV_TRY(builder_collect_over_degree(B, s));
+        JV_TRY(lap_end());
+        JV_TRY(builder_list_count(B, &over, s));
+        JV_TRY(timer.start(s));
+        st->rows_repruned += over;
+        JV_TRY(builder_reprune_slice(B, 0, 0, nullptr, nullptr, s));
+    }
+    const long long total = (long long)n * degree;
+    compact_adj_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(B->adj, B->deg, n, row_cap, degree, adj_out);
+    g_launches++;
+    JV_TRY(cudaGetLastError());
+    if (compactor) JV_TRY(launch_scatter_rows(adj_out, degree, list, nn, out_rows, s));
+    count_changed_rows_kernel<<<(n + 255) / 256, 256, 0, s>>>(adj_in, adj_out, n, degree, counts + 1);
+    g_launches++;
+    JV_TRY(cudaGetLastError());
+    unsigned long long h[2];
+    JV_TRY(cudaMemcpyAsync(h, counts, 16, cudaMemcpyDeviceToHost, s));
+    JV_TRY(lap_end());
+    BuildStats bs;
+    JV_TRY(builder_stats(B, &bs, s));
+    st->backlinks_added += (long long)h[0] - bs.dropped_backlinks;
+    st->backlinks_dropped += bs.dropped_backlinks;
+    st->rows_changed += (long long)h[1];
+    return cudaSuccess;
+}
+
+cudaError_t refine_level(const DataDesc &d, int metric, const BuildParams &bp, int beam, bool compactor, const int32_t *adj_in_dev, int degree, int32_t entry,
+                         const std::vector<int32_t> &nodes, int32_t *adj_out_dev, int sm_count, RefineStats *st, cudaStream_t s)
+{
+    if (degree < 1 || degree > 64 || beam < 1 || entry < 0 || entry >= d.n) return cudaErrorInvalidValue;
+    GraphBuilder *B = nullptr;
+    std::vector<DeviceBuffer> mem;  // the scratch goes when this returns: the stream drains first, on success and on error
+    const cudaError_t err = refine_level_enqueue(d, metric, bp, beam, compactor, adj_in_dev, degree, entry, nodes, adj_out_dev, sm_count, st, &B, mem, s);
+    const cudaError_t drained = cudaStreamSynchronize(s);
+    delete B;
     return err != cudaSuccess ? err : drained;
 }
 

@@ -145,6 +145,9 @@ struct SearchFilter {
     float rerank_floor;             // NodeQueue.rerank's rerankFloor; 0 = none
     int lenient;                    // builder only: overflowing walks are cut short and counted instead of failing
     const int *arrived;             // device int or nullptr: queries [0, *arrived) are in place (host-pointer searches overlap the H2D copy)
+    // device [nq] or nullptr: query q walks through node exclude_ids[q] but never accepts it (a refine search of a node's own row,
+    // ExcludingBits); -1 excludes nothing
+    const int32_t *exclude_ids;
 };
 cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const GraphDesc &g, int topK, int rerankK, int nq,
                         int visited_cap_hint, int list_cap_hint, int sm_count, SearchPlan *plan);
@@ -193,7 +196,7 @@ cudaError_t builder_create(const DataDesc &d, int metric, const BuildParams &bp,
 void builder_destroy(GraphBuilder *B);
 bool builder_next_batch(GraphBuilder *B, int *first, int *count);
 cudaError_t builder_insert_slice(GraphBuilder *B, int first, int count, int lo, int hi, int32_t *rows_out, int *deg_out, cudaStream_t s);
-cudaError_t builder_apply_new(GraphBuilder *B, int first, int count, const int32_t *rows, const int *rdeg, cudaStream_t s);
+cudaError_t builder_apply_new(GraphBuilder *B, int first, int count, const int32_t *rows, const int *rdeg, cudaStream_t s, const int32_t *ids = nullptr);
 cudaError_t builder_reprune_slice(GraphBuilder *B, int lo, int hi, int32_t *rows_out, int *deg_out, cudaStream_t s);
 cudaError_t builder_apply_repruned(GraphBuilder *B, int count, const int32_t *rows, const int *rdeg, cudaStream_t s);
 cudaError_t builder_collect_over_degree(GraphBuilder *B, cudaStream_t s);
@@ -214,6 +217,8 @@ bool pq_prune_fits(const DataDesc &pq);
 cudaError_t bq_padding_set(const DataDesc &bq, bool *set, cudaStream_t s);
 // whether the repair's PQ prune holds the LUT next to the largest candidate set a degree-`degree` row can gather
 bool pq_repair_fits(const DataDesc &pq, int degree);
+// whether the ragged prune's PQ tier for up to max_cands candidates per row holds the LUT
+bool pq_ragged_fits(const DataDesc &pq, int max_cands);
 
 // removeDeletedNodes on one level (see build.cu), over an fp32 data set, a PQ data set that carries the metric's pair table and
 // passes pq_repair_fits, or a BQ data set. rows: members of the level; row r is node ids_dev[r] (nullptr: node r, level 0);
@@ -248,6 +253,18 @@ cudaError_t launch_compact_assemble(int rows, int degree, int K, const int32_t *
 // [rows][degree], -1 padded. Synchronises `s`.
 cudaError_t prune_ragged_rows(const DataDesc &d, int metric, float alpha, int degree, int rows, const int32_t *cand, const int32_t *row_node,
                               const long long *cand_off, const int *cand_cnt, const std::vector<int> &hcnt, int32_t *out_rows, int sm_count, cudaStream_t s);
+// The refine pass on one level (DESIGN §4.3i, build.cu "Refinement"): rows [0, d.n) of d with adjacency adj_in_dev [d.n][degree] (-1
+// padded) and entry row `entry`; nodes (host, ascending rows) are refined in batches of bp.max_batch (0: 16384) with a search of
+// beam `beam` and the ragged prune to degree at bp.alpha. Builder form (compactor false): back-links through the builder's sorted step,
+// re-prunes past bp.overflow * degree and the final over-degree cleanup. Compactor form: every search reads adj_in, no back-links.
+// The refined adjacency goes to adj_out_dev [d.n][degree]; the counters are added to *st. Synchronises `s`.
+struct RefineStats {
+    long long nodes, candidates, rows_changed, backlinks_added, backlinks_dropped, rows_repruned;
+    int max_candidates;
+    double device_ms;  // stream time of the refine's device work (see refine_level_enqueue)
+};
+cudaError_t refine_level(const DataDesc &d, int metric, const BuildParams &bp, int beam, bool compactor, const int32_t *adj_in_dev, int degree, int32_t entry,
+                         const std::vector<int32_t> &nodes, int32_t *adj_out_dev, int sm_count, RefineStats *st, cudaStream_t s);
 // adj_dev[rows_of[a] * degree ..] = rows_dev[a * degree ..] for a < count
 cudaError_t launch_scatter_rows(int32_t *adj_dev, int degree, const int32_t *rows_of_dev, int count, const int32_t *rows_dev, cudaStream_t s);
 

@@ -54,7 +54,7 @@ struct SearchParams {
     const uint32_t *accept_bits;  // bit (node & 31) of word (node >> 5); nullptr = Bits.ALL
     long long accept_stride;      // words between two queries' bitsets (0 = one bitset shared by the batch)
     float threshold, rerank_floor;
-    int filtered;                 // accept_bits != nullptr || threshold > 0
+    int filtered;                 // accept_bits != nullptr || threshold > 0 || exclude_ids != nullptr
     const int *arrived;           // nullptr, or: query i may be read only once *arrived > i (the H2D copy is still running)
     int lenient;                  // insert searches of the builder: a full visited table ends the walk with what it has, a tie tail
                                   // that does not fit is dropped — counted in counters->overflowed, never an error (build.cu)
@@ -67,6 +67,7 @@ struct SearchParams {
     int row_prefetch;  // fp32 / NVQ walks: 1 = a bulk L2 prefetch of every newly visited row is issued by the thread that discovered it
                        // (fp32: only for a batch that does not fill the GPU)
     unsigned long long *dbg;  // JV_SEARCH_PROFILE builds only: per-phase cycle totals
+    const int32_t *exclude_ids;  // [nq]: query qi never accepts node exclude_ids[qi] (SearchFilter::exclude_ids, the EXCL instantiations)
 };
 
 __device__ __forceinline__ bool visited_insert(int32_t *t, unsigned mask, int shift, int32_t v)
@@ -227,7 +228,9 @@ constexpr uint8_t F_ACCEPTED = 2;  // acceptOrds.get(node) && score >= threshold
 // VSM: the visited set lives in shared memory (a template parameter, not a run-time flag: the two forms must not cost each other
 // registers — the fp32 walk lost 15 % when they shared one instantiation).
 // EDGE: the fp32 DOT walk over a graph with edge records (P.g.edge_rec, launch_search), a separate instantiation for the same reason
-template <int KIND, int METRIC, int MINB, bool VSM, bool EDGE = false>
+// EXCL: the walks of a refine, which never accept their query's own node (P.exclude_ids); separate so that the other walks compile
+// exactly as they do without it
+template <int KIND, int METRIC, int MINB, bool VSM, bool EDGE = false, bool EXCL = false>
 __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search_kernel(SearchParams P)
 {
     constexpr int SEARCH_THREADS = SearchThreads<KIND>::value;
@@ -326,7 +329,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
             if (lane == 0) {
                 const int32_t en = P.g.entry_node;
                 cur[0] = topk_key(sc, en);
-                fcur[0] = ((!acc || ((acc[en >> 5] >> (en & 31)) & 1u)) && sc >= P.threshold) ? F_ACCEPTED : 0;
+                fcur[0] = ((!acc || ((acc[en >> 5] >> (en & 31)) & 1u)) && sc >= P.threshold && !(EXCL && P.exclude_ids[qi] == en)) ? F_ACCEPTED : 0;
                 if (vsm) visited_insert_smem(vis, P.vis_idmask, P.vis_rlog, en, &s_vfail);
                 else visited_insert(table, vmask, P.visited_shift, en);
             }
@@ -533,7 +536,8 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         } else {                                                                                                                    \
             const int m_ = atomicAdd(&s_m, 1);                                                                                      \
             cand_keys[m_] = key_;                                                                                                   \
-            if (P.filtered) cand_acc[m_] = ((!acc || ((acc[(f_) >> 5] >> ((f_) & 31)) & 1u)) && (sc_) >= P.threshold) ? F_ACCEPTED : 0; \
+            if (P.filtered) cand_acc[m_] = ((!acc || ((acc[(f_) >> 5] >> ((f_) & 31)) & 1u)) && (sc_) >= P.threshold &&              \
+                                            !(EXCL && P.exclude_ids[qi] == (f_))) ? F_ACCEPTED : 0;                               \
         }                                                                                                                           \
     } while (0)
                 if (KIND == KIND_F32) {
@@ -900,7 +904,8 @@ static cudaError_t occupancy_of(size_t smem, int *blocks_per_sm)
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, graph_search_kernel<KIND, METRIC, MINB, VSM>, SearchThreads<KIND>::value, smem);
 }
 
-#define JV_SEARCH_DISPATCH_V(kind, metric, pq_wide, V, CALL)                                                  \
+// the fp32, PQ and BQ walks; any other kind runs OTHER
+#define JV_SEARCH_DISPATCH_FPB_V(kind, metric, pq_wide, V, CALL, OTHER)                                            \
     do {                                                                                        \
         if ((kind) == KIND_F32 && (pq_wide)) {                                                  \
             if ((metric) == JV_METRIC_EUCLIDEAN) { CALL(KIND_F32, JV_METRIC_EUCLIDEAN, MINB_ROWS_WIDE, V); } \
@@ -923,11 +928,17 @@ static cudaError_t occupancy_of(size_t smem, int *blocks_per_sm)
             else if ((metric) == JV_METRIC_DOT) { CALL(KIND_BQ, JV_METRIC_DOT, MINB_DEFAULT, V); }               \
             else { CALL(KIND_BQ, JV_METRIC_COSINE, MINB_DEFAULT, V); }                                           \
         } else {                                                                                \
-            if ((metric) == JV_METRIC_EUCLIDEAN) { CALL(KIND_NVQ, JV_METRIC_EUCLIDEAN, MINB_ROWS, V); }       \
-            else if ((metric) == JV_METRIC_DOT) { CALL(KIND_NVQ, JV_METRIC_DOT, MINB_ROWS, V); }              \
-            else { CALL(KIND_NVQ, JV_METRIC_COSINE, MINB_ROWS, V); }                                          \
+            OTHER;                                                                              \
         }                                                                                       \
     } while (0)
+#define JV_SEARCH_DISPATCH_NVQ_V(metric, V, CALL)                                               \
+    do {                                                                                        \
+        if ((metric) == JV_METRIC_EUCLIDEAN) { CALL(KIND_NVQ, JV_METRIC_EUCLIDEAN, MINB_ROWS, V); }           \
+        else if ((metric) == JV_METRIC_DOT) { CALL(KIND_NVQ, JV_METRIC_DOT, MINB_ROWS, V); }                  \
+        else { CALL(KIND_NVQ, JV_METRIC_COSINE, MINB_ROWS, V); }                                              \
+    } while (0)
+#define JV_SEARCH_DISPATCH_V(kind, metric, pq_wide, V, CALL) \
+    JV_SEARCH_DISPATCH_FPB_V(kind, metric, pq_wide, V, CALL, JV_SEARCH_DISPATCH_NVQ_V(metric, V, CALL))
 #define JV_SEARCH_DISPATCH(kind, metric, pq_wide, vsm, CALL)                    \
     do {                                                                       \
         if (vsm) JV_SEARCH_DISPATCH_V(kind, metric, pq_wide, true, CALL);      \
@@ -1098,7 +1109,8 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     P.accept_stride = filter ? filter->accept_stride_words : 0;
     P.threshold = filter ? filter->threshold : 0.f;
     P.rerank_floor = filter ? filter->rerank_floor : 0.f;
-    P.filtered = (P.accept_bits != nullptr || P.threshold > 0.f) ? 1 : 0;
+    P.exclude_ids = filter ? filter->exclude_ids : nullptr;
+    P.filtered = (P.accept_bits != nullptr || P.threshold > 0.f || P.exclude_ids != nullptr) ? 1 : 0;
     P.lenient = filter ? filter->lenient : 0;
     P.arrived = filter ? filter->arrived : nullptr;
     P.query_stride = query_stride > 0 ? query_stride : approx.dim;
@@ -1185,13 +1197,24 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
         e = cudaFuncSetAttribute(graph_search_kernel<KIND_F32, JV_METRIC_DOT, B, V, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
         if (e == cudaSuccess) graph_search_kernel<KIND_F32, JV_METRIC_DOT, B, V, true><<<plan.ctas, SearchThreads<KIND_F32>::value, plan.smem_bytes, s>>>(P); \
     } while (0)
-    if (P.g.edge_rec) {
+    // a refine's walks, over fp32, PQ or BQ rows (no NVQ data set is refined); the edge records are off for them, with the same answers
+#define CALL_EXCL(K, M, B, V)                                                                                                       \
+    do {                                                                                                                              \
+        e = cudaFuncSetAttribute(graph_search_kernel<K, M, B, V, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
+        if (e == cudaSuccess) graph_search_kernel<K, M, B, V, false, true><<<plan.ctas, SearchThreads<K>::value, plan.smem_bytes, s>>>(P); \
+    } while (0)
+    if (P.exclude_ids) {
+        P.g.edge_rec = nullptr;
+        if (plan.vis_slots_log != 0) JV_SEARCH_DISPATCH_FPB_V(approx.kind, metric, plan.pq_wide != 0, true, CALL_EXCL, e = cudaErrorInvalidValue);
+        else JV_SEARCH_DISPATCH_FPB_V(approx.kind, metric, plan.pq_wide != 0, false, CALL_EXCL, e = cudaErrorInvalidValue);
+    } else if (P.g.edge_rec) {
         if (plan.vis_slots_log != 0) {
             if (plan.pq_wide) CALL_EDGE(MINB_ROWS_WIDE, true);
             else CALL_EDGE(MINB_ROWS, true);
         } else if (plan.pq_wide) CALL_EDGE(MINB_ROWS_WIDE, false);
         else CALL_EDGE(MINB_ROWS, false);
     } else JV_SEARCH_DISPATCH(approx.kind, metric, plan.pq_wide != 0, plan.vis_slots_log != 0, CALL);
+#undef CALL_EXCL
 #undef CALL_EDGE
 #undef CALL
     if (e != cudaSuccess) return e;
