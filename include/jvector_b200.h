@@ -232,6 +232,12 @@ JV_API int jv_nvq_encode_dataset(jv_dataset f32, int nsub, const float *mean, in
 
 /* NVQ inline vectors without a host round trip: encode the resident fp32 rows into a NEW resident NVQ data set */
 JV_API int jv_nvq_encode_dataset_resident(jv_dataset f32, int nsub, const float *mean, int learn, jv_dataset *out);
+/* the same for PQ (ProductQuantization.encodeAll, unweighted): the resident fp32 rows encoded with codebooks [k * dim] (host) and an
+ * optional centroid [dim] (host) into a NEW resident PQ data set, as jv_dataset_register_pq would hold the same codes */
+JV_API int jv_pq_encode_dataset_resident(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, jv_dataset *out);
+/* a resident PQ data set read back: codes [n][M], codebooks [k * dim], centroid [dim]; any pointer may be NULL. JV_ERR_INVALID for a
+ * data set that is not PQ, or a centroid_out when it has no centroid */
+JV_API int jv_dataset_pq_download(jv_dataset pq, uint8_t *codes_out, float *codebooks_out, float *centroid_out);
 
 /* ---- PQ training: ProductQuantization.compute / refine with isotropic (UNWEIGHTED) loss, on the device ----
  * The training rows are the resident rows of `f32` (an out-of-core index registers a sample), all of them, or, above the cap, a
@@ -574,6 +580,33 @@ typedef struct {
 } jv_compact_stats;
 JV_API int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric, float alpha, jv_graph *graph_out, jv_dataset *rows_out,
                             jv_compact_stats *stats);
+
+/* Merging graphs whose nodes carry PQ codes (OnDiskGraphIndexCompactor's FusedPQ and sidecar compaction, DESIGN §4.3h). source_pq[i]
+ * holds the codes of source i's n nodes, each source with codebooks of its own. Two forms:
+ *   fused   every source graph carries FusedPQ records packed from its own source_pq[i] (jv_graph_fuse_pq): the search of another
+ *           source t walks t's records (t's plain code rows above level 0) and reranks its searchTopK survivors exactly over t's rows;
+ *           the merged graph is fused with the new codes;
+ *   sidecar no source carries records: the merge is jv_graph_compact's, graph and rows byte for byte; the merged graph has no records.
+ * Anything else (a mix, records packed from other codes) is refused. Either form then retrains PQ as PQRetrainer.retrain does: a
+ * balanced sample of at most 128 000 live rows across the sources (PQRetrainer.sampleBalanced, chunks of 32 nodes in a Fisher-Yates
+ * order drawn from `seed`), on which source 0's codebooks (and centroid) are refined by 6 unweighted Lloyd rounds (jv_pq_refine with
+ * that seed). The merged rows, encoded with the new codebooks, become a new resident PQ data set in *pq_out (M, k and centroid are
+ * source 0's). codebooks_out [k * dim] receives the new codebooks, centroid_out [dim] source 0's centroid (NULL allowed when source
+ * 0 has none), samples_per_source_out [nsources] (or NULL) the rows sampled from each source.
+ * Errors, all before any device work and leaving every output untouched: whatever jv_graph_compact refuses, with its codes, and
+ * JV_ERR_INVALID for a null argument, a source_pq that is not PQ or differs from its graph in size, dim or device, sources of both
+ * forms, a NULL centroid_out when source 0's PQ has a centroid, or fewer sampled rows than k. */
+typedef struct {
+    jv_compact_stats graph;    /* the merge's counters, as jv_graph_compact fills them (device_ms: the merge only) */
+    int fused;                 /* 1: the sources' FusedPQ records were walked and the output is fused; 0: sidecar form */
+    int64_t train_rows;        /* rows the codebooks were refined on */
+    jv_pq_train_stats train;   /* the refine's counters */
+    double retrain_ms, encode_ms, fuse_ms; /* stream time of the sample's gather and the refine, of the encoding, of the fuse */
+} jv_compact_pq_stats;
+JV_API int jv_graph_compact_pq(const jv_compact_source *sources, const jv_dataset *source_pq, int nsources, int metric, float alpha,
+                               uint64_t seed, jv_graph *graph_out, jv_dataset *rows_out, jv_dataset *pq_out,
+                               float *codebooks_out /* [k * dim] */, float *centroid_out /* [dim] or NULL when source 0 has none */,
+                               int64_t *samples_per_source_out /* [nsources] or NULL */, jv_compact_pq_stats *stats);
 
 /* The refinement pass on the device (DESIGN §4.3i). Returns a NEW graph in *out; g is untouched, its holes stay holes, and the entry
  * and the level membership are unchanged. The result has no FusedPQ records. ds holds g's rows (ds's n = g's n, same device).

@@ -15,6 +15,7 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -63,9 +64,21 @@ struct F32Vectors : Vectors {
 };
 struct PQVectors : Vectors {
     PQVectors(const uint8_t *codes, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid = nullptr)
+        : M(M), k(k), hasCentroid(centroid != nullptr)
     {
         check(jv_dataset_register_pq(codes, n, dim, M, k, codebooks, centroid, &h_));
     }
+    PQVectors(jv_dataset h, int M, int k, bool hasCentroid) : M(M), k(k), hasCentroid(hasCentroid) { h_ = h; }
+    /// the codes [n][M], codebooks [k * dim] and centroid ([dim], empty when there is none) copied back from HBM
+    void download(std::vector<uint8_t> &codes, std::vector<float> &codebooks, std::vector<float> &centroid) const
+    {
+        codes.resize((size_t)size() * M);
+        codebooks.resize((size_t)k * dimension());
+        centroid.resize(hasCentroid ? dimension() : 0);
+        check(jv_dataset_pq_download(h_, codes.data(), codebooks.data(), hasCentroid ? centroid.data() : nullptr));
+    }
+    int M = 0, k = 0;
+    bool hasCentroid = false;
 };
 struct BQVectors : Vectors {
     BQVectors(const uint64_t *words, int64_t n, int dim) { check(jv_dataset_register_bq(words, n, dim, &h_)); }
@@ -254,12 +267,67 @@ private:
 /// OnDiskGraphIndexCompactor's merge (jv_graph_compact): sources[i] is graph i with its rows, liveBits[i] its live nodes (bit
 /// node & 31 of word node >> 5; empty = every node but holes) and remappers[i] its old id -> new id map. compact() returns the
 /// merged graph and its rows in new-id order; the counters go to stats.
+/// Over (graph, rows, PQ codes) triples, compactPQ() merges with PQ (jv_graph_compact_pq: FusedPQ sources walked by their records,
+/// or sidecar codes) and returns the merged graph, its rows and their codes under the retrained codebooks (in codebooks / centroid);
+/// the counters go to pqStats and samplesPerSource.
 class GraphIndexCompactor {
 public:
     GraphIndexCompactor(std::vector<std::pair<const GraphIndex *, const F32Vectors *>> sources, std::vector<std::vector<uint32_t>> liveBits,
                         std::vector<std::vector<int32_t>> remappers, VectorSimilarityFunction vsf, float alpha = 1.2f)
         : sources_(std::move(sources)), live_(std::move(liveBits)), maps_(std::move(remappers)), vsf_(vsf), alpha_(alpha) {}
+    GraphIndexCompactor(const std::vector<std::tuple<const GraphIndex *, const F32Vectors *, const PQVectors *>> &sources,
+                        std::vector<std::vector<uint32_t>> liveBits, std::vector<std::vector<int32_t>> remappers, VectorSimilarityFunction vsf,
+                        float alpha = 1.2f, uint64_t seed = 0)
+        : live_(std::move(liveBits)), maps_(std::move(remappers)), vsf_(vsf), alpha_(alpha), seed_(seed)
+    {
+        for (const auto &t : sources) {
+            sources_.emplace_back(std::get<0>(t), std::get<1>(t));
+            pq_.push_back(std::get<2>(t));
+        }
+    }
     std::pair<GraphIndex, F32Vectors> compact()
+    {
+        const std::vector<jv_compact_source> src = sources();
+        jv_graph g = nullptr;
+        jv_dataset rows = nullptr;
+        check(jv_graph_compact(src.data(), (int)src.size(), (int)vsf_, alpha_, &g, &rows, &stats));
+        GraphIndex merged(g);
+        F32Vectors merged_rows(rows);
+        if (!refine_) return {std::move(merged), std::move(merged_rows)};
+        return {refine(merged, merged_rows), std::move(merged_rows)};
+    }
+    std::tuple<GraphIndex, F32Vectors, PQVectors> compactPQ()
+    {
+        const std::vector<jv_compact_source> src = sources();
+        if (pq_.size() != src.size() || pq_.empty()) throw Error(JV_ERR_INVALID, "compactPQ: one PQ data set per source");
+        std::vector<jv_dataset> pqs;
+        for (const PQVectors *p : pq_) pqs.push_back(p->handle());
+        const PQVectors &p0 = *pq_[0];
+        codebooks.assign((size_t)p0.k * sources_[0].second->dimension(), 0.f);
+        centroid.assign(p0.hasCentroid ? sources_[0].second->dimension() : 0, 0.f);
+        samplesPerSource.assign(src.size(), 0);
+        jv_graph g = nullptr;
+        jv_dataset rows = nullptr, codes = nullptr;
+        check(jv_graph_compact_pq(src.data(), pqs.data(), (int)src.size(), (int)vsf_, alpha_, seed_, &g, &rows, &codes, codebooks.data(),
+                                  p0.hasCentroid ? centroid.data() : nullptr, samplesPerSource.data(), &pqStats));
+        stats = pqStats.graph;
+        GraphIndex merged(g);
+        F32Vectors merged_rows(rows);
+        PQVectors merged_codes(codes, p0.M, p0.k, p0.hasCentroid);
+        if (!refine_) return {std::move(merged), std::move(merged_rows), std::move(merged_codes)};
+        GraphIndex refined = refine(merged, merged_rows);
+        if (pqStats.fused) check(jv_graph_fuse_pq(refined.handle(), merged_codes.handle()));
+        return {std::move(refined), std::move(merged_rows), std::move(merged_codes)};
+    }
+    void setRefineAfterCompaction(bool refine) { refine_ = refine; }
+    jv_compact_stats stats = {};
+    jv_refine_stats refineStats = {};
+    jv_compact_pq_stats pqStats = {};
+    std::vector<float> codebooks, centroid;
+    std::vector<int64_t> samplesPerSource;
+
+private:
+    std::vector<jv_compact_source> sources() const
     {
         if (live_.size() != sources_.size() || maps_.size() != sources_.size()) throw Error(JV_ERR_INVALID, "compact: one live set and one map per source");
         std::vector<jv_compact_source> src(sources_.size());
@@ -269,29 +337,24 @@ public:
                 throw Error(JV_ERR_INVALID, "compact: a live set or a map shorter than its graph");
             src[i] = {sources_[i].first->handle(), sources_[i].second->handle(), live_[i].empty() ? nullptr : live_[i].data(), maps_[i].data()};
         }
-        jv_graph g = nullptr;
-        jv_dataset rows = nullptr;
-        check(jv_graph_compact(src.data(), (int)src.size(), (int)vsf_, alpha_, &g, &rows, &stats));
-        GraphIndex merged(g);
-        F32Vectors merged_rows(rows);
-        if (!refine_) return {std::move(merged), std::move(merged_rows)};
-        // the compactor's refine pass (jv_graph_refine, JV_REFINE_COMPACTOR) at alpha; beam, overflow and batch are only validated
-        jv_build_params p = {merged.maxDegree(), 100, 1.2f, alpha_, 0, 0, 0, -1};
-        jv_graph r = nullptr;
-        check(jv_graph_refine(merged.handle(), merged_rows.handle(), (int)vsf_, &p, JV_REFINE_COMPACTOR, &r, &refineStats));
-        return {GraphIndex(r), std::move(merged_rows)};
+        return src;
     }
-    void setRefineAfterCompaction(bool refine) { refine_ = refine; }
-    jv_compact_stats stats = {};
-    jv_refine_stats refineStats = {};
-
-private:
+    // the compactor's refine pass (jv_graph_refine, JV_REFINE_COMPACTOR) at alpha; beam, overflow and batch are only validated
+    GraphIndex refine(const GraphIndex &merged, const F32Vectors &rows)
+    {
+        jv_build_params p = {merged.maxDegree(), 100, 1.2f, alpha_, 0, seed_, 0, -1};
+        jv_graph r = nullptr;
+        check(jv_graph_refine(merged.handle(), rows.handle(), (int)vsf_, &p, JV_REFINE_COMPACTOR, &r, &refineStats));
+        return GraphIndex(r);
+    }
     std::vector<std::pair<const GraphIndex *, const F32Vectors *>> sources_;
     std::vector<std::vector<uint32_t>> live_;
     std::vector<std::vector<int32_t>> maps_;
     VectorSimilarityFunction vsf_;
     float alpha_;
     bool refine_ = false;
+    uint64_t seed_ = 0;
+    std::vector<const PQVectors *> pq_;
 };
 
 }  // namespace jv

@@ -78,6 +78,11 @@ class PQEncodeStats(C.Structure):
     _fields_ = [("rows_moved", C.c_int64), ("moves", C.c_int64), ("max_sweeps", C.c_int32), ("device_ms", C.c_double)]
 
 
+class CompactPQStats(C.Structure):
+    _fields_ = [("graph", CompactStats), ("fused", C.c_int), ("train_rows", C.c_int64), ("train", PQTrainStats), ("retrain_ms", C.c_double),
+                ("encode_ms", C.c_double), ("fuse_ms", C.c_double)]
+
+
 # every symbol include/jvector_b200.h declares: (name, restype, argtypes)
 _F, _I, _Z, _P, _L = C.c_float, C.c_int, C.c_size_t, C.c_void_p, C.c_int64
 SYMBOLS = [
@@ -132,6 +137,7 @@ SYMBOLS = [
     ("jv_bq_encode_dataset", _I, [_P, u64p]), ("jv_pq_encode_dataset", _I, [_P, _I, _I, f32p, f32p, u8p]),
     ("jv_nvq_encode_dataset", _I, [_P, _I, f32p, _I, f32p, u8p]),
     ("jv_nvq_encode_dataset_resident", _I, [_P, _I, f32p, _I, C.POINTER(_P)]),
+    ("jv_pq_encode_dataset_resident", _I, [_P, _I, _I, f32p, f32p, C.POINTER(_P)]), ("jv_dataset_pq_download", _I, [_P, u8p, f32p, f32p]),
     ("jv_pq_train", _I, [_P, C.POINTER(PQTrainParams), f32p, f32p, C.POINTER(PQTrainStats)]),
     ("jv_pq_refine", _I, [_P, C.POINTER(PQTrainParams), f32p, f32p, f32p, C.POINTER(PQTrainStats)]),
     ("jv_pq_train_anisotropic", _I, [_P, C.POINTER(PQTrainParams), _F, f32p, f32p, C.POINTER(PQAnisotropicStats)]),
@@ -162,6 +168,8 @@ SYMBOLS = [
     ("jv_graph_add_nodes_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_builder_create_from_graph_bq", _I, [_P, _P, _I, C.POINTER(BuildParams), C.POINTER(C.c_uint32), _P, C.POINTER(_P)]),
     ("jv_graph_compact", _I, [C.POINTER(CompactSource), _I, _I, _F, C.POINTER(_P), C.POINTER(_P), C.POINTER(CompactStats)]),
+    ("jv_graph_compact_pq", _I, [C.POINTER(CompactSource), C.POINTER(_P), _I, _I, _F, C.c_uint64, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), f32p,
+                                 f32p, i64p, C.POINTER(CompactPQStats)]),
     ("jv_graph_refine", _I, [_P, _P, _I, C.POINTER(BuildParams), _I, C.POINTER(_P), C.POINTER(RefineStats)]),
     ("jv_builder_create", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]), ("jv_builder_info", _I, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
     ("jv_builder_next_batch", _I, [_P, i32p, i32p]), ("jv_builder_insert_slice", _I, [_P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),

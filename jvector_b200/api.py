@@ -93,11 +93,26 @@ class PQVectors(_Vectors):
         codebooks = c32(codebooks).reshape(-1)
         cen = c32(centroid) if centroid is not None else None
         assert codebooks.size == k * dim
-        self.M, self.k = codes.shape[1], k
+        self.M, self.k, self.has_centroid = codes.shape[1], k, cen is not None
         h = C.c_void_p()
         check(lib.jv_dataset_register_pq(bp(codes), codes.shape[0], dim, codes.shape[1], k, fp(codebooks), fp(cen), C.byref(h)))
         super().__init__(h, None)
 
+    @classmethod
+    def _adopt(cls, handle, M, k, has_centroid):
+        """a resident PQ data set the library made (jv_pq_encode_dataset_resident, jv_graph_compact_pq)"""
+        v = cls.__new__(cls)
+        v.M, v.k, v.has_centroid = M, k, has_centroid
+        _Vectors.__init__(v, handle, None)
+        return v
+
+    def download(self):
+        """(codes uint8 [n][M], codebooks float32 [k * dim], centroid float32 [dim] or None), copied back from HBM"""
+        codes = np.empty((self.size(), self.M), np.uint8)
+        codebooks = np.empty(self.k * self.dimension(), np.float32)
+        centroid = np.empty(self.dimension(), np.float32) if self.has_centroid else None
+        check(nat.load().jv_dataset_pq_download(self._h, bp(codes), fp(codebooks), fp(centroid)))
+        return codes, codebooks, centroid
 
     def build_pair_table(self, vsf):
         """ImmutablePQVectors: the triangular centroid-vs-centroid table in HBM; diversity_scores then sums table entries"""
@@ -388,6 +403,16 @@ def nvq_encode_resident(f32_vectors, mean, nsub, learn=True):
     return _Vectors(h, None)
 
 
+def pq_encode_resident(f32_vectors, codebooks, M, k=256, centroid=None):
+    """ProductQuantization.encodeAll of rows already in HBM into new resident PQVectors (no host round trip)."""
+    lib = nat.init()
+    codebooks = c32(codebooks).reshape(-1)
+    cen = c32(centroid) if centroid is not None else None
+    h = C.c_void_p()
+    check(lib.jv_pq_encode_dataset_resident(f32_vectors._h, M, k, fp(codebooks), fp(cen), C.byref(h)))
+    return PQVectors._adopt(h, M, k, cen is not None)
+
+
 class GraphIndex:
     """ImmutableGraphIndex adjacency in HBM. adj0: [n][degree] int32 (-1 padded); upper: list of (node_ids, adj)."""
 
@@ -609,12 +634,24 @@ class GraphIndexCompactor:
     or None; None (the whole list or an entry) means every node but the source's holes. remappers: per source an int array mapping
     old ids to new ids (read for live nodes, which must map onto exactly [0, live nodes)), or None: the sources in order, each one's
     live nodes in id order (a source with holes from removeDeletedNodes then needs a live mask that leaves them out). compact() returns (GraphIndex, F32Vectors): the merged graph and its rows in new-id order. The sources
-    are left as they are; `.stats` holds jv_compact_stats as a dict after compact()."""
+    are left as they are; `.stats` holds jv_compact_stats as a dict after compact().
 
-    def __init__(self, sources, liveNodes, remappers, vsf, alpha=1.2, refineAfterCompaction=False):
+    With sources of (GraphIndex, F32Vectors, PQVectors) the merge carries PQ (jv_graph_compact_pq): when every graph is fused with its
+    PQVectors, the other sources are searched over their FusedPQ records with an exact rerank and the merged graph comes back fused;
+    when none is fused, the merge is the fp32 one above. Either way PQ is retrained on a balanced sample of the live rows, warm-started
+    from source 0's codebooks (PQRetrainer), and compact() returns (GraphIndex, F32Vectors, PQVectors) with the merged rows' codes; `.pq`
+    holds the retrained ProductQuantization. seed: the sample's chunk order and the retraining's draws."""
+
+    def __init__(self, sources, liveNodes, remappers, vsf, alpha=1.2, refineAfterCompaction=False, seed=0):
         self.sources, self.vsf, self.alpha = list(sources), vsf, float(alpha)
         self.refineAfterCompaction = bool(refineAfterCompaction)
-        sizes = [g.info()["n"] for g, _ in self.sources]
+        self.seed = int(seed)
+        arity = {len(s) for s in self.sources}
+        if not self.sources or len(arity) != 1 or arity.pop() not in (2, 3):
+            raise ValueError("sources: all (GraphIndex, F32Vectors) or all (GraphIndex, F32Vectors, PQVectors)")
+        self.with_pq = len(self.sources[0]) == 3
+        self.pq = None
+        sizes = [s[0].info()["n"] for s in self.sources]
         live = liveNodes if liveNodes is not None else [None] * len(sizes)
         if len(live) != len(sizes):
             raise ValueError("one live mask per source")
@@ -649,26 +686,48 @@ class GraphIndexCompactor:
         lib = nat.init()
         bits = [None if m is None else pack_accept_bits(m) for m in self.live]
         src = (nat.CompactSource * len(self.sources))()
-        for i, ((g, v), b, r) in enumerate(zip(self.sources, bits, self.remappers)):
-            src[i] = nat.CompactSource(g._h, v._h, b.ctypes.data_as(C.POINTER(C.c_uint32)) if b is not None else None, ip(r))
-        st = nat.CompactStats()
+        for i, (s, b, r) in enumerate(zip(self.sources, bits, self.remappers)):
+            src[i] = nat.CompactSource(s[0]._h, s[1]._h, b.ctypes.data_as(C.POINTER(C.c_uint32)) if b is not None else None, ip(r))
         gh, rh = C.c_void_p(), C.c_void_p()
-        check(lib.jv_graph_compact(src, len(self.sources), int(self.vsf), self.alpha, C.byref(gh), C.byref(rh), C.byref(st)))
-        self.stats = {name: getattr(st, name) for name, _ in nat.CompactStats._fields_}
+        codes = None
+        if self.with_pq:
+            pq0, dim = self.sources[0][2], self.sources[0][1].dimension()
+            pqs = (C.c_void_p * len(self.sources))(*[s[2]._h for s in self.sources])
+            cb = np.empty(pq0.k * dim, np.float32)
+            cen = np.empty(dim, np.float32) if pq0.has_centroid else None
+            samples = np.zeros(len(self.sources), np.int64)
+            st = nat.CompactPQStats()
+            ph = C.c_void_p()
+            check(lib.jv_graph_compact_pq(src, pqs, len(self.sources), int(self.vsf), self.alpha, self.seed, C.byref(gh), C.byref(rh), C.byref(ph),
+                                          fp(cb), fp(cen), lp(samples), C.byref(st)))
+            self.stats = {name: getattr(st.graph, name) for name, _ in nat.CompactStats._fields_}
+            self.stats.update({"fused": st.fused, "train_rows": st.train_rows, "retrain_ms": st.retrain_ms, "encode_ms": st.encode_ms,
+                               "fuse_ms": st.fuse_ms, "samples_per_source": samples.tolist(), "train": ProductQuantization._stats(st.train)})
+            codes = PQVectors._adopt(ph, pq0.M, pq0.k, cen is not None)
+            self.pq = ProductQuantization(cb, pq0.M, pq0.k, dim, cen, self.stats["train"])
+        else:
+            st = nat.CompactStats()
+            check(lib.jv_graph_compact(src, len(self.sources), int(self.vsf), self.alpha, C.byref(gh), C.byref(rh), C.byref(st)))
+            self.stats = {name: getattr(st, name) for name, _ in nat.CompactStats._fields_}
         rows = F32Vectors.__new__(F32Vectors)
         _Vectors.__init__(rows, rh, None)
         g = GraphIndex(_handle=gh)
         if self.refineAfterCompaction:
-            params = nat.BuildParams(g.info()["degree"], 100, 1.2, self.alpha, 0, 0, 0, -1)
+            # the refine walks the merged fp32 rows exactly; a fused merge is fused again with the new codes afterwards
+            params = nat.BuildParams(g.info()["degree"], 100, 1.2, self.alpha, 0, self.seed, 0, -1)
             try:
                 refined = _refine(g, rows, self.vsf, params, nat.REFINE_COMPACTOR)
+                if self.with_pq and self.stats["fused"]:
+                    refined.fuse_pq(codes)
             except BaseException:
                 rows.close()
+                if codes is not None:
+                    codes.close()
                 raise
             finally:
                 g.close()
             self.refine_stats, g = refined.refine_stats, refined
-        return g, rows
+        return (g, rows, codes) if self.with_pq else (g, rows)
 
 
 def _refine(graph, vectors, vsf, params, mode):

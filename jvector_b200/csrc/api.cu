@@ -389,31 +389,56 @@ int jv_dataset_register_f32(const float *rows, int64_t n, int dim, jv_dataset *o
     return JV_OK;
 }
 
+// a new PQ data set of n rows on the current device: code rows [n][code_stride] allocated for the caller to fill, codebooks,
+// centroid (host, or NULL) and the sub-space layout uploaded and the self magnitudes computed on `s`
+static int pq_dataset(int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid, cudaStream_t s,
+                      std::unique_ptr<jv_dataset_s> &ds, uint8_t **codes_dev)
+{
+    ds.reset(new jv_dataset_s(KIND_PQ, n, dim));
+    DataDesc &d = ds->d;
+    d.M = M; d.k = k; d.code_stride = round4(M);
+    float *dcb = nullptr, *dcen = nullptr, *dmag = nullptr;
+    int *dlay = nullptr;
+    int rc;
+    if ((rc = ds->alloc(codes_dev, (size_t)n * d.code_stride)) || (rc = ds->alloc(&dcb, (size_t)k * dim * 4)) || (rc = ds->alloc(&dlay, (size_t)M * 8)) ||
+        (rc = ds->alloc(&dmag, (size_t)M * k * 4)) || (centroid && (rc = ds->alloc(&dcen, (size_t)dim * 4))))
+        return rc;
+    cudaError_t e = cudaMemcpyAsync(dcb, codebooks, (size_t)k * dim * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = upload_layout(dim, M, dlay, s);
+    if (e == cudaSuccess && centroid) e = cudaMemcpyAsync(dcen, centroid, (size_t)dim * 4, cudaMemcpyHostToDevice, s);
+    CK(e, "upload pq");
+    d.codes = *codes_dev; d.codebooks = dcb; d.sub_sizes = dlay; d.sub_offsets = dlay + M; d.centroid = dcen; d.mag = dmag;
+    CK(launch_pq_self_magnitudes(d, dmag, s), "pq self magnitudes");
+    return JV_OK;
+}
+
 int jv_dataset_register_pq(const uint8_t *codes, int64_t n, int dim, int M, int k, const float *codebooks, const float *centroid, jv_dataset *out)
 {
     NEED_INIT();
     if (!codes || !codebooks || !out || n <= 0 || dim <= 0 || M <= 0 || M > dim || k <= 0 || k > 256 || n > 0x7fffffffLL)
         return fail(JV_ERR_INVALID, "register_pq: bad arguments");
-    std::unique_ptr<jv_dataset_s> ds(new jv_dataset_s(KIND_PQ, n, dim));
-    DataDesc &d = ds->d;
-    d.M = M; d.k = k; d.code_stride = round4(M);
+    std::unique_ptr<jv_dataset_s> ds;
     uint8_t *dcodes = nullptr;
-    float *dcb = nullptr, *dcen = nullptr, *dmag = nullptr;
-    int *dlay = nullptr;
-    int rc;
-    if ((rc = ds->alloc(&dcodes, (size_t)n * d.code_stride)) || (rc = ds->alloc(&dcb, (size_t)k * dim * 4)) || (rc = ds->alloc(&dlay, (size_t)M * 8)) ||
-        (rc = ds->alloc(&dmag, (size_t)M * k * 4)) || (centroid && (rc = ds->alloc(&dcen, (size_t)dim * 4))))
-        return rc;
-    cudaError_t e = upload_padded(dcodes, codes, (size_t)n, (size_t)M, (size_t)d.code_stride);
-    if (e == cudaSuccess) e = cudaMemcpy(dcb, codebooks, (size_t)k * dim * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = upload_layout(dim, M, dlay, 0);
-    if (e == cudaSuccess && centroid) e = cudaMemcpy(dcen, centroid, (size_t)dim * 4, cudaMemcpyHostToDevice);
-    CK(e, "upload pq");
-    d.codes = dcodes; d.codebooks = dcb; d.sub_sizes = dlay; d.sub_offsets = dlay + M; d.centroid = dcen; d.mag = dmag;
-    e = launch_pq_self_magnitudes(d, dmag, 0);
+    int rc = pq_dataset(n, dim, M, k, codebooks, centroid, 0, ds, &dcodes);
+    cudaError_t e = rc ? cudaSuccess : upload_padded(dcodes, codes, (size_t)n, (size_t)M, (size_t)ds->d.code_stride);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    CK(e, "pq self magnitudes");
+    if (rc) return rc;
+    CK(e, "upload pq");
     *out = ds.release();
+    return JV_OK;
+}
+
+int jv_dataset_pq_download(jv_dataset pq, uint8_t *codes_out, float *codebooks_out, float *centroid_out)
+{
+    ON_DEVICE_OF(pq);
+    if (pq->d.kind != KIND_PQ) return fail(JV_ERR_INVALID, "dataset_pq_download: not a PQ data set");
+    if (centroid_out && !pq->d.centroid) return fail(JV_ERR_INVALID, "dataset_pq_download: the data set has no centroid");
+    const DataDesc &d = pq->d;
+    cudaError_t e = cudaSuccess;
+    if (codes_out) e = cudaMemcpy2D(codes_out, (size_t)d.M, d.codes, (size_t)d.code_stride, (size_t)d.M, (size_t)d.n, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && codebooks_out) e = cudaMemcpy(codebooks_out, d.codebooks, (size_t)d.k * d.dim * 4, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && centroid_out) e = cudaMemcpy(centroid_out, d.centroid, (size_t)d.dim * 4, cudaMemcpyDeviceToHost);
+    CK(e, "D2H pq");
     return JV_OK;
 }
 
@@ -933,6 +958,40 @@ int jv_pq_encode_dataset_anisotropic(jv_dataset f32, int M, int k, const float *
     return pq_encode_dataset_entry(f32, M, k, codebooks, centroid, codes_out, anisotropic_threshold, stats);
 }
 
+// the resident rows of f32 encoded (ProductQuantization.encodeAll) into a new resident PQ data set on `s`, no host round trip
+// (returns once the stream has drained):
+// pq_encode_kernel writes packed [n][M] rows, copied into the data set's [n][code_stride] rows when M is not a multiple of 4
+static int pq_encode_resident(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, cudaStream_t s,
+                              std::unique_ptr<jv_dataset_s> &ds)
+{
+    const int64_t n = f32->d.n;
+    uint8_t *codes;
+    int rc = pq_dataset(n, f32->d.dim, M, k, codebooks, centroid, s, ds, &codes);
+    if (rc) return rc;
+    const int stride = ds->d.code_stride;
+    DeviceBuffer packed;
+    if (stride != M) {
+        CK(packed.alloc((size_t)n * M), "cudaMalloc(packed codes)");
+        CK(cudaMemsetAsync(codes, 0, (size_t)n * stride, s), "memset codes");
+    }
+    CK(launch_pq_encode(ds->d, f32->d.rows, n, f32->d.stride, stride != M ? packed.get<uint8_t>() : codes, s), "pq_encode");
+    if (stride != M) CK(cudaMemcpy2DAsync(codes, stride, packed.get(), M, M, n, cudaMemcpyDeviceToDevice, s), "pad codes");
+    CK(cudaStreamSynchronize(s), "pq_encode_resident");  // `packed` goes on return
+    return JV_OK;
+}
+
+int jv_pq_encode_dataset_resident(jv_dataset f32, int M, int k, const float *codebooks, const float *centroid, jv_dataset *out)
+{
+    ON_DEVICE_OF(f32);
+    if (f32->d.kind != KIND_F32 || !codebooks || !out || M <= 0 || M > f32->d.dim || k <= 0 || k > 256)
+        return fail(JV_ERR_INVALID, "pq_encode_dataset_resident: bad arguments");
+    int rc;
+    std::unique_ptr<jv_dataset_s> ds;
+    if ((rc = t_ctx.init()) || (rc = pq_encode_resident(f32, M, k, codebooks, centroid, t_ctx.stream, ds))) return rc;
+    *out = ds.release();
+    return JV_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ PQ training
 constexpr int64_t MAX_PQ_TRAINING_SET_SIZE = 128000;  // ProductQuantization.java:64
 
@@ -1164,22 +1223,28 @@ int jv_graph_add_level(jv_graph g, int32_t count, const int32_t *node_ids, const
     return g->set_levels(std::move(ids), std::move(rows), g->g.entry_node);
 }
 
+// g's FusedPQ records packed from pq, enqueued on `s` (the caller synchronises before g is searched)
+static int fuse_pq(jv_graph g, jv_dataset pq, cudaStream_t s)
+{
+    const int rec = (g->g.degree * (4 + pq->d.code_stride) + 15) & ~15;
+    g->g.fused = nullptr;
+    CK(g->fused.alloc((size_t)g->g.n * rec), "cudaMalloc(fused records)");
+    CK(launch_fuse_pq(g->g, pq->d, g->fused.get<uint8_t>(), rec, s), "fuse_pq");
+    g->g.fused = g->fused.get<uint8_t>();
+    g->g.fused_codes_of = pq->d.codes;
+    g->g.fused_rec = rec;
+    g->g.fused_code_stride = pq->d.code_stride;
+    return JV_OK;
+}
+
 int jv_graph_fuse_pq(jv_graph g, jv_dataset pq)
 {
     ON_DEVICE_OF(g);
     if (!pq || pq->d.kind != KIND_PQ) return fail(JV_ERR_INVALID, "graph_fuse_pq: needs a PQ data set");
     if (pq->device != g->device || pq->d.n != g->g.n) return fail(JV_ERR_INVALID, "graph_fuse_pq: data set and graph differ in device or size");
     int rc;
-    if ((rc = t_ctx.init())) return rc;
-    const int rec = (g->g.degree * (4 + pq->d.code_stride) + 15) & ~15;
-    g->g.fused = nullptr;
-    CK(g->fused.alloc((size_t)g->g.n * rec), "cudaMalloc(fused records)");
-    CK(launch_fuse_pq(g->g, pq->d, g->fused.get<uint8_t>(), rec, t_ctx.stream), "fuse_pq");
+    if ((rc = t_ctx.init()) || (rc = fuse_pq(g, pq, t_ctx.stream))) return rc;
     CK(cudaStreamSynchronize(t_ctx.stream), "fuse_pq");
-    g->g.fused = g->fused.get<uint8_t>();
-    g->g.fused_codes_of = pq->d.codes;
-    g->g.fused_rec = rec;
-    g->g.fused_code_stride = pq->d.code_stride;
     return JV_OK;
 }
 
@@ -2443,13 +2508,16 @@ int jv_graph_remove_deleted_bq(jv_graph g, jv_dataset bq, int metric, float alph
 struct CompactSource {
     jv_graph g;
     jv_dataset ds;
+    jv_dataset pq = nullptr;  // the fused form (jv_graph_compact_pq): the source's codes, which its searches walk (ds reranks)
     std::vector<int32_t> map;
     std::vector<std::vector<int32_t>> live, live_row;
 };
 
 // source t's level L (>= 1) and everything above it as a graph of its own: node p is t's p-th member of level L, its rows are the
-// members' rows (gathered on `s`); the search of it descends from t's entry exactly as a search of t would down to level L
-static int compact_sub_hierarchy(const CompactSource &t, int L, std::unique_ptr<jv_graph_s> &sg, std::unique_ptr<jv_dataset_s> &sd, cudaStream_t s)
+// members' rows (gathered on `s`) and, when t.pq is set, sp holds their code rows (t.pq's codebooks, centroid and magnitudes; the
+// graph has no FusedPQ records); the search of it descends from t's entry exactly as a search of t would down to level L
+static int compact_sub_hierarchy(const CompactSource &t, int L, std::unique_ptr<jv_graph_s> &sg, std::unique_ptr<jv_dataset_s> &sd,
+                                 std::unique_ptr<jv_dataset_s> &sp, cudaStream_t s)
 {
     const jv_graph_s &g = *t.g;
     const std::vector<int32_t> &ids = g.level_ids[L - 1];
@@ -2468,6 +2536,15 @@ static int compact_sub_hierarchy(const CompactSource &t, int L, std::unique_ptr<
     if (rc || (rc = sd->alloc(&dids, (size_t)m * 4))) return rc;
     CK(cudaMemcpyAsync(dids, ids.data(), (size_t)m * 4, cudaMemcpyHostToDevice, s), "H2D members");
     CK(launch_gather_rows(t.ds->d, dids, m, rows, s), "gather member rows");
+    if (t.pq) {
+        sp.reset(new jv_dataset_s(KIND_PQ, m, t.pq->d.dim));
+        sp->d = t.pq->d;
+        sp->d.n = m;
+        uint8_t *codes;
+        if ((rc = sp->alloc(&codes, (size_t)m * code_row_bytes(sp->d)))) return rc;
+        CK(launch_gather_codes(t.pq->d, dids, m, codes, s), "gather member codes");
+        sp->d.codes = codes;
+    }
     const std::vector<int32_t> adj = remap(g.level_adj[L - 1]);
     if ((rc = jv_graph_s::create(m, degree, sg))) return rc;
     CK(cudaMemcpy(sg->adj0.get(), adj.data(), adj.size() * 4, cudaMemcpyHostToDevice), "H2D sub-hierarchy");
@@ -2480,20 +2557,23 @@ static int compact_sub_hierarchy(const CompactSource &t, int L, std::unique_ptr<
 }
 
 // the searchTopK best live members of source t at level `level` for every row of the level that belongs to another source, into
-// res [queries][K] (t's node ids, or member positions above level 0). qids: the queries' new ids (their rows in `merged`)
+// res [queries][K] (t's node ids, or member positions above level 0). qids: the queries' new ids (their rows in `merged`). The
+// search walks t's fp32 rows exactly, or, when t.pq is set, t's codes (its FusedPQ records at level 0) with an exact rerank of
+// its K survivors over t's rows (OnDiskGraphIndexCompactor.buildCrossSourceScoreProvider)
 static int compact_search(const CompactSource &t, int level, jv_dataset merged, int metric, int K, const std::vector<int32_t> &qids, int32_t *res,
                           jv_compact_stats *stats, cudaStream_t s)
 {
     constexpr int QUERY_CHUNK = 1 << 18;  // queries per search call: bounds the search's scratch and the gathered query rows
     std::unique_ptr<jv_graph_s> sg;
-    std::unique_ptr<jv_dataset_s> sd;
+    std::unique_ptr<jv_dataset_s> sd, sp;
     jv_graph g = t.g;
-    jv_dataset ds = t.ds;
+    jv_dataset ds = t.ds, pq = t.pq;
     int rc;
     if (level > 0) {
-        if ((rc = compact_sub_hierarchy(t, level, sg, sd, s))) return rc;
+        if ((rc = compact_sub_hierarchy(t, level, sg, sd, sp, s))) return rc;
         g = sg.get();
         ds = sd.get();
+        pq = sp.get();
     }
     // accept bits: the live nodes of the searched graph (acceptOrds = live_t)
     const int n = g->g.n;
@@ -2520,7 +2600,7 @@ static int compact_search(const CompactSource &t, int level, jv_dataset merged, 
         const int c = std::min(chunk, nq - q0);
         CK(launch_gather_rows(merged->d, dq + q0, c, qrows, s), "gather query rows");
         jv_search_stats st;
-        if ((rc = search_device(g, ds, nullptr, metric, qrows, c, K, K, &f, res + (size_t)q0 * K, scores, &st, stride))) return rc;
+        if ((rc = search_device(g, pq ? pq : ds, pq ? ds : nullptr, metric, qrows, c, K, K, &f, res + (size_t)q0 * K, scores, &st, stride))) return rc;
         stats->searches += c;
         stats->visited += st.visited;
     }
@@ -2648,10 +2728,11 @@ static int compact_level(const std::vector<CompactSource> &src, int level, int K
     return rc;
 }
 
-int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric, float alpha, jv_graph *graph_out, jv_dataset *rows_out,
-                     jv_compact_stats *stats)
+// jv_graph_compact's checks, all on the host: every refusal comes before any device work. Fills src (maps and live members per
+// level), the live total, the level count and searchTopK.
+static int compact_prepare(const jv_compact_source *sources, int nsources, int metric, float alpha, std::vector<CompactSource> &src, long long *total_out,
+                           int *levels_out, int *K_out)
 {
-    if (!sources || nsources < 1 || !graph_out || !rows_out || !stats) return fail(JV_ERR_INVALID, "graph_compact: null argument or no source");
     for (int i = 0; i < nsources; i++)
         if (!sources[i].graph || !sources[i].rows || !sources[i].old_to_new) return fail(JV_ERR_INVALID, "graph_compact: null argument");
     ON_DEVICE_OF(sources[0].graph);
@@ -2667,7 +2748,7 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
     if (rc) return rc;
     if (!(alpha >= 1.0f)) return fail(JV_ERR_INVALID, "graph_compact: need alpha >= 1");
     // the live nodes (holes are dead) and their new ids, which must be exactly [0, live nodes)
-    std::vector<CompactSource> src(S);
+    src.assign(S, CompactSource());
     long long total = 0;
     int levels = 0;
     for (int i = 0; i < S; i++) {
@@ -2711,13 +2792,24 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
             }
         }
     }
+    *total_out = total;
+    *levels_out = levels;
+    *K_out = K;
+    return JV_OK;
+}
+
+// the merge itself on the device, for the sources compact_prepare accepted: the new graph and its fp32 rows into ng / nd
+static int compact_merge(const std::vector<CompactSource> &src, int metric, float alpha, long long total, int levels, int K,
+                         std::unique_ptr<jv_graph_s> &ng, std::unique_ptr<jv_dataset_s> &nd, jv_compact_stats *stats)
+{
+    const int S = (int)src.size(), degree = src[0].g->g.degree, dim = src[0].ds->d.dim;
+    int rc;
     if ((rc = t_ctx.init())) return rc;
     cudaStream_t s = t_ctx.stream;
     memset(stats, 0, sizeof(*stats));
-    std::unique_ptr<jv_dataset_s> nd(new jv_dataset_s(KIND_F32, total, dim));
+    nd.reset(new jv_dataset_s(KIND_F32, total, dim));
     float *rows = nullptr;
     if ((rc = nd->alloc_rows(&rows))) return rc;
-    std::unique_ptr<jv_graph_s> ng;
     if ((rc = jv_graph_s::create((int32_t)total, degree, ng))) return rc;
     StreamTimer timer;
     CK(timer.start(s), "event");
@@ -2771,8 +2863,164 @@ int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric,
     stats->nodes = (int32_t)total;
     stats->levels = ng->g.levels;
     stats->device_ms = timer.ms();
+    return JV_OK;
+}
+
+int jv_graph_compact(const jv_compact_source *sources, int nsources, int metric, float alpha, jv_graph *graph_out, jv_dataset *rows_out,
+                     jv_compact_stats *stats)
+{
+    if (!sources || nsources < 1 || !graph_out || !rows_out || !stats) return fail(JV_ERR_INVALID, "graph_compact: null argument or no source");
+    std::vector<CompactSource> src;
+    long long total;
+    int levels, K, rc;
+    if ((rc = compact_prepare(sources, nsources, metric, alpha, src, &total, &levels, &K))) return rc;
+    std::unique_ptr<jv_graph_s> ng;
+    std::unique_ptr<jv_dataset_s> nd;
+    if ((rc = compact_merge(src, metric, alpha, total, levels, K, ng, nd, stats))) return rc;
     *graph_out = ng.release();
     *rows_out = nd.release();
+    return JV_OK;
+}
+
+// PQRetrainer.sampleBalanced (PQRetrainer.java:127-212) over the sources' live nodes, with counter_random in place of
+// ThreadLocalRandom: per source its sampled node ids, ascending. Every live node when there are at most 128 000; otherwise each
+// source's quota (at least min(1000, 128 000 / S), else its share of 128 000, normalised to 128 000 in total) is filled from its
+// 32-node chunks in a Fisher-Yates order, each chunk's live nodes ascending. A source short of its quota gives what it has.
+static std::vector<std::vector<int32_t>> retrain_sample(const std::vector<CompactSource> &src, uint64_t seed)
+{
+    constexpr long long MIN_SAMPLES_PER_SOURCE = 1000;
+    constexpr int SAMPLE_CHUNK_SIZE = 32;
+    const int S = (int)src.size();
+    const long long cap = MAX_PQ_TRAINING_SET_SIZE;
+    std::vector<std::vector<int32_t>> out(S);
+    long long total = 0;
+    for (const CompactSource &c : src) total += (long long)c.live[0].size();
+    if (total <= cap) {
+        for (int s = 0; s < S; s++) out[s] = src[s].live[0];  // level 0's live members, ascending
+        return out;
+    }
+    const long long min_per = std::min(MIN_SAMPLES_PER_SOURCE, cap / S);
+    std::vector<long long> quota(S);
+    long long assigned = 0;
+    for (int s = 0; s < S; s++) {
+        quota[s] = std::max(min_per, cap * (long long)src[s].live[0].size() / total);
+        assigned += quota[s];
+    }
+    while (assigned > cap)
+        for (int s = 0; s < S && assigned > cap; s++)
+            if (quota[s] > min_per) {
+                quota[s]--;
+                assigned--;
+            }
+    while (assigned < cap)
+        for (int s = 0; s < S && assigned < cap; s++) {
+            quota[s]++;
+            assigned++;
+        }
+    for (int s = 0; s < S; s++) {
+        const CompactSource &c = src[s];
+        const int n = c.g->g.n, chunks = (n + SAMPLE_CHUNK_SIZE - 1) / SAMPLE_CHUNK_SIZE;
+        std::vector<int> order(chunks);
+        for (int i = 0; i < chunks; i++) order[i] = i;
+        for (int i = chunks - 1; i > 0; i--) std::swap(order[i], order[counter_random(seed, TAG_COMPACT_SAMPLE, s, i) % (uint64_t)(i + 1)]);
+        long long count = 0;
+        for (int ci = 0; ci < chunks && count < quota[s]; ci++) {
+            const int start = order[ci] * SAMPLE_CHUNK_SIZE, end = std::min(n, start + SAMPLE_CHUNK_SIZE);
+            for (int v = start; v < end && count < quota[s]; v++)
+                if (c.map[v] >= 0) {
+                    out[s].push_back(v);
+                    count++;
+                }
+        }
+        std::sort(out[s].begin(), out[s].end());
+    }
+    return out;
+}
+
+int jv_graph_compact_pq(const jv_compact_source *sources, const jv_dataset *source_pq, int nsources, int metric, float alpha, uint64_t seed,
+                        jv_graph *graph_out, jv_dataset *rows_out, jv_dataset *pq_out, float *codebooks_out, float *centroid_out,
+                        int64_t *samples_per_source_out, jv_compact_pq_stats *stats)
+{
+    if (!sources || !source_pq || nsources < 1 || !graph_out || !rows_out || !pq_out || !codebooks_out || !stats)
+        return fail(JV_ERR_INVALID, "graph_compact_pq: null argument or no source");
+    for (int i = 0; i < nsources; i++)
+        if (!source_pq[i]) return fail(JV_ERR_INVALID, "graph_compact_pq: null argument");
+    std::vector<CompactSource> src;
+    long long total;
+    int levels, K, rc;
+    if ((rc = compact_prepare(sources, nsources, metric, alpha, src, &total, &levels, &K))) return rc;
+    const int S = nsources, dim = sources[0].rows->d.dim;
+    // the form: every source's FusedPQ records packed from its own codes (fused), or no records at all (sidecar)
+    int fused = 0, plain = 0;
+    for (int i = 0; i < S; i++) {
+        const jv_dataset pq = source_pq[i];
+        const GraphDesc &g = sources[i].graph->g;
+        if (pq->d.kind != KIND_PQ) return fail(JV_ERR_INVALID, "graph_compact_pq: source_pq must hold PQ codes");
+        if (pq->d.n != g.n || pq->d.dim != dim || pq->device != t_active)
+            return fail(JV_ERR_INVALID, "graph_compact_pq: a source's codes differ from its graph in size, dim or device");
+        if (!g.fused) plain++;
+        else if (g.fused_codes_of == pq->d.codes && g.fused_code_stride == pq->d.code_stride) fused++;
+    }
+    if (fused != S && plain != S)
+        return fail(JV_ERR_INVALID, "graph_compact_pq: either every source carries FusedPQ records packed from its own codes, or none carries records");
+    const DataDesc &p0 = source_pq[0]->d;
+    if (p0.centroid && !centroid_out) return fail(JV_ERR_INVALID, "graph_compact_pq: source 0's PQ has a centroid: need centroid_out");
+    const std::vector<std::vector<int32_t>> sample = retrain_sample(src, seed);
+    long long train_rows = 0;
+    for (const std::vector<int32_t> &x : sample) train_rows += (long long)x.size();
+    if (train_rows < p0.k) return fail(JV_ERR_INVALID, "graph_compact_pq: fewer training rows than clusters");
+    if (fused == S)
+        for (int i = 0; i < S; i++) src[i].pq = source_pq[i];
+    jv_compact_pq_stats st;
+    memset(&st, 0, sizeof(st));
+    st.fused = fused == S;
+    st.train_rows = train_rows;
+    std::unique_ptr<jv_graph_s> ng;
+    std::unique_ptr<jv_dataset_s> nd, np, tr;
+    if ((rc = compact_merge(src, metric, alpha, total, levels, K, ng, nd, &st.graph))) return rc;
+    cudaStream_t s = t_ctx.stream;
+    // retraining (PQRetrainer.retrain): source 0's codebooks refined by 6 unweighted Lloyd rounds over the sample, gathered source by
+    // source into one fp32 data set in (source, node) order
+    std::vector<float> cb0((size_t)p0.k * dim), cen0(p0.centroid ? dim : 0);
+    CK(cudaMemcpy(cb0.data(), p0.codebooks, cb0.size() * 4, cudaMemcpyDeviceToHost), "D2H source 0's codebooks");
+    if (p0.centroid) CK(cudaMemcpy(cen0.data(), p0.centroid, cen0.size() * 4, cudaMemcpyDeviceToHost), "D2H source 0's centroid");
+    const float *cen = p0.centroid ? cen0.data() : nullptr;
+    tr.reset(new jv_dataset_s(KIND_F32, train_rows, dim));
+    float *trows;
+    if ((rc = tr->alloc_rows(&trows))) return rc;
+    std::vector<int32_t> ids;
+    for (const std::vector<int32_t> &x : sample) ids.insert(ids.end(), x.begin(), x.end());
+    DeviceBuffer dids;
+    CK(dids.alloc(ids.size() * 4), "cudaMalloc(sample ids)");
+    StreamTimer t_train, t_encode, t_fuse;
+    CK(t_train.start(s), "event");
+    CK(cudaMemcpyAsync(dids.get(), ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, s), "H2D sample ids");
+    for (int i = 0, off = 0; i < S; off += (int)sample[i].size(), i++)
+        CK(launch_gather_rows(src[i].ds->d, dids.get<int32_t>() + off, (int)sample[i].size(), trows + (size_t)off * tr->d.stride, s), "gather sample");
+    const jv_pq_train_params tp = {p0.M, p0.k, 0, 6 /* K_MEANS_ITERATIONS */, MAX_PQ_TRAINING_SET_SIZE, seed};
+    rc = pq_train_impl(tr.get(), &tp, cb0.data(), cen, codebooks_out, nullptr, &st.train);
+    CK(t_train.stop(s), "event");
+    if (rc) return rc;
+    // the merged rows encoded with the new codebooks, and (fused form) the merged graph's records packed from them
+    CK(t_encode.start(s), "event");
+    if ((rc = pq_encode_resident(nd.get(), p0.M, p0.k, codebooks_out, cen, s, np))) return rc;
+    CK(t_encode.stop(s), "event");
+    if (st.fused) {
+        CK(t_fuse.start(s), "event");
+        if ((rc = fuse_pq(ng.get(), np.get(), s))) return rc;
+        CK(t_fuse.stop(s), "event");
+    }
+    CK(cudaStreamSynchronize(s), "graph_compact_pq");
+    st.retrain_ms = t_train.ms();
+    st.encode_ms = t_encode.ms();
+    st.fuse_ms = st.fused ? t_fuse.ms() : 0.0;
+    if (cen) std::copy(cen0.begin(), cen0.end(), centroid_out);
+    if (samples_per_source_out)
+        for (int i = 0; i < S; i++) samples_per_source_out[i] = (int64_t)sample[i].size();
+    *stats = st;
+    *graph_out = ng.release();
+    *rows_out = nd.release();
+    *pq_out = np.release();
     return JV_OK;
 }
 

@@ -187,7 +187,8 @@ __host__ __device__ __forceinline__ int next_pow2(int v)
 }
 
 // The library's counter-based generator: a pure function of (seed, a, b, c), so a draw does not depend on thread order.
-// Callers: the removal's random fallback (seed, level, node, attempt) and PQ training (pq_train.cu).
+// Callers: the removal's random fallback (seed, level, node, attempt), PQ training (pq_train.cu) and the compaction's retraining
+// sample (seed, TAG_COMPACT_SAMPLE, source, chunk).
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x)
 {
     x += 0x9E3779B97F4A7C15ull;
@@ -199,6 +200,9 @@ __host__ __device__ __forceinline__ uint64_t counter_random(uint64_t seed, int a
 {
     return mix64(mix64(mix64(seed ^ (uint64_t)(uint32_t)a) ^ (uint64_t)(uint32_t)b) ^ (uint64_t)(uint32_t)c);
 }
+// first counter of the compaction's chunk shuffle (PQRetrainer.sampleBalanced): no PQ-training draw uses it (those take a
+// sub-space < 2^29, sub-space | 0x20000000 or | 0x40000000, or 0x7fffffff) and the removal's fallback takes a level
+constexpr int TAG_COMPACT_SAMPLE = 0x7ffffffe;
 
 // -ln(u) for u in (0, 1] as a fixed sequence of round-to-nearest fp32 operations (no log intrinsic, no FMA), so a host model
 // repeats it bit for bit: u = m 2^e with m in [sqrt(1/2), sqrt(2)], ln m = 2 s (1 + z/3 + z^2/5 + z^3/7 + z^4/9) with

@@ -3,13 +3,20 @@
 
   python tools/compact_bench.py                          # 1M x 768 latent rows in 4 segments of 250k, DOT_PRODUCT, 10 % dead
   python tools/compact_bench.py --n 40000 --nq 1000      # a smaller world for a rehearsal
+  python tools/compact_bench.py --pq fused               # segments with PQ of their own, FusedPQ records (jv_graph_compact_pq)
+  python tools/compact_bench.py --pq sidecar             # the same codes beside the graphs instead of inside them
 
 Every segment is built with M = 32, beam 100 and hierarchy; 10 % of each segment's nodes are dead (a fixed seed). It reports the
 compaction's device time and counters, the device time of its kernels by part (graph_search_kernel: the cross-segment searches;
 compact_assemble_kernel: the candidate assembly; prune_*: the prune; the rest: row gathers and scatters) from a second, profiled
 call, the device time of a fresh build over the live rows, both graphs' recall@10 at rerankK 100 against brute force over the live
 rows, and the ratio of compaction to rebuild time. One JSON line on stdout, with the card's name and power limit read in the same
-run."""
+run.
+
+With --pq every segment also gets a PQ of its own (ProductQuantization.compute, --pq-m sub-spaces, 256 clusters), fused into its graph
+for --pq fused. The compaction then retrains PQ and encodes the merged rows (and fuses the merged graph): retrain, encode and fuse are
+reported beside the merge's parts, and recall is that of the c3-shaped search (the fused PQ walk with an fp32 rerank for --pq fused, a
+plain PQ walk with the rerank for --pq sidecar) on the merged graph and on a fresh build with a fresh PQ of the live rows."""
 import argparse
 import json
 import os
@@ -42,12 +49,14 @@ def kernel_ms(torch, fn):
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
         torch.cuda.synchronize()
-    parts = {"search": 0.0, "assembly": 0.0, "prune": 0.0, "other": 0.0}
+    parts = {"search": 0.0, "assembly": 0.0, "prune": 0.0, "retrain": 0.0, "encode": 0.0, "fuse": 0.0, "other": 0.0}
     for ev in prof.key_averages():
         t = getattr(ev, "device_time_total", getattr(ev, "cuda_time_total", 0.0)) / 1000.0
         if ev.key.startswith("cuda") or ev.key.startswith("Memcpy") or ev.key.startswith("Memset") or t == 0:
             continue
-        key = "search" if "graph_search_kernel" in ev.key else "assembly" if "compact_assemble" in ev.key else "prune" if "prune" in ev.key else "other"
+        k = ev.key
+        key = ("search" if "graph_search_kernel" in k else "assembly" if "compact_assemble" in k else "prune" if "prune" in k
+               else "encode" if ("pq_encode" in k or "pq_self" in k) else "fuse" if "fuse_pq" in k else "retrain" if "pq_train" in k else "other")
         parts[key] += t
     return parts
 
@@ -59,6 +68,8 @@ def main():
     ap.add_argument("--segments", type=int, default=4)
     ap.add_argument("--nq", type=int, default=10000)
     ap.add_argument("--dead", type=float, default=0.1)
+    ap.add_argument("--pq", choices=["fused", "sidecar"], default=None)
+    ap.add_argument("--pq-m", type=int, default=96)
     a = ap.parse_args()
     import torch
 
@@ -72,33 +83,55 @@ def main():
     rng = np.random.default_rng(SEED + 5)
     parts = np.array_split(np.arange(a.n), a.segments)
     sources, live, seg_ms = [], [], []
-    for p in parts:
+    for i, p in enumerate(parts):
         vec = jv.F32Vectors(np.ascontiguousarray(host[p]))
         b = jv.GraphIndexBuilder(DOT, **kw)
-        sources.append((b.build(vec), vec))
+        g = b.build(vec)
         seg_ms.append(b.device_ms)
+        if a.pq:
+            pqv = jv.ProductQuantization.compute(vec, a.pq_m, 256, seed=SEED + i).encodeAll(vec)
+            if a.pq == "fused":
+                g.fuse_pq(pqv)
+            sources.append((g, vec, pqv))
+        else:
+            sources.append((g, vec))
         live.append(rng.random(len(p)) >= a.dead)
     keep = np.concatenate([p[m] for p, m in zip(parts, live)])  # new id i = row keep[i]
     comp = jv.GraphIndexCompactor(sources, live, None, DOT)
-    merged, rows = comp.compact()
+    out_handles = comp.compact()
+    merged, rows = out_handles[:2]
+    codes = out_handles[2] if a.pq else None
     stats = dict(comp.stats)
     again = jv.GraphIndexCompactor(sources, live, None, DOT)
     by_part = kernel_ms(torch, lambda: [h.close() for h in again.compact()])
     sub = jv.F32Vectors(np.ascontiguousarray(host[keep]))
     fb = jv.GraphIndexBuilder(DOT, **kw)
     fresh = fb.build(sub)
+    fresh_ms = fb.device_ms
+    fresh_pq = None
+    if a.pq:
+        pq = jv.ProductQuantization.compute(sub, a.pq_m, 256, seed=SEED)
+        fresh_pq = pq.encodeAll(sub)
+        if a.pq == "fused":
+            fresh.fuse_pq(fresh_pq)
     truth, _, _ = jv.topk_bruteforce(sub, DOT, queries, 10)
-    rm = jv.GraphSearcher(merged).search(rows, queries, DOT, 10, 100)
-    rf = jv.GraphSearcher(fresh).search(sub, queries, DOT, 10, 100)
+    if a.pq:
+        rm = jv.GraphSearcher(merged).search(codes, queries, DOT, 10, 100, reranker=rows)
+        rf = jv.GraphSearcher(fresh).search(fresh_pq, queries, DOT, 10, 100, reranker=sub)
+    else:
+        rm = jv.GraphSearcher(merged).search(rows, queries, DOT, 10, 100)
+        rf = jv.GraphSearcher(fresh).search(sub, queries, DOT, 10, 100)
+    total_ms = stats["device_ms"] + stats.get("retrain_ms", 0.0) + stats.get("encode_ms", 0.0) + stats.get("fuse_ms", 0.0)
     out = {"world": {"n": a.n, "dim": a.dim, "segments": a.segments, "metric": "DOT_PRODUCT", "M": 32, "beam": 100, "hierarchy": True,
-                     "dead_fraction": a.dead, "live": int(len(keep)), "nq": a.nq, "rerankK": 100, "segment_build_ms": seg_ms},
+                     "dead_fraction": a.dead, "live": int(len(keep)), "nq": a.nq, "rerankK": 100, "segment_build_ms": seg_ms,
+                     "pq": a.pq, "pq_m": a.pq_m if a.pq else None},
            "card": card(),
-           "compact": stats, "compact_kernel_ms_by_part": by_part, "fresh_build_ms": fb.device_ms,
-           "compact_over_fresh_build": stats["device_ms"] / fb.device_ms if fb.device_ms else None,
+           "compact": stats, "compact_total_ms": total_ms, "compact_kernel_ms_by_part": by_part, "fresh_build_ms": fresh_ms,
+           "compact_over_fresh_build": total_ms / fresh_ms if fresh_ms else None,
            "recall10": {"compacted": recall(rm.nodes, truth), "fresh": recall(rf.nodes, truth)},
            "visited_per_query": {"compacted": rm.visitedCount / a.nq, "fresh": rf.visitedCount / a.nq}}
     print(json.dumps(out))
-    for h in [merged, rows, fresh, sub] + [x for s in sources for x in s]:
+    for h in [merged, rows, fresh, sub] + ([codes, fresh_pq] if a.pq else []) + [x for s in sources for x in s]:
         h.close()
 
 
