@@ -134,6 +134,10 @@ JV_API int jv_dataset_lowrank_download(jv_dataset f32, float *basis_out, uint8_t
 JV_API int jv_graph_edge_records_download(jv_graph g, uint8_t *out);
 /* New neighbours the calling thread's last graph search settled on edge records (they are part of jv_search_stats.visited). */
 JV_API int64_t jv_search_last_settled(void);
+/* Of those that the calling thread's last graph search did not settle on edge records: how many it sent straight to their full row,
+   skipping the row sketch, on the records' point estimate (*routed), and how many of these the candidate list then refused
+   (*routed_dropped). Either pointer may be NULL. */
+JV_API void jv_search_last_direct(int64_t *routed, int64_t *routed_dropped);
 /* The low-rank bound as a DOT_PRODUCT score of rows[i] against queries[i] (both [n][dim]) for basis [dim][32] (column j = basis
    vector j), computed by the device functions the search uses; records_out (may be NULL): the rows' [n][48]-byte records. */
 JV_API int jv_lowrank_bound_pairs(const float *basis, int dim, const float *rows, const float *queries, int64_t n, uint8_t *records_out, float *bounds_out);

@@ -114,6 +114,7 @@ SYMBOLS = [
     ("jv_dataset_lowrank_download", _I, [_P, f32p, _P, C.POINTER(_I)]),
     ("jv_graph_edge_records_download", _I, [_P, _P]),
     ("jv_search_last_settled", _L, []),
+    ("jv_search_last_direct", None, [i64p, i64p]),
     ("jv_lowrank_bound_pairs", _I, [f32p, _I, f32p, f32p, C.c_int64, _P, f32p]),
     ("jv_graph_search_exclude", _I, [_P, _P, _I, f32p, _I, _I, _I, i32p, i32p, f32p, i64p]),
     ("jv_dataset_pq_pair_table", _I, [_P, _I]), ("jv_dataset_pq_pair_table_download", _I, [_P, _I, f32p]),

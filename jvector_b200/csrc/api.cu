@@ -1309,6 +1309,12 @@ int jv_dataset_row_sketch_download(jv_dataset f32, int8_t *codes_out, float *met
 
 static thread_local int64_t t_last_settled = 0;
 int64_t jv_search_last_settled(void) { return t_last_settled; }
+static thread_local int64_t t_last_direct[2] = {0, 0};
+void jv_search_last_direct(int64_t *routed, int64_t *routed_dropped)
+{
+    if (routed) *routed = t_last_direct[0];
+    if (routed_dropped) *routed_dropped = t_last_direct[1];
+}
 
 int jv_lowrank_bound_pairs(const float *basis, int dim, const float *rows, const float *queries, int64_t n, uint8_t *records_out, float *bounds_out)
 {
@@ -1607,6 +1613,8 @@ static int search_device(jv_graph g, jv_dataset approx, jv_dataset reranker, int
         stats->reranked = (int64_t)hc.reranked;
     }
     t_last_settled = (int64_t)hc.settled;
+    t_last_direct[0] = (int64_t)hc.direct;
+    t_last_direct[1] = (int64_t)hc.direct_dropped;
     if (stats) {
         stats->retried = retried;
         stats->device_ms = ms;

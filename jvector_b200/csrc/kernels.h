@@ -52,6 +52,7 @@ struct GraphDesc {
 struct SearchCounters {  // device-side totals
     unsigned long long visited, expanded, expanded_base, reranked, overflowed;
     unsigned long long settled;  // new neighbours settled on their edge record (part of `visited`)
+    unsigned long long direct, direct_dropped;  // new neighbours routed direct to their full row, and of them those the list refused
 };
 
 // ---- kernels_batch.cu ----

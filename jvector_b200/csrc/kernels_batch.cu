@@ -919,7 +919,8 @@ __global__ void __launch_bounds__(128) lowrank_bound_pairs_kernel(DataDesc d, co
     prepare_lowrank<128>(d.lr_basis, d.stride, pair_blob, lr);
     if (threadIdx.x == 0) {
         const uint4 *e = reinterpret_cast<const uint4 *>(records + i * LR_SLOT);
-        out[i] = lowrank_bound(d, pair_blob, lr, e[0], e[1], *reinterpret_cast<const float4 *>(e + 2));
+        float est;
+        out[i] = lowrank_bound(d, pair_blob, lr, e[0], e[1], *reinterpret_cast<const float4 *>(e + 2), est);
     }
 }
 

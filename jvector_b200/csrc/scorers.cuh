@@ -424,8 +424,9 @@ __device__ __noinline__ void prepare_lowrank(const float *basis, int stride, con
 }
 
 // the bound of one row from its 48-byte slot (codes in c0, c1; {t, rho, beta, xn} in m), as a DOT_PRODUCT score (score_map is
-// monotone, so it stays >= score_f32's). Returns +inf when the bound is not finite.
-__device__ __forceinline__ float lowrank_bound(const DataDesc &d, const float *blob, const float *lr, uint4 c0, uint4 c1, float4 m)
+// monotone, so it stays >= score_f32's). Returns +inf when the bound is not finite. est = score_map(t fl(u . c)), the bound's point
+// estimate of the score before its slack terms: no bound in either direction, only a guess at which side of a cut the row falls.
+__device__ __forceinline__ float lowrank_bound(const DataDesc &d, const float *blob, const float *lr, uint4 c0, uint4 c1, float4 m, float &est)
 {
     const unsigned w[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
     float s = 0.f, e = 0.f;
@@ -442,6 +443,7 @@ __device__ __forceinline__ float lowrank_bound(const DataDesc &d, const float *b
     rest = __fmaf_ru(lr[2 * LR_K + 1], m.z, rest);
     rest = __fmaf_ru(__fmul_ru(g, blob[d.stride + 1]), m.w, rest);
     const float raw = __fadd_ru(__fmul_ru(m.x, s), rest);
+    est = score_map(JV_METRIC_DOT, __fmul_rn(m.x, s));
     return raw <= 3.4028235e38f ? score_map(JV_METRIC_DOT, raw) : __int_as_float(0x7f800000);
 }
 

@@ -186,12 +186,23 @@ static int search_threads_of(int kind) { return (kind == KIND_F32 || kind == KIN
 
 // optional drop statistics of the fp32 DOT walk (tools/row_bound_stats.py: build with -DJV_ROW_BOUND_STATS); compiled out of the
 // product build. [0] level-0 rows scored, [1] of them dropped by JV_EMIT against a full list; plus a 1-in-64 sample of the drops
-// as {query, row, key of the list's last entry}
+// as {query, row, key of the list's last entry}, and a 1-in-64 sample of every row scored against a full list (the rows a sketched
+// walk bounds on their edge record, then routes or bounds on their sketch) as {query, row, last key, the row's exact key}
 #ifdef JV_ROW_BOUND_STATS
 constexpr int RBS_CAP = 1 << 20;
 struct RbsSample { int32_t q, row; long long last_key; };
-__device__ unsigned long long g_rbs_count[3];  // scored, dropped, samples taken
+struct RbsRow { int32_t q, row; long long last_key, key; };
+__device__ unsigned long long g_rbs_count[4];  // scored, dropped, drop samples taken, row samples taken
 __device__ RbsSample g_rbs_sample[RBS_CAP];
+__device__ RbsRow g_rbs_row[RBS_CAP];
+#define JV_RBS_ROW(k_, f_)                                                                                                    \
+    do {                                                                                                                      \
+        if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0 && size == LC &&                                          \
+            (((unsigned)(f_) * 2246822519u) ^ ((unsigned)qi * 3266489917u)) % 64u == 0u) {                                    \
+            const unsigned long long k_r = atomicAdd(&g_rbs_count[3], 1ull);                                                  \
+            if (k_r < RBS_CAP) g_rbs_row[k_r] = RbsRow{qi, (f_), cur[LC - 1], (k_)};                                          \
+        }                                                                                                                     \
+    } while (0)
 #define JV_RBS_SCORED(n_) do { if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0) atomicAdd(&g_rbs_count[0], (unsigned long long)(n_)); } while (0)
 #define JV_RBS_DROP(f_)                                                                                                       \
     do {                                                                                                                      \
@@ -206,7 +217,13 @@ __device__ RbsSample g_rbs_sample[RBS_CAP];
 #else
 #define JV_RBS_SCORED(n_)
 #define JV_RBS_DROP(f_)
+#define JV_RBS_ROW(k_, f_)
 #endif
+
+// Edge tier (DESIGN §4.1): a new neighbour that its edge bound does not settle is routed direct to its full row, skipping its sketch,
+// when the bound's point estimate scores more than this above the list's last entry. Only bytes depend on it, never results: a wrong
+// route reads 3 072 - 784 B more at d = 768, a missed one 784 B more, so it leans towards the sketch (tools/row_bound_stats.py).
+constexpr float EDGE_DIRECT_MARGIN = 0.002f;
 
 // flags of a list entry
 constexpr uint8_t F_EXPANDED = 1;  // popped from the candidate queue at this level
@@ -263,6 +280,8 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
     __shared__ int s_q, s_n, s_m, s_hsize, s_cnt;
     __shared__ int s_settled;  // new neighbours of this hop settled on their edge record (counted as visited, never candidates)
     __shared__ unsigned long long s_settled_total;  // over this CTA's queries (thread 0 only), added to counters->settled at exit
+    __shared__ int s_nd;  // new neighbours of this hop routed direct (edge tier): cand_ids[MAX_DEGREE - 1 - j], j < s_nd
+    __shared__ unsigned long long s_direct_total[2];  // over this CTA's queries: routed direct, of them dropped by JV_EMIT
     __shared__ float s_lr[LR_QUERY];  // the query's low-rank terms (prepare_lowrank)
     __shared__ int s_drop[2];  // best sortable score that fell off the list, double-buffered like s_posv
     __shared__ int s_posv[2];
@@ -274,7 +293,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
     const int vis_limit = 3 << (P.vis_slots_log > 2 ? P.vis_slots_log - 2 : 0);  // shared-memory table: at most 3/4 full
     int32_t *table = P.visited_tables + (size_t)blockIdx.x * P.visited_cap;
     const int degree = P.g.degree;
-    if (EDGE && tid == 0) s_settled_total = 0;
+    if (EDGE && tid == 0) { s_settled_total = 0; s_direct_total[0] = 0; s_direct_total[1] = 0; }
 
     for (;;) {
         if (tid == 0) {
@@ -294,7 +313,11 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         __syncthreads();
         const int wq = s_q;
         if (wq >= P.nq) {
-            if (EDGE && tid == 0 && s_settled_total) atomicAdd(&P.counters->settled, s_settled_total);
+            if (EDGE && tid == 0) {
+                if (s_settled_total) atomicAdd(&P.counters->settled, s_settled_total);
+                if (s_direct_total[0]) atomicAdd(&P.counters->direct, s_direct_total[0]);
+                if (s_direct_total[1]) atomicAdd(&P.counters->direct_dropped, s_direct_total[1]);
+            }
             break;
         }
         const int qi = P.query_index ? P.query_index[wq] : wq;
@@ -348,7 +371,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
             int sel = 0;
             // (the list is empty when every node an upper level expanded was refused: no entry point, nothing to walk)
             if (tid == 0) { s_posv[0] = size > 0 ? 0 : INT_MAX; s_posv[1] = INT_MAX; s_n = 0; s_m = 0; s_hsize = 0; s_drop[0] = INT_MIN; s_drop[1] = INT_MIN; s_cnt = 0; }
-            if (EDGE && tid == 0) s_settled = 0;
+            if (EDGE && tid == 0) { s_settled = 0; s_nd = 0; }
             __syncthreads();
             for (;;) {
                 const int p = s_posv[sel];  // first unexpanded entry = the top of the candidate queue
@@ -410,10 +433,19 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                             if (edge_tier) {
                                 // (the record was requested towards L2 with the adjacency row, by the speculation below one or more hops ago)
                                 const uint4 *e = reinterpret_cast<const uint4 *>(P.g.edge_rec + ((size_t)node * degree + t) * LR_SLOT);
-                                const float ub = lowrank_bound(P.approx, blobA, s_lr, __ldg(e), __ldg(e + 1), __ldg(reinterpret_cast<const float4 *>(e + 2)));
-                                if (topk_key(ub, f) < cur[LC - 1]) {
+                                float est;
+                                const float ub = lowrank_bound(P.approx, blobA, s_lr, __ldg(e), __ldg(e + 1), __ldg(reinterpret_cast<const float4 *>(e + 2)), est);
+                                const long long last = cur[LC - 1];
+                                if (topk_key(ub, f) < last) {
                                     atomicAdd(&s_settled, 1);
                                     atomicMax(&s_drop[sel], float_to_sortable(ub));
+                                    continue;
+                                }
+                                if (est > key_score(last) + EDGE_DIRECT_MARGIN) {
+                                    // a likely list entrant, whose sketch bound would not settle it: routed direct to its full row
+                                    const int j = atomicAdd(&s_nd, 1);
+                                    cand_ids[MAX_DEGREE - 1 - j] = f;
+                                    bulk_prefetch_l2(P.approx.rows + (size_t)f * P.approx.stride, (unsigned)P.approx.stride * 4u);
                                     continue;
                                 }
                             }
@@ -506,13 +538,14 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     }
                 }
                 if (tid == 0) { s_drop[sel ^ 1] = INT_MIN; s_cnt = 0; }
-                const int n = s_n;
+                const int nd = EDGE ? s_nd : 0;  // routed direct, counted in n
+                const int n = s_n + nd;
                 table_cnt += n;
                 if (EDGE) {
                     const int ns = s_settled;
                     table_cnt += ns;
                     visited += ns;
-                    if (tid == 0) s_settled_total += (unsigned)ns;
+                    if (tid == 0) { s_settled_total += (unsigned)ns; s_direct_total[0] += (unsigned)nd; }
                 }
                 if (vsm ? (table_cnt > vis_limit || s_vfail) : (table_cnt * 2 > P.visited_cap)) {
                     if (P.lenient) truncated = true;
@@ -526,6 +559,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
 #define JV_EMIT(sc_, f_)                                                                                                            \
     do {                                                                                                                            \
         const long long key_ = topk_key((sc_), (f_));                                                                               \
+        JV_RBS_ROW(key_, f_);                                                                                                       \
         if (lvl == 0 && P.early_pf && key_ > s_nk) {                                                                                \
             if (KIND == KIND_PQ && P.g.fused) bulk_prefetch_l2(P.g.fused + (size_t)(f_) * P.g.fused_rec, (unsigned)P.g.fused_rec);  \
             else prefetch_l2(P.g.adj0 + (size_t)(f_) * degree);                                                                     \
@@ -546,13 +580,30 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     // so it is dropped on the bound, which also stands in for its score in s_drop (>= the exact one: the check after
                     // the merge stays conservative). Only the others read their full rows, scored exactly as below.
                     const bool sketched = METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && P.approx.sketch != nullptr;
-                    // two rows per warp at a time: twice the loads in flight, query fragment read once
-                    for (int i = group; i < n; i += 2 * NG) {
-                        const int32_t fa = cand_ids[i];
-                        const bool two = i + NG < n;
-                        const int32_t fb = two ? cand_ids[i + NG] : fa;
+                    // two rows per warp at a time: twice the loads in flight, query fragment read once. EDGE: one flat pair index
+                    // over both classes, so that the warps share them evenly: pairs [0, ps) read sketches first (rows i and i + ps of
+                    // cand_ids), pairs [ps, ps + pd) are the rows routed direct (from the top of cand_ids), scored exactly at once
+                    const int ns = n - nd, ps = (ns + 1) >> 1, pd = (nd + 1) >> 1;
+                    for (int i = group; i < (EDGE ? ps + pd : n); i += (EDGE ? NG : 2 * NG)) {
+                        const bool direct = EDGE && i >= ps;
+                        int32_t fa, fb;
+                        bool two;
+                        if (!EDGE) {
+                            fa = cand_ids[i];
+                            two = i + NG < n;
+                            fb = two ? cand_ids[i + NG] : fa;
+                        } else if (!direct) {
+                            fa = cand_ids[i];
+                            two = i + ps < ns;
+                            fb = two ? cand_ids[i + ps] : fa;
+                        } else {
+                            const int j = MAX_DEGREE - 1 - (i - ps);
+                            fa = cand_ids[j];
+                            two = i - ps + pd < nd;
+                            fb = two ? cand_ids[j - pd] : fa;
+                        }
                         bool xa = true, xb = two;  // exact score needed
-                        if (sketched) {
+                        if (sketched && !direct) {
                             float ua, ub;
                             sketch_bound_pair(P.approx, blobA, fa, fb, lane, ua, ub);
                             const long long last = cur[LC - 1];
@@ -574,6 +625,12 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                         score_f32_pair<METRIC>(P.approx, blobA, fa, fb, lane, sa, sb);
                         if (lane == 0) {
                             JV_RBS_SCORED(two ? 2 : 1);
+                            if (direct) {
+                                // a wrong route: the row JV_EMIT drops below (its exact score, <= its sketch bound, goes into s_drop)
+                                const long long last = cur[LC - 1];
+                                const int dr = (topk_key(sa, fa) < last ? 1 : 0) + (two && topk_key(sb, fb) < last ? 1 : 0);
+                                if (dr) atomicAdd(&s_direct_total[1], (unsigned long long)dr);
+                            }
                             JV_EMIT(sa, fa);
                             if (two) JV_EMIT(sb, fb);
                         }
@@ -675,7 +732,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 if (mydrop != INT_MIN) atomicMax(&s_drop[sel], mydrop);
                 if (tid == 0) {
                     s_n = 0;
-                    if (EDGE) s_settled = 0;
+                    if (EDGE) { s_settled = 0; s_nd = 0; }
                 }
                 __syncthreads();
                 JV_T(t_i3);
@@ -1181,7 +1238,7 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
 #endif
 #ifdef JV_ROW_BOUND_STATS
     {
-        const unsigned long long z[3] = {0, 0, 0};
+        const unsigned long long z[4] = {0, 0, 0, 0};
         cudaMemcpyToSymbolAsync(g_rbs_count, z, sizeof(z), 0, cudaMemcpyHostToDevice, s);
     }
 #endif
@@ -1230,20 +1287,26 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     }
 #endif
 #ifdef JV_ROW_BOUND_STATS
-    // one record per launch appended to $JV_ROW_BOUND_STATS_OUT: u64 scored, dropped, samples; then the samples (16 B each)
+    // one record per launch appended to $JV_ROW_BOUND_STATS_OUT: u64 scored, dropped, drop samples, row samples; then the drop
+    // samples (16 B each), then the row samples (24 B each)
     if (const char *out = getenv("JV_ROW_BOUND_STATS_OUT")) {
-        unsigned long long c[3];
+        unsigned long long c[4];
         cudaStreamSynchronize(s);
         cudaMemcpyFromSymbol(c, g_rbs_count, sizeof(c));
         if (c[2] > (unsigned long long)RBS_CAP) c[2] = RBS_CAP;
+        if (c[3] > (unsigned long long)RBS_CAP) c[3] = RBS_CAP;
         RbsSample *h = (RbsSample *)malloc(sizeof(RbsSample) * (c[2] ? c[2] : 1));
+        RbsRow *hr = (RbsRow *)malloc(sizeof(RbsRow) * (c[3] ? c[3] : 1));
         cudaMemcpyFromSymbol(h, g_rbs_sample, sizeof(RbsSample) * c[2]);
+        cudaMemcpyFromSymbol(hr, g_rbs_row, sizeof(RbsRow) * c[3]);
         if (FILE *f = fopen(out, "ab")) {
             fwrite(c, sizeof(c), 1, f);
             fwrite(h, sizeof(RbsSample), c[2], f);
+            fwrite(hr, sizeof(RbsRow), c[3], f);
             fclose(f);
         }
         free(h);
+        free(hr);
     }
 #endif
     return cudaGetLastError();

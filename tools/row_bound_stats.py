@@ -21,6 +21,13 @@ b1, the share of the drops that bound catches before the sketch is read, and pre
 
 where rec counts the whole edge record of every expanded node (its k + 16 B slots stored with the adjacency row).
 
+For the routing of the edge tier (a row the edge bound does not settle goes straight to its full row when the bound's point estimate,
+tests/row_bound_direct.py point_estimate, scores more than delta above the list's last entry) it replays a 1-in-64 sample of every
+row scored against a full list ({query, row, last key, exact key}) at each delta of --deltas, and reports the share of the list's
+entrants routed direct, the share of the scored rows that are drops routed direct (each reads 4 d instead of ss + 16 B), and the
+predicted bytes per scored row, rec + (ss + 16 for a row that reads its sketch) + (4 d for a row that reads its full row), against
+the same replay with no row routed direct.
+
     python tools/row_bound_stats.py [--out row_bound_stats.json]"""
 import argparse
 import json
@@ -40,6 +47,7 @@ ap.add_argument("--nq", type=int, default=10_000)
 ap.add_argument("--max-samples", type=int, default=100_000)
 ap.add_argument("--ranks", default="16,32,64")
 ap.add_argument("--basis-rows", type=int, default=4096)
+ap.add_argument("--deltas", default="0,0.0005,0.001,0.002,0.003,0.004,0.005,0.0075,0.01,0.015,0.02")
 ap.add_argument("--out", default="")
 a = ap.parse_args()
 
@@ -50,6 +58,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import bench  # noqa: E402
 import row_bound_coarse as rbc  # noqa: E402
+import row_bound_direct as rd  # noqa: E402
 import row_bound_lowrank as rl  # noqa: E402
 import row_bound_model as rb  # noqa: E402
 
@@ -65,23 +74,28 @@ os.environ["JV_ROW_BOUND_STATS_OUT"] = path
 r = s.search(w.vec, w.queries, VSF.DOT_PRODUCT, 10, 100)
 del os.environ["JV_ROW_BOUND_STATS_OUT"]
 
-# one record per launch (the first pass and any retry of overflowed queries): u64 scored, dropped, samples; samples of 16 B
+# one record per launch (the first pass and any retry of overflowed queries): u64 scored, dropped, drop samples, row samples; drop
+# samples of 16 B, then row samples of 24 B
 scored = dropped = 0
-samples = []
+samples, row_samples = [], []
 raw = np.fromfile(path, dtype=np.uint8)
 os.unlink(path)
 off = 0
 while off < raw.size:
-    c = raw[off:off + 24].view(np.uint64)
+    c = raw[off:off + 32].view(np.uint64)
     scored, dropped = scored + int(c[0]), dropped + int(c[1])
-    off += 24
-    k = int(c[2])
+    off += 32
+    k, kr = int(c[2]), int(c[3])
     samples.append(raw[off:off + 16 * k].view(np.dtype([("q", "<i4"), ("row", "<i4"), ("last_key", "<i8")])))
     off += 16 * k
-smp = np.concatenate(samples)
+    row_samples.append(raw[off:off + 24 * kr].view(np.dtype([("q", "<i4"), ("row", "<i4"), ("last_key", "<i8"), ("key", "<i8")])))
+    off += 24 * kr
+smp, rsmp = np.concatenate(samples), np.concatenate(row_samples)
 rs = np.random.default_rng(bench.SEED)
 if smp.size > a.max_samples:
     smp = smp[np.sort(rs.choice(smp.size, a.max_samples, replace=False))]
+if rsmp.size > a.max_samples:
+    rsmp = rsmp[np.sort(rs.choice(rsmp.size, a.max_samples, replace=False))]
 f = dropped / max(scored, 1)
 
 import torch  # noqa: E402
@@ -127,6 +141,43 @@ for k in (int(v) for v in a.ranks.split(",")):
     out["lowrank"]["ranks"][str(k)] = {"b1": b1l, "b1_not_caught_by_int8": float((caughtl & ~caught).mean()), "record_bytes_per_new_row": rec,
                                        "predicted_bytes_per_row": pred, "vs_today": pred / today, "median_rho": float(np.median(rho)),
                                        "median_sigma": float(np.median(sig)), "median_beta": float(np.median(beta))}
+# the edge tier's routing, replayed over the row samples with the k = 32 basis (the device's LR_K)
+B = rl.basis(xs, rl.LR_K)
+rrows = w.base_dev[torch.from_numpy(rsmp["row"].astype(np.int64)).cuda()].cpu().numpy()
+rqs = w.queries[rsmp["q"]]
+codes, t, rho, beta, xn = rl.encode_rows(rrows, B)
+settled = rb.topk_key(rb.dot_score_up(rl.upper_bound_raw(rqs, B, codes, t, rho, beta, xn, stride)), rsmp["row"]) < rsmp["last_key"]
+y8, s8, r8 = rb.encode_int8(rrows, stride)
+sketch_caught = rb.topk_key(rb.dot_score_up(rb.upper_bound_raw(rqs, y8, s8, r8, stride)), rsmp["row"]) < rsmp["last_key"]
+entrant = rsmp["key"] >= rsmp["last_key"]
+est = ((np.float32(1) + rd.point_estimate(rqs, B, codes, t)) / np.float32(2)).astype(np.float32)
+
+
+def key_score(k):
+    """the score of a top-k key (the inverse of floatToSortableInt on its high word)"""
+    b = np.asarray(k, dtype=np.int64) >> 32
+    return np.where(b < 0, b ^ 0x7fffffff, b).astype(np.int32).view(np.float32)
+
+
+cut = key_score(rsmp["last_key"])
+err = est.astype(np.float64) - key_score(rsmp["key"]).astype(np.float64)
+rec = deg * (rl.LR_K + 16) / new_per_hop
+row_b, sk_b = 4 * stride, ss + 16
+today_cost = np.where(settled, 0.0, sk_b + np.where(sketch_caught, 0.0, row_b))
+bytes_today = rec + float(today_cost.mean())
+lead = ~settled
+out["edge_direct"] = {"row_samples": int(rsmp.size), "settled_by_edge_bound": float(settled.mean()), "entrants": float(entrant.mean()),
+                      "entrants_not_settled_by_sketch": float((entrant & ~sketch_caught).mean() / max(entrant.mean(), 1e-30)),
+                      "point_estimate_error_score_units": {q_: float(np.quantile(err[lead], q_)) for q_ in (0.01, 0.1, 0.5, 0.9, 0.99)},
+                      "bytes_per_scored_row_today": bytes_today, "deltas": {}}
+for dl in (float(v) for v in a.deltas.split(",")):
+    direct = lead & (est > (cut + np.float32(dl)).astype(np.float32))
+    cost = np.where(settled, 0.0, np.where(direct, row_b, sk_b + np.where(sketch_caught, 0.0, row_b)))
+    pred = rec + float(cost.mean())
+    out["edge_direct"]["deltas"][str(dl)] = {"entrants_routed_direct": float((direct & entrant).sum() / max(entrant.sum(), 1)),
+                                             "drops_routed_direct_per_scored_row": float((direct & ~entrant).mean()),
+                                             "routed_direct_per_scored_row": float(direct.mean()),
+                                             "predicted_bytes_per_scored_row": pred, "vs_today": pred / bytes_today}
 print(json.dumps(out, indent=1))
 if a.out:
     os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
