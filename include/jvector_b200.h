@@ -103,6 +103,10 @@ JV_API const char *jv_version(void);
 JV_API int jv_gpu_sm_count(void);
 
 /* ---- data sets (the RandomAccessVectorValues / CompressedVectors a ScoreFunction reads) ---- */
+/* Data sets and graphs may be shared across threads: any thread may search, build from, score or train on them concurrently. Their
+ * rows, codes and adjacency do not change after creation. What is built lazily on them — an fp32 data set's row sketch and low-rank
+ * rows, a graph's edge records, a PQ data set's centroid-pair tables — is built once, under a lock of the handle, by whichever call
+ * needs it first. The one exception is jv_graph_fuse_pq (below), which rewrites its graph. */
 /* rows: [n][dim] fp32 row-major (base:graph/RandomAccessVectorValues.java) */
 JV_API int jv_dataset_register_f32(const float *rows, int64_t n, int dim, jv_dataset *out);
 /* PQVectors: codes [n][M] u8 (base:quantization/PQVectors.java:377-395), codebooks concatenated in sub-space order,
@@ -151,7 +155,8 @@ JV_API int jv_dataset_device(jv_dataset ds);
  * centroid-vs-centroid table of ProductQuantization.createCodebookPartialSums (ProductQuantization.java:609-628; 12.6 MB at M = 96,
  * k = 256) in HBM; jv_score_pairs on this data set then sums table entries — assembleAndSumPQ, native-c:
  * src/jvector_simd_kernels.cpp:729-815 — instead of recomputing centroid distances. EUCLIDEAN and DOT_PRODUCT have their own
- * tables, COSINE uses the dot-product one. */
+ * tables, COSINE uses the dot-product one. Each table is built once per data set, by this call or by the first build, add,
+ * removal or refine over the codes that needs it (threads that race for it wait for one build), and freed with the data set. */
 JV_API int jv_dataset_pq_pair_table(jv_dataset pq, int metric);
 JV_API int jv_dataset_pq_pair_table_download(jv_dataset pq, int metric, float *table_out /* [M][k (k + 1) / 2] */);
 JV_API int jv_dataset_free(jv_dataset ds);
@@ -318,7 +323,8 @@ JV_API int jv_graph_add_level(jv_graph g, int32_t count, const int32_t *node_ids
  * node's record — FusedPQDecoder.similarityToNeighbor (base:quantization/FusedPQDecoder.java:84-114), the
  * "useEdgeLoading && level == 0" branch of OnDiskGraphIndex.java:639-651 — one contiguous read per hop; upper levels and the
  * entry node use the plain code rows (the hierarchy's cached source features, FusedPQDecoder.java:96-105). Scores are those of
- * the plain PQ walk. JV_FUSED_PQ=0 in the environment ignores the records (A/B timing). */
+ * the plain PQ walk. JV_FUSED_PQ=0 in the environment ignores the records (A/B timing). This call rewrites the graph and frees its
+ * previous records: it must not run while another thread searches, fuses or otherwise uses g. */
 JV_API int jv_graph_fuse_pq(jv_graph g, jv_dataset pq);
 /* records_out [n][*record_bytes] (query the size with records_out = NULL first) */
 JV_API int jv_graph_fused_download(jv_graph g, uint8_t *records_out, int *record_bytes);

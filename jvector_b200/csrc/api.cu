@@ -188,6 +188,9 @@ struct jv_dataset_s {
     uint64_t lr_id = 0;
     bool lr_off = false;
     std::mutex sketch_mu;
+    // PQ: guards the lazily built centroid-pair tables (d.pair_table, jv_dataset_pq_pair_table), whose allocation also grows
+    // `allocs` and `bytes`: callers on several threads build each table once
+    std::mutex pair_mu;
     // an empty data set of n rows of `kind` on the active device: every other field of `d` is zero
     jv_dataset_s(int kind, long long n, int dim)
     {
@@ -506,6 +509,7 @@ int jv_dataset_pq_pair_table(jv_dataset pq, int metric)
     int rc = check_metric(pq->d, metric);
     if (rc) return rc;
     const int which = metric == JV_METRIC_EUCLIDEAN ? 0 : 1;  // cosine sums the dot-product table (ImmutablePQVectors.java:78-92)
+    std::lock_guard<std::mutex> lk(pq->pair_mu);
     if (pq->d.pair_table[which]) return JV_OK;
     if ((rc = t_ctx.init())) return rc;
     float *t = nullptr;
@@ -521,6 +525,7 @@ int jv_dataset_pq_pair_table_download(jv_dataset pq, int metric, float *table_ou
 {
     ON_DEVICE_OF(pq);
     const int which = metric == JV_METRIC_EUCLIDEAN ? 0 : 1;
+    std::lock_guard<std::mutex> lk(pq->pair_mu);
     if (pq->d.kind != KIND_PQ || !pq->d.pair_table[which] || !table_out) return fail(JV_ERR_INVALID, "pq_pair_table_download: no table for this metric");
     const size_t entries = (size_t)pq->d.M * ((size_t)pq->d.k * (pq->d.k + 1) / 2);
     CK(cudaMemcpy(table_out, pq->d.pair_table[which], entries * 4, cudaMemcpyDeviceToHost), "D2H pair table");
