@@ -356,7 +356,9 @@ JV_API int jv_graph_search_batch(jv_graph g, jv_dataset approx, jv_dataset reran
  * otherwise query i uses accept_bits + i * accept_stride_words. threshold: minimum approximate score of a result (the
  * TwoPhaseTracker early-termination heuristic of ScoreTracker.java is NOT run: a threshold search here visits at least what
  * the reference visits). rerank_floor: NodeQueue.rerank's rerankFloor (NodeQueue.java:168-230). NULL = {NULL, 0, 0, 0}.
- * A filter that rejects most nodes needs a long candidate list; beyond 8192 live candidates the call fails with JV_ERR_OVERFLOW. */
+ * A filter that rejects most nodes needs a long candidate list; beyond 8192 live candidates the call fails with JV_ERR_OVERFLOW.
+ * For filters that selective (roughly under rerankK / 8192 of the rows accepted), jv_exhaustive_search_batch scores the accepted
+ * rows instead, at about what they cost, with the same options and outputs. */
 typedef struct {
     const uint32_t *accept_bits;
     int64_t accept_stride_words;
@@ -376,6 +378,21 @@ JV_API int jv_graph_search_batch_device_ex(jv_graph g, jv_dataset approx, jv_dat
                                            const float *queries_device, int nq, int topK, int rerankK,
                                            const jv_search_options *opts_device_bits, int32_t *nodes_out_device,
                                            float *scores_out_device, jv_search_stats *stats);
+
+/* jv_topk_bruteforce restricted to the rows each query accepts (opts->accept_bits, host memory, the layout and stride above; bits
+ * at positions >= n are ignored) and, when opts->threshold > 0, to the rows scoring >= it. Same keys: best first, ties to the
+ * smaller id, padded with INT64_MIN. opts == NULL, or accept_bits == NULL at threshold 0, is jv_topk_bruteforce byte for byte.
+ * rerank_floor must be 0. Every storage kind; BQ takes the popcount kernels (DESIGN §4.2a). */
+JV_API int jv_topk_bruteforce_ex(jv_dataset ds, int metric, const float *queries, int nq, int k, const jv_search_options *opts,
+                                 int64_t *keys_out);
+/* jv_graph_search_batch_ex without a graph: the candidates are the jv_topk_bruteforce_ex keys at k = rerankK (rerankK <= 2048).
+ * No reranker: the first topK. With one (fp32 or NVQ): NodeQueue.rerank's take rule at opts->rerank_floor (the candidates whose
+ * approximate score is >= it, or the best one when none is), rescored exactly and returned in key order (equal exact scores: the
+ * smaller id first). nodes_out / scores_out [nq][topK], -1 / 0 padded. stats: visited = accepted rows scored (summed over queries),
+ * reranked = candidates rescored, expanded = expanded_base = retried = 0, device_ms = CUDA-event time of the call. */
+JV_API int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, int metric, const float *queries, int nq, int topK,
+                                      int rerankK, const jv_search_options *opts, int32_t *nodes_out, float *scores_out,
+                                      jv_search_stats *stats);
 
 /* Replicas: graph + data sets registered once per device (jv_gpu_set_device(d), then the ordinary create / register calls); the
  * batch is split into contiguous slices, one per replica, searched concurrently (no data-path exchange). stats sums the counters,

@@ -170,6 +170,33 @@ private:
     const GraphIndex &g_;
 };
 
+/// GraphSearcher::search without a graph: every row the options accept is scored (jv_exhaustive_search_batch), for filters too
+/// selective for the walk. opts: acceptOrds bitsets, threshold, rerankFloor (nullptr: none)
+class ExhaustiveSearcher {
+public:
+    SearchResult search(const Vectors &approx, const float *queries, int nq, VectorSimilarityFunction vsf, int topK, int rerankK, const Vectors *reranker = nullptr,
+                        const jv_search_options *opts = nullptr) const
+    {
+        SearchResult r;
+        r.topK = topK;
+        r.nodes.resize((size_t)nq * topK);
+        r.scores.resize((size_t)nq * topK);
+        jv_search_stats st;
+        check(jv_exhaustive_search_batch(approx.handle(), reranker ? reranker->handle() : nullptr, (int)vsf, queries, nq, topK, rerankK, opts, r.nodes.data(),
+                                         r.scores.data(), &st));
+        r.visitedCount = st.visited; r.expandedCount = st.expanded; r.expandedCountBaseLayer = st.expanded_base; r.rerankedCount = st.reranked; r.deviceMs = st.device_ms;
+        return r;
+    }
+};
+
+/// exhaustive top-k keys [nq][k] over the rows the options accept (jv_topk_bruteforce_ex; opts nullptr: every row)
+inline std::vector<int64_t> topkBruteforce(const Vectors &v, const float *queries, int nq, VectorSimilarityFunction vsf, int k, const jv_search_options *opts = nullptr)
+{
+    std::vector<int64_t> keys((size_t)nq * k);
+    check(jv_topk_bruteforce_ex(v.handle(), (int)vsf, queries, nq, k, opts, keys.data()));
+    return keys;
+}
+
 class GraphIndexBuilder {
 public:
     GraphIndexBuilder(VectorSimilarityFunction vsf, int M, int beamWidth, float neighborOverflow, float alpha, bool addHierarchy, uint64_t seed = 0)

@@ -153,6 +153,8 @@ SYMBOLS = [
     ("jv_graph_search_batch_device", _I, [_P, _P, _P, _I, _P, _I, _I, _I, _P, _P, C.POINTER(SearchStats)]),
     ("jv_graph_search_batch_ex", _I, [_P, _P, _P, _I, f32p, _I, _I, _I, C.POINTER(SearchOptions), i32p, f32p, C.POINTER(SearchStats)]),
     ("jv_graph_search_batch_device_ex", _I, [_P, _P, _P, _I, _P, _I, _I, _I, C.POINTER(SearchOptions), _P, _P, C.POINTER(SearchStats)]),
+    ("jv_topk_bruteforce_ex", _I, [_P, _I, f32p, _I, _I, C.POINTER(SearchOptions), i64p]),
+    ("jv_exhaustive_search_batch", _I, [_P, _P, _I, f32p, _I, _I, _I, C.POINTER(SearchOptions), i32p, f32p, C.POINTER(SearchStats)]),
     ("jv_graph_build", _I, [_P, _I, C.POINTER(BuildParams), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_graph_build_pq", _I, [_P, _I, C.POINTER(BuildParams), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_builder_create_pq", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]),

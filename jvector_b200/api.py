@@ -317,12 +317,32 @@ def score_multi(vectors, vsf, queries, ids, offsets):
     return out
 
 
-def topk_bruteforce(vectors, vsf, queries, k):
-    """Exhaustive first pass with the reference's ordering key; returns (nodes [nq][k], scores [nq][k], keys)."""
+def _search_options(threshold, rerankFloor, acceptOrds):
+    """jv_search_options for GraphSearcher.search's filter arguments (None when there is no filter), and the packed bitsets it
+    points at (keep them alive for the call)"""
+    if acceptOrds is None and threshold == 0 and rerankFloor == 0:
+        return None, None
+    opts = nat.SearchOptions(None, 0, float(threshold), float(rerankFloor))
+    bits = None
+    if acceptOrds is not None:
+        bits = pack_accept_bits(acceptOrds)
+        opts.accept_bits = bits.ctypes.data
+        opts.accept_stride_words = bits.shape[1] if bits.ndim == 2 else 0
+    return opts, bits
+
+
+def topk_bruteforce(vectors, vsf, queries, k, acceptOrds=None, threshold=0.0):
+    """Exhaustive first pass with the reference's ordering key; returns (nodes [nq][k], scores [nq][k], keys).
+    acceptOrds (a bool array [n] shared by the batch, or [nq][n] one per query) and threshold restrict it to the accepted rows
+    scoring >= threshold (jv_topk_bruteforce_ex)."""
     lib = nat.init()
     queries = c32(queries)
     keys = np.empty((queries.shape[0], k), dtype=np.int64)
-    check(lib.jv_topk_bruteforce(vectors._h, int(vsf), fp(queries), queries.shape[0], k, lp(keys)))
+    if acceptOrds is None and threshold == 0:
+        check(lib.jv_topk_bruteforce(vectors._h, int(vsf), fp(queries), queries.shape[0], k, lp(keys)))
+    else:
+        opts, bits = _search_options(threshold, 0.0, acceptOrds)
+        check(lib.jv_topk_bruteforce_ex(vectors._h, int(vsf), fp(queries), queries.shape[0], k, C.byref(opts) if opts is not None else None, lp(keys)))
     nodes = (~(keys & 0xffffffff)).astype(np.int64) & 0xffffffff
     nodes = nodes.astype(np.int64)
     s = (keys >> 32).astype(np.int32)
@@ -510,6 +530,27 @@ class GraphSearcher:
                 opts.accept_stride_words = bits.shape[1] if bits.ndim == 2 else 0
         check(lib.jv_graph_search_batch_ex(self.graph._h, approx._h, reranker._h if reranker is not None else None, int(vsf), fp(queries), nq,
                                            topK, rerankK, C.byref(opts) if opts is not None else None, ip(nodes), fp(scores), C.byref(st)))
+        return SearchResult(nodes, scores, st)
+
+
+class ExhaustiveSearcher:
+    """GraphSearcher.search without a graph: every row acceptOrds accepts is scored exactly by `approx` (jv_exhaustive_search_batch),
+    at about what the accepted rows cost. For filters too selective for the graph walk; same arguments and SearchResult, so a caller
+    can pick the searcher per batch on the filter's density."""
+
+    def search(self, approx, queries, vsf, topK, rerankK=None, reranker=None, threshold=0.0, rerankFloor=0.0, acceptOrds=None):
+        lib = nat.init()
+        queries = c32(queries)
+        if queries.shape[1] != approx.dimension():
+            raise ValueError("query dimension %d != data set dimension %d" % (queries.shape[1], approx.dimension()))
+        rerankK = rerankK or topK
+        nq = queries.shape[0]
+        nodes = np.empty((nq, topK), dtype=np.int32)
+        scores = np.empty((nq, topK), dtype=np.float32)
+        st = nat.SearchStats()
+        opts, bits = _search_options(threshold, rerankFloor, acceptOrds)
+        check(lib.jv_exhaustive_search_batch(approx._h, reranker._h if reranker is not None else None, int(vsf), fp(queries), nq, topK, rerankK,
+                                             C.byref(opts) if opts is not None else None, ip(nodes), fp(scores), C.byref(st)))
         return SearchResult(nodes, scores, st)
 
 

@@ -85,6 +85,8 @@ struct ThreadCtx {
     DeviceBuffer bq_async;      // jv_topk_bruteforce_device_async: still read on the caller's stream after the call returns
     DeviceBuffer search_scratch, search_aux;  // the search kernel's scratch; its counters and per-query overflow codes
     DeviceBuffer accept_bits;   // host-pointer searches: the uploaded acceptOrds bitsets
+    DeviceBuffer accept_lists;  // filtered top-k: accepted counts, accepted-row lists, the sampled tier's query list
+    DeviceBuffer rerank;        // exhaustive search: candidate keys, the reranker's prepared queries, taken ids, exact scores
     DeviceBuffer watermark;     // host-pointer searches: the arrival watermark the copy stream writes
     StreamTimer timer;
     // host-pointer searches: a second stream carries the query chunks while the search kernel already runs (arrival watermark)
@@ -110,7 +112,7 @@ struct ThreadCtx {
     template <typename F>
     void each_owner(F f)
     {
-        for (DeviceBuffer *b : {&input, &aux, &blobs, &output, &topk_scratch, &bq_scratch, &flag, &bq_async, &search_scratch, &search_aux, &accept_bits, &watermark})
+        for (DeviceBuffer *b : {&input, &aux, &blobs, &output, &topk_scratch, &bq_scratch, &flag, &bq_async, &search_scratch, &search_aux, &accept_bits, &accept_lists, &rerank, &watermark})
             f(*b);
         f(marks);
         f(timer);
@@ -828,6 +830,194 @@ int jv_topk_merge_device_async(const int64_t *keys_in_device, int nq, int parts,
     NEED_INIT();
     if (!keys_in_device || !keys_out_device || nq <= 0 || parts <= 0 || k <= 0 || (long long)parts * k > 16384) return fail(JV_ERR_INVALID, "topk_merge: bad arguments");
     CK(launch_topk_merge_strided((const long long *)keys_in_device, nq, parts, k, (long long *)keys_out_device, (cudaStream_t)cuda_stream), "topk_merge");
+    return JV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ filtered exhaustive top-k
+// the acceptOrds / threshold fields of jv_search_options over a data set of n rows (the graph search's checks and wording)
+static int check_accept_options(const jv_search_options *opts, long long n, const char *who)
+{
+    if (!opts) return JV_OK;
+    if (opts->threshold < 0.f || opts->rerank_floor < 0.f || opts->accept_stride_words < 0)
+        return fail(JV_ERR_INVALID, std::string(who) + ": negative threshold / rerankFloor / stride");
+    const long long words = (n + 31) / 32;
+    if (opts->accept_bits && opts->accept_stride_words != 0 && opts->accept_stride_words < words)
+        return fail(JV_ERR_INVALID, std::string(who) + ": accept_stride_words shorter than one bitset");
+    return JV_OK;
+}
+
+// the lowest top-k key whose score passes `score >= threshold` (threshold > 0): every key below it scores less
+static long long threshold_key(float threshold)
+{
+    if (!(threshold > 0.f)) return KEY_MIN;
+    int32_t b;
+    memcpy(&b, &threshold, 4);
+    b ^= (b >> 31) & 0x7fffffff;
+    return (long long)((unsigned long long)(uint32_t)b << 32);
+}
+
+// Keys of the k best rows each query accepts (opts->accept_bits: host bitsets, NULL = every row; opts->threshold), queries in HBM.
+// The bitsets are compacted on the device (a shared one once, per-query ones chunk by chunk with the queries) and each query goes
+// to the whole or the sampled tier on its accepted count (launch_topk_accepted). *visited += the accepted rows of every query.
+static int topk_accepted_device(jv_dataset ds, int metric, const float *queries_dev, int nq, int k, const jv_search_options *opts, long long *keys_dev,
+                                int64_t *visited)
+{
+    cudaStream_t s = t_ctx.stream;
+    int rc;
+    const long long n = ds->d.n;
+    const size_t words = (size_t)((n + 31) / 32);
+    const int S = accept_sample_size(n);
+    const bool per_query = opts->accept_bits && opts->accept_stride_words != 0;
+    const long long stride = per_query ? opts->accept_stride_words : 0;
+    const size_t bf = (size_t)blob_floats(ds->d);
+    const int chunk_max = (int)std::max<size_t>(1, std::min<size_t>(4096, ((size_t)512 << 20) / (bf * 4)));
+    const int chunk = std::min(nq, chunk_max);
+    const int nsets = per_query ? chunk : 1;
+    const size_t bit_words = per_query ? (size_t)stride * (size_t)(chunk - 1) + words : words;
+    int *dcnt, *dsampled;
+    int32_t *dids;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dcnt = c.take<int>(nsets);
+        dids = c.take<int32_t>((size_t)nsets * S);
+        dsampled = c.take<int>(chunk);
+        return c.bytes;
+    };
+    if ((rc = grow(t_ctx.accept_bits, bit_words * 4)) || (rc = grow(t_ctx.accept_lists, carve(nullptr))) || (rc = grow(t_ctx.blobs, (size_t)chunk * bf * 4)) ||
+        (rc = grow(t_ctx.topk_scratch, topk_scratch_bytes(ds->d, chunk, k))) || (rc = grow(t_ctx.flag, 64)))
+        return rc;
+    carve(t_ctx.accept_lists.get());
+    uint32_t *dbits = t_ctx.accept_bits.get<uint32_t>();
+    std::vector<int> cnt(nsets), sampled;
+    if (!per_query) {
+        if (opts->accept_bits) CK(cudaMemcpyAsync(dbits, opts->accept_bits, words * 4, cudaMemcpyHostToDevice, s), "H2D accept bits");
+        else CK(cudaMemsetAsync(dbits, 0xff, words * 4, s), "memset accept bits");  // a threshold alone: every row is accepted
+        CK(launch_accept_compact(dbits, 0, 1, n, dcnt, dids, s), "accept_compact");
+        CK(cudaMemcpyAsync(cnt.data(), dcnt, sizeof(int), cudaMemcpyDeviceToHost, s), "D2H accepted count");
+        CK(cudaStreamSynchronize(s), "sync");
+    }
+    const long long floor_key = threshold_key(opts->threshold);
+    for (int q0 = 0; q0 < nq; q0 += chunk) {
+        const int cq = std::min(chunk, nq - q0);
+        if (per_query) {
+            CK(cudaMemcpyAsync(dbits, opts->accept_bits + (size_t)q0 * stride, ((size_t)stride * (cq - 1) + words) * 4, cudaMemcpyHostToDevice, s), "H2D accept bits");
+            CK(launch_accept_compact(dbits, stride, cq, n, dcnt, dids, s), "accept_compact");
+            CK(cudaMemcpyAsync(cnt.data(), dcnt, (size_t)cq * sizeof(int), cudaMemcpyDeviceToHost, s), "D2H accepted counts");
+            CK(cudaStreamSynchronize(s), "sync");
+        }
+        AcceptLists acc{dbits, stride, per_query, dcnt, dids, 0, dsampled, 0};
+        sampled.clear();
+        for (int i = 0; i < cq; i++) {
+            const int c = cnt[per_query ? i : 0];
+            acc.max_listed = std::max(acc.max_listed, std::min(c, S));
+            if (c > S) sampled.push_back(i);
+            *visited += c;
+        }
+        acc.n_sampled = (int)sampled.size();
+        if (acc.n_sampled) CK(cudaMemcpyAsync(dsampled, sampled.data(), sampled.size() * sizeof(int), cudaMemcpyHostToDevice, s), "H2D sampled queries");
+        int *dflag = t_ctx.flag.get<int>();
+        CK(cudaMemsetAsync(dflag, 0, sizeof(int), s), "memset flag");
+        CK(launch_prepare(ds->d, metric, queries_dev + (size_t)q0 * ds->d.dim, cq, t_ctx.blobs.get<float>(), s), "prepare");
+        CK(launch_topk_accepted(ds->d, metric, t_ctx.blobs.get<float>(), cq, k, acc, floor_key, t_ctx.topk_scratch.get(), keys_dev + (size_t)q0 * k, dflag, s),
+           "topk_accepted");
+        int flag = 0;
+        CK(cudaMemcpyAsync(&flag, dflag, sizeof(int), cudaMemcpyDeviceToHost, s), "D2H flag");
+        CK(cudaStreamSynchronize(s), "sync");
+        if (flag) return fail(JV_ERR_OVERFLOW, "topk_bruteforce_ex: candidate buffer overflow (adversarial score distribution)");
+    }
+    return JV_OK;
+}
+
+int jv_topk_bruteforce_ex(jv_dataset ds, int metric, const float *queries, int nq, int k, const jv_search_options *opts, int64_t *keys_out)
+{
+    ON_DEVICE_OF(ds);
+    if (!queries || !keys_out || nq <= 0 || k <= 0) return fail(JV_ERR_INVALID, "topk_bruteforce_ex: bad arguments");
+    if (k > 2048) return fail(JV_ERR_INVALID, "topk_bruteforce_ex: k <= 2048");
+    int rc = check_accept_options(opts, ds->d.n, "topk_bruteforce_ex");
+    if (rc) return rc;
+    if (opts && opts->rerank_floor != 0.f) return fail(JV_ERR_INVALID, "topk_bruteforce_ex: rerank_floor must be 0 (nothing is reranked)");
+    if (!opts || (!opts->accept_bits && !(opts->threshold > 0.f))) return jv_topk_bruteforce(ds, metric, queries, nq, k, keys_out);
+    if ((rc = check_metric(ds->d, metric))) return rc;
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)nq * ds->d.dim * 4)) || (rc = grow(t_ctx.output, (size_t)nq * k * 8))) return rc;
+    cudaStream_t s = t_ctx.stream;
+    CK(cudaMemcpyAsync(t_ctx.input.get(), queries, (size_t)nq * ds->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+    int64_t visited = 0;
+    if ((rc = topk_accepted_device(ds, metric, t_ctx.input.get<float>(), nq, k, opts, t_ctx.output.get<long long>(), &visited))) return rc;
+    CK(cudaMemcpyAsync(keys_out, t_ctx.output.get(), (size_t)nq * k * 8, cudaMemcpyDeviceToHost, s), "D2H keys");
+    CK(cudaStreamSynchronize(s), "sync");
+    return JV_OK;
+}
+
+constexpr int EXHAUSTIVE_QUERY_CHUNK = 4096;  // queries per candidate / rerank step (bounds the candidate keys and rerank scratch)
+
+int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, int metric, const float *queries, int nq, int topK, int rerankK,
+                               const jv_search_options *opts, int32_t *nodes_out, float *scores_out, jv_search_stats *stats)
+{
+    ON_DEVICE_OF(approx);
+    if (!queries || !nodes_out || !scores_out || nq <= 0) return fail(JV_ERR_INVALID, "exhaustive_search: bad arguments");
+    if (topK < 1 || rerankK < topK) return fail(JV_ERR_INVALID, "exhaustive_search: need 1 <= topK <= rerankK");
+    if (rerankK > 2048) return fail(JV_ERR_INVALID, "exhaustive_search: rerankK <= 2048");
+    if (reranker && reranker->device != approx->device) return fail(JV_ERR_INVALID, "exhaustive_search: data sets live on different devices");
+    if (reranker && (reranker->d.n != approx->d.n || reranker->d.dim != approx->d.dim)) return fail(JV_ERR_INVALID, "exhaustive_search: reranker shape mismatch");
+    if (reranker && reranker->d.kind != KIND_F32 && reranker->d.kind != KIND_NVQ)
+        return fail(JV_ERR_UNSUPPORTED, "exhaustive_search: the reranker must be fp32 or NVQ (OnDiskGraphIndex.java:705-713)");
+    int rc = check_accept_options(opts, approx->d.n, "exhaustive_search");
+    if (rc || (rc = check_metric(approx->d, metric))) return rc;
+    const bool filtered = opts && (opts->accept_bits || opts->threshold > 0.f);
+    const float floor = opts ? opts->rerank_floor : 0.f;
+    const int R = rerankK, chunk = std::min(nq, EXHAUSTIVE_QUERY_CHUNK);
+    const size_t rbf = reranker ? (size_t)blob_floats(reranker->d) : 0;
+    long long *dcand;
+    int32_t *dnodes, *dids, *doffsets;
+    float *dscores, *drblobs, *dexact;
+    unsigned long long *dtaken;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dcand = c.take<long long>((size_t)chunk * R);
+        dnodes = c.take<int32_t>((size_t)chunk * topK);
+        dscores = c.take<float>((size_t)chunk * topK);
+        dtaken = c.take<unsigned long long>(1);
+        drblobs = c.take<float>(reranker ? (size_t)chunk * rbf : 0);
+        dids = c.take<int32_t>(reranker ? (size_t)chunk * R : 0);
+        doffsets = c.take<int32_t>(reranker ? (size_t)chunk + 1 : 0);
+        dexact = c.take<float>(reranker ? (size_t)chunk * R : 0);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)chunk * approx->d.dim * 4)) || (rc = grow(t_ctx.rerank, carve(nullptr)))) return rc;
+    carve(t_ctx.rerank.get());
+    cudaStream_t s = t_ctx.stream;
+    float *dq = t_ctx.input.get<float>();
+    int64_t visited = 0;
+    CK(cudaMemsetAsync(dtaken, 0, sizeof(unsigned long long), s), "memset taken");
+    CK(t_ctx.timer.start(s), "event");
+    for (int q0 = 0; q0 < nq; q0 += chunk) {
+        const int cq = std::min(chunk, nq - q0);
+        const float *qh = queries + (size_t)q0 * approx->d.dim;
+        CK(cudaMemcpyAsync(dq, qh, (size_t)cq * approx->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+        if (filtered) {
+            jv_search_options o = *opts;
+            if (o.accept_bits && o.accept_stride_words) o.accept_bits += (size_t)q0 * o.accept_stride_words;
+            if ((rc = topk_accepted_device(approx, metric, dq, cq, R, &o, dcand, &visited))) return rc;
+        } else {
+            if ((rc = topk_device(approx, metric, dq, cq, R, 0, dcand))) return rc;
+            visited += (int64_t)cq * approx->d.n;
+        }
+        if (reranker) CK(launch_prepare(reranker->d, metric, dq, cq, drblobs, s), "prepare reranker");
+        CK(launch_rerank_accepted(reranker ? &reranker->d : nullptr, metric, drblobs, cq, R, topK, floor, dcand, dids, doffsets, dexact, dtaken, dnodes, dscores, s),
+           "rerank");
+        CK(cudaMemcpyAsync(nodes_out + (size_t)q0 * topK, dnodes, (size_t)cq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H nodes");
+        CK(cudaMemcpyAsync(scores_out + (size_t)q0 * topK, dscores, (size_t)cq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    }
+    CK(t_ctx.timer.stop(s), "event");
+    unsigned long long taken = 0;
+    CK(cudaMemcpyAsync(&taken, dtaken, sizeof(taken), cudaMemcpyDeviceToHost, s), "D2H taken");
+    CK(cudaStreamSynchronize(s), "sync");
+    if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        stats->visited = visited;
+        stats->reranked = (int64_t)taken;
+        stats->device_ms = t_ctx.timer.ms();
+    }
     return JV_OK;
 }
 

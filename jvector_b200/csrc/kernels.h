@@ -74,6 +74,33 @@ size_t topk_scratch_bytes(const DataDesc &d, int nq, int k);
 cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, void *scratch_dev,
                                    long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s);
 
+// acceptOrds-filtered top-k (jv_topk_bruteforce_ex). S = accept_sample_size(n) = launch_topk_bruteforce's sample size.
+// launch_accept_compact: per bitset (bits + b * stride_words), cnt[b] = its rows < n whose bit is set, and ids[b * S + i],
+// i < min(cnt, S): the accepted row of rank floor(i cnt / min(cnt, S)) (every accepted row in ascending order when cnt <= S).
+int accept_sample_size(long long n);
+cudaError_t launch_accept_compact(const uint32_t *bits_dev, long long stride_words, int nsets, long long n, int *cnt_dev, int32_t *ids_dev, cudaStream_t s);
+struct AcceptLists {
+    const uint32_t *bits;      // device: the bitsets
+    long long stride_words;    // between two queries' bitsets; 0 = one bitset shared by the batch
+    bool per_query;            // cnt / ids hold one entry per query (else one shared)
+    const int *cnt;            // launch_accept_compact's counts
+    const int32_t *ids;        // and lists
+    int max_listed;            // max over the batch of min(cnt, S)
+    const int *sampled;        // device: the queries with cnt > S (the sampled tier), n_sampled of them
+    int n_sampled;
+};
+// keys of the k best accepted rows scoring >= the threshold (floor_key: its lowest key; KEY_MIN = none) per query, padded with KEY_MIN.
+// scratch: topk_scratch_bytes(d, nq, k); *overflow_flag_dev as launch_topk_bruteforce's
+cudaError_t launch_topk_accepted(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, const AcceptLists &acc, long long floor_key,
+                                 void *scratch_dev, long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s);
+// exhaustive search's last step over R sorted candidate keys per query: rr == nullptr: the first topK; else NodeQueue.rerank's take
+// rule at `floor` (ids_dev [nq][R]: taken nodes, -1 elsewhere, offsets_dev [nq + 1]; *taken_dev += their count), their exact scores
+// under the reranker (rblobs_dev: its prepared queries; exact_dev [nq][R]), the topK best exact keys. Out: nodes / scores [nq][topK],
+// -1 / 0 padded
+cudaError_t launch_rerank_accepted(const DataDesc *rr, int metric, const float *rblobs_dev, int nq, int R, int topK, float floor, const long long *cand_dev,
+                                   int32_t *ids_dev, int32_t *offsets_dev, float *exact_dev, unsigned long long *taken_dev, int32_t *nodes_dev, float *scores_dev,
+                                   cudaStream_t s);
+
 cudaError_t launch_add_int(int *dst_dev, const int *src_dev, cudaStream_t s);
 // keys[i] -> same score, node id + id_base (KEY_MIN pads untouched)
 cudaError_t launch_key_rebase(long long *keys_dev, long long count, long long id_base, cudaStream_t s);

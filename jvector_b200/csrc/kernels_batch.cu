@@ -270,9 +270,21 @@ __global__ void __launch_bounds__(256) topk_threshold_kernel(const float *__rest
 constexpr int BF_THREADS = 256;
 constexpr int BF_TILE = 2048;  // rows per CTA
 
-template <int KIND, int METRIC>
+// word w of an accept bitset over n rows, the bits at positions >= n cleared
+__device__ __forceinline__ uint32_t accept_word(const uint32_t *__restrict__ bits, long long w, long long n)
+{
+    uint32_t x = __ldg(bits + w);
+    const long long left = n - w * 32;
+    if (left < 32) x &= (1u << (int)left) - 1u;
+    return x;
+}
+
+// ACC (jv_topk_bruteforce_ex): only the rows whose bit is set in the query's accept bitset (acc + q * acc_stride words) are scored;
+// each warp takes one 32-row word of the tile at a time, so an all-zero word costs the warp one load
+template <int KIND, int METRIC, bool ACC = false>
 __global__ void __launch_bounds__(BF_THREADS) topk_filter_kernel(DataDesc d, const float *__restrict__ blobs, int blob_stride, const long long *__restrict__ thr,
-                                                                 long long *__restrict__ buf, int *__restrict__ cnt, int cap, const int *__restrict__ qlist)
+                                                                 long long *__restrict__ buf, int *__restrict__ cnt, int cap, const int *__restrict__ qlist,
+                                                                 const uint32_t *__restrict__ acc = nullptr, long long acc_stride = 0)
 {
     constexpr int G = GroupOf<KIND>::value;
     constexpr int NG = BF_THREADS / G;
@@ -283,13 +295,34 @@ __global__ void __launch_bounds__(BF_THREADS) topk_filter_kernel(DataDesc d, con
     const long long t = thr[q];
     if (t == KEY_DONE) return;
     const int group = threadIdx.x / G, lane = threadIdx.x % G;
-    for (long long r = r0 + group; r < r1; r += NG) {
-        const float sc = score_row<KIND, METRIC>(d, blob, (int)r, lane);
-        if (lane == 0) {
-            const long long key = topk_key(sc, (int32_t)r);
-            if (key >= t) {
-                const int pos = atomicAdd(&cnt[q], 1);
-                if (pos < cap) buf[(size_t)q * cap + pos] = key;
+    if constexpr (!ACC) {
+        for (long long r = r0 + group; r < r1; r += NG) {
+            const float sc = score_row<KIND, METRIC>(d, blob, (int)r, lane);
+            if (lane == 0) {
+                const long long key = topk_key(sc, (int32_t)r);
+                if (key >= t) {
+                    const int pos = atomicAdd(&cnt[q], 1);
+                    if (pos < cap) buf[(size_t)q * cap + pos] = key;
+                }
+            }
+        }
+    } else {
+        const uint32_t *bits = acc + (size_t)q * acc_stride;
+        constexpr int GPW = 32 / G;  // lane groups per warp
+        const int gw = (threadIdx.x & 31) / G;
+        for (long long w = r0 / 32 + (threadIdx.x >> 5); w * 32 < r1; w += BF_THREADS / 32) {
+            const uint32_t x = accept_word(bits, w, d.n);
+            const int p = __popc(x);
+            for (int i = gw; i < p; i += GPW) {
+                const int r = (int)(w * 32) + (int)__fns(x, 0, i + 1);
+                const float sc = score_row<KIND, METRIC>(d, blob, r, lane);
+                if (lane == 0) {
+                    const long long key = topk_key(sc, r);
+                    if (key >= t) {
+                        const int pos = atomicAdd(&cnt[q], 1);
+                        if (pos < cap) buf[(size_t)q * cap + pos] = key;
+                    }
+                }
             }
         }
     }
@@ -352,10 +385,13 @@ __device__ __forceinline__ int hamming_csa(const unsigned long long (&r)[MAXW], 
 // Hamming bound derived from the sample threshold.
 constexpr int BQF_THREADS = 256;
 
-template <int MAXW>
+// ACC: a row is scored against a query only when its bit is set in that query's accept bitset. A warp's 32 rows are one bitset word:
+// a shared bitset's all-zero word skips the warp's row loads, a per-query bitset's all-zero word skips that query for the warp.
+template <int MAXW, bool ACC = false>
 __global__ void __launch_bounds__(BQF_THREADS) topk_filter_bq_kernel(DataDesc d, const float *__restrict__ blobs, int blob_stride, int nq,
                                                                      const long long *__restrict__ thr, long long *__restrict__ buf,
-                                                                     int *__restrict__ cnt, int cap, const int *__restrict__ qlist)
+                                                                     int *__restrict__ cnt, int cap, const int *__restrict__ qlist,
+                                                                     const uint32_t *__restrict__ acc = nullptr, long long acc_stride = 0)
 {
     constexpr int BQF_QCHUNK = MAXW <= 16 ? 256 : 128;  // queries staged per pass (<= 32 KB of bit packs)
     __shared__ __align__(16) unsigned long long qs[BQF_QCHUNK * MAXW];
@@ -366,7 +402,8 @@ __global__ void __launch_bounds__(BQF_THREADS) topk_filter_bq_kernel(DataDesc d,
     const long long row_stride = (long long)gridDim.x * BQF_THREADS;
     for (long long r = (long long)blockIdx.x * BQF_THREADS + threadIdx.x; r - threadIdx.x < d.n; r += row_stride) {
         unsigned long long rw[MAXW];
-        const bool live = r < d.n;
+        bool live = r < d.n;
+        if (ACC && acc_stride == 0) live = live && ((accept_word(acc, r >> 5, d.n) >> (r & 31)) & 1u);
         const unsigned long long *row = d.words + (size_t)(live ? r : 0) * W;
 #pragma unroll
         for (int w = 0; w < MAXW; w++) rw[w] = (live && w < W) ? __ldg(row + w) : 0ull;
@@ -397,6 +434,10 @@ __global__ void __launch_bounds__(BQF_THREADS) topk_filter_bq_kernel(DataDesc d,
             __syncthreads();
             if (live) {
                 for (int q = 0; q < qc; q++) {
+                    if (ACC && acc_stride != 0) {
+                        const uint32_t x = accept_word(acc + (size_t)sq[q] * acc_stride, r >> 5, d.n);
+                        if (!((x >> (r & 31)) & 1u)) continue;
+                    }
                     int hd;
                     if constexpr (MAXW >= 8) hd = hamming_csa<MAXW>(rw, qs + q * MAXW);
                     else {
@@ -423,10 +464,12 @@ __global__ void __launch_bounds__(BQF_THREADS) topk_filter_bq_kernel(DataDesc d,
 constexpr int PQF_THREADS = 256;
 constexpr int PQF_TILE = 16384;
 
-template <int METRIC>
+// ACC: as topk_filter_kernel's, one warp per 32-row bitset word
+template <int METRIC, bool ACC = false>
 __global__ void __launch_bounds__(PQF_THREADS) topk_filter_pq_kernel(DataDesc d, const float *__restrict__ blobs, int blob_stride,
                                                                      const long long *__restrict__ thr, long long *__restrict__ buf,
-                                                                     int *__restrict__ cnt, int cap, const int *__restrict__ qlist)
+                                                                     int *__restrict__ cnt, int cap, const int *__restrict__ qlist,
+                                                                     const uint32_t *__restrict__ acc = nullptr, long long acc_stride = 0)
 {
     extern __shared__ __align__(128) unsigned char pq_smem[];
     float *lut = reinterpret_cast<float *>(pq_smem);
@@ -450,13 +493,34 @@ __global__ void __launch_bounds__(PQF_THREADS) topk_filter_pq_kernel(DataDesc d,
     const long long r1 = min(d.n, r0 + PQF_TILE);
     const long long t = thr[q];
     const int group = threadIdx.x / G, lane = threadIdx.x % G;
-    for (long long r = r0 + group; r < r1; r += NG) {
-        const float sc = score_pq<METRIC>(d, lut, (int)r, lane);
-        if (lane == 0) {
-            const long long key = topk_key(sc, (int32_t)r);
-            if (key >= t) {
-                const int pos = atomicAdd(&cnt[q], 1);
-                if (pos < cap) buf[(size_t)q * cap + pos] = key;
+    if constexpr (!ACC) {
+        for (long long r = r0 + group; r < r1; r += NG) {
+            const float sc = score_pq<METRIC>(d, lut, (int)r, lane);
+            if (lane == 0) {
+                const long long key = topk_key(sc, (int32_t)r);
+                if (key >= t) {
+                    const int pos = atomicAdd(&cnt[q], 1);
+                    if (pos < cap) buf[(size_t)q * cap + pos] = key;
+                }
+            }
+        }
+    } else {
+        const uint32_t *bits = acc + (size_t)q * acc_stride;
+        constexpr int GPW = 32 / G;
+        const int gw = (threadIdx.x & 31) / G;
+        for (long long w = r0 / 32 + (threadIdx.x >> 5); w * 32 < r1; w += PQF_THREADS / 32) {
+            const uint32_t x = accept_word(bits, w, d.n);
+            const int p = __popc(x);
+            for (int i = gw; i < p; i += GPW) {
+                const int r = (int)(w * 32) + (int)__fns(x, 0, i + 1);
+                const float sc = score_pq<METRIC>(d, lut, r, lane);
+                if (lane == 0) {
+                    const long long key = topk_key(sc, r);
+                    if (key >= t) {
+                        const int pos = atomicAdd(&cnt[q], 1);
+                        if (pos < cap) buf[(size_t)q * cap + pos] = key;
+                    }
+                }
             }
         }
     }
@@ -491,7 +555,7 @@ __global__ void __launch_bounds__(256) topk_select_kernel(const long long *__res
 
 // aggressive threshold = j-th best of the sample with the smallest j such that j - 6 sqrt(j) >= k S / n: the j-th best of a
 // random sample has rank ~ j n / S (std sqrt(j) n / S) in the full set, so fewer than k survivors is a > 6 sigma event
-int topk_aggressive_rank(int k, int S, long long n)
+__host__ __device__ inline int aggressive_rank(int k, int S, long long n)
 {
     if (n <= S) return k;
     const double kf = (double)k * S / (double)n;
@@ -499,6 +563,7 @@ int topk_aggressive_rank(int k, int S, long long n)
         if ((double)j - 6.0 * sqrt((double)j) >= kf) return j;
     return k;
 }
+int topk_aggressive_rank(int k, int S, long long n) { return aggressive_rank(k, S, n); }
 
 // launch_topk_bruteforce's device scratch for nq queries, carved from `base` (nullptr: only measured)
 struct TopkScratch {
@@ -534,6 +599,66 @@ struct TopkScratch {
 
 size_t topk_scratch_bytes(const DataDesc &d, int nq, int k) { return TopkScratch(d, nq, k, nullptr).bytes; }
 
+// The filtered passes of the sampled top-k: `active` queries (qlist, nullptr = 0 .. active) hold thresholds in ts.thr; each pass
+// captures the keys >= thr, then topk_select_kernel finishes the exact queries and lists the rest for the next pass. acc != nullptr:
+// only the rows accepted by each query's bitset (acc + q * acc_stride words) take part (the ACC kernel instantiations).
+template <bool ACC>
+static cudaError_t topk_filter_passes(const DataDesc &d, int metric, const float *blobs_dev, int active, const int *qlist, int k, const TopkScratch &ts,
+                                      const uint32_t *acc, long long acc_stride, long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s)
+{
+    cudaError_t e;
+    const int cap2 = next_pow2(ts.cap);
+    if ((size_t)cap2 * sizeof(long long) > 48 * 1024)
+        if ((e = cudaFuncSetAttribute(topk_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap2 * (int)sizeof(long long))) != cudaSuccess) return e;
+    for (int pass = 0; pass < 8; pass++) {
+        int *qnext = (pass & 1) ? ts.qlist_a : ts.qlist_b;
+        if ((e = cudaMemsetAsync(overflow_flag_dev, 0, sizeof(int), s)) != cudaSuccess) return e;
+        if (d.kind == KIND_BQ && d.W <= 32) {
+            // popcount-bound: every CTA walks a slice of the rows against ALL active queries (rows in registers, queries in smem)
+            long long want = (d.n + BQF_THREADS - 1) / BQF_THREADS;
+            int dev = 0, sms = 0;
+            if ((e = cudaGetDevice(&dev)) != cudaSuccess || (e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+            int gridx = (int)(want < sms * 8LL ? want : sms * 8LL);
+#define CALLBQ(MW) topk_filter_bq_kernel<MW, ACC><<<gridx, BQF_THREADS, 0, s>>>(d, blobs_dev, blob_floats(d), active, ts.thr, ts.buf, ts.cnt, ts.cap, qlist, acc, acc_stride)
+            if (d.W <= 4) CALLBQ(4);
+            else if (d.W <= 8) CALLBQ(8);
+            else if (d.W <= 16) CALLBQ(16);
+            else if (d.W <= 24) CALLBQ(24);
+            else CALLBQ(32);
+#undef CALLBQ
+        } else if (d.kind == KIND_PQ && (size_t)blob_floats(d) * 4 <= 200 * 1024) {
+            dim3 grid(active, (unsigned)((d.n + PQF_TILE - 1) / PQF_TILE));
+            const int smem = blob_floats(d) * 4;
+#define CALLPQ(M)                                                                                                             \
+    do {                                                                                                                      \
+        if ((e = cudaFuncSetAttribute(topk_filter_pq_kernel<M, ACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e; \
+        topk_filter_pq_kernel<M, ACC><<<grid, PQF_THREADS, smem, s>>>(d, blobs_dev, blob_floats(d), ts.thr, ts.buf, ts.cnt, ts.cap, qlist, acc, acc_stride); \
+    } while (0)
+            if (metric == JV_METRIC_EUCLIDEAN) CALLPQ(JV_METRIC_EUCLIDEAN);
+            else if (metric == JV_METRIC_DOT) CALLPQ(JV_METRIC_DOT);
+            else CALLPQ(JV_METRIC_COSINE);
+#undef CALLPQ
+        } else {
+            dim3 grid(active, (unsigned)((d.n + BF_TILE - 1) / BF_TILE));
+            if (grid.y > 65535u) return cudaErrorInvalidValue;
+#define CALL(K, M) topk_filter_kernel<K, M, ACC><<<grid, BF_THREADS, 0, s>>>(d, blobs_dev, blob_floats(d), ts.thr, ts.buf, ts.cnt, ts.cap, qlist, acc, acc_stride)
+            JV_DISPATCH_KIND_METRIC(d.kind, metric, CALL);
+#undef CALL
+        }
+        g_launches++;
+        topk_select_kernel<<<active, 256, (size_t)cap2 * sizeof(long long), s>>>(ts.buf, ts.cnt, ts.cap, cap2, k, d.n, ts.thr, ts.thr_safe, keys_out_dev, overflow_flag_dev,
+                                                                                qlist, qnext);
+        g_launches++;
+        int redo = 0;
+        if ((e = cudaMemcpyAsync(&redo, overflow_flag_dev, sizeof(int), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
+        if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
+        if (redo == 0) return cudaGetLastError();  // overflow_flag_dev is left at 0
+        active = redo;
+        qlist = qnext;
+    }
+    return cudaGetLastError();  // overflow_flag_dev still holds the number of unresolved queries
+}
+
 cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, void *scratch_dev,
                                    long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s)
 {
@@ -551,58 +676,219 @@ cudaError_t launch_topk_bruteforce(const DataDesc &d, int metric, const float *b
     const int ja = topk_aggressive_rank(k, S, d.n);
     topk_threshold_kernel<<<nq, 256, (size_t)S2 * sizeof(long long), s>>>(ts.sample_scores, ts.sample_ids, S, S2, k, ja, whole, ts.thr, ts.thr_safe, ts.cnt);
     g_launches++;
-    const int cap2 = next_pow2(ts.cap);
-    if ((size_t)cap2 * sizeof(long long) > 48 * 1024)
-        if ((e = cudaFuncSetAttribute(topk_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap2 * (int)sizeof(long long))) != cudaSuccess) return e;
-    int active = nq;
-    const int *qlist = nullptr;
-    for (int pass = 0; pass < 8; pass++) {
-        int *qnext = (pass & 1) ? ts.qlist_a : ts.qlist_b;
-        if ((e = cudaMemsetAsync(overflow_flag_dev, 0, sizeof(int), s)) != cudaSuccess) return e;
-        if (d.kind == KIND_BQ && d.W <= 32) {
-            // popcount-bound: every CTA walks a slice of the rows against ALL active queries (rows in registers, queries in smem)
-            long long want = (d.n + BQF_THREADS - 1) / BQF_THREADS;
-            int dev = 0, sms = 0;
-            if ((e = cudaGetDevice(&dev)) != cudaSuccess || (e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
-            int gridx = (int)(want < sms * 8LL ? want : sms * 8LL);
-#define CALLBQ(MW) topk_filter_bq_kernel<MW><<<gridx, BQF_THREADS, 0, s>>>(d, blobs_dev, blob_floats(d), active, ts.thr, ts.buf, ts.cnt, ts.cap, qlist)
-            if (d.W <= 4) CALLBQ(4);
-            else if (d.W <= 8) CALLBQ(8);
-            else if (d.W <= 16) CALLBQ(16);
-            else if (d.W <= 24) CALLBQ(24);
-            else CALLBQ(32);
-#undef CALLBQ
-        } else if (d.kind == KIND_PQ && (size_t)blob_floats(d) * 4 <= 200 * 1024) {
-            dim3 grid(active, (unsigned)((d.n + PQF_TILE - 1) / PQF_TILE));
-            const int smem = blob_floats(d) * 4;
-#define CALLPQ(M)                                                                                                             \
-    do {                                                                                                                      \
-        if ((e = cudaFuncSetAttribute(topk_filter_pq_kernel<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)) != cudaSuccess) return e; \
-        topk_filter_pq_kernel<M><<<grid, PQF_THREADS, smem, s>>>(d, blobs_dev, blob_floats(d), ts.thr, ts.buf, ts.cnt, ts.cap, qlist);  \
-    } while (0)
-            if (metric == JV_METRIC_EUCLIDEAN) CALLPQ(JV_METRIC_EUCLIDEAN);
-            else if (metric == JV_METRIC_DOT) CALLPQ(JV_METRIC_DOT);
-            else CALLPQ(JV_METRIC_COSINE);
-#undef CALLPQ
-        } else {
-            dim3 grid(active, (unsigned)((d.n + BF_TILE - 1) / BF_TILE));
-            if (grid.y > 65535u) return cudaErrorInvalidValue;
-#define CALL(K, M) topk_filter_kernel<K, M><<<grid, BF_THREADS, 0, s>>>(d, blobs_dev, blob_floats(d), ts.thr, ts.buf, ts.cnt, ts.cap, qlist)
-            JV_DISPATCH_KIND_METRIC(d.kind, metric, CALL);
-#undef CALL
-        }
-        g_launches++;
-        topk_select_kernel<<<active, 256, (size_t)cap2 * sizeof(long long), s>>>(ts.buf, ts.cnt, ts.cap, cap2, k, d.n, ts.thr, ts.thr_safe, keys_out_dev, overflow_flag_dev,
-                                                                                qlist, qnext);
-        g_launches++;
-        int redo = 0;
-        if ((e = cudaMemcpyAsync(&redo, overflow_flag_dev, sizeof(int), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
-        if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
-        if (redo == 0) return cudaGetLastError();  // overflow_flag_dev is left at 0
-        active = redo;
-        qlist = qnext;
+    return topk_filter_passes<false>(d, metric, blobs_dev, nq, nullptr, k, ts, nullptr, 0, keys_out_dev, overflow_flag_dev, s);
+}
+
+// ---- acceptOrds-filtered top-k (jv_topk_bruteforce_ex, DESIGN §4.2a)
+constexpr int ACC_THREADS = 1024;  // 32 warps: the block scan's second level is one warp
+
+int accept_sample_size(long long n) { return n < 16384 ? (int)n : 16384; }  // = TopkScratch::S
+
+// One CTA per bitset: the popcounts of its words (bits at positions >= n cleared), an exclusive scan over the CTA, then the
+// accepted rows in ascending order. cnt[b] = accepted rows; ids[b * S + i], i < m = min(cnt, S) = the row of accepted rank
+// floor(i cnt / m): every accepted row when cnt <= S, else S evenly spaced ranks (the sampled tier's sample).
+__global__ void __launch_bounds__(ACC_THREADS) accept_compact_kernel(const uint32_t *__restrict__ bits, long long stride, long long n, int S,
+                                                                     int *__restrict__ cnt, int32_t *__restrict__ ids)
+{
+    __shared__ int warp_base[32];
+    __shared__ int s_total;
+    const uint32_t *b = bits + (size_t)blockIdx.x * stride;
+    const long long words = (n + 31) / 32;
+    const long long per = (words + ACC_THREADS - 1) / ACC_THREADS;
+    const long long w0 = min(words, (long long)threadIdx.x * per), w1 = min(words, w0 + per);
+    int c = 0;
+    for (long long w = w0; w < w1; w++) c += __popc(accept_word(b, w, n));
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int inc = c;
+    for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(FULL, inc, o);
+        if (lane >= o) inc += v;
     }
-    return cudaGetLastError();  // overflow_flag_dev still holds the number of unresolved queries
+    if (lane == 31) warp_base[wid] = inc;
+    __syncthreads();
+    if (wid == 0) {
+        const int t = warp_base[lane];
+        int ti = t;
+        for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(FULL, ti, o);
+            if (lane >= o) ti += v;
+        }
+        warp_base[lane] = ti - t;
+        if (lane == 31) s_total = ti;
+    }
+    __syncthreads();
+    const long long total = s_total, base = warp_base[wid] + inc - c;
+    if (threadIdx.x == 0) cnt[blockIdx.x] = (int)total;
+    const long long m = total < S ? total : S;
+    if (c == 0) return;
+    int32_t *out = ids + (size_t)blockIdx.x * S;
+    // the samples whose rank falls in this thread's [base, base + c): the first is i = ceil(base m / total)
+    long long i = (base * m + total - 1) / total, r = i * total / m, rank = base;
+    for (long long w = w0; w < w1 && i < m; w++) {
+        const uint32_t x = accept_word(b, w, n);
+        const int p = __popc(x);
+        while (i < m && r < rank + p) {
+            out[i] = (int32_t)(w * 32 + __fns(x, 0, (int)(r - rank) + 1));
+            i++;
+            r = i * total / m;
+        }
+        rank += p;
+    }
+}
+
+cudaError_t launch_accept_compact(const uint32_t *bits_dev, long long stride_words, int nsets, long long n, int *cnt_dev, int32_t *ids_dev, cudaStream_t s)
+{
+    if (nsets <= 0) return cudaSuccess;
+    accept_compact_kernel<<<nsets, ACC_THREADS, 0, s>>>(bits_dev, stride_words, n, accept_sample_size(n), cnt_dev, ids_dev);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+// the rows of accept_compact_kernel's lists, scored by gather: grid = (chunks, nq); query q scores ids[q * ids_stride + i],
+// i < min(cnt[q * cnt_stride], S), into scores[q * S + i]
+template <int KIND, int METRIC>
+__global__ void __launch_bounds__(RAGGED_THREADS) score_accepted_kernel(DataDesc d, const float *__restrict__ blobs, int blob_stride, const int32_t *__restrict__ ids,
+                                                                        long long ids_stride, const int *__restrict__ cnt, int cnt_stride, int S,
+                                                                        float *__restrict__ scores)
+{
+    constexpr int G = GroupOf<KIND>::value;
+    constexpr int NG = RAGGED_THREADS / G;
+    const int q = blockIdx.y;
+    const int m = min(cnt[q * cnt_stride], S);
+    const int c0 = blockIdx.x * RAGGED_CHUNK, c1 = min(m, c0 + RAGGED_CHUNK);
+    const float *blob = blobs + (size_t)q * blob_stride;
+    const int32_t *qi = ids + (size_t)q * ids_stride;
+    const int group = threadIdx.x / G, lane = threadIdx.x % G;
+    for (int i = c0 + group; i < c1; i += NG) {
+        const float sc = score_row<KIND, METRIC>(d, blob, qi[i], lane);
+        if (lane == 0) scores[(size_t)q * S + i] = sc;
+    }
+}
+
+// Per query: the keys of its accepted list (keys below floor_key, the score threshold, masked), their best next_pow2(k) sorted.
+// cnt <= S (whole tier): the list held every accepted row, so the best k are the answer. Otherwise the sampled thresholds of
+// topk_threshold_kernel with the 6-sigma rank taken over the accepted count, each raised to floor_key.
+__global__ void __launch_bounds__(256) topk_threshold_acc_kernel(const float *__restrict__ sample_scores, const int32_t *__restrict__ ids, long long ids_stride,
+                                                                 const int *__restrict__ acc_cnt, int cnt_stride, int S, int S_pow2, int k, long long floor_key,
+                                                                 long long *__restrict__ thr, long long *__restrict__ thr_safe, int *__restrict__ cnt,
+                                                                 long long *__restrict__ keys_out)
+{
+    extern __shared__ long long skeys[];
+    const int q = blockIdx.x;
+    const int total = acc_cnt[q * cnt_stride], m = min(total, S);
+    const int32_t *qi = ids + (size_t)q * ids_stride;
+    for (int i = threadIdx.x; i < S_pow2; i += blockDim.x) {
+        long long key = KEY_MIN;
+        if (i < m) {
+            key = topk_key(sample_scores[(size_t)q * S + i], qi[i]);
+            if (key < floor_key) key = KEY_MIN;
+        }
+        skeys[i] = key;
+    }
+    __syncthreads();
+    bitonic_top_desc(skeys, S_pow2, next_pow2(k));
+    if (total <= S) {
+        for (int i = threadIdx.x; i < k; i += blockDim.x) keys_out[(size_t)q * k + i] = skeys[i];
+        if (threadIdx.x == 0) thr[q] = KEY_DONE;
+        return;
+    }
+    if (threadIdx.x == 0) {
+        const int j = aggressive_rank(k, S, total);
+        const long long safe = max(skeys[k - 1], floor_key);
+        thr_safe[q] = safe;
+        thr[q] = j < k ? max(skeys[j - 1], floor_key) : safe;
+        cnt[q] = 0;
+    }
+}
+
+cudaError_t launch_topk_accepted(const DataDesc &d, int metric, const float *blobs_dev, int nq, int k, const AcceptLists &acc, long long floor_key,
+                                 void *scratch_dev, long long *keys_out_dev, int *overflow_flag_dev, cudaStream_t s)
+{
+    if (nq <= 0) return cudaSuccess;
+    cudaError_t e;
+    const TopkScratch ts(d, nq, k, scratch_dev);
+    const int S = ts.S;
+    const int cs = acc.per_query ? 1 : 0;
+    const long long is = acc.per_query ? S : 0;
+    if (acc.max_listed > 0) {
+        dim3 grid((acc.max_listed + RAGGED_CHUNK - 1) / RAGGED_CHUNK, nq);
+        if (grid.y > 65535u) return cudaErrorInvalidValue;
+#define CALL(K, M) score_accepted_kernel<K, M><<<grid, RAGGED_THREADS, 0, s>>>(d, blobs_dev, blob_floats(d), acc.ids, is, acc.cnt, cs, S, ts.sample_scores)
+        JV_DISPATCH_KIND_METRIC(d.kind, metric, CALL);
+#undef CALL
+        g_launches++;
+    }
+    const int S2 = next_pow2(std::max(std::max(acc.max_listed, k), 1));
+    if ((size_t)S2 * sizeof(long long) > 48 * 1024)
+        if ((e = cudaFuncSetAttribute(topk_threshold_acc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, S2 * (int)sizeof(long long))) != cudaSuccess) return e;
+    topk_threshold_acc_kernel<<<nq, 256, (size_t)S2 * sizeof(long long), s>>>(ts.sample_scores, acc.ids, is, acc.cnt, cs, S, S2, k, floor_key, ts.thr, ts.thr_safe, ts.cnt,
+                                                                              keys_out_dev);
+    g_launches++;
+    if (acc.n_sampled == 0) return cudaGetLastError();
+    return topk_filter_passes<true>(d, metric, blobs_dev, acc.n_sampled, acc.sampled, k, ts, acc.bits, acc.stride_words, keys_out_dev, overflow_flag_dev, s);
+}
+
+// ---- exhaustive search: NodeQueue.rerank's take rule over the candidates, exact rescoring, key order
+// ids[q][i] = the candidate's node when it is reranked, else -1: a candidate is taken when its approximate score is >= floor, and the
+// best one (i = 0, the keys are sorted) when none is
+__global__ void __launch_bounds__(256) rerank_take_kernel(const long long *__restrict__ cand, int nq, int R, float floor, int32_t *__restrict__ ids,
+                                                          int32_t *__restrict__ offsets, unsigned long long *__restrict__ taken)
+{
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t <= nq) offsets[t] = (int32_t)(t * R);  // query q's candidates are ids[q R .. (q + 1) R)
+    bool take = false;
+    if (t < (long long)nq * R) {
+        const long long key = cand[t];
+        take = key != KEY_MIN && (t % R == 0 || key_score(key) >= floor);
+        ids[t] = take ? key_node(key) : -1;
+    }
+    const unsigned b = __ballot_sync(FULL, take);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(taken, (unsigned long long)__popc(b));
+}
+
+// one CTA per query: the topK best of its taken candidates by exact key (exact == nullptr: the first topK candidates as they are),
+// nodes -1 and scores 0 past the end
+__global__ void __launch_bounds__(256) rerank_finish_kernel(const long long *__restrict__ cand, const int32_t *__restrict__ ids, const float *__restrict__ exact, int R,
+                                                            int R_pow2, int topK, int32_t *__restrict__ nodes, float *__restrict__ scores)
+{
+    extern __shared__ long long skeys[];
+    const int q = blockIdx.x;
+    const long long *src = cand + (size_t)q * R;
+    if (exact) {
+        for (int i = threadIdx.x; i < R_pow2; i += blockDim.x) {
+            const int32_t f = i < R ? ids[(size_t)q * R + i] : -1;
+            skeys[i] = f >= 0 ? topk_key(exact[(size_t)q * R + i], f) : KEY_MIN;
+        }
+        __syncthreads();
+        bitonic_top_desc(skeys, R_pow2, next_pow2(topK));
+        src = skeys;
+    }
+    for (int i = threadIdx.x; i < topK; i += blockDim.x) {
+        const long long key = src[i];
+        nodes[(size_t)q * topK + i] = key == KEY_MIN ? -1 : key_node(key);
+        scores[(size_t)q * topK + i] = key == KEY_MIN ? 0.f : key_score(key);
+    }
+}
+
+cudaError_t launch_rerank_accepted(const DataDesc *rr, int metric, const float *rblobs_dev, int nq, int R, int topK, float floor, const long long *cand_dev,
+                                   int32_t *ids_dev, int32_t *offsets_dev, float *exact_dev, unsigned long long *taken_dev, int32_t *nodes_dev, float *scores_dev,
+                                   cudaStream_t s)
+{
+    if (nq <= 0) return cudaSuccess;
+    cudaError_t e;
+    int R2 = 0;
+    if (rr) {
+        const long long threads = std::max((long long)nq * R, (long long)nq + 1);
+        rerank_take_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(cand_dev, nq, R, floor, ids_dev, offsets_dev, taken_dev);
+        g_launches++;
+        if ((e = launch_score_ragged(*rr, metric, rblobs_dev, nq, ids_dev, offsets_dev, 0, R, exact_dev, s)) != cudaSuccess) return e;
+        R2 = next_pow2(std::max(R, topK));
+        if ((size_t)R2 * sizeof(long long) > 48 * 1024)
+            if ((e = cudaFuncSetAttribute(rerank_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R2 * (int)sizeof(long long))) != cudaSuccess) return e;
+    }
+    rerank_finish_kernel<<<nq, 256, (size_t)R2 * sizeof(long long), s>>>(cand_dev, ids_dev, rr ? exact_dev : nullptr, R, R2, topK, nodes_dev, scores_dev);
+    g_launches++;
+    return cudaGetLastError();
 }
 
 __global__ void add_int_kernel(int *dst, const int *src) { *dst += *src; }
