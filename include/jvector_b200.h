@@ -394,6 +394,30 @@ JV_API int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, in
                                       int rerankK, const jv_search_options *opts, int32_t *nodes_out, float *scores_out,
                                       jv_search_stats *stats);
 
+/* Segments: one index split into segment graphs, each over its own rows (data arrives as small segment indexes that are compacted
+ * from time to time, jv_graph_compact), searched in one call. Segment s answers what
+ *   jv_graph_search_batch_ex(graph, approx, reranker, metric, queries, nq, topK, rerankK, {accept_bits, 0, threshold, rerank_floor})
+ * answers, or, with graph == NULL, what jv_exhaustive_search_batch answers with the same arguments; a graph whose every node was
+ * removed answers nothing. Each query's output is the first topK entries of the stable merge of those lists: padding dropped, score
+ * descending (compared as the top-k key's sortable score), equal scores in segment order, then in list order; padded with segment -1,
+ * node -1, score 0. With one segment, nodes_out and scores_out are jv_graph_search_batch_ex's bytes.
+ * Every walked (segment, query) pair runs in one launch per kind of walk (segments with and without edge records, DESIGN §4.1); the
+ * merge runs on the device. Segments keep their own codebooks; they must share the device, the storage kind and dim (PQ: M and k,
+ * NVQ: sub-vectors) and the reranker kind (all NULL or all of one kind). stats sums the segments' visited, expanded, expanded_base
+ * and reranked; retried counts the (segment, query) pairs re-run; device_ms is the CUDA-event time of the call. segment_stats
+ * (NULL or [nsegments]): each segment's counters as its own call reports them, with this call's retried and device_ms.
+ * JV_ERR_UNSUPPORTED: nsegments > 1024, nsegments * topK > 16384, rerankK > 4096 (2048 with a segment without graph), or what the
+ * segment's own call refuses as unsupported. All checks precede any device work: a refused call writes no output. */
+typedef struct {
+    jv_graph graph;              /* NULL: the segment is searched as jv_exhaustive_search_batch searches it */
+    jv_dataset approx;           /* walked (or scanned) scores; its n is the graph's n */
+    jv_dataset reranker;         /* NULL, or fp32 / NVQ, as for jv_graph_search_batch_ex */
+    const uint32_t *accept_bits; /* host; one bitset over the segment's n, shared by every query (the segment's live rows); NULL = all */
+} jv_search_segment;
+JV_API int jv_segments_search_batch(const jv_search_segment *segments, int nsegments, int metric, const float *queries, int nq, int topK,
+                                    int rerankK, float threshold, float rerank_floor, int32_t *segments_out, int32_t *nodes_out,
+                                    float *scores_out, jv_search_stats *stats, jv_search_stats *segment_stats);
+
 /* Replicas: graph + data sets registered once per device (jv_gpu_set_device(d), then the ordinary create / register calls); the
  * batch is split into contiguous slices, one per replica, searched concurrently (no data-path exchange). stats sums the counters,
  * device_ms is the slowest replica. */

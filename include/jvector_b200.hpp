@@ -189,6 +189,48 @@ public:
     }
 };
 
+/// SegmentSearcher::search's answer: segments / nodes / scores [nq][topK] best first (-1, -1, 0 padded), the call's counters and each
+/// segment's (jv_segments_search_batch)
+struct SegmentSearchResult {
+    std::vector<int32_t> segments, nodes;
+    std::vector<float> scores;
+    int topK = 0;
+    jv_search_stats stats{};
+    std::vector<jv_search_stats> segmentStats;
+};
+
+/// GraphSearcher::search over several segment graphs (a segment without graph: ExhaustiveSearcher::search), the answers merged per
+/// query on the device: score descending, equal scores in segment order, then in the segment's own order
+class SegmentSearcher {
+public:
+    struct Segment {
+        const GraphIndex *graph;         // nullptr: every accepted row is scored
+        const Vectors *approx;
+        const Vectors *reranker;         // nullptr: none
+        const uint32_t *acceptBits;      // one bitset over the segment's rows, shared by every query (its live rows); nullptr: all
+    };
+    explicit SegmentSearcher(std::vector<Segment> segments) : segs_(std::move(segments)) {}
+    SegmentSearchResult search(const float *queries, int nq, VectorSimilarityFunction vsf, int topK, int rerankK, float threshold = 0.f,
+                               float rerankFloor = 0.f) const
+    {
+        std::vector<jv_search_segment> s;
+        for (const Segment &g : segs_)
+            s.push_back({g.graph ? g.graph->handle() : nullptr, g.approx ? g.approx->handle() : nullptr, g.reranker ? g.reranker->handle() : nullptr, g.acceptBits});
+        SegmentSearchResult r;
+        r.topK = topK;
+        r.segments.resize((size_t)nq * topK);
+        r.nodes.resize((size_t)nq * topK);
+        r.scores.resize((size_t)nq * topK);
+        r.segmentStats.resize(s.size());
+        check(jv_segments_search_batch(s.data(), (int)s.size(), (int)vsf, queries, nq, topK, rerankK, threshold, rerankFloor, r.segments.data(), r.nodes.data(),
+                                       r.scores.data(), &r.stats, r.segmentStats.data()));
+        return r;
+    }
+
+private:
+    std::vector<Segment> segs_;
+};
+
 /// exhaustive top-k keys [nq][k] over the rows the options accept (jv_topk_bruteforce_ex; opts nullptr: every row)
 inline std::vector<int64_t> topkBruteforce(const Vectors &v, const float *queries, int nq, VectorSimilarityFunction vsf, int k, const jv_search_options *opts = nullptr)
 {

@@ -9,6 +9,7 @@ mirror of the reference's interface for that path, used by the tests and the ben
   ScoreFunction (similarityTo / similarityToBatch)  base:graph/similarity/ScoreFunction.java
   GraphIndex, GraphSearcher.search              base:graph/GraphSearcher.java:222
   ExhaustiveSearcher.search                     GraphSearcher.search's arguments over every accepted row (no graph)
+  SegmentSearcher.search                        GraphSearcher.search over several segment graphs, answers merged on the device
   GraphIndexBuilder.build                       base:graph/GraphIndexBuilder.java:436
   GraphIndexBuilder.refine                      base:graph/GraphIndexBuilder.java:472-538 (cleanup's improveConnections)
   GraphIndexCompactor.compact                   graph/disk/OnDiskGraphIndexCompactor.java (the per-node merge, fp32, FusedPQ or
@@ -16,10 +17,10 @@ mirror of the reference's interface for that path, used by the tests and the ben
 """
 from . import api
 from .api import (BQVectors, ExhaustiveSearcher, F32Vectors, GraphIndex, GraphIndexBuilder, GraphIndexCompactor, GraphSearcher, NVQVectors, PQVectors,
-                  ProductQuantization, QueryBatch, ScoreFunction, SearchResult, VectorSimilarityFunction, bq_encode_all, kmeans_assign, nvq_encode_all, nvq_encode_resident,
+                  ProductQuantization, QueryBatch, ScoreFunction, SearchResult, SegmentSearcher, SegmentSearchResult, VectorSimilarityFunction, bq_encode_all, kmeans_assign, nvq_encode_all, nvq_encode_resident,
                   pack_accept_bits, pq_encode_all, pq_encode_all_anisotropic, pq_encode_resident, score_multi, topk_bruteforce)
 from ._native import JVectorB200Error, init, load
 
 __all__ = ["VectorSimilarityFunction", "F32Vectors", "PQVectors", "BQVectors", "NVQVectors", "ProductQuantization", "ScoreFunction", "GraphIndex",
-           "GraphSearcher", "ExhaustiveSearcher", "GraphIndexBuilder", "GraphIndexCompactor", "SearchResult", "score_multi", "topk_bruteforce", "bq_encode_all",
+           "GraphSearcher", "ExhaustiveSearcher", "SegmentSearcher", "SegmentSearchResult", "GraphIndexBuilder", "GraphIndexCompactor", "SearchResult", "score_multi", "topk_bruteforce", "bq_encode_all",
            "pq_encode_all", "pq_encode_all_anisotropic", "pq_encode_resident", "nvq_encode_all", "nvq_encode_resident", "QueryBatch", "kmeans_assign", "pack_accept_bits", "JVectorB200Error", "init", "load"]

@@ -31,6 +31,10 @@ class SearchOptions(C.Structure):
     _fields_ = [("accept_bits", C.c_void_p), ("accept_stride_words", C.c_int64), ("threshold", C.c_float), ("rerank_floor", C.c_float)]
 
 
+class SearchSegment(C.Structure):
+    _fields_ = [("graph", C.c_void_p), ("approx", C.c_void_p), ("reranker", C.c_void_p), ("accept_bits", C.c_void_p)]
+
+
 class BuildParams(C.Structure):
     _fields_ = [("degree", C.c_int), ("beam_width", C.c_int), ("overflow", C.c_float), ("alpha", C.c_float),
                 ("add_hierarchy", C.c_int), ("seed", C.c_uint64), ("max_batch", C.c_int), ("concurrent_window", C.c_int)]
@@ -155,6 +159,8 @@ SYMBOLS = [
     ("jv_graph_search_batch_device_ex", _I, [_P, _P, _P, _I, _P, _I, _I, _I, C.POINTER(SearchOptions), _P, _P, C.POINTER(SearchStats)]),
     ("jv_topk_bruteforce_ex", _I, [_P, _I, f32p, _I, _I, C.POINTER(SearchOptions), i64p]),
     ("jv_exhaustive_search_batch", _I, [_P, _P, _I, f32p, _I, _I, _I, C.POINTER(SearchOptions), i32p, f32p, C.POINTER(SearchStats)]),
+    ("jv_segments_search_batch", _I, [C.POINTER(SearchSegment), _I, _I, f32p, _I, _I, _I, _F, _F, i32p, i32p, f32p, C.POINTER(SearchStats),
+                                      C.POINTER(SearchStats)]),
     ("jv_graph_build", _I, [_P, _I, C.POINTER(BuildParams), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_graph_build_pq", _I, [_P, _I, C.POINTER(BuildParams), C.POINTER(_P), C.POINTER(C.c_double)]),
     ("jv_builder_create_pq", _I, [_P, _I, C.POINTER(BuildParams), _P, C.POINTER(_P)]),

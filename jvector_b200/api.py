@@ -554,6 +554,56 @@ class ExhaustiveSearcher:
         return SearchResult(nodes, scores, st)
 
 
+class SegmentSearchResult:
+    """SegmentSearcher.search's answer: segments / nodes / scores [nq][topK] best first (segment -1, node -1, score 0 padded), the
+    call's counters (`stats`, a SearchResult's counters without its arrays) and each segment's (`segment_stats`, a list)."""
+
+    def __init__(self, segments, nodes, scores, stats, segment_stats):
+        self.segments, self.nodes, self.scores = segments, nodes, scores
+        self.stats = SearchResult(None, None, stats)
+        self.segment_stats = [SearchResult(None, None, st) for st in segment_stats]
+
+
+class SegmentSearcher:
+    """One index split into segments, each searched as GraphSearcher.search (or, without a graph, ExhaustiveSearcher.search) searches
+    it, and the answers merged per query on the device (jv_segments_search_batch): score descending, equal scores in segment order,
+    then in each segment's own order. segments: a list of (graph or None, approx, reranker=None, acceptOrds=None), acceptOrds a bool
+    array over the segment's rows shared by every query (its live rows)."""
+
+    def __init__(self, segments):
+        self.segments = [tuple(s) + (None,) * (4 - len(s)) for s in segments]
+        if not self.segments:
+            raise ValueError("SegmentSearcher needs at least one segment")
+
+    def search(self, queries, vsf, topK, rerankK=None, threshold=0.0, rerankFloor=0.0):
+        lib = nat.init()
+        queries = c32(queries)
+        dim = self.segments[0][1].dimension()
+        if queries.shape[1] != dim:
+            raise ValueError("query dimension %d != data set dimension %d" % (queries.shape[1], dim))
+        rerankK = rerankK or topK
+        nq, S = queries.shape[0], len(self.segments)
+        arr = (nat.SearchSegment * S)()
+        keep = []  # the packed bitsets live until the call returns
+        for i, (graph, approx, reranker, accept) in enumerate(self.segments):
+            bits = None
+            if accept is not None:
+                bits = pack_accept_bits(accept)
+                if bits.ndim != 1:
+                    raise ValueError("segment %d: acceptOrds is one bool array over the segment's rows" % i)
+                keep.append(bits)
+            arr[i] = nat.SearchSegment(graph._h if graph is not None else None, approx._h, reranker._h if reranker is not None else None,
+                                       bits.ctypes.data if bits is not None else None)
+        segs = np.empty((nq, topK), dtype=np.int32)
+        nodes = np.empty((nq, topK), dtype=np.int32)
+        scores = np.empty((nq, topK), dtype=np.float32)
+        st = nat.SearchStats()
+        sst = (nat.SearchStats * S)()
+        check(lib.jv_segments_search_batch(arr, S, int(vsf), fp(queries), nq, topK, rerankK, float(threshold), float(rerankFloor), ip(segs), ip(nodes),
+                                           fp(scores), C.byref(st), sst))
+        return SegmentSearchResult(segs, nodes, scores, st, list(sst))
+
+
 def pack_accept_bits(mask):
     """bool [n] or [nq][n] -> uint32 words, bit (node & 31) of word (node >> 5) (the layout jv_search_options.accept_bits takes)"""
     m = np.asarray(mask, dtype=bool)

@@ -88,6 +88,7 @@ struct ThreadCtx {
     DeviceBuffer accept_lists;  // filtered top-k: accepted counts, accepted-row lists, the sampled tier's query list
     DeviceBuffer rerank;        // exhaustive search: candidate keys, the reranker's prepared queries, taken ids, exact scores
     DeviceBuffer watermark;     // host-pointer searches: the arrival watermark the copy stream writes
+    DeviceBuffer segments;      // multi-segment search: queries, bitsets, segment descriptors, per-segment answers and counters, merged answers
     StreamTimer timer;
     // host-pointer searches: a second stream carries the query chunks while the search kernel already runs (arrival watermark)
     cudaStream_t copy_stream = nullptr;
@@ -112,7 +113,7 @@ struct ThreadCtx {
     template <typename F>
     void each_owner(F f)
     {
-        for (DeviceBuffer *b : {&input, &aux, &blobs, &output, &topk_scratch, &bq_scratch, &flag, &bq_async, &search_scratch, &search_aux, &accept_bits, &accept_lists, &rerank, &watermark})
+        for (DeviceBuffer *b : {&input, &aux, &blobs, &output, &topk_scratch, &bq_scratch, &flag, &bq_async, &search_scratch, &search_aux, &accept_bits, &accept_lists, &rerank, &watermark, &segments})
             f(*b);
         f(marks);
         f(timer);
@@ -950,19 +951,27 @@ int jv_topk_bruteforce_ex(jv_dataset ds, int metric, const float *queries, int n
 
 constexpr int EXHAUSTIVE_QUERY_CHUNK = 4096;  // queries per candidate / rerank step (bounds the candidate keys and rerank scratch)
 
-int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, int metric, const float *queries, int nq, int topK, int rerankK,
-                               const jv_search_options *opts, int32_t *nodes_out, float *scores_out, jv_search_stats *stats)
+// jv_exhaustive_search_batch's checks of its arguments (rerankK's bound excepted)
+static int exhaustive_check(jv_dataset approx, jv_dataset reranker, int metric, int topK, int rerankK, const jv_search_options *opts)
 {
-    ON_DEVICE_OF(approx);
-    if (!queries || !nodes_out || !scores_out || nq <= 0) return fail(JV_ERR_INVALID, "exhaustive_search: bad arguments");
     if (topK < 1 || rerankK < topK) return fail(JV_ERR_INVALID, "exhaustive_search: need 1 <= topK <= rerankK");
-    if (rerankK > 2048) return fail(JV_ERR_INVALID, "exhaustive_search: rerankK <= 2048");
     if (reranker && reranker->device != approx->device) return fail(JV_ERR_INVALID, "exhaustive_search: data sets live on different devices");
     if (reranker && (reranker->d.n != approx->d.n || reranker->d.dim != approx->d.dim)) return fail(JV_ERR_INVALID, "exhaustive_search: reranker shape mismatch");
     if (reranker && reranker->d.kind != KIND_F32 && reranker->d.kind != KIND_NVQ)
         return fail(JV_ERR_UNSUPPORTED, "exhaustive_search: the reranker must be fp32 or NVQ (OnDiskGraphIndex.java:705-713)");
     int rc = check_accept_options(opts, approx->d.n, "exhaustive_search");
     if (rc || (rc = check_metric(approx->d, metric))) return rc;
+    return JV_OK;
+}
+
+// jv_exhaustive_search_batch's device work: the queries' answers [nq][topK] from the nq queries in HBM (queries_dev; nullptr: copied
+// chunk by chunk from the host `queries` into the thread's input buffer) into nodes_dev / scores_dev (nullptr: each chunk is
+// downloaded to the host nodes_out / scores_out); *visited += the rows scored, *taken = the candidates reranked. Asynchronous on the
+// thread's stream, which the host must synchronise before it reads what the call downloads, *taken included.
+static int exhaustive_device(jv_dataset approx, jv_dataset reranker, int metric, const float *queries, const float *queries_dev, int nq, int topK,
+                             int rerankK, const jv_search_options *opts, int32_t *nodes_out, float *scores_out, int32_t *nodes_dev, float *scores_dev,
+                             int64_t *visited, unsigned long long *taken)
+{
     const bool filtered = opts && (opts->accept_bits || opts->threshold > 0.f);
     const float floor = opts ? opts->rerank_floor : 0.f;
     const int R = rerankK, chunk = std::min(nq, EXHAUSTIVE_QUERY_CHUNK);
@@ -974,8 +983,8 @@ int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, int metri
     auto carve = [&](void *base) {
         Carver c(base);
         dcand = c.take<long long>((size_t)chunk * R);
-        dnodes = c.take<int32_t>((size_t)chunk * topK);
-        dscores = c.take<float>((size_t)chunk * topK);
+        dnodes = c.take<int32_t>(nodes_dev ? 0 : (size_t)chunk * topK);
+        dscores = c.take<float>(nodes_dev ? 0 : (size_t)chunk * topK);
         dtaken = c.take<unsigned long long>(1);
         drblobs = c.take<float>(reranker ? (size_t)chunk * rbf : 0);
         dids = c.take<int32_t>(reranker ? (size_t)chunk * R : 0);
@@ -983,34 +992,58 @@ int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, int metri
         dexact = c.take<float>(reranker ? (size_t)chunk * R : 0);
         return c.bytes;
     };
-    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.input, (size_t)chunk * approx->d.dim * 4)) || (rc = grow(t_ctx.rerank, carve(nullptr)))) return rc;
+    int rc;
+    if ((rc = t_ctx.init()) || (!queries_dev && (rc = grow(t_ctx.input, (size_t)chunk * approx->d.dim * 4))) || (rc = grow(t_ctx.rerank, carve(nullptr)))) return rc;
     carve(t_ctx.rerank.get());
     cudaStream_t s = t_ctx.stream;
-    float *dq = t_ctx.input.get<float>();
-    int64_t visited = 0;
     CK(cudaMemsetAsync(dtaken, 0, sizeof(unsigned long long), s), "memset taken");
-    CK(t_ctx.timer.start(s), "event");
     for (int q0 = 0; q0 < nq; q0 += chunk) {
         const int cq = std::min(chunk, nq - q0);
-        const float *qh = queries + (size_t)q0 * approx->d.dim;
-        CK(cudaMemcpyAsync(dq, qh, (size_t)cq * approx->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+        const float *dq;
+        if (queries_dev) dq = queries_dev + (size_t)q0 * approx->d.dim;
+        else {
+            CK(cudaMemcpyAsync(t_ctx.input.get(), queries + (size_t)q0 * approx->d.dim, (size_t)cq * approx->d.dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+            dq = t_ctx.input.get<float>();
+        }
         if (filtered) {
             jv_search_options o = *opts;
             if (o.accept_bits && o.accept_stride_words) o.accept_bits += (size_t)q0 * o.accept_stride_words;
-            if ((rc = topk_accepted_device(approx, metric, dq, cq, R, &o, dcand, &visited))) return rc;
+            if ((rc = topk_accepted_device(approx, metric, dq, cq, R, &o, dcand, visited))) return rc;
         } else {
             if ((rc = topk_device(approx, metric, dq, cq, R, 0, dcand))) return rc;
-            visited += (int64_t)cq * approx->d.n;
+            *visited += (int64_t)cq * approx->d.n;
         }
+        int32_t *on = nodes_dev ? nodes_dev + (size_t)q0 * topK : dnodes;
+        float *os = nodes_dev ? scores_dev + (size_t)q0 * topK : dscores;
         if (reranker) CK(launch_prepare(reranker->d, metric, dq, cq, drblobs, s), "prepare reranker");
-        CK(launch_rerank_accepted(reranker ? &reranker->d : nullptr, metric, drblobs, cq, R, topK, floor, dcand, dids, doffsets, dexact, dtaken, dnodes, dscores, s),
+        CK(launch_rerank_accepted(reranker ? &reranker->d : nullptr, metric, drblobs, cq, R, topK, floor, dcand, dids, doffsets, dexact, dtaken, on, os, s),
            "rerank");
-        CK(cudaMemcpyAsync(nodes_out + (size_t)q0 * topK, dnodes, (size_t)cq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H nodes");
-        CK(cudaMemcpyAsync(scores_out + (size_t)q0 * topK, dscores, (size_t)cq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+        if (!nodes_dev) {
+            CK(cudaMemcpyAsync(nodes_out + (size_t)q0 * topK, dnodes, (size_t)cq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H nodes");
+            CK(cudaMemcpyAsync(scores_out + (size_t)q0 * topK, dscores, (size_t)cq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+        }
     }
-    CK(t_ctx.timer.stop(s), "event");
+    CK(cudaMemcpyAsync(taken, dtaken, sizeof(*taken), cudaMemcpyDeviceToHost, s), "D2H taken");
+    return JV_OK;
+}
+
+int jv_exhaustive_search_batch(jv_dataset approx, jv_dataset reranker, int metric, const float *queries, int nq, int topK, int rerankK,
+                               const jv_search_options *opts, int32_t *nodes_out, float *scores_out, jv_search_stats *stats)
+{
+    ON_DEVICE_OF(approx);
+    if (!queries || !nodes_out || !scores_out || nq <= 0) return fail(JV_ERR_INVALID, "exhaustive_search: bad arguments");
+    if (topK < 1 || rerankK < topK) return fail(JV_ERR_INVALID, "exhaustive_search: need 1 <= topK <= rerankK");
+    if (rerankK > 2048) return fail(JV_ERR_INVALID, "exhaustive_search: rerankK <= 2048");
+    int rc = exhaustive_check(approx, reranker, metric, topK, rerankK, opts);
+    if (rc) return rc;
+    if ((rc = t_ctx.init())) return rc;
+    cudaStream_t s = t_ctx.stream;
+    int64_t visited = 0;
     unsigned long long taken = 0;
-    CK(cudaMemcpyAsync(&taken, dtaken, sizeof(taken), cudaMemcpyDeviceToHost, s), "D2H taken");
+    CK(t_ctx.timer.start(s), "event");
+    if ((rc = exhaustive_device(approx, reranker, metric, queries, nullptr, nq, topK, rerankK, opts, nodes_out, scores_out, nullptr, nullptr, &visited, &taken)))
+        return rc;
+    CK(t_ctx.timer.stop(s), "event");
     CK(cudaStreamSynchronize(s), "sync");
     if (stats) {
         memset(stats, 0, sizeof(*stats));
@@ -1936,6 +1969,287 @@ int jv_graph_search_batch(jv_graph g, jv_dataset approx, jv_dataset reranker, in
                           int32_t *nodes_out, float *scores_out, jv_search_stats *stats)
 {
     return jv_graph_search_batch_ex(g, approx, reranker, metric, queries, nq, topK, rerankK, nullptr, nodes_out, scores_out, stats);
+}
+
+// ------------------------------------------------------------------------------------------------ segments
+constexpr int MAX_SEGMENTS = 1024;  // the merge key holds the segment in 10 bits (and the list position in 12)
+
+int jv_segments_search_batch(const jv_search_segment *segments, int nsegments, int metric, const float *queries, int nq, int topK, int rerankK,
+                             float threshold, float rerank_floor, int32_t *segments_out, int32_t *nodes_out, float *scores_out, jv_search_stats *stats,
+                             jv_search_stats *segment_stats)
+{
+    if (!segments || !queries || !segments_out || !nodes_out || !scores_out) return fail(JV_ERR_INVALID, "segments_search: bad arguments");
+    if (nsegments < 1 || nq <= 0 || topK < 1 || rerankK < topK) return fail(JV_ERR_INVALID, "segments_search: need nsegments >= 1, nq >= 1 and 1 <= topK <= rerankK");
+    const int S = nsegments;
+    for (int i = 0; i < S; i++)
+        if (!segments[i].approx) return fail(JV_ERR_INVALID, "segments_search: segment " + std::to_string(i) + " has no data set");
+    ON_DEVICE_OF(segments[0].approx);
+    // ---- every check before any device work
+    const jv_dataset a0 = segments[0].approx, r0 = segments[0].reranker;
+    bool exhaustive = false;
+    for (int i = 0; i < S; i++) {
+        const jv_search_segment &sg = segments[i];
+        const std::string who = "segments_search: segment " + std::to_string(i);
+        const jv_dataset a = sg.approx, r = sg.reranker;
+        if (a->device != a0->device || (sg.graph && sg.graph->device != a0->device) || (r && r->device != a0->device))
+            return fail(JV_ERR_INVALID, who + " lives on another device");
+        if (sg.graph && sg.graph->g.n != a->d.n) return fail(JV_ERR_INVALID, who + ": data set and graph sizes differ");
+        if (a->d.kind != a0->d.kind || a->d.dim != a0->d.dim) return fail(JV_ERR_INVALID, who + ": data sets of different kinds or dims");
+        if ((a->d.kind == KIND_PQ && (a->d.M != a0->d.M || a->d.k != a0->d.k)) || (a->d.kind == KIND_NVQ && a->d.nsub != a0->d.nsub))
+            return fail(JV_ERR_INVALID, who + ": PQ data sets of different M or k, or NVQ data sets of different sub-vectors");
+        if ((r == nullptr) != (r0 == nullptr) || (r && (r->d.kind != r0->d.kind || (r->d.kind == KIND_NVQ && r->d.nsub != r0->d.nsub))))
+            return fail(JV_ERR_INVALID, who + ": rerankers mixed or of different kinds");
+        if (!sg.graph) exhaustive = true;
+    }
+    int rc = check_metric(a0->d, metric);
+    if (rc) return rc;
+    if (!(threshold >= 0.f) || !(rerank_floor >= 0.f)) return fail(JV_ERR_INVALID, "segments_search: negative threshold / rerankFloor");
+    if (S > MAX_SEGMENTS) return fail(JV_ERR_UNSUPPORTED, "segments_search: nsegments <= 1024");
+    if ((long long)S * topK > SEGMENT_MERGE_MAX_KEYS) return fail(JV_ERR_UNSUPPORTED, "segments_search: nsegments * topK <= 16384 (the merge sorts them in shared memory)");
+    if (rerankK > 4096 || (exhaustive && rerankK > 2048))
+        return fail(JV_ERR_UNSUPPORTED, "segments_search: rerankK <= 4096, and <= 2048 with a segment without graph");
+    std::vector<int> walked;  // the segments with a graph that has an entry, in segment order
+    GraphDesc gmax;           // what the plan sizes for: the largest n and degree among them
+    memset(&gmax, 0, sizeof(gmax));
+    for (int i = 0; i < S; i++) {
+        const jv_search_segment &sg = segments[i];
+        const jv_dataset a = sg.approx, r = sg.reranker;
+        jv_search_options o = {sg.accept_bits, 0, threshold, rerank_floor};
+        if (!sg.graph) {
+            if ((rc = exhaustive_check(a, r, metric, topK, rerankK, &o))) return rc;
+            continue;
+        }
+        if (r && (r->d.n != a->d.n || r->d.dim != a->d.dim)) return fail(JV_ERR_INVALID, "segments_search: segment " + std::to_string(i) + ": reranker shape mismatch");
+        if (r && r->d.kind != KIND_F32 && r->d.kind != KIND_NVQ)
+            return fail(JV_ERR_UNSUPPORTED, "segments_search: the reranker must be fp32 or NVQ (OnDiskGraphIndex.java:705-713)");
+        if (sg.graph->g.entry_node < 0) continue;  // every node removed: nothing to walk
+        walked.push_back(i);
+        gmax.n = std::max(gmax.n, sg.graph->g.n);
+        gmax.degree = std::max(gmax.degree, sg.graph->g.degree);
+    }
+    const int W = (int)walked.size();
+    const DataDesc *rr0 = r0 ? &r0->d : nullptr;
+    const char *cap_env = getenv("JV_VISITED_CAP");
+    const char *lcap_env = getenv("JV_LIST_CAP");
+    const int cap_hint = cap_env ? std::max(0, atoi(cap_env)) : 0, lcap_hint = lcap_env ? std::max(0, atoi(lcap_env)) : 0;
+    SearchPlan plan;
+    if (W && (plan_search(a0->d, rr0, gmax, topK, rerankK, W * nq, cap_hint, lcap_hint, g_sm_count, &plan) != cudaSuccess ||
+              plan.smem_bytes + sizeof(SegmentDesc) > 227 * 1024)) {
+        cudaGetLastError();
+        return fail(JV_ERR_UNSUPPORTED, "segments_search: no walk of these segments fits an SM (degree, rerankK or codebook too large)");
+    }
+
+    // ---- device buffers: queries, the walked segments' bitsets, descriptors, answers [S][nq][topK], overflow codes [S][nq],
+    // counters [S], retry index, merged answers [nq][topK]
+    std::vector<size_t> bits_off(S, 0);
+    size_t bit_words = 0;
+    for (int i : walked)
+        if (segments[i].accept_bits) {
+            bits_off[i] = bit_words;
+            bit_words += ((size_t)segments[i].approx->d.n + 31) / 32;
+        }
+    const size_t rows = (size_t)S * nq, dim = (size_t)a0->d.dim;
+    float *dq, *dscores, *mscores;
+    uint32_t *dbits;
+    SegmentDesc *ddesc;
+    int32_t *dnodes, *dindex, *mseg, *mnodes;
+    uint8_t *dover;
+    SearchCounters *dcnt;
+    int *dwork;
+    auto carve = [&](void *base) {
+        Carver c(base);
+        dq = c.take<float>((size_t)nq * dim);
+        dbits = c.take<uint32_t>(bit_words);
+        ddesc = c.take<SegmentDesc>(W);
+        dnodes = c.take<int32_t>(rows * topK);
+        dscores = c.take<float>(rows * topK);
+        dover = c.take<uint8_t>(rows);
+        dcnt = c.take<SearchCounters>(S);
+        dwork = c.take<int>(1);
+        dindex = c.take<int32_t>(rows);
+        mseg = c.take<int32_t>((size_t)nq * topK);
+        mnodes = c.take<int32_t>((size_t)nq * topK);
+        mscores = c.take<float>((size_t)nq * topK);
+        return c.bytes;
+    };
+    if ((rc = t_ctx.init()) || (rc = grow(t_ctx.segments, carve(nullptr)))) return rc;
+    carve(t_ctx.segments.get());
+    cudaStream_t s = t_ctx.stream;
+    CK(t_ctx.timer.start(s), "event");
+    CK(cudaMemcpyAsync(dq, queries, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, s), "H2D queries");
+    if (bit_words) {
+        std::vector<uint32_t> hb(bit_words);
+        for (int i : walked)
+            if (segments[i].accept_bits) memcpy(hb.data() + bits_off[i], segments[i].accept_bits, (((size_t)segments[i].approx->d.n + 31) / 32) * 4);
+        CK(cudaMemcpyAsync(dbits, hb.data(), bit_words * 4, cudaMemcpyHostToDevice, s), "H2D accept bits");
+        CK(cudaStreamSynchronize(s), "H2D accept bits");  // hb is a pageable host vector
+    }
+    CK(cudaMemsetAsync(dcnt, 0, sizeof(SearchCounters) * S, s), "memset counters");
+    for (int i = 0; i < S; i++)
+        if (segments[i].graph && segments[i].graph->g.entry_node < 0) {
+            // every node removed: the segment answers nothing
+            CK(cudaMemsetAsync(dnodes + (size_t)i * nq * topK, 0xff, (size_t)nq * topK * 4, s), "memset nodes");
+            CK(cudaMemsetAsync(dscores + (size_t)i * nq * topK, 0, (size_t)nq * topK * 4, s), "memset scores");
+        }
+
+    // ---- the walks: one launch per group of segments prepared alike (with edge records, without), as search_device prepares one
+    std::vector<long long> retried(S, 0);
+    std::vector<SearchCounters> hc(S);
+    memset(hc.data(), 0, sizeof(SearchCounters) * S);
+    if (W) {
+        const bool sketch = search_uses_sketch(a0->d, metric, plan, W * nq);
+        std::vector<std::shared_ptr<DeviceBuffer>> edge_recs(W);  // held until the call returns: every path out of it synchronises `s`
+        std::vector<SegmentDesc> desc(W);
+        for (int l = 0; l < W; l++) {
+            const int i = walked[l];
+            const jv_dataset a = segments[i].approx;
+            if (sketch && (rc = ensure_sketch(a, s))) return rc;
+            SegmentDesc &d = desc[l];
+            memset(&d, 0, sizeof(d));
+            d.approx = a->d;
+            if (d.approx.kind == KIND_F32) {
+                std::lock_guard<std::mutex> lk(a->sketch_mu);
+                d.approx.sketch = a->sketch.get<int8_t>();
+                d.approx.sketch_meta = a->sketch_meta.get<float2>();
+                d.approx.sketch_stride = sketch_stride(d.approx.stride);
+                d.approx.lr_basis = a->lr_basis.get<float>();
+            }
+            d.g = segments[i].graph->g;
+            if (d.approx.sketch && d.approx.lr_basis && sketch && (rc = ensure_edge_records(segments[i].graph, a, s, &edge_recs[l]))) return rc;
+            d.g.edge_rec = edge_recs[l] ? edge_recs[l]->get<uint8_t>() : nullptr;
+            search_walk_descs(d.g, d.approx, metric, sketch);
+            d.rerank = r0 ? segments[i].reranker->d : d.approx;
+            d.accept_bits = segments[i].accept_bits ? dbits + bits_off[i] : nullptr;
+            d.slot = i;
+        }
+        // groups: the segments with edge records first, then the others (a stable partition keeps segment order inside each)
+        std::vector<int> order(W);
+        for (int l = 0; l < W; l++) order[l] = l;
+        std::stable_partition(order.begin(), order.end(), [&](int l) { return desc[l].g.edge_rec != nullptr; });
+        std::vector<SegmentDesc> sorted(W);
+        for (int l = 0; l < W; l++) sorted[l] = desc[order[l]];
+        CK(cudaMemcpyAsync(ddesc, sorted.data(), sizeof(SegmentDesc) * W, cudaMemcpyHostToDevice, s), "H2D segment descriptors");
+        const int nedge = (int)std::count_if(sorted.begin(), sorted.end(), [](const SegmentDesc &d) { return d.g.edge_rec != nullptr; });
+        struct Group { int first, count; std::vector<int32_t> idx; };
+        std::vector<Group> groups;
+        if (nedge) groups.push_back({0, nedge, {}});
+        if (W > nedge) groups.push_back({nedge, W - nedge, {}});
+        SearchFilter f;
+        memset(&f, 0, sizeof(f));
+        f.threshold = threshold;
+        f.rerank_floor = rerank_floor;
+        f.accept_bits = bit_words ? dbits : nullptr;  // marks the walk filtered: each segment reads its own bitset from its descriptor
+        int cap = plan.visited_cap, lcap = plan.list_cap;
+        for (int attempt = 0;; attempt++) {
+            for (const Group &gr : groups) {
+                const int cnt = attempt ? (int)gr.idx.size() : gr.count * nq;
+                if (cnt == 0) continue;
+                SearchPlan pl = plan;
+                if (attempt) CK(plan_search(a0->d, rr0, gmax, topK, rerankK, cnt, cap, lcap, g_sm_count, &pl), "plan_search(retry)");
+                else pl.ctas = (int)std::min<long long>((long long)plan.ctas, cnt);
+                if ((rc = grow(t_ctx.search_scratch, search_scratch_bytes(pl)))) return rc;
+                int32_t *gidx = dindex + (size_t)gr.first * nq;
+                if (attempt) CK(cudaMemcpyAsync(gidx, gr.idx.data(), gr.idx.size() * 4, cudaMemcpyHostToDevice, s), "H2D retry index");
+                GraphDesc gg = sorted[gr.first].g;  // the group's walk: its kind of walk, sized for the largest degree
+                gg.n = gmax.n;
+                gg.degree = gmax.degree;
+                const SegmentGroup sgp{ddesc + gr.first, gr.count, nq};
+                CK(launch_search(gg, sorted[gr.first].approx, r0 ? &sorted[gr.first].rerank : nullptr, metric, dq, cnt, topK, rerankK, pl,
+                                 t_ctx.search_scratch.get(), dwork, dnodes, dscores, dcnt, dover, attempt ? gidx : nullptr, 0, &f, s, &sgp),
+                   "launch_search(segments)");
+                if (attempt) CK(cudaStreamSynchronize(s), "segments search");  // gr.idx is read by the copy above
+            }
+            CK(cudaMemcpyAsync(hc.data(), dcnt, sizeof(SearchCounters) * S, cudaMemcpyDeviceToHost, s), "D2H counters");
+            CK(cudaStreamSynchronize(s), "segments search");
+            bool over = false;
+            for (int i : walked) over = over || hc[i].overflowed > 0;
+            if (!over || attempt == 6) break;
+            // pairs whose visited table filled up (code 1) or whose list could not hold a tie tail (code 2) are re-run with 4x, as
+            // search_device re-runs queries
+            std::vector<uint8_t> hover(rows);
+            CK(cudaMemcpy(hover.data(), dover, rows, cudaMemcpyDeviceToHost), "D2H overflow flags");
+            bool need_table = false, need_list = false;
+            for (Group &gr : groups) {
+                gr.idx.clear();
+                for (int l = 0; l < gr.count; l++) {
+                    const int slot = sorted[gr.first + l].slot;
+                    if (!hc[slot].overflowed) continue;
+                    for (int q = 0; q < nq; q++) {
+                        const uint8_t o = hover[(size_t)slot * nq + q];
+                        if (!o) continue;
+                        gr.idx.push_back(l * nq + q);
+                        retried[slot]++;
+                        if (o == 1) need_table = true;
+                        else need_list = true;
+                    }
+                    CK(cudaMemsetAsync(&dcnt[slot].overflowed, 0, sizeof(unsigned long long), s), "reset overflow");
+                }
+            }
+            if (need_table) cap *= 4;
+            if (need_list) {
+                if (lcap >= MAX_LIST_CAP)
+                    for (int i : walked)
+                        if (hc[i].overflowed)
+                            return fail(JV_ERR_OVERFLOW, "segments_search: segment " + std::to_string(i) +
+                                                             ": more equal-score (or filtered-out) candidates than the longest candidate list holds");
+                lcap = std::min(MAX_LIST_CAP, lcap * 4);
+            }
+        }
+        for (int i : walked)
+            if (hc[i].overflowed > 0) return fail(JV_ERR_OVERFLOW, "segments_search: segment " + std::to_string(i) + ": visited table / candidate list overflow after retries");
+    }
+
+    // ---- segments without a graph: jv_exhaustive_search_batch's device work into their rows of the same answers
+    std::vector<int64_t> ex_visited(S, 0);
+    std::vector<unsigned long long> ex_taken(S, 0);
+    for (int i = 0; i < S; i++) {
+        if (segments[i].graph) continue;
+        const jv_search_options o = {segments[i].accept_bits, 0, threshold, rerank_floor};
+        if ((rc = exhaustive_device(segments[i].approx, segments[i].reranker, metric, nullptr, dq, nq, topK, rerankK, &o, nullptr, nullptr,
+                                    dnodes + (size_t)i * nq * topK, dscores + (size_t)i * nq * topK, &ex_visited[i], &ex_taken[i])))
+            return rc;
+    }
+
+    // ---- the merge, and the answers back
+    CK(launch_segment_merge(dnodes, dscores, nq, S, topK, mseg, mnodes, mscores, s), "segment_merge");
+    CK(cudaMemcpyAsync(segments_out, mseg, (size_t)nq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H segments");
+    CK(cudaMemcpyAsync(nodes_out, mnodes, (size_t)nq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H nodes");
+    CK(cudaMemcpyAsync(scores_out, mscores, (size_t)nq * topK * 4, cudaMemcpyDeviceToHost, s), "D2H scores");
+    CK(t_ctx.timer.stop(s), "event");
+    CK(cudaStreamSynchronize(s), "sync");
+    const double ms = t_ctx.timer.ms();
+    t_last_settled = t_last_direct[0] = t_last_direct[1] = 0;
+    for (int i : walked) {
+        t_last_settled += (int64_t)hc[i].settled;
+        t_last_direct[0] += (int64_t)hc[i].direct;
+        t_last_direct[1] += (int64_t)hc[i].direct_dropped;
+    }
+    jv_search_stats total;
+    memset(&total, 0, sizeof(total));
+    for (int i = 0; i < S; i++) {
+        jv_search_stats st;
+        memset(&st, 0, sizeof(st));
+        if (segments[i].graph) {
+            st.visited = (int64_t)hc[i].visited;
+            st.expanded = (int64_t)hc[i].expanded;
+            st.expanded_base = (int64_t)hc[i].expanded_base;
+            st.reranked = (int64_t)hc[i].reranked;
+        } else {
+            st.visited = ex_visited[i];
+            st.reranked = (int64_t)ex_taken[i];
+        }
+        st.retried = retried[i];
+        st.device_ms = ms;
+        total.visited += st.visited;
+        total.expanded += st.expanded;
+        total.expanded_base += st.expanded_base;
+        total.reranked += st.reranked;
+        total.retried += st.retried;
+        if (segment_stats) segment_stats[i] = st;
+    }
+    total.device_ms = ms;
+    if (stats) *stats = total;
+    return JV_OK;
 }
 
 int jv_graph_search_exclude(jv_graph g, jv_dataset approx, int metric, const float *queries, int nq, int topK, int rerankK,

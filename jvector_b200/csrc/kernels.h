@@ -108,6 +108,12 @@ cudaError_t launch_key_rebase(long long *keys_dev, long long count, long long id
 cudaError_t launch_topk_merge(const long long *keys_in_dev, int nq, int parts, int k, long long *keys_out_dev, cudaStream_t s);
 // the same for keys laid out [parts][nq][k] (shard-major, what peer copies / all_gather produce)
 cudaError_t launch_topk_merge_strided(const long long *keys_in_dev, int nq, int parts, int k, long long *keys_out_dev, cudaStream_t s);
+// the stable merge of per-segment answers nodes / scores [parts][nq][k] (node -1 = padding) into the k best per query: score
+// descending, equal scores in segment order, then in list order; out: segment, node, score [nq][k], padded with -1, -1, 0.
+// k <= SEGMENT_MERGE_MAX_K, parts * k <= SEGMENT_MERGE_MAX_KEYS (the keys are sorted in shared memory)
+constexpr int SEGMENT_MERGE_MAX_K = 4096, SEGMENT_MERGE_MAX_KEYS = 16384;
+cudaError_t launch_segment_merge(const int32_t *nodes_in_dev, const float *scores_in_dev, int nq, int parts, int k, int32_t *seg_out_dev, int32_t *nodes_out_dev,
+                                 float *scores_out_dev, cudaStream_t s);
 
 // int8 row sketch + {scale, radius} per row of an fp32 data set (the search kernel's sketch bound, see sketch_bound_pair)
 cudaError_t launch_row_sketch(const float *rows_dev, long long n, int stride, int sketch_stride, int8_t *sketch_dev, float2 *meta_dev, cudaStream_t s);
@@ -177,6 +183,23 @@ struct SearchFilter {
     // ExcludingBits); -1 excludes nothing
     const int32_t *exclude_ids;
 };
+// One walked segment of a multi-segment search (api.cu jv_segments_search_batch, the walk's SEG instantiations): its graph and data
+// sets as search_walk_descs leaves them, its acceptOrds bitset (device, shared by the batch; nullptr = every node) and its slot: it
+// adds to counters[slot] and writes output rows [slot * nq, (slot + 1) * nq)
+struct SegmentDesc {
+    GraphDesc g;
+    DataDesc approx, rerank;
+    const uint32_t *accept_bits;
+    int slot;
+};
+// segments walked in one launch: descs_dev [nseg], all with edge records or all without; nq queries each
+struct SegmentGroup {
+    const SegmentDesc *descs_dev;
+    int nseg, nq;
+};
+// the graph and data set a walk reads: FusedPQ records only over the codes they were packed from, the row sketch only when `sketch`,
+// the edge records only next to the sketch and the low-rank basis of an fp32 DOT walk
+void search_walk_descs(GraphDesc &g, DataDesc &approx, int metric, bool sketch);
 cudaError_t plan_search(const DataDesc &approx, const DataDesc *rerank, const GraphDesc &g, int topK, int rerankK, int nq,
                         int visited_cap_hint, int list_cap_hint, int sm_count, SearchPlan *plan);
 size_t search_scratch_bytes(const SearchPlan &p);
@@ -186,7 +209,8 @@ int sketch_stride(int stride);  // int8 sketch bytes per row of an fp32 data set
 cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const DataDesc *rerank, int metric, const float *queries_dev,
                           int nq, int topK, int rerankK, const SearchPlan &plan, void *scratch_dev, int *work_counter_dev,
                           int32_t *nodes_out_dev, float *scores_out_dev, SearchCounters *counters_dev, uint8_t *overflow_flags_dev,
-                          const int32_t *query_index_dev, int query_stride, const SearchFilter *filter, cudaStream_t s);
+                          const int32_t *query_index_dev, int query_stride, const SearchFilter *filter, cudaStream_t s,
+                          const SegmentGroup *segments = nullptr);
 
 // ---- build.cu ----
 struct BuildParams {

@@ -925,18 +925,73 @@ __global__ void __launch_bounds__(256) topk_merge_kernel(const long long *__rest
     for (int i = threadIdx.x; i < k; i += blockDim.x) out[(size_t)q * k + i] = i < total ? skeys[i] : KEY_MIN;
 }
 
+// the sort step of the strided merges: skeys[i] = load(p, j) for entry j of part p (i = p * k + j < parts * k), KEY_MIN past
+// them, sorted descending
+template <typename Load>
+__device__ __forceinline__ void strided_load_sort(long long *skeys, int parts, int k, int total_pow2, Load load)
+{
+    const int total = parts * k;
+    for (int i = threadIdx.x; i < total_pow2; i += blockDim.x) {
+        const int p = i / k, j = i - p * k;
+        skeys[i] = i < total ? load(p, j) : KEY_MIN;
+    }
+    __syncthreads();
+    bitonic_sort_desc(skeys, total_pow2);
+}
+
 // same merge over the layout the peer copies produce: in [parts][nq][k]
 __global__ void __launch_bounds__(256) topk_merge_strided_kernel(const long long *__restrict__ in, int nq, int parts, int k, int total_pow2, long long *__restrict__ out)
 {
     extern __shared__ long long skeys[];
     const int q = blockIdx.x, total = parts * k;
-    for (int i = threadIdx.x; i < total_pow2; i += blockDim.x) {
-        const int p = i / k, j = i - p * k;
-        skeys[i] = i < total ? in[((size_t)p * nq + q) * k + j] : KEY_MIN;
-    }
-    __syncthreads();
-    bitonic_sort_desc(skeys, total_pow2);
+    strided_load_sort(skeys, parts, k, total_pow2, [&](int p, int j) { return in[((size_t)p * nq + q) * k + j]; });
     for (int i = threadIdx.x; i < k; i += blockDim.x) out[(size_t)q * k + i] = i < total ? skeys[i] : KEY_MIN;
+}
+
+// the stable merge of jv_segments_search_batch over the segments' answers nodes_in / scores_in [parts][nq][k] (node -1 = padding):
+// entry j of segment p is keyed (float_to_sortable(score) << 32) | ~((p << 12) | j), so that the key order (the greater key first)
+// is the score descending, then the lower segment, then the earlier entry of that segment's list; padding is KEY_MIN. The first k
+// keys are unpacked into (segment, node, score) read back from the inputs, padded with -1, -1, 0.
+__global__ void __launch_bounds__(256) segment_merge_kernel(const int32_t *__restrict__ nodes_in, const float *__restrict__ scores_in, int nq, int parts, int k,
+                                                            int total_pow2, int32_t *__restrict__ seg_out, int32_t *__restrict__ nodes_out,
+                                                            float *__restrict__ scores_out)
+{
+    extern __shared__ long long skeys[];
+    const int q = blockIdx.x;
+    strided_load_sort(skeys, parts, k, total_pow2, [&](int p, int j) {
+        const size_t at = ((size_t)p * nq + q) * k + j;
+        if (nodes_in[at] < 0) return KEY_MIN;
+        return (long long)(((unsigned long long)(uint32_t)float_to_sortable(scores_in[at]) << 32) | (unsigned long long)(uint32_t)~(uint32_t)((p << 12) | j));
+    });
+    for (int i = threadIdx.x; i < k; i += blockDim.x) {
+        const long long key = skeys[i];
+        const size_t o = (size_t)q * k + i;
+        if (key == KEY_MIN) {
+            seg_out[o] = -1;
+            nodes_out[o] = -1;
+            scores_out[o] = 0.f;
+        } else {
+            const uint32_t tag = ~(uint32_t)((unsigned long long)key & 0xffffffffull);
+            const int p = (int)(tag >> 12), j = (int)(tag & 4095u);
+            const size_t at = ((size_t)p * nq + q) * k + j;
+            seg_out[o] = p;
+            nodes_out[o] = nodes_in[at];
+            scores_out[o] = scores_in[at];
+        }
+    }
+}
+
+cudaError_t launch_segment_merge(const int32_t *nodes_in_dev, const float *scores_in_dev, int nq, int parts, int k, int32_t *seg_out_dev, int32_t *nodes_out_dev,
+                                 float *scores_out_dev, cudaStream_t s)
+{
+    if (k > SEGMENT_MERGE_MAX_K || (long long)parts * k > SEGMENT_MERGE_MAX_KEYS) return cudaErrorInvalidValue;
+    const int p2 = next_pow2(parts * k);
+    cudaError_t e;
+    if ((size_t)p2 * 8 > 48 * 1024)
+        if ((e = cudaFuncSetAttribute(segment_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p2 * 8)) != cudaSuccess) return e;
+    segment_merge_kernel<<<nq, 256, (size_t)p2 * 8, s>>>(nodes_in_dev, scores_in_dev, nq, parts, k, p2, seg_out_dev, nodes_out_dev, scores_out_dev);
+    g_launches++;
+    return cudaGetLastError();
 }
 
 cudaError_t launch_topk_merge_strided(const long long *keys_in_dev, int nq, int parts, int k, long long *keys_out_dev, cudaStream_t s)

@@ -68,6 +68,9 @@ struct SearchParams {
                        // (fp32: only for a batch that does not fill the GPU)
     unsigned long long *dbg;  // JV_SEARCH_PROFILE builds only: per-phase cycle totals
     const int32_t *exclude_ids;  // [nq]: query qi never accepts node exclude_ids[qi] (SearchFilter::exclude_ids, the EXCL instantiations)
+    // SEG instantiations: the walked segments' descriptors; nq counts (segment, query) items, seg_nq the queries per segment
+    const SegmentDesc *segs;
+    int seg_nq;
 };
 
 __device__ __forceinline__ bool visited_insert(int32_t *t, unsigned mask, int shift, int32_t v)
@@ -247,7 +250,10 @@ constexpr uint8_t F_ACCEPTED = 2;  // acceptOrds.get(node) && score >= threshold
 // EDGE: the fp32 DOT walk over a graph with edge records (P.g.edge_rec, launch_search), a separate instantiation for the same reason
 // EXCL: the walks of a refine, which never accept their query's own node (P.exclude_ids); separate so that the other walks compile
 // exactly as they do without it
-template <int KIND, int METRIC, int MINB, bool VSM, bool EDGE = false, bool EXCL = false>
+// SEG: the walks of a multi-segment search (jv_segments_search_batch): work item w (or P.query_index[w]) is the pair
+// (segment s, query q) = (w / P.seg_nq, w % P.seg_nq), and each item reads its segment's graph, data sets, bitset, counters and
+// output rows from P.segs[s] instead of P; separate for the same reason as EXCL
+template <int KIND, int METRIC, int MINB, bool VSM, bool EDGE = false, bool EXCL = false, bool SEG = false>
 __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search_kernel(SearchParams P)
 {
     constexpr int SEARCH_THREADS = SearchThreads<KIND>::value;
@@ -285,6 +291,13 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
     __shared__ float s_lr[LR_QUERY];  // the query's low-rank terms (prepare_lowrank)
     __shared__ int s_drop[2];  // best sortable score that fell off the list, double-buffered like s_posv
     __shared__ int s_posv[2];
+    // the descriptor of the work item's segment (SEG); every other walk reads P's own through the same names (macros, not
+    // references: a reference to P compiles the other walks differently)
+    __shared__ __align__(16) SegmentDesc s_seg;
+#define PG (SEG ? s_seg.g : P.g)
+#define PA (SEG ? s_seg.approx : P.approx)
+#define PR (SEG ? s_seg.rerank : P.rerank)
+#define PC (SEG ? P.counters + s_seg.slot : P.counters)
 
     const int tid = threadIdx.x;
     const int group = tid / G, lane = tid % G;
@@ -292,7 +305,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
     const unsigned vmask = (unsigned)P.visited_cap - 1u;
     const int vis_limit = 3 << (P.vis_slots_log > 2 ? P.vis_slots_log - 2 : 0);  // shared-memory table: at most 3/4 full
     int32_t *table = P.visited_tables + (size_t)blockIdx.x * P.visited_cap;
-    const int degree = P.g.degree;
+    int degree = P.g.degree;
     if (EDGE && tid == 0) { s_settled_total = 0; s_direct_total[0] = 0; s_direct_total[1] = 0; }
 
     for (;;) {
@@ -313,23 +326,34 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         __syncthreads();
         const int wq = s_q;
         if (wq >= P.nq) {
-            if (EDGE && tid == 0) {
+            if (EDGE && !SEG && tid == 0) {
                 if (s_settled_total) atomicAdd(&P.counters->settled, s_settled_total);
                 if (s_direct_total[0]) atomicAdd(&P.counters->direct, s_direct_total[0]);
                 if (s_direct_total[1]) atomicAdd(&P.counters->direct_dropped, s_direct_total[1]);
             }
             break;
         }
-        const int qi = P.query_index ? P.query_index[wq] : wq;
+        int qi = P.query_index ? P.query_index[wq] : wq;
         const float *q = P.queries + (size_t)qi * P.query_stride;
         const uint32_t *acc = P.accept_bits ? P.accept_bits + (size_t)qi * P.accept_stride : nullptr;
+        if constexpr (SEG) {
+            // item = (segment sg, query qq): load the segment's descriptor; qi becomes the query's output row (and overflow code)
+            const int sg = qi / P.seg_nq, qq = qi - sg * P.seg_nq;
+            const int *src = reinterpret_cast<const int *>(P.segs + sg);
+            for (int i = tid; i < (int)(sizeof(SegmentDesc) / 4); i += SEARCH_THREADS) reinterpret_cast<int *>(&s_seg)[i] = __ldg(src + i);
+            __syncthreads();
+            degree = s_seg.g.degree;
+            q = P.queries + (size_t)qq * P.query_stride;
+            acc = s_seg.accept_bits;
+            qi = s_seg.slot * P.seg_nq + qq;
+        }
 #ifdef JV_SEARCH_PROFILE
         unsigned long long dbg_local[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 #endif
         JV_T(t_q0);
-        prepare_blob<SEARCH_THREADS>(P.approx, P.metric, q, blobA, red, blobH, splitm);
-        if (P.has_rerank) prepare_blob<SEARCH_THREADS>(P.rerank, P.metric, q, blobR, red);
-        if (EDGE) prepare_lowrank<SEARCH_THREADS>(P.approx.lr_basis, P.approx.stride, blobA, s_lr);
+        prepare_blob<SEARCH_THREADS>(PA, P.metric, q, blobA, red, blobH, splitm);
+        if (P.has_rerank) prepare_blob<SEARCH_THREADS>(PR, P.metric, q, blobR, red);
+        if (EDGE) prepare_lowrank<SEARCH_THREADS>(PA.lr_basis, PA.stride, blobA, s_lr);
         if (vsm) {
             int4 *t4 = reinterpret_cast<int4 *>(vis);
             const int4 z = make_int4(0, 0, 0, 0);
@@ -348,9 +372,9 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         uint8_t *fcur = flags0, *fnxt = flags1;
         // initializeInternal: score the entry node, mark it visited (GraphSearcher.java:346-348)
         if (group == 0) {
-            const float sc = KIND == KIND_PQ ? score_pq<METRIC>(P.approx, blobA, P.g.entry_node, lane, blobH, splitm) : score_row<KIND, METRIC>(P.approx, blobA, P.g.entry_node, lane);
+            const float sc = KIND == KIND_PQ ? score_pq<METRIC>(PA, blobA, PG.entry_node, lane, blobH, splitm) : score_row<KIND, METRIC>(PA, blobA, PG.entry_node, lane);
             if (lane == 0) {
-                const int32_t en = P.g.entry_node;
+                const int32_t en = PG.entry_node;
                 cur[0] = topk_key(sc, en);
                 fcur[0] = ((!acc || ((acc[en >> 5] >> (en & 31)) & 1u)) && sc >= P.threshold && !(EXCL && P.exclude_ids[qi] == en)) ? F_ACCEPTED : 0;
                 if (vsm) visited_insert_smem(vis, P.vis_idmask, P.vis_rlog, en, &s_vfail);
@@ -364,7 +388,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         bool truncated = false, inexact = false;  // lenient mode: the walk was cut short / a tie tail was dropped
         __syncthreads();
 
-        for (int lvl = P.g.entry_level; lvl >= 0 && !failed && !truncated; --lvl) {
+        for (int lvl = PG.entry_level; lvl >= 0 && !failed && !truncated; --lvl) {
             const int K = lvl > 0 ? 1 : L;
             // a new level: results + evicted are candidates again (setEntryPointsFromPreviousLayer), the result heap is empty
             for (int i = tid; i < size; i += SEARCH_THREADS) fcur[i] &= F_ACCEPTED;
@@ -393,22 +417,22 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 expanded++;
                 if (lvl == 0) expanded_base++;
                 const int32_t *nb;
-                if (lvl == 0) nb = P.g.adj0 + (size_t)node * degree;
+                if (lvl == 0) nb = PG.adj0 + (size_t)node * degree;
                 else {
-                    const int32_t row = P.g.upper_row[(size_t)(lvl - 1) * P.g.n + node];
-                    nb = row >= 0 ? P.g.upper_adj + ((size_t)P.g.upper_off[lvl - 1] + row) * degree : nullptr;
+                    const int32_t row = PG.upper_row[(size_t)(lvl - 1) * PG.n + node];
+                    nb = row >= 0 ? PG.upper_adj + ((size_t)PG.upper_off[lvl - 1] + row) * degree : nullptr;
                 }
                 // FusedPQ (OnDiskGraphIndex.java:639-651, "useEdgeLoading && level == 0"): ids and the neighbours' codes come from the
                 // expanded node's own record
-                const bool fused = KIND == KIND_PQ && lvl == 0 && P.g.fused != nullptr;
-                const uint8_t *rec = fused ? P.g.fused + (size_t)node * P.g.fused_rec : nullptr;
+                const bool fused = KIND == KIND_PQ && lvl == 0 && PG.fused != nullptr;
+                const uint8_t *rec = fused ? PG.fused + (size_t)node * PG.fused_rec : nullptr;
                 if (fused) {
                     nb = reinterpret_cast<const int32_t *>(rec);
                     if (P.pq_rows) {
                         // the record's code rows do not depend on which neighbours turn out to be new: the warps that have no
                         // neighbour to test copy ALL of them (degree x code_stride contiguous bytes) into shared memory while
                         // warp 0 runs visited.add(); the scoring phase then finds candidate i's codes at slot cand_slot[i]
-                        const int cw = P.approx.code_stride >> 2, cws = cw + 1;
+                        const int cw = PA.code_stride >> 2, cws = cw + 1;
                         const uint32_t *src = reinterpret_cast<const uint32_t *>(rec + 4 * degree);
                         for (int t = tid - 64; t >= 0 && t < degree * cw; t += SEARCH_THREADS - 64) {
                             const int i = t / cw;
@@ -417,7 +441,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     } else if (tid >= 64) {
                         // the code rows of this record are needed one barrier from now: pull the whole record towards L2 at once
                         const int o = (tid - 64) * 128;
-                        if (o < P.g.fused_rec) prefetch_l2(rec + o);
+                        if (o < PG.fused_rec) prefetch_l2(rec + o);
                     }
                 }
                 // sketched DOT walk over a graph with edge records (the condition of `sketched` below): a new neighbour whose low-rank
@@ -432,9 +456,9 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                         if (f >= 0 && (vsm ? visited_insert_smem(vis, P.vis_idmask, P.vis_rlog, f, &s_vfail) : visited_insert(table, vmask, P.visited_shift, f))) {
                             if (edge_tier) {
                                 // (the record was requested towards L2 with the adjacency row, by the speculation below one or more hops ago)
-                                const uint4 *e = reinterpret_cast<const uint4 *>(P.g.edge_rec + ((size_t)node * degree + t) * LR_SLOT);
+                                const uint4 *e = reinterpret_cast<const uint4 *>(PG.edge_rec + ((size_t)node * degree + t) * LR_SLOT);
                                 float est;
-                                const float ub = lowrank_bound(P.approx, blobA, s_lr, __ldg(e), __ldg(e + 1), __ldg(reinterpret_cast<const float4 *>(e + 2)), est);
+                                const float ub = lowrank_bound(PA, blobA, s_lr, __ldg(e), __ldg(e + 1), __ldg(reinterpret_cast<const float4 *>(e + 2)), est);
                                 const long long last = cur[LC - 1];
                                 if (topk_key(ub, f) < last) {
                                     atomicAdd(&s_settled, 1);
@@ -445,7 +469,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                                     // a likely list entrant, whose sketch bound would not settle it: routed direct to its full row
                                     const int j = atomicAdd(&s_nd, 1);
                                     cand_ids[MAX_DEGREE - 1 - j] = f;
-                                    bulk_prefetch_l2(P.approx.rows + (size_t)f * P.approx.stride, (unsigned)P.approx.stride * 4u);
+                                    bulk_prefetch_l2(PA.rows + (size_t)f * PA.stride, (unsigned)PA.stride * 4u);
                                     continue;
                                 }
                             }
@@ -454,19 +478,19 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                             if (KIND == KIND_PQ) cand_slot[slot] = (uint8_t)t;
                             // the row is needed one barrier from now: start the DRAM -> L2 transfer of all of it at once (one
                             // UBLKPF per row; bytes in flight that occupy no registers and no shared memory)
-                            if (KIND == KIND_F32 && P.row_prefetch == 1) bulk_prefetch_l2(P.approx.rows + (size_t)f * P.approx.stride, (unsigned)P.approx.stride * 4u);
+                            if (KIND == KIND_F32 && P.row_prefetch == 1) bulk_prefetch_l2(PA.rows + (size_t)f * PA.stride, (unsigned)PA.stride * 4u);
                             // a sketched walk (the condition of `sketched` below) reads this row's sketch and {s, r} first, one barrier
                             // from now: request them (768 + 8 B at d = 768) so that the bound waits on L2, not DRAM. The full rows are
                             // not prefetched: only the ~17 % the bound does not settle read them, and they would not fit in L2.
-                            if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && P.approx.sketch != nullptr) {
-                                const char *sk = reinterpret_cast<const char *>(P.approx.sketch) + (size_t)f * P.approx.sketch_stride;
-                                for (int o = 0; o < P.approx.sketch_stride; o += 128) prefetch_l2(sk + o);
-                                prefetch_l2(sk + P.approx.sketch_stride - 1);
-                                prefetch_l2(P.approx.sketch_meta + f);
+                            if (KIND == KIND_F32 && METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && PA.sketch != nullptr) {
+                                const char *sk = reinterpret_cast<const char *>(PA.sketch) + (size_t)f * PA.sketch_stride;
+                                for (int o = 0; o < PA.sketch_stride; o += 128) prefetch_l2(sk + o);
+                                prefetch_l2(sk + PA.sketch_stride - 1);
+                                prefetch_l2(PA.sketch_meta + f);
                             }
                             if (KIND == KIND_NVQ && P.row_prefetch == 1) {
-                                bulk_prefetch_l2(P.approx.bytes + (size_t)f * P.approx.byte_stride, (unsigned)P.approx.byte_stride);
-                                prefetch_l2(P.approx.params + (size_t)f * 4 * P.approx.nsub);  // {min, max, growthRate, midpoint} per sub-vector
+                                bulk_prefetch_l2(PA.bytes + (size_t)f * PA.byte_stride, (unsigned)PA.byte_stride);
+                                prefetch_l2(PA.params + (size_t)f * 4 * PA.nsub);  // {min, max, growthRate, midpoint} per sub-vector
                             }
                         }
                     }
@@ -480,9 +504,9 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     if (tid >= 32 && tid < 36) {
                         const int pp = p + (tid - 31);
                         if (pp < size && !(fcur[pp] & F_EXPANDED)) {
-                            prefetch_l2(P.g.adj0 + (size_t)key_node(cur[pp]) * degree);
+                            prefetch_l2(PG.adj0 + (size_t)key_node(cur[pp]) * degree);
                             // and their edge records (degree x 48 B), so that a hop's record reads wait on L2 like its adjacency row
-                            if (edge_tier) bulk_prefetch_l2(P.g.edge_rec + (size_t)key_node(cur[pp]) * degree * LR_SLOT, (unsigned)(degree * LR_SLOT));
+                            if (edge_tier) bulk_prefetch_l2(PG.edge_rec + (size_t)key_node(cur[pp]) * degree * LR_SLOT, (unsigned)(degree * LR_SLOT));
                         }
                     }
                 }
@@ -502,22 +526,22 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     const int w = tid >> 5;
                     if (w >= 1 && w <= 3) {
                         const int pp = p + w;
-                        if (pp < size && !(fcur[pp] & F_EXPANDED) && KIND == KIND_PQ && P.g.fused) {
+                        if (pp < size && !(fcur[pp] & F_EXPANDED) && KIND == KIND_PQ && PG.fused) {
                             // one record = ids + codes: pull its lines towards L2 (25 x 128 B at degree 32, M = 96)
-                            const char *r2 = reinterpret_cast<const char *>(P.g.fused + (size_t)key_node(cur[pp]) * P.g.fused_rec);
-                            for (int o = (tid & 31) * 128; o < P.g.fused_rec; o += 32 * 128) prefetch_l2(r2 + o);
+                            const char *r2 = reinterpret_cast<const char *>(PG.fused + (size_t)key_node(cur[pp]) * PG.fused_rec);
+                            for (int o = (tid & 31) * 128; o < PG.fused_rec; o += 32 * 128) prefetch_l2(r2 + o);
                         } else if (pp < size && !(fcur[pp] & F_EXPANDED)) {
-                            const int32_t *nb2 = P.g.adj0 + (size_t)key_node(cur[pp]) * degree;
+                            const int32_t *nb2 = PG.adj0 + (size_t)key_node(cur[pp]) * degree;
                             for (int t = tid & 31; t < degree; t += 32) {
                                 const int32_t f = __ldg(nb2 + t);
                                 if (KIND == KIND_PQ && f >= 0) {
-                                    const char *a = reinterpret_cast<const char *>(P.approx.codes + (size_t)f * P.approx.code_stride);
+                                    const char *a = reinterpret_cast<const char *>(PA.codes + (size_t)f * PA.code_stride);
                                     prefetch_l2(a);
-                                    prefetch_l2(a + P.approx.M - 1);
+                                    prefetch_l2(a + PA.M - 1);
                                 } else if (KIND == KIND_BQ && f >= 0) {
-                                    const char *a = reinterpret_cast<const char *>(P.approx.words + (size_t)f * P.approx.W);
-                                    for (int o = 0; o < P.approx.W * 8; o += 128) prefetch_l2(a + o);
-                                    prefetch_l2(a + P.approx.W * 8 - 1);
+                                    const char *a = reinterpret_cast<const char *>(PA.words + (size_t)f * PA.W);
+                                    for (int o = 0; o < PA.W * 8; o += 128) prefetch_l2(a + o);
+                                    prefetch_l2(a + PA.W * 8 - 1);
                                 }
                             }
                         }
@@ -561,8 +585,8 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         const long long key_ = topk_key((sc_), (f_));                                                                               \
         JV_RBS_ROW(key_, f_);                                                                                                       \
         if (lvl == 0 && P.early_pf && key_ > s_nk) {                                                                                \
-            if (KIND == KIND_PQ && P.g.fused) bulk_prefetch_l2(P.g.fused + (size_t)(f_) * P.g.fused_rec, (unsigned)P.g.fused_rec);  \
-            else prefetch_l2(P.g.adj0 + (size_t)(f_) * degree);                                                                     \
+            if (KIND == KIND_PQ && PG.fused) bulk_prefetch_l2(PG.fused + (size_t)(f_) * PG.fused_rec, (unsigned)PG.fused_rec);  \
+            else prefetch_l2(PG.adj0 + (size_t)(f_) * degree);                                                                     \
         }                                                                                                                           \
         if (dead < 0 && size == LC && key_ < cur[LC - 1]) {                                                                         \
             JV_RBS_DROP(f_);                                                                                                        \
@@ -579,7 +603,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     // (half the bytes) already falls under the list's last key would be dropped by JV_EMIT whatever its exact score,
                     // so it is dropped on the bound, which also stands in for its score in s_drop (>= the exact one: the check after
                     // the merge stays conservative). Only the others read their full rows, scored exactly as below.
-                    const bool sketched = METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && P.approx.sketch != nullptr;
+                    const bool sketched = METRIC == JV_METRIC_DOT && lvl == 0 && size == LC && PA.sketch != nullptr;
                     // two rows per warp at a time: twice the loads in flight, query fragment read once. EDGE: one flat pair index
                     // over both classes, so that the warps share them evenly: pairs [0, ps) read sketches first (rows i and i + ps of
                     // cand_ids), pairs [ps, ps + pd) are the rows routed direct (from the top of cand_ids), scored exactly at once
@@ -605,7 +629,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                         bool xa = true, xb = two;  // exact score needed
                         if (sketched && !direct) {
                             float ua, ub;
-                            sketch_bound_pair(P.approx, blobA, fa, fb, lane, ua, ub);
+                            sketch_bound_pair(PA, blobA, fa, fb, lane, ua, ub);
                             const long long last = cur[LC - 1];
                             xa = !(topk_key(ua, fa) < last);
                             xb = two && !(topk_key(ub, fb) < last);
@@ -616,13 +640,13 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                             if (!xa && !xb) continue;
                             if (!xa || !xb) {
                                 const int32_t f = xa ? fa : fb;
-                                const float sc = score_f32<METRIC>(P.approx, blobA, f, lane);
+                                const float sc = score_f32<METRIC>(PA, blobA, f, lane);
                                 if (lane == 0) JV_EMIT(sc, f);
                                 continue;
                             }
                         }
                         float sa, sb;
-                        score_f32_pair<METRIC>(P.approx, blobA, fa, fb, lane, sa, sb);
+                        score_f32_pair<METRIC>(PA, blobA, fa, fb, lane, sa, sb);
                         if (lane == 0) {
                             JV_RBS_SCORED(two ? 2 : 1);
                             if (direct) {
@@ -638,11 +662,11 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 } else if (KIND == KIND_PQ && P.pq_rows) {
                     // lane = candidate, warp = one of the 8 partial sums of the ADC score (score_pq_partial): the code rows of the
                     // hop are staged in shared memory by one coalesced pass, then every gather instruction of a warp reads ONE LUT row
-                    const int cw = P.approx.code_stride >> 2, cws = cw + 1;  // odd word stride: no bank conflicts across candidates
+                    const int cw = PA.code_stride >> 2, cws = cw + 1;  // odd word stride: no bank conflicts across candidates
                     if (!fused) {
                         for (int t = tid; t < n * cw; t += SEARCH_THREADS) {
                             const int i = t / cw, wd = t - i * cw;
-                            pq_stage[i * cws + wd] = __ldg(reinterpret_cast<const uint32_t *>(P.approx.codes + (size_t)cand_ids[i] * P.approx.code_stride) + wd);
+                            pq_stage[i * cws + wd] = __ldg(reinterpret_cast<const uint32_t *>(PA.codes + (size_t)cand_ids[i] * PA.code_stride) + wd);
                         }
                         __syncthreads();
                     }
@@ -650,7 +674,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     for (int g = tid >> 5; g < 8; g += SEARCH_THREADS / 32)
                         for (int i = tid & 31; i < n; i += 32) {
                             float ps, pa;
-                            score_pq_partial<METRIC>(P.approx, blobA, blobH, splitm, reinterpret_cast<const uint8_t *>(pq_stage + (fused ? (int)cand_slot[i] : i) * cws), g, ps, pa);
+                            score_pq_partial<METRIC>(PA, blobA, blobH, splitm, reinterpret_cast<const uint8_t *>(pq_stage + (fused ? (int)cand_slot[i] : i) * cws), g, ps, pa);
                             pq_part[g * pstride + i] = ps;
                             if (METRIC == JV_METRIC_COSINE) pq_part[(8 + g) * pstride + i] = pa;
                         }
@@ -658,7 +682,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     for (int i = tid; i < n; i += SEARCH_THREADS) {
                         float sraw = pq_fold8(pq_part + i, pstride);
                         if (METRIC == JV_METRIC_COSINE)
-                            sraw = __fdiv_rn(sraw, __fsqrt_rn(__fmul_rn(pq_fold8(pq_part + 8 * pstride + i, pstride), blobH[P.approx.M * P.approx.k])));
+                            sraw = __fdiv_rn(sraw, __fsqrt_rn(__fmul_rn(pq_fold8(pq_part + 8 * pstride + i, pstride), blobH[PA.M * PA.k])));
                         const float sc = score_map(METRIC, sraw);
                         const int32_t f = cand_ids[i];
                         JV_EMIT(sc, f);
@@ -668,13 +692,13 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                     const uint8_t *codes0 = rec + 4 * degree;
                     for (int i = group; i < n; i += NG) {
                         const int32_t f = cand_ids[i];
-                        const float sc = score_pq_codes<METRIC>(P.approx, blobA, codes0 + (size_t)cand_slot[i] * P.g.fused_code_stride, lane, blobH, splitm);
+                        const float sc = score_pq_codes<METRIC>(PA, blobA, codes0 + (size_t)cand_slot[i] * PG.fused_code_stride, lane, blobH, splitm);
                         if (lane == 0) JV_EMIT(sc, f);
                     }
                 } else {
                     for (int i = group; i < n; i += NG) {
                         const int32_t f = cand_ids[i];
-                        const float sc = KIND == KIND_PQ ? score_pq<METRIC>(P.approx, blobA, f, lane, blobH, splitm) : score_row<KIND, METRIC>(P.approx, blobA, f, lane);
+                        const float sc = KIND == KIND_PQ ? score_pq<METRIC>(PA, blobA, f, lane, blobH, splitm) : score_row<KIND, METRIC>(PA, blobA, f, lane);
                         if (lane == 0) JV_EMIT(sc, f);
                     }
                 }
@@ -720,10 +744,10 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                             // a new candidate that lands at the very front is the likeliest next expansion: start pulling
                             // its adjacency row towards L2 now (128 B; reads only)
                             if (c < 2 && lvl == 0) {
-                                if (KIND == KIND_PQ && P.g.fused) prefetch_l2(P.g.fused + (size_t)key_node(k) * P.g.fused_rec);
-                                else prefetch_l2(P.g.adj0 + (size_t)key_node(k) * degree);
+                                if (KIND == KIND_PQ && PG.fused) prefetch_l2(PG.fused + (size_t)key_node(k) * PG.fused_rec);
+                                else prefetch_l2(PG.adj0 + (size_t)key_node(k) * degree);
                                 if (EDGE && size == LC)
-                                    bulk_prefetch_l2(P.g.edge_rec + (size_t)key_node(k) * degree * LR_SLOT, (unsigned)(degree * LR_SLOT));
+                                    bulk_prefetch_l2(PG.edge_rec + (size_t)key_node(k) * degree * LR_SLOT, (unsigned)(degree * LR_SLOT));
                             }
                         } else mydrop = max(mydrop, float_to_sortable(key_score(k)));
                     }
@@ -775,11 +799,11 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         unsigned reranked = 0;
         if (failed) {
             for (int i = tid; i < P.topK; i += SEARCH_THREADS) { no[i] = -1; so[i] = 0.f; }
-            if (tid == 0) { P.overflow[qi] = (uint8_t)failed; atomicAdd(&P.counters->overflowed, 1ull); }
+            if (tid == 0) { P.overflow[qi] = (uint8_t)failed; atomicAdd(&PC->overflowed, 1ull); }
         } else {
             if (tid == 0) {
                 P.overflow[qi] = 0;
-                if (truncated || inexact) atomicAdd(&P.counters->overflowed, 1ull);
+                if (truncated || inexact) atomicAdd(&PC->overflowed, 1ull);
             }
             const int hs = s_hsize;  // the results: heap[1 .. hs]
             if (P.has_rerank) {
@@ -817,25 +841,25 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 }
                 if (KIND == KIND_PQ || KIND == KIND_BQ) {
                     // the approximate walk left HBM idle: pull every survivor's exact row towards L2 before the rescoring loop
-                    const int lines = P.rerank.kind == KIND_F32 ? (P.rerank.stride * 4 + 127) / 128 : (P.rerank.byte_stride + 127) / 128;
+                    const int lines = PR.kind == KIND_F32 ? (PR.stride * 4 + 127) / 128 : (PR.byte_stride + 127) / 128;
                     for (int t = tid; t < hs * lines; t += SEARCH_THREADS) {
                         const int i = t / lines, l = t - i * lines;
                         if (!fcur[i]) continue;
                         const int32_t f = key_node(heap[1 + i]);
-                        const char *a = P.rerank.kind == KIND_F32 ? reinterpret_cast<const char *>(P.rerank.rows + (size_t)f * P.rerank.stride)
-                                                                  : reinterpret_cast<const char *>(P.rerank.bytes + (size_t)f * P.rerank.byte_stride);
+                        const char *a = PR.kind == KIND_F32 ? reinterpret_cast<const char *>(PR.rows + (size_t)f * PR.stride)
+                                                                  : reinterpret_cast<const char *>(PR.bytes + (size_t)f * PR.byte_stride);
                         prefetch_l2(a + (size_t)l * 128);
                     }
                 }
                 // exact keys in array order -> cur[0 .. hs) (KEY_MIN = not reranked)
-                if (P.rerank.kind == KIND_F32) {
+                if (PR.kind == KIND_F32) {
                     for (int i = wgroup; i < hs; i += 2 * NGR) {
                         const int32_t fa = key_node(heap[1 + i]);
                         const bool two = i + NGR < hs;
                         const int32_t fb = two ? key_node(heap[1 + i + NGR]) : fa;
                         const bool da = fcur[i] != 0, db = two && fcur[i + NGR] != 0;
                         float sa = 0.f, sb = 0.f;
-                        if (da || db) score_f32_pair<METRIC>(P.rerank, blobR, da ? fa : fb, db ? fb : fa, wlane, sa, sb);
+                        if (da || db) score_f32_pair<METRIC>(PR, blobR, da ? fa : fb, db ? fb : fa, wlane, sa, sb);
                         if (wlane == 0) {
                             cur[i] = da ? topk_key(sa, fa) : KEY_MIN;
                             if (two) cur[i + NGR] = db ? topk_key(sb, fb) : KEY_MIN;
@@ -846,7 +870,7 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                         const int32_t f = key_node(heap[1 + i]);
                         float sc = 0.f;
                         const bool d = fcur[i] != 0;
-                        if (d) sc = score_row<KIND_NVQ, METRIC>(P.rerank, blobR, f, wlane);
+                        if (d) sc = score_row<KIND_NVQ, METRIC>(PR, blobR, f, wlane);
                         if (wlane == 0) cur[i] = d ? topk_key(sc, f) : KEY_MIN;
                     }
                 }
@@ -890,10 +914,19 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
                 }
             }
             if (tid == 0) {
-                atomicAdd(&P.counters->visited, (unsigned long long)visited);
-                atomicAdd(&P.counters->expanded, (unsigned long long)expanded);
-                atomicAdd(&P.counters->expanded_base, (unsigned long long)expanded_base);
-                atomicAdd(&P.counters->reranked, (unsigned long long)reranked);
+                atomicAdd(&PC->visited, (unsigned long long)visited);
+                atomicAdd(&PC->expanded, (unsigned long long)expanded);
+                atomicAdd(&PC->expanded_base, (unsigned long long)expanded_base);
+                atomicAdd(&PC->reranked, (unsigned long long)reranked);
+            }
+        }
+        if constexpr (SEG && EDGE) {
+            // the next item may belong to another segment: this one's edge-tier totals go to its own counters now
+            if (tid == 0) {
+                if (s_settled_total) atomicAdd(&PC->settled, s_settled_total);
+                if (s_direct_total[0]) atomicAdd(&PC->direct, s_direct_total[0]);
+                if (s_direct_total[1]) atomicAdd(&PC->direct_dropped, s_direct_total[1]);
+                s_settled_total = 0; s_direct_total[0] = 0; s_direct_total[1] = 0;
             }
         }
         __syncthreads();
@@ -907,6 +940,10 @@ __global__ void __launch_bounds__(SearchThreads<KIND>::value, MINB) graph_search
         }
 #endif
     }
+#undef PC
+#undef PR
+#undef PA
+#undef PG
 }
 
 // shared-memory floats of the walking scorer's prepared query: everything, except for a PQ LUT of which only the rows of the
@@ -1155,10 +1192,28 @@ bool search_uses_sketch(const DataDesc &approx, int metric, const SearchPlan &pl
 
 int sketch_stride(int stride) { return (stride + 7) & ~7; }
 
+void search_walk_descs(GraphDesc &g, DataDesc &approx, int metric, bool sketch)
+{
+    if (!(approx.kind == KIND_PQ && g.fused && g.fused_codes_of == approx.codes && g.fused_code_stride == approx.code_stride)) g.fused = nullptr;
+    {
+        const char *fe = getenv("JV_FUSED_PQ");
+        if (fe && fe[0] == '0') g.fused = nullptr;
+    }
+    if (!sketch) {
+        approx.sketch = nullptr;
+        approx.sketch_meta = nullptr;
+    }
+#ifdef JV_ROW_BOUND_STATS
+    approx.sketch = nullptr;  // the drop statistics describe the walk that reads every row
+#endif
+    if (!approx.sketch || !approx.lr_basis || approx.kind != KIND_F32 || metric != JV_METRIC_DOT) g.edge_rec = nullptr;
+}
+
 cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const DataDesc *rerank, int metric, const float *queries_dev,
                           int nq, int topK, int rerankK, const SearchPlan &plan, void *scratch_dev, int *work_counter_dev,
                           int32_t *nodes_out_dev, float *scores_out_dev, SearchCounters *counters_dev, uint8_t *overflow_flags_dev,
-                          const int32_t *query_index_dev, int query_stride, const SearchFilter *filter, cudaStream_t s)
+                          const int32_t *query_index_dev, int query_stride, const SearchFilter *filter, cudaStream_t s,
+                          const SegmentGroup *segments)
 {
     if (nq <= 0) return cudaSuccess;
     SearchParams P;
@@ -1171,13 +1226,12 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     P.lenient = filter ? filter->lenient : 0;
     P.arrived = filter ? filter->arrived : nullptr;
     P.query_stride = query_stride > 0 ? query_stride : approx.dim;
+    // SEG walks (segments != nullptr): g and approx stand for the group (its largest degree, the first segment's data set), each
+    // item reads its own segment's from segments->descs_dev
     P.g = g;
-    if (!(approx.kind == KIND_PQ && g.fused && g.fused_codes_of == approx.codes && g.fused_code_stride == approx.code_stride)) P.g.fused = nullptr;
-    {
-        const char *fe = getenv("JV_FUSED_PQ");
-        if (fe && fe[0] == '0') P.g.fused = nullptr;
-    }
     P.approx = approx;
+    P.segs = segments ? segments->descs_dev : nullptr;
+    P.seg_nq = segments ? segments->nq : 0;
     P.has_rerank = rerank ? 1 : 0;
     P.rerank = rerank ? *rerank : approx;
     P.metric = metric;
@@ -1213,14 +1267,8 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
     // read from DRAM twice (c2: 35.2 ms with the prefetch, 30.7 ms without)
     P.row_prefetch = (approx.kind == KIND_F32 && fills_gpu(plan, nq)) ? 0 : plan.row_prefetch;
     // the same batches, when they are DOT walks, use the row sketch where the caller passes one
-    if (!search_uses_sketch(approx, metric, plan, nq)) {
-        P.approx.sketch = nullptr;
-        P.approx.sketch_meta = nullptr;
-    }
-#ifdef JV_ROW_BOUND_STATS
-    P.approx.sketch = nullptr;  // the drop statistics describe the walk that reads every row
-#endif
-    if (!P.approx.sketch || !P.approx.lr_basis || approx.kind != KIND_F32 || metric != JV_METRIC_DOT) P.g.edge_rec = nullptr;
+    // (SEG walks: the caller decided for the whole call and prepared every segment's descriptor so, search_walk_descs included)
+    if (!segments) search_walk_descs(P.g, P.approx, metric, search_uses_sketch(approx, metric, plan, nq));
     P.pq_rows = plan.pq_rows;
     {
         // on for the latency-bound walks (PQ / BQ: c3 12.0 -> 11.5 ms); off where HBM is already saturated and a wasted adjacency
@@ -1260,7 +1308,26 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
         e = cudaFuncSetAttribute(graph_search_kernel<K, M, B, V, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
         if (e == cudaSuccess) graph_search_kernel<K, M, B, V, false, true><<<plan.ctas, SearchThreads<K>::value, plan.smem_bytes, s>>>(P); \
     } while (0)
-    if (P.exclude_ids) {
+#define CALL_SEG(K, M, B, V)                                                                                                        \
+    do {                                                                                                                              \
+        e = cudaFuncSetAttribute(graph_search_kernel<K, M, B, V, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
+        if (e == cudaSuccess) graph_search_kernel<K, M, B, V, false, false, true><<<plan.ctas, SearchThreads<K>::value, plan.smem_bytes, s>>>(P); \
+    } while (0)
+#define CALL_EDGE_SEG(B, V)                                                                                                            \
+    do {                                                                                                                              \
+        e = cudaFuncSetAttribute(graph_search_kernel<KIND_F32, JV_METRIC_DOT, B, V, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem_bytes); \
+        if (e == cudaSuccess) graph_search_kernel<KIND_F32, JV_METRIC_DOT, B, V, true, false, true><<<plan.ctas, SearchThreads<KIND_F32>::value, plan.smem_bytes, s>>>(P); \
+    } while (0)
+    if (segments) {
+        if (P.exclude_ids) e = cudaErrorInvalidValue;
+        else if (P.g.edge_rec) {
+            if (plan.vis_slots_log != 0) {
+                if (plan.pq_wide) CALL_EDGE_SEG(MINB_ROWS_WIDE, true);
+                else CALL_EDGE_SEG(MINB_ROWS, true);
+            } else if (plan.pq_wide) CALL_EDGE_SEG(MINB_ROWS_WIDE, false);
+            else CALL_EDGE_SEG(MINB_ROWS, false);
+        } else JV_SEARCH_DISPATCH(approx.kind, metric, plan.pq_wide != 0, plan.vis_slots_log != 0, CALL_SEG);
+    } else if (P.exclude_ids) {
         P.g.edge_rec = nullptr;
         if (plan.vis_slots_log != 0) JV_SEARCH_DISPATCH_FPB_V(approx.kind, metric, plan.pq_wide != 0, true, CALL_EXCL, e = cudaErrorInvalidValue);
         else JV_SEARCH_DISPATCH_FPB_V(approx.kind, metric, plan.pq_wide != 0, false, CALL_EXCL, e = cudaErrorInvalidValue);
@@ -1271,6 +1338,8 @@ cudaError_t launch_search(const GraphDesc &g, const DataDesc &approx, const Data
         } else if (plan.pq_wide) CALL_EDGE(MINB_ROWS_WIDE, false);
         else CALL_EDGE(MINB_ROWS, false);
     } else JV_SEARCH_DISPATCH(approx.kind, metric, plan.pq_wide != 0, plan.vis_slots_log != 0, CALL);
+#undef CALL_EDGE_SEG
+#undef CALL_SEG
 #undef CALL_EXCL
 #undef CALL_EDGE
 #undef CALL
